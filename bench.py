@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- mel-frames/sec through Text2Mel (AR, 210 steps) + SSRN on N B200s.
+"""bench.py -- mel-frames/sec through Text2Mel (AR, 210 steps) + SSRN on N H100s.
 
 Workload (BASELINE.json config 4 per-GPU shard; config.workload names it): every rank
 synthesises `--batch` (default 32) synthetic 100-character utterances: TextEnc once, the 210
@@ -34,11 +34,12 @@ def measured_peaks():
         p = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return dict(hbm_gbs=p["hbm_gbs"], tf=p["bf16_tflops"], tf_sustained=p.get("bf16_tflops_sustained"), src="measured")
     except Exception:
-        return dict(hbm_gbs=6650.0, tf=1590.0, tf_sustained=1400.0, src="fallback")   # B200_PROFILING.md
+        # NVIDIA H100 SXM data sheet (700 W card): HBM3 bandwidth, dense FP16 tensor rate -- not measured here
+        return dict(hbm_gbs=3350.0, tf=989.0, tf_sustained=None, src="fallback (H100 SXM data sheet)")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -179,26 +180,16 @@ def workload_config(args, world):
             "batch_per_gpu": args.batch, "global_batch": args.batch * world, "max_N": 180, "max_T": 210,
             "parallelism": "utterance-shard x%d + one NCCL gather of Z to rank 0 (chunked, overlapped with the SSRN)" % world,
             "l2": "flushed between timed steps (256 MiB write, untimed); per-step working set "
-                  "(weights 210 MB + activations) also exceeds the 126 MB L2"}
+                  "(weights 210 MB + activations) also exceeds the 50 MB L2"}
 
 
-# ------------------------------------------------------------------------------ B200 arm
+# ------------------------------------------------------------------------------ CUDA arm
 # Algorithmic work of the path (SURVEY.md 8a / 8d), per utterance
 MAC_TEXTENC_PER_CHAR = 17104896            # TextEnc, per character position (N = 180 positions)
 MAC_AUDIOENC_PER_FRAME = 4083712
 MAC_AUDIODEC_PER_FRAME = 2707456
 MAC_SSRN_PER_FRAME = 93655052
 DECODE_WEIGHT_BYTES = (4101376 + 2719984) * 4          # AudioEnc + AudioDec parameters, fp32: read once per mel frame
-
-
-def ncu_traffic(name):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed ncu summary of this round
-    (profiles/r02_ncu_traffic.json, written by tools/ncu_traffic.py from the .ncu-rep), or None."""
-    try:
-        d = json.load(open(os.path.join(ROOT, "profiles", "r02_ncu_traffic.json")))
-        return d.get(name)
-    except Exception:
-        return None
 
 
 def parity_sample(eng, params, L_row, Y_row, Z_row, P_row):
@@ -223,6 +214,31 @@ def parity_sample(eng, params, L_row, Y_row, Z_row, P_row):
     if not (same_p and dy <= 1e-3 and (dz is None or dz <= 1e-3)):
         raise AssertionError("bench parity check failed: %s" % json.dumps(out))
     return out
+
+
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, Y, Z, P):
+    """What the last timed step returned, as float32 / float64 .npy files, over the global batch of all ranks (U = N * batch
+    utterances in rank order): mel (U, T, n_mels), mag (U, 4T, 1+n_fft/2) and the attention window of every frame (U, T).
+    When everything does not fit DUMP_BYTES, mag keeps a fixed, seeded sample of utterances; mag_rows.npy lists their
+    indices into the global batch."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    mel = Y.float().cpu().numpy()
+    win = P.cpu().numpy().astype(np.float64)
+    per_utt = Z[0].numel() * 4
+    room = DUMP_BYTES - mel.nbytes - win.nbytes
+    rows = np.arange(Z.shape[0])
+    if room < per_utt * Z.shape[0]:
+        k = max(1, room // per_utt)
+        rows = np.sort(np.random.default_rng(0).choice(Z.shape[0], size=k, replace=False))
+        np.save(os.path.join(out_dir, "mag_rows.npy"), rows.astype(np.float64))
+    np.save(os.path.join(out_dir, "mel.npy"), mel)
+    np.save(os.path.join(out_dir, "mag.npy"), Z[torch.as_tensor(rows, device=Z.device)].float().cpu().numpy())
+    np.save(os.path.join(out_dir, "attention_windows.npy"), win)
 
 
 def run_b200(args, rank, local_rank, world):
@@ -297,6 +313,15 @@ def run_b200(args, rank, local_rank, world):
         Y, Z, P = step(marks=(evs[k][1], evs[k][2]))
         evs[k][3].record()
     barrier()
+    if args.dump_outputs:
+        Yd, Pd = Y, P
+        if world > 1:                              # rank 0 holds the gathered magnitudes: gather mel and windows too
+            Yd = torch.empty((total,) + tuple(Y.shape[1:]), dtype=Y.dtype, device=dev)
+            Pd = torch.empty((total,) + tuple(P.shape[1:]), dtype=P.dtype, device=dev)
+            dist.all_gather_into_tensor(Yd, Y.contiguous())
+            dist.all_gather_into_tensor(Pd, P.contiguous())
+        if rank == 0:
+            dump_outputs(args.dump_outputs, Yd, Z, Pd)
     ms = sum(e[0].elapsed_time(e[3]) for e in evs)
     ms_t2m = sum(e[0].elapsed_time(e[1]) for e in evs) / args.steps
     ms_ssrn = sum(e[1].elapsed_time(e[2]) for e in evs) / args.steps
@@ -363,7 +388,7 @@ def run_b200(args, rank, local_rank, world):
                            "dp%d (all-reduce of %d gradients)" % (B, hp.dropout_rate, world, grads.numel()),
                  "ms_per_step": tms, "steps_per_sec": 1e3 / tms, "mel_frames_per_sec": world * B * T * 1e3 / tms, "steps": args.train_steps,
                  "achieved_tflops": world * tfl / (tms * 1e-3) / 1e12, "gpu_launches_per_step": (teng.launch_count() - n0) // args.train_steps,
-                 "dtype": ("f32 tensors; forward / data-gradient / weight-gradient GEMMs as split-fp16 x3 on tcgen05, fp32 accumulate"
+                 "dtype": ("f32 tensors; forward / data-gradient / weight-gradient GEMMs as split-fp16 x3 on wgmma, fp32 accumulate"
                            if args.train_tc else "f32 (CUDA-core kernels)"),
                  "loss_first": first["loss"], "loss_last": last["loss"], "scaling": "weak"}
         teng.close()
@@ -390,7 +415,7 @@ def run_b200(args, rank, local_rank, world):
         by_dec = float(T) * (DECODE_WEIGHT_BYTES + B * 4 * (hp.n_mels * 2 + 24 * 256 * 4))    # weights once per frame + rows in/out
         tf_peak = peaks["tf_sustained"] or peaks["tf"]
         stages = [
-            {"stage": "TextEnc (tcgen05 blocks, once per batch)", "ms": ms_te, "share": ms_te / step_ms, "bound": "tensor",
+            {"stage": "TextEnc (wgmma blocks, once per batch)", "ms": ms_te, "share": ms_te / step_ms, "bound": "tensor",
              "algorithmic_flops": fl_te, "achieved_tflops": fl_te / ms_te / 1e9, "frac": fl_te / ms_te / 1e9 / tf_peak},
             {"stage": "decode: 210 frames of AudioEnc + Attention + AudioDec (%s)"
                       % ("ONE persistent cluster kernel" if args.decode_mode == 1 else "one CUDA graph per frame"),
@@ -403,7 +428,7 @@ def run_b200(args, rank, local_rank, world):
              "window_moves": (None if dstats is None else {"cluster_frames_with_recompute": dstats[0],
                                                            "utterance_frames_recomputed": dstats[1], "clusters": dstats[2],
                                                            "of_utterance_frames": B * T})},
-            {"stage": "SSRN (tcgen05 blocks)", "ms": ms_ssrn, "share": ms_ssrn / step_ms, "bound": "tensor",
+            {"stage": "SSRN (wgmma blocks)", "ms": ms_ssrn, "share": ms_ssrn / step_ms, "bound": "tensor",
              "algorithmic_flops": fl_ssrn, "achieved_tflops": fl_ssrn / ms_ssrn / 1e9, "frac": fl_ssrn / ms_ssrn / 1e9 / tf_peak,
              "tensor_pipe_frac_executed": 3 * fl_ssrn / ms_ssrn / 1e9 / tf_peak},
             {"stage": "gather tail (exposed part of the NCCL gather)", "ms": ms_tail, "share": ms_tail / step_ms},
@@ -414,10 +439,9 @@ def run_b200(args, rank, local_rank, world):
         flops = 2.0 * rows * 3 * 1024 * 2048
         k_ms = kms[1] if tensor else kms[0]          # tensor path: [fp32->planes, fused block]; fp32 path: [GEMM, LN]
         ach = flops / (k_ms * 1e-3) / 1e12
-        hc11 = {"kernel": ("conv_ln_tc_kernel: SSRN/HC_11 fused hc block on tcgen05 (M=%d, K=3x1024, N=2048, 3 fp16 MMA "
+        hc11 = {"kernel": ("conv_ln_tc_kernel: SSRN/HC_11 fused hc block on wgmma (M=%d, K=3x1024, N=2048, 3 fp16 MMA "
                            "passes per k-step)" if tensor else "conv_gemm_tiled: SSRN/HC_11 conv-GEMM on fp32 cores (M=%d, K=3x1024, N=2048)") % rows,
                 "bound": "tensor", "achieved": ach, "peak": peaks["tf"], "unit": "TFLOP/s", "frac": ach / peaks["tf"],
-                "traffic": ncu_traffic("conv_ln_tc_kernel_hc11_b32") if (tensor and B == 32) else None,
                 "algorithmic_bytes": int(rows * 1024 * 4 * 2 + 2 * 3 * 1024 * 2048 * 2),
                 "peak_source": peaks["src"] + " bf16/fp16 dense (burst)",
                 "kernel_ms": k_ms, "other_kernels_of_block_ms": [m for i, m in enumerate(kms) if m != k_ms],
@@ -429,11 +453,11 @@ def run_b200(args, rank, local_rank, world):
             roof = {"kernel": "decode_cluster_kernel: the whole AR loop (210 frames x 24 conv blocks + attention) in one launch, "
                               "%d clusters x 16 CTAs" % (dstats[2] if dstats else 0),
                     "bound": "hbm", "achieved": by_dec / ms_dec / 1e6, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                    "frac": by_dec / ms_dec / 1e6 / peaks["hbm_gbs"], "traffic": ncu_traffic("decode_cluster_kernel_b32"),
+                    "frac": by_dec / ms_dec / 1e6 / peaks["hbm_gbs"],
                     "algorithmic_bytes": int(by_dec), "peak_source": peaks["src"] + " HBM copy bandwidth", "kernel_ms": ms_dec,
                     "share_of_step": ms_dec / step_ms,
                     "note": "dominant kernel of the timed step; a dependent-latency chain (24 blocks x 210 frames), not a streaming "
-                            "kernel: its weights stay in L2 (27 MB << 126 MB), so DRAM traffic per launch is far below the "
+                            "kernel: its weights stay in L2 (27 MB < 50 MB), so DRAM traffic per launch is far below the "
                             "algorithmic bytes and the HBM roofline fraction mostly measures how short the chain is"}
         else:
             roof = hc11
@@ -472,7 +496,7 @@ def run_b200(args, rank, local_rank, world):
                    "hbm_bytes_algorithmic": int(hbm), "hbm_frac_of_measured_peak": hbm / dtv / 1e9 / peaks["hbm_gbs"]}
         line = {"metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps,
                 "warmup": args.warmup, "ms_per_step": ms / args.steps, "higher_is_better": True,
-                "scaling": "weak", "vs_baseline": None, "dtype": "f32 (decode: fp32 FMA; TextEnc/SSRN: fp16x2 split operands on tcgen05, fp32 accumulate)" if args.tensor_path else "f32", "data": "synthetic",
+                "scaling": "weak", "vs_baseline": None, "dtype": "f32 (decode: fp32 FMA; TextEnc/SSRN: fp16x2 split operands on wgmma, fp32 accumulate)" if args.tensor_path else "f32", "data": "synthetic",
                 "config": workload_config(args, world),
                 "clocks": clocks, "gpu_launches": launches,
                 "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": int(L_host.numel() * 4),
@@ -505,12 +529,14 @@ def main():
     ap.add_argument("--cpu-passes", type=int, default=6, help="full-graph passes (at the benchmark batch) of the CPU baseline sample (0 = skip)")
     ap.add_argument("--decode-mode", type=int, default=1, choices=[0, 1], help="1 = persistent cluster decode kernel (default), 0 = one CUDA graph per frame")
     ap.add_argument("--gather-chunks", type=int, default=0, help="N > 1: SSRN / gather chunks per rank (transfer of a chunk runs under the next chunk's SSRN); "
-                    "0 = auto: 1 up to 4 GPUs, 2 beyond (measured at N = 2: every extra chunk costs the SSRN ~0.55 ms of wave quantisation, "
-                    "41.04 / 41.62 / 42.26 ms for 1 / 2 / 3 chunks, while one rank's 110 MB leave in ~0.3 ms; rank 0's ingest grows with N)")
+                    "0 = auto: 1 up to 4 GPUs, 2 beyond (every extra chunk leaves partly filled waves in the SSRN, while rank 0's ingest "
+                    "grows with N)")
     ap.add_argument("--no-parity-check", dest="parity_check", action="store_false", help="skip the oracle check of the timed output")
-    ap.add_argument("--tensor-path", type=int, default=1, choices=[0, 1], help="1 = tcgen05 blocks (default), 0 = fp32 CUDA-core kernels only")
+    ap.add_argument("--tensor-path", type=int, default=1, choices=[0, 1], help="1 = tensor-core (wgmma) blocks (default), 0 = fp32 CUDA-core kernels only")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write what the last timed step computed (mel, mag, "
+                    "attention windows) as .npy files under DIR")
     ap.add_argument("--train-steps", type=int, default=5, help="timed steps of the BASELINE config 5 training step reported as train_config5 (0 = skip)")
-    ap.add_argument("--train-tc", type=int, default=7, help="training GEMMs on tcgen05, bit mask (1 forward, 2 data gradient, 4 weight gradient); 0 = fp32 CUDA cores")
+    ap.add_argument("--train-tc", type=int, default=7, help="training GEMMs on the tensor cores, bit mask (1 forward, 2 data gradient, 4 weight gradient); 0 = fp32 CUDA cores")
     args = ap.parse_args()
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))

@@ -2,7 +2,7 @@
 
 There is deliberately no fallback: if the shared library has not been built
 (`python -m dc_tts_b200.build`) importing this module raises ImportError, and if no
-sm_100 GPU is present `dctts_create` fails -- the product path never computes on the CPU.
+sm_90 GPU is present `dctts_create` fails -- the product path never computes on the CPU.
 """
 import ctypes as C
 import os

@@ -1,7 +1,7 @@
-"""In-tree build of libdctts_b200.so (nvcc, sm_100a only).
+"""In-tree build of libdctts_b200.so (nvcc, sm_90a only).
 
 `python -m dc_tts_b200.build` or `__graft_entry__.build()`.  The .so is written next to
-this file so that it travels with the repo snapshot to the GPU box; it is git-ignored.
+this file, so that the package is importable from the source tree; it is git-ignored.
 """
 import os
 import subprocess
@@ -12,7 +12,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libdctts_b200.so")
 SOURCES = ["dctts_api.cu", "kernels_simt.cu", "kernels_tc.cu", "kernels_attn_tc.cu", "kernels_vocoder.cu", "kernels_train.cu", "kernels_decode.cu", "kernels_gemm_tc.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--use_fast_math" if False else "-DDCTTS_NO_FAST_MATH",     # accuracy first: no fast-math
     "-Xcompiler", "-fPIC,-O3,-Wall", "-Xptxas", "-v", "--expt-relaxed-constexpr",
 ]
@@ -51,7 +51,7 @@ def build(force=False, verbose=False):
                 sys.stderr.write(r.stderr)
         objs.append(o)
     if force or _stale(LIB, objs):
-        cmd = [_nvcc(), "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a",
+        cmd = [_nvcc(), "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a",
                                                          "-cudart", "static", "-Xcompiler", "-fPIC"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:

@@ -94,6 +94,7 @@ struct DevBuf {
 struct dctts_handle_s {
     dctts_hparams hp{};
     int device = 0;
+    int num_sms = 132;            // streaming multiprocessors of the device (set at creation)
     int F = 0;
     cudaStream_t stream = nullptr;
     cudaStream_t copy_stream = nullptr;      // device->host copies of finished spectrogram chunks (dctts_synthesize_host)
@@ -124,7 +125,7 @@ struct dctts_handle_s {
     DevBuf lbuf;                  // (B, N) ids staging for the host entry point
     DevBuf zbuf;                  // (B, 4T, F) staging for the host entry point
     DevBuf plane[4];              // tensor-core path activations: {hi,lo} x ping-pong, rows x 1032 fp16
-    DevBuf attpl[6];              // tcgen05 attention operands: Q, K planes and transposed V planes ({hi,lo} each)
+    DevBuf attpl[6];              // wgmma attention operands: Q, K planes and transposed V planes ({hi,lo} each)
     DevBuf arpl[10];              // AR decode planes: R (B,T,2d) and four AudioDec outputs (B,T,d), {hi,lo} each
 
     // training step (Text2Mel, reference train.py mode "train"): see the "training" section below
@@ -141,7 +142,7 @@ struct dctts_handle_s {
         std::map<std::string, TrainTensor> tensors;            // by TF variable name
         DevBuf pre, out, emb, R, align, dS, gbuf[4], dy, wT, zeros, gts, sums, ids, grads, mom, vel, entries;
         long long n_grad = 0; int n_entries = 0; float* d_table = nullptr;
-        DevBuf tc_a_hi, tc_a_lo, tc_b_hi, tc_b_lo, tc_slots;    // operand planes of the tcgen05 training GEMMs (kernels_gemm_tc.cu)
+        DevBuf tc_a_hi, tc_a_lo, tc_b_hi, tc_b_lo, tc_slots;    // operand planes of the wgmma training GEMMs (kernels_gemm_tc.cu)
         GemmTcWs tc;
         int first[3] = {0, 0, 0}, last[3] = {0, 0, 0};         // layer index ranges: TextEnc, AudioEnc, AudioDec
     } tr;
@@ -158,14 +159,12 @@ struct dctts_handle_s {
     int ar_B = 0;
     int64_t ar_nodes = 0;
 
-    int tensor_path = 1;          // tcgen05 blocks wherever they apply; 0 forces the fp32 CUDA-core kernels
+    int tensor_path = 1;          // wgmma blocks wherever they apply; 0 forces the fp32 CUDA-core kernels
     int64_t launches = 0;
 
     // kernel-variant switches (dctts_set_option); the defaults are the measured-best configuration
     struct {
-        int tc_occ2 = 1;          // two tcgen05 CTAs per SM (32-wide slab, 2 stages) on launches that fill the machine
-        int tc_cg2 = 0;           // CTA pairs (cta_group::2): 0 off, 1 wide (N = 512 per pair), 2 narrow (N = 256 per pair)
-        int tc_tile_pair = 0;     // two 128-row tiles per CTA sharing one weight slab
+        int tc_occ2 = 1;          // two-stage ring on launches wider than the device
         int tc_mcast = 1;         // TMA multicast of the activation tile across the cluster
         int tc_resid_tma = 1;     // hc: residual in / planes out through TMA
         int tc_debug = 0;         // progress markers + in-kernel cycle stamps (synchronising)
@@ -173,7 +172,7 @@ struct dctts_handle_s {
         int decode_prof = 0;      // persistent decode: record SM-clock lap timers of cluster 0 / rank 0 (dctts_decode_profile)
         int decode_mode = 1;      // 1 = persistent cluster kernel (kernels_decode.cu), 0 = one CUDA graph per frame (round-1 path)
         int train_probe = 0;      // measurement only (tools/bench_train.py --probe): the training GEMMs fetch their operands but issue no MMA
-        int train_tc = 7;         // training GEMMs on tcgen05, bit mask: 1 forward conv, 2 data gradient, 4 weight gradient; 0 = fp32 CUDA-core kernels
+        int train_tc = 7;         // training GEMMs on wgmma, bit mask: 1 forward conv, 2 data gradient, 4 weight gradient; 0 = fp32 CUDA-core kernels
     } opt;
 
     // persistent decode (kernels_decode.cu)
@@ -302,7 +301,7 @@ float* upload_vec(H* h, const std::string& name, int n, int padded) {
     return d;
 }
 
-// Split-fp16 packing for the tcgen05 kernel (kernels_tc.cu).  Rows are accumulator columns in
+// Split-fp16 packing for the wgmma kernel (kernels_tc.cu).  Rows are accumulator columns in
 // cluster-slice order (CTA i owns rows [i*bn, (i+1)*bn); for hc / transposed conv its first
 // `half` rows are the first LN half, the rest the second), columns are k = tap*cin_pad + ci.
 // Weights are multiplied by a power of two that brings max|W| into [2^10, 2^11) so that the
@@ -455,11 +454,11 @@ void pack_decode(H* h) {
     for (int li = P.n_enc; li < P.nl; ++li)                        // the receptive-field blocks must be a prefix of AudioDec
         if (P.L[li].prow > 1 && li > P.n_enc && P.L[li - 1].prow <= 1) { D.why = "persistent decode: receptive-field blocks not contiguous"; return; }
     P.nch = nch;
-    // the receptive-field blocks a second time, as split-fp16 MMA slabs (tcgen05 pre-pass): same chunk sizes, appended
+    // the receptive-field blocks a second time, as split-fp16 MMA slabs (tensor-core pre-pass): same chunk sizes, appended
     for (int li = 0; li < P.nl; ++li) {
         const DecLayer& L = P.L[li];
         if (L.prow <= 1) continue;
-        if (L.krows % 128 || (L.ns != 32 && L.ns != 16)) { D.why = "persistent decode: tcgen05 pre-pass geometry"; return; }
+        if (L.krows % 128 || (L.ns != 32 && L.ns != 16)) { D.why = "persistent decode: tensor-core pre-pass geometry"; return; }
         for (int c = L.ch0; c < L.ch0 + L.nch; ++c) { P.C[c].off16 = off; off += L.krows * L.ns; }
     }
     P.stream_len = off;
@@ -723,7 +722,7 @@ Planes ws_planes(H* h, int which, int C) {
     return p;
 }
 
-// One reference block as ONE tcgen05 kernel (kernels_tc.cu).  X are the split planes of the
+// One reference block as ONE wgmma kernel (kernels_tc.cu).  X are the split planes of the
 // (B, L, cin) input; the output goes to planes and/or fp32 tensors.
 void run_block_tc(Launch& lc, const LayerDev& l, int rate, bool causal, int act, Planes X, RowWin win,
                   int TT, int TB, int tiles_t, Planes out, float* out_f32, int ld_f32, float* sig_f32, int ld_sig,
@@ -734,46 +733,24 @@ void run_block_tc(Launch& lc, const LayerDev& l, int rate, bool causal, int act,
     a.bias = l.bias; a.g1 = l.g1; a.b1 = l.b1; a.g2 = (p.mode == 1) ? l.g2 : l.g1; a.b2 = (p.mode == 1) ? l.b2 : l.b1;
     a.mode = p.mode; a.act = act; a.C = l.cout; a.bn = p.bn; a.half = p.half; a.inv_scale = p.inv_scale;
     const int tiles = ((win.B + TB - 1) / TB) * tiles_t;
-    // CTA pairs (tcgen05 cta_group::2): hc / transposed-conv blocks packed with 128-channel halves, on full
-    // sequences.  Ranks (2s, 2s+1) of the cluster share channel slice s (256 channels), take consecutive tiles,
-    // each stages half of the slice's weight slab; the accumulator is 512 columns (256 gate + 256 info).
-    // Two CTAs per SM (default for launches that fill the machine): 32-wide slab, two pipeline stages -> ~105 KB of
-    // shared memory and 256 TMEM columns per CTA, so one tile's epilogue runs under the other tile's main loop
-    // (SSRN at B=32: 5.61 -> 4.66 ms).  Option tc_occ2 = 0 turns it off; tc_cg2 = 1 selects CTA pairs instead
-    // (cta_group::2 needs all 512 TMEM columns, so the two cannot be combined).
+    // Option tc_occ2 = 1 (default): launches wider than the device take a two-stage ring; 0 lets the ring grow to what
+    // shared memory holds (three stages for a 256-column hc block).  The kernel runs one CTA per SM either way, and on an
+    // H100 SXM (400 W limit) the two measured the same: SSRN at B = 32, T = 210 32.8 vs 32.7-32.8 ms per pass.
     H* h = lc.h;
-    const bool occ2_mode = h->opt.tc_occ2 != 0;
-    // option tc_cg2: 1 = wide pairs (N = 512 per pair, all of TMEM, one CTA per SM), 2 = narrow pairs (N = 256 per pair,
-    // 256 TMEM columns per CTA, so two CTAs per SM still overlap epilogue and main loop; the cluster doubles to
-    // 2 x slices CTAs, 16 for the C = 1024 blocks)
-    const int cg2_mode = h->opt.tc_cg2;
-    const bool pairable = p.mode != 0 && p.half == 128 && p.bn == 256 && !win.jptr && TT == 128 && TB == 1;
-    // Only when the paired grid still fills the machine: pairs halve the CTA count (B=1 SSRN: 1.09 vs 0.74 ms).
-    const bool wide_pairs = cg2_mode == 1 && pairable && (p.ncta % 2) == 0 && tiles * p.ncta >= 4 * 148;
-    const bool narrow_pairs = cg2_mode == 2 && pairable && 2 * p.ncta <= 16 && tiles * p.ncta >= 2 * 148;
-    const int cg = (wide_pairs || narrow_pairs) ? 2 : 1;
-    if (wide_pairs) { a.bn = 512; a.half = 256; }
-    const int cluster = narrow_pairs ? 2 * p.ncta : p.ncta;
-    // option tc_tile_pair: two 128-row tiles per CTA sharing one weight slab (a third fewer bytes per MMA).
-    // Measured no gain (SSRN/HC_11: 1.27 vs 1.26 ms), like TMA multicast and a deeper pipeline.
-    const bool pair = h->opt.tc_tile_pair != 0;
-    const int mt = (cg == 1 && pair && !win.jptr && TT == 128 && TB == 1 && tiles * p.ncta >= 4 * 148) ? 2 : 1;
-    const bool occ2 = occ2_mode && cg == 1 && mt == 1 && !win.jptr && TT == 128 && TB == 1 && tiles * p.ncta >= 148;
-    const int bk = (mt == 2 || occ2 || narrow_pairs) ? 32 : (cg == 2 ? 64 : tc_bk());
+    const bool occ2 = h->opt.tc_occ2 != 0 && !win.jptr && TT == 128 && TB == 1 && tiles * p.ncta >= h->num_sms;
+    const int bk = tc_bk();
     a.ntaps = p.ntaps; a.kb_per_tap = p.kb_per_tap * (64 / bk);
     if (p.mode == 2) { a.shifts[0] = 0; a.shifts[1] = -1; }
     else {
         const int tot = (l.size - 1) * rate, left = causal ? tot : tot / 2;
         for (int j = 0; j < l.size; ++j) a.shifts[j] = j * rate - left + extra_shift;
     }
-    // decode-window launches: two stages keep the CTA under half an SM's shared memory, so two of them co-reside
-    a.stages = std::min(narrow_pairs ? 3 : ((occ2 || win.jptr) ? 2 : tc_stages_for(p.bn, bk, mt)), std::max(1, a.ntaps * a.kb_per_tap));   // p.bn = weight rows staged per CTA
     a.TT = TT; a.TB = TB; a.tiles_t = tiles_t; a.ntiles = tiles; a.win = win;
     a.X = X; a.out = out; a.out_f32 = out_f32; a.ld_f32 = ld_f32; a.sig_f32 = sig_f32; a.ld_sig = ld_sig; a.sig = sig;
     // the A tile is identical in all CTAs of the cluster: fetch it once (TMA multicast) when the
     // tile is 128 consecutive time rows, each CTA contributing 128/ncta of them
     const bool no_mcast = h->opt.tc_mcast == 0;
-    a.mcast = (!no_mcast && cg == 1 && p.ncta > 1 && TT == 128 && TB == 1) ? 1 : 0;
+    a.mcast = (!no_mcast && p.ncta > 1 && TT == 128 && TB == 1) ? 1 : 0;
     const int box_rows = a.mcast ? TT / p.ncta : TT;
     CUtensorMap mAh, mAl;
     tc_make_act_map(&mAh, X.hi, l.cin, X.ld, win.L, win.B, box_rows, TB, bk);
@@ -785,20 +762,15 @@ void run_block_tc(Launch& lc, const LayerDev& l, int rate, bool causal, int act,
         if (!dbg_host) CUDA_CHECK(cudaHostAlloc(&dbg_host, 16 * 64 * sizeof(int), cudaHostAllocMapped));
         memset(dbg_host, 0, 16 * 64 * sizeof(int));
         CUDA_CHECK(cudaHostGetDevicePointer(&a.dbg, dbg_host, 0));
-        fprintf(stderr, "[tc] %s mode=%d ncta=%d bn=%d half=%d stages=%d nkb=%d tiles=%d TT=%d TB=%d L=%d B=%d\n", l.scope.c_str(),
-                a.mode, p.ncta, a.bn, a.half, a.stages, a.ntaps * a.kb_per_tap, tiles, TT, TB, win.L, win.B);
     }
-    CUtensorMap mWh = p.mWhi, mWl = p.mWlo;
-    if (cg == 2) { tc_make_w_map(&mWh, p.Whi, p.Ktot, p.nrows, a.half / 2, bk); tc_make_w_map(&mWl, p.Wlo, p.Ktot, p.nrows, a.half / 2, bk); }   // gate / info boxes
-    else if (bk != tc_bk()) { tc_make_w_map(&mWh, p.Whi, p.Ktot, p.nrows, p.bn, bk); tc_make_w_map(&mWl, p.Wlo, p.Ktot, p.nrows, p.bn, bk); }
+    const CUtensorMap mWh = p.mWhi, mWl = p.mWlo;
     // hc on full sequences: the residual tile comes in by TMA and the output planes leave by TMA (staged in the
-    // same drained pipeline stage), instead of row-scattered 32-byte loads / stores from the epilogue threads
+    // same shared-memory tile), instead of row-scattered 32-byte loads / stores from the epilogue threads
     const bool no_rtma = h->opt.tc_resid_tma == 0;
     CUtensorMap io[4];
     a.resid_tma = 0;
     a.out_tma = 0;
-    if (!no_rtma && p.mode == 1 && cg == 1 && mt == 1 && TT == 128 && TB == 1 && (a.half % 64) == 0 &&
-        2 * a.half * 128 * 2 <= 2 * 128 * bk * 2 + 2 * a.bn * bk * 2) {
+    if (!no_rtma && p.mode == 1 && TT == 128 && TB == 1 && (a.half % 64) == 0) {
         a.resid_tma = 1;
         // TMA stores only on full sequences: in the decode window the tile starts at a negative time coordinate
         // (measured: the launch traps), and there the few output rows are cheap to store directly
@@ -810,8 +782,13 @@ void run_block_tc(Launch& lc, const LayerDev& l, int rate, bool causal, int act,
             tc_make_act_map(&io[3], out.lo, l.cout, out.ld, win.L, win.B, 128, 1, 64);
         } else { io[2] = io[0]; io[3] = io[1]; }
     }
-    launch_conv_ln_tc(mAh, mAl, mWh, mWl, a.resid_tma ? io : nullptr, a, cluster, (tiles + mt * cg - 1) / (mt * cg), bk, mt, cg,
-                      lc.s); lc.count();
+    // decode-window launches and launches that fill the machine: two stages (more CTAs in flight on a wide grid,
+    // fewer idle bytes on a short reduction); otherwise as many as shared memory holds
+    a.stages = std::min((occ2 || win.jptr) ? 2 : tc_stages_for(p.bn, bk, a.resid_tma, a.half), std::max(1, a.ntaps * a.kb_per_tap));
+    if (debug)
+        fprintf(stderr, "[tc] %s mode=%d ncta=%d bn=%d half=%d stages=%d nkb=%d tiles=%d TT=%d TB=%d L=%d B=%d\n", l.scope.c_str(),
+                a.mode, p.ncta, a.bn, a.half, a.stages, a.ntaps * a.kb_per_tap, tiles, TT, TB, win.L, win.B);
+    launch_conv_ln_tc(mAh, mAl, mWh, mWl, a.resid_tma ? io : nullptr, a, p.ncta, tiles, bk, lc.s); lc.count();
     if (debug) {
         cudaError_t e = cudaStreamSynchronize(lc.s);
         for (int c = 0; c < std::min(16, p.ncta * tiles); ++c)
@@ -1088,7 +1065,7 @@ void text2mel_forward(H* h, const int* L, const float* mels, const int* pma, int
     run_textenc(lc, L, B, h->kv.as<float>());
     const float* K = h->kv.as<float>();
     if (chain_tc_ok(h, h->audioenc) && chain_tc_ok(h, h->audiodec)) {
-        // tensor-core path: every block over all B*T rows as one tcgen05 kernel
+        // tensor-core path: every block over all B*T rows as one wgmma kernel
         Planes mp = ws_planes(h, 0, hp.n_mels);
         launch_f32_to_planes(mels, hp.n_mels, mp, (long long)B * T, hp.n_mels, lc.s); lc.count();
         float* Q = h->ae_out.back().as<float>();
@@ -1444,7 +1421,7 @@ void train_forward_backward(H* h, const int* L, const float* mels, int B, uint32
     train_fwd(h, lc, tr.first[1], tr.last[1], B, seed);
     const float* KV = tr.layers[tr.last[0]].out;               // (B, N, 2d): K | V
     const float* Q = tr.layers[tr.last[1]].out;                // (B, T, d)
-    // dense softmax attention (training: no window, networks.py:140-153): the tcgen05 kernel of the synthesis path when the
+    // dense softmax attention (training: no window, networks.py:140-153): the wgmma kernel of the synthesis path when the
     // forward GEMMs are on the tensor cores (it does not touch the weights), else one warp per query row on CUDA cores
     if ((h->opt.train_tc & 1) && d == 256 && N <= attn_tc_padded_keys())
         run_attention_tc(lc, Q, d, KV, 2 * d, KV + d, 2 * d, B, T, N, nullptr, tr.R.as<float>(), tr.align.as<float>(), nullptr, Planes{});
@@ -1518,7 +1495,7 @@ void trim_from_mse(const float* m, int nfr, int Ly, int32_t* out) {
 // ==================================================================================== C-ABI
 extern "C" {
 
-const char* dctts_version(void) { return "dc_tts_b200 0.1.0 (sm_100a)"; }
+const char* dctts_version(void) { return "dc_tts_b200 0.1.0 (sm_90a)"; }
 
 const char* dctts_last_error(dctts_handle h) { return h ? h->err.c_str() : g_create_error.c_str(); }
 
@@ -1530,11 +1507,11 @@ int dctts_create(const dctts_hparams* hp, int device, dctts_handle* out) {
         if (device < 0 || device >= ndev) throw std::runtime_error("dctts_create: no such CUDA device (no CPU fallback exists)");
         cudaDeviceProp prop;
         CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
-        if (prop.major != 10) throw std::runtime_error("dctts_create: this library is built for sm_100a (B200) only");
+        if (prop.major != 9 || prop.minor != 0) throw std::runtime_error("dctts_create: this library is built for sm_90a (H100) only");
         if (hp->d > 256 || hp->d % 8 || hp->e % 4 || hp->max_N > 192 || hp->r != 4)
             throw std::runtime_error("dctts_create: unsupported hyper-parameters");
         std::unique_ptr<dctts_handle_s> h(new dctts_handle_s());
-        h->hp = *hp; h->device = device; h->F = 1 + hp->n_fft / 2;
+        h->hp = *hp; h->device = device; h->F = 1 + hp->n_fft / 2; h->num_sms = prop.multiProcessorCount;
         CUDA_CHECK(cudaSetDevice(device));
         CUDA_CHECK(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
         build_tables(h.get());
@@ -2019,7 +1996,7 @@ int dctts_set_tensor_path(dctts_handle h, int32_t mode) {
     return guarded(h, [&] {
         REQUIRE(mode == 0 || mode == 1, "dctts_set_tensor_path: mode must be 0 or 1");
         REQUIRE(!(h->tr.ready && mode == 1), "dctts_set_tensor_path: this handle has been trained -- its packed fp16 weight planes "
-                "are stale; load the trained variables (dctts_train_tensor) into a new handle for the tcgen05 kernel set");
+                "are stale; load the trained variables (dctts_train_tensor) into a new handle for the wgmma kernel set");
         if (mode != h->tensor_path && h->ar_exec) {      // the captured AR step depends on the mode
             CUDA_CHECK(cudaDeviceSynchronize());
             cudaGraphExecDestroy(h->ar_exec); h->ar_exec = nullptr; h->ar_B = 0;
@@ -2034,8 +2011,6 @@ int dctts_set_tensor_path(dctts_handle h, int32_t mode) {
 static int* option_slot(dctts_handle h, const char* name) {
     const std::string n = name ? name : "";
     if (n == "tc_occ2") return &h->opt.tc_occ2;
-    if (n == "tc_cg2") return &h->opt.tc_cg2;
-    if (n == "tc_tile_pair") return &h->opt.tc_tile_pair;
     if (n == "tc_mcast") return &h->opt.tc_mcast;
     if (n == "tc_resid_tma") return &h->opt.tc_resid_tma;
     if (n == "tc_debug") return &h->opt.tc_debug;

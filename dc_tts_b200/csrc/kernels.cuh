@@ -177,7 +177,7 @@ void launch_guided_attention(float* W, int N, int T, cudaStream_t s);
 void launch_embed_bwd(const int* ids, const float* g, float* dtable, int rows, int e, cudaStream_t s);
 void launch_adam(const AdamEntry* entries_dev, int n_entries, float lr_t, float beta1, float beta2, float eps, cudaStream_t s);
 
-// ---- the training GEMMs on tcgen05 (kernels_gemm_tc.cu): drop-ins for launch_conv_gemm (tiled path) / launch_conv_wgrad ----
+// ---- the training GEMMs on wgmma (kernels_gemm_tc.cu): drop-ins for launch_conv_gemm (tiled path) / launch_conv_wgrad ----
 struct GemmTcWs {
     __half* a_hi = nullptr; __half* a_lo = nullptr; size_t a_elems = 0;   // operand A planes (activations / gradients, plain or transposed)
     __half* b_hi = nullptr; __half* b_lo = nullptr; size_t b_elems = 0;   // operand B planes (weights / transposed gradients)

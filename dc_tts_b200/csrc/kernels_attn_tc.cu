@@ -1,9 +1,10 @@
 // kernels_attn_tc.cu -- the dot-product attention (reference networks.py:126-155) as ONE
-// tcgen05 kernel: S = Q K^T / sqrt(d) -> window mask -> softmax -> argmax -> A V -> [A V ; Q],
-// alignments written transposed.  One CTA per (128 query rows, utterance).
+// wgmma kernel: S = Q K^T / sqrt(d) -> window mask -> softmax -> argmax -> A V -> [A V ; Q],
+// alignments written transposed.  One CTA per (128 query rows, utterance): a TMA producer
+// warp and two consumer warpgroups of 64 query rows each.
 //
 //   GEMM 1  S[128 x 192]  = Q[128 x 256] . K^T        (keys padded 180 -> 192 by TMA zero fill)
-//   softmax in the epilogue warps, one query row per thread, straight out of tensor memory;
+//   softmax on the register accumulators, four threads per query row (quad shuffles);
 //           the probabilities are written back to shared memory as split-fp16 planes in the
 //           128B-swizzled K-major layout the tensor core reads (no global round trip)
 //   GEMM 2  C[128 x 256]  = P[128 x 192] . V          (V pre-transposed to [d][keys] planes)
@@ -22,7 +23,7 @@ namespace dctts {
 
 using namespace ptx;
 
-constexpr int AT_THREADS = 192;
+constexpr int AT_THREADS = 384;
 constexpr int AT_NP = 192;                        // padded key count (3 x 64)
 constexpr int AT_D = 256;                         // head width (hp.d)
 constexpr int AT_Q_PLANE = 128 * 64 * 2;          // 16 KB: 128 query rows x 64 channels fp16
@@ -31,7 +32,6 @@ constexpr int AT_STAGE1 = 2 * AT_Q_PLANE + 2 * AT_K_PLANE;   // 80 KB
 constexpr int AT_P_PLANE = 3 * AT_Q_PLANE;        // 48 KB: 3 key blocks of [128 x 64]
 constexpr int AT_VT_PLANE = AT_D * 64 * 2;        // 32 KB: 256 channels x 64 keys
 constexpr int AT_SMEM_MAIN = 2 * AT_STAGE1;       // 160 KB
-constexpr int AT_TMEM_COLS = 512;                 // S at [0,192), context at [256,512)
 
 __global__ void __launch_bounds__(AT_THREADS, 1)
 attention_tc_kernel(const __grid_constant__ CUtensorMap mapQ_hi, const __grid_constant__ CUtensorMap mapQ_lo,
@@ -43,29 +43,22 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap mapQ_hi, const __grid_co
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + AT_SMEM_MAIN);
     uint64_t* full_bar = bars;            // [2]
     uint64_t* empty_bar = bars + 2;       // [2]
-    uint64_t* s_full = bars + 4;
-    uint64_t* p_full = bars + 5;
+    uint64_t* s_full = bars + 4;          // GEMM 1 done in both consumer warpgroups: its stages are free
     uint64_t* vt_full = bars + 6;
     uint64_t* vt_empty = bars + 7;
-    uint64_t* ctx_full = bars + 8;
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 9);
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
     const int b = blockIdx.y, t0 = blockIdx.x * 128;
     const int T = a.T, N = a.N;
 
     if (warp == 0 && lane == 0) {
         prefetch_tmap(&mapQ_hi); prefetch_tmap(&mapQ_lo); prefetch_tmap(&mapK_hi); prefetch_tmap(&mapK_lo);
         prefetch_tmap(&mapV_hi); prefetch_tmap(&mapV_lo);
-        for (int s = 0; s < 2; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        mbar_init(s_full, 1); mbar_init(p_full, 128); mbar_init(vt_full, 1); mbar_init(vt_empty, 1); mbar_init(ctx_full, 1);
+        for (int s = 0; s < 2; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
+        mbar_init(s_full, 2); mbar_init(vt_full, 1); mbar_init(vt_empty, 2);
         fence_mbar_init();
     }
-    if (warp == 1) tmem_alloc<AT_TMEM_COLS>(tmem_ptr_smem);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
 
     uint8_t* p_hi = smem;                          // [3][128 rows][128 B]
     uint8_t* p_lo = smem + AT_P_PLANE;
@@ -93,158 +86,172 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap mapQ_hi, const __grid_co
             }
         }
         __syncwarp();
-    } else if (warp == 1) {
-        // =========================== MMA issuer ===========================
-        const uint32_t idesc1 = umma_idesc_f16(128, AT_NP);
-        const uint32_t idesc2 = umma_idesc_f16(128, AT_D);
-        for (int kb = 0; kb < AT_D / 64; ++kb) {
-            const int s = kb & 1;
-            mbar_wait(&full_bar[s], (uint32_t)(kb >> 1) & 1u);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t st = smem_u32(smem + (size_t)s * AT_STAGE1);
-                const uint64_t dQ_hi = umma_desc_kmajor<128>(st), dQ_lo = umma_desc_kmajor<128>(st + AT_Q_PLANE);
-                const uint64_t dK_hi = umma_desc_kmajor<128>(st + 2 * AT_Q_PLANE);
-                const uint64_t dK_lo = umma_desc_kmajor<128>(st + 2 * AT_Q_PLANE + AT_K_PLANE);
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    const uint64_t adv = (uint64_t)(k * 2);
-                    tc_mma_f16(tmem_base, dQ_hi + adv, dK_hi + adv, idesc1, (kb | k) != 0);
-                    tc_mma_f16(tmem_base, dQ_hi + adv, dK_lo + adv, idesc1, 1u);
-                    tc_mma_f16(tmem_base, dQ_lo + adv, dK_hi + adv, idesc1, 1u);
-                }
-                tc_commit(&empty_bar[s]);
-                if (kb == AT_D / 64 - 1) tc_commit(s_full);
-            }
-            __syncwarp();
-        }
-        mbar_wait(p_full, 0);                      // probabilities are in shared memory (async-proxy visible)
-        tc_fence_after();
-        for (int kb = 0; kb < AT_NP / 64; ++kb) {
-            mbar_wait(vt_full, (uint32_t)kb & 1u);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint64_t dP_hi = umma_desc_kmajor<128>(smem_u32(p_hi + kb * AT_Q_PLANE));
-                const uint64_t dP_lo = umma_desc_kmajor<128>(smem_u32(p_lo + kb * AT_Q_PLANE));
-                const uint64_t dV_hi = umma_desc_kmajor<128>(smem_u32(vt_st));
-                const uint64_t dV_lo = umma_desc_kmajor<128>(smem_u32(vt_st + AT_VT_PLANE));
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    const uint64_t adv = (uint64_t)(k * 2);
-                    tc_mma_f16(tmem_base + 256, dP_hi + adv, dV_hi + adv, idesc2, (kb | k) != 0);
-                    tc_mma_f16(tmem_base + 256, dP_hi + adv, dV_lo + adv, idesc2, 1u);
-                    tc_mma_f16(tmem_base + 256, dP_lo + adv, dV_hi + adv, idesc2, 1u);
-                }
-                tc_commit(vt_empty);
-                if (kb == AT_NP / 64 - 1) tc_commit(ctx_full);
-            }
-            __syncwarp();
-        }
-    } else {
-        // =========================== softmax / epilogue ===========================
-        const int q = warp & 3;
-        const int r = q * 32 + lane;
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
-        const int t = t0 + r;
-        const bool row_ok = t < T;
-        int n_lo = 0, n_hi = N;
-        if (a.pma) {                               // monotonic window [p, p + win) (networks.py:141-147)
-            const int p = __ldg(a.pma + b);
-            n_lo = min(max(p, 0), N - 1);
-            n_hi = min(n_lo + a.win_size, N);
-        }
-        mbar_wait(s_full, 0);
-        tc_fence_after();
-        // pass 1: row maximum over the live keys
-        float mx = -INFINITY;
-        for (int c = 0; c < AT_NP; c += 16) {
-            float v[16];
-            tmem_ld16(taddr + c, v);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) if (c + i >= n_lo && c + i < n_hi) mx = fmaxf(mx, v[i] * a.scale);
-        }
-        // pass 2: normaliser
-        float sum = 0.f;
-        for (int c = 0; c < AT_NP; c += 16) {
-            float v[16];
-            tmem_ld16(taddr + c, v);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) if (c + i >= n_lo && c + i < n_hi) sum += expf(v[i] * a.scale - mx);
-        }
-        // pass 3: probabilities -> split planes in shared memory (swizzled), alignments, argmax
-        float best = -1.f; int besti = 0;
-        float* al = a.align ? a.align + (size_t)b * N * T + t : nullptr;
-        for (int c = 0; c < AT_NP; c += 16) {
-            float v[16];
-            tmem_ld16(taddr + c, v);
-            __align__(16) __half ph[16];
-            __align__(16) __half pl[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-                const int n = c + i;
-                float p = 0.f;                     // masked keys are exactly 0 in the reference (exp underflow)
-                if (n >= n_lo && n < n_hi) p = expf(v[i] * a.scale - mx) / sum;
-                if (p > best) { best = p; besti = n; }
-                ph[i] = __float2half_rn(p);
-                pl[i] = __float2half_rn(p - __half2float(ph[i]));
-                if (al && row_ok && n < N) al[(size_t)n * T] = p;
-            }
-            const int kb = c >> 6, c8 = (c & 63) >> 3;           // two 16-byte chunks: c8 and c8+1
-            uint8_t* rowh = p_hi + kb * AT_Q_PLANE + r * 128;
-            uint8_t* rowl = p_lo + kb * AT_Q_PLANE + r * 128;
-            *reinterpret_cast<uint4*>(rowh + (((c8) ^ (r & 7)) << 4)) = reinterpret_cast<const uint4*>(ph)[0];
-            *reinterpret_cast<uint4*>(rowh + (((c8 + 1) ^ (r & 7)) << 4)) = reinterpret_cast<const uint4*>(ph)[1];
-            *reinterpret_cast<uint4*>(rowl + (((c8) ^ (r & 7)) << 4)) = reinterpret_cast<const uint4*>(pl)[0];
-            *reinterpret_cast<uint4*>(rowl + (((c8 + 1) ^ (r & 7)) << 4)) = reinterpret_cast<const uint4*>(pl)[1];
-        }
-        if (row_ok && a.maxatt) a.maxatt[(size_t)b * T + t] = (long long)besti;
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> visible to the tensor core
-        tc_fence_before();
-        asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(smem_u32(p_full)) : "memory");
-
-        // context rows out of tensor memory; R = [context ; Q]
-        mbar_wait(ctx_full, 0);
-        tc_fence_after();
-        const size_t row = (size_t)b * T + t;
-        for (int c = 0; c < AT_D; c += 16) {
-            float v[16];
-            tmem_ld16(taddr + 256 + c, v);
-            if (row_ok) {
-                float* ro = a.R + row * a.ldr + c;
-#pragma unroll
-                for (int i = 0; i < 16; i += 4) *reinterpret_cast<float4*>(ro + i) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-                const float* qs = a.Q + row * a.ldq + c;
-                float qv[16];
-#pragma unroll
-                for (int i = 0; i < 16; i += 4) {
-                    const float4 x = __ldg(reinterpret_cast<const float4*>(qs + i));
-                    qv[i] = x.x; qv[i + 1] = x.y; qv[i + 2] = x.z; qv[i + 3] = x.w;
-                    *reinterpret_cast<float4*>(ro + AT_D + i) = x;
-                }
-                if (a.Rpl.hi) {
-                    __align__(16) __half h[16];
-                    __align__(16) __half l[16];
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) { h[i] = __float2half_rn(v[i]); l[i] = __float2half_rn(v[i] - __half2float(h[i])); }
-                    uint4* dh = reinterpret_cast<uint4*>(a.Rpl.hi + row * a.Rpl.ld + c);
-                    uint4* dl = reinterpret_cast<uint4*>(a.Rpl.lo + row * a.Rpl.ld + c);
-                    dh[0] = reinterpret_cast<const uint4*>(h)[0]; dh[1] = reinterpret_cast<const uint4*>(h)[1];
-                    dl[0] = reinterpret_cast<const uint4*>(l)[0]; dl[1] = reinterpret_cast<const uint4*>(l)[1];
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) { h[i] = __float2half_rn(qv[i]); l[i] = __float2half_rn(qv[i] - __half2float(h[i])); }
-                    dh = reinterpret_cast<uint4*>(a.Rpl.hi + row * a.Rpl.ld + AT_D + c);
-                    dl = reinterpret_cast<uint4*>(a.Rpl.lo + row * a.Rpl.ld + AT_D + c);
-                    dh[0] = reinterpret_cast<const uint4*>(h)[0]; dh[1] = reinterpret_cast<const uint4*>(h)[1];
-                    dl[0] = reinterpret_cast<const uint4*>(l)[0]; dl[1] = reinterpret_cast<const uint4*>(l)[1];
-                }
-            }
-        }
-        tc_fence_before();
+        return;
     }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc<AT_TMEM_COLS>(tmem_base);
+    if (wg == 0) return;                           // warps 1-3: no role
+    // =========================== consumers: query rows 64 * mh .. +64 of the tile ===========================
+    const int mh = wg - 1;
+    const bool leader = (threadIdx.x & 127) == 0;
+    const int rq = mh * 64 + (warp & 3) * 16 + (lane >> 2);        // fragment rows rq, rq + 8; columns 8 i + 2 (lane & 3) + {0, 1}
+    // ---- GEMM 1: S = Q K^T, 64 x 192 per warpgroup (three 64-key chunks) ----
+    float sacc[3][32];
+#pragma unroll
+    for (int j = 0; j < 3; ++j)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) sacc[j][i] = 0.f;
+    for (int kb = 0; kb < AT_D / 64; ++kb) {
+        const int s = kb & 1;
+        mbar_wait(&full_bar[s], (uint32_t)(kb >> 1) & 1u);
+        const uint32_t st = smem_u32(smem + (size_t)s * AT_STAGE1);
+        const uint64_t dQ_hi = gmma_desc_kmajor<128>(st + mh * 64 * 128), dQ_lo = gmma_desc_kmajor<128>(st + AT_Q_PLANE + mh * 64 * 128);
+        wg_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const uint64_t adv = (uint64_t)(k * 2);
+#pragma unroll
+            for (int j = 0; j < 3; ++j) {
+                const uint64_t dK_hi = gmma_desc_kmajor<128>(st + 2 * AT_Q_PLANE + j * 64 * 128);
+                const uint64_t dK_lo = gmma_desc_kmajor<128>(st + 2 * AT_Q_PLANE + AT_K_PLANE + j * 64 * 128);
+                wgmma_f16<4>(sacc[j], dQ_hi + adv, dK_hi + adv, (kb | k) != 0);
+                wgmma_f16<4>(sacc[j], dQ_hi + adv, dK_lo + adv, 1u);
+                wgmma_f16<4>(sacc[j], dQ_lo + adv, dK_hi + adv, 1u);
+            }
+        }
+        wg_commit();
+        wg_wait<0>();
+#pragma unroll
+        for (int j = 0; j < 3; ++j) wg_fence_regs(sacc[j]);
+        if (leader) mbar_arrive(&empty_bar[s]);
+    }
+    if (leader) mbar_arrive(s_full);
+    named_sync(1, 256);                            // both warpgroups are done with GEMM 1's stages: P may overwrite them
+
+    // ---- softmax over the live keys, four threads per query row (quad shuffles) ----
+    int n_lo = 0, n_hi = N;
+    if (a.pma) {                                   // monotonic window [p, p + win) (networks.py:141-147)
+        const int p = __ldg(a.pma + b);
+        n_lo = min(max(p, 0), N - 1);
+        n_hi = min(n_lo + a.win_size, N);
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {                  // the thread's two rows
+        const int r = rq + 8 * h, t = t0 + r;
+        const bool row_ok = t < T;
+        float mx = -INFINITY;
+#pragma unroll
+        for (int j = 0; j < 3; ++j)
+#pragma unroll
+            for (int i = 0; i < 8; ++i)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int n = j * 64 + i * 8 + 2 * (lane & 3) + e;
+                    if (n >= n_lo && n < n_hi) mx = fmaxf(mx, sacc[j][i * 4 + 2 * h + e] * a.scale);
+                }
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+        float sum = 0.f;
+#pragma unroll
+        for (int j = 0; j < 3; ++j)
+#pragma unroll
+            for (int i = 0; i < 8; ++i)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int n = j * 64 + i * 8 + 2 * (lane & 3) + e;
+                    if (n >= n_lo && n < n_hi) sum += expf(sacc[j][i * 4 + 2 * h + e] * a.scale - mx);
+                }
+        sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+        sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+        // probabilities -> split planes in shared memory (128B-swizzled K-major, GEMM 2's A operand), alignments, argmax
+        float best = -1.f; int besti = 0;
+        float* al = (a.align && row_ok) ? a.align + (size_t)b * N * T + t : nullptr;
+#pragma unroll
+        for (int j = 0; j < 3; ++j)
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                float p2[2];
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int n = j * 64 + i * 8 + 2 * (lane & 3) + e;
+                    float p = 0.f;                 // masked keys are exactly 0 in the reference (exp underflow)
+                    if (n >= n_lo && n < n_hi) p = expf(sacc[j][i * 4 + 2 * h + e] * a.scale - mx) / sum;
+                    if (p > best) { best = p; besti = n; }
+                    if (al && n < N) al[(size_t)n * T] = p;
+                    p2[e] = p;
+                }
+                const __half h0 = __float2half_rn(p2[0]), h1 = __float2half_rn(p2[1]);
+                const __half l0 = __float2half_rn(p2[0] - __half2float(h0)), l1 = __float2half_rn(p2[1] - __half2float(h1));
+                const int off = j * AT_Q_PLANE + r * 128 + ((i ^ (r & 7)) << 4) + 4 * (lane & 3);
+                *reinterpret_cast<__half2*>(p_hi + off) = __halves2half2(h0, h1);
+                *reinterpret_cast<__half2*>(p_lo + off) = __halves2half2(l0, l1);
+            }
+        // argmax over the quad: the first key of the largest probability, as a sequential scan finds it
+#pragma unroll
+        for (int o = 1; o <= 2; o <<= 1) {
+            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+            const int oi = __shfl_xor_sync(0xffffffffu, besti, o);
+            if (ob > best || (ob == best && oi < besti)) { best = ob; besti = oi; }
+        }
+        if (row_ok && a.maxatt && (lane & 3) == 0) a.maxatt[(size_t)b * T + t] = (long long)besti;
+    }
+    fence_proxy_async_smem();                      // generic-proxy stores -> visible to the tensor core
+    named_sync(1, 256);
+
+    // ---- GEMM 2: context = P V, 64 x 256 per warpgroup (four 64-channel chunks) ----
+    float cacc[4][32];
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) cacc[j][i] = 0.f;
+    for (int kb = 0; kb < AT_NP / 64; ++kb) {
+        mbar_wait(vt_full, (uint32_t)kb & 1u);
+        const uint64_t dP_hi = gmma_desc_kmajor<128>(smem_u32(p_hi + kb * AT_Q_PLANE + mh * 64 * 128));
+        const uint64_t dP_lo = gmma_desc_kmajor<128>(smem_u32(p_lo + kb * AT_Q_PLANE + mh * 64 * 128));
+        wg_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const uint64_t adv = (uint64_t)(k * 2);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const uint64_t dV_hi = gmma_desc_kmajor<128>(smem_u32(vt_st + j * 64 * 128));
+                const uint64_t dV_lo = gmma_desc_kmajor<128>(smem_u32(vt_st + AT_VT_PLANE + j * 64 * 128));
+                wgmma_f16<4>(cacc[j], dP_hi + adv, dV_hi + adv, (kb | k) != 0);
+                wgmma_f16<4>(cacc[j], dP_hi + adv, dV_lo + adv, 1u);
+                wgmma_f16<4>(cacc[j], dP_lo + adv, dV_hi + adv, 1u);
+            }
+        }
+        wg_commit();
+        wg_wait<0>();
+#pragma unroll
+        for (int j = 0; j < 4; ++j) wg_fence_regs(cacc[j]);
+        if (leader) mbar_arrive(vt_empty);
+    }
+
+    // ---- R = [context ; Q] straight from the fragments ----
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int t = t0 + rq + 8 * h;
+        if (t >= T) continue;
+        const size_t row = (size_t)b * T + t;
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                const int c = j * 64 + i * 8 + 2 * (lane & 3);
+                const float2 v = make_float2(cacc[j][i * 4 + 2 * h], cacc[j][i * 4 + 2 * h + 1]);
+                const float2 q = __ldg(reinterpret_cast<const float2*>(a.Q + row * a.ldq + c));
+                *reinterpret_cast<float2*>(a.R + row * a.ldr + c) = v;
+                *reinterpret_cast<float2*>(a.R + row * a.ldr + AT_D + c) = q;
+                if (a.Rpl.hi) {
+                    const __half vh0 = __float2half_rn(v.x), vh1 = __float2half_rn(v.y);
+                    const __half qh0 = __float2half_rn(q.x), qh1 = __float2half_rn(q.y);
+                    __half* dh = a.Rpl.hi + row * a.Rpl.ld;
+                    __half* dl = a.Rpl.lo + row * a.Rpl.ld;
+                    *reinterpret_cast<__half2*>(dh + c) = __halves2half2(vh0, vh1);
+                    *reinterpret_cast<__half2*>(dl + c) = __halves2half2(__float2half_rn(v.x - __half2float(vh0)), __float2half_rn(v.y - __half2float(vh1)));
+                    *reinterpret_cast<__half2*>(dh + AT_D + c) = __halves2half2(qh0, qh1);
+                    *reinterpret_cast<__half2*>(dl + AT_D + c) = __halves2half2(__float2half_rn(q.x - __half2float(qh0)), __float2half_rn(q.y - __half2float(qh1)));
+                }
+            }
     }
 }
 

@@ -24,7 +24,7 @@
 //     the window of an utterance does not move, the cached rows are exactly what a recompute would
 //     give.  When it moves, a PRE-PASS refreshes the rows t < j of its AudioDec receptive field
 //     (84/82/76/58/4/2 rows of C_1, HC_2..HC_6) under the new window -- attention one warp per row, a
-//     tcgen05 GEMM per utterance (split-fp16 planes staged per 16-channel slab in the no-swizzle K-major
+//     wgmma GEMM per utterance (split-fp16 planes staged per 16-channel slab in the no-swizzle K-major
 //     layout, the three taps being the same slab read through shifted descriptors), pre-LN rows through
 //     an L2 scratch, LayerNorm one warp per row over the whole cluster -- and the ordinary one-row pass
 //     then runs for every utterance.  The pre-pass consumes the same weight chunks a second time: the
@@ -58,7 +58,7 @@ static_assert(WRK_F >= GMAX * NT && WRK_F >= 1024, "work buffer: partial sums of
 struct Smem {
     float ring[DEC_NSLOT][NWARP][DEC_REG_F];
     union {                             // never live together: the pre-pass stages A here while no per-frame block is in flight
-        float wrk[WRK_F];               // tcgen05 pre-pass A slab stages (its reads run up to 128 + 54 rows past a slab start: xin follows)
+        float wrk[WRK_F];               // pre-pass A slab stages (its reads run up to 128 + 54 rows past a slab start: xin follows)
         float red[GMAX][NT];            // per-frame path: partial sums per warp; pre-pass: LayerNorm parameters of the block
     };
     float xin[2][GMAX][XLD];
@@ -67,10 +67,9 @@ struct Smem {
     float prm[2][DEC_PRM_F];
     unsigned long long fullw[DEC_NSLOT][NWARP];
     unsigned long long gbar[2];
-    unsigned long long sbar[TC_NSTG], abar[TC_NSTG], dbar;   // tcgen05 pre-pass: slab stage free / slab stage filled / accumulator complete
-    uint32_t tmem_base, pad_;
+    unsigned long long sbar[TC_NSTG], abar[TC_NSTG];   // pre-pass: slab stage free / slab stage filled
     float stat[GMAX][2][2];             // per utterance and LN half: mean, 1/sqrt(var + eps)
-    uint32_t tc_baddr[96];              // tcgen05 pre-pass: descriptor start field of every weight slab of the current block
+    uint32_t tc_baddr[96];              // pre-pass: descriptor start field of every weight slab of the current block
     int n_moved_frames, n_moved_utt;
     DecParams P;                        // the kernel's parameter block: indexed per block / chunk on the critical path; in the
                                         // constant bank those indexed loads missed the (instruction-shared) constant cache
@@ -115,6 +114,8 @@ __device__ __forceinline__ void bulk_s2peer(uint32_t dst_cluster, const void* sr
                  :: "r"(dst_cluster), "r"(smem_u32(src)), "r"(bytes), "r"(bar_cluster) : "memory");
 }
 __device__ __forceinline__ void cluster_sync_all() { cluster_arrive(); cluster_wait(); }
+// two independent fp32 FMAs on (x, y) pairs
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 __device__ __forceinline__ float4 ldcg4(const float* p) { return __ldcg(reinterpret_cast<const float4*>(p)); }
 __device__ __forceinline__ uint64_t* bar64(unsigned long long* p) { return reinterpret_cast<uint64_t*>(p); }
 
@@ -134,7 +135,7 @@ struct Stream {
     const float* base;          // this rank's packed stream
     Cur prod;                   // chunk that will be loaded into the slot the consumer frees next (the consumer itself walks the blocks' chunk ranges)
     unsigned pos;               // number of chunks consumed so far
-    unsigned tcq, tca;          // tcgen05 pre-pass: slabs staged / accumulators completed so far (mbarrier phase parities)
+    unsigned tcq;               // pre-pass: slabs staged so far (mbarrier phase parities)
 };
 // one lane of warp `warp`: load the warp's rows of chunk `u` into its region of `slot`
 __device__ __forceinline__ void stream_issue(const DecParams& P, Smem& S, const Stream& st, const Cur& u, int slot, int warp) {
@@ -198,9 +199,7 @@ __device__ __forceinline__ void gemv_warp(const float* __restrict__ wreg, const 
     const float* w = wreg + ((size_t)((sg * kper) >> 2) * ns + n) * 4;
     const float* xs = x + sg * kper;
     const int wstep = ns * 4;
-    // packed fp32 FMA (FFMA2, new on sm_100): one instruction multiplies two consecutive k of the column -- half the issue
-    // slots of the fma pipe, which two warps per scheduler otherwise saturate (ncu: the GEMV was fma-pipe bound at G = 5).
-    // Four partial sums per utterance (k mod 4 = {0,1} and {2,3} of either float4), added at the end.
+    // Four partial sums per utterance (k mod 4 = {0,1} and {2,3} of either float4), added at the end: independent FMA chains.
     float2 p0[GT], p1[GT];
 #pragma unroll
     for (int g = 0; g < GT; ++g) { p0[g] = make_float2(acc[g], 0.f); p1[g] = make_float2(0.f, 0.f); }
@@ -214,10 +213,10 @@ __device__ __forceinline__ void gemv_warp(const float* __restrict__ wreg, const 
             const float4 x0 = *reinterpret_cast<const float4*>(xs + g * XLD + k);
             const float4 x1 = *reinterpret_cast<const float4*>(xs + g * XLD + k + 4);
             float2 a = p0[g], c = p1[g];
-            a = __ffma2_rn(make_float2(x0.x, x0.y), make_float2(w0.x, w0.y), a);
-            c = __ffma2_rn(make_float2(x1.x, x1.y), make_float2(w1.x, w1.y), c);
-            a = __ffma2_rn(make_float2(x0.z, x0.w), make_float2(w0.z, w0.w), a);
-            c = __ffma2_rn(make_float2(x1.z, x1.w), make_float2(w1.z, w1.w), c);
+            a = ffma2(make_float2(x0.x, x0.y), make_float2(w0.x, w0.y), a);
+            c = ffma2(make_float2(x1.x, x1.y), make_float2(w1.x, w1.y), c);
+            a = ffma2(make_float2(x0.z, x0.w), make_float2(w0.z, w0.w), a);
+            c = ffma2(make_float2(x1.z, x1.w), make_float2(w1.z, w1.w), c);
             p0[g] = a; p1[g] = c;
         }
     }
@@ -248,10 +247,10 @@ __device__ __forceinline__ void gemv_warp32(const float* __restrict__ wreg, cons
         for (int g = 0; g < GT; ++g) {
             const float4 xv = *reinterpret_cast<const float4*>(xs + g * XLD + k);
             float2 a = pe[g], c = po[g];
-            a = __ffma2_rn(make_float2(xv.x, xv.y), make_float2(wa.x, wa.y), a);
-            c = __ffma2_rn(make_float2(xv.x, xv.y), make_float2(wb.x, wb.y), c);
-            a = __ffma2_rn(make_float2(xv.z, xv.w), make_float2(wa.z, wa.w), a);
-            c = __ffma2_rn(make_float2(xv.z, xv.w), make_float2(wb.z, wb.w), c);
+            a = ffma2(make_float2(xv.x, xv.y), make_float2(wa.x, wa.y), a);
+            c = ffma2(make_float2(xv.x, xv.y), make_float2(wb.x, wb.y), c);
+            a = ffma2(make_float2(xv.z, xv.w), make_float2(wa.z, wa.w), a);
+            c = ffma2(make_float2(xv.z, xv.w), make_float2(wb.z, wb.w), c);
             pe[g] = a; po[g] = c;
         }
     }
@@ -490,31 +489,18 @@ __device__ __forceinline__ void pre_row_of(const PreRows& r, int m, int& g, int&
 }
 __device__ __forceinline__ int pre_off_of(const PreRows& r, int g) { return r.n * __popc(r.mask & ((1u << g) - 1u)); }
 // address of W[k][n] (k = row within the layer's K) inside the ring; the layer's chunks occupy consecutive slots from pos0
-// ---- the pre-pass GEMM on the 5th-generation tensor cores ---------------------------------------------------------------
+// ---- the pre-pass GEMM on the tensor cores (wgmma) ---------------------------------------------------------------------
 // One utterance, <= 96 source rows.  A = the source rows as split-fp16 planes (hi = fp16(x), lo = fp16(x - hi)), staged per
 // 16-channel slab in the NO-SWIZZLE K-major core-matrix layout [k8][row][8 halfs]: rows are consecutive 16-byte chunks, so
 // the three taps of the dilated conv are the SAME slab read through descriptors whose start address is shifted by
 // tap * rate rows -- staged once, multiplied three times.  B = this CTA's weight columns, pre-packed in the same layout
 // ([plane][k8][column][8 halfs], 2 KB per 16-k slab) and streamed through the ring like the fp32 weights.  D = 128 x ns fp32
-// in tensor memory; per slab and tap hi*Whi + hi*Wlo + lo*Whi (the dropped lo*lo term is 2^-22 relative).
-__device__ __forceinline__ uint64_t umma_desc_noswz(uint32_t addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((addr & 0x3FFFF) >> 4);
-    d |= static_cast<uint64_t>(lbo_bytes >> 4) << 16;               // between the two 8-wide k groups of one MMA
-    d |= static_cast<uint64_t>(sbo_bytes >> 4) << 32;               // between 8-row groups
-    d |= 1ull << 46;                                                // descriptor version (sm_100); layout type 0 = no swizzle
-    return d;
-}
+// in the registers of warpgroup 1 (two M = 64 halves); per slab and tap hi*Whi + hi*Wlo + lo*Whi (the dropped lo*lo term is
+// 2^-22 relative).
 constexpr int TC_LOADW = 3;                                         // warps 0..2 stage A (one thread per source row, <= 96 rows)
-constexpr int TC_NISS = 3;                                          // lane 0 of warps 3, 4, 5: one MMA issuer per split-fp16 product
-constexpr int TC_COLS = 128;                                        // tensor-memory columns: three 32-column accumulators (power of two)
-
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(smem_u32(bar)) : "memory");
-}
 
 // (descriptor start-address field, i.e. address >> 4) of every weight slab of block li, tap-major: S.tc_baddr[tap * nslab + ks].
-// One division chain per entry, computed by 96 threads in parallel, OFF the single-thread MMA issue paths.
+// One division chain per entry, computed by 96 threads in parallel, OFF the MMA issue path.
 __device__ __forceinline__ void pyr_tc_table(const DecParams& P, Smem& S, int li, unsigned pos0) {
     const DecLayer& l = P.L[li];
     const int nslab = l.cin / 16, spc = l.krows / 16, spr = spc / 8, slab_f = 16 * l.ns;
@@ -525,23 +511,77 @@ __device__ __forceinline__ void pyr_tc_table(const DecParams& P, Smem& S, int li
     }
 }
 
-// The slab pipeline has no block barrier.  Loader warps fill stage s and arrive on abar[s].  THREE issuer threads (in three
-// warps, so on three schedulers) wait for abar[s]; issuer i issues product i of the split-fp16 scheme for every tap --
-// 0: hi x Whi, 1: hi x Wlo, 2: lo x Whi -- into ITS OWN 32-column accumulator and commits to sbar[s] (count 3), which the
-// loaders wait for before they overwrite the stage.  One thread issuing all nine MMAs of a slab was the bottleneck of the
-// whole pre-pass (ncu: the loaders spent their time waiting for the stage to be released).  Slabs are numbered through the
-// whole launch (st.tcq): slab q lives in stage q % TC_NSTG and is that stage's (q / TC_NSTG)-th use, which gives every wait
-// its phase parity without any shared counter.
-__device__ __forceinline__ void pyr_tc_utt(const DecParams& P, Smem& S, int li, unsigned q0, unsigned acc_use, int b, int t_lo, int n_out,
+// warpgroup 1: the MMAs of every slab and tap into acc[row half], then the scaled, biased rows -> scratch
+template <int NS>
+__device__ __forceinline__ void pyr_mma_rows(const DecParams& P, Smem& S, int li, unsigned& use, int& stg, int n_out, int rank,
+                                             float* scr_rows) {
+    const DecLayer& l = P.L[li];
+    const int nslab = l.cin / 16, lane = threadIdx.x & 31, w4 = (threadIdx.x >> 5) & 3;
+    unsigned char* As = reinterpret_cast<unsigned char*>(S.wrk);
+    const uint64_t dA0 = gmma_desc_noswz(0, TC_RA * 16, 128), dB0 = gmma_desc_noswz(0, (uint32_t)NS * 16, 128);
+    const uint32_t a_base = (smem_u32(As) & 0x3FFFFu) >> 4, b_lo = (uint32_t)NS * 2, tap_step = (uint32_t)l.rate;
+    float acc[2][NS / 2];
+#pragma unroll
+    for (int m = 0; m < 2; ++m)
+#pragma unroll
+        for (int i = 0; i < NS / 2; ++i) acc[m][i] = 0.f;
+#pragma unroll 1
+    for (int ks = 0; ks < nslab; ++ks) {
+        mbar_wait(bar64(&S.abar[stg]), use & 1u);                     // the slab is staged (all loader warps arrived)
+        uint32_t aa = a_base + (uint32_t)stg * (TC_ASTAGE >> 4);
+        const uint32_t* bt = &S.tc_baddr[ks];
+        wg_fence();
+#pragma unroll 1
+        for (int tap = 0; tap < l.ntaps; ++tap, aa += tap_step, bt += nslab) {
+            const uint64_t db_hi = dB0 | *bt, db_lo = dB0 | (*bt + b_lo);
+#pragma unroll
+            for (int m = 0; m < 2; ++m) {                             // rows 64 m .. 64 m + 63: 64 rows of 16 bytes further
+                const uint64_t da_hi = dA0 | (aa + 64u * m), da_lo = dA0 | (aa + 64u * m + (TC_APLANE >> 4));
+                wgmma_f16<NS / 16>(acc[m], da_hi, db_hi, (ks | tap) != 0);
+                wgmma_f16<NS / 16>(acc[m], da_hi, db_lo, 1u);
+                wgmma_f16<NS / 16>(acc[m], da_lo, db_hi, 1u);
+            }
+        }
+        wg_commit();
+        wg_wait<0>();
+        wg_fence_regs(acc[0]); wg_fence_regs(acc[1]);
+        if ((threadIdx.x & 127) == 0) mbar_arrive(bar64(&S.sbar[stg]));   // the loaders may overwrite the stage
+        if (++stg == TC_NSTG) { stg = 0; ++use; }
+    }
+    const float inv = P.inv_scale[li];
+    const float* bs = P.bias[li];
+#pragma unroll
+    for (int m = 0; m < 2; ++m)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = 64 * m + 16 * w4 + (lane >> 2) + 8 * h;
+            if (row >= n_out) continue;
+            float* orow = scr_rows + (size_t)row * 512;
+#pragma unroll
+            for (int i = 0; i < NS / 8; ++i) {
+                // hc: columns [0,16) gate, [16,32) info of channels rank*16..; conv: [0,16)
+                const int n = i * 8 + 2 * (lane & 3), hf = n >> 4, nn = n & 15;
+                const int col = hf * 256 + rank * 16 + nn, bi = hf * l.cout + rank * 16 + nn;
+                const float2 bq = __ldg(reinterpret_cast<const float2*>(bs + bi));
+                *reinterpret_cast<float2*>(orow + col) = make_float2(fmaf(acc[m][i * 4 + 2 * h], inv, bq.x),
+                                                                     fmaf(acc[m][i * 4 + 2 * h + 1], inv, bq.y));
+            }
+        }
+}
+
+// The slab pipeline has no block barrier.  Loader warps fill stage s and arrive on abar[s]; warpgroup 1 waits for abar[s],
+// issues the split-fp16 products of every tap and releases the stage through sbar[s], which the loaders wait for before
+// they overwrite it.  Slabs are numbered through the whole launch (st.tcq): slab q lives in stage q % TC_NSTG and is that
+// stage's (q / TC_NSTG)-th use, which gives every wait its phase parity without any shared counter.
+__device__ __forceinline__ void pyr_tc_utt(const DecParams& P, Smem& S, int li, unsigned q0, int b, int t_lo, int n_out,
                                         int rank, float* scr_rows) {
     const DecLayer& l = P.L[li];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int halo = (l.ntaps - 1) * l.rate, n_src = n_out + halo;   // <= 96
-    const int nslab = l.cin / 16, ns = l.ns;
+    const int nslab = l.cin / 16;
     unsigned char* As = reinterpret_cast<unsigned char*>(S.wrk);
     unsigned use = q0 / TC_NSTG;
     int stg = (int)(q0 - use * TC_NSTG);
-    const uint32_t tacc = S.tmem_base;
     if (warp < TC_LOADW) {
         const bool loader = tid < n_src;
         const int t_src = t_lo - halo + tid;
@@ -587,79 +627,11 @@ __device__ __forceinline__ void pyr_tc_utt(const DecParams& P, Smem& S, int li, 
                 }
             }
         }
-    } else if (warp < TC_LOADW + TC_NISS && lane == 0) {
-        const int prod = warp - TC_LOADW;                            // 0: hi x Whi, 1: hi x Wlo, 2: lo x Whi
-        const uint32_t idesc = umma_idesc_f16(128, (uint32_t)ns);
-        const uint64_t dA0 = umma_desc_noswz(0, TC_RA * 16, 128), dB0 = umma_desc_noswz(0, (uint32_t)ns * 16, 128);
-        const uint32_t a_base = ((smem_u32(As) & 0x3FFFFu) >> 4) + (prod == 2 ? (TC_APLANE >> 4) : 0u);
-        const uint32_t b_plane = prod == 1 ? (uint32_t)ns * 2 : 0u, tap_step = (uint32_t)l.rate;
-        const uint32_t dacc = tacc + (uint32_t)prod * 32u;
-        const int ntaps = l.ntaps;
-#pragma unroll 1
-        for (int ks = 0; ks < nslab; ++ks) {
-            mbar_wait(bar64(&S.abar[stg]), use & 1u);                 // the slab is staged (all loader warps arrived)
-            tc_fence_after();
-            uint32_t aa = a_base + (uint32_t)stg * (TC_ASTAGE >> 4);
-            const uint32_t* bt = &S.tc_baddr[ks];
-#pragma unroll 1
-            for (int tap = 0; tap < ntaps; ++tap, aa += tap_step, bt += nslab)
-                tc_mma_f16(dacc, dA0 | aa, dB0 | (*bt + b_plane), idesc, (ks | tap) != 0);
-            tc_commit(bar64(&S.sbar[stg]));                           // the stage may be overwritten once all three issuers' MMAs have read it
-            if (++stg == TC_NSTG) { stg = 0; ++use; }
-        }
-        tc_commit(bar64(&S.dbar));                                    // this product's accumulator is complete
+    } else if (warp >= 4) {
+        if (l.ns == 32) pyr_mma_rows<32>(P, S, li, use, stg, n_out, rank, scr_rows);
+        else pyr_mma_rows<16>(P, S, li, use, stg, n_out, rank, scr_rows);
     }
-    // epilogue: thread == output row (TMEM lane); the three partial accumulators summed, scaled, + bias -> scratch
-    if (warp < 4) {
-        mbar_wait(bar64(&S.dbar), acc_use & 1u);
-        tc_fence_after();
-        const int m = tid;
-        const uint32_t taddr = tacc + ((uint32_t)(warp * 32) << 16);
-        const float inv = P.inv_scale[li];
-        float v[32];
-        if (ns == 32) {
-            float w[32];
-            tmem_ld32_nowait(taddr, v); tmem_ld32_nowait(taddr + 32, w); tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] += w[i];
-            tmem_ld32_nowait(taddr + 64, w); tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] += w[i];
-        } else {
-            float w16[16], x16[16];
-            tmem_ld16(taddr, w16); tmem_ld16(taddr + 32, x16);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] = w16[i] + x16[i];
-            tmem_ld16(taddr + 64, x16);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] += x16[i];
-        }
-        if (m < n_out) {
-            float* orow = scr_rows + (size_t)m * 512;
-            const float* bs = P.bias[li];
-            if (l.kind == 1) {                                        // columns [0,16) gate, [16,32) info of channels rank*16..
-#pragma unroll
-                for (int hf = 0; hf < 2; ++hf)
-#pragma unroll
-                    for (int q4 = 0; q4 < 4; ++q4) {
-                        const int n = hf * 16 + q4 * 4, col = hf * 256 + rank * 16 + q4 * 4;
-                        const float4 bq = __ldg(reinterpret_cast<const float4*>(bs + hf * l.cout + rank * 16 + q4 * 4));
-                        *reinterpret_cast<float4*>(orow + col) = make_float4(fmaf(v[n], inv, bq.x), fmaf(v[n + 1], inv, bq.y),
-                                                                             fmaf(v[n + 2], inv, bq.z), fmaf(v[n + 3], inv, bq.w));
-                    }
-            } else {
-#pragma unroll
-                for (int q4 = 0; q4 < 4; ++q4) {
-                    const int col = rank * 16 + q4 * 4;
-                    const float4 bq = __ldg(reinterpret_cast<const float4*>(bs + col));
-                    *reinterpret_cast<float4*>(orow + col) = make_float4(fmaf(v[q4 * 4], inv, bq.x), fmaf(v[q4 * 4 + 1], inv, bq.y),
-                                                                         fmaf(v[q4 * 4 + 2], inv, bq.z), fmaf(v[q4 * 4 + 3], inv, bq.w));
-                }
-            }
-        }
-        tc_fence_before();
-    }
-    __syncthreads();                                                  // the accumulators have been read: the next utterance may overwrite them
+    __syncthreads();                                                  // every stage of this utterance is released and its rows stored
 }
 
 // LayerNorm / gate / highway mix of the refreshed rows: one warp per row over the whole cluster (parameters in S.red)
@@ -749,8 +721,8 @@ __device__ __noinline__ Stream prepass(const DecParams& P, Smem& S, Stream st, i
                     for (int g = 0; g < G; ++g) {
                         if (!((rl.mask >> g) & 1u)) continue;
                         float* rows = scr + (size_t)pre_off_of(rl, g) * 512;
-                        pyr_tc_utt(P, S, lp, st.tcq, st.tca, b0 + g, rl.t_lo, rl.n, rank, rows);
-                        st.tcq += l.cin / 16; st.tca++;
+                        pyr_tc_utt(P, S, lp, st.tcq, b0 + g, rl.t_lo, rl.n, rank, rows);
+                        st.tcq += l.cin / 16;
                     }
                 }
                 __syncthreads();                          // every warp is done with every region of these chunks
@@ -794,11 +766,9 @@ decode_cluster_kernel(const __grid_constant__ DecParams Pc) {
         for (int s = 0; s < DEC_NSLOT; ++s)
             for (int w = 0; w < NWARP; ++w) mbar_init(bar64(&S.fullw[s][w]), 1);
         mbar_init(bar64(&S.gbar[0]), 1); mbar_init(bar64(&S.gbar[1]), 1);
-        for (int i = 0; i < TC_NSTG; ++i) { mbar_init(bar64(&S.sbar[i]), TC_NISS); mbar_init(bar64(&S.abar[i]), TC_LOADW); }
-        mbar_init(bar64(&S.dbar), TC_NISS);
+        for (int i = 0; i < TC_NSTG; ++i) { mbar_init(bar64(&S.sbar[i]), 1); mbar_init(bar64(&S.abar[i]), TC_LOADW); }
         fence_mbar_init();
     }
-    if (warp == 0) tmem_alloc<TC_COLS>(&S.tmem_base);          // 128 lanes x 32 fp32 columns: the pre-pass accumulator
     for (int i = tid; i < 2 * GMAX * XLD; i += NT) (&S.xin[0][0][0])[i] = 0.f;
     for (int i = tid; i < 2 * NC * PLD; i += NT) (&S.pre[0][0][0])[i] = 0.f;
     if (tid < GMAX) { S.p_cur[tid] = 0; S.p_prev[tid] = 0; S.p_next[tid] = 0; S.moved[tid] = 0; }
@@ -809,7 +779,7 @@ decode_cluster_kernel(const __grid_constant__ DecParams Pc) {
 
     Stream st;
     st.base = P.wstream + (size_t)rank * P.stream_len;
-    st.prod = Cur{0, 0, 0}; st.pos = 0; st.tcq = 0; st.tca = 0;
+    st.prod = Cur{0, 0, 0}; st.pos = 0; st.tcq = 0;
     for (int s = 0; s < DEC_NSLOT; ++s) {                // the first chunks are AudioEnc chunks of frame 0 (nch_enc > DEC_NSLOT)
         if (lane == 0) stream_issue(P, S, st, st.prod, s, warp);
         cur_next(P, S, st.prod);
@@ -820,7 +790,7 @@ decode_cluster_kernel(const __grid_constant__ DecParams Pc) {
 
     int cb = 0;
     unsigned lcount = 0;
-    tc_fence_before(); __syncthreads(); tc_fence_after();
+    __syncthreads();
     if (tid == 0) S.prof_last = clock64();
     for (int j = 0; j < P.steps; ++j) {
         if (tid < GMAX) S.moved[tid] = (tid < G && j > 0 && S.p_cur[tid] != S.p_prev[tid]) ? 1 : 0;
@@ -867,7 +837,6 @@ decode_cluster_kernel(const __grid_constant__ DecParams Pc) {
     if (PROF && P.prof && cluster == 0 && rank == 0 && tid < 16) P.prof[tid] = S.prof[tid];
     cp_async_wait<0>();
     cluster_sync_all();                                   // no CTA exits while a peer may still write into its shared memory
-    if (warp == 0) tmem_dealloc<TC_COLS>(S.tmem_base);
 }
 
 size_t decode_smem_bytes() { return sizeof(Smem) + 128; }

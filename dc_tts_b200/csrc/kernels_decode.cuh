@@ -9,7 +9,7 @@
 namespace dctts {
 
 constexpr int DEC_NC = 16;          // CTAs per cluster (non-portable cluster size)
-constexpr int DEC_GMAX = 5;         // utterances per cluster (7 clusters of 16 CTAs are co-resident on a B200: 35 >= the benchmark's 32)
+constexpr int DEC_GMAX = 5;         // utterances per cluster (the benchmark's 32 utterances need 7 co-resident 16-CTA clusters)
 constexpr int DEC_THREADS = 256;
 constexpr int DEC_NSLOT = 3;        // ring slots
 constexpr int DEC_REG_F = 1536;     // floats per warp region of a slot (6 KB): every warp streams and frees its own k-rows
@@ -48,7 +48,7 @@ struct DecParams {
     float* pre_scr;                    // [clusters][G * max prow][512] pre-LN scratch of the recompute path
     int* p_hist;                       // (B, T) window used at every step
     int* p_final;                      // (B) window after the last step
-    float inv_scale[DEC_MAXL];         // 1 / (power-of-two scale of the block's split-fp16 weight planes), tcgen05 pre-pass
+    float inv_scale[DEC_MAXL];         // 1 / (power-of-two scale of the block's split-fp16 weight planes), tensor-core pre-pass
     int* stats;                        // [clusters][2]: frames with a window move, utterance-frames recomputed
     long long* prof;                   // optional [16] SM-clock lap timers of cluster 0 / rank 0 (option decode_prof), else nullptr
     int nl, n_enc, nch, nch_enc, pyr_ch0, pyr_ch1, stream_len;   // pyr_ch0..pyr_ch1: chunks of the AudioDec blocks with prow > 1

@@ -5,10 +5,10 @@
 //   forward / data gradient (mode 0):  Y[b,t,n] (+)= bias[n] + sum_tap sum_k X[b, t+shift_tap, k] W_tap[k][n]
 //   weight gradient        (mode 1):  dW[tap][k][n] += sum_b sum_t X[b, t+shift_tap, k] dY[b,t,n]
 //
-// fp32 operands cannot feed tcgen05 directly, and bf16 / single fp16 operands miss the gradient-parity budget, so every
+// fp32 operands cannot feed the tensor cores directly, and bf16 / single fp16 operands miss the gradient-parity budget, so every
 // operand is first written as two fp16 planes hi = fp16(s x), lo = fp16(s x - hi) with a per-tensor power-of-two scale s
 // (the largest magnitude lands in [2^13, 2^14): gradients of 1e-7 and weights of 1e-2 both use fp16's normal range), and
-// each k-step issues hi*hi + hi*lo + lo*hi into one fp32 accumulator in tensor memory -- the scheme of the synthesis
+// each k-step issues hi*hi + hi*lo + lo*hi into one fp32 accumulator -- the scheme of the synthesis
 // kernels (kernels_tc.cuh).  The planes are laid out so that BOTH operands of all three GEMMs are K-major tiles that TMA
 // delivers in the 64-byte swizzle, the reduction index being contiguous:
 //   mode 0: A = activation planes (B, L, C) box {32 ch, 128 t, 1 b}: the conv tap is the box's time coordinate and TMA's
@@ -16,9 +16,9 @@
 //   mode 1: A = TRANSPOSED activation planes (tap, B, C, L) box {32 t, 128 k, 1 b} (one pre-shifted copy per tap), B = transposed
 //           gradient planes (B, N, L) box {32 t, bn n, 1 b}; the reduction runs over (b, t-block), split over CTAs, and the
 //           partial tiles are added to dW with vector reductions (red.global.add.v4.f32).
-// One 128 x bn accumulator tile per CTA (bn <= 256), 32-wide slabs, two pipeline stages: ~97 KB of shared memory and 256
-// TMEM columns, so two CTAs share an SM and one tile's epilogue runs under the other's main loop (the arrangement measured
-// best for conv_ln_tc_kernel, DESIGN.md section 5).  Warp 0 = TMA producer, warp 1 = MMA issuer, warps 2-5 = epilogue.
+// One 128 x bn accumulator tile per CTA (bn <= 256), 32-wide slabs, up to four pipeline stages.  Warp 0 = TMA producer,
+// warpgroups 1 and 2 = wgmma consumers of rows 0-63 / 64-127 (fp32 register accumulators), which then write the tile to
+// shared memory (over the drained ring) and store it one row per thread, each warpgroup half of the columns.
 #include "kernels.cuh"
 #include "kernels_tc.cuh"
 #include "tc_ptx.cuh"
@@ -32,7 +32,7 @@ using namespace ptx;
 
 namespace {
 
-constexpr int G_BM = 128, G_BK = 32, G_THREADS = 192, G_TMEM_COLS = 256, G_MAX_STAGES = 4;
+constexpr int G_BM = 128, G_BK = 32, G_THREADS = 384, G_MAX_STAGES = 4;
 constexpr int G_SW = G_BK * 2;                         // bytes per tile row = swizzle span (64)
 constexpr int G_APLANE = G_BM * G_SW;                  // one plane of the A tile (8 KB)
 constexpr int G_AUX = 256;
@@ -61,22 +61,26 @@ struct GemmTcArgs {
     int probe;                // measurement only: 1 = the operands are fetched but no MMA is issued and nothing is stored
 };
 
-__device__ __forceinline__ void mbar_arrive_local(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(smem_u32(bar)) : "memory");
+__host__ __device__ inline int g_acc_ld(int bn) { return bn + 4; }
+// ring of `stages` stages, reused after the main loop for the 128 x (bn + 4) fp32 accumulator tile
+__host__ __device__ inline int g_ring_bytes(int stages, int bn) {
+    const int ring = stages * (2 * G_APLANE + 2 * bn * G_SW) + 64 * G_SW;      // a 64-column wgmma past bn reads <= 48 rows more
+    const int acc = G_BM * g_acc_ld(bn) * 4;
+    return ((ring > acc ? ring : acc) + 1023) & ~1023;
 }
 
-__global__ void __launch_bounds__(G_THREADS)
+__global__ void __launch_bounds__(G_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constant__ CUtensorMap mapA_lo,
                const __grid_constant__ CUtensorMap mapB_hi, const __grid_constant__ CUtensorMap mapB_lo, const GemmTcArgs a) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
     const int bn = a.bn, b_plane = bn * G_SW, stage_bytes = 2 * G_APLANE + 2 * b_plane, stages = a.stages;
-    uint8_t* aux = smem + (size_t)stages * stage_bytes;
+    const int acc_ld = g_acc_ld(bn);
+    float* s_acc = reinterpret_cast<float*>(smem);
+    uint8_t* aux = smem + g_ring_bytes(stages, bn);
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(aux);
     uint64_t* empty_bar = full_bar + G_MAX_STAGES;
-    uint64_t* tmem_full_bar = empty_bar + G_MAX_STAGES;
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
 
     // ---- tile coordinates and the reduction schedule ----
     const int n0 = blockIdx.x * bn;
@@ -94,15 +98,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
 
     if (warp == 0 && lane == 0) {
         prefetch_tmap(&mapA_hi); prefetch_tmap(&mapA_lo); prefetch_tmap(&mapB_hi); prefetch_tmap(&mapB_lo);
-        for (int s = 0; s < stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        mbar_init(tmem_full_bar, 1);
+        for (int s = 0; s < stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }   // one release per consumer warpgroup
         fence_mbar_init();
     }
-    if (warp == 1) tmem_alloc<G_TMEM_COLS>(tmem_ptr_smem);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
 
     if (warp == 0) {
         // =========================== TMA producer ===========================
@@ -128,100 +127,106 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
             }
         }
         __syncwarp();
-    } else if (warp == 1) {
-        // =========================== MMA issuer ===========================
-        const uint32_t idesc = umma_idesc_f16(G_BM, (uint32_t)bn);
-        for (int kb = 0; kb < nkb; ++kb) {
-            const int s = kb % stages;
-            mbar_wait(&full_bar[s], ((uint32_t)(kb / stages)) & 1u);
-            tc_fence_after();
-            if (lane == 0 && a.probe) {                             // ingest probe: release the stage at once
-                mbar_arrive_local(&empty_bar[s]);
-                if (kb == nkb - 1) mbar_arrive_local(tmem_full_bar);
-            } else if (lane == 0) {
-                const uint32_t st = smem_u32(smem + (size_t)s * stage_bytes);
-                const uint64_t dA_hi = umma_desc_kmajor<G_SW>(st), dA_lo = umma_desc_kmajor<G_SW>(st + G_APLANE);
-                const uint64_t dB_hi = umma_desc_kmajor<G_SW>(st + 2 * G_APLANE), dB_lo = umma_desc_kmajor<G_SW>(st + 2 * G_APLANE + b_plane);
+        return;
+    }
+    if (wg == 0) return;                                            // warps 1-3: no role
+    // =========================== wgmma consumers: rows 64 * (wg - 1) .. +64 ===========================
+    const int mh = wg - 1;
+    float acc[4][32];
 #pragma unroll
-                for (int k = 0; k < G_BK / 16; ++k) {
-                    const uint64_t adv = (uint64_t)(k * 32 >> 4);          // 16 fp16 = 32 bytes inside the swizzle atom
-                    tc_mma_f16(tmem_base, dA_hi + adv, dB_hi + adv, idesc, (kb | k) != 0);
-                    tc_mma_f16(tmem_base, dA_hi + adv, dB_lo + adv, idesc, 1u);
-                    tc_mma_f16(tmem_base, dA_lo + adv, dB_hi + adv, idesc, 1u);
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc[j][i] = 0.f;
+    for (int kb = 0; kb < nkb; ++kb) {
+        const int s = kb % stages;
+        mbar_wait(&full_bar[s], ((uint32_t)(kb / stages)) & 1u);
+        if (!a.probe) {
+            const uint32_t st = smem_u32(smem + (size_t)s * stage_bytes);
+            const uint64_t dA_hi = gmma_desc_kmajor<G_SW>(st + mh * 64 * G_SW), dA_lo = gmma_desc_kmajor<G_SW>(st + G_APLANE + mh * 64 * G_SW);
+            const uint64_t dB_hi = gmma_desc_kmajor<G_SW>(st + 2 * G_APLANE), dB_lo = gmma_desc_kmajor<G_SW>(st + 2 * G_APLANE + b_plane);
+            wg_fence();
+#pragma unroll
+            for (int k = 0; k < G_BK / 16; ++k) {
+                const uint64_t adv = (uint64_t)(k * 32 >> 4);          // 16 fp16 = 32 bytes inside the swizzle atom
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    if (j * 64 < bn) {
+                        const uint64_t cb = (uint64_t)((j * 64 * G_SW) >> 4);
+                        wgmma_split3(acc[j], min(64, bn - j * 64), dA_hi + adv, dA_lo + adv, dB_hi + cb + adv, dB_lo + cb + adv,
+                                     (kb | k) != 0);
+                    }
                 }
-                tc_commit(&empty_bar[s]);
-                if (kb == nkb - 1) tc_commit(tmem_full_bar);
             }
-            __syncwarp();
+            wg_commit();
+            wg_wait<0>();
+#pragma unroll
+            for (int j = 0; j < 4; ++j) wg_fence_regs(acc[j]);
+        }
+        if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[s]);     // stage drained (ingest probe: at once)
+    }
+    if (a.probe) return;
+    named_sync(1, 256);                                             // both halves done reading the ring: it becomes the tile
+    {
+        const int r0 = mh * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+#pragma unroll
+            for (int i8 = 0; i8 < 8; ++i8) {
+                const int col = j * 64 + i8 * 8 + 2 * (lane & 3);
+                if (col < bn) {
+                    *reinterpret_cast<float2*>(s_acc + (size_t)r0 * acc_ld + col) = make_float2(acc[j][i8 * 4], acc[j][i8 * 4 + 1]);
+                    *reinterpret_cast<float2*>(s_acc + (size_t)(r0 + 8) * acc_ld + col) = make_float2(acc[j][i8 * 4 + 2], acc[j][i8 * 4 + 3]);
+                }
+            }
+    }
+    named_sync(1, 256);
+    // =========================== epilogue: thread == accumulator row (both warpgroups, half the columns each) ===========================
+    const int r = threadIdx.x & 127;
+    const float* arow = s_acc + (size_t)r * acc_ld;
+    const int c_beg = mh == 0 ? 0 : ((bn / 2 + 31) & ~31), c_end = mh == 0 ? ((bn / 2 + 31) & ~31) : bn;
+    const float inv = 1.0f / (slot_scale(a.slot_a) * slot_scale(a.slot_b));      // both powers of two: exact
+    if (a.mode == 0) {
+        const int t = t0 + r;
+        if (t < a.L) {
+            float* yrow = a.Y + ((size_t)b0 * a.Lout + t) * a.ldy;
+            for (int c = c_beg; c < c_end; c += 4) {
+                const int n = n0 + c;
+                const float4 v = *reinterpret_cast<const float4*>(arow + c);
+                if (n + 3 < a.N) {
+                    const float4 bq = __ldg(reinterpret_cast<const float4*>(a.bias + n));
+                    float4 o = make_float4(fmaf(v.x, inv, bq.x), fmaf(v.y, inv, bq.y), fmaf(v.z, inv, bq.z), fmaf(v.w, inv, bq.w));
+                    float4* p = reinterpret_cast<float4*>(yrow + n);
+                    if (a.accumulate) { const float4 y = *p; o.x += y.x; o.y += y.y; o.z += y.z; o.w += y.w; }
+                    *p = o;
+                } else {
+                    const float vv[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+                    for (int e = 0; e < 4; ++e)
+                        if (n + e < a.N) {
+                            const float o = fmaf(vv[e], inv, __ldg(a.bias + n + e));
+                            yrow[n + e] = a.accumulate ? yrow[n + e] + o : o;
+                        }
+                }
+            }
         }
     } else {
-        // =========================== epilogue: thread == accumulator row ===========================
-        // (a per-warp shared-memory transpose that writes whole 128-byte row segments was measured SLOWER than these
-        // row-scattered 16-byte stores / vector reductions: 105 vs 57 us on the (2, 64) forward launches)
-        const int q = warp & 3, r = q * 32 + lane;
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
-        const float inv = 1.0f / (slot_scale(a.slot_a) * slot_scale(a.slot_b));      // both powers of two: exact
-        mbar_wait(tmem_full_bar, 0);
-        tc_fence_after();
-        if (a.probe) {
-        } else if (a.mode == 0) {
-            const int t = t0 + r;
-            const bool ok = t < a.L;
-            float* yrow = a.Y + ((size_t)b0 * a.Lout + (ok ? t : 0)) * a.ldy;
-            for (int c = 0; c < bn; c += 32) {
-                float v[32];
-                __syncwarp();                                       // tcgen05.ld is warp-collective: converge before it
-                tmem_ld32_nowait(taddr + c, v);
-                tmem_ld_wait();
-                if (ok) {
+        const int k = m0 + r;
+        if (k < a.K) {
+            float* wrow = a.dW + (size_t)tap * a.tap_stride + (size_t)k * a.ldw;
+            for (int c = c_beg; c < c_end; c += 4) {
+                const int n = n0 + c;
+                const float4 v = *reinterpret_cast<const float4*>(arow + c);
+                if (n + 3 < a.N) {
+                    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};"
+                                 :: "l"(wrow + n), "f"(v.x * inv), "f"(v.y * inv), "f"(v.z * inv), "f"(v.w * inv) : "memory");
+                } else {
+                    const float vv[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
-                    for (int i = 0; i < 32; i += 4) {
-                        const int n = n0 + c + i;
-                        if (n + 3 < a.N) {
-                            const float4 bq = __ldg(reinterpret_cast<const float4*>(a.bias + n));
-                            float4 o = make_float4(fmaf(v[i], inv, bq.x), fmaf(v[i + 1], inv, bq.y), fmaf(v[i + 2], inv, bq.z), fmaf(v[i + 3], inv, bq.w));
-                            float4* p = reinterpret_cast<float4*>(yrow + n);
-                            if (a.accumulate) { const float4 y = *p; o.x += y.x; o.y += y.y; o.z += y.z; o.w += y.w; }
-                            *p = o;
-                        } else {
-#pragma unroll
-                            for (int e = 0; e < 4; ++e)
-                                if (n + e < a.N) {
-                                    const float o = fmaf(v[i + e], inv, __ldg(a.bias + n + e));
-                                    yrow[n + e] = a.accumulate ? yrow[n + e] + o : o;
-                                }
-                        }
-                    }
-                }
-            }
-        } else {
-            const int k = m0 + r;
-            const bool ok = k < a.K;
-            float* wrow = a.dW + (size_t)tap * a.tap_stride + (size_t)(ok ? k : 0) * a.ldw;
-            for (int c = 0; c < bn; c += 32) {
-                float v[32];
-                __syncwarp();
-                tmem_ld32_nowait(taddr + c, v);
-                tmem_ld_wait();
-                if (ok) {
-#pragma unroll
-                    for (int i = 0; i < 32; i += 4) {
-                        const int n = n0 + c + i;
-                        if (n + 3 < a.N) {
-                            asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};"
-                                         :: "l"(wrow + n), "f"(v[i] * inv), "f"(v[i + 1] * inv), "f"(v[i + 2] * inv), "f"(v[i + 3] * inv) : "memory");
-                        } else {
-#pragma unroll
-                            for (int e = 0; e < 4; ++e) if (n + e < a.N) atomicAdd(wrow + n + e, v[i + e] * inv);
-                        }
-                    }
+                    for (int e = 0; e < 4; ++e) if (n + e < a.N) atomicAdd(wrow + n + e, vv[e] * inv);
                 }
             }
         }
-        tc_fence_before();
     }
-    __syncthreads();
-    if (warp == 1) { tc_fence_after(); tmem_dealloc<G_TMEM_COLS>(tmem_base); }
 }
 
 // ---- operand conversion ------------------------------------------------------------------------------------------------
@@ -386,12 +391,10 @@ int pick_bn(int N) { return std::min(256, roundup_i(N, 16)); }
 
 void launch_gemm(const CUtensorMap m[4], GemmTcArgs& a, dim3 grid, cudaStream_t s) {
     prepare_gemm_kernel();
-    const int stage = 2 * G_APLANE + 2 * a.bn * G_SW;
-    // two stages keep the CTA under half an SM's shared memory (two CTAs per SM: one tile's epilogue under the other's main
-    // loop); a launch that cannot give every SM two CTAs anyway takes a deeper ring instead
-    const long long ctas = (long long)grid.x * grid.y * grid.z;
-    a.stages = ctas > 148 ? 2 : std::min(G_MAX_STAGES, (200 * 1024) / stage);
-    const size_t smem = (size_t)a.stages * stage + G_AUX + 1024;
+    // the deepest ring (<= 4 stages) that fits beside nothing else: after the main loop the ring holds the fp32 tile
+    a.stages = G_MAX_STAGES;
+    while (a.stages > 2 && (size_t)g_ring_bytes(a.stages, a.bn) + G_AUX + 1024 > (size_t)227 * 1024) --a.stages;
+    const size_t smem = (size_t)g_ring_bytes(a.stages, a.bn) + G_AUX + 1024;
     gemm_tc_kernel<<<grid, G_THREADS, smem, s>>>(m[0], m[1], m[2], m[3], a);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) throw std::runtime_error(std::string("gemm_tc_kernel launch: ") + cudaGetErrorString(e));
@@ -485,7 +488,10 @@ int launch_conv_wgrad_tc(const WgradArgs& w, int B, GemmTcWs& ws, cudaStream_t s
     GemmTcArgs a{};
     a.mode = 1; a.bn = bn; a.N = w.N; a.K = w.K; a.B = B; a.tblocks = (L + G_BK - 1) / G_BK;
     const int base = n_tiles * k_tiles * w.ntaps;
-    int ksplit = std::max(1, std::min(B, (2 * 148 + base - 1) / base));
+    int dev = 0, sms = 132;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    int ksplit = std::max(1, std::min(B, (2 * sms + base - 1) / base));
     a.nb_per_split = (B + ksplit - 1) / ksplit;
     a.ksplit = (B + a.nb_per_split - 1) / a.nb_per_split;          // no empty split
     a.dW = w.dW; a.ldw = w.ldw; a.tap_stride = (long long)w.K * w.ldw;

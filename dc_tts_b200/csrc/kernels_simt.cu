@@ -1,4 +1,4 @@
-// kernels_simt.cu -- fp32 CUDA-core kernels of the DC-TTS synthesis path (sm_100a).
+// kernels_simt.cu -- fp32 CUDA-core kernels of the DC-TTS synthesis path (sm_90a).
 //
 // These are the exact-fp32 building blocks: an implicit-GEMM dilated/causal conv
 // (reference modules.py:121-134,173-187 and the stride-2 transposed conv :232-239 as

@@ -1,22 +1,22 @@
-// kernels_tc.cu -- tcgen05 / TMEM / TMA fused block kernel for sm_100a.
+// kernels_tc.cu -- wgmma / TMA fused block kernel for sm_90a.
 //
 // ONE kernel per reference block (modules.py:91-141 conv1d, :143-197 hc, :199-247
-// conv1d_transpose): the dilated / causal conv as an implicit GEMM on the 5th-generation
-// tensor cores, and the whole epilogue -- bias, LayerNorm (two of them for hc), relu /
-// sigmoid gate / highway mix -- applied to the accumulator straight out of tensor memory.
+// conv1d_transpose): the dilated / causal conv as an implicit GEMM on the Hopper tensor
+// cores, and the whole epilogue -- bias, LayerNorm (two of them for hc), relu / sigmoid
+// gate / highway mix -- applied to the accumulator tile.
 //
 //   grid    (ncta, tiles); a thread-block CLUSTER of `ncta` CTAs shares one 128-row tile and
 //           splits the output channels; LayerNorm statistics are combined across the
 //           cluster through distributed shared memory (Chan's parallel mean/M2 merge).
-//   warp 0  TMA producer: per k-block (64 channels of one tap) one {64 x 128 rows} box of
+//   warp 0  TMA producer: per k-block (BK channels of one tap) one {BK x 128 rows} box of
 //           each activation plane -- the tap's time shift is just the box coordinate, and
 //           TMA's out-of-bounds zero fill IS the reference's zero padding -- plus the
-//           {64 x bn} box of each weight plane, 128B-swizzled, mbarrier pipelined.
-//   warp 1  allocates TMEM and issues tcgen05.mma (kind::f16, M=128, N=bn, K=16):
-//           hi*Whi + hi*Wlo + lo*Whi per k-step into one fp32 accumulator.
-//   warps 2-5  epilogue: tcgen05.ld rows (thread == row, so LN reductions are thread-local),
-//           three sweeps over TMEM (sum, centred M2, normalise+store); TMEM re-reads are
-//           cheaper than holding 256 columns in registers.
+//           {BK x bn} box of each weight plane, swizzled, mbarrier pipelined.
+//   warpgroups 1, 2  wgmma (M=64 each, N=bn in chunks of <= 64, K=16):
+//           hi*Whi + hi*Wlo + lo*Whi per k-step into fp32 register accumulators, which
+//           then go to shared memory as one 128 x bn tile.
+//   warpgroup 1  epilogue: thread == row, so LN reductions are thread-local; one
+//           statistics sweep and one normalise+store sweep over the tile.
 #include "kernels_tc.cuh"
 #include "tc_ptx.cuh"
 
@@ -29,10 +29,10 @@ namespace dctts {
 using namespace ptx;
 
 constexpr int TC_BM = 128;
-constexpr int TC_THREADS = 192;
-constexpr int TC_TMEM_COLS = 256;
+constexpr int TC_THREADS = 384;
 constexpr int TC_MAX_STAGES = 8;
 constexpr int TC_AUX_BYTES = 256 /*barriers*/ + 3 * 512 * 4 /*bias,gamma,beta*/ + 128 * 16 /*this CTA's LN partials*/;
+constexpr int TC_MAX_SMEM = 227 * 1024;
 
 __device__ __forceinline__ float sigmoid_acc(float x) { return 1.0f / (1.0f + expf(-x)); }
 
@@ -78,12 +78,21 @@ __device__ __forceinline__ void store_planes(const Planes& p, size_t row, int co
     }
 }
 
-// MT = 128-row tiles per CTA (1 or 2).  With MT = 2 one weight slab feeds two accumulators, i.e. a
-// third fewer bytes per MMA through the SM's ~50 GB/s L2 port -- the measured limiter of this kernel.
-// CG = CTAs per MMA (tcgen05 cta_group): 1, or 2 = CTA pairs -- ranks (2s, 2s+1) of the cluster share channel slice s,
-// take two consecutive 128-row tiles, each loads HALF of the slice's weight slab, and the even CTA issues M = 256 MMAs
-// that fill both CTAs' tensor memory (512 columns each: the slice's gate half then its info half).
-template <int TC_BK, int MT, int CG>
+// Shared memory: [ring of `stages` stages | after the main loop: the 128 x (bn + 4) fp32 accumulator tile] [residual /
+// output staging tile (hc with resid_tma)] [barriers, epilogue vectors, LN partials].  The accumulator tile reuses the ring:
+// it is written only once every k-block has been multiplied, and every multicast box aimed at this CTA has landed by then
+// (each one completes on a full barrier that the consumers waited for).
+__host__ __device__ inline int tc_acc_ld(int bn) { return bn + 4; }                  // row pitch: float4 rows hit distinct banks
+__host__ __device__ inline int tc_ring_bytes(int stages, int stage_bytes, int bn, int sw) {
+    const int ring = stages * stage_bytes + 64 * sw;                                   // a 64-column wgmma past bn reads <= 48 rows more
+    const int acc = TC_BM * tc_acc_ld(bn) * 4;
+    return ((ring > acc ? ring : acc) + 1023) & ~1023;
+}
+__host__ __device__ inline int tc_resid_bytes(int resid_tma, int half) { return resid_tma ? 2 * (half / 64) * 16384 : 0; }
+
+// One 128-row tile per CTA, split over two consumer warpgroups (rows 0-63 / 64-127), each holding its 64 x bn accumulator in
+// registers (wgmma m64nNk16, N in chunks of <= 64 columns).
+template <int TC_BK>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constant__ CUtensorMap mapA_lo,
                   const __grid_constant__ CUtensorMap mapW_hi, const __grid_constant__ CUtensorMap mapW_lo,
@@ -95,87 +104,75 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
     pdl_launch_dependents();          // PDL: let the next kernel's CTAs be scheduled behind this one
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7;                                 // 0: producer warpgroup, 1 / 2: consumers of rows 0-63 / 64-127
+    const bool epi = wg == 1;                                        // the first consumer warpgroup also runs the epilogue
     if (threadIdx.x == 0) dbg_time(a.dbg, 8);                        // t0: kernel entry
-    static_assert(CG == 1 || (CG == 2 && MT == 1), "CTA pairs take one tile each");
-    const int crank = (int)cluster_ctarank();
+    const int rank = (int)cluster_ctarank();                         // channel slice of this CTA
     const int ncta = (int)cluster_nctarank();
-    const int rank = crank / CG;                                     // channel slice of this CTA
-    const int peer = crank % CG;                                     // position inside the CTA pair (0 = leader)
-    const int nslices = ncta / CG;
+    const int nslices = ncta;
     const int bn = a.bn, half = a.half;                              // accumulator columns per CTA / per LN half
     constexpr int TC_A_PLANE = TC_BM * TC_BK * 2;                    // bytes of one activation plane tile
     constexpr int SW = TC_BK * 2;                                    // swizzle span = row bytes (128 or 64)
-    const int bn_load = bn / CG;                                     // weight rows this CTA stages (a pair splits the slab)
-    const int b_plane = bn_load * SW;                                // bytes of one weight plane tile
-    constexpr int A_BYTES = MT * 2 * TC_A_PLANE;                     // hi+lo planes of MT tiles
+    const int b_plane = bn * SW;                                     // bytes of one weight plane tile
+    constexpr int A_BYTES = 2 * TC_A_PLANE;                          // hi+lo planes
     const int stage_bytes = A_BYTES + 2 * b_plane;
     const int stages = a.stages;
     const int nkb = a.ntaps * a.kb_per_tap;
+    const int acc_ld = tc_acc_ld(bn);
 
-    uint8_t* aux = smem + (size_t)stages * stage_bytes;
+    float* s_acc = reinterpret_cast<float*>(smem);
+    uint8_t* rs = smem + tc_ring_bytes(stages, stage_bytes, bn, SW);   // residual / output staging tile
+    uint8_t* aux = rs + tc_resid_bytes(a.resid_tma, half);
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(aux);              // [stages]
     uint64_t* empty_bar = full_bar + TC_MAX_STAGES;                      // [stages]
-    uint64_t* tmem_full_bar = empty_bar + TC_MAX_STAGES;
-    uint64_t* resid_bar = tmem_full_bar + 1;
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(resid_bar + 1);
+    uint64_t* resid_bar = empty_bar + TC_MAX_STAGES;
     float* s_bias = reinterpret_cast<float*>(aux + 256);
     float* s_gam = s_bias + 512;
     float* s_bet = s_gam + 512;
     float4* s_part = reinterpret_cast<float4*>(s_bet + 512);            // [128 rows]: this CTA's partial (sum, M2) x 2 halves, read by its peers
 
     pdl_wait();                       // upstream grid complete, its writes visible
-    // ---- tile coordinates (MT tiles per CTA; a tile index past the end loads zeros and stores nothing) ----
+    // ---- tile coordinates (a tile index past the end loads zeros and stores nothing) ----
     const int L = a.win.L;
     int t_end, t_lo;
     if (a.win.jptr) { t_end = __ldg(a.win.jptr); t_lo = max(0, t_end - a.win.R + 1); }
     else { t_end = L - 1; t_lo = 0; }
-    int b0s[MT], t0s[MT];
-#pragma unroll
-    for (int m = 0; m < MT; ++m) {
-        const int tile = (blockIdx.y * MT + m) * CG + peer;
+    int b0s, t0s;
+    {
+        const int tile = blockIdx.y;
         const int bg = tile / a.tiles_t, tt = tile - bg * a.tiles_t;
-        b0s[m] = (tile < a.ntiles) ? bg * a.TB : a.win.B;               // batch coordinate out of range -> TMA zero fill
-        t0s[m] = a.win.jptr ? (t_end - a.tiles_t * a.TT + 1 + tt * a.TT) : tt * a.TT;
+        b0s = (tile < a.ntiles) ? bg * a.TB : a.win.B;                  // batch coordinate out of range -> TMA zero fill
+        t0s = a.win.jptr ? (t_end - a.tiles_t * a.TT + 1 + tt * a.TT) : tt * a.TT;
     }
+    const bool mcast = a.mcast != 0 && ncta > 1;
 
     // ---- one-time setup ----
     if (warp == 0 && lane == 0) {
         prefetch_tmap(&mapA_hi); prefetch_tmap(&mapA_lo); prefetch_tmap(&mapW_hi); prefetch_tmap(&mapW_lo);
-        // with the multicast A tile a stage may only be refilled once EVERY CTA of the cluster has
-        // drained it: each MMA warp commits to all CTAs' empty barriers
-        for (int s = 0; s < stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], a.mcast ? (uint32_t)ncta : 1u); }
-        mbar_init(tmem_full_bar, 1); mbar_init(resid_bar, 1);
+        // each consumer warpgroup releases a stage once; with the multicast A tile a stage may only be refilled once EVERY
+        // CTA of the cluster has drained it, so the consumers arrive on all CTAs' empty barriers
+        for (int s = 0; s < stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], mcast ? 2u * (uint32_t)ncta : 2u); }
+        mbar_init(resid_bar, 1);
         fence_mbar_init();
     }
-    if (CG == 2) { cluster_arrive(); cluster_wait(); }      // the pair allocator needs both CTAs up
-    if (warp == 1) {
-        if (CG == 2) { if (bn > 256) tmem_alloc_pair<512>(tmem_ptr_smem); else tmem_alloc_pair<256>(tmem_ptr_smem); }
-        else tmem_alloc<MT * TC_TMEM_COLS>(tmem_ptr_smem);
-    }
-    if (warp >= 2) {
-        // epilogue vectors, indexed by accumulator column
-        for (int c = threadIdx.x - 64; c < bn; c += 128) {
-            float bi = 0.f, g = 0.f, be = 0.f;
-            if (a.mode == 0) {
-                int col = rank * bn + c;
-                if (col < a.C) { bi = a.bias[col]; g = a.g1[col]; be = a.b1[col]; }
-            } else {
-                int second = c >= half;
-                int col = rank * half + (second ? c - half : c);
-                bi = (a.mode == 1 && second) ? a.bias[a.C + col] : a.bias[col];
-                g = second ? a.g2[col] : a.g1[col];
-                be = second ? a.b2[col] : a.b1[col];
-            }
-            s_bias[c] = bi; s_gam[c] = g; s_bet[c] = be;
+    // epilogue vectors, indexed by accumulator column
+    for (int c = threadIdx.x; c < bn; c += TC_THREADS) {
+        float bi = 0.f, g = 0.f, be = 0.f;
+        if (a.mode == 0) {
+            int col = rank * bn + c;
+            if (col < a.C) { bi = a.bias[col]; g = a.g1[col]; be = a.b1[col]; }
+        } else {
+            int second = c >= half;
+            int col = rank * half + (second ? c - half : c);
+            bi = (a.mode == 1 && second) ? a.bias[a.C + col] : a.bias[col];
+            g = second ? a.g2[col] : a.g1[col];
+            be = second ? a.b2[col] : a.b1[col];
         }
+        s_bias[c] = bi; s_gam[c] = g; s_bet[c] = be;
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
-    if (threadIdx.x == 0) { dbg_mark(a.dbg, 0, 1); dbg_mark(a.dbg, 1, (int)tmem_base); dbg_mark(a.dbg, 2, nkb); dbg_time(a.dbg, 9); }   // t1: setup done
+    if (threadIdx.x == 0) { dbg_mark(a.dbg, 0, 1); dbg_mark(a.dbg, 2, nkb); dbg_time(a.dbg, 9); }   // t1: setup done
     if (ncta > 1) { cluster_arrive(); cluster_wait(); }   // phase 1: every CTA is running, its barriers initialised
-    const bool mcast = a.mcast != 0 && ncta > 1;
     const uint16_t cta_mask = (uint16_t)((1u << ncta) - 1u);
     const int slice_rows = TC_BM / ncta;
 
@@ -186,165 +183,136 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
                 const int s = kb % stages;
                 const uint32_t ph = (uint32_t)(kb / stages) & 1u;
                 mbar_wait(&empty_bar[s], ph ^ 1u);
-                if (CG == 1) mbar_expect_tx(&full_bar[s], (uint32_t)stage_bytes);
-                else if (peer == 0) mbar_expect_tx(&full_bar[s], 2u * (uint32_t)stage_bytes);   // both CTAs' bytes land on the leader's barrier
+                mbar_expect_tx(&full_bar[s], (uint32_t)stage_bytes);
                 uint8_t* st = smem + (size_t)s * stage_bytes;
                 const int tap = kb / a.kb_per_tap, kc = kb - tap * a.kb_per_tap;
-#pragma unroll
-                for (int m = 0; m < MT; ++m) {
-                    uint8_t* sa = st + m * 2 * TC_A_PLANE;
-                    const int tcoord = t0s[m] + a.shifts[tap];
-                    if (mcast) {
-                        // this CTA fetches rows [rank*slice, +slice) of the tile for the whole cluster
-                        const int off = rank * slice_rows * SW;
-                        tma_load_3d_mc(&mapA_hi, &full_bar[s], sa + off, kc * TC_BK, tcoord + rank * slice_rows, b0s[m], cta_mask);
-                        tma_load_3d_mc(&mapA_lo, &full_bar[s], sa + TC_A_PLANE + off, kc * TC_BK, tcoord + rank * slice_rows, b0s[m], cta_mask);
-                    } else if (CG == 2) {
-                        tma_load_3d_pair(&mapA_hi, &full_bar[s], sa, kc * TC_BK, tcoord, b0s[m]);
-                        tma_load_3d_pair(&mapA_lo, &full_bar[s], sa + TC_A_PLANE, kc * TC_BK, tcoord, b0s[m]);
-                    } else {
-                        tma_load_3d(&mapA_hi, &full_bar[s], sa, kc * TC_BK, tcoord, b0s[m]);
-                        tma_load_3d(&mapA_lo, &full_bar[s], sa + TC_A_PLANE, kc * TC_BK, tcoord, b0s[m]);
-                    }
-                }
-                if (CG == 2) {
-                    // this CTA's half/2 gate channels and the matching info channels: two boxes of the slab, which is
-                    // packed in 128-channel halves [gate 128 | info 128] (pack_tc)
-                    const int ch0 = rank * half + peer * (half / 2);
-                    const int g0 = (ch0 / 128) * 256 + (ch0 % 128);
-                    const int wbox_bytes = (half / 2) * SW;
-                    tma_load_2d_pair(&mapW_hi, &full_bar[s], st + A_BYTES, kb * TC_BK, g0);
-                    tma_load_2d_pair(&mapW_hi, &full_bar[s], st + A_BYTES + wbox_bytes, kb * TC_BK, g0 + 128);
-                    tma_load_2d_pair(&mapW_lo, &full_bar[s], st + A_BYTES + b_plane, kb * TC_BK, g0);
-                    tma_load_2d_pair(&mapW_lo, &full_bar[s], st + A_BYTES + b_plane + wbox_bytes, kb * TC_BK, g0 + 128);
+                const int tcoord = t0s + a.shifts[tap];
+                if (mcast) {
+                    // this CTA fetches rows [rank*slice, +slice) of the tile for the whole cluster
+                    const int off = rank * slice_rows * SW;
+                    tma_load_3d_mc(&mapA_hi, &full_bar[s], st + off, kc * TC_BK, tcoord + rank * slice_rows, b0s, cta_mask);
+                    tma_load_3d_mc(&mapA_lo, &full_bar[s], st + TC_A_PLANE + off, kc * TC_BK, tcoord + rank * slice_rows, b0s, cta_mask);
                 } else {
-                    tma_load_2d(&mapW_hi, &full_bar[s], st + A_BYTES, kb * TC_BK, rank * bn);
-                    tma_load_2d(&mapW_lo, &full_bar[s], st + A_BYTES + b_plane, kb * TC_BK, rank * bn);
+                    tma_load_3d(&mapA_hi, &full_bar[s], st, kc * TC_BK, tcoord, b0s);
+                    tma_load_3d(&mapA_lo, &full_bar[s], st + TC_A_PLANE, kc * TC_BK, tcoord, b0s);
                 }
+                tma_load_2d(&mapW_hi, &full_bar[s], st + A_BYTES, kb * TC_BK, rank * bn);
+                tma_load_2d(&mapW_lo, &full_bar[s], st + A_BYTES + b_plane, kb * TC_BK, rank * bn);
             }
             dbg_mark(a.dbg, 3, nkb);
             if (a.resid_tma) {
-                // highway residual = this CTA's 'half' channels of the same rows: fetched into the next ring stage
-                // as soon as it has drained, i.e. while the last k-blocks are still being multiplied
-                const int s = nkb % stages;
-                mbar_wait(&empty_bar[s], ((uint32_t)(nkb / stages) & 1u) ^ 1u);
-                uint8_t* st = smem + (size_t)s * stage_bytes;
+                // highway residual = this CTA's 'half' channels of the same rows, into its own staging tile: it arrives
+                // while the k-blocks are still being multiplied
                 const int nbox = half / 64;
                 mbar_expect_tx(resid_bar, (uint32_t)(2 * nbox * 16384));
                 for (int i = 0; i < nbox; ++i) {
-                    tma_load_3d(&mapX_hi, resid_bar, st + i * 16384, rank * half + i * 64, t0s[0], b0s[0]);
-                    tma_load_3d(&mapX_lo, resid_bar, st + (nbox + i) * 16384, rank * half + i * 64, t0s[0], b0s[0]);
+                    tma_load_3d(&mapX_hi, resid_bar, rs + i * 16384, rank * half + i * 64, t0s, b0s);
+                    tma_load_3d(&mapX_lo, resid_bar, rs + (nbox + i) * 16384, rank * half + i * 64, t0s, b0s);
                 }
             }
         }
         __syncwarp();
-    } else if (warp == 1 && peer == 0) {
-        // =========================== MMA issuer (the pair's leader only) ===========================
-        const uint32_t idesc = (CG == 2) ? umma_idesc_f16(256, (uint32_t)half) : umma_idesc_f16(TC_BM, (uint32_t)bn);
-        const uint16_t pair_mask = (uint16_t)(3u << (crank & ~1));
+    } else if (wg >= 1) {
+        // =========================== wgmma consumers ===========================
+        const int mh = wg - 1;                                           // row half of the tile
+        float acc[4][32];
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+#pragma unroll
+            for (int i = 0; i < 32; ++i) acc[j][i] = 0.f;
         for (int kb = 0; kb < nkb; ++kb) {
             const int s = kb % stages;
-            const uint32_t ph = (uint32_t)(kb / stages) & 1u;
-            mbar_wait(&full_bar[s], ph);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t st = smem_u32(smem + (size_t)s * stage_bytes);
-                const uint64_t dB_hi = umma_desc_kmajor<SW>(st + A_BYTES);
-                const uint64_t dB_lo = umma_desc_kmajor<SW>(st + A_BYTES + b_plane);
-                if (CG == 2) {
-                    // two N = half chunks: the gate box / the info box of each CTA's weight tile (half/2 rows from each CTA
-                    // of the pair, in channel order) -> TMEM columns [0,half) / [half,2 half)
-                    const uint64_t dA_hi = umma_desc_kmajor<SW>(st), dA_lo = umma_desc_kmajor<SW>(st + TC_A_PLANE);
+            mbar_wait(&full_bar[s], (uint32_t)(kb / stages) & 1u);
+            const uint32_t st = smem_u32(smem + (size_t)s * stage_bytes);
+            const uint64_t dA_hi = gmma_desc_kmajor<SW>(st + mh * 64 * SW), dA_lo = gmma_desc_kmajor<SW>(st + TC_A_PLANE + mh * 64 * SW);
+            const uint64_t dB_hi = gmma_desc_kmajor<SW>(st + A_BYTES), dB_lo = gmma_desc_kmajor<SW>(st + A_BYTES + b_plane);
+            wg_fence();
 #pragma unroll
-                    for (int ck = 0; ck < 2; ++ck) {
-                        const uint64_t cb = (uint64_t)((ck * (half / 2) * SW) >> 4);
-                        const uint32_t acc = tmem_base + ck * half;
+            for (int k = 0; k < TC_BK / 16; ++k) {
+                const uint64_t adv = (uint64_t)(k * 32 >> 4);            // 16 fp16 = 32 B inside the swizzle atom
 #pragma unroll
-                        for (int k = 0; k < TC_BK / 16; ++k) {
-                            const uint64_t adv = (uint64_t)(k * 32 >> 4);
-                            tc_mma_f16_pair(acc, dA_hi + adv, dB_hi + cb + adv, idesc, (kb | k) != 0);
-                            tc_mma_f16_pair(acc, dA_hi + adv, dB_lo + cb + adv, idesc, 1u);
-                            tc_mma_f16_pair(acc, dA_lo + adv, dB_hi + cb + adv, idesc, 1u);
-                        }
+                for (int j = 0; j < 4; ++j) {
+                    if (j * 64 < bn) {
+                        const uint64_t cb = (uint64_t)((j * 64 * SW) >> 4);
+                        wgmma_split3(acc[j], min(64, bn - j * 64), dA_hi + adv, dA_lo + adv, dB_hi + cb + adv, dB_lo + cb + adv,
+                                     (kb | k) != 0);
                     }
-                    tc_commit_pair(&empty_bar[s], pair_mask);                  // frees the stage in both CTAs
-                    if (kb == nkb - 1) tc_commit_pair(tmem_full_bar, pair_mask);
-                } else {
-#pragma unroll
-                for (int m = 0; m < MT; ++m) {
-                    const uint64_t dA_hi = umma_desc_kmajor<SW>(st + m * 2 * TC_A_PLANE);
-                    const uint64_t dA_lo = umma_desc_kmajor<SW>(st + m * 2 * TC_A_PLANE + TC_A_PLANE);
-                    const uint32_t acc = tmem_base + m * TC_TMEM_COLS;
-#pragma unroll
-                    for (int k = 0; k < TC_BK / 16; ++k) {
-                        const uint64_t adv = (uint64_t)(k * 32 >> 4);      // 16 fp16 = 32 B inside the swizzle atom
-                        tc_mma_f16(acc, dA_hi + adv, dB_hi + adv, idesc, (kb | k) != 0);
-                        tc_mma_f16(acc, dA_hi + adv, dB_lo + adv, idesc, 1u);
-                        tc_mma_f16(acc, dA_lo + adv, dB_hi + adv, idesc, 1u);
-                    }
-                }
-                if (mcast) tc_commit_mc(&empty_bar[s], cta_mask);          // frees the stage in every CTA's view
-                else tc_commit(&empty_bar[s]);                             // frees the smem stage
-                if (kb == nkb - 1) tc_commit(tmem_full_bar);               // accumulator complete
                 }
             }
-            __syncwarp();
+            wg_commit();
+            wg_wait<0>();
+#pragma unroll
+            for (int j = 0; j < 4; ++j) wg_fence_regs(acc[j]);
+            if ((threadIdx.x & 127) == 0) {                                  // the stage is drained: release it
+                if (mcast) { for (int p = 0; p < ncta; ++p) mbar_arrive_cluster(&empty_bar[s], (uint32_t)p); }
+                else mbar_arrive(&empty_bar[s]);
+            }
         }
-        if (lane == 0) dbg_mark(a.dbg, 4, nkb);
-    } else if (warp >= 2) {
-        // =========================== epilogue ===========================
-        const int q = warp & 3;                                            // TMEM lane quarter of this warp
-        const int r = q * 32 + lane;                                       // tile row == TMEM lane
+        if (threadIdx.x == 128) dbg_mark(a.dbg, 4, nkb);
+        named_sync(1, 256);                                              // both halves done reading the ring
+        {
+            const int w4 = (threadIdx.x >> 5) & 3;
+            const int r0 = mh * 64 + w4 * 16 + (lane >> 2);
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+#pragma unroll
+                for (int i8 = 0; i8 < 8; ++i8) {
+                    const int col = j * 64 + i8 * 8 + 2 * (lane & 3);
+                    if (col < bn) {
+                        *reinterpret_cast<float2*>(s_acc + (size_t)r0 * acc_ld + col) = make_float2(acc[j][i8 * 4], acc[j][i8 * 4 + 1]);
+                        *reinterpret_cast<float2*>(s_acc + (size_t)(r0 + 8) * acc_ld + col) = make_float2(acc[j][i8 * 4 + 2], acc[j][i8 * 4 + 3]);
+                    }
+                }
+        }
+        named_sync(1, 256);                                              // accumulator tile complete in shared memory
+    }
+    if (epi) {
+        // =========================== epilogue: thread == tile row ===========================
+        const int r = threadIdx.x - 128;
+        const float* arow = s_acc + (size_t)r * acc_ld;
+        auto ld16 = [&](int c, float (&v)[16]) {
+#pragma unroll
+            for (int i = 0; i < 16; i += 4) {
+                const float4 x = *reinterpret_cast<const float4*>(arow + c + i);
+                v[i] = x.x; v[i + 1] = x.y; v[i + 2] = x.z; v[i + 3] = x.w;
+            }
+        };
         const int bi = r / a.TT, ti = r - bi * a.TT;
         const float inv_s = a.inv_scale;
         const int n1 = (a.mode == 0) ? min(max(a.C - rank * bn, 0), bn) : half;
-
-        mbar_wait(tmem_full_bar, 0);
-        tc_fence_after();
         if (r == 0) { dbg_mark(a.dbg, 5, 1); dbg_time(a.dbg, 10); }       // t2: accumulator complete (main loop over)
 
-      for (int m = 0; m < MT; ++m) {                 // the MT accumulators, one after the other
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + m * TC_TMEM_COLS;
-        const int b = b0s[m] + bi, t = t0s[m] + ti;
+        const int b = b0s + bi, t = t0s + ti;
         const bool row_ok = (b < a.win.B) && (t >= t_lo) && (t <= t_end) && (t < L);
 
-        // ONE statistics sweep (was two): shifted sums about a pivot taken from the row itself, so that
-        // M2 = Q - S^2/n does not cancel; 64 columns per tcgen05.wait (two x32 loads in flight).
+        // ONE statistics sweep: shifted sums about a pivot taken from the row itself, so that M2 = Q - S^2/n does not cancel
         float s1, s2 = 0.f, q1, q2 = 0.f, m1, m2 = 0.f;
         {
             float piv = 0.f, S = 0.f, Q = 0.f;
-            for (int c = 0; c < n1; c += 64) {
-                float v[2][32];
-                tmem_ld32_nowait(taddr + c, v[0]);
-                if (c + 32 < n1) tmem_ld32_nowait(taddr + c + 32, v[1]);
-                tmem_ld_wait();
-                if (c == 0) piv = fmaf(v[0][0], inv_s, s_bias[0]);
+            for (int c = 0; c < n1; c += 16) {
+                float v[16];
+                ld16(c, v);
+                if (c == 0) piv = fmaf(v[0], inv_s, s_bias[0]);
 #pragma unroll
-                for (int h = 0; h < 2; ++h)
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) {
-                        const int cc = c + h * 32 + i;
-                        if (cc < n1) { const float d = fmaf(v[h][i], inv_s, s_bias[cc]) - piv; S += d; Q = fmaf(d, d, Q); }
-                    }
+                for (int i = 0; i < 16; ++i) {
+                    const int cc = c + i;
+                    if (cc < n1) { const float d = fmaf(v[i], inv_s, s_bias[cc]) - piv; S += d; Q = fmaf(d, d, Q); }
+                }
             }
             const float n = (float)max(n1, 1);
             s1 = piv * (float)n1 + S; m1 = n1 > 0 ? s1 / n : 0.f; q1 = fmaxf(Q - S * S / n, 0.f);
         }
         if (a.mode != 0) {
             float piv = 0.f, S = 0.f, Q = 0.f;
-            for (int c = 0; c < half; c += 64) {
-                float v[2][32];
-                tmem_ld32_nowait(taddr + half + c, v[0]);
-                if (c + 32 < half) tmem_ld32_nowait(taddr + half + c + 32, v[1]);
-                tmem_ld_wait();
-                if (c == 0) piv = fmaf(v[0][0], inv_s, s_bias[half]);
+            for (int c = 0; c < half; c += 16) {
+                float v[16];
+                ld16(half + c, v);
+                if (c == 0) piv = fmaf(v[0], inv_s, s_bias[half]);
 #pragma unroll
-                for (int h = 0; h < 2; ++h)
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) {
-                        const int cc = c + h * 32 + i;
-                        if (cc < half) { const float d = fmaf(v[h][i], inv_s, s_bias[half + cc]) - piv; S += d; Q = fmaf(d, d, Q); }
-                    }
+                for (int i = 0; i < 16; ++i) {
+                    const int cc = c + i;
+                    if (cc < half) { const float d = fmaf(v[i], inv_s, s_bias[half + cc]) - piv; S += d; Q = fmaf(d, d, Q); }
+                }
             }
             s2 = piv * (float)half + S; m2 = s2 / (float)half; q2 = fmaxf(Q - S * S / (float)half, 0.f);
         }
@@ -352,7 +320,7 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
         float mean1, rstd1, mean2 = 0.f, rstd2 = 0.f;
         if (ncta > 1) {
             // each CTA publishes its partials in its OWN shared memory; after the cluster barrier every CTA reads
-            // the slices' partials through distributed shared memory (2 KB per CTA instead of a 16 KB mailbox)
+            // the slices' partials through distributed shared memory
             s_part[r] = make_float4(s1, q1, s2, q2);
             if (r == 0) { dbg_mark(a.dbg, 6, 1); dbg_time(a.dbg, 11); }   // t3: statistics sweep done, partials published
             cluster_arrive();                                              // phase 2: partials published
@@ -361,7 +329,7 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
             const uint32_t my_slot = smem_u32(&s_part[r]);
             float4 pv[8];
 #pragma unroll
-            for (int p = 0; p < 8; ++p) pv[p] = (p < nslices) ? ld_cluster_f4(mapa(my_slot, (uint32_t)(p * CG + peer))) : make_float4(0.f, 0.f, 0.f, 0.f);
+            for (int p = 0; p < 8; ++p) pv[p] = (p < nslices) ? ld_cluster_f4(mapa(my_slot, (uint32_t)p)) : make_float4(0.f, 0.f, 0.f, 0.f);
             float S1 = 0.f, S2 = 0.f;
 #pragma unroll
             for (int p = 0; p < 8; ++p) if (p < nslices) { S1 += pv[p].x; S2 += pv[p].z; }
@@ -382,14 +350,13 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
             mean2 = m2; rstd2 = 1.0f / sqrtf(q2 / (float)a.C + 1e-12f);
         }
 
-        // sweep 3: normalise, activate, mix, store.  tcgen05.ld is warp-collective (.sync.aligned):
-        // every lane runs the loads, only the stores are predicated on the row being valid.
+        // sweep 2: normalise, activate, mix, store
         {
             if (a.mode == 0) {
                 const size_t row = (size_t)b * L + t;
                 for (int c = 0; c < n1; c += 16) {
                     float v[16], o[16];
-                    tmem_ld16(taddr + c, v);
+                    ld16(c, v);
                     const int col = rank * bn + c;
 #pragma unroll
                     for (int i = 0; i < 16; ++i) {
@@ -416,8 +383,7 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
                 }
             } else if (a.mode == 1) {
                 const size_t row = (size_t)b * L + t;
-                // residual / output staging tile in the drained ring stage: [plane][box of 64 ch][128 rows][128 B], 128B swizzle
-                uint8_t* rs = smem + (size_t)(nkb % stages) * stage_bytes;
+                // residual / output staging tile: [plane][box of 64 ch][128 rows][128 B], 128B swizzle
                 const int nbox = half / 64;
                 if (a.resid_tma) mbar_wait(resid_bar, 0);
                 for (int c = 0; c < half; c += 16) {
@@ -440,8 +406,8 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
                         reinterpret_cast<uint4*>(xh)[0] = __ldg(ph); reinterpret_cast<uint4*>(xh)[1] = __ldg(ph + 1);
                         reinterpret_cast<uint4*>(xl)[0] = __ldg(pl); reinterpret_cast<uint4*>(xl)[1] = __ldg(pl + 1);
                     }
-                    tmem_ld16(taddr + c, v1);
-                    tmem_ld16(taddr + half + c, v2);
+                    ld16(c, v1);
+                    ld16(half + c, v2);
 #pragma unroll
                     for (int i = 0; i < 16; ++i) {
                         float z1 = (fmaf(v1[i], inv_s, s_bias[c + i]) - mean1) * rstd1 * s_gam[c + i] + s_bet[c + i];
@@ -472,11 +438,11 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
                 if (a.out_tma) {
                     // whole tile staged: one thread hands it to the TMA engine (rows past the end are clipped)
                     fence_proxy_async_smem();
-                    asm volatile("bar.sync 1, 128;" ::: "memory");                // the four epilogue warps only
-                    if (warp == 2 && lane == 0) {
+                    named_sync(2, 128);                                          // the epilogue warpgroup only
+                    if (r == 0) {
                         for (int i = 0; i < nbox; ++i) {
-                            tma_store_3d(&mapO_hi, rs + i * 16384, rank * half + i * 64, t0s[m], b0s[m]);
-                            tma_store_3d(&mapO_lo, rs + (nbox + i) * 16384, rank * half + i * 64, t0s[m], b0s[m]);
+                            tma_store_3d(&mapO_hi, rs + i * 16384, rank * half + i * 64, t0s, b0s);
+                            tma_store_3d(&mapO_lo, rs + (nbox + i) * 16384, rank * half + i * 64, t0s, b0s);
                         }
                         tma_store_commit_and_wait();
                     }
@@ -488,7 +454,7 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
                     const float mean = hsel ? mean2 : mean1, rstd = hsel ? rstd2 : rstd1;
                     for (int c = 0; c < half; c += 16) {
                         float v[16], o[16];
-                        tmem_ld16(taddr + hsel * half + c, v);
+                        ld16(hsel * half + c, v);
                         const int col = rank * half + c;
 #pragma unroll
                         for (int i = 0; i < 16; ++i) {
@@ -505,29 +471,16 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
                 }
             }
         }
-        // the statistics slots are reused by the next tile: wait until every CTA has read them
-        if (ncta > 1 && m + 1 < MT) { cluster_arrive(); cluster_wait(); }
-      }
-        tc_fence_before();
         if (r == 0) dbg_time(a.dbg, 13);                                  // t5: stores issued
     }
 
-    // ---- teardown: match the cluster barrier phases of the epilogue warps (2*MT-1 of them) ----
+    // ---- teardown: the other warps match the epilogue's cluster barrier phase ----
     if (ncta > 1) {
-        if (warp < 2) {
-#pragma unroll
-            for (int i = 0; i < 2 * MT - 1; ++i) { cluster_arrive(); cluster_wait(); }
-        }
+        if (!epi) { cluster_arrive(); cluster_wait(); }
         cluster_arrive();                     // last phase: nobody reads my shared memory any more
         cluster_wait();
     }
-    __syncthreads();
     if (threadIdx.x == 0) dbg_time(a.dbg, 14);                            // t6: teardown barrier passed
-    if (warp == 1) {
-        tc_fence_after();
-        if (CG == 2) { if (bn > 256) tmem_dealloc_pair<512>(tmem_base); else tmem_dealloc_pair<256>(tmem_base); }
-        else tmem_dealloc<MT * TC_TMEM_COLS>(tmem_base);
-    }
 }
 
 // ------------------------------------------------------------------------------------------
@@ -617,19 +570,24 @@ void tc_make_w_map(CUtensorMap* m, const __half* base, int Ktot, int Nrows, int 
 }
 
 int tc_bk() {
-    // measured (SSRN/HC_11, B=32): BK=64 / 2 stages 1.24 ms, BK=32 / 4 stages 1.32 ms -- the kernel is bound by
-    // bytes delivered per SM, not by pipeline depth, so the wider slab (half as many TMA rows) wins
-    return 64;
+    // 32-wide slabs (64-byte swizzle): the fp32 accumulator tile of a 256-column block (130 KB) and the highway residual tile
+    // (64 KB) leave room for two or more 48 KB stages, where 64-wide stages would fit only one
+    return 32;
 }
 
-int tc_stages_for(int bn, int bk, int mt) {      // bn = weight rows staged per CTA
-    const int stage = mt * 2 * TC_BM * bk * 2 + 2 * bn * bk * 2;
-    int s = (200 * 1024) / stage;
-    return s < 2 ? 2 : (s > TC_MAX_STAGES ? TC_MAX_STAGES : s);
+static size_t conv_ln_smem(int stages, int bn, int half, int resid_tma, int bk) {
+    const int stage = 2 * TC_BM * bk * 2 + 2 * bn * bk * 2;
+    return (size_t)tc_ring_bytes(stages, stage, bn, 2 * bk) + tc_resid_bytes(resid_tma, half) + TC_AUX_BYTES + 1024;
+}
+
+int tc_stages_for(int bn, int bk, int resid_tma, int half) {      // bn = accumulator columns per CTA
+    int s = TC_MAX_STAGES;
+    while (s > 2 && conv_ln_smem(s, bn, half, resid_tma, bk) > (size_t)TC_MAX_SMEM) --s;
+    return s;
 }
 
 void launch_conv_ln_tc(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& w_hi,
-                       const CUtensorMap& w_lo, const CUtensorMap* io, const TcArgs& a, int ncta, int ctas_y, int bk, int mt, int cg,
+                       const CUtensorMap& w_lo, const CUtensorMap* io, const TcArgs& a, int ncta, int ctas_y, int bk,
                        cudaStream_t s) {
     // the attributes are per device: cache them per device, not per process (a second Engine on another GPU
     // of the same process must raise its own limits)
@@ -637,23 +595,15 @@ void launch_conv_ln_tc(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const C
     int dev = 0;
     cudaGetDevice(&dev);
     bool& attr_set = attr_set_dev[dev & 63];
-    const int max_smem = 227 * 1024;
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(conv_ln_tc_kernel<64, 1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_ln_tc_kernel<32, 1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_ln_tc_kernel<32, 2, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_ln_tc_kernel<64, 1, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_ln_tc_kernel<32, 1, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
-        // C = 1024 blocks as CTA pairs span 16 CTAs (8 slices x 2): larger than the portable cluster size
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_ln_tc_kernel<32, 1, 2>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_ln_tc_kernel<64, 1, 2>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+        cudaError_t e = cudaFuncSetAttribute(conv_ln_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_MAX_SMEM);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_ln_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_MAX_SMEM);
         if (e != cudaSuccess) throw std::runtime_error(std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e));
         attr_set = true;
     }
-    if (mt == 2 && bk != 32) throw std::runtime_error("conv_ln_tc: paired tiles need the 32-wide slab");
-    if (cg == 2 && (mt != 1 || (ncta & 1) || ncta > 16)) throw std::runtime_error("conv_ln_tc: bad CTA-pair configuration");
-    const size_t smem = (size_t)a.stages * (mt * 2 * TC_BM * bk * 2 + 2 * (a.bn / cg) * bk * 2) + TC_AUX_BYTES + 1024;
-    if (smem > (size_t)max_smem) throw std::runtime_error("conv_ln_tc: shared memory budget exceeded");
+    if (a.bn > 256 || a.bn % 16 || ncta > 8) throw std::runtime_error("conv_ln_tc: unsupported tile (bn <= 256, multiple of 16; cluster <= 8)");
+    const size_t smem = conv_ln_smem(a.stages, a.bn, a.half, a.resid_tma, bk);
+    if (smem > (size_t)TC_MAX_SMEM) throw std::runtime_error("conv_ln_tc: shared memory budget exceeded");
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3((unsigned)ncta, (unsigned)ctas_y, 1);
     cfg.blockDim = dim3(TC_THREADS, 1, 1);
@@ -671,11 +621,8 @@ void launch_conv_ln_tc(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const C
     const CUtensorMap& o_hi = io ? io[2] : a_hi;
     const CUtensorMap& o_lo = io ? io[3] : a_lo;
     cudaError_t e;
-    if (cg == 2 && bk == 64) e = cudaLaunchKernelEx(&cfg, conv_ln_tc_kernel<64, 1, 2>, a_hi, a_lo, w_hi, w_lo, x_hi, x_lo, o_hi, o_lo, a);
-    else if (cg == 2)  e = cudaLaunchKernelEx(&cfg, conv_ln_tc_kernel<32, 1, 2>, a_hi, a_lo, w_hi, w_lo, x_hi, x_lo, o_hi, o_lo, a);
-    else if (mt == 2)  e = cudaLaunchKernelEx(&cfg, conv_ln_tc_kernel<32, 2, 1>, a_hi, a_lo, w_hi, w_lo, x_hi, x_lo, o_hi, o_lo, a);
-    else if (bk == 64) e = cudaLaunchKernelEx(&cfg, conv_ln_tc_kernel<64, 1, 1>, a_hi, a_lo, w_hi, w_lo, x_hi, x_lo, o_hi, o_lo, a);
-    else               e = cudaLaunchKernelEx(&cfg, conv_ln_tc_kernel<32, 1, 1>, a_hi, a_lo, w_hi, w_lo, x_hi, x_lo, o_hi, o_lo, a);
+    if (bk == 64) e = cudaLaunchKernelEx(&cfg, conv_ln_tc_kernel<64>, a_hi, a_lo, w_hi, w_lo, x_hi, x_lo, o_hi, o_lo, a);
+    else          e = cudaLaunchKernelEx(&cfg, conv_ln_tc_kernel<32>, a_hi, a_lo, w_hi, w_lo, x_hi, x_lo, o_hi, o_lo, a);
     if (e != cudaSuccess) throw std::runtime_error(std::string("conv_ln_tc launch: ") + cudaGetErrorString(e));
 }
 

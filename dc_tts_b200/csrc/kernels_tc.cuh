@@ -1,9 +1,9 @@
-// kernels_tc.cuh -- interface of the tcgen05 fused conv + LayerNorm / highway kernels.
+// kernels_tc.cuh -- interface of the wgmma fused conv + LayerNorm / highway kernels.
 //
 // Activation format on the tensor-core path ("split planes"): every fp32 activation x is
 // held as two fp16 tensors hi = fp16(x), lo = fp16(x - hi) (22 significand bits together,
-// 4 bytes per element like fp32).  A conv-GEMM is three tcgen05.mma passes per k-step:
-// hi*Whi + hi*Wlo + lo*Whi accumulated in fp32 in TMEM -- fp32-grade results on the fp16
+// 4 bytes per element like fp32).  A conv-GEMM is three wgmma passes per k-step:
+// hi*Whi + hi*Wlo + lo*Whi accumulated in fp32 registers -- fp32-grade results on the fp16
 // tensor pipe.  Single-pass fp16/tf32 operands miss the 1e-3 parity budget (DESIGN.md).
 #pragma once
 #include <cuda.h>
@@ -34,10 +34,10 @@ struct TcArgs {
     // reduction schedule
     int ntaps; int shifts[3]; int kb_per_tap; int stages;   // kb_per_tap in units of the kernel's BK (64 or 32)
     int mcast;                     // 1: the A tile is fetched once per cluster (each CTA loads 128/ncta rows, TMA multicast)
-    int resid_tma;                 // 1 (hc): residual tile via TMA into a drained pipeline stage
+    int resid_tma;                 // 1 (hc): residual tile via TMA into its own shared-memory tile
     int out_tma;                   // 1 (hc, full sequences, needs resid_tma): output planes staged in that stage and TMA-stored
     // tiling: 128 rows = TT time rows x TB batch rows
-    int TT, TB, tiles_t, ntiles;   // ntiles = batch groups x tiles_t (a CTA takes MT consecutive tiles)
+    int TT, TB, tiles_t, ntiles;   // ntiles = batch groups x tiles_t (one tile per CTA row of the grid)
     RowWin win;
     // residual (mode 1) and outputs
     Planes X;                      // highway residual, same row index as the output
@@ -57,15 +57,15 @@ void tc_make_w_map(CUtensorMap* m, const __half* base, int Ktot, int Nrows, int 
 void tc_make_map3(CUtensorMap* m, const __half* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t stride1_bytes,
                   uint64_t stride2_bytes, uint32_t b0, uint32_t b1);
 
-// pipeline depth that fits the shared-memory budget for `bn` accumulator columns per CTA
-int tc_stages_for(int bn, int bk, int mt);
-// reduction slab per pipeline stage (fp16 elements): 64 (128B swizzle); DCTTS_TC_BK=32 selects 32 (64B swizzle, deeper pipeline)
+// pipeline depth that fits the shared-memory budget for `bn` accumulator columns per CTA (with or without the residual tile)
+int tc_stages_for(int bn, int bk, int resid_tma, int half);
+// reduction slab per pipeline stage (fp16 elements): 32 (64B swizzle)
 int tc_bk();
 // grid = (ncta, tiles); cluster (ncta,1,1)
 void launch_conv_ln_tc(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& w_hi,
-                       const CUtensorMap& w_lo, const CUtensorMap* io /* [4]: X hi, X lo, out hi, out lo ({64,128,1} boxes) or null */, const TcArgs& a, int ncta, int ctas_y, int bk, int mt, int cg, cudaStream_t s);
+                       const CUtensorMap& w_lo, const CUtensorMap* io /* [4]: X hi, X lo, out hi, out lo ({64,128,1} boxes) or null */, const TcArgs& a, int ncta, int ctas_y, int bk, cudaStream_t s);
 
-// ---- tcgen05 attention (kernels_attn_tc.cu) ----
+// ---- wgmma attention (kernels_attn_tc.cu) ----
 struct AttnTcArgs {
     const float* Q; int ldq;       // fp32 queries (copied verbatim into R[:, d:2d])
     float* R; int ldr;             // (B,T,2d) = [A.V ; Q]

@@ -1,6 +1,6 @@
-// tc_ptx.cuh -- thin inline-PTX wrappers for the sm_100a features the tensor-core kernels
-// use: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (TMEM alloc / mma / commit / ld),
-// thread-block clusters and distributed shared memory.
+// tc_ptx.cuh -- thin inline-PTX wrappers for the sm_90a features the tensor-core kernels
+// use: mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA from shared-memory
+// descriptors), thread-block clusters and distributed shared memory.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -76,113 +76,92 @@ __device__ __forceinline__ void tma_store_commit_and_wait() {
 }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// ---- tcgen05 / TMEM -----------------------------------------------------------------------
-template <uint32_t COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_in_smem) {      // whole warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(dst_in_smem)), "n"(COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {            // whole warp
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(taddr), "n"(COLS) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// one thread: all previously issued tcgen05.mma of this thread arrive on `bar` when complete
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(smem_u32(bar)) : "memory");
-}
-// multicast variant: arrives on the barrier at the same offset in every CTA of `mask`
-__device__ __forceinline__ void tc_commit_mc(uint64_t* bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 :: "r"(smem_u32(bar)), "h"(mask) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]^T, fp16 inputs, fp32 accumulate
-__device__ __forceinline__ void tc_mma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        :: "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-// 32 lanes x 16 consecutive 32-bit columns -> 16 registers per thread (thread i <-> lane base+i)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// ---- wgmma (sm_90a warpgroup MMA) ---------------------------------------------------------
+// D (registers of the 128 threads of a warpgroup) (+)= A[smem desc] * B[smem desc]^T, fp16 inputs, fp32 accumulate,
+// M = 64.  Fragment of m64nNk16: register i of thread t (warp w = t/32 of the warpgroup, lane l) holds
+// row 16w + l/4 + 8*((i>>1)&1), column 8*(i>>2) + 2*(l&3) + (i&1).
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" :: "n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void wg_fence_regs(float (&d)[R]) {
 #pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i]) :: "memory");
 }
 
-// 32 lanes x 32 consecutive columns, NOT waited for: issue several, then tmem_ld_wait() once
-__device__ __forceinline__ void tmem_ld32_nowait(uint32_t taddr, float (&v)[32]) {
-    uint32_t* r = reinterpret_cast<uint32_t*>(v);
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-                 "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                   "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-                   "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                 : "r"(taddr));
+#define DCTTS_WG_D8(o) "+f"(d[o + 0]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), "+f"(d[o + 6]), "+f"(d[o + 7])
+// N = 16 * NQ columns (NQ = 1..4): the first 8 * NQ registers of d
+template <int NQ, int R>
+__device__ __forceinline__ void wgmma_f16(float (&d)[R], uint64_t da, uint64_t db, uint32_t accumulate) {
+    static_assert(NQ >= 1 && NQ <= 4 && 8 * NQ <= R, "wgmma_f16: 16..64 columns");
+    if constexpr (NQ == 1) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+                     : DCTTS_WG_D8(0) : "l"(da), "l"(db), "r"(accumulate));
+    } else if constexpr (NQ == 2) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15},"
+                     " %16, %17, p, 1, 1, 0, 0;\n\t}"
+                     : DCTTS_WG_D8(0), DCTTS_WG_D8(8) : "l"(da), "l"(db), "r"(accumulate));
+    } else if constexpr (NQ == 3) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+                     "%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1, 0, 0;\n\t}"
+                     : DCTTS_WG_D8(0), DCTTS_WG_D8(8), DCTTS_WG_D8(16) : "l"(da), "l"(db), "r"(accumulate));
+    } else {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+                     "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+                     : DCTTS_WG_D8(0), DCTTS_WG_D8(8), DCTTS_WG_D8(16), DCTTS_WG_D8(24) : "l"(da), "l"(db), "r"(accumulate));
+    }
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+#undef DCTTS_WG_D8
 
-// K-major swizzled operand tile, rows of SW bytes (SW = 128 or 64), 8-row atoms of 8*SW bytes: the
-// layout TMA writes with CU_TENSOR_MAP_SWIZZLE_{128B,64B}.  sm_100 descriptor: start>>4 [0,14),
-// LBO>>4 [16,30) (unused for swizzled K-major), SBO>>4 [32,46) = 8*SW, version=1 [46,48),
-// layout [61,64): SWIZZLE_128B = 2, SWIZZLE_64B = 4.
+// hi*Bhi + hi*Blo + lo*Bhi into one accumulator of `cols` (16, 32, 48 or 64) columns, chosen at run time
+template <int R>
+__device__ __forceinline__ void wgmma_split3(float (&d)[R], int cols, uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo,
+                                             uint32_t accumulate) {
+    if (cols >= 64) { wgmma_f16<4>(d, a_hi, b_hi, accumulate); wgmma_f16<4>(d, a_hi, b_lo, 1u); wgmma_f16<4>(d, a_lo, b_hi, 1u); }
+    else if (cols == 48) { wgmma_f16<3>(d, a_hi, b_hi, accumulate); wgmma_f16<3>(d, a_hi, b_lo, 1u); wgmma_f16<3>(d, a_lo, b_hi, 1u); }
+    else if (cols == 32) { wgmma_f16<2>(d, a_hi, b_hi, accumulate); wgmma_f16<2>(d, a_hi, b_lo, 1u); wgmma_f16<2>(d, a_lo, b_hi, 1u); }
+    else { wgmma_f16<1>(d, a_hi, b_hi, accumulate); wgmma_f16<1>(d, a_hi, b_lo, 1u); wgmma_f16<1>(d, a_lo, b_hi, 1u); }
+}
+
+// K-major swizzled operand tile, rows of SW bytes (SW = 128 or 64), 8-row atoms of 8*SW bytes: the layout TMA writes with
+// CU_TENSOR_MAP_SWIZZLE_{128B,64B}.  sm_90 descriptor: start>>4 [0,14), LBO>>4 [16,30) (unused for swizzled K-major),
+// SBO>>4 [32,46) = 8*SW, layout [62,64): SWIZZLE_128B = 1, SWIZZLE_64B = 2.  Tiles start on a swizzle-atom boundary; a
+// k step of 16 halfs inside the atom adds 32 bytes to the start address.
 template <int SW>
-__device__ __forceinline__ uint64_t umma_desc_kmajor(uint32_t smem_addr) {
+__device__ __forceinline__ uint64_t gmma_desc_kmajor(uint32_t smem_addr) {
     static_assert(SW == 128 || SW == 64, "swizzle span");
     uint64_t d = 0;
     d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
+    d |= 1ull << 16;
     d |= static_cast<uint64_t>((8 * SW) >> 4) << 32;
-    d |= 1ull << 46;
-    d |= static_cast<uint64_t>(SW == 128 ? 2 : 4) << 61;
+    d |= static_cast<uint64_t>(SW == 128 ? 1 : 2) << 62;
     return d;
 }
-// kind::f16 instruction descriptor: D=f32 [4,6)=1, A/B=f16 [7,10)/[10,13)=0, both K-major, N>>3 [17,23), M>>4 [24,29)
-__device__ __forceinline__ uint32_t umma_idesc_f16(uint32_t M, uint32_t N) {
-    return (1u << 4) | ((N >> 3) << 17) | ((M >> 4) << 24);
+// no-swizzle K-major core-matrix layout: LBO = bytes between the two 8-wide k groups, SBO = bytes between 8-row groups
+__device__ __forceinline__ uint64_t gmma_desc_noswz(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+    uint64_t d = 0;
+    d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
+    d |= static_cast<uint64_t>(lbo_bytes >> 4) << 16;
+    d |= static_cast<uint64_t>(sbo_bytes >> 4) << 32;
+    return d;
 }
 
-// ---- CTA pairs (cta_group::2): one MMA spans two SMs (M = 256), each CTA holds its own 128 rows of A and
-// HALF of the B tile, and its own 128 accumulator rows in its TMEM.  Only the even ("leader") CTA issues.
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;     // clears the pair-parity bit of a shared::cluster address -> the leader's copy
-template <uint32_t COLS>
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* dst_in_smem) {     // warp 1 of BOTH CTAs
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(dst_in_smem)), "n"(COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(smem_u32(bar)) : "memory");
 }
-template <uint32_t COLS>
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" :: "r"(taddr), "n"(COLS) : "memory");
+__device__ __forceinline__ uint32_t mapa(uint32_t smem_addr, uint32_t rank);
+// arrive on the barrier at the same offset in CTA `rank` of the cluster
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
+    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" :: "r"(mapa(smem_u32(bar), rank)) : "memory");
 }
-__device__ __forceinline__ void tc_mma_f16_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        :: "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tc_commit_pair(uint64_t* bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 :: "r"(smem_u32(bar)), "h"(mask) : "memory");
-}
-// TMA load issued by either CTA of a pair into its OWN shared memory, completing on the LEADER's barrier
-__device__ __forceinline__ void tma_load_2d_pair(const void* tmap, uint64_t* bar, void* dst, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                 :: "r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-                 : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_pair(const void* tmap, uint64_t* bar, void* dst, int c0, int c1, int c2) {
-    asm volatile("cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-                 :: "r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2)
-                 : "memory");
-}
+// named barrier of `n` threads (ids 1..15; 0 is __syncthreads)
+__device__ __forceinline__ void named_sync(int id, int n) { asm volatile("bar.sync %0, %1;" :: "r"(id), "r"(n) : "memory"); }
 
 // ---- clusters / DSMEM ---------------------------------------------------------------------
 __device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }

@@ -26,7 +26,7 @@ class Engine:
     def __init__(self, device=0, hparams=hp):
         self._lib = _lib.load()
         if not torch.cuda.is_available():
-            raise DcttsError("dc_tts_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise DcttsError("dc_tts_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         self.device = torch.device("cuda", device)
         self.hp = hparams
         self.F = 1 + hparams.n_fft // 2

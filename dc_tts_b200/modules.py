@@ -1,5 +1,5 @@
 """Building blocks with the reference's signatures (/root/reference/modules.py), each
-executed as fused sm_100a kernels through the C-ABI.
+executed as fused sm_90a kernels through the C-ABI.
 
 `embed` :13, `normalize` :45, `conv1d` :91, `hc` :143, `conv1d_transpose` :199 keep the
 reference argument names and order.  Variables are not created here: they live in the

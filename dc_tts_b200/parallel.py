@@ -55,7 +55,7 @@ class OverlappedGather:
     """The same single gather, hidden under the SSRN (VERDICT r1 item 5): SSRN runs in utterance chunks and every finished
     chunk leaves at once on a side stream into a receive buffer that is allocated ONCE, so only the last chunk's transfer
     is exposed.  Round 1 gathered after the whole SSRN, allocating the receive tensor every step: a fixed ~2.4 ms at every
-    N > 1 (SCALE_r01: 0.964).  Rows keep global order and are bit-identical to the per-rank results (no arithmetic here).
+    N > 1.  Rows keep global order and are bit-identical to the per-rank results (no arithmetic here).
 
         og = OverlappedGather(total, shape_tail, dtype, device, chunks=4)
         for step:  og.begin(); for c in og.chunks(): z = produce(c.lo, c.hi); og.send(c, z);  Z = og.finish()

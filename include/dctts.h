@@ -1,5 +1,5 @@
 /*
- * dctts.h -- C-ABI of the B200-native DC-TTS synthesis path (libdctts_b200.so).
+ * dctts.h -- C-ABI of the H100-native DC-TTS synthesis path (libdctts_b200.so).
  *
  * The reference (Kyubyong/dc_tts) has no FFI layer: its operator API is the set of
  * Python signatures in modules.py / networks.py and the Graph attributes fetched by
@@ -153,7 +153,7 @@ int dctts_get_spectrograms(dctts_handle h, const float* wav, int64_t n_samples, 
  * attention), elementwise clipping to [-1, 1] and tf.train.AdamOptimizer defaults with the Noam learning rate
  * (train.py:122-132, utils.py:141-145) -- for fixed-size batches L (B, max_N) int32, mels (B, max_T, n_mels), DEVICE
  * pointers.  All tensors are float32; the three GEMMs of every block (forward conv, data gradient, weight gradient) run on
- * tcgen05 as split-fp16 x3 with per-tensor power-of-two scales (option "train_tc", default 7; 0 = the float32 CUDA-core
+ * wgmma as split-fp16 x3 with per-tensor power-of-two scales (option "train_tc", default 7; 0 = the float32 CUDA-core
  * kernels).  dctts_train_init allocates the saved activations and the gradient / Adam arenas and switches the handle's
  * SYNTHESIS entry points to the fp32 kernel set (the optimiser updates the fp32 weights only, the packed planes go stale).
  * Dropout uses a stateless hash of (element, block index, seed) -- TF's random stream cannot be reproduced.
@@ -187,18 +187,18 @@ int64_t dctts_launch_count(dctts_handle h);
  * block and every tensor restored at synthesize.py:31-41.  No handle, no GPU. */
 uint32_t dctts_crc32c(uint32_t crc, const void* data, int64_t n);
 /* Selects the kernel set: 0 = one fp32 CUDA-core GEMM + one LN kernel per block (baseline),
- * 1 = default: tcgen05 split-fp16 (3-MMA, fp32-grade) fused blocks where they apply (whole
+ * 1 = default: wgmma split-fp16 (3-MMA, fp32-grade) fused blocks where they apply (whole
  * networks, full-sequence attention, and the wide AudioDec rows of the graph decode step when B >= 8). */
 int dctts_set_tensor_path(dctts_handle h, int32_t mode);
 
 /* Kernel-variant switches (every value is a parity-tested code path; defaults = measured best):
  *   "decode_mode"  1 = the whole AR loop (synthesize.py:45-54) as ONE persistent cluster kernel (default),
  *                  0 = one captured CUDA graph per mel frame (round-1 path)
- *   "tc_occ2" 0/1, "tc_cg2" 0/1/2, "tc_tile_pair" 0/1, "tc_mcast" 0/1, "tc_resid_tma" 0/1: tcgen05 block kernel variants
+ *   "tc_occ2" 0/1, "tc_mcast" 0/1, "tc_resid_tma" 0/1: wgmma block kernel variants
  *   "fused_ln" 0/1: graph decode, GEMM + LN in one launch;  "tc_debug" 0/1;  "decode_prof" 0/1;  "pdl" 0/1 (process-wide)
- *   "train_tc" 0..7: training GEMMs on tcgen05, bit mask 1 forward conv (+ tcgen05 attention), 2 data gradient, 4 weight gradient
+ *   "train_tc" 0..7: training GEMMs on wgmma, bit mask 1 forward conv (+ wgmma attention), 2 data gradient, 4 weight gradient
  * dctts_get_option also answers "decode_available" (1 when this handle / device can run the persistent decode) and
- * "decode_max_clusters" (16-CTA clusters of the decode kernel that are co-resident on this device; 7 on a B200). */
+ * "decode_max_clusters" (16-CTA clusters of the decode kernel that are co-resident on this device). */
 int dctts_set_option(dctts_handle h, const char* name, int32_t value);
 int dctts_get_option(dctts_handle h, const char* name, int32_t* value);
 /* Of the last dctts_text2mel_generate on the persistent decode path: frames in which a cluster had to recompute the

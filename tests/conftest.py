@@ -11,7 +11,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -52,8 +52,8 @@ def golden(name):
     return np.load(os.path.join(GOLDEN, name))
 
 
-# (tensor_path, decode_mode): fp32 CUDA-core blocks + graph-per-frame decode; tcgen05 blocks + graph-per-frame decode;
-# the product default: tcgen05 blocks + the persistent cluster decode kernel
+# (tensor_path, decode_mode): fp32 CUDA-core blocks + graph-per-frame decode; wgmma blocks + graph-per-frame decode;
+# the product default: wgmma blocks + the persistent cluster decode kernel
 KERNEL_SETS = {"fp32path": (0, 0), "tensorpath": (1, 0), "cluster": (1, 1)}
 
 

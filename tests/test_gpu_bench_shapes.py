@@ -1,7 +1,7 @@
 """GPU parity at the shapes the benchmark runs (BASELINE configs 2, 3, 4): SSRN B=32 T=210, TextEnc B=32,
-the 210-frame autoregressive loop at B=32 and B=1 -- the kernel specialisations that produce the headline
-numbers (conv_ln_tc_kernel<32,1,1> with two CTAs per SM, the persistent cluster decode with G=4 utterances
-per cluster) against the oracle.  Reference: networks.py:214-292, synthesize.py:45-57, hyperparams.py:39-47 (B=32)."""
+the 210-frame autoregressive loop at B=32 and B=1 -- the kernel configurations that produce the headline
+numbers (conv_ln_tc_kernel<32> on launches wider than the device, the persistent cluster decode) against the
+oracle.  Reference: networks.py:214-292, synthesize.py:45-57, hyperparams.py:39-47 (B=32)."""
 import numpy as np
 import pytest
 import torch
@@ -23,7 +23,7 @@ def default_engine(engine):
 
 
 def test_ssrn_config3_b32_t210(default_engine, params):
-    """BASELINE config 3: every wide SSRN block runs conv_ln_tc_kernel<32,1,1> (tiles x cluster >= 148)."""
+    """BASELINE config 3: every wide SSRN block runs conv_ln_tc_kernel<32> on more CTAs than the device has SMs."""
     Y = np.random.default_rng(0).uniform(0, 1, (B, hp.max_T, hp.n_mels)).astype(np.float32)
     _, Z = default_engine.ssrn(Y, want_logits=False)
     Z = Z.cpu().numpy()
@@ -77,7 +77,7 @@ def test_generate_config4_b32_210_frames(default_engine, params, decode_mode):
         assert checked >= 2 * hp.max_T                              # not everything may hide behind a tie
         if decode_mode == 1:
             frames, utt, clusters = e.decode_stats()
-            # every cluster co-resident: 7 clusters of 16 CTAs fit a B200, so 32 utterances go 5 per cluster
+            # every cluster co-resident: 32 utterances go 5 per cluster when 7 clusters of 16 CTAs fit the device
             assert clusters <= e.get_option("decode_max_clusters") and 0 < utt <= B * hp.max_T and frames <= clusters * hp.max_T
             # the recompute count must equal the number of window moves of the whole batch
             Pn = P.cpu().numpy()

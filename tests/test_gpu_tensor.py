@@ -1,4 +1,4 @@
-"""GPU parity tests of the tcgen05 (tensor-core, split-fp16 3-MMA) path against the oracle
+"""GPU parity tests of the wgmma (tensor-core, split-fp16 3-MMA) path against the oracle
 and against the fp32 CUDA-core path.  Same tolerances as the fp32 path: the split-plane
 arithmetic is fp32-grade (|err| ~ 1e-5), which is what makes the tensor pipe usable under
 the 1e-3 parity budget at all."""
@@ -113,7 +113,7 @@ def test_tensor_path_close_to_fp32_path(engine):
 
 @pytest.mark.parametrize("decode_mode", [0, 1], ids=["graph", "cluster"])
 def test_generate_tensor_pyramid_vs_oracle(tc, params, decode_mode):
-    """graph decode: B >= 8 moves the 85..59-row AudioDec pyramid of every AR step onto tcgen05 (windowed
+    """graph decode: B >= 8 moves the 85..59-row AudioDec pyramid of every AR step onto wgmma (windowed
     128-row tiles ending at row j); free-running 40 steps against the oracle's literal schedule."""
     tc.set_option("decode_mode", decode_mode)
     L = np.concatenate([synthetic_text(1, 40 + 15 * i, seed=60 + i) for i in range(8)])

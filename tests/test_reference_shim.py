@@ -4,8 +4,10 @@ stand-in tests/golden/tf_shim.py (generator: tests/golden/make_golden_refshim.py
 reference's Python decides (topology, dilations, paddings, scopes/variable names, the decoder shift, the window
 mask); the TF op semantics themselves are the shim's restatement (see its header).
 
-  * CPU: the oracle's two restatements vs these fixtures; where /root/reference exists (this container) the
-    reference code is also executed live for a few decode steps and the variable-name schema is checked.
+  * CPU: the oracle's two restatements vs these fixtures, and vs refshim_live.npz / refshim_host.npz (a few decode
+    steps, the variable names the graph asks for, the text adaptor, the training constants, the vocoder and feature
+    composition; generator: tests/golden/make_golden_refchecks.py).  Where a checkout of the reference is present the
+    same checks also run against the reference code live.
   * GPU: the CUDA path vs these fixtures."""
 import os
 import sys
@@ -70,6 +72,20 @@ def test_oracle_synthesis_loop_vs_reference_code():
     assert np.abs(g["Z_sub"] - g0["Z_sub"]).max() < 1e-4
 
 
+def test_oracle_few_steps_vs_reference_output(P):
+    """A few steps of the reference's loop and its SSRN on their first 8 frames, and the variables its graph asked for."""
+    g = golden("refshim_live.npz")
+    L = synthetic_text(2, 40, seed=5)
+    with torch.no_grad():
+        o = rt.synthesize(P, L, steps=3, literal=True, record=True)
+    assert np.abs(g["Y3"] - o["Y"].numpy()[:, :3]).max() < 2e-5
+    assert np.array_equal(g["p_hist"], o["p_hist"].numpy()[:, :3])
+    _, z2 = rt.SSRN(P, torch.from_numpy(g["Y8"].copy()))
+    assert np.abs(g["Z8"] - z2.numpy()).max() < 2e-5
+    # the graph asked for exactly the variables of the schema (SURVEY.md App. C)
+    assert set(g["requested"].tolist()) == set(P)
+
+
 @pytest.mark.skipif(not HAVE_REF, reason="/root/reference is not present on this machine")
 def test_reference_code_live_few_steps(P):
     sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
@@ -127,6 +143,53 @@ def test_cuda_synthesis_vs_reference_code(engine):
 
 
 # ------------------------------------------------------------------------------------------- host-side pieces
+def _vocoder_inputs():
+    """(magnitudes, waveform): the seeded inputs of the vocoder / feature checks (make_golden_refchecks.py draws the same)."""
+    rng = np.random.default_rng(0)
+    mag = rng.uniform(0.2, 0.8, (40, 1 + hp.n_fft // 2)).astype(np.float32)
+    t = np.arange(int(hp.sr * 0.8)) / hp.sr
+    y = (0.2 * np.sin(2 * np.pi * 300 * t) + 0.02 * rng.standard_normal(t.size)).astype(np.float32)
+    y[:2000] *= 1e-5
+    return mag, y
+
+
+def test_text_adaptor_vs_reference_output():
+    """The reference's data_load.load_data("synthesize") ids on its harvard_sentences.txt and its vocabulary vs the mirror
+    in dc_tts_b200/data_load.py: all 20 sentences, every id."""
+    g = golden("refshim_host.npz")
+    from dc_tts_b200.data_load import load_data, load_vocab
+    mine = load_data("synthesize", os.path.join(ROOT, "harvard_sentences.txt"))
+    assert g["ids"].shape == (20, hp.max_N) and g["ids"].dtype == np.int32
+    assert np.array_equal(g["ids"], mine)
+    char2idx, idx2char = load_vocab()
+    vocab = g["vocab"].tolist()
+    assert [idx2char[i] for i in range(len(idx2char))] == vocab and all(char2idx[c] == i for i, c in enumerate(vocab))
+    assert np.array_equal(golden("refshim_synth_harvard1.npz")["L"], g["ids"][:1])
+
+
+def test_training_constants_vs_reference_output():
+    """utils.guided_attention (utils.py:134-140) and the Noam schedule (utils.py:141-145) as the reference computed them."""
+    from oracle import ref_train as rtr
+    g = golden("refshim_host.npz")
+    np.testing.assert_allclose(g["guided_attention"], rtr.guided_attention(), rtol=0, atol=1e-7)
+    for gs, v in zip(g["lr_steps"], g["lr"]):
+        assert float(v) == pytest.approx(rtr.learning_rate(int(gs)), rel=1e-6)
+
+
+def test_vocoder_and_feature_composition_vs_reference_output():
+    """utils.spectrogram2wav (3 iterations) / load_spectrograms as the reference composed them (with the restated
+    primitives standing in for librosa) vs the oracle's composition."""
+    from oracle import ref_features as rf
+    from oracle import ref_vocoder as rv
+    g = golden("refshim_host.npz")
+    mag, y = _vocoder_inputs()
+    mine, _, _ = rv.spectrogram2wav(mag, n_iter=3)
+    assert g["wav"].shape == mine.shape and np.abs(g["wav"] - mine).max() <= 1e-6 * max(1.0, np.abs(mine).max())
+    mel2, mg2 = rf.load_spectrograms(y)
+    assert g["mel"].shape == mel2.shape and g["mag"].shape == mg2.shape
+    assert np.abs(g["mel"] - mel2).max() < 1e-6 and np.abs(g["mag"] - mg2).max() < 1e-6
+
+
 @pytest.mark.skipif(not HAVE_REF, reason="/root/reference is not present on this machine")
 def test_text_adaptor_vs_reference_code(monkeypatch):
     """data_load.load_data("synthesize") of the reference itself (data_load.py:79-86) on its own harvard_sentences.txt

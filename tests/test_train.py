@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 import torch
 
-from conftest import ROOT
+from conftest import ROOT, golden
 from dc_tts_b200.hyperparams import Hyperparams as hp
 from dc_tts_b200.params import init_params, synthetic_text
 from oracle import ref_train as rtr
@@ -39,6 +39,34 @@ def test_schedule_and_guided_attention():
     W = rtr.guided_attention()
     assert W.shape == (hp.max_N, hp.max_T) and W[0, 0] == 0 and W.max() < 1
     assert abs(W[90, 0] - (1 - np.exp(-(0.5 ** 2) / 0.08))) < 1e-6
+
+
+def test_oracle_losses_vs_reference_training_graph_output():
+    """Losses of the reference's own Text2Mel training graph (refshim_train.npz, tests/golden/make_golden_refchecks.py)
+    with and without the shared deterministic dropout mask vs the autograd oracle."""
+    g = golden("refshim_train.npz")
+    P = init_params(0, "perturbed")
+    L, mels = _batch(2)
+    T = {n: torch.tensor(np.asarray(P[n], np.float32)) for n in rtr.text2mel_names()}
+    for tag, seed, rate in (("drop", 11, hp.dropout_rate), ("nodrop", 0, 0.0)):
+        assert int(g["t2m_%s_ncalls" % tag]) == (38 if rate > 0 else 0)                # one dropout per block
+        with torch.no_grad():
+            o = rtr.forward(T, L, mels, seed, rate)
+        for k, ref in zip(("loss", "loss_mels", "loss_bd1", "loss_att"), g["t2m_" + tag]):
+            assert abs(float(o[k]) - ref) < 2e-6 * max(1.0, abs(ref)), (tag, k, float(o[k]), ref)
+
+
+def test_oracle_ssrn_losses_vs_reference_training_graph_output():
+    g = golden("refshim_train.npz")
+    P = init_params(0, "perturbed")
+    mels = np.random.default_rng(3).uniform(0, 1, (2, 12, hp.n_mels)).astype(np.float32)
+    mags = np.random.default_rng(4).uniform(0, 1, (2, 48, 1 + hp.n_fft // 2)).astype(np.float32)
+    assert int(g["ssrn_ncalls"]) == 16
+    T = {n: torch.tensor(np.asarray(P[n], np.float32)) for n in rtr.ssrn_names()}
+    with torch.no_grad():
+        o = rtr.forward_ssrn(T, mels, mags, 9)
+    for k, ref in zip(("loss", "loss_mags", "loss_bd2"), g["ssrn"]):
+        assert abs(float(o[k]) - ref) < 2e-6 * max(1.0, abs(ref)), (k, float(o[k]), ref)
 
 
 @pytest.mark.skipif(not HAVE_REF, reason="/root/reference is not present on this machine")
@@ -158,7 +186,7 @@ def test_tie_free_set_has_no_relu_near_zero():
 @pytest.mark.parametrize("B,rate,seed,tc", [(2, 0.0, 0, 7), (2, 0.05, 11, 7), (3, 0.05, 4, 7), (2, 0.0, 0, 0), (2, 0.05, 11, 0), (3, 0.05, 4, 0),
                                             (32, 0.05, 5, 7)])
 def test_cuda_train_step_vs_oracle(B, rate, seed, tc):
-    """tc = 7: the three conv-GEMMs of every block (forward, data gradient, weight gradient) on tcgen05 (split-fp16 x3,
+    """tc = 7: the three conv-GEMMs of every block (forward, data gradient, weight gradient) on wgmma (split-fp16 x3,
     kernels_gemm_tc.cu), compared on the tie-free parameter set; tc = 0: fp32 CUDA-core kernels on the plain set.
     B = 32 is BASELINE config 5's batch."""
     from dc_tts_b200.engine import Engine
@@ -210,7 +238,7 @@ def test_cuda_training_reduces_loss_and_is_deterministic():
 @pytest.mark.gpu
 def test_cuda_train_checkpoint_roundtrip(tmp_path):
     """train -> save (TF bundle, train.py:152) -> restore into a fresh handle (synthesize.py:31-41) -> same outputs as
-    the trained handle; and the trained handle refuses the stale tcgen05 weight planes."""
+    the trained handle; and the trained handle refuses the stale wgmma weight planes."""
     from dc_tts_b200 import checkpoint as ck
     from dc_tts_b200.engine import Engine
     P = init_params(2)

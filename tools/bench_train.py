@@ -20,9 +20,9 @@ ap = argparse.ArgumentParser()
 ap.add_argument("--steps", type=int, default=10)
 ap.add_argument("--warmup", type=int, default=3)
 ap.add_argument("--batch", type=int, default=32)
-ap.add_argument("--probe", type=int, default=0, help="measurement only: 1 = the tcgen05 GEMMs fetch their operands but issue no MMA (results are garbage)")
+ap.add_argument("--probe", type=int, default=0, help="measurement only: 1 = the wgmma GEMMs fetch their operands but issue no MMA (results are garbage)")
 ap.add_argument("--net", type=int, default=1, choices=[1, 2], help="1 = Text2Mel trainer (BASELINE config 5), 2 = SSRN trainer (train.py num=2) at T = 210")
-ap.add_argument("--train-tc", type=int, default=7, help="bit mask: 1 forward conv, 2 data gradient, 4 weight gradient on tcgen05 (default 7 = all), 0 = fp32 CUDA-core kernels")
+ap.add_argument("--train-tc", type=int, default=7, help="bit mask: 1 forward conv, 2 data gradient, 4 weight gradient on wgmma (default 7 = all), 0 = fp32 CUDA-core kernels")
 a = ap.parse_args()
 rank, world, local = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
 torch.cuda.set_device(local)
@@ -80,7 +80,7 @@ if rank == 0:
                       "config": {"workload": ("BASELINE config 5: Text2Mel train step (fwd + bwd + clip + Adam), B=%d per GPU, N=180, T=210, dropout %.2f" if a.net == 1 else
                                               "SSRN train step (train.py num=2: fwd + bwd + clip + Adam), B=%d per GPU, T=210 -> 840 frames x 1025 bins, dropout %.2f") % (B, hp.dropout_rate),
                                  "parallelism": "dp%d (all-reduce of %d gradients)" % (world, grads.numel())},
-                      "dtype": ("f32 tensors; GEMMs as split-fp16 x3 on tcgen05, fp32 accumulate" if a.train_tc else "f32 (CUDA-core kernels)"), "data": "synthetic",
+                      "dtype": ("f32 tensors; GEMMs as split-fp16 x3 on wgmma, fp32 accumulate" if a.train_tc else "f32 (CUDA-core kernels)"), "data": "synthetic",
                       "achieved_tflops": world * flops / (ms * 1e-3) / 1e12, "gpu_launches_per_step": (eng.launch_count() - n0) // a.steps,
                       "loss_first": first["loss"], "loss_last": last["loss"]}))
 if world > 1:

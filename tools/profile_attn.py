@@ -25,4 +25,4 @@ a.record()
 for it in range(10):
     e.attention(Q, K, V, False, None)
 b.record(); torch.cuda.synchronize()
-print("dense attention B=%d: %.1f us per call (3 kernels: planes, K/V^T planes, tcgen05 attention)" % (B, a.elapsed_time(b) * 100))
+print("dense attention B=%d: %.1f us per call (3 kernels: planes, K/V^T planes, wgmma attention)" % (B, a.elapsed_time(b) * 100))

@@ -1,4 +1,4 @@
-"""Probe of the tcgen05 block kernel: one block on both paths, error printed (debugging aid;
+"""Probe of the wgmma block kernel: one block on both paths, error printed (debugging aid;
 run with DCTTS_TC_DEBUG=1 for per-CTA progress markers)."""
 import os
 import sys

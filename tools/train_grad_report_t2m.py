@@ -1,5 +1,5 @@
 """Per-tensor gradient deviation of the CUDA Text2Mel training step from the autograd oracle (max |g - g_ref| / max |g_ref|),
-tcgen05 GEMMs (train_tc 1) next to the fp32 CUDA-core kernels (train_tc 0)."""
+wgmma GEMMs (train_tc 1) next to the fp32 CUDA-core kernels (train_tc 0)."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
