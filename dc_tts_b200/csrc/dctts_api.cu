@@ -170,6 +170,7 @@ struct dctts_handle_s {
         int tc_debug = 0;         // progress markers + in-kernel cycle stamps (synchronising)
         int fused_ln = 0;         // graph decode: split-K GEMM and LN epilogue in one launch
         int decode_prof = 0;      // persistent decode: record SM-clock lap timers of cluster 0 / rank 0 (dctts_decode_profile)
+        int decode_force_prepass = 0;   // persistent decode, measurement / test only: every utterance recomputes its receptive field at every frame j >= 1
         int decode_mode = 1;      // 1 = persistent cluster kernel (kernels_decode.cu), 0 = one CUDA graph per frame (round-1 path)
         int train_probe = 0;      // measurement only (tools/bench_train.py --probe): the training GEMMs fetch their operands but issue no MMA
         int train_tc = 7;         // training GEMMs on wgmma, bit mask: 1 forward conv, 2 data gradient, 4 weight gradient; 0 = fp32 CUDA-core kernels
@@ -179,7 +180,7 @@ struct dctts_handle_s {
     struct {
         bool ok = false;          // stream packed, geometry supported, 16-CTA clusters schedulable
         DecParams tab{};          // layer / chunk tables (+ parameter pointers); per-call fields filled by text2mel_generate
-        DevBuf wstream, lnp, scr, stats, pfinal, prof;
+        DevBuf wstream, lnp, scr, stats, pfinal, prof, pl;
         int max_clusters = 0;
         std::string why;          // why not ok
         int last_moved_frames = -1, last_moved_utt = -1, last_clusters = 0;
@@ -191,7 +192,7 @@ struct dctts_handle_s {
         for (DevBuf* b : {&tr.pre, &tr.out, &tr.emb, &tr.R, &tr.align, &tr.dS, &tr.gbuf[0], &tr.gbuf[1], &tr.gbuf[2], &tr.gbuf[3], &tr.dy,
                           &tr.wT, &tr.zeros, &tr.gts, &tr.sums, &tr.ids, &tr.grads, &tr.mom, &tr.vel, &tr.entries, &tr.tc_a_hi, &tr.tc_a_lo, &tr.tc_b_hi,
                           &tr.tc_b_lo, &tr.tc_slots}) b->release();
-        dec.prof.release(); dec.wstream.release(); dec.lnp.release(); dec.scr.release(); dec.stats.release(); dec.pfinal.release();
+        dec.prof.release(); dec.wstream.release(); dec.lnp.release(); dec.scr.release(); dec.stats.release(); dec.pfinal.release(); dec.pl.release();
         tickets.release(); scratch.release(); act0.release(); act1.release(); kv.release(); ybuf.release();
         rbuf.release(); ad_sig.release(); ibuf.release(); lbuf.release(); zbuf.release();
         for (auto& b : plane) b.release();
@@ -458,7 +459,13 @@ void pack_decode(H* h) {
     for (int li = 0; li < P.nl; ++li) {
         const DecLayer& L = P.L[li];
         if (L.prow <= 1) continue;
-        if (L.krows % 128 || (L.ns != 32 && L.ns != 16)) { D.why = "persistent decode: tensor-core pre-pass geometry"; return; }
+        // kernels_decode.cu instantiates pyr_mma_rows<NS, NTAPS, 1 or 2> for exactly these two shapes -- hc blocks
+        // <32, 3, *> and 1x1 convolutions <16, 1, *> -- and stages the first block's input, [ctx | q], from the re-attention
+        // (2d channels, lane-strided: d = 256); a new shape needs a new instantiation there, not just a change here
+        if (L.krows % 128 || !((L.ns == 32 && L.ntaps == 3) || (L.ns == 16 && L.ntaps == 1)) ||
+            (li == P.n_enc && (L.cin != 2 * d || d != 256)) || (li > P.n_enc && L.cin != 256)) {
+            D.why = "persistent decode: tensor-core pre-pass geometry"; return;
+        }
         for (int c = L.ch0; c < L.ch0 + L.nch; ++c) { P.C[c].off16 = off; off += L.krows * L.ns; }
     }
     P.stream_len = off;
@@ -570,6 +577,23 @@ void commit_params(H* h) {
 }
 
 // ---------------------------------------------------------------------------- workspace
+// Persistent decode, split-fp16 planes of the recompute's inputs (kernels_decode.cuh: pl_hist, pl_c1), in halfs:
+// the input history of every receptive-field block after the first ((DEC_PL_PAD + T) rows per utterance), then one
+// DEC_PL_PAD-row stage image per slab of the first block's input for every utterance slot of every cluster.
+// `set` (optional) receives the pointers.
+size_t decode_plane_halfs(H* h, int B, __half* base = nullptr, DecParams* set = nullptr) {
+    const int T = h->hp.max_T;
+    const std::vector<int> rows = audiodec_rows(h->audiodec, T);
+    size_t off = 0;
+    for (size_t i = 1; i < rows.size() && rows[i] > 1; ++i) {
+        if (set) set->pl_hist[set->n_enc + i] = base + off;
+        off += (size_t)B * h->audiodec[i].cin * 2 * (DEC_PL_PAD + T);
+    }
+    if (set) { set->pl_c1 = base + off; set->pl_rows = DEC_PL_PAD + T; }
+    if (!h->audiodec.empty()) off += (size_t)(B + DEC_GMAX) * h->audiodec[0].cin * 2 * DEC_PL_PAD;
+    return off;
+}
+
 void ensure_ws(H* h, int B) {
     if (B <= h->ws_B) return;
     const dctts_hparams& hp = h->hp;
@@ -602,6 +626,8 @@ void ensure_ws(H* h, int B) {
         CUDA_CHECK(cudaMemset(h->arpl[i].p, 0, h->arpl[i].bytes));
     }
     h->dec.scr.ensure((size_t)(B + DEC_GMAX) * 85 * 512 * sizeof(float));
+    h->dec.pl.ensure(decode_plane_halfs(h, B) * sizeof(__half));
+    CUDA_CHECK(cudaMemset(h->dec.pl.p, 0, h->dec.pl.bytes));     // the DEC_PL_PAD rows in front of t = 0 stay zero
     h->dec.stats.ensure((size_t)2 * B * sizeof(int));
     h->dec.pfinal.ensure((size_t)B * sizeof(int));
     h->ws_B = B;
@@ -992,8 +1018,10 @@ bool decode_cluster(H* h, int B, int steps, cudaStream_t s) {
         P.in_hist[li] = li == 0 ? nullptr : (li == P.n_enc ? h->rbuf.as<float>() : P.out_hist[li - 1]);
     }
     P.kv = h->kv.as<float>(); P.ybuf = h->ybuf.as<float>(); P.rbuf = h->rbuf.as<float>(); P.pre_scr = D.scr.as<float>();
+    decode_plane_halfs(h, h->ws_B, D.pl.as<__half>(), &P);
     P.p_hist = ib.p_hist; P.p_final = D.pfinal.as<int>(); P.stats = D.stats.as<int>();
     P.prof = nullptr;
+    P.force_prepass = h->opt.decode_force_prepass != 0;
     if (h->opt.decode_prof) { D.prof.ensure(16 * sizeof(long long)); CUDA_CHECK(cudaMemsetAsync(D.prof.p, 0, 16 * sizeof(long long), s)); P.prof = D.prof.as<long long>(); }
     P.B = B;
     {   // utterances per cluster: the fewest that let every cluster be co-resident (a second wave doubles the time)
@@ -2017,6 +2045,7 @@ static int* option_slot(dctts_handle h, const char* name) {
     if (n == "fused_ln") return &h->opt.fused_ln;
     if (n == "decode_mode") return &h->opt.decode_mode;
     if (n == "decode_prof") return &h->opt.decode_prof;
+    if (n == "decode_force_prepass") return &h->opt.decode_force_prepass;
     if (n == "train_tc") return &h->opt.train_tc;
     if (n == "train_probe") return &h->opt.train_probe;
     return nullptr;

@@ -51,18 +51,19 @@ constexpr int PLD = GMAX * 32 + 16;            // pitch between the ranks' slice
 constexpr int TC_RA = 96;                      // pre-pass: rows per k8 group of an A slab plane (<= 96 source rows per utterance)
 constexpr int TC_APLANE = 2 * TC_RA * 16;      // bytes of one plane of one 16-channel slab (2 k8 groups)
 constexpr int TC_ASTAGE = 2 * TC_APLANE;       // hi + lo planes
-constexpr int TC_NSTG = 2;                     // A slab stages
-constexpr int WRK_F = TC_NSTG * TC_ASTAGE / 4; // the pre-pass work buffer, shared with the per-frame partial sums
-static_assert(WRK_F >= GMAX * NT && WRK_F >= 1024, "work buffer: partial sums of the per-frame path / LayerNorm parameters of the pre-pass");
+constexpr int TC_NSTG = 3;                     // A slab stages
+static_assert(GMAX * NT >= 1024, "red: LayerNorm parameters of the pre-pass");
+static_assert(TC_RA == DEC_PL_PAD, "pl_c1 rows are staged as whole slabs");
 
 struct Smem {
     float ring[DEC_NSLOT][NWARP][DEC_REG_F];
-    union {                             // never live together: the pre-pass stages A here while no per-frame block is in flight
-        float wrk[WRK_F];               // pre-pass A slab stages (its reads run up to 128 + 54 rows past a slab start: xin follows)
-        float red[GMAX][NT];            // per-frame path: partial sums per warp; pre-pass: LayerNorm parameters of the block
-    };
+    float red[GMAX][NT];                // per-frame path: partial sums per warp; pre-pass: LayerNorm parameters of the block
     float xin[2][GMAX][XLD];
-    float pre[2][NC][PLD];
+    union {                             // never live together: between the cluster barriers that enclose the pre-pass no peer
+                                        // sends pre-LN slices, so the pre-pass stages A here
+        float pre[2][NC][PLD];
+        unsigned char tca[TC_NSTG][TC_ASTAGE];   // (the MMAs read up to 128 + 54 rows past a slab start: outv / prm follow)
+    };
     float outv[2][GMAX * 32];
     float prm[2][DEC_PRM_F];
     unsigned long long fullw[DEC_NSLOT][NWARP];
@@ -79,6 +80,7 @@ struct Smem {
 };
 
 static_assert(sizeof(Smem) + 128 <= 232448, "decode kernel: shared memory budget (227 KB per CTA)");
+static_assert(sizeof(float) * 2 * NC * PLD >= TC_NSTG * TC_ASTAGE, "A stages inside pre");
 
 // lap timer (option decode_prof): thread 0 attributes the cycles since the previous lap to bucket i
 #define LAP(i) do { if constexpr (PROF) { if (threadIdx.x == 0) { const long long now_ = clock64(); S.prof[i] += now_ - S.prof_last; S.prof_last = now_; } } } while (0)
@@ -114,6 +116,35 @@ __device__ __forceinline__ void bulk_s2peer(uint32_t dst_cluster, const void* sr
                  :: "r"(dst_cluster), "r"(smem_u32(src)), "r"(bytes), "r"(bar_cluster) : "memory");
 }
 __device__ __forceinline__ void cluster_sync_all() { cluster_arrive(); cluster_wait(); }
+// generic-proxy global stores (the plane histories) -> visible to later bulk copies (async proxy) once a barrier orders them
+__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+
+// ---- split-fp16 plane histories (DecParams::pl_hist): hi = fp16(x), lo = fp16(x - hi) ----------------------------------
+// index (in halfs) of channel c of row t of utterance b in the hi plane; the lo plane follows at + 2 * rows * 8
+__device__ __forceinline__ size_t pl_idx(int nslab, int rows, int b, int c, int t) {
+    return ((size_t)(b * nslab + (c >> 4)) * 4 + ((c >> 3) & 1)) * (size_t)rows * 8 + (size_t)(t + DEC_PL_PAD) * 8 + (c & 7);
+}
+__device__ __forceinline__ void split_h(float v, __half& hi, __half& lo) {
+    hi = __float2half_rn(v);
+    lo = __float2half_rn(v - __half2float(hi));
+}
+// eight consecutive channels -> 16 bytes of the hi plane at p, 16 bytes of the lo plane TC_APLANE bytes further (a stage image)
+__device__ __forceinline__ void store_split8(__half* p, const float (&v)[8]) {
+    __align__(16) __half hi[8];
+    __align__(16) __half lo[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) split_h(v[i], hi[i], lo[i]);
+    *reinterpret_cast<uint4*>(p) = *reinterpret_cast<const uint4*>(hi);
+    *reinterpret_cast<uint4*>(p + TC_APLANE / 2) = *reinterpret_cast<const uint4*>(lo);
+}
+// four consecutive channels (c % 4 == 0) of one row
+__device__ __forceinline__ void pl_store4(__half* pl, size_t idx, size_t lo_off, float a, float b, float c, float d) {
+    __align__(8) __half hi[4];
+    __align__(8) __half lo[4];
+    split_h(a, hi[0], lo[0]); split_h(b, hi[1], lo[1]); split_h(c, hi[2], lo[2]); split_h(d, hi[3], lo[3]);
+    *reinterpret_cast<uint2*>(pl + idx) = *reinterpret_cast<const uint2*>(hi);
+    *reinterpret_cast<uint2*>(pl + idx + lo_off) = *reinterpret_cast<const uint2*>(lo);
+}
 // two independent fp32 FMAs on (x, y) pairs
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 __device__ __forceinline__ float4 ldcg4(const float* p) { return __ldcg(reinterpret_cast<const float4*>(p)); }
@@ -377,10 +408,12 @@ __device__ __forceinline__ int layer_row(const DecParams& P, Smem& S, Stream& st
         const int cur_off = (l.ntaps - 1) * 256;
         const int next_off = (last || li + 1 == P.n_enc) ? 0 : (P.L[li + 1].ntaps - 1) * 256;
         float* oh = P.out_hist[li];
+        __half* pl = last ? nullptr : P.pl_hist[li + 1];             // the same row as split-fp16 planes (this CTA's slice = one slab)
         const int c = tid;
         if (c < C) {
             const int po = pre_off(c);
             const bool mine = (po / PLD == rank) && oh;
+            const size_t pl_lo = (size_t)P.pl_rows * 16;
             const float g1 = prm[c], b1 = prm[256 + c], g2 = prm[512 + c], b2 = prm[768 + c];
             float o[GT];
 #pragma unroll
@@ -403,7 +436,13 @@ __device__ __forceinline__ int layer_row(const DecParams& P, Smem& S, Stream& st
 #pragma unroll
             for (int g = 0; g < GT; ++g) {
                 const size_t row = (size_t)(b0 + g) * P.T + j;
-                if (mine && g < G) oh[row * C + c] = o[g];           // this CTA's slice of the history row
+                if (mine && g < G) {                                  // this CTA's slice of the history row
+                    oh[row * C + c] = o[g];
+                    if (pl) {
+                        const size_t ix = pl_idx(C >> 4, P.pl_rows, b0 + g, c, j);
+                        split_h(o[g], pl[ix], pl[ix + pl_lo]);
+                    }
+                }
                 if (last) {                                           // Y = sigmoid(logits), networks.py:210; next frame's AudioEnc input
                     o[g] = sigmoid_fast(o[g]);
                     if (rank == 0 && g < G) P.ybuf[row * C + c] = o[g];
@@ -495,9 +534,9 @@ __device__ __forceinline__ int pre_off_of(const PreRows& r, int g) { return r.n 
 // the three taps of the dilated conv are the SAME slab read through descriptors whose start address is shifted by
 // tap * rate rows -- staged once, multiplied three times.  B = this CTA's weight columns, pre-packed in the same layout
 // ([plane][k8][column][8 halfs], 2 KB per 16-k slab) and streamed through the ring like the fp32 weights.  D = 128 x ns fp32
-// in the registers of warpgroup 1 (two M = 64 halves); per slab and tap hi*Whi + hi*Wlo + lo*Whi (the dropped lo*lo term is
-// 2^-22 relative).
-constexpr int TC_LOADW = 3;                                         // warps 0..2 stage A (one thread per source row, <= 96 rows)
+// in the registers of warpgroup 1 (the M = 64 halves that hold output rows); per slab and tap hi*Whi + hi*Wlo + lo*Whi (the
+// dropped lo*lo term is 2^-22 relative).  The planes are kept in HBM in the same layout (pl_hist, pl_c1), so staging a slab
+// is four bulk copies -- no conversion on the way.
 
 // (descriptor start-address field, i.e. address >> 4) of every weight slab of block li, tap-major: S.tc_baddr[tap * nslab + ks].
 // One division chain per entry, computed by 96 threads in parallel, OFF the MMA issue path.
@@ -511,47 +550,60 @@ __device__ __forceinline__ void pyr_tc_table(const DecParams& P, Smem& S, int li
     }
 }
 
-// warpgroup 1: the MMAs of every slab and tap into acc[row half], then the scaled, biased rows -> scratch
-template <int NS>
+// warpgroup 1: the MMAs of every slab and tap into acc[row half], then the scaled, biased rows -> scratch.
+// The shape is compile-time -- NS weight columns, NTAPS taps, MH live row halves of 64 (MH = 1 when every output row is below
+// 64: the other half would multiply rows that are thrown away) -- so that the products of one slab are ONE straight
+// fence -> MMAs -> commit sequence.  (With a run-time tap loop ptxas serialised every wgmma: C7520.)  One slab stays in
+// flight: slab ks is issued before the wait for slab ks - 1, whose stage is released only after that wait.
+template <int NS, int NTAPS, int MH>
 __device__ __forceinline__ void pyr_mma_rows(const DecParams& P, Smem& S, int li, unsigned& use, int& stg, int n_out, int rank,
                                              float* scr_rows) {
     const DecLayer& l = P.L[li];
     const int nslab = l.cin / 16, lane = threadIdx.x & 31, w4 = (threadIdx.x >> 5) & 3;
-    unsigned char* As = reinterpret_cast<unsigned char*>(S.wrk);
+    const bool leader = (threadIdx.x & 127) == 0;
+    unsigned char* As = &S.tca[0][0];
     const uint64_t dA0 = gmma_desc_noswz(0, TC_RA * 16, 128), dB0 = gmma_desc_noswz(0, (uint32_t)NS * 16, 128);
     const uint32_t a_base = (smem_u32(As) & 0x3FFFFu) >> 4, b_lo = (uint32_t)NS * 2, tap_step = (uint32_t)l.rate;
-    float acc[2][NS / 2];
+    float acc[MH][NS / 2];
 #pragma unroll
-    for (int m = 0; m < 2; ++m)
+    for (int m = 0; m < MH; ++m)
 #pragma unroll
         for (int i = 0; i < NS / 2; ++i) acc[m][i] = 0.f;
+    int prev = 0;                                                     // stage of the slab still in flight
 #pragma unroll 1
     for (int ks = 0; ks < nslab; ++ks) {
-        mbar_wait(bar64(&S.abar[stg]), use & 1u);                     // the slab is staged (all loader warps arrived)
-        uint32_t aa = a_base + (uint32_t)stg * (TC_ASTAGE >> 4);
-        const uint32_t* bt = &S.tc_baddr[ks];
-        wg_fence();
-#pragma unroll 1
-        for (int tap = 0; tap < l.ntaps; ++tap, aa += tap_step, bt += nslab) {
-            const uint64_t db_hi = dB0 | *bt, db_lo = dB0 | (*bt + b_lo);
+        uint32_t bt[NTAPS];
 #pragma unroll
-            for (int m = 0; m < 2; ++m) {                             // rows 64 m .. 64 m + 63: 64 rows of 16 bytes further
-                const uint64_t da_hi = dA0 | (aa + 64u * m), da_lo = dA0 | (aa + 64u * m + (TC_APLANE >> 4));
+        for (int tap = 0; tap < NTAPS; ++tap) bt[tap] = S.tc_baddr[tap * nslab + ks];
+        const uint32_t aa = a_base + (uint32_t)stg * (TC_ASTAGE >> 4);
+        mbar_wait(bar64(&S.abar[stg]), use & 1u);                     // the slab is staged (its bulk copies completed)
+        wg_fence();
+#pragma unroll
+        for (int tap = 0; tap < NTAPS; ++tap) {
+            const uint64_t db_hi = dB0 | bt[tap], db_lo = dB0 | (bt[tap] + b_lo);
+#pragma unroll
+            for (int m = 0; m < MH; ++m) {                            // rows 64 m .. 64 m + 63: 64 rows of 16 bytes further
+                const uint32_t a = aa + (uint32_t)tap * tap_step + 64u * m;
+                const uint64_t da_hi = dA0 | a, da_lo = dA0 | (a + (TC_APLANE >> 4));
                 wgmma_f16<NS / 16>(acc[m], da_hi, db_hi, (ks | tap) != 0);
                 wgmma_f16<NS / 16>(acc[m], da_hi, db_lo, 1u);
                 wgmma_f16<NS / 16>(acc[m], da_lo, db_hi, 1u);
             }
         }
         wg_commit();
-        wg_wait<0>();
-        wg_fence_regs(acc[0]); wg_fence_regs(acc[1]);
-        if ((threadIdx.x & 127) == 0) mbar_arrive(bar64(&S.sbar[stg]));   // the loaders may overwrite the stage
+        wg_wait<1>();                                                 // slab ks - 1 is multiplied: its stage may be refilled
+        if (ks > 0 && leader) mbar_arrive(bar64(&S.sbar[prev]));
+        prev = stg;
         if (++stg == TC_NSTG) { stg = 0; ++use; }
     }
+    wg_wait<0>();
+#pragma unroll
+    for (int m = 0; m < MH; ++m) wg_fence_regs(acc[m]);
+    if (leader) mbar_arrive(bar64(&S.sbar[prev]));
     const float inv = P.inv_scale[li];
     const float* bs = P.bias[li];
 #pragma unroll
-    for (int m = 0; m < 2; ++m)
+    for (int m = 0; m < MH; ++m)
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int row = 64 * m + 16 * w4 + (lane >> 2) + 8 * h;
@@ -569,69 +621,53 @@ __device__ __forceinline__ void pyr_mma_rows(const DecParams& P, Smem& S, int li
         }
 }
 
-// The slab pipeline has no block barrier.  Loader warps fill stage s and arrive on abar[s]; warpgroup 1 waits for abar[s],
-// issues the split-fp16 products of every tap and releases the stage through sbar[s], which the loaders wait for before
-// they overwrite it.  Slabs are numbered through the whole launch (st.tcq): slab q lives in stage q % TC_NSTG and is that
-// stage's (q / TC_NSTG)-th use, which gives every wait its phase parity without any shared counter.
+// The slab pipeline has no block barrier.  Thread 0 stages slab q into stage s with bulk copies completing on abar[s];
+// warpgroup 1 waits for abar[s], issues the split-fp16 products of every tap and releases the stage through sbar[s], which
+// thread 0 waits for before it overwrites it.  Slabs are numbered through the whole launch (st.tcq): slab q lives in stage
+// q % TC_NSTG and is that stage's (q / TC_NSTG)-th use, which gives every wait its phase parity without any shared counter.
+// Source of the slabs: the plane history of the block's input (rows t_lo - halo .. t_lo + n_out - 1 of utterance b: four
+// runs of n_src rows, the zero rows in front of t = 0 included), or for the first AudioDec block the cluster's plane
+// scratch of the recomputed rows, `c1` (a whole stage per slab).
 __device__ __forceinline__ void pyr_tc_utt(const DecParams& P, Smem& S, int li, unsigned q0, int b, int t_lo, int n_out,
-                                        int rank, float* scr_rows) {
+                                        int rank, float* scr_rows, const __half* c1) {
     const DecLayer& l = P.L[li];
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int halo = (l.ntaps - 1) * l.rate, n_src = n_out + halo;   // <= 96
-    const int nslab = l.cin / 16;
-    unsigned char* As = reinterpret_cast<unsigned char*>(S.wrk);
+    const int tid = threadIdx.x, warp = tid >> 5;
     unsigned use = q0 / TC_NSTG;
     int stg = (int)(q0 - use * TC_NSTG);
-    if (warp < TC_LOADW) {
-        const bool loader = tid < n_src;
-        const int t_src = t_lo - halo + tid;
-        const float* src = P.in_hist[li] + ((size_t)b * P.T + (t_src < 0 ? 0 : t_src)) * l.ldin;
-        const bool have = loader && t_src >= 0;                      // rows before the utterance start: TF zero padding
-        // The loop is bound by the latency of the activation loads (L2, ~700 cycles), not by the conversion or the MMAs: each
-        // thread keeps FOUR slabs (4 x 64 bytes of its row) in flight in registers.  (nslab is 16 or 32.)
-        constexpr int PF = 4;
-        float4 r[PF][4];
-#pragma unroll
-        for (int u = 0; u < PF; ++u)
-#pragma unroll
-            for (int i = 0; i < 4; ++i) r[u][i] = (have && u < nslab) ? ldcg4(src + u * 16 + i * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
-        unsigned char* dst0 = As + tid * 16;
+    if (tid == 0) {
+        const int halo = (l.ntaps - 1) * l.rate, n_src = n_out + halo;   // <= 96 (pack_decode)
+        const int nslab = l.cin / 16;
+        const size_t run = (size_t)P.pl_rows * 8;                     // halfs between the four (plane, k8) runs of a slab
+        const __half* src = c1 ? c1 : P.pl_hist[li] + pl_idx(nslab, P.pl_rows, b, 0, t_lo - halo);
+        const size_t sstep = c1 ? (size_t)TC_ASTAGE / 2 : 4 * run;    // halfs per slab
+        const uint32_t rb = (uint32_t)n_src * 16;
+        fence_proxy_async_global();
 #pragma unroll 1
-        for (int ks0 = 0; ks0 < nslab; ks0 += PF) {
+        for (int ks = 0; ks < nslab; ++ks, src += sstep) {
+            if (use > 0) mbar_wait(bar64(&S.sbar[stg]), (use - 1) & 1u);   // the MMAs that read this stage are done
+            unsigned char* dst = &S.tca[stg][0];
+            if (c1) {
+                mbar_expect_tx(bar64(&S.abar[stg]), TC_ASTAGE);
+                bulk_g2s(dst, src, TC_ASTAGE, &S.abar[stg]);
+            } else {
+                mbar_expect_tx(bar64(&S.abar[stg]), 4 * rb);
 #pragma unroll
-            for (int u = 0; u < PF; ++u) {
-                if (ks0 + u < nslab) {
-                    if (use > 0) mbar_wait(bar64(&S.sbar[stg]), (use - 1) & 1u);   // the MMAs that read this stage are done
-                    if (loader) {
-                        unsigned char* dst = dst0 + stg * TC_ASTAGE;
-#pragma unroll
-                        for (int h8 = 0; h8 < 2; ++h8) {              // the two 8-channel k groups of the slab
-                            const float4 p0 = r[u][2 * h8], p1 = r[u][2 * h8 + 1];
-                            const float v[8] = {p0.x, p0.y, p0.z, p0.w, p1.x, p1.y, p1.z, p1.w};
-                            __align__(16) __half hi[8];
-                            __align__(16) __half lo[8];
-#pragma unroll
-                            for (int i = 0; i < 8; ++i) { hi[i] = __float2half_rn(v[i]); lo[i] = __float2half_rn(v[i] - __half2float(hi[i])); }
-                            *reinterpret_cast<uint4*>(dst + h8 * (TC_RA * 16)) = *reinterpret_cast<const uint4*>(hi);
-                            *reinterpret_cast<uint4*>(dst + h8 * (TC_RA * 16) + TC_APLANE) = *reinterpret_cast<const uint4*>(lo);
-                        }
-                    }
-                    if (have && ks0 + u + PF < nslab) {
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) r[u][i] = ldcg4(src + (ks0 + u + PF) * 16 + i * 4);
-                    }
-                    fence_proxy_async_smem();                         // generic-proxy stores -> visible to the tensor core's reads
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(bar64(&S.abar[stg]));
-                    if (++stg == TC_NSTG) { stg = 0; ++use; }
-                }
+                for (int r = 0; r < 4; ++r)                           // (plane, k8 group) = (r >> 1, r & 1)
+                    bulk_g2s(dst + (r >> 1) * TC_APLANE + (r & 1) * (TC_RA * 16), src + r * run, rb, &S.abar[stg]);
             }
+            if (++stg == TC_NSTG) { stg = 0; ++use; }
         }
-    } else if (warp >= 4) {
-        if (l.ns == 32) pyr_mma_rows<32>(P, S, li, use, stg, n_out, rank, scr_rows);
-        else pyr_mma_rows<16>(P, S, li, use, stg, n_out, rank, scr_rows);
+    } else if (warp >= 4) {                                           // shapes checked by pack_decode: hc 32 columns x 3 taps, conv 16 x 1
+        if (l.ns == 32) {
+            if (n_out > 64) pyr_mma_rows<32, 3, 2>(P, S, li, use, stg, n_out, rank, scr_rows);
+            else pyr_mma_rows<32, 3, 1>(P, S, li, use, stg, n_out, rank, scr_rows);
+        } else {
+            if (n_out > 64) pyr_mma_rows<16, 1, 2>(P, S, li, use, stg, n_out, rank, scr_rows);
+            else pyr_mma_rows<16, 1, 1>(P, S, li, use, stg, n_out, rank, scr_rows);
+        }
     }
-    __syncthreads();                                                  // every stage of this utterance is released and its rows stored
+    // no block barrier: thread 0 goes on to the next utterance's slabs while this one's rows are stored (the stage
+    // mbarriers order them); the caller synchronises once after the block's last utterance
 }
 
 // LayerNorm / gate / highway mix of the refreshed rows: one warp per row over the whole cluster (parameters in S.red)
@@ -676,16 +712,23 @@ __device__ __forceinline__ void pyr_ln(const DecParams& P, Smem& S, int li, int 
         float* orow = P.out_hist[li] + row * 256;
         *reinterpret_cast<float4*>(orow + lane * 4) = make_float4(o[0], o[1], o[2], o[3]);
         *reinterpret_cast<float4*>(orow + 128 + lane * 4) = make_float4(o[4], o[5], o[6], o[7]);
+        if (__half* pl = P.pl_hist[li + 1]) {                        // the next block's recompute reads these rows as planes
+            const size_t lo = (size_t)P.pl_rows * 16;
+            pl_store4(pl, pl_idx(16, P.pl_rows, b0 + g, lane * 4, t), lo, o[0], o[1], o[2], o[3]);
+            pl_store4(pl, pl_idx(16, P.pl_rows, b0 + g, 128 + lane * 4, t), lo, o[4], o[5], o[6], o[7]);
+        }
     }
 }
 
 }  // namespace
 
-// ---- the pre-pass as ONE out-of-line function: cold code (most frames do not have it) kept out of the per-frame
-// instruction stream.  The stream cursors go in and come back by value; everything else lives in shared memory.
+// ---- the pre-pass.  Inlined: a wgmma pipeline must not cross a call boundary -- with the pre-pass out of line ptxas
+// serialised every MMA in it (C7510).  The stream cursors go in and come back by value; everything else lives in shared memory.
 template <bool PROF>
-__device__ __noinline__ Stream prepass(const DecParams& P, Smem& S, Stream st, int j, int b0, int G, int rank, float* scr) {
+__device__ __forceinline__ Stream prepass(const DecParams& P, Smem& S, Stream st, int j, int b0, int G, int rank, float* scr,
+                                          __half* c1s) {
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const size_t c1_utt = (size_t)(P.L[P.n_enc].cin / 16) * (TC_ASTAGE / 2);   // halfs of one utterance's C_1 planes
 
             // ---- pre-pass: rows t < j of the moved utterances under the new window (uniform branch: see the file header) ----
             if (threadIdx.x == 0) { S.n_moved_frames++; for (int g = 0; g < G; ++g) S.n_moved_utt += S.moved[g]; }
@@ -703,7 +746,13 @@ __device__ __noinline__ Stream prepass(const DecParams& P, Smem& S, Stream st, i
                 *reinterpret_cast<float4*>(rr + lane * 8 + 4) = make_float4(ctx[4], ctx[5], ctx[6], ctx[7]);
                 *reinterpret_cast<float4*>(rr + P.d + lane * 8) = q0;
                 *reinterpret_cast<float4*>(rr + P.d + lane * 8 + 4) = q1;
+                // the same row as the first AudioDec block's A operand: slab-major planes, row t - t_lo of utterance g's stage
+                // images (lane holds channels lane * 8 .. + 8 of [ctx | q]: slab lane / 2 (+ d / 16), k8 group lane % 2)
+                __half* cs = c1s + (size_t)g * c1_utt + (size_t)(lane >> 1) * (TC_ASTAGE / 2) + (lane & 1) * (TC_RA * 8) + (t - ra.t_lo) * 8;
+                store_split8(cs, ctx);
+                store_split8(cs + (size_t)(P.d >> 4) * (TC_ASTAGE / 2), qv);
             }
+            fence_proxy_async_global();                   // the plane rows are read by bulk copies after the barrier
             cluster_sync_all();
             LAP(LP_PYR_ATT);
             for (int lp = P.n_enc; lp < P.nl && P.L[lp].prow > 1; ++lp) {
@@ -721,7 +770,7 @@ __device__ __noinline__ Stream prepass(const DecParams& P, Smem& S, Stream st, i
                     for (int g = 0; g < G; ++g) {
                         if (!((rl.mask >> g) & 1u)) continue;
                         float* rows = scr + (size_t)pre_off_of(rl, g) * 512;
-                        pyr_tc_utt(P, S, lp, st.tcq, b0 + g, rl.t_lo, rl.n, rank, rows);
+                        pyr_tc_utt(P, S, lp, st.tcq, b0 + g, rl.t_lo, rl.n, rank, rows, lp == P.n_enc ? c1s + (size_t)g * c1_utt : nullptr);
                         st.tcq += l.cin / 16;
                     }
                 }
@@ -737,6 +786,7 @@ __device__ __noinline__ Stream prepass(const DecParams& P, Smem& S, Stream st, i
                 LAP(LP_PYR_BAR);
                 pyr_ln(P, S, lp, b0, rl, rank, scr);
                 LAP(LP_PYR_LN);
+                fence_proxy_async_global();               // refreshed plane rows -> the next block's bulk copies
                 cluster_sync_all();
                 LAP(LP_PYR_BAR);
             }
@@ -761,12 +811,13 @@ decode_cluster_kernel(const __grid_constant__ DecParams Pc) {
     const int b0 = cluster * P.G;
     const int G = min(P.G, P.B - b0);
     float* scr = P.pre_scr + (size_t)cluster * P.G * 85 * 512;
+    __half* c1s = P.pl_c1 + (size_t)cluster * P.G * (P.L[P.n_enc].cin / 16) * (TC_ASTAGE / 2);
 
     if (tid == 0) {
         for (int s = 0; s < DEC_NSLOT; ++s)
             for (int w = 0; w < NWARP; ++w) mbar_init(bar64(&S.fullw[s][w]), 1);
         mbar_init(bar64(&S.gbar[0]), 1); mbar_init(bar64(&S.gbar[1]), 1);
-        for (int i = 0; i < TC_NSTG; ++i) { mbar_init(bar64(&S.sbar[i]), 1); mbar_init(bar64(&S.abar[i]), TC_LOADW); }
+        for (int i = 0; i < TC_NSTG; ++i) { mbar_init(bar64(&S.sbar[i]), 1); mbar_init(bar64(&S.abar[i]), 1); }
         fence_mbar_init();
     }
     for (int i = tid; i < 2 * GMAX * XLD; i += NT) (&S.xin[0][0][0])[i] = 0.f;
@@ -793,10 +844,10 @@ decode_cluster_kernel(const __grid_constant__ DecParams Pc) {
     __syncthreads();
     if (tid == 0) S.prof_last = clock64();
     for (int j = 0; j < P.steps; ++j) {
-        if (tid < GMAX) S.moved[tid] = (tid < G && j > 0 && S.p_cur[tid] != S.p_prev[tid]) ? 1 : 0;
+        if (tid < GMAX) S.moved[tid] = (tid < G && j > 0 && (P.force_prepass || S.p_cur[tid] != S.p_prev[tid])) ? 1 : 0;
         if (tid == 0) {
             int any = 0;
-            for (int g = 0; g < G; ++g) any |= (j > 0 && S.p_cur[g] != S.p_prev[g]) ? 1 : 0;
+            for (int g = 0; g < G; ++g) any |= (j > 0 && (P.force_prepass || S.p_cur[g] != S.p_prev[g])) ? 1 : 0;
             S.fmoved[j & 1] = any;
         }
         __syncthreads();
@@ -822,13 +873,14 @@ decode_cluster_kernel(const __grid_constant__ DecParams Pc) {
         cb ^= 1;
         LAP(LP_ATT);
 
-        if (any_moved) st = prepass<PROF>(P, S, st, j, b0, G, rank, scr);
+        if (any_moved) st = prepass<PROF>(P, S, st, j, b0, G, rank, scr, c1s);
         }   // li == n_enc
         cb = layer_row<PROF, GT>(P, S, st, li, j, b0, G, rank, cb, lcount);
         }   // blocks
 
         __syncthreads();
         if (tid < GMAX) { S.p_prev[tid] = S.p_cur[tid]; S.p_cur[tid] = S.p_next[tid]; }
+        fence_proxy_async_global();                       // this frame's plane rows: read by bulk copies in later frames
         cluster_sync_all();                               // this frame's history rows are visible to the whole cluster
         LAP(LP_FRAME);
     }

@@ -3,6 +3,7 @@
 // Attention -> AudioDec for all mel frames, streaming its slice of the 27 MB of decode weights
 // from L2 through a TMA-bulk ring.  See kernels_decode.cu for the design.
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -17,6 +18,7 @@ constexpr int DEC_SLOT_F = 8 * DEC_REG_F;   // 48 KB per slot
 constexpr int DEC_MAXL = 24;        // 13 AudioEnc + 11 AudioDec blocks
 constexpr int DEC_MAXCH = 48;       // weight chunks per frame
 constexpr int DEC_PRM_F = 1024 + 64;   // per-layer parameter block: gamma1 | beta1 | gamma2 | beta2 (256 each) | bias slice
+constexpr int DEC_PL_PAD = 96;      // zero rows in front of t = 0 in the split-fp16 plane histories (>= the tallest source window)
 
 struct DecLayer {
     int kind;        // 0 conv1d (LN, optional relu), 1 hc (two LNs, sigmoid gate, highway mix)
@@ -46,6 +48,12 @@ struct DecParams {
     float* ybuf;                       // (B, T, n_mels)
     float* rbuf;                       // (B, T, 2d)
     float* pre_scr;                    // [clusters][G * max prow][512] pre-LN scratch of the recompute path
+    // The recompute path's A operand: the layer's input history a second time as split-fp16 planes in the wgmma no-swizzle
+    // K-major slab layout, per utterance [cin/16 slabs][plane hi, lo][k8 group][DEC_PL_PAD + T rows][8 halfs]; the first
+    // DEC_PL_PAD rows stay zero (TF's causal zero padding).  nullptr for layers the recompute does not read this way.
+    __half* pl_hist[DEC_MAXL];
+    __half* pl_c1;                     // [clusters * G][cin/16][2][2][DEC_PL_PAD][8]: the recomputed rows of the first AudioDec block's input
+    int pl_rows;                       // DEC_PL_PAD + T
     int* p_hist;                       // (B, T) window used at every step
     int* p_final;                      // (B) window after the last step
     float inv_scale[DEC_MAXL];         // 1 / (power-of-two scale of the block's split-fp16 weight planes), tensor-core pre-pass
@@ -53,6 +61,7 @@ struct DecParams {
     long long* prof;                   // optional [16] SM-clock lap timers of cluster 0 / rank 0 (option decode_prof), else nullptr
     int nl, n_enc, nch, nch_enc, pyr_ch0, pyr_ch1, stream_len;   // pyr_ch0..pyr_ch1: chunks of the AudioDec blocks with prow > 1
     int B, G, T, N, d, n_mels, win_size, steps;
+    int force_prepass;                 // option decode_force_prepass: every utterance recomputes at every frame j >= 1
 };
 static_assert(sizeof(DecParams) <= 4000, "DecParams must fit the kernel parameter space");
 

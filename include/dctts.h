@@ -196,6 +196,8 @@ int dctts_set_tensor_path(dctts_handle h, int32_t mode);
  *                  0 = one captured CUDA graph per mel frame (round-1 path)
  *   "tc_occ2" 0/1, "tc_mcast" 0/1, "tc_resid_tma" 0/1: wgmma block kernel variants
  *   "fused_ln" 0/1: graph decode, GEMM + LN in one launch;  "tc_debug" 0/1;  "decode_prof" 0/1;  "pdl" 0/1 (process-wide)
+ *   "decode_force_prepass" 0/1: measurement / test switch of the persistent decode (default 0): every utterance takes the
+ *                  receptive-field recompute at every frame j >= 1, as if its attention window had moved (the worst case)
  *   "train_tc" 0..7: training GEMMs on wgmma, bit mask 1 forward conv (+ wgmma attention), 2 data gradient, 4 weight gradient
  * dctts_get_option also answers "decode_available" (1 when this handle / device can run the persistent decode) and
  * "decode_max_clusters" (16-CTA clusters of the decode kernel that are co-resident on this device). */

@@ -17,9 +17,14 @@ ap.add_argument("--steps", type=int, default=210)
 ap.add_argument("--modes", default="1,0", help="decode modes to time: 1 persistent cluster kernel, 0 graph per frame")
 ap.add_argument("--iters", type=int, default=5)
 ap.add_argument("--prof", action="store_true", help="print the in-kernel lap timers of the persistent decode")
+ap.add_argument("--option", action="append", default=[], metavar="NAME=VALUE",
+                help="engine option to set first, e.g. decode_force_prepass=1 (the recompute at every frame)")
 a = ap.parse_args()
 e = Engine(0)
 e.load_params(init_params(0, "perturbed"))
+for kv in a.option:
+    name, val = kv.split("=")
+    e.set_option(name, int(val))
 print("decode_available", e.get_option("decode_available"), "max co-resident clusters", e.get_option("decode_max_clusters"), flush=True)
 for B in a.batches:
     L = synthetic_text(B, 100, seed=0)
