@@ -130,6 +130,7 @@ struct dctts_handle_s {
 
     // training step (Text2Mel, reference train.py mode "train"): see the "training" section below
     struct TrainLayer {
+        // rows / L / L_in are this step's extents (train_set_shape); pre / out point at capacity-sized slices
         LayerDev* l = nullptr; int li = 0; long long rows = 0; int L = 0, L_in = 0, ld_out = 0; const float* in = nullptr; int ld_in = 0;
         float* pre = nullptr; float* out = nullptr; int extra_shift = 0; bool need_dgrad = true;
         float *dW = nullptr, *dbias = nullptr, *dg1 = nullptr, *db1 = nullptr, *dg2 = nullptr, *db2 = nullptr;
@@ -137,7 +138,7 @@ struct dctts_handle_s {
     };
     struct TrainTensor { float* p; float* g; float* m; float* v; long long n; int layout, d0, d1, d2, ld; };
     struct {
-        bool ready = false; int B = 0, num = 1, T_in = 0; float rate = 0.f;
+        bool ready = false; int B = 0, num = 1, T_in = 0; float rate = 0.f;   // T_in: capacity in mel frames (num = 1: hp.max_T)
         std::vector<TrainLayer> layers;
         std::map<std::string, TrainTensor> tensors;            // by TF variable name
         DevBuf pre, out, emb, R, align, dS, gbuf[4], dy, wT, zeros, gts, sums, ids, grads, mom, vel, entries;
@@ -1196,6 +1197,25 @@ void ensure_scratch(H* h, size_t bytes) {
 // config 5).  Forward = the fp32 block kernels with every pre-LN tensor kept; backward = kernels_train.cu.  Gradients, Adam
 // moments and the pointers of all trained variables live in three arenas with identical offsets (the gradient arena is
 // what a data-parallel all-reduce sums).  Activation / gradient rows use a leading dimension rounded to 4 floats (F = 1025).
+// Buffers are sized for a capacity -- (hp.max_N, hp.max_T) for Text2Mel, (T_in) for SSRN -- and every step runs at its
+// batch's own (N, T) up to it (train_set_shape), as the reference's dynamically padded buckets do (data_load.py:122-129).
+
+// The extents of every block for a step at (N, T): TextEnc runs over N text positions, the other networks over T frames,
+// doubled by each transposed convolution.  Rows are packed at this shape from the start of each capacity-sized buffer, so
+// the dropout mask -- a hash of the flat element index -- is the one of the tensor at the step's shape.
+void train_set_shape(H* h, int N, int T) {
+    auto& tr = h->tr;
+    for (int net = 0; net < (tr.num == 1 ? 3 : 1); ++net) {
+        int L = (tr.num == 1 && net == 0) ? N : T;
+        for (int i = tr.first[net]; i <= tr.last[net]; ++i) {
+            auto& t = tr.layers[i];
+            t.L_in = L;
+            if (t.l->kind == K_D) L *= 2;
+            t.L = L; t.rows = (long long)tr.B * L;
+        }
+    }
+}
+
 void train_init(H* h, int B, float rate, int num, int T_in) {
     REQUIRE(h->committed, "dctts_train_init: parameters must be committed first");
     REQUIRE(B >= 1 && rate >= 0.f && rate < 1.f && (num == 1 || num == 2) && T_in >= 1, "dctts_train_init: bad arguments");
@@ -1220,30 +1240,33 @@ void train_init(H* h, int B, float rate, int num, int T_in) {
     int li = 0;
     for (size_t net = 0; net < nets.size(); ++net) {
         tr.first[net] = li;
-        int L = (num == 1 && net == 0) ? N : T;
         for (auto& l : *nets[net]) {
             H::TrainLayer t;
-            t.l = &l; t.li = li++; t.L_in = L;
-            if (l.kind == K_D) L *= 2;
-            t.L = L; t.rows = (long long)B * L; t.ld_out = roundup(l.cout, 4);
-            pre_f += (size_t)t.rows * l.ldw; out_f += (size_t)t.rows * t.ld_out;
-            g_f = std::max(g_f, (size_t)t.rows * std::max(t.ld_out, roundup(l.cin, 4)));
-            dy_f = std::max(dy_f, (size_t)t.rows * l.ldw);
-            wt_f = std::max(wt_f, (size_t)l.size * l.ldw * roundup(l.cin, 4));
-            {   // operand planes of the tensor-core GEMMs: activations / gradients (plain and transposed), packed weights
-                const size_t rows_in = (size_t)B * t.L_in, cmax = (size_t)roundup(std::max(l.cin, l.ldw), 8);
-                tca_f = std::max(tca_f, std::max(rows_in * cmax, (size_t)l.size * B * roundup(l.cin, 8) * roundup(t.L_in, 8)));
-                tcb_f = std::max(tcb_f, std::max((size_t)B * cmax * roundup(t.L_in, 8),
-                                                 (size_t)l.size * roundup(std::max(l.cin, l.ldw) + 255, 256) * roundup(std::max(l.cin, l.ldw), 32)));
-            }
-            Off o{};
-            o.W = reserve((long long)l.size * l.cin * l.ldw); o.bias = reserve(l.ldw);
-            o.g1 = reserve(l.cout); o.b1 = reserve(l.cout);
-            if (l.kind == K_HC) { o.g2 = reserve(l.cout); o.b2 = reserve(l.cout); }
-            offs.push_back(o);
+            t.l = &l; t.li = li++;
             tr.layers.push_back(t);
         }
         tr.last[net] = li - 1;
+    }
+    tr.B = B; tr.num = num;
+    train_set_shape(h, N, T);                                    // the capacity: every buffer below is sized for it
+    for (auto& t : tr.layers) {
+        const LayerDev& l = *t.l;
+        t.ld_out = roundup(l.cout, 4);
+        pre_f += (size_t)t.rows * l.ldw; out_f += (size_t)t.rows * t.ld_out;
+        g_f = std::max(g_f, (size_t)t.rows * std::max(t.ld_out, roundup(l.cin, 4)));
+        dy_f = std::max(dy_f, (size_t)t.rows * l.ldw);
+        wt_f = std::max(wt_f, (size_t)l.size * l.ldw * roundup(l.cin, 4));
+        {   // operand planes of the tensor-core GEMMs: activations / gradients (plain and transposed), packed weights
+            const size_t rows_in = (size_t)B * t.L_in, cmax = (size_t)roundup(std::max(l.cin, l.ldw), 8);
+            tca_f = std::max(tca_f, std::max(rows_in * cmax, (size_t)l.size * B * roundup(l.cin, 8) * roundup(t.L_in, 8)));
+            tcb_f = std::max(tcb_f, std::max((size_t)B * cmax * roundup(t.L_in, 8),
+                                             (size_t)l.size * roundup(std::max(l.cin, l.ldw) + 255, 256) * roundup(std::max(l.cin, l.ldw), 32)));
+        }
+        Off o{};
+        o.W = reserve((long long)l.size * l.cin * l.ldw); o.bias = reserve(l.ldw);
+        o.g1 = reserve(l.cout); o.b1 = reserve(l.cout);
+        if (l.kind == K_HC) { o.g2 = reserve(l.cout); o.b2 = reserve(l.cout); }
+        offs.push_back(o);
     }
     tr.pre.ensure(pre_f * sizeof(float)); tr.out.ensure(out_f * sizeof(float));
     if (num == 1) {
@@ -1434,11 +1457,19 @@ void train_read_losses(H* h, float* losses_host, double n_el, double n_att, cuda
     losses_host[0] = losses_host[1] + losses_host[2] + losses_host[3];
 }
 
-void train_forward_backward(H* h, const int* L, const float* mels, int B, uint32_t seed, float* losses_host, cudaStream_t s) {
+// One Text2Mel step on L (B, N) and mels (B, T, n_mels), packed at that shape, N <= hp.max_N and T <= hp.max_T.  The losses
+// are the reference's at this shape (train.py:83-95): means over B T n_mels, the guided-attention sum over the N x T corner of
+// the (max_N, max_T) table divided by B N T.  The softmax sees N keys and TextEnc's SAME padding the edge at N.
+void train_forward_backward(H* h, const int* L, int N, const float* mels, int T, int B, uint32_t seed, float* losses_host,
+                            cudaStream_t s) {
     auto& tr = h->tr;
     REQUIRE(tr.ready && tr.num == 1 && tr.B == B, "dctts_train_step: call dctts_train_init with this batch size first");
     const dctts_hparams& hp = h->hp;
-    const int N = hp.max_N, T = hp.max_T, d = hp.d;
+    REQUIRE(N >= 1 && N <= hp.max_N && T >= 1 && T <= hp.max_T,
+            "dctts_train_step: N = " + std::to_string(N) + ", T = " + std::to_string(T) + " outside the handle's capacity (1..max_N = " +
+            std::to_string(hp.max_N) + ", 1..max_T = " + std::to_string(hp.max_T) + ")");
+    const int d = hp.d;
+    train_set_shape(h, N, T);
     Launch lc{h, s};
     CUDA_CHECK(cudaMemsetAsync(tr.grads.p, 0, tr.n_grad * sizeof(float), s));
     CUDA_CHECK(cudaMemsetAsync(tr.sums.p, 0, 4 * sizeof(double), s));
@@ -1463,7 +1494,7 @@ void train_forward_backward(H* h, const int* L, const float* mels, int B, uint32
     float* gR = train_bwd(h, lc, tr.first[2], tr.last[2], B, seed, tr.gbuf[0].as<float>(), tr.gbuf[1].as<float>());
     AttnBwdArgs ab{};
     ab.gR = gR; ab.Q = Q; ab.ldq = d; ab.K = KV; ab.V = KV + d; ab.ldkv = 2 * d; ab.align = tr.align.as<float>();
-    ab.gts = tr.gts.as<float>(); ab.dS = tr.dS.as<float>(); ab.gQ = tr.gbuf[2].as<float>(); ab.gKV = tr.gbuf[3].as<float>();
+    ab.gts = tr.gts.as<float>(); ab.ld_gts = hp.max_T; ab.dS = tr.dS.as<float>(); ab.gQ = tr.gbuf[2].as<float>(); ab.gKV = tr.gbuf[3].as<float>();
     ab.B = B; ab.T = T; ab.N = N; ab.d = d; ab.att_scale = 1.0f / ((float)B * (float)N * (float)T);
     launch_attn_bwd(ab, tr.sums.as<double>(), s); lc.count(3);
     float* free_a = (gR == tr.gbuf[0].as<float>()) ? tr.gbuf[1].as<float>() : tr.gbuf[0].as<float>();
@@ -1474,10 +1505,15 @@ void train_forward_backward(H* h, const int* L, const float* mels, int B, uint32
     train_read_losses(h, losses_host, (double)B * T * hp.n_mels, (double)B * N * T, s);
 }
 
-// SSRN (num = 2): ground-truth mels in, L1 + binary divergence against the linear magnitudes (train.py:100-108)
-void train_forward_backward_ssrn(H* h, const float* mels, const float* mags, int B, uint32_t seed, float* losses_host, cudaStream_t s) {
+// SSRN (num = 2): ground-truth mels (B, T, n_mels) in, L1 + binary divergence against the linear magnitudes (B, 4T, F), means
+// over B 4T F (train.py:100-108); T up to the capacity given to dctts_train_init_ssrn
+void train_forward_backward_ssrn(H* h, const float* mels, const float* mags, int B, int T, uint32_t seed, float* losses_host,
+                                 cudaStream_t s) {
     auto& tr = h->tr;
     REQUIRE(tr.ready && tr.num == 2 && tr.B == B, "dctts_train_step_ssrn: call dctts_train_init_ssrn with this batch size first");
+    REQUIRE(T >= 1 && T <= tr.T_in, "dctts_train_step_ssrn: T = " + std::to_string(T) + " outside the handle's capacity (1.." +
+            std::to_string(tr.T_in) + ", set by dctts_train_init_ssrn)");
+    train_set_shape(h, 0, T);
     Launch lc{h, s};
     CUDA_CHECK(cudaMemsetAsync(tr.grads.p, 0, tr.n_grad * sizeof(float), s));
     CUDA_CHECK(cudaMemsetAsync(tr.sums.p, 0, 4 * sizeof(double), s));
@@ -1890,14 +1926,19 @@ int dctts_train_init(dctts_handle h, int32_t B, float dropout_rate) {
     return guarded(h, [&] { train_init(h, B, dropout_rate, 1, h->hp.max_T); });
 }
 
-int dctts_train_step(dctts_handle h, const int32_t* L, const float* mels, int32_t B, int64_t global_step, uint32_t seed, float lr,
-                     int32_t apply, float* losses_host, void* stream) {
+int dctts_train_step_shaped(dctts_handle h, const int32_t* L, int32_t N, const float* mels, int32_t T, int32_t B, int64_t global_step,
+                            uint32_t seed, float lr, int32_t apply, float* losses_host, void* stream) {
     return guarded(h, [&] {
         REQUIRE(L && mels && B >= 1 && global_step >= 0, "dctts_train_step: bad arguments");
         cudaStream_t s = S(h, stream);
-        train_forward_backward(h, reinterpret_cast<const int*>(L), mels, B, seed, losses_host, s);
+        train_forward_backward(h, reinterpret_cast<const int*>(L), N, mels, T, B, seed, losses_host, s);
         if (apply) train_apply(h, global_step, lr, s);
     });
+}
+
+int dctts_train_step(dctts_handle h, const int32_t* L, const float* mels, int32_t B, int64_t global_step, uint32_t seed, float lr,
+                     int32_t apply, float* losses_host, void* stream) {
+    return dctts_train_step_shaped(h, L, h ? h->hp.max_N : 0, mels, h ? h->hp.max_T : 0, B, global_step, seed, lr, apply, losses_host, stream);
 }
 
 int dctts_train_apply(dctts_handle h, int64_t global_step, float lr, void* stream) {
@@ -1915,14 +1956,20 @@ int dctts_train_init_ssrn(dctts_handle h, int32_t B, int32_t T, float dropout_ra
     return guarded(h, [&] { train_init(h, B, dropout_rate, 2, T); });
 }
 
-int dctts_train_step_ssrn(dctts_handle h, const float* mels, const float* mags, int32_t B, int64_t global_step, uint32_t seed, float lr,
-                          int32_t apply, float* losses_host, void* stream) {
+int dctts_train_step_ssrn_shaped(dctts_handle h, const float* mels, const float* mags, int32_t B, int32_t T, int64_t global_step,
+                                 uint32_t seed, float lr, int32_t apply, float* losses_host, void* stream) {
     return guarded(h, [&] {
         REQUIRE(mels && mags && B >= 1 && global_step >= 0, "dctts_train_step_ssrn: bad arguments");
         cudaStream_t s = S(h, stream);
-        train_forward_backward_ssrn(h, mels, mags, B, seed, losses_host, s);
+        train_forward_backward_ssrn(h, mels, mags, B, T, seed, losses_host, s);
         if (apply) train_apply(h, global_step, lr, s);
     });
+}
+
+int dctts_train_step_ssrn(dctts_handle h, const float* mels, const float* mags, int32_t B, int64_t global_step, uint32_t seed, float lr,
+                          int32_t apply, float* losses_host, void* stream) {
+    const int32_t T = h ? h->tr.T_in : 0;              // the capacity given to dctts_train_init_ssrn
+    return dctts_train_step_ssrn_shaped(h, mels, mags, B, T, global_step, seed, lr, apply, losses_host, stream);
 }
 
 int dctts_train_tensor(dctts_handle h, const char* tf_name, int32_t what, float* host_out, int64_t count) {

@@ -159,7 +159,7 @@ struct AttnBwdArgs {
     const float* gR;                   // (B,T,2d) gradient of [ctx ; Q]
     const float* Q; int ldq; const float* K; const float* V; int ldkv;
     const float* align;                // (B,N,T) probabilities of the forward pass
-    const float* gts;                  // (N,T) guided-attention weights
+    const float* gts; int ld_gts;      // guided-attention weights (max_N, max_T), row stride ld_gts; the (N, T) corner is read
     float* dS;                         // (B,T,N) scratch
     float* gQ;                         // (B,T,d)
     float* gKV;                        // (B,N,2d)

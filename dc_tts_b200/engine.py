@@ -298,29 +298,44 @@ class Engine:
         self._check(self._lib.dctts_train_init(self._h, int(B), float(rate)), "dctts_train_init")
 
     def train_step(self, L, mels, global_step=0, seed=0, lr=None, apply=True):
-        """One Text2Mel optimiser step on L (B, max_N) int32 / mels (B, max_T, n_mels): forward with dropout, losses
-        (train.py:83-99), backward, clip, Adam (train.py:122-132).  Returns {loss, loss_mels, loss_bd1, loss_att}."""
+        """One Text2Mel optimiser step on L (B, N) int32 / mels (B, T, n_mels) at the batch's own shape -- a bucket padded
+        to its longest member (trainer.bucketed_batches) or the fixed (max_N, max_T) -- up to N = hp.max_N, T = hp.max_T:
+        forward with dropout, losses (train.py:83-99), backward, clip, Adam (train.py:122-132).
+        Returns {loss, loss_mels, loss_bd1, loss_att}."""
         L = self._i32(L); mels = self._f32(mels)
+        if L.dim() != 2:
+            raise DcttsError("train_step: L must be (B, N), got shape %s" % (tuple(L.shape),))
+        B, N = L.shape
+        if mels.dim() != 3 or mels.shape[0] != B or mels.shape[2] != self.hp.n_mels:
+            raise DcttsError("train_step: mels must be (B=%d, T, n_mels=%d), got shape %s" % (B, self.hp.n_mels, tuple(mels.shape)))
         out = (C.c_float * 4)()
-        self._check(self._lib.dctts_train_step(self._h, _ptr(L), _ptr(mels), L.shape[0], int(global_step), int(seed) & 0xffffffff,
-                                               float(self.hp.lr if lr is None else lr), 1 if apply else 0, out, self._stream()),
-                    "dctts_train_step")
+        self._check(self._lib.dctts_train_step_shaped(self._h, _ptr(L), N, _ptr(mels), mels.shape[1], B, int(global_step),
+                                                      int(seed) & 0xffffffff, float(self.hp.lr if lr is None else lr),
+                                                      1 if apply else 0, out, self._stream()), "dctts_train_step")
         return {"loss": out[0], "loss_mels": out[1], "loss_bd1": out[2], "loss_att": out[3]}
 
     def train_init_ssrn(self, B, T=None, dropout_rate=None):
-        """Training workspace for the SSRN trainer (train.py num=2): mels (B, T, n_mels) -> mags (B, 4T, F).
+        """Training workspace for the SSRN trainer (train.py num=2): mels (B, T, n_mels) -> mags (B, 4T, F) for any T up
+        to the capacity `T` (default hp.max_T).
         Measured parity: all 80 gradient tensors within 6e-6 of the autograd checker's (DESIGN.md 8e)."""
         rate = self.hp.dropout_rate if dropout_rate is None else dropout_rate
         self._check(self._lib.dctts_train_init_ssrn(self._h, int(B), int(self.hp.max_T if T is None else T), float(rate)),
                     "dctts_train_init_ssrn")
 
     def train_step_ssrn(self, mels, mags, global_step=0, seed=0, lr=None, apply=True):
-        """One SSRN optimiser step on ground-truth mels / mags (train.py:69-72,100-108,122-132)."""
+        """One SSRN optimiser step on ground-truth mels (B, T, n_mels) / mags (B, 4T, F) at the batch's own T, up to the
+        capacity of train_init_ssrn (train.py:69-72,100-108,122-132)."""
         mels = self._f32(mels); mags = self._f32(mags)
+        if mels.dim() != 3 or mels.shape[2] != self.hp.n_mels:
+            raise DcttsError("train_step_ssrn: mels must be (B, T, n_mels=%d), got shape %s" % (self.hp.n_mels, tuple(mels.shape)))
+        B, T = mels.shape[0], mels.shape[1]
+        if tuple(mags.shape) != (B, self.hp.r * T, self.F):
+            raise DcttsError("train_step_ssrn: mags must be (B, %d T, F) = %s for mels %s, got %s"
+                             % (self.hp.r, (B, self.hp.r * T, self.F), tuple(mels.shape), tuple(mags.shape)))
         out = (C.c_float * 4)()
-        self._check(self._lib.dctts_train_step_ssrn(self._h, _ptr(mels), _ptr(mags), mels.shape[0], int(global_step), int(seed) & 0xffffffff,
-                                                    float(self.hp.lr if lr is None else lr), 1 if apply else 0, out, self._stream()),
-                    "dctts_train_step_ssrn")
+        self._check(self._lib.dctts_train_step_ssrn_shaped(self._h, _ptr(mels), _ptr(mags), B, T, int(global_step),
+                                                           int(seed) & 0xffffffff, float(self.hp.lr if lr is None else lr),
+                                                           1 if apply else 0, out, self._stream()), "dctts_train_step_ssrn")
         return {"loss": out[0], "loss_mags": out[1], "loss_bd2": out[2]}
 
     def train_apply(self, global_step, lr=None):

@@ -94,3 +94,19 @@ def synthetic_text(batch, n_chars=100, seed=0, first_index=0):
         L[i, :n_chars] = rng.integers(2, len(hp.vocab), size=n_chars)
         L[i, n_chars] = 1
     return L
+
+
+def synthetic_bucket(batch, N, T, seed=0):
+    """A synthetic length-bucketed batch in the shape trainer.bucketed_batches emits (dynamic padding to the longest
+    member): L (batch, N) int32 and mels (batch, T, n_mels).  Row 0 is the longest member (N - 1 ids uniform in [2, 31],
+    then E); row b has N - bN/(2 batch) positions and T - bT/(2 batch) frames uniform in [0, 1), zero padded after them."""
+    from .hyperparams import Hyperparams as hp
+    rng = np.random.default_rng([seed, N, T])
+    L = np.zeros((batch, N), np.int32)
+    mels = np.zeros((batch, T, hp.n_mels), np.float32)
+    for b in range(batch):
+        n, t = N - (b * N) // (2 * batch), T - (b * T) // (2 * batch)
+        L[b, :n - 1] = rng.integers(2, len(hp.vocab), size=n - 1)
+        L[b, n - 1] = 1
+        mels[b, :t] = rng.uniform(0, 1, (t, hp.n_mels))
+    return L, mels

@@ -45,7 +45,9 @@ _TRAIN = {1: ("loss", "loss_mels", "loss_bd1", "loss_att"), 2: ("loss", "loss_ma
 class Graph:
     def __init__(self, num=1, mode="train", engine=None, fused=True, batches=None, num_batch=None, global_step=0):
         """mode "synthesize": the inference graph.  mode "train" (the reference default): `num` = 1 trains Text2Mel, 2 SSRN;
-        `batches` is the input pipeline, an iterator of (L, mels, mags, ...) tuples with fixed shapes (trainer.py)."""
+        `batches` is the input pipeline, an iterator of (L, mels, mags, ...) tuples -- trainer.bucketed_batches(...) at each
+        batch's own shape, or trainer.fixed_size_batches(...).  Batches beyond the capacity (hp.max_N, hp.max_T) are
+        skipped and counted in `skipped_batches`."""
         if mode not in ("train", "synthesize"):
             raise ValueError("mode: 'train' or 'synthesize' (train.py:22)")
         self.char2idx, self.idx2char = load_vocab()
@@ -57,11 +59,12 @@ class Graph:
                 raise ValueError("num: 1 for Text2Mel, 2 for SSRN (train.py:24)")
             if batches is None:
                 raise ValueError("Graph(mode='train') needs `batches`: the reference reads them from data_load.get_batch(); "
-                                 "here pass trainer.fixed_size_batches(...) or bucketed batches through pad_to_fixed")
+                                 "here pass trainer.bucketed_batches(...) or trainer.fixed_size_batches(...)")
             self.batches = iter(batches)
             self.num_batch = num_batch                       # train.py:33; only used for the progress bar
             self.global_step_value = int(global_step)
             self.last = {}
+            self.skipped_batches = 0
             self._initialised = False
             for name in ("global_step", "train_op", "lr") + _TRAIN[num]:
                 setattr(self, name, Symbol(self, name))
@@ -91,14 +94,19 @@ class Graph:
 
     def _train_run(self, names):
         """One `sess.run` of the training graph: fetching train_op consumes a batch and applies one update."""
+        from .trainer import over_capacity
         from .utils import learning_rate_decay
         if "train_op" in names:
+            cap = getattr(self.engine, "hp", hp)
             L, mels, mags = next(self.batches)[:3]
+            while over_capacity(self.num, L, mels, cap):          # the workspace is not re-allocated: that would reset Adam
+                self.skipped_batches += 1
+                L, mels, mags = next(self.batches)[:3]
             if not self._initialised:
                 if self.num == 1:
                     self.engine.train_init(len(L))
                 else:
-                    self.engine.train_init_ssrn(len(L), mels.shape[1])
+                    self.engine.train_init_ssrn(len(L), cap.max_T)
                 self._initialised = True
             gs = self.global_step_value
             if self.num == 1:

@@ -5,11 +5,10 @@ pre-computed `mels/*.npy`, `mags/*.npy` of prepo.py (data_load.py:104-112).
 
 Batching: `bucketed_batches` restates the reference's length-bucketed, dynamically padded queue (data_load.py:88-131:
 shuffled stream, buckets by text length every 20 characters, a full bucket emits a batch padded to its own longest
-member).  The CUDA training step takes FIXED shapes (B, max_N) / (B, max_T, n_mels) / (B, 4 max_T, F) -- BASELINE
-config 5 -- so `pad_to_fixed` extends the bucket's zero padding to hp.max_N / hp.max_T (`fixed_size_batches` is the plain
-shuffled variant without buckets).  Remaining difference, documented in DESIGN.md: the reference's losses average over
-the bucket's own padded extent (train.py:85-88 have no mask), here over the fixed extent, and the non-causal TextEnc sees
-zero-INPUT positions beyond the bucket length where TF sees the edge of the tensor.
+member).  `train` and `Graph(num, mode="train")` take those batches as they are: the CUDA step runs at each batch's own
+(N_b, T_b), up to the capacity (hp.max_N, hp.max_T), and its losses are the reference's at that shape.  A batch beyond
+the capacity is skipped and counted.  `fixed_size_batches` (plain shuffled batches padded to (max_N, max_T), BASELINE
+config 5) and `pad_to_fixed` (a bucket padded further to the fixed shapes) remain for fixed-shape training.
 """
 import codecs
 import os
@@ -90,14 +89,15 @@ def bucket_index(length, boundaries):
     return int(np.searchsorted(np.asarray(boundaries), length, side="right"))
 
 
-def bucketed_batches(fpaths, text_lengths, texts, B=None, seed=0, loader=_load_spectrograms_npy, epochs=None):
+def bucketed_batches(fpaths, text_lengths, texts, B=None, seed=0, loader=_load_spectrograms_npy, epochs=None, rank=0, world=1):
     """The reference's input pipeline (data_load.py:88-131) without TensorFlow queues: a shuffled stream of utterances
     (slice_input_producer :99) is routed by TEXT length into buckets (boundaries :125); a bucket that has collected B
     utterances emits them as one batch, every tensor padded with zeros to the longest member of THAT batch
     (dynamic_pad=True, :128): L (B, N_b) int32, mels (B, T_b, n_mels), mags (B, 4 T_b', F).  Buckets keep their partial
     contents across epochs like the TF queue does; nothing is dropped except what never fills a bucket.
-    Yields (L, mels, mags, names, bucket).  `pad_to_fixed` turns a batch into the fixed (max_N, max_T) shapes the CUDA
-    training step takes."""
+    Yields (L, mels, mags, names, bucket), which `train` and `Graph(mode="train")` take directly.  Data-parallel runs:
+    like fixed_size_batches, every rank draws the SAME permutation (same seed) and keeps every world-th utterance, so the
+    ranks' batches are disjoint (their shapes may differ from rank to rank)."""
     B = B or hp.B
     bounds = bucket_boundaries(text_lengths)
     pending = [[] for _ in range(len(bounds) + 1)]
@@ -105,7 +105,7 @@ def bucketed_batches(fpaths, text_lengths, texts, B=None, seed=0, loader=_load_s
     epoch = 0
     while epochs is None or epoch < epochs:
         emitted = 0
-        for i in rng.permutation(len(fpaths)):
+        for i in rng.permutation(len(fpaths))[rank::world]:
             k = bucket_index(text_lengths[i], bounds)
             fname, mel, mag = loader(fpaths[i])
             pending[k].append((texts[i], mel, mag, fname))
@@ -127,9 +127,9 @@ def bucketed_batches(fpaths, text_lengths, texts, B=None, seed=0, loader=_load_s
 
 
 def pad_to_fixed(L, mels, mags):
-    """A bucketed batch in the fixed shapes of the CUDA training step ((B, max_N), (B, max_T, n_mels), (B, 4 max_T, F)),
-    or None when the bucket is longer than those (the reference has no such limit while training; BASELINE config 5 fixes
-    N = 180, T = 210).  Zero padding is what dynamic_pad already appended, just further."""
+    """A bucketed batch in the fixed shapes of BASELINE config 5 ((B, max_N), (B, max_T, n_mels), (B, 4 max_T, F)),
+    or None when the bucket is longer than those.  Zero padding is what dynamic_pad already appended, just further.
+    (The trainers take bucketed batches directly; padding changes the losses, see DESIGN.md 8e.)"""
     B, N_b = L.shape
     T_b, Tm_b = mels.shape[1], mags.shape[1]
     if N_b > hp.max_N or T_b > hp.max_T or Tm_b > hp.max_T * hp.r:
@@ -145,10 +145,17 @@ def checkpoint_name(logdir, gs):
     return os.path.join(logdir, "model_gs_{}".format(str(gs // 1000).zfill(3) + "k"))
 
 
+def over_capacity(num, L, mels, cap=hp):
+    """True when a batch does not fit the training workspace: Text2Mel N_b > max_N or T_b > max_T, SSRN T_b > max_T."""
+    return mels.shape[1] > cap.max_T or (num == 1 and L.shape[1] > cap.max_N)
+
+
 def train(num, engine, batches, num_iterations=None, logdir=None, global_step=None, save_every=1000, log=print, resume=True,
           rank=0, world=1, allreduce=None):
-    """train.py:137-160 for num = 1 (Text2Mel) or 2 (SSRN).  `batches` yields (L, mels, mags, names); `engine` is an
-    `Engine` with parameters loaded.  Like tf.train.Supervisor (train.py:144), a `logdir` that already holds a checkpoint
+    """train.py:137-160 for num = 1 (Text2Mel) or 2 (SSRN).  `batches` yields (L, mels, mags, names, ...): the bucketed
+    batches of `bucketed_batches` at their own shapes or fixed-size ones; `engine` is an `Engine` with parameters loaded.
+    The workspace is allocated once for the capacity (hp.max_N, hp.max_T); a batch beyond it is skipped and counted in the
+    log (re-allocating would reset the Adam state).  Like tf.train.Supervisor (train.py:144), a `logdir` that already holds a checkpoint
     is RESUMED: variables, Adam slots and the global step come back from it (`resume=False` or an explicit `global_step`
     starts over).  Data parallel (BASELINE config 5, `world` > 1): every rank feeds its own disjoint `batches`, the step
     runs with apply=False, `allreduce` (default dc_tts_b200.parallel.allreduce_mean_) averages the flat gradient arena,
@@ -160,13 +167,21 @@ def train(num, engine, batches, num_iterations=None, logdir=None, global_step=No
     logdir = logdir or (hp.logdir + "-" + str(num))
     os.makedirs(logdir, exist_ok=True)
     gs = int(global_step or 0)
+    cap = getattr(engine, "hp", hp)
     initialised = False
-    for L, mels, mags, _names in batches:
+    skipped = 0
+    for batch in batches:
+        L, mels, mags = batch[:3]
+        if over_capacity(num, L, mels, cap):
+            skipped += 1
+            log("skipped a batch of shape N=%d, T=%d beyond the capacity (max_N=%d, max_T=%d); %d skipped so far"
+                % (L.shape[1], mels.shape[1], cap.max_N, cap.max_T, skipped))
+            continue
         if not initialised:
             if num == 1:
                 engine.train_init(len(L))
             else:
-                engine.train_init_ssrn(len(L), mels.shape[1])
+                engine.train_init_ssrn(len(L), cap.max_T)
             if resume and global_step is None:
                 restored = engine.restore_training(logdir, "Text2Mel" if num == 1 else "SSRN")
                 if restored is not None:

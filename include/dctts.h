@@ -164,13 +164,26 @@ int dctts_get_spectrograms(dctts_handle h, const float* wav, int64_t n_samples, 
 int dctts_train_init(dctts_handle h, int32_t B, float dropout_rate);
 int dctts_train_step(dctts_handle h, const int32_t* L, const float* mels, int32_t B, int64_t global_step, uint32_t seed, float lr,
                      int32_t apply, float* losses_host, void* stream);
+/* The same step on a length-bucketed batch at its own shape (the reference's dynamic_pad=True, data_load.py:122-129):
+ * L (B, N) int32 and mels (B, T, n_mels), packed at that shape.  Capacity: 1 <= N <= max_N and 1 <= T <= max_T of the
+ * hparams the handle was created with (texts longer than 180 need a handle with a larger max_N, at most 192); B must be
+ * the batch size given to dctts_train_init.  A step outside the capacity fails with a message and launches nothing.
+ * The losses are the reference's at this shape: means over B T n_mels; the guided-attention sum over the N x T corner of
+ * the (max_N, max_T) weight table divided by B N T (train.py:91-95).  The softmax runs over the N keys and TextEnc's SAME
+ * padding sees the edge of the tensor at N.  dctts_train_step is this call at (max_N, max_T). */
+int dctts_train_step_shaped(dctts_handle h, const int32_t* L, int32_t N, const float* mels, int32_t T, int32_t B, int64_t global_step,
+                            uint32_t seed, float lr, int32_t apply, float* losses_host, void* stream);
 int dctts_train_apply(dctts_handle h, int64_t global_step, float lr, void* stream);
 /* The SSRN trainer (train.py num = 2: SSRN on the GROUND-TRUTH mels :69-72, losses :100-108, same optimiser): mels
  * (B, T, n_mels), mags (B, 4T, 1 + n_fft/2) DEVICE pointers; losses_host = {total, mags L1, binary divergence, 0}.
- * A handle trains one of the two networks at a time (the init call selects which). */
+ * A handle trains one of the two networks at a time (the init call selects which).  The T given to dctts_train_init_ssrn
+ * is a capacity: dctts_train_step_ssrn_shaped steps at any 1 <= T <= capacity (means over B 4T F), keeping the Adam state;
+ * a step beyond it fails with a message and launches nothing.  dctts_train_step_ssrn is this call at the capacity. */
 int dctts_train_init_ssrn(dctts_handle h, int32_t B, int32_t T, float dropout_rate);
 int dctts_train_step_ssrn(dctts_handle h, const float* mels, const float* mags, int32_t B, int64_t global_step, uint32_t seed, float lr,
                           int32_t apply, float* losses_host, void* stream);
+int dctts_train_step_ssrn_shaped(dctts_handle h, const float* mels, const float* mags, int32_t B, int32_t T, int64_t global_step,
+                                 uint32_t seed, float lr, int32_t apply, float* losses_host, void* stream);
 int dctts_train_grads(dctts_handle h, float** grads, int64_t* count);
 int dctts_train_tensor(dctts_handle h, const char* tf_name, int32_t what, float* host_out, int64_t count);
 /* Inverse of dctts_train_tensor for what = 0 (variable), 2 (Adam m), 3 (Adam v): restores a training state (resume). */

@@ -1,6 +1,7 @@
 """BASELINE config 5: Text2Mel training step, B = 32 per GPU, fixed N = 180 / T = 210, synthetic batch, dropout on,
 data-parallel over the launched ranks (gradient all-reduce of the flat arena over NCCL).  Prints one JSON line.
-    python tools/bench_train.py [--steps 10 --warmup 3 --batch 32]
+`--shape N,T` steps at a length bucket's own shape instead (the workspace keeps its (max_N, max_T) capacity).
+    python tools/bench_train.py [--steps 10 --warmup 3 --batch 32 --net 1 --shape 180,210]
     python -m torch.distributed.run --nproc-per-node N --master-addr 127.0.0.1 tools/bench_train.py"""
 import argparse
 import json
@@ -22,8 +23,10 @@ ap.add_argument("--warmup", type=int, default=3)
 ap.add_argument("--batch", type=int, default=32)
 ap.add_argument("--probe", type=int, default=0, help="measurement only: 1 = the wgmma GEMMs fetch their operands but issue no MMA (results are garbage)")
 ap.add_argument("--net", type=int, default=1, choices=[1, 2], help="1 = Text2Mel trainer (BASELINE config 5), 2 = SSRN trainer (train.py num=2) at T = 210")
+ap.add_argument("--shape", default="%d,%d" % (hp.max_N, hp.max_T), help="N,T of every step's batch (text positions, mel frames); SSRN uses T")
 ap.add_argument("--train-tc", type=int, default=7, help="bit mask: 1 forward conv, 2 data gradient, 4 weight gradient on wgmma (default 7 = all), 0 = fp32 CUDA-core kernels")
 a = ap.parse_args()
+N, T = (int(x) for x in a.shape.split(","))
 rank, world, local = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
 torch.cuda.set_device(local)
 if world > 1:
@@ -37,9 +40,9 @@ if a.net == 1:
     eng.train_init(B)
 else:
     eng.train_init_ssrn(B, hp.max_T)
-L = torch.from_numpy(synthetic_text(B, 100, seed=rank)).cuda()
-mels = torch.from_numpy(np.random.default_rng(rank).uniform(0, 1, (B, hp.max_T, hp.n_mels)).astype(np.float32)).cuda()
-mags = torch.from_numpy(np.random.default_rng(rank + 100).uniform(0, 1, (B, hp.max_T * hp.r, 1 + hp.n_fft // 2)).astype(np.float32)).cuda() if a.net == 2 else None
+L = torch.from_numpy(synthetic_text(B, min(100, N - 1), seed=rank)[:, :N]).cuda()
+mels = torch.from_numpy(np.random.default_rng(rank).uniform(0, 1, (B, T, hp.n_mels)).astype(np.float32)).cuda()
+mags = torch.from_numpy(np.random.default_rng(rank + 100).uniform(0, 1, (B, T * hp.r, 1 + hp.n_fft // 2)).astype(np.float32)).cuda() if a.net == 2 else None
 grads = eng.train_grads()
 
 
@@ -72,13 +75,15 @@ if world > 1:
     dist.all_reduce(ms, op=dist.ReduceOp.MAX)
 if rank == 0:
     ms = float(ms)
-    flops = 3 * 2 * B * (hp.max_N * 17.10e6 + hp.max_T * (4.08e6 + 2.71e6 + 0.09e6))          # SURVEY 8(d) config 5: fwd MACs x 2 x 3
+    flops = 3 * 2 * B * (N * 17.10e6 + T * (4.08e6 + 2.71e6 + 0.09e6))                    # SURVEY 8(d) config 5: fwd MACs x 2 x 3
     if a.net == 2:
-        flops = 3 * 2 * B * hp.max_T * 93.66e6                                                    # SSRN: 93.7 MMAC per mel frame
+        flops = 3 * 2 * B * T * 93.66e6                                                          # SSRN: 93.7 MMAC per mel frame
     print(json.dumps({"metric": "train_steps_per_sec", "value": 1e3 / ms, "unit": "steps/s", "n_gpus": world, "ms_per_step": ms,
-                      "mel_frames_per_sec": world * B * hp.max_T * 1e3 / ms, "steps": a.steps, "warmup": a.warmup,
-                      "config": {"workload": ("BASELINE config 5: Text2Mel train step (fwd + bwd + clip + Adam), B=%d per GPU, N=180, T=210, dropout %.2f" if a.net == 1 else
-                                              "SSRN train step (train.py num=2: fwd + bwd + clip + Adam), B=%d per GPU, T=210 -> 840 frames x 1025 bins, dropout %.2f") % (B, hp.dropout_rate),
+                      "mel_frames_per_sec": world * B * T * 1e3 / ms, "steps": a.steps, "warmup": a.warmup, "shape": {"N": N, "T": T},
+                      "config": {"workload": ("Text2Mel train step (fwd + bwd + clip + Adam), B=%d per GPU, N=%d, T=%d, dropout %.2f" % (B, N, T, hp.dropout_rate)
+                                              if a.net == 1 else
+                                              "SSRN train step (train.py num=2: fwd + bwd + clip + Adam), B=%d per GPU, T=%d -> %d frames x 1025 bins, dropout %.2f"
+                                              % (B, T, T * hp.r, hp.dropout_rate)),
                                  "parallelism": "dp%d (all-reduce of %d gradients)" % (world, grads.numel())},
                       "dtype": ("f32 tensors; GEMMs as split-fp16 x3 on wgmma, fp32 accumulate" if a.train_tc else "f32 (CUDA-core kernels)"), "data": "synthetic",
                       "achieved_tflops": world * flops / (ms * 1e-3) / 1e12, "gpu_launches_per_step": (eng.launch_count() - n0) // a.steps,
