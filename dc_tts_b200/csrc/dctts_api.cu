@@ -125,6 +125,7 @@ struct dctts_handle_s {
     DevBuf lbuf;                  // (B, N) ids staging for the host entry point
     DevBuf zbuf;                  // (B, 4T, F) staging for the host entry point
     DevBuf plane[4];              // tensor-core path activations: {hi,lo} x ping-pong, rows x 1032 fp16
+    DevBuf in_inv;                // (B) inverse per-utterance scales of a network input's planes (launch_f32_to_planes_scaled)
     DevBuf attpl[6];              // wgmma attention operands: Q, K planes and transposed V planes ({hi,lo} each)
     DevBuf arpl[10];              // AR decode planes: R (B,T,2d) and four AudioDec outputs (B,T,d), {hi,lo} each
 
@@ -197,6 +198,7 @@ struct dctts_handle_s {
         tickets.release(); scratch.release(); act0.release(); act1.release(); kv.release(); ybuf.release();
         rbuf.release(); ad_sig.release(); ibuf.release(); lbuf.release(); zbuf.release();
         for (auto& b : plane) b.release();
+        in_inv.release();
         for (auto& b : arpl) b.release();
         for (auto& b : attpl) b.release();
         voc_S.release(); voc_X.release(); voc_frames.release(); voc_mse.release(); voc_tw.release(); voc_window.release(); voc_wss.release(); voc_deemph.release();
@@ -621,6 +623,7 @@ void ensure_ws(H* h, int B) {
     h->ibuf.ensure((size_t)(4 + 3 * B + (size_t)B * T) * sizeof(int));
     h->lbuf.ensure((size_t)B * N * sizeof(int));
     for (auto& pb : h->plane) pb.ensure(rows_ssrn * (size_t)roundup(std::max(std::max(2 * hp.c, F), 2 * d), 8) * sizeof(__half));
+    h->in_inv.ensure((size_t)B * sizeof(float));
     for (int i = 0; i < 10; ++i) {
         const size_t bytes = (size_t)B * T * (i < 2 ? 2 * d : d) * sizeof(__half);
         h->arpl[i].ensure(bytes);
@@ -714,7 +717,7 @@ void run_deconv(Launch& lc, const LayerDev& l, const float* X, int ldx, int B, i
 
 bool chain_tc_ok(H* h, const std::vector<LayerDev>& net);
 void run_chain_tc_planes(Launch& lc, const std::vector<LayerDev>& net, Planes cur, int which, int B, int L,
-                         float* out, float* out_sig, int first_extra_shift);
+                         float* out, float* out_sig, int first_extra_shift, const float* in_inv);
 void run_chain_full_tc(Launch& lc, const std::vector<LayerDev>& net, const float* X, int ldx, int B, int L,
                        float* out, float* out_sig);
 
@@ -753,12 +756,14 @@ Planes ws_planes(H* h, int which, int C) {
 // (B, L, cin) input; the output goes to planes and/or fp32 tensors.
 void run_block_tc(Launch& lc, const LayerDev& l, int rate, bool causal, int act, Planes X, RowWin win,
                   int TT, int TB, int tiles_t, Planes out, float* out_f32, int ld_f32, float* sig_f32, int ld_sig,
-                  Planes sig, int extra_shift = 0) {
+                  Planes sig, int extra_shift = 0, const float* in_inv = nullptr) {
     const LayerDev::TcPack& p = l.tc;
     REQUIRE(p.ok, "tensor-core path not available for this block");
+    // the highway residual is read from the input planes unscaled; scaled input planes only reach conv1d blocks
+    REQUIRE(!in_inv || p.mode != 1, "hc block with scaled input planes");
     TcArgs a{};
     a.bias = l.bias; a.g1 = l.g1; a.b1 = l.b1; a.g2 = (p.mode == 1) ? l.g2 : l.g1; a.b2 = (p.mode == 1) ? l.b2 : l.b1;
-    a.mode = p.mode; a.act = act; a.C = l.cout; a.bn = p.bn; a.half = p.half; a.inv_scale = p.inv_scale;
+    a.mode = p.mode; a.act = act; a.C = l.cout; a.bn = p.bn; a.half = p.half; a.inv_scale = p.inv_scale; a.in_inv = in_inv;
     const int tiles = ((win.B + TB - 1) / TB) * tiles_t;
     // Option tc_occ2 = 1 (default): launches wider than the device take a two-stage ring; 0 lets the ring grow to what
     // shared memory holds (three stages for a 256-column hc block).  The kernel runs one CTA per SM either way, and on an
@@ -840,8 +845,9 @@ bool chain_tc_ok(H* h, const std::vector<LayerDev>& net) {
 
 // Whole chain on the tensor-core path, starting from split planes `cur` (buffer index `which`
 // of the ping-pong pair, or -1 for an external buffer): ... -> fp32 out (+ sigmoid).
+// in_inv: inverse per-utterance scales of `cur` (launch_f32_to_planes_scaled), or null.
 void run_chain_tc_planes(Launch& lc, const std::vector<LayerDev>& net, Planes cur, int which, int B, int L,
-                         float* out, float* out_sig, int first_extra_shift) {
+                         float* out, float* out_sig, int first_extra_shift, const float* in_inv) {
     H* h = lc.h;
     int len = L;
     int nxt = (which == 0) ? 1 : 0;
@@ -851,10 +857,38 @@ void run_chain_tc_planes(Launch& lc, const std::vector<LayerDev>& net, Planes cu
         Planes dst = last ? Planes{} : ws_planes(h, nxt, l.cout);
         run_block_tc(lc, l, l.rate, l.causal, l.act, cur, RowWin{B, len, len, nullptr}, 128, 1, (len + 127) / 128,
                      dst, last ? out : nullptr, l.cout, last ? out_sig : nullptr, l.cout, Planes{},
-                     i == 0 ? first_extra_shift : 0);
+                     i == 0 ? first_extra_shift : 0, i == 0 ? in_inv : nullptr);
         if (l.kind == K_D) len *= 2;
         cur = dst; nxt ^= 1;
     }
+}
+
+// (B) device floats for the inverse input scales; grows (after a device sync) for an op-level call beyond the workspace
+float* input_inv_scales(H* h, int B) {
+    if (h->in_inv.bytes < (size_t)B * sizeof(float)) {
+        CUDA_CHECK(cudaDeviceSynchronize());
+        h->in_inv.ensure((size_t)B * sizeof(float));
+    }
+    return h->in_inv.as<float>();
+}
+
+// The fp32 (B, L, l.cin) input of block l -> its split planes, the way the chains carry that block's input: the first
+// block of AudioEnc, AudioDec and SSRN reads audio-level data (mels, R), which silence puts at 1e-8 and below, so its
+// planes get a power-of-two scale per utterance (the inverses are returned for the block's epilogue).  Every other
+// block reads a LayerNorm output, O(1) per row, or an embedding row, whose magnitude is the committed table's: unscaled
+// planes (null).  The op-level entry points follow the same rule, so a network composed block by block computes
+// exactly what its chain computes.
+const float* block_input_planes(Launch& lc, const LayerDev& l, const float* x, int ldx, Planes p, int B, int L) {
+    H* h = lc.h;
+    const bool net_input = (!h->audioenc.empty() && &l == &h->audioenc[0]) || (!h->audiodec.empty() && &l == &h->audiodec[0]) ||
+                           (!h->ssrn.empty() && &l == &h->ssrn[0]);
+    if (!net_input) {
+        launch_f32_to_planes(x, ldx, p, (long long)B * L, l.cin, lc.s); lc.count();
+        return nullptr;
+    }
+    float* in_inv = input_inv_scales(h, B);
+    launch_f32_to_planes_scaled(x, ldx, p, B, L, l.cin, in_inv, lc.s); lc.count();
+    return in_inv;
 }
 
 // fp32 in -> planes -> chain
@@ -862,8 +896,8 @@ void run_chain_full_tc(Launch& lc, const std::vector<LayerDev>& net, const float
                        float* out, float* out_sig) {
     H* h = lc.h;
     Planes cur = ws_planes(h, 0, net[0].cin);
-    launch_f32_to_planes(X, ldx, cur, (long long)B * L, net[0].cin, lc.s); lc.count();
-    run_chain_tc_planes(lc, net, cur, 0, B, L, out, out_sig, 0);
+    const float* in_inv = block_input_planes(lc, net[0], X, ldx, cur, B, L);
+    run_chain_tc_planes(lc, net, cur, 0, B, L, out, out_sig, 0, in_inv);
 }
 
 void run_attention(Launch& lc, const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
@@ -896,6 +930,8 @@ void run_attention_tc(Launch& lc, const float* Q, int ldq, const float* K, int l
     qp.hi = h->attpl[0].as<__half>(); qp.lo = h->attpl[1].as<__half>(); qp.ld = d;
     kp.hi = h->attpl[2].as<__half>(); kp.lo = h->attpl[3].as<__half>(); kp.ld = d;
     vp.hi = h->attpl[4].as<__half>(); vp.lo = h->attpl[5].as<__half>(); vp.ld = NP;
+    // Q is AudioEnc's last highway output, h1 * LN(.) + (1 - h1) * x: O(1) per row whatever the mels' level, so its planes
+    // need no scale (a network input is scaled before AudioEnc's first block instead)
     launch_f32_to_planes(Q, ldq, qp, (long long)B * T, d, lc.s); lc.count();
     launch_attn_kv_planes(K, ldk, V, ldv, kp, vp, B, N, d, lc.s); lc.count();
     AttnTcArgs a{};
@@ -1096,16 +1132,16 @@ void text2mel_forward(H* h, const int* L, const float* mels, const int* pma, int
     if (chain_tc_ok(h, h->audioenc) && chain_tc_ok(h, h->audiodec)) {
         // tensor-core path: every block over all B*T rows as one wgmma kernel
         Planes mp = ws_planes(h, 0, hp.n_mels);
-        launch_f32_to_planes(mels, hp.n_mels, mp, (long long)B * T, hp.n_mels, lc.s); lc.count();
+        const float* in_inv = block_input_planes(lc, h->audioenc[0], mels, hp.n_mels, mp, B, T);
         float* Q = h->ae_out.back().as<float>();
-        run_chain_tc_planes(lc, h->audioenc, mp, 0, B, T, Q, nullptr, -1);          // shift: train.py:51
+        run_chain_tc_planes(lc, h->audioenc, mp, 0, B, T, Q, nullptr, -1, in_inv);  // shift: train.py:51
         Planes Rpl; Rpl.hi = h->arpl[0].as<__half>(); Rpl.lo = h->arpl[1].as<__half>(); Rpl.ld = 2 * d;
         if (attention_tc_ok(h, N))
             run_attention_tc(lc, Q, d, K, 2 * d, K + d, 2 * d, B, T, N, pma, h->rbuf.as<float>(), align, maxatt, Rpl);
         else
             run_attention(lc, Q, d, K, 2 * d, K + d, 2 * d, RowWin{B, T, T, nullptr}, N, pma, h->rbuf.as<float>(),
                           align, maxatt, nullptr, nullptr, Rpl);
-        run_chain_tc_planes(lc, h->audiodec, Rpl, -1, B, T, h->ad_out.back().as<float>(), Y, 0);
+        run_chain_tc_planes(lc, h->audiodec, Rpl, -1, B, T, h->ad_out.back().as<float>(), Y, 0, nullptr);
         return;
     }
     // AudioEnc over all rows, reading mels shifted by one frame (train.py:51)
@@ -1141,9 +1177,9 @@ void run_block_op(Launch& lc, const LayerDev& l, int rate, bool causal, int act,
             h->plane[0].ensure(need); h->plane[1].ensure(need);
         }
         Planes X = ws_planes(h, 0, l.cin);
-        launch_f32_to_planes(x, l.cin, X, (long long)B * L, l.cin, lc.s); lc.count();
+        const float* in_inv = block_input_planes(lc, l, x, l.cin, X, B, L);
         run_block_tc(lc, l, rate, causal, act, X, RowWin{B, L, L, nullptr}, 128, 1, (L + 127) / 128, Planes{}, out, l.cout,
-                     nullptr, 0, Planes{});
+                     nullptr, 0, Planes{}, 0, in_inv);
         return;
     }
     ensure_scratch(h, (size_t)B * Lout * l.ldw * sizeof(float));

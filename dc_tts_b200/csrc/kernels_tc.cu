@@ -278,12 +278,14 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
             }
         };
         const int bi = r / a.TT, ti = r - bi * a.TT;
-        const float inv_s = a.inv_scale;
         const int n1 = (a.mode == 0) ? min(max(a.C - rank * bn, 0), bn) : half;
         if (r == 0) { dbg_mark(a.dbg, 5, 1); dbg_time(a.dbg, 10); }       // t2: accumulator complete (main loop over)
 
         const int b = b0s + bi, t = t0s + ti;
         const bool row_ok = (b < a.win.B) && (t >= t_lo) && (t <= t_end) && (t < L);
+        // a row reads input rows of its own utterance only, so one input scale per row; both scales are powers of two
+        const float in_s = (a.in_inv && b < a.win.B) ? __ldg(a.in_inv + b) : 1.f;
+        const float inv_s = a.inv_scale * in_s;
 
         // ONE statistics sweep: shifted sums about a pivot taken from the row itself, so that M2 = Q - S^2/n does not cancel
         float s1, s2 = 0.f, q1, q2 = 0.f, m1, m2 = 0.f;
@@ -503,9 +505,54 @@ __global__ void planes_to_f32_kernel(Planes p, float* __restrict__ y, int ldy, l
     long long r = i / C; int c = (int)(i - r * C);
     y[r * ldy + c] = __half2float(p.hi[r * p.ld + c]) + __half2float(p.lo[r * p.ld + c]);
 }
+// One CTA per utterance: abs-max of its L x C inputs -> s = 2^k with max * s in [2^14, 2^15) (1 for an all-zero or
+// non-finite utterance), then hi = fp16(s x), lo = fp16(s x - hi).  s x is exact in fp32, so s only moves the values into
+// fp16's normal range: unscaled, 1e-8 flushes to zero and 1e-6 .. 1e-4 keep a few bits.
+constexpr int PLANES_SCALED_THREADS = 512;
+__global__ void __launch_bounds__(PLANES_SCALED_THREADS)
+f32_to_planes_scaled_kernel(const float* __restrict__ x, int ldx, Planes p, int L, int C, float* __restrict__ in_inv) {
+    __shared__ float s_red[PLANES_SCALED_THREADS / 32];
+    __shared__ float s_scale;
+    const int b = blockIdx.x, n = L * C;
+    const float* xb = x + (size_t)b * L * ldx;
+    float m = 0.f;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const int r = i / C, c = i - r * C;
+        m = fmaxf(m, fabsf(xb[(size_t)r * ldx + c]));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = m;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < (int)(blockDim.x >> 5); ++w) m = fmaxf(m, s_red[w]);
+        float sc = 1.f;
+        if (m > 0.f && isfinite(m)) {
+            int e;
+            frexpf(m, &e);                                     // m in [2^(e-1), 2^e)
+            sc = ldexpf(1.f, min(15 - e, 100));                // 1/s stays a normal float
+        }
+        s_scale = sc;
+        in_inv[b] = 1.f / sc;
+    }
+    __syncthreads();
+    const float sc = s_scale;
+    const size_t row0 = (size_t)b * L;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const int r = i / C, c = i - r * C;
+        const float v = xb[(size_t)r * ldx + c] * sc;
+        const __half h = __float2half_rn(v);
+        p.hi[(row0 + r) * p.ld + c] = h;
+        p.lo[(row0 + r) * p.ld + c] = __float2half_rn(v - __half2float(h));
+    }
+}
 void launch_f32_to_planes(const float* x, int ldx, Planes p, long long rows, int C, cudaStream_t s) {
     long long n = rows * C;
     if (n > 0) f32_to_planes_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(x, ldx, p, rows, C);
+}
+void launch_f32_to_planes_scaled(const float* x, int ldx, Planes p, int B, int L, int C, float* in_inv, cudaStream_t s) {
+    if (B > 0 && (long long)L * C > 0x7fffffffLL) throw std::runtime_error("f32_to_planes_scaled: L x C exceeds 2^31");
+    if (B > 0) f32_to_planes_scaled_kernel<<<(unsigned)B, PLANES_SCALED_THREADS, 0, s>>>(x, ldx, p, L, C, in_inv);
 }
 void launch_planes_to_f32(Planes p, float* y, int ldy, long long rows, int C, cudaStream_t s) {
     long long n = rows * C;
