@@ -152,6 +152,7 @@ struct dctts_handle_s {
     // vocoder (Griffin-Lim) state
     struct { int hop = 275, win = 1102, n_iter = 50; float power = 1.5f, max_db = 100.f, ref_db = 20.f, preemph = 0.97f; } voc;
     DevBuf feat_melw, feat_range, feat_tw, feat_window, feat_wss;   // feature extraction tables (dctts_get_spectrograms)
+    DevBuf feat_seg;                                                // per-utterance segment tables of a feature batch
     int feat_sr = 0, feat_win = 0;
     DevBuf voc_S, voc_X, voc_frames, voc_mse, voc_tw, voc_window, voc_wss, voc_deemph;
     int voc_tables_T = 0, voc_tables_win = 0, voc_tables_hop = 0;
@@ -202,7 +203,7 @@ struct dctts_handle_s {
         for (auto& b : arpl) b.release();
         for (auto& b : attpl) b.release();
         voc_S.release(); voc_X.release(); voc_frames.release(); voc_mse.release(); voc_tw.release(); voc_window.release(); voc_wss.release(); voc_deemph.release();
-        feat_melw.release(); feat_range.release(); feat_tw.release(); feat_window.release(); feat_wss.release();
+        feat_melw.release(); feat_range.release(); feat_tw.release(); feat_window.release(); feat_wss.release(); feat_seg.release();
         for (auto& b : ae_out) b.release();
         for (auto& b : ad_out) b.release();
         if (copy_stream) { cudaStreamDestroy(copy_stream); for (auto e : chunk_done) if (e) cudaEventDestroy(e); }
@@ -1590,6 +1591,97 @@ void trim_from_mse(const float* m, int nfr, int Ly, int32_t* out) {
     out[1] = first < 0 ? 0 : std::min(Ly, (last + 1) * 512);
 }
 
+// The mel basis, FFT twiddles and Hann window of the feature kernels, rebuilt when the sample rate or window changes.
+void feat_tables(H* h, int sample_rate, cudaStream_t s) {
+    const int win = h->voc.win, hop = h->voc.hop;
+    if (h->feat_sr == sample_rate && h->feat_win == win) return;
+    std::vector<float> w; std::vector<int> range;
+    feat_make_mel_basis(sample_rate, h->hp.n_fft, h->hp.n_mels, w, range);
+    h->feat_melw.ensure(w.size() * sizeof(float)); h->feat_range.ensure(range.size() * sizeof(int));
+    h->feat_tw.ensure(2048 * sizeof(float2)); h->feat_window.ensure(win * sizeof(float)); h->feat_wss.ensure(2048 * sizeof(float));
+    CUDA_CHECK(cudaMemcpyAsync(h->feat_melw.p, w.data(), w.size() * sizeof(float), cudaMemcpyHostToDevice, s));
+    CUDA_CHECK(cudaMemcpyAsync(h->feat_range.p, range.data(), range.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    voc_make_tables(h->feat_tw.as<float2>(), h->feat_window.as<float>(), h->feat_wss.as<float>(), 1, win, hop, s);   // synchronises
+    h->feat_sr = sample_rate; h->feat_win = win;
+}
+
+// load_spectrograms (utils.py:147-162) for B utterances packed back to back in `wav` (offsets: B + 1 host sample
+// offsets), reduced by r and padded with zeros to the batch's longest member: mel (B, T_b, n_mels), mag (B, r T_b, F).
+// r = 1 is get_spectrograms (utils.py:20-65): every frame, T_b = T for one utterance.  Two kernels whatever B is:
+// the trim energies of every utterance (one copy back, thresholded on the host: the call's one synchronisation), then
+// the features, one CTA per STFT frame of the flattened batch.  Nothing is written to mel or mag unless every
+// utterance survives trimming and T_b <= t_capacity.
+void feat_batch(H* h, const char* who, const void* wav, int dtype, const int64_t* offsets, int B, int sample_rate, float* mel,
+                float* mag, int t_capacity, int r, int32_t* t_host, int32_t* trim_host, int32_t* T_b_out, cudaStream_t s) {
+    const std::string fn(who);
+    REQUIRE(wav && offsets && mel && mag && B >= 1 && (dtype == 0 || dtype == 1) && sample_rate > 0 && t_capacity >= 1 && r >= 1,
+            fn + ": bad arguments");
+    REQUIRE(h->F == 1025, fn + ": the FFT kernel is built for n_fft = 2048");
+    std::vector<FeatSeg> seg(2 * (size_t)(B + 1));
+    FeatSeg* mseg = seg.data();                     // whole utterances, frames of the trim energies
+    FeatSeg* fseg = seg.data() + B + 1;             // trimmed utterances, STFT frames
+    long long nfr_total = 0;
+    for (int b = 0; b < B; ++b) {
+        const long long n = offsets[b + 1] - offsets[b];
+        REQUIRE(offsets[b] >= 0 && n >= 2 && n < (1ll << 30),
+                fn + ": utterance " + std::to_string(b) + " has " + std::to_string(n) + " samples (need 2 to 2^30)");
+        mseg[b] = FeatSeg{offsets[b], (int)n, (int)nfr_total};
+        nfr_total += 1 + n / 512;
+    }
+    REQUIRE(nfr_total < (1ll << 31), fn + ": batch too long");
+    mseg[B] = FeatSeg{0, 0, (int)nfr_total};
+    feat_tables(h, sample_rate, s);
+    const int F = h->F, hop = h->voc.hop, n_mels = h->hp.n_mels;
+    h->feat_seg.ensure(seg.size() * sizeof(FeatSeg));
+    FeatSeg* seg_dev = h->feat_seg.as<FeatSeg>();
+    h->voc_mse.ensure((size_t)nfr_total * sizeof(float));
+    // librosa.effects.trim (utils.py:36): frame energies on the device, threshold on the host
+    CUDA_CHECK(cudaMemcpyAsync(seg_dev, mseg, (B + 1) * sizeof(FeatSeg), cudaMemcpyHostToDevice, s));
+    feat_frame_mse(wav, dtype, seg_dev, B, (int)nfr_total, h->voc_mse.as<float>(), s);
+    h->launches += 1;
+    CUDA_CHECK(cudaGetLastError());
+    std::vector<float> mse((size_t)nfr_total);
+    CUDA_CHECK(cudaMemcpyAsync(mse.data(), h->voc_mse.p, mse.size() * sizeof(float), cudaMemcpyDeviceToHost, s));
+    CUDA_CHECK(cudaStreamSynchronize(s));
+    long long frames = 0;
+    int T_b = 0, longest = 0;
+    bool padded = false;
+    std::vector<int> T(B);
+    for (int b = 0; b < B; ++b) {
+        int se[2];
+        trim_from_mse(mse.data() + mseg[b].f0, 1 + mseg[b].len / 512, mseg[b].len, se);
+        if (trim_host) { trim_host[2 * b] = se[0]; trim_host[2 * b + 1] = se[1]; }
+        const int len = se[1] - se[0];
+        REQUIRE(len >= 2, fn + ": utterance " + std::to_string(b) + " has nothing left after trimming (silent input)");
+        T[b] = 1 + len / hop;
+        const int t = (T[b] + r - 1) / r;           // reduced rows after padding T to a multiple of r
+        if (t_host) t_host[b] = t;
+        if (t > T_b) { T_b = t; longest = b; }
+        fseg[b] = FeatSeg{mseg[b].src + se[0], len, (int)frames};
+        frames += T[b];
+    }
+    for (int b = 0; b < B; ++b) padded = padded || T[b] != r * T_b;
+    fseg[B] = FeatSeg{0, 0, (int)frames};
+    if (T_b_out) *T_b_out = T_b;
+    REQUIRE(T_b <= t_capacity, fn + ": output buffers too small: utterance " + std::to_string(longest) + " needs " +
+                               std::to_string(T_b) + " rows, t_capacity is " + std::to_string(t_capacity));
+    REQUIRE(frames < (1ll << 31), fn + ": batch too long");
+    CUDA_CHECK(cudaMemcpyAsync(seg_dev + B + 1, fseg, (B + 1) * sizeof(FeatSeg), cudaMemcpyHostToDevice, s));
+    if (padded) {                                   // bucket padding (data_load.py:128, dynamic_pad) and utils.py:154-158
+        CUDA_CHECK(cudaMemsetAsync(mel, 0, (size_t)B * T_b * n_mels * sizeof(float), s));
+        CUDA_CHECK(cudaMemsetAsync(mag, 0, (size_t)B * r * T_b * F * sizeof(float), s));
+    }
+    FeatArgs a{};
+    a.wav = wav; a.dtype = dtype; a.seg = seg_dev + B + 1; a.B = B; a.frames = (int)frames;
+    a.mag = mag; a.mel = mel; a.mag_rows = r * T_b; a.mel_rows = T_b; a.r = r;
+    a.melw = h->feat_melw.as<float>(); a.melrange = h->feat_range.as<int>(); a.tw = h->feat_tw.as<float2>();
+    a.window = h->feat_window.as<float>(); a.F = F; a.n_mels = n_mels; a.win = h->voc.win; a.hop = hop;
+    a.preemph = h->voc.preemph; a.ref_db = h->voc.ref_db; a.max_db = h->voc.max_db;
+    feat_run(a, s);
+    h->launches += 1;
+    CUDA_CHECK(cudaGetLastError());
+}
+
 }  // namespace
 
 // ==================================================================================== C-ABI
@@ -1921,40 +2013,19 @@ int dctts_spectrogram2wav(dctts_handle h, const float* mag, int32_t B, int32_t T
 int dctts_get_spectrograms(dctts_handle h, const float* wav, int64_t n_samples, int32_t sample_rate, float* mel, float* mag,
                            int32_t t_capacity, int32_t* t_out, int32_t* trim_host, void* stream) {
     return guarded(h, [&] {
-        REQUIRE(wav && mel && mag && t_out && n_samples >= 2 && n_samples < (1ll << 30) && sample_rate > 0,
-                "dctts_get_spectrograms: bad arguments");
-        REQUIRE(h->F == 1025, "dctts_get_spectrograms: the FFT kernel is built for n_fft = 2048");
-        cudaStream_t s = S(h, stream);
-        const int n = (int)n_samples, F = h->F, win = h->voc.win, hop = h->voc.hop, n_mels = h->hp.n_mels;
-        if (h->feat_sr != sample_rate || h->feat_win != win) {
-            std::vector<float> w; std::vector<int> range;
-            feat_make_mel_basis(sample_rate, h->hp.n_fft, n_mels, w, range);
-            h->feat_melw.ensure(w.size() * sizeof(float)); h->feat_range.ensure(range.size() * sizeof(int));
-            h->feat_tw.ensure(2048 * sizeof(float2)); h->feat_window.ensure(win * sizeof(float)); h->feat_wss.ensure(2048 * sizeof(float));
-            CUDA_CHECK(cudaMemcpyAsync(h->feat_melw.p, w.data(), w.size() * sizeof(float), cudaMemcpyHostToDevice, s));
-            CUDA_CHECK(cudaMemcpyAsync(h->feat_range.p, range.data(), range.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-            voc_make_tables(h->feat_tw.as<float2>(), h->feat_window.as<float>(), h->feat_wss.as<float>(), 1, win, hop, s);   // synchronises
-            h->feat_sr = sample_rate; h->feat_win = win;
-        }
-        // librosa.effects.trim (utils.py:36): frame energies on the device, threshold on the host
-        const int nfr = 1 + n / 512;
-        h->voc_mse.ensure((size_t)nfr * sizeof(float));
-        feat_frame_mse(wav, h->voc_mse.as<float>(), n, nfr, s);
-        std::vector<float> mse(nfr);
-        CUDA_CHECK(cudaMemcpyAsync(mse.data(), h->voc_mse.p, mse.size() * sizeof(float), cudaMemcpyDeviceToHost, s));
-        CUDA_CHECK(cudaStreamSynchronize(s));
-        int se[2];
-        trim_from_mse(mse.data(), nfr, n, se);
-        if (trim_host) { trim_host[0] = se[0]; trim_host[1] = se[1]; }
-        const int len = se[1] - se[0];
-        REQUIRE(len >= 2, "dctts_get_spectrograms: nothing left after trimming (silent input)");
-        const int T = 1 + len / hop;
-        *t_out = T;
-        REQUIRE(T <= t_capacity, "dctts_get_spectrograms: output buffers too small (need 1 + n_samples / hop_length rows)");
-        feat_run(wav + se[0], len, h->voc.preemph, mag, mel, h->feat_melw.as<float>(), h->feat_range.as<int>(), h->feat_tw.as<float2>(),
-                 h->feat_window.as<float>(), T, F, n_mels, win, hop, h->voc.ref_db, h->voc.max_db, s);
-        h->launches += 2;
-        CUDA_CHECK(cudaGetLastError());
+        REQUIRE(t_out, "dctts_get_spectrograms: bad arguments");
+        const int64_t offsets[2] = {0, n_samples};
+        feat_batch(h, "dctts_get_spectrograms", wav, 0, offsets, 1, sample_rate, mel, mag, t_capacity, 1, t_out, trim_host, nullptr,
+                   S(h, stream));
+    });
+}
+
+int dctts_load_spectrograms_batch(dctts_handle h, const void* wav, int32_t dtype, const int64_t* offsets_host, int32_t B,
+                                  int32_t sample_rate, float* mel, float* mag, int32_t t_capacity,
+                                  int32_t* t_host, int32_t* trim_host, int32_t* T_b_out, void* stream) {
+    return guarded(h, [&] {
+        feat_batch(h, "dctts_load_spectrograms_batch", wav, dtype, offsets_host, B, sample_rate, mel, mag, t_capacity, h->hp.r,
+                   t_host, trim_host, T_b_out, S(h, stream));
     });
 }
 

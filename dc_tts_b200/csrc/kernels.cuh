@@ -130,12 +130,25 @@ void voc_make_tables(float2* tw_dev, float* window_dev, float* wss_dev, int T, i
 void voc_run(const VocoderArgs& a, cudaStream_t s);
 int voc_launches_per_call(int n_iter);
 size_t voc_deemph_scratch_bytes(int B, int T, int hop);
-// feature extraction (reference utils.py:20-65)
+// feature extraction (reference utils.py:20-65,147-162) for a ragged batch of utterances packed back to back
+struct FeatSeg {
+    long long src;             // first sample of the utterance (after trimming, for feat_run) in the packed waveform
+    int len;                   // its samples
+    int f0;                    // its first frame in the flattened batch; entry B holds the total
+};
+struct FeatArgs {
+    const void* wav; int dtype;        // packed waveform: 0 = float32, 1 = int16 PCM (value / 32768)
+    const FeatSeg* seg; int B;         // DEVICE table of B + 1 entries
+    int frames;                        // sum of the utterances' STFT frames (one CTA each)
+    float* mag; float* mel;            // (B, mag_rows, F), (B, mel_rows, n_mels): frame t -> mag row t, mel row t / r if t % r == 0
+    int mag_rows, mel_rows, r;
+    const float* melw; const int* melrange; const float2* tw; const float* window;
+    int F, n_mels, win, hop;
+    float preemph, ref_db, max_db;
+};
 void feat_make_mel_basis(int sr, int n_fft, int n_mels, std::vector<float>& w, std::vector<int>& range);
-void feat_frame_mse(const float* y, float* mse, int n, int nfr, cudaStream_t s);
-void feat_run(const float* y, int len, float preemph, float* mag, float* mel, const float* melw, const int* melrange,
-              const float2* tw, const float* window, int T, int F, int n_mels, int win, int hop, float ref_db, float max_db,
-              cudaStream_t s);
+void feat_frame_mse(const void* wav, int dtype, const FeatSeg* seg, int B, int frames, float* mse, cudaStream_t s);
+void feat_run(const FeatArgs& a, cudaStream_t s);
 
 
 // ---- training step (kernels_train.cu; reference train.py mode "train") ----

@@ -216,43 +216,87 @@ __global__ void voc_deemph_apply_kernel(float* __restrict__ y, const double* __r
     for (int i = 0; i < n; ++i) { acc = (double)p[i] + c * acc; p[i] = (float)acc; }
 }
 
-// librosa.feature.rmse(y, 2048, 512)**2 per centred frame (reflect padding): mse (B, nfr)
-__global__ void __launch_bounds__(256) voc_frame_mse_kernel(const float* __restrict__ y, float* __restrict__ mse, int Ly, int nfr,
-                                                           int flen, int fhop) {
-    __shared__ float red[8];
-    const int f = blockIdx.x, b = blockIdx.y;
-    const float* yb = y + (size_t)b * Ly;
+// A waveform sample as float32: float input as is, int16 PCM as value / 32768 (exact: what utils._load_wav returns)
+__device__ __forceinline__ float wav_sample(const float* __restrict__ y, long long i) { return y[i]; }
+__device__ __forceinline__ float wav_sample(const int16_t* __restrict__ y, long long i) { return (float)y[i] * (1.0f / 32768.0f); }
+
+// librosa.feature.rmse(y, flen, fhop)**2 of centred frame f (reflect padding) of the signal yb[0, Ly), Ly >= 2.  256
+// threads; the result is valid in thread 0.  A signal shorter than the padding is reflected again and again, as
+// np.pad(mode='reflect') does: the padded signal is periodic with period 2 (Ly - 1).
+template <typename In>
+__device__ __forceinline__ float frame_mse(const In* __restrict__ yb, int Ly, int f, int flen, int fhop, float* red) {
+    const int period = 2 * (Ly - 1);
     float acc = 0.f;
     for (int n = threadIdx.x; n < flen; n += 256) {
         int u = f * fhop + n - flen / 2;
         if (u < 0) u = -u;
-        if (u >= Ly) u = 2 * (Ly - 1) - u;
-        const float v = yb[u];
+        if (u >= Ly) {
+            u %= period;
+            if (u >= Ly) u = period - u;
+        }
+        const float v = wav_sample(yb, u);
         acc = fmaf(v, v, acc);
     }
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
     if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
     __syncthreads();
-    if (threadIdx.x == 0) {
-        float t = 0.f;
+    float t = 0.f;
+    if (threadIdx.x == 0)
         for (int i = 0; i < 8; ++i) t += red[i];
-        mse[(size_t)b * nfr + f] = t / (float)flen;
-    }
+    return t / (float)flen;
+}
+
+// frame energies of B equally long signals: mse (B, nfr), grid (nfr, B)
+__global__ void __launch_bounds__(256) voc_frame_mse_kernel(const float* __restrict__ y, float* __restrict__ mse, int Ly, int nfr,
+                                                           int flen, int fhop) {
+    __shared__ float red[8];
+    const float m = frame_mse(y + (size_t)blockIdx.y * Ly, Ly, blockIdx.x, flen, fhop, red);
+    if (threadIdx.x == 0) mse[(size_t)blockIdx.y * nfr + blockIdx.x] = m;
 }
 
 // ---------------------------------------------------------------------------------------- features
-// get_spectrograms (reference utils.py:20-65) for one trimmed utterance, one CTA per STFT frame: pre-emphasis
-// (float32 multiply then subtract, like numpy), reflect-padded Hann frame, the same real-packed FFT, |X|,
-// the mel filterbank (each mel bin is a contiguous run of FFT bins), 20 log10, normalisation.  grid (T).
-__global__ void __launch_bounds__(VC_THREADS) feat_stft_mel_kernel(const float* __restrict__ y, int len, float preemph,
+// The utterance of flattened frame g: seg[b].f0 <= g < seg[b + 1].f0 (seg has B + 1 entries).
+__device__ __forceinline__ int feat_segment(const FeatSeg* __restrict__ seg, int B, int g) {
+    int lo = 0, hi = B;
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (seg[mid].f0 <= g) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
+// frame energies of B ragged signals for librosa.effects.trim (2048-sample frames, hop 512): one CTA per frame over the
+// flattened batch, mse[g] for frame g - seg[b].f0 of utterance b
+template <typename In>
+__global__ void __launch_bounds__(256) feat_frame_mse_kernel(const In* __restrict__ wav, const FeatSeg* __restrict__ seg, int B,
+                                                            float* __restrict__ mse) {
+    __shared__ float red[8];
+    const int g = blockIdx.x, b = feat_segment(seg, B, g);
+    const FeatSeg sg = seg[b];
+    const float m = frame_mse(wav + sg.src, sg.len, g - sg.f0, 2048, 512, red);
+    if (threadIdx.x == 0) mse[g] = m;
+}
+
+// get_spectrograms (reference utils.py:20-65) for B trimmed utterances, one CTA per STFT frame over the flattened batch
+// (seg: the utterance's trimmed start, length and first flattened frame): pre-emphasis (float32 multiply then subtract,
+// like numpy), reflect-padded Hann frame, the same real-packed FFT, |X|, the mel filterbank (each mel bin is a
+// contiguous run of FFT bins), 20 log10, normalisation.  Frame t of utterance b writes mag row b * mag_rows + t; frames
+// with t % r == 0 also write mel row b * mel_rows + t / r (load_spectrograms' reduction, utils.py:155-160).
+template <typename In>
+__global__ void __launch_bounds__(VC_THREADS) feat_stft_mel_kernel(const In* __restrict__ wav, const FeatSeg* __restrict__ seg,
+                                                                   int B, float preemph,
                                                                    float* __restrict__ mag_out, float* __restrict__ mel_out,
+                                                                   int mag_rows, int mel_rows, int r,
                                                                    const float* __restrict__ melw, const int2* __restrict__ melrange,
                                                                    const float2* __restrict__ tw, const float* __restrict__ window,
                                                                    int F, int n_mels, int win, int lpad, int hop, float ref_db,
                                                                    float max_db) {
     __shared__ __align__(16) float2 s0[VC_H];
     __shared__ __align__(16) float2 s1[VC_H];
-    const int t = blockIdx.x, tid = threadIdx.x;
+    const int tid = threadIdx.x, b = feat_segment(seg, B, blockIdx.x);
+    const FeatSeg sg = seg[b];
+    const int t = blockIdx.x - sg.f0, len = sg.len;
+    const In* y = wav + sg.src;
     auto sample = [&](int n) -> float {
         const int m = n - lpad;
         if (m < 0 || m >= win) return 0.f;
@@ -260,7 +304,7 @@ __global__ void __launch_bounds__(VC_THREADS) feat_stft_mel_kernel(const float* 
         if (u < 0) u = -u;
         if (u >= len) u = 2 * (len - 1) - u;
         u = min(max(u, 0), len - 1);
-        const float v = (u > 0) ? __fsub_rn(y[u], __fmul_rn(preemph, y[u - 1])) : y[0];      // utils.py:39
+        const float v = (u > 0) ? __fsub_rn(wav_sample(y, u), __fmul_rn(preemph, wav_sample(y, u - 1))) : wav_sample(y, 0);   // utils.py:39
         return v * window[m];
     };
     float2 v[4];
@@ -271,7 +315,7 @@ __global__ void __launch_bounds__(VC_THREADS) feat_stft_mel_kernel(const float* 
     for (int k = 0; k < 4; ++k) s0[tid + 256 * k] = v[k];
     __syncthreads();
     float* lin = reinterpret_cast<float*>(s1);             // |X[k]|, k <= 1024 (s1 was last read inside the FFT)
-    float* mo = mag_out + (size_t)t * F;
+    float* mo = mag_out + ((size_t)b * mag_rows + t) * F;
     auto emit = [&](int kk, float2 e) {
         const float a = sqrtf(e.x * e.x + e.y * e.y);
         lin[kk] = a;
@@ -289,7 +333,9 @@ __global__ void __launch_bounds__(VC_THREADS) feat_stft_mel_kernel(const float* 
         emit(kk, make_float2(e.x + o.x, e.y + o.y));
         if (kk == 0) emit(VC_H, make_float2(zk.x - zk.y, 0.f));
     }
+    if (t % r != 0) return;                                // a frame the reduction drops: mag only
     __syncthreads();
+    float* mel_row = mel_out + ((size_t)b * mel_rows + t / r) * n_mels;
     const int warp = tid >> 5, lane = tid & 31;
     for (int m = warp; m < n_mels; m += VC_THREADS / 32) {
         const int2 r = melrange[m];
@@ -299,7 +345,7 @@ __global__ void __launch_bounds__(VC_THREADS) feat_stft_mel_kernel(const float* 
         for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
         if (lane == 0) {
             const float db = 20.0f * log10f(fmaxf(1e-5f, acc));
-            mel_out[(size_t)t * n_mels + m] = fminf(fmaxf((db - ref_db + max_db) / max_db, 1e-8f), 1.0f);
+            mel_row[m] = fminf(fmaxf((db - ref_db + max_db) / max_db, 1e-8f), 1.0f);
         }
     }
 }
@@ -351,15 +397,24 @@ void feat_make_mel_basis(int sr, int n_fft, int n_mels, std::vector<float>& w, s
     }
 }
 
-void feat_frame_mse(const float* y, float* mse, int n, int nfr, cudaStream_t s) {
-    voc_frame_mse_kernel<<<dim3(nfr, 1), 256, 0, s>>>(y, mse, n, nfr, 2048, 512);
+void feat_frame_mse(const void* wav, int dtype, const FeatSeg* seg, int B, int frames, float* mse, cudaStream_t s) {
+    if (dtype == 1)
+        feat_frame_mse_kernel<int16_t><<<frames, 256, 0, s>>>(static_cast<const int16_t*>(wav), seg, B, mse);
+    else
+        feat_frame_mse_kernel<float><<<frames, 256, 0, s>>>(static_cast<const float*>(wav), seg, B, mse);
 }
 
-void feat_run(const float* y, int len, float preemph, float* mag, float* mel, const float* melw, const int* melrange,
-              const float2* tw, const float* window, int T, int F, int n_mels, int win, int hop, float ref_db, float max_db,
-              cudaStream_t s) {
-    feat_stft_mel_kernel<<<T, VC_THREADS, 0, s>>>(y, len, preemph, mag, mel, melw, reinterpret_cast<const int2*>(melrange), tw,
-                                                  window, F, n_mels, win, (VC_N - win) / 2, hop, ref_db, max_db);
+void feat_run(const FeatArgs& a, cudaStream_t s) {
+    const int2* range = reinterpret_cast<const int2*>(a.melrange);
+    const int lpad = (VC_N - a.win) / 2;
+    if (a.dtype == 1)
+        feat_stft_mel_kernel<int16_t><<<a.frames, VC_THREADS, 0, s>>>(
+            static_cast<const int16_t*>(a.wav), a.seg, a.B, a.preemph, a.mag, a.mel, a.mag_rows, a.mel_rows, a.r, a.melw, range,
+            a.tw, a.window, a.F, a.n_mels, a.win, lpad, a.hop, a.ref_db, a.max_db);
+    else
+        feat_stft_mel_kernel<float><<<a.frames, VC_THREADS, 0, s>>>(
+            static_cast<const float*>(a.wav), a.seg, a.B, a.preemph, a.mag, a.mel, a.mag_rows, a.mel_rows, a.r, a.melw, range,
+            a.tw, a.window, a.F, a.n_mels, a.win, lpad, a.hop, a.ref_db, a.max_db);
 }
 
 int voc_launches_per_call(int n_iter) { return 1 + 3 * n_iter + 2 + 3 + 1; }

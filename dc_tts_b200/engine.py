@@ -291,6 +291,48 @@ class Engine:
                                                      C.byref(t), trim, self._stream()), "dctts_get_spectrograms")
         return mel[:t.value], mag[:t.value], (int(trim[0]), int(trim[1]))
 
+    def load_spectrograms_batch(self, wavs, sr=None, t_capacity=None):
+        """utils.py:147-162 for a list of 1-D int16 (PCM, value / 32768) or float32 waveforms at hp.sr, as ONE bucketed
+        batch: the waveforms cross to the device in one copy from a pinned buffer (int16 stays int16 when every member
+        is int16), two kernels compute all the features, and the call synchronises once.  Returns
+        (mels (B, T_b, n_mels), mags (B, r T_b, F)) contiguous CUDA tensors zero-padded to the longest member, the
+        reduced rows per utterance t (B,) int32 and the kept sample ranges trim (B, 2) int32 (numpy).  `t_capacity`
+        (reduced rows per utterance; default: enough for the untrimmed lengths) sizes the outputs."""
+        h = self.hp
+        arrs = [np.asarray(w).reshape(-1) for w in wavs]
+        if not arrs:
+            raise DcttsError("load_spectrograms_batch: empty batch")
+        pcm = all(a.dtype == np.int16 for a in arrs)
+        if not pcm:
+            arrs = [a.astype(np.float32) / np.float32(32768.0) if a.dtype == np.int16 else np.asarray(a, np.float32) for a in arrs]
+        B = len(arrs)
+        offsets = np.zeros(B + 1, np.int64)
+        offsets[1:] = np.cumsum([a.size for a in arrs])
+        host = torch.empty(int(offsets[-1]), dtype=torch.int16 if pcm else torch.float32, pin_memory=True)
+        hv = host.numpy()
+        for b, a in enumerate(arrs):
+            hv[offsets[b]:offsets[b + 1]] = a
+        wav = host.to(self.device, non_blocking=True)
+        if t_capacity is None:
+            t_capacity = max(-(-(1 + a.size // h.hop_length) // h.r) for a in arrs)
+        self._check(self._lib.dctts_set_vocoder_params(self._h, h.hop_length, h.win_length, float(h.power), float(h.max_db),
+                                                       float(h.ref_db), float(h.preemphasis), int(h.n_iter)),
+                    "dctts_set_vocoder_params")
+        mel = self._empty(B * t_capacity * h.n_mels)
+        mag = self._empty(B * t_capacity * h.r * self.F)
+        t = np.zeros(B, np.int32)
+        trim = np.zeros((B, 2), np.int32)
+        T_b = C.c_int32(0)
+        i32p = C.POINTER(C.c_int32)
+        self._check(self._lib.dctts_load_spectrograms_batch(
+            self._h, _ptr(wav), 1 if pcm else 0, offsets.ctypes.data_as(C.POINTER(C.c_int64)), B, int(sr or h.sr), _ptr(mel),
+            _ptr(mag), int(t_capacity), t.ctypes.data_as(i32p), trim.ctypes.data_as(i32p), C.byref(T_b), self._stream()),
+            "dctts_load_spectrograms_batch")
+        T_b = T_b.value
+        mel = mel[:B * T_b * h.n_mels].view(B, T_b, h.n_mels)
+        mag = mag[:B * h.r * T_b * self.F].view(B, h.r * T_b, self.F)
+        return mel, mag, t, trim
+
     # ------------------------------------------------------------------ training step (BASELINE config 5)
     def train_init(self, B, dropout_rate=None):
         """Allocates the training workspace for batches of B utterances (train.py mode "train", num=1)."""

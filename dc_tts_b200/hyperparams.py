@@ -13,7 +13,7 @@ not the 276 its comment claims; win_length = 1102.
 
 class Hyperparams:
     # --- pipeline -----------------------------------------------------------
-    prepro = True
+    prepro = True            # False: trainer.bucketed_batches computes the features from the wavs on the device
 
     # --- signal processing (only used by the out-of-scope vocoder/feature code)
     sr = 22050

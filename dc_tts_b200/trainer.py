@@ -1,7 +1,8 @@
 """The trainer loop around `Engine.train_step` / `train_step_ssrn` -- what `python train.py 1|2` does in the reference
 (/root/reference/train.py:137-160: one optimiser step per batch, a checkpoint `model_gs_{NNN}k` every 1000 steps in
 `hp.logdir + "-" + num`, stop after hp.num_iterations) on top of the LJ transcript parser of data_load.py:41-56 and the
-pre-computed `mels/*.npy`, `mags/*.npy` of prepo.py (data_load.py:104-112).
+pre-computed `mels/*.npy`, `mags/*.npy` of prepo.py (data_load.py:104-112), or, with hp.prepro = False, features computed
+on the device from the wav files one bucket at a time.
 
 Batching: `bucketed_batches` restates the reference's length-bucketed, dynamically padded queue (data_load.py:88-131:
 shuffled stream, buckets by text length every 20 characters, a full bucket emits a batch padded to its own longest
@@ -89,7 +90,19 @@ def bucket_index(length, boundaries):
     return int(np.searchsorted(np.asarray(boundaries), length, side="right"))
 
 
-def bucketed_batches(fpaths, text_lengths, texts, B=None, seed=0, loader=_load_spectrograms_npy, epochs=None, rank=0, world=1):
+def _pad_spectrograms(items):
+    """dynamic_pad (data_load.py:128) of the npy route: [(mel, mag), ...] -> zero-padded (mels, mags) numpy arrays."""
+    T_b = max(m.shape[0] for m, _ in items)
+    Tm_b = max(g.shape[0] for _, g in items)
+    mels = np.zeros((len(items), T_b, hp.n_mels), np.float32)
+    mags = np.zeros((len(items), Tm_b, items[0][1].shape[1]), np.float32)
+    for b, (m, g) in enumerate(items):
+        mels[b, :m.shape[0]] = m; mags[b, :g.shape[0]] = g
+    return mels, mags
+
+
+def bucketed_batches(fpaths, text_lengths, texts, B=None, seed=0, loader=_load_spectrograms_npy, epochs=None, rank=0, world=1,
+                     prepro=None, engine=None, features=None):
     """The reference's input pipeline (data_load.py:88-131) without TensorFlow queues: a shuffled stream of utterances
     (slice_input_producer :99) is routed by TEXT length into buckets (boundaries :125); a bucket that has collected B
     utterances emits them as one batch, every tensor padded with zeros to the longest member of THAT batch
@@ -97,8 +110,22 @@ def bucketed_batches(fpaths, text_lengths, texts, B=None, seed=0, loader=_load_s
     contents across epochs like the TF queue does; nothing is dropped except what never fills a bucket.
     Yields (L, mels, mags, names, bucket), which `train` and `Graph(mode="train")` take directly.  Data-parallel runs:
     like fixed_size_batches, every rank draws the SAME permutation (same seed) and keeps every world-th utterance, so the
-    ranks' batches are disjoint (their shapes may differ from rank to rank)."""
+    ranks' batches are disjoint (their shapes may differ from rank to rank).
+
+    `prepro` (default hp.prepro) picks where the spectrograms come from, as in data_load.py:104-113.  True: `loader`
+    reads what prepo.py wrote (numpy batches).  False: the buckets collect the wav files' samples and a full bucket gets
+    its features from ONE batched device call, `features(pcms) -> (mels, mags)` (default
+    `(engine or get_engine()).load_spectrograms_batch`), so mels and mags are CUDA tensors and no mels/ or mags/
+    directory is needed.  The features run on the caller's thread (an engine handle is not thread-safe).  Routing,
+    sharding and padding are the same loop for both routes."""
     B = B or hp.B
+    from_wavs = not (hp.prepro if prepro is None else prepro)
+    if from_wavs:
+        from .utils import _load_pcm
+        if features is None:
+            def features(pcms):
+                from .engine import get_engine
+                return (engine or get_engine()).load_spectrograms_batch(pcms)[:2]
     bounds = bucket_boundaries(text_lengths)
     pending = [[] for _ in range(len(bounds) + 1)]
     rng = np.random.default_rng(seed)
@@ -107,20 +134,19 @@ def bucketed_batches(fpaths, text_lengths, texts, B=None, seed=0, loader=_load_s
         emitted = 0
         for i in rng.permutation(len(fpaths))[rank::world]:
             k = bucket_index(text_lengths[i], bounds)
-            fname, mel, mag = loader(fpaths[i])
-            pending[k].append((texts[i], mel, mag, fname))
+            if from_wavs:
+                pending[k].append((texts[i], _load_pcm(fpaths[i]), os.path.basename(fpaths[i])))
+            else:
+                fname, mel, mag = loader(fpaths[i])
+                pending[k].append((texts[i], (mel, mag), fname))
             if len(pending[k]) == B:
                 items, pending[k] = pending[k], []
-                N_b = max(len(t) for t, _, _, _ in items)
-                T_b = max(m.shape[0] for _, m, _, _ in items)
-                Tm_b = max(g.shape[0] for _, _, g, _ in items)
-                L = np.zeros((B, N_b), np.int32)
-                mels = np.zeros((B, T_b, hp.n_mels), np.float32)
-                mags = np.zeros((B, Tm_b, items[0][2].shape[1]), np.float32)
-                for b, (t, m, g, _) in enumerate(items):
-                    L[b, :len(t)] = t; mels[b, :m.shape[0]] = m; mags[b, :g.shape[0]] = g
+                L = np.zeros((B, max(len(t) for t, _, _ in items)), np.int32)
+                for b, (t, _, _) in enumerate(items):
+                    L[b, :len(t)] = t
+                mels, mags = (features if from_wavs else _pad_spectrograms)([it[1] for it in items])
                 emitted += 1
-                yield L, mels, mags, [it[3] for it in items], k
+                yield L, mels, mags, [it[2] for it in items], k
         if emitted == 0 and epochs is None and epoch >= 64:
             raise ValueError("bucketed_batches: no bucket reaches B=%d utterances" % B)
         epoch += 1

@@ -5,8 +5,9 @@ The reference runs librosa's stft / istft on the CPU, 50 + 51 times per utteranc
 Griffin-Lim loop runs on the GPU (csrc/kernels_vocoder.cu: one CTA per STFT frame, a 2048-point FFT
 in shared memory) behind `dctts_spectrogram2wav`.  This is the first "next" row of SURVEY.md 8(f), not part
 of the Text2Mel + SSRN hot path.  Feature extraction (`get_spectrograms`, `load_spectrograms`,
-utils.py:20-65,147-162) runs on the GPU too (`dctts_get_spectrograms`: trim, pre-emphasis, STFT, mel
-filterbank, dB, normalisation in one kernel per utterance); `librosa.load` is replaced by scipy's WAV reader
+utils.py:20-65,147-162) runs on the GPU too (`dctts_get_spectrograms` / `dctts_load_spectrograms_batch`: trim,
+pre-emphasis, STFT, mel filterbank, dB, normalisation in two kernels per call, for one utterance or a whole bucket);
+`librosa.load` is replaced by scipy's WAV reader
 for files that already have hp.sr (LJ Speech does) -- resampling, plotting and the training helpers of the
 reference's utils.py stay out of scope.
 """
@@ -63,12 +64,28 @@ def invert_spectrogram(spectrogram):
     return x.astype(np.float32)
 
 
-def _load_wav(fpath):
-    """What `librosa.load(fpath, sr=hp.sr)` returns for a mono PCM / float WAV that already has hp.sr."""
+def _read_wav(fpath):
+    """The samples of a WAV file at hp.sr as scipy reads them (raises for another sample rate)."""
     from scipy.io import wavfile
     sr, y = wavfile.read(fpath)
     if sr != hp.sr:
         raise ValueError("%s: sample rate %d != hp.sr %d (resampling is not implemented)" % (fpath, sr, hp.sr))
+    return y
+
+
+def _load_pcm(fpath):
+    """A WAV file for the batched feature path: mono int16 stays int16 (the device divides by 32768, exactly as
+    `_load_wav` does); every other format is converted on the host by `_load_wav`'s rules."""
+    y = _read_wav(fpath)
+    return y if (y.ndim == 1 and y.dtype == np.int16) else _load_wav_samples(y)
+
+
+def _load_wav(fpath):
+    """What `librosa.load(fpath, sr=hp.sr)` returns for a mono PCM / float WAV that already has hp.sr."""
+    return _load_wav_samples(_read_wav(fpath))
+
+
+def _load_wav_samples(y):
     if y.ndim > 1:
         y = y.mean(axis=1)
     if y.dtype == np.int16:
@@ -98,6 +115,15 @@ def load_spectrograms(fpath):
     mag = np.pad(mag, [[0, num_paddings], [0, 0]], mode="constant")
     mel = mel[::hp.r, :]
     return fname, mel, mag
+
+
+def load_spectrograms_batch(fpaths, engine=None):
+    """`load_spectrograms` for several WAV files in one device call (`Engine.load_spectrograms_batch`), padded with zeros
+    as one bucketed batch.  Returns (fnames, mels (B, T_b, n_mels), mags (B, r T_b, F), t): CUDA tensors, and the reduced
+    rows t (B,) of each utterance -- utterance b is mels[b, :t[b]], mags[b, :r t[b]], bit for bit what
+    `load_spectrograms` returns for it."""
+    mels, mags, t, _ = (engine or get_engine()).load_spectrograms_batch([_load_pcm(p) for p in fpaths])
+    return [os.path.basename(p) for p in fpaths], mels, mags, t
 
 
 def guided_attention(g=0.2):

@@ -143,9 +143,24 @@ int dctts_spectrogram2wav(dctts_handle h, const float* mag, int32_t B, int32_t T
  * (librosa.filters.mel(sample_rate, n_fft, n_mels)), 20 log10, normalisation with the constants of
  * dctts_set_vocoder_params.  `wav` DEVICE float32 [n_samples]; `mel` (t_capacity, n_mels) and `mag`
  * (t_capacity, 1 + n_fft/2) DEVICE outputs, rows [0, *t_out) written, t_capacity >= 1 + n_samples / hop_length;
- * `trim_host` (optional) receives the [start, end) sample range kept.  Synchronises the stream once. */
+ * `trim_host` (optional) receives the [start, end) sample range kept.  Synchronises the stream once.
+ * This is dctts_load_spectrograms_batch at B = 1 without the reduction (every frame is a mel row) and without padding:
+ * the same two kernels compute it. */
 int dctts_get_spectrograms(dctts_handle h, const float* wav, int64_t n_samples, int32_t sample_rate, float* mel, float* mag,
                            int32_t t_capacity, int32_t* t_out, int32_t* trim_host, void* stream);
+/* load_spectrograms (utils.py:147-162) for B utterances at once, padded as one bucketed batch (data_load.py:122-129,
+ * dynamic_pad).  wav: DEVICE, the B waveforms back to back; offsets_host: B+1 HOST int64 sample offsets;
+ * dtype 0 = float32, 1 = int16 PCM (value / 32768, what utils._load_wav returns for int16 files).
+ * Outputs are packed at the batch's own shape from the start of the caller's buffers (which hold t_capacity reduced
+ * rows per utterance):  mel (B, T_b, n_mels) = every r-th frame,  mag (B, r*T_b, F);  rows past an utterance's own
+ * length are zero.  t_host (B): reduced rows per utterance; trim_host (2B): [start, end) kept; *T_b_out = max t_host.
+ * Each utterance's rows are bit for bit what dctts_get_spectrograms computes for it alone, then padded and reduced.
+ * Two kernels per call whatever B is (trim energies of every utterance, then one CTA per STFT frame of the flattened
+ * batch).  Fails, naming the utterance and writing nothing to mel or mag, when an utterance has fewer than 2 samples
+ * left after trimming or T_b > t_capacity.  Synchronises once. */
+int dctts_load_spectrograms_batch(dctts_handle h, const void* wav, int32_t dtype, const int64_t* offsets_host, int32_t B,
+                                  int32_t sample_rate, float* mel, float* mag, int32_t t_capacity,
+                                  int32_t* t_host, int32_t* trim_host, int32_t* T_b_out, void* stream);
 
 /* ---- training step (BASELINE config 5; SURVEY 8f-3) --------------------------------------
  * One optimiser step of the reference's Text2Mel trainer -- graph train.py:43-68 in mode "train" (dropout after
