@@ -47,6 +47,10 @@ SIGNATURES = {
     "dctts_get_spectrograms": (C.c_int, [Handle, _p, _i64, _i32, _p, _p, _i32, C.POINTER(_i32), C.POINTER(_i32), _p]),
     "dctts_load_spectrograms_batch": (C.c_int, [Handle, _p, _i32, C.POINTER(_i64), _i32, _i32, _p, _p, _i32, C.POINTER(_i32),
                                                 C.POINTER(_i32), C.POINTER(_i32), _p]),
+    "dctts_resample_batch": (C.c_int, [Handle, _p, _i32, C.POINTER(_i64), C.POINTER(_i32), _i32, _i32, _p, _i64, C.POINTER(_i64),
+                                       _p]),
+    "dctts_resample_time_register": (_i32, [_i64, _i32, _i32, C.POINTER(_i64), C.POINTER(C.c_double), C.POINTER(C.c_double),
+                                            _i32]),
     "dctts_train_init": (C.c_int, [Handle, _i32, C.c_float]),
     "dctts_train_step": (C.c_int, [Handle, _p, _p, _i32, _i64, C.c_uint32, C.c_float, _i32, C.POINTER(C.c_float), _p]),
     "dctts_train_step_shaped": (C.c_int, [Handle, _p, _i32, _p, _i32, _i32, _i64, C.c_uint32, C.c_float, _i32, C.POINTER(C.c_float), _p]),

@@ -153,6 +153,7 @@ struct dctts_handle_s {
     struct { int hop = 275, win = 1102, n_iter = 50; float power = 1.5f, max_db = 100.f, ref_db = 20.f, preemph = 0.97f; } voc;
     DevBuf feat_melw, feat_range, feat_tw, feat_window, feat_wss;   // feature extraction tables (dctts_get_spectrograms)
     DevBuf feat_seg;                                                // per-utterance segment tables of a feature batch
+    DevBuf rs_win, rs_tab;                                          // resampling: kaiser_best filter, per-call tables
     int feat_sr = 0, feat_win = 0;
     DevBuf voc_S, voc_X, voc_frames, voc_mse, voc_tw, voc_window, voc_wss, voc_deemph;
     int voc_tables_T = 0, voc_tables_win = 0, voc_tables_hop = 0;
@@ -203,7 +204,7 @@ struct dctts_handle_s {
         for (auto& b : arpl) b.release();
         for (auto& b : attpl) b.release();
         voc_S.release(); voc_X.release(); voc_frames.release(); voc_mse.release(); voc_tw.release(); voc_window.release(); voc_wss.release(); voc_deemph.release();
-        feat_melw.release(); feat_range.release(); feat_tw.release(); feat_window.release(); feat_wss.release(); feat_seg.release();
+        feat_melw.release(); feat_range.release(); feat_tw.release(); feat_window.release(); feat_wss.release(); feat_seg.release(); rs_win.release(); rs_tab.release();
         for (auto& b : ae_out) b.release();
         for (auto& b : ad_out) b.release();
         if (copy_stream) { cudaStreamDestroy(copy_stream); for (auto e : chunk_done) if (e) cudaEventDestroy(e); }
@@ -2027,6 +2028,76 @@ int dctts_load_spectrograms_batch(dctts_handle h, const void* wav, int32_t dtype
         feat_batch(h, "dctts_load_spectrograms_batch", wav, dtype, offsets_host, B, sample_rate, mel, mag, t_capacity, h->hp.r,
                    t_host, trim_host, T_b_out, S(h, stream));
     });
+}
+
+int dctts_resample_batch(dctts_handle h, const void* wav, int32_t dtype, const int64_t* offsets_host, const int32_t* sr_host,
+                         int32_t B, int32_t sr_out, float* out, int64_t out_capacity, int64_t* out_offsets_host, void* stream) {
+    return guarded(h, [&] {
+        const std::string fn = "dctts_resample_batch";
+        REQUIRE(wav && offsets_host && sr_host && out && out_offsets_host && B >= 1 && (dtype == 0 || dtype == 1) && sr_out > 0 &&
+                out_capacity >= 0, fn + ": bad arguments");
+        std::vector<ResampleUtt> utt(B + 1);
+        std::vector<TimeSeg> seg;
+        long long total = 0;
+        for (int b = 0; b < B; ++b) {
+            const std::string who = fn + ": utterance " + std::to_string(b);
+            const long long n = offsets_host[b + 1] - offsets_host[b];
+            REQUIRE(offsets_host[b] >= 0 && n >= 1 && n < (1ll << 31),
+                    who + " has " + std::to_string(n) + " samples (need 1 to 2^31 - 1)");
+            REQUIRE(sr_host[b] > 0, who + " has sample rate " + std::to_string(sr_host[b]));
+            ResampleUtt& u = utt[b];
+            u = ResampleUtt{offsets_host[b], total, n, (int)n, (int)seg.size(), 0, 0, 1.0, 1.0};
+            long long n_out = n;
+            if (sr_host[b] != sr_out) {                        // resampy.resample (librosa.core.resample, fix=True)
+                const double ratio = (double)sr_out / (double)sr_host[b];
+                const double x = (double)n * ratio;
+                u.n_valid = (long long)x;
+                REQUIRE(u.n_valid >= 1, who + ": " + std::to_string(n) + " samples at " + std::to_string(sr_host[b]) +
+                                        " Hz are too short to resample to " + std::to_string(sr_out) + " Hz");
+                n_out = (long long)std::ceil(x);
+                u.ratio = ratio;
+                u.scale = std::min(1.0, ratio);
+                u.index_step = (int)(u.scale * RS_TABLE);
+                REQUIRE(u.index_step >= 1, who + ": sample rate " + std::to_string(sr_host[b]) + " is over 512 times " +
+                                           std::to_string(sr_out));
+                u.nseg = resample_time_register(u.n_valid, 1.0 / ratio, seg);
+            }
+            total += n_out;
+            REQUIRE(total <= out_capacity, who + " ends at output sample " + std::to_string(total) + ", past out_capacity " +
+                                           std::to_string(out_capacity));
+        }
+        utt[B] = ResampleUtt{0, total, 0, 0, (int)seg.size(), 0, 0, 1.0, 1.0};
+        cudaStream_t s = S(h, stream);
+        if (!h->rs_win.p) {
+            std::vector<double> w;
+            resample_filter_table(w);
+            h->rs_win.ensure(w.size() * sizeof(double));
+            CUDA_CHECK(cudaMemcpyAsync(h->rs_win.p, w.data(), w.size() * sizeof(double), cudaMemcpyHostToDevice, s));
+        }
+        // one host-to-device copy: B + 1 utterance records, then the time-register segments
+        const size_t ub = utt.size() * sizeof(ResampleUtt), sb = seg.size() * sizeof(TimeSeg);
+        std::vector<char> tab(ub + sb);
+        std::memcpy(tab.data(), utt.data(), ub);
+        if (sb) std::memcpy(tab.data() + ub, seg.data(), sb);
+        h->rs_tab.ensure(tab.size());
+        CUDA_CHECK(cudaMemcpyAsync(h->rs_tab.p, tab.data(), tab.size(), cudaMemcpyHostToDevice, s));
+        const ResampleUtt* utt_dev = h->rs_tab.as<ResampleUtt>();
+        resample_run(wav, dtype, utt_dev, B, reinterpret_cast<const TimeSeg*>(h->rs_tab.as<char>() + ub), h->rs_win.as<double>(),
+                     out, total, s);
+        h->launches += 1;
+        CUDA_CHECK(cudaGetLastError());
+        for (int b = 0; b <= B; ++b) out_offsets_host[b] = utt[b].dst;
+    });
+}
+
+int32_t dctts_resample_time_register(int64_t n_out, int32_t sr_in, int32_t sr_out, int64_t* t0, double* v0, double* step,
+                                     int32_t capacity) {
+    if (n_out < 0 || sr_in <= 0 || sr_out <= 0 || capacity < 0) return -1;
+    std::vector<TimeSeg> seg;
+    const int n = resample_time_register(n_out, 1.0 / ((double)sr_out / (double)sr_in), seg);
+    if (n > capacity) return -1;
+    for (int i = 0; i < n; ++i) { t0[i] = seg[i].t0; v0[i] = seg[i].v0; step[i] = seg[i].step; }
+    return n;
 }
 
 int dctts_train_init(dctts_handle h, int32_t B, float dropout_rate) {

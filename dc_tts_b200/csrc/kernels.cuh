@@ -149,6 +149,28 @@ struct FeatArgs {
 void feat_make_mel_basis(int sr, int n_fft, int n_mels, std::vector<float>& w, std::vector<int>& range);
 void feat_frame_mse(const void* wav, int dtype, const FeatSeg* seg, int B, int frames, float* mse, cudaStream_t s);
 void feat_run(const FeatArgs& a, cudaStream_t s);
+// resampling in front of the features: librosa 0.6 core.resample(y, sr_orig, sr, res_type='kaiser_best', fix=True),
+// i.e. resampy 0.2 resample / resample_f, for a ragged batch with one native rate per utterance
+constexpr int RS_ZEROS = 64, RS_TABLE = 512, RS_NWIN = RS_ZEROS * RS_TABLE + 1;   // kaiser_best: 64 zeros, precision 9
+struct ResampleUtt {
+    long long src;             // first input sample in the packed waveform
+    long long dst;             // first output sample in the packed output; entry B holds the total
+    long long n_valid;         // int(n_in * ratio) samples resampy computes; [n_valid, next dst) are fix_length's zeros
+    int n_in;                  // input samples
+    int seg0, nseg;            // the utterance's time-register segments
+    int index_step;            // int(scale * 512); 0: already at the output rate, only converted to float32
+    double ratio, scale;       // sr_out / sr_in, min(1, ratio)
+};
+// The float64 time register of resample_f (time_register += time_increment once per output) for outputs
+// [t0, next segment's t0): exactly v0 + (t - t0) * step.
+struct TimeSeg {
+    long long t0;
+    double v0, step;
+};
+void resample_filter_table(std::vector<double>& win);
+int resample_time_register(long long n_out, double inc, std::vector<TimeSeg>& out);
+void resample_run(const void* wav, int dtype, const ResampleUtt* utt, int B, const TimeSeg* seg, const double* win, float* out,
+                  long long total, cudaStream_t s);
 
 
 // ---- training step (kernels_train.cu; reference train.py mode "train") ----

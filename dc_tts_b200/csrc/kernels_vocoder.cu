@@ -15,6 +15,7 @@
 // and the frame energies librosa.effects.trim thresholds.
 #include "kernels.cuh"
 
+#include <algorithm>
 #include <cmath>
 #include <vector>
 
@@ -415,6 +416,144 @@ void feat_run(const FeatArgs& a, cudaStream_t s) {
         feat_stft_mel_kernel<float><<<a.frames, VC_THREADS, 0, s>>>(
             static_cast<const float*>(a.wav), a.seg, a.B, a.preemph, a.mag, a.mel, a.mag_rows, a.mel_rows, a.r, a.melw, range,
             a.tw, a.window, a.F, a.n_mels, a.win, lpad, a.hop, a.ref_db, a.max_db);
+}
+
+// ---------------------------------------------------------------------------------------- resampling
+// resampy 0.2 resample_f for output t of one utterance, one thread per output sample over the flattened batch.  Every
+// float64 operation is an explicit round-to-nearest intrinsic, so nothing is contracted into an FMA (numba does not
+// contract either).  `win` is the unscaled interp_win; for ratio < 1 resampy scales it by the ratio before taking
+// interp_delta = diff(interp_win), and so does `tap`.  The accumulator is float32 and every tap rounds
+// float32(double(y) + weight * double(x)), numba's semantics for `y[t] += weight * x[...]` with a float32 y.
+template <typename In>
+__global__ void __launch_bounds__(256) resample_kernel(const In* __restrict__ wav, const ResampleUtt* __restrict__ utt, int B,
+                                                       const TimeSeg* __restrict__ seg, const double* __restrict__ win,
+                                                       float* __restrict__ out, long long total) {
+    const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= total) return;
+    int lo = 0, hi = B;
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (utt[mid].dst <= g) lo = mid; else hi = mid;
+    }
+    const ResampleUtt u = utt[lo];
+    const long long t = g - u.dst;
+    const In* x = wav + u.src;
+    if (t >= u.n_valid) { out[g] = 0.f; return; }                        // librosa util.fix_length
+    if (u.index_step == 0) { out[g] = wav_sample(x, t); return; }        // librosa: orig_sr == target_sr returns y
+    int a = u.seg0, b = u.seg0 + u.nseg;
+    while (b - a > 1) {
+        const int mid = (a + b) >> 1;
+        if (seg[mid].t0 <= t) a = mid; else b = mid;
+    }
+    const double reg = __dadd_rn(seg[a].v0, __dmul_rn((double)(t - seg[a].t0), seg[a].step));   // exact (see TimeSeg)
+    const double ratio = u.ratio, scale = u.scale;
+    const bool scaled = ratio < 1.0;
+    const int step = u.index_step;
+    double eta;
+    auto weight = [&](int j) -> double {                  // interp_win[j] + eta * interp_delta[j]
+        double w0 = win[j], d = 0.0;
+        if (scaled) w0 = __dmul_rn(w0, ratio);
+        if (j + 1 < RS_NWIN) {
+            const double w1 = scaled ? __dmul_rn(win[j + 1], ratio) : win[j + 1];
+            d = __dsub_rn(w1, w0);
+        }
+        return __dadd_rn(w0, __dmul_rn(eta, d));
+    };
+    const long long n = (long long)reg;
+    double frac = __dmul_rn(scale, __dsub_rn(reg, (double)n));
+    double index_frac = __dmul_rn(frac, (double)RS_TABLE);
+    int offset = (int)index_frac;
+    eta = __dsub_rn(index_frac, (double)offset);
+    float y = 0.f;
+    const long long i_max = min(n + 1, (long long)((RS_NWIN - offset) / step));          // left wing
+    for (int i = 0; i < i_max; ++i)
+        y = (float)__dadd_rn((double)y, __dmul_rn(weight(offset + i * step), (double)wav_sample(x, n - i)));
+    frac = __dsub_rn(scale, frac);
+    index_frac = __dmul_rn(frac, (double)RS_TABLE);
+    offset = (int)index_frac;
+    eta = __dsub_rn(index_frac, (double)offset);
+    const long long k_max = min((long long)u.n_in - n - 1, (long long)((RS_NWIN - offset) / step));   // right wing
+    for (int k = 0; k < k_max; ++k)
+        y = (float)__dadd_rn((double)y, __dmul_rn(weight(offset + k * step), (double)wav_sample(x, n + k + 1)));
+    out[g] = y;
+}
+
+namespace {
+// I0 by its power series sum (x/2)^2k / (k!)^2, in long double
+double bessel_i0(double x) {
+    const long double q = (long double)x * x / 4;
+    long double term = 1, sum = 1;
+    for (int k = 1; k < 1000 && term > sum * 1e-22L; ++k) {
+        term *= q / ((long double)k * k);
+        sum += term;
+    }
+    return (double)sum;
+}
+}  // namespace
+
+// resampy 0.2 filters.sinc_window(num_zeros=64, precision=9, window=kaiser(beta), rolloff) for 'kaiser_best':
+// rolloff * sinc(rolloff * linspace(0, 64, 64*512 + 1)) times the right half of scipy.signal.kaiser(2*64*512 + 1, beta).
+void resample_filter_table(std::vector<double>& win) {
+    const double beta = 14.769656459379492, rolloff = 0.9475937167399596, pi = 3.141592653589793;
+    const int n = RS_NWIN - 1;
+    win.resize(RS_NWIN);
+    const double i0_beta = bessel_i0(beta);
+    for (int j = 0; j <= n; ++j) {
+        const double z = rolloff * ((double)j * (64.0 / n));                 // linspace: j * step, exact here
+        const double y = pi * (z == 0.0 ? 1.0e-20 : z);                      // np.sinc
+        const double r = (double)j / n;                                      // (m - alpha) / alpha, m = n + j
+        win[j] = bessel_i0(beta * std::sqrt(1.0 - r * r)) / i0_beta * (rolloff * (std::sin(y) / y));
+    }
+}
+
+// The register values 0, inc, fl(inc + inc), ... of n_out outputs as affine segments.  Inside one binade
+// [2^k, 2^(k+1)) every double is a multiple V g of g = 2^(k-52), and fl(V g + inc) = (V + S) g with S = inc / g rounded
+// to the nearest integer, as long as the result stays below 2^(k+1): one segment per binade.  When inc / g lies exactly
+// halfway, rounding goes to the even neighbour, so from an even V every step adds the even one of S0, S0 + 1; an odd V
+// takes one explicit addition first.  The first value (0) and each addition that leaves a binade are done in float64.
+// Appends to `out`; returns the number of segments.
+int resample_time_register(long long n_out, double inc, std::vector<TimeSeg>& out) {
+    const size_t first = out.size();
+    long long t = 0;
+    double v = 0.0;
+    while (t < n_out) {
+        long long S = -1, V = 0;
+        double g = 0.0;
+        if (v > 0.0) {
+            int e;
+            std::frexp(v, &e);                                  // v in [2^(e-1), 2^e)
+            g = std::ldexp(1.0, e - 53);
+            V = (long long)(v / g);                             // exact, in [2^52, 2^53)
+            const double q = inc / g, q0 = std::floor(q), fr = q - q0;   // exact (v >= inc, so q < 2^53)
+            const long long S0 = (long long)q0;
+            if (fr > 0.5) S = S0 + 1;
+            else if (fr < 0.5) S = S0;
+            else if (!(V & 1)) S = S0 + (S0 & 1);
+        }
+        if (S < 0) {                                            // zero, or a tie from an odd V: one explicit addition
+            out.push_back(TimeSeg{t, v, 0.0});
+            ++t;
+            v = v + inc;
+            continue;
+        }
+        const long long H = 1ll << 53;
+        const long long m = S > 0 ? (H - 1 - V) / S : n_out;    // additions that stay inside the binade
+        const long long len = std::min(m + 1, n_out - t);
+        out.push_back(TimeSeg{t, v, (double)S * g});
+        t += len;
+        v = (double)(V + (len - 1) * S) * g;
+        if (t < n_out) v = v + inc;                             // the addition that leaves the binade
+    }
+    return (int)(out.size() - first);
+}
+
+void resample_run(const void* wav, int dtype, const ResampleUtt* utt, int B, const TimeSeg* seg, const double* win, float* out,
+                  long long total, cudaStream_t s) {
+    const unsigned grid = (unsigned)((total + 255) / 256);
+    if (dtype == 1)
+        resample_kernel<int16_t><<<grid, 256, 0, s>>>(static_cast<const int16_t*>(wav), utt, B, seg, win, out, total);
+    else
+        resample_kernel<float><<<grid, 256, 0, s>>>(static_cast<const float*>(wav), utt, B, seg, win, out, total);
 }
 
 int voc_launches_per_call(int n_iter) { return 1 + 3 * n_iter + 2 + 3 + 1; }

@@ -291,30 +291,68 @@ class Engine:
                                                      C.byref(t), trim, self._stream()), "dctts_get_spectrograms")
         return mel[:t.value], mag[:t.value], (int(trim[0]), int(trim[1]))
 
-    def load_spectrograms_batch(self, wavs, sr=None, t_capacity=None):
-        """utils.py:147-162 for a list of 1-D int16 (PCM, value / 32768) or float32 waveforms at hp.sr, as ONE bucketed
-        batch: the waveforms cross to the device in one copy from a pinned buffer (int16 stays int16 when every member
-        is int16), two kernels compute all the features, and the call synchronises once.  Returns
-        (mels (B, T_b, n_mels), mags (B, r T_b, F)) contiguous CUDA tensors zero-padded to the longest member, the
-        reduced rows per utterance t (B,) int32 and the kept sample ranges trim (B, 2) int32 (numpy).  `t_capacity`
-        (reduced rows per utterance; default: enough for the untrimmed lengths) sizes the outputs."""
-        h = self.hp
+    def _pack(self, wavs, what):
+        """1-D int16 / float32 waveforms -> (device tensor of them back to back, 1 if int16 else 0, int64 offsets (B+1)),
+        through one pinned host buffer and one copy.  int16 stays int16 when every member is int16."""
         arrs = [np.asarray(w).reshape(-1) for w in wavs]
         if not arrs:
-            raise DcttsError("load_spectrograms_batch: empty batch")
+            raise DcttsError("%s: empty batch" % what)
         pcm = all(a.dtype == np.int16 for a in arrs)
         if not pcm:
             arrs = [a.astype(np.float32) / np.float32(32768.0) if a.dtype == np.int16 else np.asarray(a, np.float32) for a in arrs]
-        B = len(arrs)
-        offsets = np.zeros(B + 1, np.int64)
+        offsets = np.zeros(len(arrs) + 1, np.int64)
         offsets[1:] = np.cumsum([a.size for a in arrs])
         host = torch.empty(int(offsets[-1]), dtype=torch.int16 if pcm else torch.float32, pin_memory=True)
         hv = host.numpy()
         for b, a in enumerate(arrs):
             hv[offsets[b]:offsets[b + 1]] = a
-        wav = host.to(self.device, non_blocking=True)
+        return host.to(self.device, non_blocking=True), 1 if pcm else 0, offsets
+
+    def _resample(self, wav, dtype, offsets, rates, sr_out, out=None):
+        """dctts_resample_batch on packed device samples: -> (float32 outputs back to back, int64 offsets (B+1))."""
+        B = len(offsets) - 1
+        rates = np.ascontiguousarray(rates, np.int32)
+        if rates.shape != (B,):
+            raise DcttsError("resample: %d rates for %d utterances" % (rates.size, B))
+        ratio = sr_out / np.maximum(rates, 1).astype(np.float64)
+        cap = int(np.ceil(np.diff(offsets) * np.where(rates == sr_out, 1.0, ratio)).sum())
+        if out is None or out.numel() < cap:
+            out = self._empty(max(cap, 1))
+        out_offsets = np.zeros(B + 1, np.int64)
+        i64p = C.POINTER(C.c_int64)
+        self._check(self._lib.dctts_resample_batch(
+            self._h, _ptr(wav), dtype, offsets.ctypes.data_as(i64p), rates.ctypes.data_as(C.POINTER(C.c_int32)), B, int(sr_out),
+            _ptr(out), out.numel(), out_offsets.ctypes.data_as(i64p), self._stream()), "dctts_resample_batch")
+        return out, out_offsets
+
+    def resample_batch(self, wavs, rates, sr_out=None):
+        """What librosa.load(..., sr=sr_out) does after decoding (librosa 0.6 core.resample, res_type='kaiser_best',
+        fix=True) for a list of 1-D int16 (PCM, value / 32768) or float32 waveforms at their native `rates`: one copy to
+        the device, one kernel, no synchronisation.  Returns the float32 results as a list of CUDA tensors (views of one
+        buffer); an utterance already at sr_out (default hp.sr) comes back unchanged, as float32."""
+        wav, dtype, offsets = self._pack(wavs, "resample_batch")
+        out, oo = self._resample(wav, dtype, offsets, rates, int(sr_out or self.hp.sr))
+        return [out[oo[b]:oo[b + 1]] for b in range(len(oo) - 1)]
+
+    def load_spectrograms_batch(self, wavs, sr=None, t_capacity=None, rates=None):
+        """utils.py:147-162 for a list of 1-D int16 (PCM, value / 32768) or float32 waveforms, as ONE bucketed
+        batch: the waveforms cross to the device in one copy from a pinned buffer (int16 stays int16 when every member
+        is int16), two kernels compute all the features, and the call synchronises once.  `rates` gives each waveform's
+        native sample rate (None: all at `sr`, default hp.sr); when some differ, one more kernel first resamples the
+        batch to `sr` as librosa.load(..., sr=hp.sr) does (`resample_batch`) into a buffer the engine keeps, and the
+        features read that.  Returns (mels (B, T_b, n_mels), mags (B, r T_b, F)) contiguous CUDA tensors zero-padded to
+        the longest member, the reduced rows per utterance t (B,) int32 and the kept sample ranges trim (B, 2) int32
+        (numpy; at `sr`).  `t_capacity` (reduced rows per utterance; default: enough for the untrimmed lengths) sizes
+        the outputs."""
+        h = self.hp
+        sr = int(sr or h.sr)
+        wav, dtype, offsets = self._pack(wavs, "load_spectrograms_batch")
+        B = len(offsets) - 1
+        if rates is not None and any(int(r) != sr for r in rates):
+            self._rs_out, offsets = self._resample(wav, dtype, offsets, rates, sr, getattr(self, "_rs_out", None))
+            wav, dtype = self._rs_out, 0
         if t_capacity is None:
-            t_capacity = max(-(-(1 + a.size // h.hop_length) // h.r) for a in arrs)
+            t_capacity = max(-(-(1 + int(n) // h.hop_length) // h.r) for n in np.diff(offsets))
         self._check(self._lib.dctts_set_vocoder_params(self._h, h.hop_length, h.win_length, float(h.power), float(h.max_db),
                                                        float(h.ref_db), float(h.preemphasis), int(h.n_iter)),
                     "dctts_set_vocoder_params")
@@ -325,7 +363,7 @@ class Engine:
         T_b = C.c_int32(0)
         i32p = C.POINTER(C.c_int32)
         self._check(self._lib.dctts_load_spectrograms_batch(
-            self._h, _ptr(wav), 1 if pcm else 0, offsets.ctypes.data_as(C.POINTER(C.c_int64)), B, int(sr or h.sr), _ptr(mel),
+            self._h, _ptr(wav), dtype, offsets.ctypes.data_as(C.POINTER(C.c_int64)), B, sr, _ptr(mel),
             _ptr(mag), int(t_capacity), t.ctypes.data_as(i32p), trim.ctypes.data_as(i32p), C.byref(T_b), self._stream()),
             "dctts_load_spectrograms_batch")
         T_b = T_b.value

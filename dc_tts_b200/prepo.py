@@ -17,9 +17,10 @@ def _save(out_dir, fname, mel, mag):
     np.save(os.path.join(out_dir, "mags", fname.replace("wav", "npy")), mag)
 
 
-def prepo(data_dir=None, out_dir=".", load_spectrograms=None, progress=None, batch_size=None, engine=None):
+def prepo(data_dir=None, out_dir=".", load_spectrograms=None, progress=None, batch_size=None, engine=None, resample=False):
     """`load_spectrograms(fpath) -> (fname, mel, mag)`, when given, is called file by file; by default the files go to the
-    device `batch_size` (hp.B) at a time."""
+    device `batch_size` (hp.B) at a time.  `resample=True` accepts files at any sample rate and resamples them to hp.sr on
+    the device (utils.load_spectrograms_batch); otherwise a file at another rate is refused."""
     fpaths, _, _ = load_train_data(data_dir)
     for sub in ("mels", "mags"):
         os.makedirs(os.path.join(out_dir, sub), exist_ok=True)
@@ -33,16 +34,16 @@ def prepo(data_dir=None, out_dir=".", load_spectrograms=None, progress=None, bat
     for fpath in stream:
         chunk.append(fpath)
         if len(chunk) == batch_size:
-            _save_batch(out_dir, chunk, engine)
+            _save_batch(out_dir, chunk, engine, resample)
             chunk = []
     if chunk:
-        _save_batch(out_dir, chunk, engine)
+        _save_batch(out_dir, chunk, engine, resample)
     return len(fpaths)
 
 
-def _save_batch(out_dir, fpaths, engine):
+def _save_batch(out_dir, fpaths, engine, resample):
     from .utils import load_spectrograms_batch
-    fnames, mels, mags, t = load_spectrograms_batch(fpaths, engine)
+    fnames, mels, mags, t = load_spectrograms_batch(fpaths, engine, resample)
     mels, mags = mels.cpu().numpy(), mags.cpu().numpy()
     for b, fname in enumerate(fnames):
         _save(out_dir, fname, mels[b, :t[b]], mags[b, :hp.r * t[b]])

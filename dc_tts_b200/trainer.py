@@ -1,6 +1,6 @@
 """The trainer loop around `Engine.train_step` / `train_step_ssrn` -- what `python train.py 1|2` does in the reference
 (/root/reference/train.py:137-160: one optimiser step per batch, a checkpoint `model_gs_{NNN}k` every 1000 steps in
-`hp.logdir + "-" + num`, stop after hp.num_iterations) on top of the LJ transcript parser of data_load.py:41-56 and the
+`hp.logdir + "-" + num`, stop after hp.num_iterations) on top of the transcript parser of data_load.py:41-77 and the
 pre-computed `mels/*.npy`, `mags/*.npy` of prepo.py (data_load.py:104-112), or, with hp.prepro = False, features computed
 on the device from the wav files one bucket at a time.
 
@@ -20,15 +20,35 @@ from .data_load import load_vocab, text_normalize
 from .hyperparams import Hyperparams as hp
 
 
+def _text_ids(char2idx, text, transcript, lineno):
+    """`[char2idx[char] for char in text]` (data_load.py:54,73); a character outside hp.vocab raises, naming the line."""
+    try:
+        return np.array([char2idx[ch] for ch in text], np.int32)
+    except KeyError as e:
+        raise ValueError("%s:%d: character %r is not in hp.vocab" % (transcript, lineno, e.args[0])) from None
+
+
 def load_train_data(data_dir=None):
-    """data_load.py:41-56 (LJ Speech): transcript.csv -> (wav paths, text lengths, int32 id arrays ending in E)."""
+    """data_load.py:41-77: transcript.csv -> (wav paths, text lengths, int32 id arrays ending in E).  As in the reference,
+    a data path containing "LJ" is LJ Speech (`fname|raw|text`, wavs/<fname>.wav, text normalised); any other is the
+    five-field format of its other corpora (`fname|raw|text|is_inside_quotes|duration`, the path joined to fname as is,
+    no normalisation, clips longer than 10 s skipped)."""
     data_dir = data_dir or hp.data
     char2idx, _ = load_vocab()
+    transcript = os.path.join(data_dir, "transcript.csv")
+    lj = "LJ" in data_dir
     fpaths, text_lengths, texts = [], [], []
-    for line in codecs.open(os.path.join(data_dir, "transcript.csv"), "r", "utf-8").readlines():
-        fname, _, text = line.strip().split("|")
-        ids = np.array([char2idx[ch] for ch in text_normalize(text) + "E"], np.int32)
-        fpaths.append(os.path.join(data_dir, "wavs", fname + ".wav"))
+    for lineno, line in enumerate(codecs.open(transcript, "r", "utf-8").readlines(), 1):
+        if lj:
+            fname, _, text = line.strip().split("|")
+            fpath, text = os.path.join(data_dir, "wavs", fname + ".wav"), text_normalize(text)
+        else:
+            fname, _, text, _, duration = line.strip().split("|")
+            if float(duration) > 10.:
+                continue
+            fpath = os.path.join(data_dir, fname)
+        ids = _text_ids(char2idx, text + "E", transcript, lineno)
+        fpaths.append(fpath)
         text_lengths.append(len(ids))
         texts.append(ids)
     return fpaths, text_lengths, texts
@@ -102,7 +122,7 @@ def _pad_spectrograms(items):
 
 
 def bucketed_batches(fpaths, text_lengths, texts, B=None, seed=0, loader=_load_spectrograms_npy, epochs=None, rank=0, world=1,
-                     prepro=None, engine=None, features=None):
+                     prepro=None, engine=None, features=None, resample=False):
     """The reference's input pipeline (data_load.py:88-131) without TensorFlow queues: a shuffled stream of utterances
     (slice_input_producer :99) is routed by TEXT length into buckets (boundaries :125); a bucket that has collected B
     utterances emits them as one batch, every tensor padded with zeros to the longest member of THAT batch
@@ -113,19 +133,20 @@ def bucketed_batches(fpaths, text_lengths, texts, B=None, seed=0, loader=_load_s
     ranks' batches are disjoint (their shapes may differ from rank to rank).
 
     `prepro` (default hp.prepro) picks where the spectrograms come from, as in data_load.py:104-113.  True: `loader`
-    reads what prepo.py wrote (numpy batches).  False: the buckets collect the wav files' samples and a full bucket gets
-    its features from ONE batched device call, `features(pcms) -> (mels, mags)` (default
-    `(engine or get_engine()).load_spectrograms_batch`), so mels and mags are CUDA tensors and no mels/ or mags/
-    directory is needed.  The features run on the caller's thread (an engine handle is not thread-safe).  Routing,
+    reads what prepo.py wrote (numpy batches).  False: the buckets collect the wav files' samples and native sample
+    rates, and a full bucket gets its features from ONE batched device call, `features(pcms) -> (mels, mags)` when every
+    file is at hp.sr and `features(pcms, rates)` otherwise (default `(engine or get_engine()).load_spectrograms_batch`,
+    which resamples to hp.sr on the device first), so mels and mags are CUDA tensors and no mels/ or mags/ directory is
+    needed.  A file at another rate than hp.sr is refused unless `resample=True` (a corpus at 16, 44.1 or 48 kHz).  The features run on the caller's thread (an engine handle is not thread-safe).  Routing,
     sharding and padding are the same loop for both routes."""
     B = B or hp.B
     from_wavs = not (hp.prepro if prepro is None else prepro)
     if from_wavs:
-        from .utils import _load_pcm
+        from .utils import _read_pcm_for
         if features is None:
-            def features(pcms):
+            def features(pcms, rates=None):
                 from .engine import get_engine
-                return (engine or get_engine()).load_spectrograms_batch(pcms)[:2]
+                return (engine or get_engine()).load_spectrograms_batch(pcms, rates=rates)[:2]
     bounds = bucket_boundaries(text_lengths)
     pending = [[] for _ in range(len(bounds) + 1)]
     rng = np.random.default_rng(seed)
@@ -135,7 +156,7 @@ def bucketed_batches(fpaths, text_lengths, texts, B=None, seed=0, loader=_load_s
         for i in rng.permutation(len(fpaths))[rank::world]:
             k = bucket_index(text_lengths[i], bounds)
             if from_wavs:
-                pending[k].append((texts[i], _load_pcm(fpaths[i]), os.path.basename(fpaths[i])))
+                pending[k].append((texts[i], _read_pcm_for(fpaths[i], resample), os.path.basename(fpaths[i])))
             else:
                 fname, mel, mag = loader(fpaths[i])
                 pending[k].append((texts[i], (mel, mag), fname))
@@ -144,7 +165,11 @@ def bucketed_batches(fpaths, text_lengths, texts, B=None, seed=0, loader=_load_s
                 L = np.zeros((B, max(len(t) for t, _, _ in items)), np.int32)
                 for b, (t, _, _) in enumerate(items):
                     L[b, :len(t)] = t
-                mels, mags = (features if from_wavs else _pad_spectrograms)([it[1] for it in items])
+                if not from_wavs:
+                    mels, mags = _pad_spectrograms([it[1] for it in items])
+                else:
+                    pcms, rates = [it[1][0] for it in items], [it[1][1] for it in items]
+                    mels, mags = features(pcms) if all(r == hp.sr for r in rates) else features(pcms, rates)
                 emitted += 1
                 yield L, mels, mags, [it[2] for it in items], k
         if emitted == 0 and epochs is None and epoch >= 64:

@@ -7,9 +7,11 @@ in shared memory) behind `dctts_spectrogram2wav`.  This is the first "next" row 
 of the Text2Mel + SSRN hot path.  Feature extraction (`get_spectrograms`, `load_spectrograms`,
 utils.py:20-65,147-162) runs on the GPU too (`dctts_get_spectrograms` / `dctts_load_spectrograms_batch`: trim,
 pre-emphasis, STFT, mel filterbank, dB, normalisation in two kernels per call, for one utterance or a whole bucket);
-`librosa.load` is replaced by scipy's WAV reader
-for files that already have hp.sr (LJ Speech does) -- resampling, plotting and the training helpers of the
-reference's utils.py stay out of scope.
+`librosa.load` is replaced by scipy's WAV reader,
+and with `resample=True` a file at another sample rate is resampled to hp.sr on the GPU as librosa.load(fpath, sr=hp.sr)
+does (`dctts_resample_batch`: librosa 0.6 / resampy 'kaiser_best'); without it such a file is refused, so a corpus at an
+unexpected rate is never converted silently.  Other file formats, plotting and the training helpers
+of the reference's utils.py stay out of scope.
 """
 import os
 
@@ -66,18 +68,37 @@ def invert_spectrogram(spectrogram):
 
 def _read_wav(fpath):
     """The samples of a WAV file at hp.sr as scipy reads them (raises for another sample rate)."""
-    from scipy.io import wavfile
-    sr, y = wavfile.read(fpath)
+    y, sr = _read_raw(fpath)
     if sr != hp.sr:
-        raise ValueError("%s: sample rate %d != hp.sr %d (resampling is not implemented)" % (fpath, sr, hp.sr))
+        raise ValueError("%s: sample rate %d != hp.sr %d (this reader does not resample; _read_pcm returns the native rate)"
+                         % (fpath, sr, hp.sr))
     return y
 
 
+def _read_raw(fpath):
+    from scipy.io import wavfile
+    sr, y = wavfile.read(fpath)
+    return y, int(sr)
+
+
+def _read_pcm(fpath):
+    """(samples, native sample rate) of a WAV file for the batched feature path: mono int16 stays int16 (the device
+    divides by 32768, exactly as `_load_wav` does); every other format is converted on the host by `_load_wav`'s rules."""
+    y, sr = _read_raw(fpath)
+    return (y if (y.ndim == 1 and y.dtype == np.int16) else _load_wav_samples(y)), sr
+
+
+def _read_pcm_for(fpath, resample):
+    """`_read_pcm`, refusing a file at another rate than hp.sr unless the caller asked to `resample` it."""
+    y, sr = _read_pcm(fpath)
+    if sr != hp.sr and not resample:
+        raise ValueError("%s: sample rate %d != hp.sr %d (pass resample=True to resample it to hp.sr)" % (fpath, sr, hp.sr))
+    return y, sr
+
+
 def _load_pcm(fpath):
-    """A WAV file for the batched feature path: mono int16 stays int16 (the device divides by 32768, exactly as
-    `_load_wav` does); every other format is converted on the host by `_load_wav`'s rules."""
-    y = _read_wav(fpath)
-    return y if (y.ndim == 1 and y.dtype == np.int16) else _load_wav_samples(y)
+    """`_read_pcm` for a file that must already be at hp.sr (raises for another sample rate)."""
+    return _read_pcm_for(fpath, False)[0]
 
 
 def _load_wav(fpath):
@@ -86,29 +107,41 @@ def _load_wav(fpath):
 
 
 def _load_wav_samples(y):
-    if y.ndim > 1:
-        y = y.mean(axis=1)
+    """librosa's buf_to_float then to_mono: each channel is scaled to float32 first, then the channels are averaged."""
     if y.dtype == np.int16:
         y = y.astype(np.float32) / 32768.0
     elif y.dtype == np.int32:
         y = y.astype(np.float32) / 2147483648.0
     elif y.dtype == np.uint8:
         y = (y.astype(np.float32) - 128.0) / 128.0
+    y = np.asarray(y, np.float32)
+    if y.ndim > 1:
+        y = y.mean(axis=1)
     return np.ascontiguousarray(y, np.float32)
 
 
-def get_spectrograms(fpath):
-    """utils.py:20-65.  `fpath`: a WAV file path, or the already loaded waveform (1-D float array at hp.sr).
+def _path(fpath):
+    return isinstance(fpath, (str, bytes, os.PathLike))
+
+
+def get_spectrograms(fpath, resample=False):
+    """utils.py:20-65.  `fpath`: a WAV file path at hp.sr -- or at any rate with `resample=True`, resampled to hp.sr on
+    the device first as librosa.load(fpath, sr=hp.sr) does -- or the already loaded waveform (1-D float array at hp.sr).
     Returns normalised mel (T, n_mels) and linear magnitude (T, 1+n_fft/2), float32 numpy."""
-    y = _load_wav(fpath) if isinstance(fpath, (str, bytes, os.PathLike)) else np.asarray(fpath, np.float32)
-    mel, mag, _ = get_engine().get_spectrograms(y)
+    e = get_engine()
+    if _path(fpath):
+        y, sr = _read_pcm_for(fpath, resample)
+        y = e.resample_batch([y], [sr])[0] if sr != hp.sr else _load_wav_samples(y)
+    else:
+        y = np.asarray(fpath, np.float32)
+    mel, mag, _ = e.get_spectrograms(y)
     return mel.cpu().numpy(), mag.cpu().numpy()
 
 
-def load_spectrograms(fpath):
-    """utils.py:147-162: pads T to a multiple of hp.r and keeps every r-th mel frame."""
-    fname = os.path.basename(fpath) if isinstance(fpath, (str, bytes, os.PathLike)) else None
-    mel, mag = get_spectrograms(fpath)
+def load_spectrograms(fpath, resample=False):
+    """utils.py:147-162: pads T to a multiple of hp.r and keeps every r-th mel frame (`resample`: see get_spectrograms)."""
+    fname = os.path.basename(fpath) if _path(fpath) else None
+    mel, mag = get_spectrograms(fpath, resample)
     t = mel.shape[0]
     num_paddings = hp.r - (t % hp.r) if t % hp.r != 0 else 0
     mel = np.pad(mel, [[0, num_paddings], [0, 0]], mode="constant")
@@ -117,12 +150,13 @@ def load_spectrograms(fpath):
     return fname, mel, mag
 
 
-def load_spectrograms_batch(fpaths, engine=None):
+def load_spectrograms_batch(fpaths, engine=None, resample=False):
     """`load_spectrograms` for several WAV files in one device call (`Engine.load_spectrograms_batch`), padded with zeros
-    as one bucketed batch.  Returns (fnames, mels (B, T_b, n_mels), mags (B, r T_b, F), t): CUDA tensors, and the reduced
-    rows t (B,) of each utterance -- utterance b is mels[b, :t[b]], mags[b, :r t[b]], bit for bit what
-    `load_spectrograms` returns for it."""
-    mels, mags, t, _ = (engine or get_engine()).load_spectrograms_batch([_load_pcm(p) for p in fpaths])
+    as one bucketed batch; with `resample=True` the files may be at any sample rates and are resampled to hp.sr first.
+    Returns (fnames, mels (B, T_b, n_mels), mags (B, r T_b, F), t): CUDA tensors, and the reduced rows t (B,) of each
+    utterance -- utterance b is mels[b, :t[b]], mags[b, :r t[b]], bit for bit what `load_spectrograms` returns for it."""
+    pcms, rates = zip(*[_read_pcm_for(p, resample) for p in fpaths])
+    mels, mags, t, _ = (engine or get_engine()).load_spectrograms_batch(list(pcms), rates=list(rates))
     return [os.path.basename(p) for p in fpaths], mels, mags, t
 
 

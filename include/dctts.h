@@ -161,6 +161,31 @@ int dctts_get_spectrograms(dctts_handle h, const float* wav, int64_t n_samples, 
 int dctts_load_spectrograms_batch(dctts_handle h, const void* wav, int32_t dtype, const int64_t* offsets_host, int32_t B,
                                   int32_t sample_rate, float* mel, float* mag, int32_t t_capacity,
                                   int32_t* t_host, int32_t* trim_host, int32_t* T_b_out, void* stream);
+/* What librosa.load(fpath, sr=sr_out) adds after decoding, for B utterances packed back to back: librosa 0.6
+ * core.resample(y, sr_host[b], sr_out, res_type='kaiser_best', fix=True) = resampy 0.2 resample / resample_f.
+ * wav: DEVICE, dtype 0 = float32, 1 = int16 PCM (value / 32768); offsets_host: B+1 HOST int64 sample offsets;
+ * sr_host: B HOST native rates.  out: DEVICE float32, the B results back to back, at most out_capacity samples;
+ * out_offsets_host (B+1) receives their offsets.  Per utterance, with ratio = float(sr_out) / sr_in:
+ *   - sr_in == sr_out: returned unchanged (librosa's early return), only converted to float32;
+ *   - otherwise int(n ratio) samples of resample_f, zero-padded to ceil(n ratio) (util.fix_length).  Output t:
+ *     n = int(reg), frac = scale (reg - n), scale = min(1, ratio), offset = int(512 frac), eta = 512 frac - offset;
+ *     left wing i < min(n + 1, (nwin - offset) // index_step) on x[n - i], then frac = scale - frac and the right wing
+ *     k < min(n_in - n - 1, (nwin - offset) // index_step) on x[n + k + 1], weight win[j] + eta delta[j] at
+ *     j = offset + i index_step, index_step = int(512 scale); a float32 accumulator, each tap rounded
+ *     float32(double(y) + weight double(x)).  reg is the float64 register resampy advances by 1 / ratio per output.
+ *   - the filter is kaiser_best: the half window rolloff sinc(rolloff linspace(0, 64, 64*512 + 1)) times the right half
+ *     of a Kaiser window (beta 14.769656459379492, rolloff 0.9475937167399596), times ratio when ratio < 1; delta is its
+ *     first difference, 0 at the end.
+ * One kernel, no synchronisation: a following dctts_load_spectrograms_batch(dtype = 0) on the same stream keeps its one.
+ * Fails, naming the utterance, with nothing written or launched, on a rate <= 0, an input of 0 samples, an output
+ * shorter than 1 sample (int(n ratio) < 1, where resampy raises) or more than out_capacity samples in all. */
+int dctts_resample_batch(dctts_handle h, const void* wav, int32_t dtype, const int64_t* offsets_host, const int32_t* sr_host,
+                         int32_t B, int32_t sr_out, float* out, int64_t out_capacity, int64_t* out_offsets_host, void* stream);
+/* The time register dctts_resample_batch computes for n_out outputs from sr_in to sr_out, as the affine segments the
+ * kernel evaluates: register(t) = v0[i] + (t - t0[i]) step[i] for t0[i] <= t < t0[i+1].  Returns the number of
+ * segments, or -1 for bad arguments or more than `capacity`.  No handle, no GPU. */
+int32_t dctts_resample_time_register(int64_t n_out, int32_t sr_in, int32_t sr_out, int64_t* t0, double* v0, double* step,
+                                     int32_t capacity);
 
 /* ---- training step (BASELINE config 5; SURVEY 8f-3) --------------------------------------
  * One optimiser step of the reference's Text2Mel trainer -- graph train.py:43-68 in mode "train" (dropout after
