@@ -42,6 +42,8 @@ SIGNATURES = {
     "dctts_synthesize_host": (C.c_int, [Handle, _p, _i32, _p, _p]),
     "dctts_bench_block": (C.c_int, [Handle, C.c_char_p, _i32, _i32, _i32, _i32, C.POINTER(C.c_float),
                                     C.POINTER(_i32), _p]),
+    "dctts_conv_gemm": (C.c_int, [Handle, _i32, _i32, _p, _i32, _i32, _i32, _i32, _p, _i32, _i32, _i32, C.POINTER(_i32), _p,
+                                  _i32, _p, _i32, _p]),
     "dctts_set_vocoder_params": (C.c_int, [Handle, _i32, _i32, C.c_float, C.c_float, C.c_float, C.c_float, _i32]),
     "dctts_spectrogram2wav": (C.c_int, [Handle, _p, _i32, _i32, _i32, _p, _p, _p]),
     "dctts_get_spectrograms": (C.c_int, [Handle, _p, _i64, _i32, _p, _p, _i32, C.POINTER(_i32), C.POINTER(_i32), _p]),

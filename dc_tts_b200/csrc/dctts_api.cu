@@ -1966,6 +1966,71 @@ int dctts_bench_block(dctts_handle h, const char* scope, int32_t B, int32_t L, i
     });
 }
 
+int dctts_conv_gemm(dctts_handle h, int32_t impl, int32_t mode, const float* X, int32_t ldx, int32_t B, int32_t L, int32_t K,
+                    const float* Wd, int32_t ldwd, int32_t N, int32_t ntaps, const int32_t* shifts_host, const float* bias,
+                    int32_t accumulate, float* out, int32_t ldo, void* stream) {
+    struct Bufs {                                   // the call's own wgmma workspace, freed on every exit
+        DevBuf b[5];
+        ~Bufs() { for (auto& d : b) d.release(); }
+    } bufs;
+    return guarded(h, [&] {
+        REQUIRE(impl == 0 || impl == 1, "dctts_conv_gemm: impl must be 0 (fp32 CUDA cores) or 1 (wgmma)");
+        REQUIRE(mode == 0 || mode == 1, "dctts_conv_gemm: mode must be 0 (conv) or 1 (weight gradient)");
+        REQUIRE(X && Wd && out && shifts_host && B >= 1 && L >= 1 && K >= 1 && N >= 1 && ntaps >= 1 && ntaps <= 3,
+                "dctts_conv_gemm: bad arguments");
+        REQUIRE(ldx % 4 == 0 && ldwd % 4 == 0 && ldo % 4 == 0, "dctts_conv_gemm: ldx, ldwd and ldo must be multiples of 4");
+        REQUIRE(ldx >= K && ldwd >= N && ldo >= N, "dctts_conv_gemm: a pitch is narrower than its tensor's width");
+        auto aligned = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+        REQUIRE(aligned(X) && aligned(Wd) && aligned(out) && aligned(bias), "dctts_conv_gemm: every tensor must be 16-byte aligned");
+        if (mode == 0) {
+            // the fp32 kernel reads W and bias and writes out over the whole pitch ldwd (ConvArgs: ldy == ldw)
+            REQUIRE(bias && ldo == ldwd && (accumulate == 0 || accumulate == 1),
+                    "dctts_conv_gemm: mode 0 needs a bias of ldwd floats, ldo == ldwd and accumulate 0 or 1");
+        } else {
+            REQUIRE(!bias && accumulate == 1, "dctts_conv_gemm: mode 1 adds into out (accumulate = 1) and takes no bias");
+        }
+        cudaStream_t s = S(h, stream);
+        GemmTcWs ws;
+        if (impl == 1) {
+            const size_t a_el = mode == 0 ? (size_t)B * L * roundup(K, 8) : (size_t)ntaps * B * K * roundup(L, 8);
+            const size_t b_el = mode == 0 ? (size_t)roundup(N, 256) * ntaps * roundup(K, 32) : (size_t)B * N * roundup(L, 8);
+            for (int i = 0; i < 2; ++i) bufs.b[i].ensure(a_el * sizeof(__half));
+            for (int i = 2; i < 4; ++i) bufs.b[i].ensure(b_el * sizeof(__half));
+            bufs.b[4].ensure(4 * sizeof(unsigned));
+            ws.a_hi = bufs.b[0].as<__half>(); ws.a_lo = bufs.b[1].as<__half>(); ws.a_elems = a_el;
+            ws.b_hi = bufs.b[2].as<__half>(); ws.b_lo = bufs.b[3].as<__half>(); ws.b_elems = b_el;
+            ws.slots = bufs.b[4].as<unsigned>(); ws.n_slots = 4;
+            gemm_tc_begin_step(ws, s);
+        }
+        int launches = 1;
+        if (mode == 0) {
+            ConvArgs c{};
+            c.X = X; c.ldx = ldx; c.Y = out; c.ldy = ldo; c.bias = bias; c.K = K; c.N = N; c.ldw = ldwd;
+            c.ntaps = ntaps;
+            for (int j = 0; j < ntaps; ++j) c.taps[j] = ConvTap{Wd + (size_t)j * K * ldwd, shifts_host[j]};
+            c.win = RowWin{B, L, L, nullptr}; c.Lout = L; c.ostride = 1; c.ooff = 0; c.accumulate = accumulate;
+            if (impl == 0) launch_conv_gemm(c, s, 0, false);
+            else {
+                REQUIRE(conv_gemm_tc_ok(c, ws), "dctts_conv_gemm: conv_gemm_tc_ok does not hold for this call");
+                launches = launch_conv_gemm_tc(c, ws, s);
+            }
+        } else {
+            WgradArgs w{};
+            w.X = X; w.ldx = ldx; w.dy = Wd; w.ldy = ldwd; w.dW = out; w.ldw = ldo;
+            w.rows = (long long)B * L; w.L = L; w.K = K; w.N = N; w.ntaps = ntaps;
+            for (int j = 0; j < ntaps; ++j) w.shifts[j] = shifts_host[j];
+            if (impl == 0) launch_conv_wgrad(w, s);
+            else {
+                REQUIRE(conv_wgrad_tc_ok(w, B, ws), "dctts_conv_gemm: conv_wgrad_tc_ok does not hold for this call");
+                launches = launch_conv_wgrad_tc(w, B, ws, s);
+            }
+        }
+        h->launches += launches;
+        CUDA_CHECK(cudaGetLastError());
+        CUDA_CHECK(cudaStreamSynchronize(s));      // before the workspace is freed
+    });
+}
+
 int dctts_set_vocoder_params(dctts_handle h, int32_t hop_length, int32_t win_length, float power, float max_db,
                              float ref_db, float preemphasis, int32_t n_iter) {
     return guarded(h, [&] {

@@ -184,7 +184,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
     const int r = threadIdx.x & 127;
     const float* arow = s_acc + (size_t)r * acc_ld;
     const int c_beg = mh == 0 ? 0 : ((bn / 2 + 31) & ~31), c_end = mh == 0 ? ((bn / 2 + 31) & ~31) : bn;
-    const float inv = 1.0f / (slot_scale(a.slot_a) * slot_scale(a.slot_b));      // both powers of two: exact
+    // both scales are powers of two up to 2^127: their product overflows for operands of max ~1e-16 (and would zero every
+    // output), so the inverses are taken one at a time -- each is exact, and so is theirs down to 2^-149
+    const float inv = (1.0f / slot_scale(a.slot_a)) * (1.0f / slot_scale(a.slot_b));
     if (a.mode == 0) {
         const int t = t0 + r;
         if (t < a.L) {

@@ -140,6 +140,26 @@ class Engine:
                                                 self._stream()), "dctts_bench_block")
         return [float(ms[i]) for i in range(n.value)]
 
+    def conv_gemm(self, impl, mode, X, K, Wd, N, shifts, out, bias=None, accumulate=0):
+        """Test aid (include/dctts.h: dctts_conv_gemm): one conv-GEMM of the training step, in place on `out`.
+        impl 0 = fp32 CUDA-core kernels, 1 = wgmma.  Every tensor is a CUDA float32 view with unit stride in its last dim;
+        the row pitches are the views' strides.  X (B, L, >= K).  Mode 0: Wd (ntaps, K, >= N) = W, out (B, L, ldo), bias.
+        Mode 1: Wd (B, L, >= N) = dY, out (ntaps, K, >= N) += the weight gradient."""
+        ts = [X, Wd, out] + ([bias] if bias is not None else [])
+        if not all(t.is_cuda and t.dtype == torch.float32 and t.stride(-1) == 1 for t in ts):
+            raise DcttsError("conv_gemm: CUDA float32 tensors with a unit inner stride expected")
+        B, L = X.shape[0], X.shape[1]
+        rows_ok = X.stride(0) == L * X.stride(1) and (mode == 1 or out.stride(0) == L * out.stride(1))
+        taps_ok = (Wd.stride(0) == K * Wd.stride(1)) if mode == 0 else (out.stride(0) == K * out.stride(1))
+        dy_ok = mode == 0 or (Wd.shape[0] == B and Wd.shape[1] == L and Wd.stride(0) == L * Wd.stride(1))
+        if not (rows_ok and taps_ok and dy_ok):
+            raise DcttsError("conv_gemm: rows or taps of a tensor are not evenly pitched")
+        sh = (C.c_int32 * len(shifts))(*[int(s) for s in shifts])
+        self._check(self._lib.dctts_conv_gemm(self._h, int(impl), int(mode), _ptr(X), X.stride(1), B, L, int(K), _ptr(Wd),
+                                              Wd.stride(1), int(N), len(shifts), sh, _ptr(bias), int(accumulate), _ptr(out),
+                                              out.stride(1), self._stream()), "dctts_conv_gemm")
+        return out
+
     def launch_count(self):
         return int(self._lib.dctts_launch_count(self._h))
 

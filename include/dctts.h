@@ -269,6 +269,19 @@ int dctts_decode_profile(dctts_handle h, int64_t* cycles, int32_t n);
  * kernels (CUDA events on `stream` around every launch), ms_per_kernel[0..*n_kernels), <= 8. */
 int dctts_bench_block(dctts_handle h, const char* scope, int32_t B, int32_t L, int32_t iters,
                       int32_t warmup, float* ms_per_kernel, int32_t* n_kernels, void* stream);
+/* Test aid: ONE conv-GEMM of the training step on caller DEVICE tensors, through the launch functions the step calls;
+ * the training state is not touched (the wgmma set gets a workspace and fresh abs-max slots of its own).
+ *   impl 0: the float32 CUDA-core kernels (tiled conv GEMM, conv_wgrad_kernel); impl 1: the wgmma split-fp16 kernels.
+ *   mode 0: out[b,t,n] (+)= bias[n] + sum_j sum_k X[b, t+shifts[j], k] W_j[k][n]   (zero outside [0, L) of utterance b)
+ *           Wd = W_0 | W_1 | ... each [K][ldwd]; out (B, L, ldo) with ldo == ldwd; bias has ldwd floats; accumulate 0 or 1.
+ *   mode 1: out_j[k][n] += sum_b sum_t X[b, t+shifts[j], k] dY[b,t,n]
+ *           Wd = dY, B*L rows of pitch ldwd; out = out_0 | out_1 | ... each [K][ldo]; bias NULL, accumulate 1.
+ * X: B*L rows of pitch ldx.  1 <= ntaps <= 3; shifts_host: ntaps HOST ints.  Fails with a message, leaving out untouched, when
+ * a pitch is not a multiple of 4 or narrower than its width, a tensor is not 16-byte aligned, or (impl 1) the wgmma
+ * kernels' preconditions do not hold: it never switches to the other kernel set.  Synchronises `stream`. */
+int dctts_conv_gemm(dctts_handle h, int32_t impl, int32_t mode, const float* X, int32_t ldx, int32_t B, int32_t L, int32_t K,
+                    const float* Wd, int32_t ldwd, int32_t N, int32_t ntaps, const int32_t* shifts_host, const float* bias,
+                    int32_t accumulate, float* out, int32_t ldo, void* stream);
 /* Raw device memory helpers so that a host without torch can drive the library. */
 int dctts_malloc(dctts_handle h, void** ptr, int64_t bytes);
 int dctts_free(dctts_handle h, void* ptr);

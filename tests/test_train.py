@@ -184,11 +184,12 @@ def test_tie_free_set_has_no_relu_near_zero():
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("B,rate,seed,tc", [(2, 0.0, 0, 7), (2, 0.05, 11, 7), (3, 0.05, 4, 7), (2, 0.0, 0, 0), (2, 0.05, 11, 0), (3, 0.05, 4, 0),
-                                            (32, 0.05, 5, 7)])
+                                            (32, 0.05, 5, 7)] + [(2, 0.05, 11, tc) for tc in range(1, 7)])
 def test_cuda_train_step_vs_oracle(B, rate, seed, tc):
     """tc = 7: the three conv-GEMMs of every block (forward, data gradient, weight gradient) on wgmma (split-fp16 x3,
     kernels_gemm_tc.cu), compared on the tie-free parameter set; tc = 0: fp32 CUDA-core kernels on the plain set.
-    B = 32 is BASELINE config 5's batch."""
+    B = 32 is BASELINE config 5's batch.  tc = 1..6 mix the two kernel sets: there the abs-max slots handed from the
+    forward to the gradients (train_bwd) are found empty or filled by the other set's GEMMs."""
     from dc_tts_b200.engine import Engine
     P = init_params(0, "perturbed")
     if tc:
@@ -311,10 +312,22 @@ def test_ssrn_relu_margins_explain_the_tie_case():
 def test_cuda_ssrn_train_step_vs_oracle(B, T, rate, seed):
     """The SSRN trainer (train.py num=2): transposed-conv blocks, C = 1024 highway blocks and the F = 1025 wide blocks.
     The first case is kept as a documented ReLU tie (see _RELU_TIE)."""
+    _ssrn_step_vs_oracle(B, T, rate, seed, 7)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("B,T,rate,seed", [(2, 12, 0.05, 9), (2, 14, 0.0, 7)])
+def test_cuda_ssrn_train_step_on_fp32_kernels_vs_oracle(B, T, rate, seed):
+    """The SSRN trainer with every GEMM on the float32 CUDA-core kernels (train_tc = 0), on green cases of the test above."""
+    _ssrn_step_vs_oracle(B, T, rate, seed, 0)
+
+
+def _ssrn_step_vs_oracle(B, T, rate, seed, tc):
     from dc_tts_b200.engine import Engine
     P = init_params(0, "perturbed")
     eng = Engine(0)
     eng.load_params(P)
+    eng.set_option("train_tc", tc)
     eng.train_init_ssrn(B, T, rate)
     mels = np.random.default_rng(3).uniform(0, 1, (B, T, hp.n_mels)).astype(np.float32)
     mags = np.random.default_rng(4).uniform(0, 1, (B, 4 * T, 1 + hp.n_fft // 2)).astype(np.float32)
