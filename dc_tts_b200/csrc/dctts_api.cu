@@ -168,7 +168,7 @@ struct dctts_handle_s {
 
     // kernel-variant switches (dctts_set_option); the defaults are the measured-best configuration
     struct {
-        int tc_occ2 = 1;          // two-stage ring on launches wider than the device
+        int tc_occ2 = 0;          // 1: two-stage ring on launches wider than the device
         int tc_mcast = 1;         // TMA multicast of the activation tile across the cluster
         int tc_resid_tma = 1;     // hc: residual in / planes out through TMA
         int tc_debug = 0;         // progress markers + in-kernel cycle stamps (synchronising)
@@ -767,9 +767,10 @@ void run_block_tc(Launch& lc, const LayerDev& l, int rate, bool causal, int act,
     a.bias = l.bias; a.g1 = l.g1; a.b1 = l.b1; a.g2 = (p.mode == 1) ? l.g2 : l.g1; a.b2 = (p.mode == 1) ? l.b2 : l.b1;
     a.mode = p.mode; a.act = act; a.C = l.cout; a.bn = p.bn; a.half = p.half; a.inv_scale = p.inv_scale; a.in_inv = in_inv;
     const int tiles = ((win.B + TB - 1) / TB) * tiles_t;
-    // Option tc_occ2 = 1 (default): launches wider than the device take a two-stage ring; 0 lets the ring grow to what
-    // shared memory holds (three stages for a 256-column hc block).  The kernel runs one CTA per SM either way, and on an
-    // H100 SXM (400 W limit) the two measured the same: SSRN at B = 32, T = 210 32.8 vs 32.7-32.8 ms per pass.
+    // Option tc_occ2 = 0 (default): the ring holds as many stages as shared memory allows (three for a 256-column hc block,
+    // four for a 256-column conv1d, six at 144 columns); 1 gives launches wider than the device a two-stage ring.  The kernel
+    // runs one CTA per SM either way.  With one k-block of MMAs in flight the deeper ring is faster: on an H100 SXM (400 W
+    // limit) SSRN at B = 32, T = 210 took 13.9 ms per pass against 18.9 ms with two stages.
     H* h = lc.h;
     const bool occ2 = h->opt.tc_occ2 != 0 && !win.jptr && TT == 128 && TB == 1 && tiles * p.ncta >= h->num_sms;
     const int bk = tc_bk();

@@ -12,9 +12,10 @@
 //           each activation plane -- the tap's time shift is just the box coordinate, and
 //           TMA's out-of-bounds zero fill IS the reference's zero padding -- plus the
 //           {BK x bn} box of each weight plane, swizzled, mbarrier pipelined.
-//   warpgroups 1, 2  wgmma (M=64 each, N=bn in chunks of <= 64, K=16):
-//           hi*Whi + hi*Wlo + lo*Whi per k-step into fp32 register accumulators, which
-//           then go to shared memory as one 128 x bn tile.
+//   warpgroups 1, 2  wgmma (M=64 each, N=bn: one instruction over the CTA's whole width, K=16):
+//           hi*Whi + hi*Wlo + lo*Whi per k-step into fp32 register accumulators, one k-block
+//           in flight while the next is issued; then the accumulators go to shared memory as
+//           one 128 x bn tile.
 //   warpgroup 1  epilogue: thread == row, so LN reductions are thread-local; one
 //           statistics sweep and one normalise+store sweep over the tile.
 #include "kernels_tc.cuh"
@@ -83,16 +84,18 @@ __device__ __forceinline__ void store_planes(const Planes& p, size_t row, int co
 // it is written only once every k-block has been multiplied, and every multicast box aimed at this CTA has landed by then
 // (each one completes on a full barrier that the consumers waited for).
 __host__ __device__ inline int tc_acc_ld(int bn) { return bn + 4; }                  // row pitch: float4 rows hit distinct banks
-__host__ __device__ inline int tc_ring_bytes(int stages, int stage_bytes, int bn, int sw) {
-    const int ring = stages * stage_bytes + 64 * sw;                                   // a 64-column wgmma past bn reads <= 48 rows more
+__host__ __device__ inline int tc_ring_bytes(int stages, int stage_bytes, int bn) {
+    const int ring = stages * stage_bytes;                                             // each wgmma reads exactly bn weight rows
     const int acc = TC_BM * tc_acc_ld(bn) * 4;
     return ((ring > acc ? ring : acc) + 1023) & ~1023;
 }
 __host__ __device__ inline int tc_resid_bytes(int resid_tma, int half) { return resid_tma ? 2 * (half / 64) * 16384 : 0; }
 
-// One 128-row tile per CTA, split over two consumer warpgroups (rows 0-63 / 64-127), each holding its 64 x bn accumulator in
-// registers (wgmma m64nNk16, N in chunks of <= 64 columns).
-template <int TC_BK>
+// One 128-row tile per CTA, split over two consumer warpgroups (rows 0-63 / 64-127), each holding its 64 x BN accumulator in
+// registers.  BN (accumulator columns per CTA) is a template parameter so that each product of a k-step is ONE wgmma
+// m64nBNk16: the A tile is read from shared memory once per product instead of once per 64 columns, and no run-time
+// width switch sits between the MMAs.
+template <int TC_BK, int BN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constant__ CUtensorMap mapA_lo,
                   const __grid_constant__ CUtensorMap mapW_hi, const __grid_constant__ CUtensorMap mapW_lo,
@@ -110,18 +113,19 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
     const int rank = (int)cluster_ctarank();                         // channel slice of this CTA
     const int ncta = (int)cluster_nctarank();
     const int nslices = ncta;
-    const int bn = a.bn, half = a.half;                              // accumulator columns per CTA / per LN half
+    constexpr int bn = BN;                                           // accumulator columns per CTA
+    const int half = a.half;                                         // columns per LN half
     constexpr int TC_A_PLANE = TC_BM * TC_BK * 2;                    // bytes of one activation plane tile
     constexpr int SW = TC_BK * 2;                                    // swizzle span = row bytes (128 or 64)
-    const int b_plane = bn * SW;                                     // bytes of one weight plane tile
+    constexpr int b_plane = bn * SW;                                 // bytes of one weight plane tile
     constexpr int A_BYTES = 2 * TC_A_PLANE;                          // hi+lo planes
-    const int stage_bytes = A_BYTES + 2 * b_plane;
+    constexpr int stage_bytes = A_BYTES + 2 * b_plane;
     const int stages = a.stages;
     const int nkb = a.ntaps * a.kb_per_tap;
     const int acc_ld = tc_acc_ld(bn);
 
     float* s_acc = reinterpret_cast<float*>(smem);
-    uint8_t* rs = smem + tc_ring_bytes(stages, stage_bytes, bn, SW);   // residual / output staging tile
+    uint8_t* rs = smem + tc_ring_bytes(stages, stage_bytes, bn);   // residual / output staging tile
     uint8_t* aux = rs + tc_resid_bytes(a.resid_tma, half);
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(aux);              // [stages]
     uint64_t* empty_bar = full_bar + TC_MAX_STAGES;                      // [stages]
@@ -215,11 +219,17 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
     } else if (wg >= 1) {
         // =========================== wgmma consumers ===========================
         const int mh = wg - 1;                                           // row half of the tile
-        float acc[4][32];
+        float acc[BN / 2];                                               // m64nBN fragment (tc_ptx.cuh)
 #pragma unroll
-        for (int j = 0; j < 4; ++j)
-#pragma unroll
-            for (int i = 0; i < 32; ++i) acc[j][i] = 0.f;
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        // stage s is drained: let the producer(s) refill it.  With the multicast A tile every CTA of the cluster waits for
+        // this release, and thread p of the warpgroup signals CTA p, so the cluster-scope arrives go out side by side
+        // instead of one after another on a single thread
+        auto release = [&](int s) {
+            const int t = threadIdx.x & 127;
+            if (mcast) { if (t < ncta) mbar_arrive_cluster(&empty_bar[s], (uint32_t)t); }
+            else if (t == 0) mbar_arrive(&empty_bar[s]);
+        };
         for (int kb = 0; kb < nkb; ++kb) {
             const int s = kb % stages;
             mbar_wait(&full_bar[s], (uint32_t)(kb / stages) & 1u);
@@ -230,39 +240,28 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
 #pragma unroll
             for (int k = 0; k < TC_BK / 16; ++k) {
                 const uint64_t adv = (uint64_t)(k * 32 >> 4);            // 16 fp16 = 32 B inside the swizzle atom
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    if (j * 64 < bn) {
-                        const uint64_t cb = (uint64_t)((j * 64 * SW) >> 4);
-                        wgmma_split3(acc[j], min(64, bn - j * 64), dA_hi + adv, dA_lo + adv, dB_hi + cb + adv, dB_lo + cb + adv,
-                                     (kb | k) != 0);
-                    }
-                }
+                wgmma_full<BN>(acc, dA_hi + adv, dB_hi + adv, (kb | k) != 0);
+                wgmma_full<BN>(acc, dA_hi + adv, dB_lo + adv, 1u);
+                wgmma_full<BN>(acc, dA_lo + adv, dB_hi + adv, 1u);
             }
             wg_commit();
-            wg_wait<0>();
-#pragma unroll
-            for (int j = 0; j < 4; ++j) wg_fence_regs(acc[j]);
-            if ((threadIdx.x & 127) == 0) {                                  // the stage is drained: release it
-                if (mcast) { for (int p = 0; p < ncta; ++p) mbar_arrive_cluster(&empty_bar[s], (uint32_t)p); }
-                else mbar_arrive(&empty_bar[s]);
-            }
+            // keep this k-block's MMAs in flight; the previous one is finished once at most one group is pending
+            wg_wait<1>();
+            if (kb > 0) release((kb - 1) % stages);
         }
+        wg_wait<0>();                                                    // the last k-block (its stage is never refilled)
+        wg_fence_regs(acc);
         if (threadIdx.x == 128) dbg_mark(a.dbg, 4, nkb);
         named_sync(1, 256);                                              // both halves done reading the ring
         {
             const int w4 = (threadIdx.x >> 5) & 3;
             const int r0 = mh * 64 + w4 * 16 + (lane >> 2);
 #pragma unroll
-            for (int j = 0; j < 4; ++j)
-#pragma unroll
-                for (int i8 = 0; i8 < 8; ++i8) {
-                    const int col = j * 64 + i8 * 8 + 2 * (lane & 3);
-                    if (col < bn) {
-                        *reinterpret_cast<float2*>(s_acc + (size_t)r0 * acc_ld + col) = make_float2(acc[j][i8 * 4], acc[j][i8 * 4 + 1]);
-                        *reinterpret_cast<float2*>(s_acc + (size_t)(r0 + 8) * acc_ld + col) = make_float2(acc[j][i8 * 4 + 2], acc[j][i8 * 4 + 3]);
-                    }
-                }
+            for (int q = 0; q < BN / 8; ++q) {
+                const int col = q * 8 + 2 * (lane & 3);
+                *reinterpret_cast<float2*>(s_acc + (size_t)r0 * acc_ld + col) = make_float2(acc[q * 4], acc[q * 4 + 1]);
+                *reinterpret_cast<float2*>(s_acc + (size_t)(r0 + 8) * acc_ld + col) = make_float2(acc[q * 4 + 2], acc[q * 4 + 3]);
+            }
         }
         named_sync(1, 256);                                              // accumulator tile complete in shared memory
     }
@@ -624,7 +623,7 @@ int tc_bk() {
 
 static size_t conv_ln_smem(int stages, int bn, int half, int resid_tma, int bk) {
     const int stage = 2 * TC_BM * bk * 2 + 2 * bn * bk * 2;
-    return (size_t)tc_ring_bytes(stages, stage, bn, 2 * bk) + tc_resid_bytes(resid_tma, half) + TC_AUX_BYTES + 1024;
+    return (size_t)tc_ring_bytes(stages, stage, bn) + tc_resid_bytes(resid_tma, half) + TC_AUX_BYTES + 1024;
 }
 
 int tc_stages_for(int bn, int bk, int resid_tma, int half) {      // bn = accumulator columns per CTA
@@ -633,22 +632,39 @@ int tc_stages_for(int bn, int bk, int resid_tma, int half) {      // bn = accumu
     return s;
 }
 
+// the kernel instantiation for (bk, bn): the accumulator widths of the networks' blocks -- 64 (Text2Mel's 256-channel
+// blocks), 80 (the mel output), 144 (the F = 1025 blocks over 8 CTAs), 256 (the 512- and 1024-channel blocks)
+typedef void (*ConvLnKernel)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
+                             const CUtensorMap, const CUtensorMap, const CUtensorMap, const TcArgs);
+template <int BK>
+static ConvLnKernel conv_ln_kernel_bn(int bn) {
+    switch (bn) {
+        case 64: return conv_ln_tc_kernel<BK, 64>;
+        case 80: return conv_ln_tc_kernel<BK, 80>;
+        case 144: return conv_ln_tc_kernel<BK, 144>;
+        case 256: return conv_ln_tc_kernel<BK, 256>;
+        default: throw std::runtime_error("conv_ln_tc: no kernel for " + std::to_string(bn) + " accumulator columns per CTA "
+                                          "(64, 80, 144, 256)");
+    }
+}
+
 void launch_conv_ln_tc(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& w_hi,
                        const CUtensorMap& w_lo, const CUtensorMap* io, const TcArgs& a, int ncta, int ctas_y, int bk,
                        cudaStream_t s) {
-    // the attributes are per device: cache them per device, not per process (a second Engine on another GPU
-    // of the same process must raise its own limits)
-    static bool attr_set_dev[64] = {};
+    if (ncta > 8) throw std::runtime_error("conv_ln_tc: unsupported tile (cluster <= 8)");
+    const ConvLnKernel kern = bk == 64 ? conv_ln_kernel_bn<64>(a.bn) : conv_ln_kernel_bn<32>(a.bn);
+    // the attributes are per device and per instantiation: cache them per device, not per process (a second Engine on
+    // another GPU of the same process must raise its own limits)
+    static bool attr_set_dev[64][8] = {};
     int dev = 0;
     cudaGetDevice(&dev);
-    bool& attr_set = attr_set_dev[dev & 63];
+    const int inst = (bk == 64 ? 4 : 0) + (a.bn == 64 ? 0 : a.bn == 80 ? 1 : a.bn == 144 ? 2 : 3);
+    bool& attr_set = attr_set_dev[dev & 63][inst];
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(conv_ln_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_MAX_SMEM);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_ln_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_MAX_SMEM);
+        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_MAX_SMEM);
         if (e != cudaSuccess) throw std::runtime_error(std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e));
         attr_set = true;
     }
-    if (a.bn > 256 || a.bn % 16 || ncta > 8) throw std::runtime_error("conv_ln_tc: unsupported tile (bn <= 256, multiple of 16; cluster <= 8)");
     const size_t smem = conv_ln_smem(a.stages, a.bn, a.half, a.resid_tma, bk);
     if (smem > (size_t)TC_MAX_SMEM) throw std::runtime_error("conv_ln_tc: shared memory budget exceeded");
     cudaLaunchConfig_t cfg{};
@@ -667,9 +683,7 @@ void launch_conv_ln_tc(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const C
     const CUtensorMap& x_lo = io ? io[1] : a_lo;
     const CUtensorMap& o_hi = io ? io[2] : a_hi;
     const CUtensorMap& o_lo = io ? io[3] : a_lo;
-    cudaError_t e;
-    if (bk == 64) e = cudaLaunchKernelEx(&cfg, conv_ln_tc_kernel<64>, a_hi, a_lo, w_hi, w_lo, x_hi, x_lo, o_hi, o_lo, a);
-    else          e = cudaLaunchKernelEx(&cfg, conv_ln_tc_kernel<32>, a_hi, a_lo, w_hi, w_lo, x_hi, x_lo, o_hi, o_lo, a);
+    const cudaError_t e = cudaLaunchKernelEx(&cfg, kern, a_hi, a_lo, w_hi, w_lo, x_hi, x_lo, o_hi, o_lo, a);
     if (e != cudaSuccess) throw std::runtime_error(std::string("conv_ln_tc launch: ") + cudaGetErrorString(e));
 }
 

@@ -31,7 +31,7 @@ struct TcArgs {
     int mode;                      // 0 conv1d (one LN), 1 hc (two LNs + gate + mix), 2 transposed conv (two LNs, two rows)
     int act;                       // mode 0: 0 none, 1 relu
     int C;                         // LN width (mode 0: cout; modes 1,2: cout of one half)
-    int bn;                        // accumulator columns per CTA (modes 1,2: both halves)
+    int bn;                        // accumulator columns per CTA (modes 1,2: both halves): 64, 80, 144 or 256
     int half;                      // columns per LN half per CTA (mode 0: == bn)
     float inv_scale;               // 1 / (power-of-two weight scale)
     const float* in_inv;           // [B] 1 / (power-of-two scale of utterance b's input planes), or null for unscaled

@@ -117,6 +117,34 @@ __device__ __forceinline__ void wgmma_f16(float (&d)[R], uint64_t da, uint64_t d
                      : DCTTS_WG_D8(0), DCTTS_WG_D8(8), DCTTS_WG_D8(16), DCTTS_WG_D8(24) : "l"(da), "l"(db), "r"(accumulate));
     }
 }
+// One m64nNk16 over the full accumulator width of a CTA: N = 64, 80, 144 or 256 (the widths the networks' blocks use),
+// d holds the N / 2 fp32 registers of the fragment above
+template <int N>
+__device__ __forceinline__ void wgmma_full(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
+    static_assert(N == 64 || N == 80 || N == 144 || N == 256, "wgmma_full: unsupported width");
+    if constexpr (N == 64) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31},"
+                     " %32, %33, p, 1, 1, 0, 0;\n\t}"
+                     : DCTTS_WG_D8(0), DCTTS_WG_D8(8), DCTTS_WG_D8(16), DCTTS_WG_D8(24) : "l"(da), "l"(db), "r"(accumulate));
+    } else if constexpr (N == 80) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %42, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n80k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39},"
+                     " %40, %41, p, 1, 1, 0, 0;\n\t}"
+                     : DCTTS_WG_D8(0), DCTTS_WG_D8(8), DCTTS_WG_D8(16), DCTTS_WG_D8(24), DCTTS_WG_D8(32) : "l"(da), "l"(db), "r"(accumulate));
+    } else if constexpr (N == 144) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n144k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71},"
+                     " %72, %73, p, 1, 1, 0, 0;\n\t}"
+                     : DCTTS_WG_D8(0), DCTTS_WG_D8(8), DCTTS_WG_D8(16), DCTTS_WG_D8(24), DCTTS_WG_D8(32), DCTTS_WG_D8(40), DCTTS_WG_D8(48), DCTTS_WG_D8(56), DCTTS_WG_D8(64) : "l"(da), "l"(db), "r"(accumulate));
+    } else if constexpr (N == 256) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127},"
+                     " %128, %129, p, 1, 1, 0, 0;\n\t}"
+                     : DCTTS_WG_D8(0), DCTTS_WG_D8(8), DCTTS_WG_D8(16), DCTTS_WG_D8(24), DCTTS_WG_D8(32), DCTTS_WG_D8(40), DCTTS_WG_D8(48), DCTTS_WG_D8(56), DCTTS_WG_D8(64), DCTTS_WG_D8(72), DCTTS_WG_D8(80), DCTTS_WG_D8(88), DCTTS_WG_D8(96), DCTTS_WG_D8(104), DCTTS_WG_D8(112), DCTTS_WG_D8(120) : "l"(da), "l"(db), "r"(accumulate));
+    }
+
+}
 #undef DCTTS_WG_D8
 
 // hi*Bhi + hi*Blo + lo*Bhi into one accumulator of `cols` (16, 32, 48 or 64) columns, chosen at run time
