@@ -907,7 +907,6 @@ void run_attention(Launch& lc, const float* Q, int ldq, const float* K, int ldk,
                    RowWin win, int N, const int* pma, float* R, float* align, long long* maxatt,
                    int* p_next, int* p_hist, Planes Rpl = Planes{}) {
     H* h = lc.h;
-    REQUIRE(N <= 192, "attention: N exceeds the kernel's key capacity (192)");
     REQUIRE(h->hp.d <= 256, "attention: d exceeds 256");
     AttnArgs a{};
     a.Q = Q; a.ldq = ldq; a.K = K; a.ldk = ldk; a.V = V; a.ldv = ldv;
@@ -920,12 +919,12 @@ void run_attention(Launch& lc, const float* Q, int ldq, const float* K, int ldk,
 
 // Full-sequence attention on the tensor cores (kernels_attn_tc.cu): dense or with the monotonic
 // window.  Q, K, V are fp32 device tensors; their split planes are built here.
-bool attention_tc_ok(H* h, int N) { return h->tensor_path == 1 && h->hp.d == 256 && N <= attn_tc_padded_keys(); }
+bool attention_tc_ok(H* h) { return h->tensor_path == 1 && h->hp.d == 256; }
 
 void run_attention_tc(Launch& lc, const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv, int B, int T,
                       int N, const int* pma, float* R, float* align, long long* maxatt, Planes Rpl) {
     H* h = lc.h;
-    const int d = h->hp.d, NP = attn_tc_padded_keys();
+    const int d = h->hp.d, NP = attn_tc_padded_keys(N);
     const size_t need[3] = {(size_t)B * T * d * sizeof(__half), (size_t)B * N * d * sizeof(__half), (size_t)B * d * NP * sizeof(__half)};
     for (int i = 0; i < 6; ++i)
         if (h->attpl[i].bytes < need[i / 2]) { CUDA_CHECK(cudaDeviceSynchronize()); h->attpl[i].ensure(need[i / 2]); }
@@ -1139,7 +1138,7 @@ void text2mel_forward(H* h, const int* L, const float* mels, const int* pma, int
         float* Q = h->ae_out.back().as<float>();
         run_chain_tc_planes(lc, h->audioenc, mp, 0, B, T, Q, nullptr, -1, in_inv);  // shift: train.py:51
         Planes Rpl; Rpl.hi = h->arpl[0].as<__half>(); Rpl.lo = h->arpl[1].as<__half>(); Rpl.ld = 2 * d;
-        if (attention_tc_ok(h, N))
+        if (attention_tc_ok(h))
             run_attention_tc(lc, Q, d, K, 2 * d, K + d, 2 * d, B, T, N, pma, h->rbuf.as<float>(), align, maxatt, Rpl);
         else
             run_attention(lc, Q, d, K, 2 * d, K + d, 2 * d, RowWin{B, T, T, nullptr}, N, pma, h->rbuf.as<float>(),
@@ -1521,7 +1520,7 @@ void train_forward_backward(H* h, const int* L, int N, const float* mels, int T,
     const float* Q = tr.layers[tr.last[1]].out;                // (B, T, d)
     // dense softmax attention (training: no window, networks.py:140-153): the wgmma kernel of the synthesis path when the
     // forward GEMMs are on the tensor cores (it does not touch the weights), else one warp per query row on CUDA cores
-    if ((h->opt.train_tc & 1) && d == 256 && N <= attn_tc_padded_keys())
+    if ((h->opt.train_tc & 1) && d == 256)
         run_attention_tc(lc, Q, d, KV, 2 * d, KV + d, 2 * d, B, T, N, nullptr, tr.R.as<float>(), tr.align.as<float>(), nullptr, Planes{});
     else
         run_attention(lc, Q, d, KV, 2 * d, KV + d, 2 * d, RowWin{B, T, T, nullptr}, N, nullptr, tr.R.as<float>(), tr.align.as<float>(),
@@ -1702,7 +1701,7 @@ int dctts_create(const dctts_hparams* hp, int device, dctts_handle* out) {
         cudaDeviceProp prop;
         CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
         if (prop.major != 9 || prop.minor != 0) throw std::runtime_error("dctts_create: this library is built for sm_90a (H100) only");
-        if (hp->d > 256 || hp->d % 8 || hp->e % 4 || hp->max_N > 192 || hp->r != 4)
+        if (hp->d > 256 || hp->d % 8 || hp->e % 4 || hp->max_N < 1 || hp->r != 4)
             throw std::runtime_error("dctts_create: unsupported hyper-parameters");
         std::unique_ptr<dctts_handle_s> h(new dctts_handle_s());
         h->hp = *hp; h->device = device; h->F = 1 + hp->n_fft / 2; h->num_sms = prop.multiProcessorCount;
@@ -1829,7 +1828,7 @@ int dctts_attention(dctts_handle h, const float* Q, const float* K, const float*
         REQUIRE(!monotonic || pma, "dctts_attention: monotonic attention needs prev_max_attentions");
         Launch lc{h, S(h, stream)};
         const int d = h->hp.d;
-        if (attention_tc_ok(h, N))
+        if (attention_tc_ok(h))
             run_attention_tc(lc, Q, d, K, d, V, d, B, T, N, monotonic ? pma : nullptr, R, alignments,
                              reinterpret_cast<long long*>(max_attentions), Planes{});
         else

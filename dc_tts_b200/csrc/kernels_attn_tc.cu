@@ -1,17 +1,26 @@
 // kernels_attn_tc.cu -- the dot-product attention (reference networks.py:126-155) as ONE
 // wgmma kernel: S = Q K^T / sqrt(d) -> window mask -> softmax -> argmax -> A V -> [A V ; Q],
-// alignments written transposed.  One CTA per (128 query rows, utterance): a TMA producer
-// warp and two consumer warpgroups of 64 query rows each.
+// alignments written transposed.  One CTA per (64 query rows, utterance): one consumer
+// warpgroup, which holds C (128 registers) beside one S block, and a TMA producer warp.
+// Any key count N: the keys are visited in blocks of 64 (nb = ceil(N / 64), the last one
+// zero-filled by TMA past N), and S is never held for more than one block:
 //
-//   GEMM 1  S[128 x 192]  = Q[128 x 256] . K^T        (keys padded 180 -> 192 by TMA zero fill)
-//   softmax on the register accumulators, four threads per query row (quad shuffles);
-//           the probabilities are written back to shared memory as split-fp16 planes in the
-//           128B-swizzled K-major layout the tensor core reads (no global round trip)
-//   GEMM 2  C[128 x 256]  = P[128 x 192] . V          (V pre-transposed to [d][keys] planes)
+//   pass 1  per key block: S[64 x 64] = Q[64 x 256] . K_blk^T     -> row max
+//   pass 2  per key block: S again                                 -> per-thread sum of exp(s - max)
+//   pass 3  per key block: S again -> probabilities, alignments, argmax, P block in shared memory
+//           (split-fp16 planes, 128B-swizzled K-major: GEMM 2's A operand) -> C[64 x 256] += P_blk . V_blk
+//
+// Each S accumulator sees the wgmma sequence d-slab, k-step, hi*hi, hi*lo, lo*hi in all three
+// passes, each C accumulator key block, k-step and the same three products, and the sums and
+// the argmax scan visit the keys in (block, i, e) order: the same arithmetic as holding all of S
+// in registers, which the three 64-key blocks of N <= 192 would allow.  With the monotonic window only the blocks that hold a
+// live key are computed; the others are exactly 0 in every output.
 // Both GEMMs use the split-fp16 three-pass scheme (hi*hi + hi*lo + lo*hi, fp32 accumulate):
 // the argmax of these probabilities is fed back into the next decode step, so the scores
-// need fp32-grade accuracy.  Shared memory (160 KB) is reused: GEMM 1's two 80 KB pipeline
-// stages become P (96 KB) and one 64 KB V^T stage.
+// need fp32-grade accuracy.
+// Shared memory does not depend on N (176 KB): Q stays resident (4 d-slabs x hi/lo, 64 KB),
+// the P block (16 KB), and a 6-stage ring of 16 KB stages carrying K slabs (64 keys x 64
+// channels) and, in pass 3, V^T chunks (64 channels x 64 keys), both as hi | lo.
 #include "kernels_tc.cuh"
 #include "tc_ptx.cuh"
 
@@ -23,15 +32,28 @@ namespace dctts {
 
 using namespace ptx;
 
-constexpr int AT_THREADS = 384;
-constexpr int AT_NP = 192;                        // padded key count (3 x 64)
+constexpr int AT_THREADS = 160;                   // warpgroup 0: consumer; warp 4: TMA producer
 constexpr int AT_D = 256;                         // head width (hp.d)
-constexpr int AT_Q_PLANE = 128 * 64 * 2;          // 16 KB: 128 query rows x 64 channels fp16
-constexpr int AT_K_PLANE = AT_NP * 64 * 2;        // 24 KB
-constexpr int AT_STAGE1 = 2 * AT_Q_PLANE + 2 * AT_K_PLANE;   // 80 KB
-constexpr int AT_P_PLANE = 3 * AT_Q_PLANE;        // 48 KB: 3 key blocks of [128 x 64]
-constexpr int AT_VT_PLANE = AT_D * 64 * 2;        // 32 KB: 256 channels x 64 keys
-constexpr int AT_SMEM_MAIN = 2 * AT_STAGE1;       // 160 KB
+constexpr int AT_ROWS = 64;                       // query rows per CTA
+constexpr int AT_Q_PLANE = AT_ROWS * 64 * 2;      // 8 KB: 64 query rows x 64 channels fp16
+constexpr int AT_Q_BYTES = 2 * (AT_D / 64) * AT_Q_PLANE;   // 64 KB: every d-slab, hi and lo
+constexpr int AT_P_PLANE = AT_ROWS * 64 * 2;      // 8 KB: 64 query rows x 64 keys fp16
+constexpr int AT_HALF = 64 * 64 * 2;              // 8 KB: one plane of a ring stage
+constexpr int AT_STAGE = 2 * AT_HALF;             // 16 KB: hi | lo
+constexpr int AT_STAGES = 6;
+constexpr int AT_SMEM_MAIN = AT_Q_BYTES + 2 * AT_P_PLANE + AT_STAGES * AT_STAGE;   // 176 KB
+
+// the key blocks holding a live key of [n_lo, n_hi): [jb0, jb1)
+__device__ __forceinline__ void attn_live_blocks(const AttnTcArgs& a, int b, int& n_lo, int& n_hi, int& jb0, int& jb1) {
+    n_lo = 0; n_hi = a.N;
+    if (a.pma) {                                   // monotonic window [p, p + win) (networks.py:141-147)
+        const int p = __ldg(a.pma + b);
+        n_lo = min(max(p, 0), a.N - 1);
+        n_hi = min(n_lo + a.win_size, a.N);
+    }
+    jb0 = n_lo >> 6;
+    jb1 = n_hi > n_lo ? ((n_hi - 1) >> 6) + 1 : jb0;
+}
 
 __global__ void __launch_bounds__(AT_THREADS, 1)
 attention_tc_kernel(const __grid_constant__ CUtensorMap mapQ_hi, const __grid_constant__ CUtensorMap mapQ_lo,
@@ -40,190 +62,222 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap mapQ_hi, const __grid_co
                     const AttnTcArgs a) {
     extern __shared__ uint8_t at_smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(at_smem_raw) + 1023) & ~uintptr_t(1023));
+    uint8_t* q_st = smem;                                  // [d-slab][hi, lo][64 rows][128 B]
+    uint8_t* p_hi = smem + AT_Q_BYTES;                     // [64 rows][128 B]
+    uint8_t* p_lo = p_hi + AT_P_PLANE;
+    uint8_t* ring = p_lo + AT_P_PLANE;                     // [stage][hi, lo][64 rows][128 B]
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + AT_SMEM_MAIN);
-    uint64_t* full_bar = bars;            // [2]
-    uint64_t* empty_bar = bars + 2;       // [2]
-    uint64_t* s_full = bars + 4;          // GEMM 1 done in both consumer warpgroups: its stages are free
-    uint64_t* vt_full = bars + 6;
-    uint64_t* vt_empty = bars + 7;
+    uint64_t* full_bar = bars;                     // [AT_STAGES]
+    uint64_t* empty_bar = bars + AT_STAGES;        // [AT_STAGES]
+    uint64_t* q_full = bars + 2 * AT_STAGES;
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
-    const int b = blockIdx.y, t0 = blockIdx.x * 128;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int b = blockIdx.y, t0 = blockIdx.x * AT_ROWS;
     const int T = a.T, N = a.N;
+    const int nb = (N + 63) >> 6;
+    int n_lo, n_hi, jb0, jb1;
+    attn_live_blocks(a, b, n_lo, n_hi, jb0, jb1);
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 4 && lane == 0) {
         prefetch_tmap(&mapQ_hi); prefetch_tmap(&mapQ_lo); prefetch_tmap(&mapK_hi); prefetch_tmap(&mapK_lo);
         prefetch_tmap(&mapV_hi); prefetch_tmap(&mapV_lo);
-        for (int s = 0; s < 2; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
-        mbar_init(s_full, 2); mbar_init(vt_full, 1); mbar_init(vt_empty, 2);
+        for (int s = 0; s < AT_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
+        mbar_init(q_full, 1);
         fence_mbar_init();
     }
     __syncthreads();
 
-    uint8_t* p_hi = smem;                          // [3][128 rows][128 B]
-    uint8_t* p_lo = smem + AT_P_PLANE;
-    uint8_t* vt_st = smem + 2 * AT_P_PLANE;        // V^T hi (32 KB) | lo (32 KB)
-
-    if (warp == 0) {
-        // =========================== TMA producer ===========================
+    if (warp == 4) {
+        // =========================== TMA producer: Q once, then the ring in the consumer's order ===========================
         if (lane == 0) {
+            mbar_expect_tx(q_full, AT_Q_BYTES);
             for (int kb = 0; kb < AT_D / 64; ++kb) {
-                const int s = kb & 1;
-                mbar_wait(&empty_bar[s], ((uint32_t)(kb >> 1) & 1u) ^ 1u);
-                mbar_expect_tx(&full_bar[s], AT_STAGE1);
-                uint8_t* st = smem + (size_t)s * AT_STAGE1;
-                tma_load_3d(&mapQ_hi, &full_bar[s], st, kb * 64, t0, b);
-                tma_load_3d(&mapQ_lo, &full_bar[s], st + AT_Q_PLANE, kb * 64, t0, b);
-                tma_load_3d(&mapK_hi, &full_bar[s], st + 2 * AT_Q_PLANE, kb * 64, 0, b);
-                tma_load_3d(&mapK_lo, &full_bar[s], st + 2 * AT_Q_PLANE + AT_K_PLANE, kb * 64, 0, b);
+                tma_load_3d(&mapQ_hi, q_full, q_st + (2 * kb) * AT_Q_PLANE, kb * 64, t0, b);
+                tma_load_3d(&mapQ_lo, q_full, q_st + (2 * kb + 1) * AT_Q_PLANE, kb * 64, t0, b);
             }
-            mbar_wait(s_full, 0);                  // GEMM 1 has consumed its stages: the memory is free
-            for (int kb = 0; kb < AT_NP / 64; ++kb) {
-                mbar_wait(vt_empty, ((uint32_t)kb & 1u) ^ 1u);
-                mbar_expect_tx(vt_full, 2 * AT_VT_PLANE);
-                tma_load_3d(&mapV_hi, vt_full, vt_st, kb * 64, 0, b);
-                tma_load_3d(&mapV_lo, vt_full, vt_st + AT_VT_PLANE, kb * 64, 0, b);
-            }
+            uint32_t it = 0;
+            auto next_stage = [&](uint32_t bytes) {
+                const int s = (int)(it % AT_STAGES);
+                mbar_wait(&empty_bar[s], ((it / AT_STAGES) & 1u) ^ 1u);
+                mbar_expect_tx(&full_bar[s], bytes);
+                ++it;
+                return s;
+            };
+            for (int pass = 0; pass < 3; ++pass)
+                for (int jb = jb0; jb < jb1; ++jb) {
+                    for (int kb = 0; kb < AT_D / 64; ++kb) {           // K slab: keys jb*64.., channels kb*64..
+                        const int s = next_stage(AT_STAGE);
+                        uint8_t* st = ring + (size_t)s * AT_STAGE;
+                        tma_load_3d(&mapK_hi, &full_bar[s], st, kb * 64, jb * 64, b);
+                        tma_load_3d(&mapK_lo, &full_bar[s], st + AT_HALF, kb * 64, jb * 64, b);
+                    }
+                    if (pass == 2)
+                        for (int j = 0; j < AT_D / 64; ++j) {          // V^T chunk: channels j*64.., keys jb*64..
+                            const int s = next_stage(AT_STAGE);
+                            uint8_t* st = ring + (size_t)s * AT_STAGE;
+                            tma_load_3d(&mapV_hi, &full_bar[s], st, jb * 64, j * 64, b);
+                            tma_load_3d(&mapV_lo, &full_bar[s], st + AT_HALF, jb * 64, j * 64, b);
+                        }
+                }
         }
         __syncwarp();
         return;
     }
-    if (wg == 0) return;                           // warps 1-3: no role
-    // =========================== consumers: query rows 64 * mh .. +64 of the tile ===========================
-    const int mh = wg - 1;
-    const bool leader = (threadIdx.x & 127) == 0;
-    const int rq = mh * 64 + (warp & 3) * 16 + (lane >> 2);        // fragment rows rq, rq + 8; columns 8 i + 2 (lane & 3) + {0, 1}
-    // ---- GEMM 1: S = Q K^T, 64 x 192 per warpgroup (three 64-key chunks) ----
-    float sacc[3][32];
+    // =========================== consumer warpgroup ===========================
+    const bool leader = threadIdx.x == 0;
+    const int rq = warp * 16 + (lane >> 2);       // fragment rows rq, rq + 8; columns 8 i + 2 (lane & 3) + {0, 1}
+    uint32_t it = 0;                               // ring position, in step with the producer
+    mbar_wait(q_full, 0);
+
+    // S for the ring's next key block, 64 x 64: one ring stage per d-slab, the previous slab's MMAs still in flight
+    auto gemm_s = [&](float (&sacc)[32]) {
+        for (int kb = 0; kb < AT_D / 64; ++kb) {
+            const int s = (int)(it % AT_STAGES);
+            mbar_wait(&full_bar[s], (it / AT_STAGES) & 1u);
+            const uint32_t st = smem_u32(ring + (size_t)s * AT_STAGE);
+            const uint64_t dQ_hi = gmma_desc_kmajor<128>(smem_u32(q_st + (2 * kb) * AT_Q_PLANE));
+            const uint64_t dQ_lo = gmma_desc_kmajor<128>(smem_u32(q_st + (2 * kb + 1) * AT_Q_PLANE));
+            const uint64_t dK_hi = gmma_desc_kmajor<128>(st), dK_lo = gmma_desc_kmajor<128>(st + AT_HALF);
+            wg_fence();
 #pragma unroll
-    for (int j = 0; j < 3; ++j)
-#pragma unroll
-        for (int i = 0; i < 32; ++i) sacc[j][i] = 0.f;
-    for (int kb = 0; kb < AT_D / 64; ++kb) {
-        const int s = kb & 1;
-        mbar_wait(&full_bar[s], (uint32_t)(kb >> 1) & 1u);
-        const uint32_t st = smem_u32(smem + (size_t)s * AT_STAGE1);
-        const uint64_t dQ_hi = gmma_desc_kmajor<128>(st + mh * 64 * 128), dQ_lo = gmma_desc_kmajor<128>(st + AT_Q_PLANE + mh * 64 * 128);
-        wg_fence();
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const uint64_t adv = (uint64_t)(k * 2);
-#pragma unroll
-            for (int j = 0; j < 3; ++j) {
-                const uint64_t dK_hi = gmma_desc_kmajor<128>(st + 2 * AT_Q_PLANE + j * 64 * 128);
-                const uint64_t dK_lo = gmma_desc_kmajor<128>(st + 2 * AT_Q_PLANE + AT_K_PLANE + j * 64 * 128);
-                wgmma_f16<4>(sacc[j], dQ_hi + adv, dK_hi + adv, (kb | k) != 0);
-                wgmma_f16<4>(sacc[j], dQ_hi + adv, dK_lo + adv, 1u);
-                wgmma_f16<4>(sacc[j], dQ_lo + adv, dK_hi + adv, 1u);
+            for (int k = 0; k < 4; ++k) {
+                const uint64_t adv = (uint64_t)(k * 2);
+                wgmma_f16<4>(sacc, dQ_hi + adv, dK_hi + adv, (kb | k) != 0);
+                wgmma_f16<4>(sacc, dQ_hi + adv, dK_lo + adv, 1u);
+                wgmma_f16<4>(sacc, dQ_lo + adv, dK_hi + adv, 1u);
             }
+            wg_commit();
+            if (kb > 0) {
+                wg_wait<1>();
+                if (leader) mbar_arrive(&empty_bar[(it - 1) % AT_STAGES]);
+            }
+            ++it;
         }
-        wg_commit();
         wg_wait<0>();
-#pragma unroll
-        for (int j = 0; j < 3; ++j) wg_fence_regs(sacc[j]);
-        if (leader) mbar_arrive(&empty_bar[s]);
-    }
-    if (leader) mbar_arrive(s_full);
-    named_sync(1, 256);                            // both warpgroups are done with GEMM 1's stages: P may overwrite them
+        wg_fence_regs(sacc);
+        if (leader) mbar_arrive(&empty_bar[(it - 1) % AT_STAGES]);
+    };
 
-    // ---- softmax over the live keys, four threads per query row (quad shuffles) ----
-    int n_lo = 0, n_hi = N;
-    if (a.pma) {                                   // monotonic window [p, p + win) (networks.py:141-147)
-        const int p = __ldg(a.pma + b);
-        n_lo = min(max(p, 0), N - 1);
-        n_hi = min(n_lo + a.win_size, N);
-    }
+    float sacc[32];
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {                  // the thread's two rows
-        const int r = rq + 8 * h, t = t0 + r;
-        const bool row_ok = t < T;
-        float mx = -INFINITY;
+    for (int i = 0; i < 32; ++i) sacc[i] = 0.f;
+    // ---- pass 1: row max over the live keys (four threads per query row, quad shuffles) ----
+    float mx[2] = {-INFINITY, -INFINITY};
+    for (int jb = jb0; jb < jb1; ++jb) {
+        gemm_s(sacc);
 #pragma unroll
-        for (int j = 0; j < 3; ++j)
+        for (int h = 0; h < 2; ++h)
 #pragma unroll
             for (int i = 0; i < 8; ++i)
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
-                    const int n = j * 64 + i * 8 + 2 * (lane & 3) + e;
-                    if (n >= n_lo && n < n_hi) mx = fmaxf(mx, sacc[j][i * 4 + 2 * h + e] * a.scale);
+                    const int n = jb * 64 + i * 8 + 2 * (lane & 3) + e;
+                    if (n >= n_lo && n < n_hi) mx[h] = fmaxf(mx[h], sacc[i * 4 + 2 * h + e] * a.scale);
                 }
-        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-        float sum = 0.f;
+    }
 #pragma unroll
-        for (int j = 0; j < 3; ++j)
+    for (int h = 0; h < 2; ++h) {
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+    }
+    // ---- pass 2: the softmax denominators ----
+    float sum[2] = {0.f, 0.f};
+    for (int jb = jb0; jb < jb1; ++jb) {
+        gemm_s(sacc);
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
 #pragma unroll
             for (int i = 0; i < 8; ++i)
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
-                    const int n = j * 64 + i * 8 + 2 * (lane & 3) + e;
-                    if (n >= n_lo && n < n_hi) sum += expf(sacc[j][i * 4 + 2 * h + e] * a.scale - mx);
+                    const int n = jb * 64 + i * 8 + 2 * (lane & 3) + e;
+                    if (n >= n_lo && n < n_hi) sum[h] += expf(sacc[i * 4 + 2 * h + e] * a.scale - mx[h]);
                 }
-        sum += __shfl_xor_sync(0xffffffffu, sum, 1);
-        sum += __shfl_xor_sync(0xffffffffu, sum, 2);
-        // probabilities -> split planes in shared memory (128B-swizzled K-major, GEMM 2's A operand), alignments, argmax
-        float best = -1.f; int besti = 0;
-        float* al = (a.align && row_ok) ? a.align + (size_t)b * N * T + t : nullptr;
-#pragma unroll
-        for (int j = 0; j < 3; ++j)
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                float p2[2];
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    const int n = j * 64 + i * 8 + 2 * (lane & 3) + e;
-                    float p = 0.f;                 // masked keys are exactly 0 in the reference (exp underflow)
-                    if (n >= n_lo && n < n_hi) p = expf(sacc[j][i * 4 + 2 * h + e] * a.scale - mx) / sum;
-                    if (p > best) { best = p; besti = n; }
-                    if (al && n < N) al[(size_t)n * T] = p;
-                    p2[e] = p;
-                }
-                const __half h0 = __float2half_rn(p2[0]), h1 = __float2half_rn(p2[1]);
-                const __half l0 = __float2half_rn(p2[0] - __half2float(h0)), l1 = __float2half_rn(p2[1] - __half2float(h1));
-                const int off = j * AT_Q_PLANE + r * 128 + ((i ^ (r & 7)) << 4) + 4 * (lane & 3);
-                *reinterpret_cast<__half2*>(p_hi + off) = __halves2half2(h0, h1);
-                *reinterpret_cast<__half2*>(p_lo + off) = __halves2half2(l0, l1);
-            }
-        // argmax over the quad: the first key of the largest probability, as a sequential scan finds it
-#pragma unroll
-        for (int o = 1; o <= 2; o <<= 1) {
-            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-            const int oi = __shfl_xor_sync(0xffffffffu, besti, o);
-            if (ob > best || (ob == best && oi < besti)) { best = ob; besti = oi; }
-        }
-        if (row_ok && a.maxatt && (lane & 3) == 0) a.maxatt[(size_t)b * T + t] = (long long)besti;
     }
-    fence_proxy_async_smem();                      // generic-proxy stores -> visible to the tensor core
-    named_sync(1, 256);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], 1);
+        sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], 2);
+    }
 
-    // ---- GEMM 2: context = P V, 64 x 256 per warpgroup (four 64-channel chunks) ----
+    // ---- pass 3: probabilities -> alignments, argmax, P block; context = P V, 64 x 256 ----
     float cacc[4][32];
 #pragma unroll
     for (int j = 0; j < 4; ++j)
 #pragma unroll
         for (int i = 0; i < 32; ++i) cacc[j][i] = 0.f;
-    for (int kb = 0; kb < AT_NP / 64; ++kb) {
-        mbar_wait(vt_full, (uint32_t)kb & 1u);
-        const uint64_t dP_hi = gmma_desc_kmajor<128>(smem_u32(p_hi + kb * AT_Q_PLANE + mh * 64 * 128));
-        const uint64_t dP_lo = gmma_desc_kmajor<128>(smem_u32(p_lo + kb * AT_Q_PLANE + mh * 64 * 128));
-        wg_fence();
+    float best[2] = {-1.f, -1.f};
+    int besti[2] = {0, 0};
+    const uint64_t dP_hi = gmma_desc_kmajor<128>(smem_u32(p_hi));
+    const uint64_t dP_lo = gmma_desc_kmajor<128>(smem_u32(p_lo));
+    for (int jb = 0; jb < nb; ++jb) {
+        const bool live = jb >= jb0 && jb < jb1;
+        if (live) gemm_s(sacc);
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const uint64_t adv = (uint64_t)(k * 2);
+        for (int h = 0; h < 2; ++h) {              // the thread's two rows
+            const int r = rq + 8 * h, t = t0 + r;
+            float* al = (a.align && t < T) ? a.align + (size_t)b * N * T + t : nullptr;
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const uint64_t dV_hi = gmma_desc_kmajor<128>(smem_u32(vt_st + j * 64 * 128));
-                const uint64_t dV_lo = gmma_desc_kmajor<128>(smem_u32(vt_st + AT_VT_PLANE + j * 64 * 128));
-                wgmma_f16<4>(cacc[j], dP_hi + adv, dV_hi + adv, (kb | k) != 0);
+            for (int i = 0; i < 8; ++i) {
+                float p2[2];
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int n = jb * 64 + i * 8 + 2 * (lane & 3) + e;
+                    float p = 0.f;                 // masked keys are exactly 0 in the reference (exp underflow)
+                    if (live && n >= n_lo && n < n_hi) p = expf(sacc[i * 4 + 2 * h + e] * a.scale - mx[h]) / sum[h];
+                    if (p > best[h]) { best[h] = p; besti[h] = n; }
+                    if (al && n < N) al[(size_t)n * T] = p;
+                    p2[e] = p;
+                }
+                if (live) {
+                    const __half h0 = __float2half_rn(p2[0]), h1 = __float2half_rn(p2[1]);
+                    const __half l0 = __float2half_rn(p2[0] - __half2float(h0)), l1 = __float2half_rn(p2[1] - __half2float(h1));
+                    const int off = r * 128 + ((i ^ (r & 7)) << 4) + 4 * (lane & 3);
+                    *reinterpret_cast<__half2*>(p_hi + off) = __halves2half2(h0, h1);
+                    *reinterpret_cast<__half2*>(p_lo + off) = __halves2half2(l0, l1);
+                }
+            }
+        }
+        if (!live) continue;
+        fence_proxy_async_smem();                  // generic-proxy stores -> visible to the tensor core
+        named_sync(1, 128);
+        for (int j = 0; j < 4; ++j) {              // one V^T chunk (64 channels) per ring stage
+            const int s = (int)(it % AT_STAGES);
+            mbar_wait(&full_bar[s], (it / AT_STAGES) & 1u);
+            const uint32_t st = smem_u32(ring + (size_t)s * AT_STAGE);
+            const uint64_t dV_hi = gmma_desc_kmajor<128>(st), dV_lo = gmma_desc_kmajor<128>(st + AT_HALF);
+            wg_fence();
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const uint64_t adv = (uint64_t)(k * 2);
+                wgmma_f16<4>(cacc[j], dP_hi + adv, dV_hi + adv, (jb != jb0 || k != 0) ? 1u : 0u);
                 wgmma_f16<4>(cacc[j], dP_hi + adv, dV_lo + adv, 1u);
                 wgmma_f16<4>(cacc[j], dP_lo + adv, dV_hi + adv, 1u);
             }
+            wg_commit();
+            if (j > 0) {
+                wg_wait<1>();
+                if (leader) mbar_arrive(&empty_bar[(it - 1) % AT_STAGES]);
+            }
+            ++it;
         }
-        wg_commit();
         wg_wait<0>();
 #pragma unroll
         for (int j = 0; j < 4; ++j) wg_fence_regs(cacc[j]);
-        if (leader) mbar_arrive(vt_empty);
+        if (leader) mbar_arrive(&empty_bar[(it - 1) % AT_STAGES]);
+        named_sync(1, 128);                        // the P block is read: the next block may overwrite it
+    }
+    // argmax over the quad: the first key of the largest probability, as a sequential scan finds it
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int o = 1; o <= 2; o <<= 1) {
+            const float ob = __shfl_xor_sync(0xffffffffu, best[h], o);
+            const int oi = __shfl_xor_sync(0xffffffffu, besti[h], o);
+            if (ob > best[h] || (ob == best[h] && oi < besti[h])) { best[h] = ob; besti[h] = oi; }
+        }
+        const int t = t0 + rq + 8 * h;
+        if (t < T && a.maxatt && (lane & 3) == 0) a.maxatt[(size_t)b * T + t] = (long long)besti[h];
     }
 
     // ---- R = [context ; Q] straight from the fragments ----
@@ -255,14 +309,16 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap mapQ_hi, const __grid_co
     }
 }
 
-// K (B,N,d) and V (B,N,d) fp32 (leading dimension ld) -> K planes (B,N,d) and V^T planes (B,d,192)
+// K (B,N,d) and V (B,N,d) fp32 (leading dimension ld) -> K planes (B,N,d) and V^T planes (B,d,NP), NP = vtp.ld >= N keys
+// (attn_tc_padded_keys), keys >= N written as zeros
 __global__ void attn_kv_planes_kernel(const float* __restrict__ K, int ldk, const float* __restrict__ V, int ldv,
                                       Planes kp, Planes vtp, int B, int N, int d) {
-    const long long total = (long long)B * AT_NP * d;
+    const int NP = vtp.ld;
+    const long long total = (long long)B * NP * d;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const int c = (int)(i % d);
-        const int n = (int)((i / d) % AT_NP);
-        const int b = (int)(i / ((long long)d * AT_NP));
+        const int n = (int)((i / d) % NP);
+        const int b = (int)(i / ((long long)d * NP));
         float kv = 0.f, vv = 0.f;
         if (n < N) { kv = K[((size_t)b * N + n) * ldk + c]; vv = V[((size_t)b * N + n) * ldv + c]; }
         if (n < N) {
@@ -278,15 +334,17 @@ __global__ void attn_kv_planes_kernel(const float* __restrict__ K, int ldk, cons
 
 void launch_attn_kv_planes(const float* K, int ldk, const float* V, int ldv, Planes kp, Planes vtp, int B, int N, int d,
                            cudaStream_t s) {
-    const long long total = (long long)B * AT_NP * d;
+    if (vtp.ld < attn_tc_padded_keys(N)) throw std::runtime_error("attn_kv_planes: V^T planes narrower than the padded key count");
+    const long long total = (long long)B * vtp.ld * d;
     const int grid = (int)std::min<long long>((total + 255) / 256, 4096);
     attn_kv_planes_kernel<<<grid, 256, 0, s>>>(K, ldk, V, ldv, kp, vtp, B, N, d);
 }
 
-int attn_tc_padded_keys() { return AT_NP; }
+int attn_tc_padded_keys(int N) { return (N + 63) / 64 * 64; }
 
 void launch_attention_tc(const Planes& Q, const Planes& K, const Planes& Vt, const AttnTcArgs& a, int B, cudaStream_t s) {
-    if (a.d != AT_D || a.N > AT_NP) throw std::runtime_error("attention_tc: unsupported d / N");
+    if (a.d != AT_D || a.N < 1) throw std::runtime_error("attention_tc: unsupported d / N");
+    if (Vt.ld < attn_tc_padded_keys(a.N)) throw std::runtime_error("attention_tc: V^T planes narrower than the padded key count");
     static bool attr_set_dev[64] = {};      // per device (the attribute is per device, not per process)
     int dev = 0;
     cudaGetDevice(&dev);
@@ -298,13 +356,13 @@ void launch_attention_tc(const Planes& Q, const Planes& K, const Planes& Vt, con
         attr_set = true;
     }
     CUtensorMap mq_h, mq_l, mk_h, mk_l, mv_h, mv_l;
-    tc_make_act_map(&mq_h, Q.hi, a.d, Q.ld, a.T, B, 128, 1, 64);
-    tc_make_act_map(&mq_l, Q.lo, a.d, Q.ld, a.T, B, 128, 1, 64);
-    tc_make_act_map(&mk_h, K.hi, a.d, K.ld, a.N, B, AT_NP, 1, 64);     // rows N..191 out of bounds -> zeros
-    tc_make_act_map(&mk_l, K.lo, a.d, K.ld, a.N, B, AT_NP, 1, 64);
-    tc_make_act_map(&mv_h, Vt.hi, AT_NP, Vt.ld, a.d, B, AT_D, 1, 64);  // (keys, channels, batch), box {64 keys, 256 channels}
-    tc_make_act_map(&mv_l, Vt.lo, AT_NP, Vt.ld, a.d, B, AT_D, 1, 64);
-    dim3 grid((a.T + 127) / 128, B);
+    tc_make_act_map(&mq_h, Q.hi, a.d, Q.ld, a.T, B, AT_ROWS, 1, 64);   // rows >= T read zeros
+    tc_make_act_map(&mq_l, Q.lo, a.d, Q.ld, a.T, B, AT_ROWS, 1, 64);
+    tc_make_act_map(&mk_h, K.hi, a.d, K.ld, a.N, B, 64, 1, 64);        // {64 channels, 64 keys}; keys >= N read zeros
+    tc_make_act_map(&mk_l, K.lo, a.d, K.ld, a.N, B, 64, 1, 64);
+    tc_make_act_map(&mv_h, Vt.hi, Vt.ld, Vt.ld, a.d, B, 64, 1, 64);    // (keys, channels, batch), box {64 keys, 64 channels}
+    tc_make_act_map(&mv_l, Vt.lo, Vt.ld, Vt.ld, a.d, B, 64, 1, 64);
+    dim3 grid((a.T + AT_ROWS - 1) / AT_ROWS, B);
     attention_tc_kernel<<<grid, AT_THREADS, smem, s>>>(mq_h, mq_l, mk_h, mk_l, mv_h, mv_l, a);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) throw std::runtime_error(std::string("attention_tc launch: ") + cudaGetErrorString(e));

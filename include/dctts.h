@@ -206,7 +206,8 @@ int dctts_train_step(dctts_handle h, const int32_t* L, const float* mels, int32_
                      int32_t apply, float* losses_host, void* stream);
 /* The same step on a length-bucketed batch at its own shape (the reference's dynamic_pad=True, data_load.py:122-129):
  * L (B, N) int32 and mels (B, T, n_mels), packed at that shape.  Capacity: 1 <= N <= max_N and 1 <= T <= max_T of the
- * hparams the handle was created with (texts longer than 180 need a handle with a larger max_N, at most 192); B must be
+ * hparams the handle was created with (texts longer than 180 need a handle with a larger max_N; any max_N >= 1 is accepted, and one too large for device
+ * memory fails where its workspace is allocated); B must be
  * the batch size given to dctts_train_init.  A step outside the capacity fails with a message and launches nothing.
  * The losses are the reference's at this shape: means over B T n_mels; the guided-attention sum over the N x T corner of
  * the (max_N, max_T) weight table divided by B N T (train.py:91-95).  The softmax runs over the N keys and TextEnc's SAME
