@@ -139,7 +139,8 @@ struct dctts_handle_s {
     };
     struct TrainTensor { float* p; float* g; float* m; float* v; long long n; int layout, d0, d1, d2, ld; };
     struct {
-        bool ready = false; int B = 0, num = 1, T_in = 0; float rate = 0.f;   // T_in: capacity in mel frames (num = 1: hp.max_T)
+        bool ready = false; int B = 0, num = 1, T_in = 0; float rate = 0.f;   // T_in: capacity in mel frames given at init (num = 1: hp.max_T)
+        int N_cap = 0, T_cap = 0;                               // the workspace's capacity: init's (max_N, T_in), grown by dctts_train_reserve
         std::vector<TrainLayer> layers;
         std::map<std::string, TrainTensor> tensors;            // by TF variable name
         DevBuf pre, out, emb, R, align, dS, gbuf[4], dy, wT, zeros, gts, sums, ids, grads, mom, vel, entries;
@@ -1235,8 +1236,9 @@ void ensure_scratch(H* h, size_t bytes) {
 // config 5).  Forward = the fp32 block kernels with every pre-LN tensor kept; backward = kernels_train.cu.  Gradients, Adam
 // moments and the pointers of all trained variables live in three arenas with identical offsets (the gradient arena is
 // what a data-parallel all-reduce sums).  Activation / gradient rows use a leading dimension rounded to 4 floats (F = 1025).
-// Buffers are sized for a capacity -- (hp.max_N, hp.max_T) for Text2Mel, (T_in) for SSRN -- and every step runs at its
-// batch's own (N, T) up to it (train_set_shape), as the reference's dynamically padded buckets do (data_load.py:122-129).
+// Buffers are sized for a capacity -- (hp.max_N, hp.max_T) for Text2Mel, (T_in) for SSRN, or more after
+// dctts_train_reserve -- and every step runs at its batch's own (N, T) up to it (train_set_shape), as the reference's
+// dynamically padded buckets do (data_load.py:122-129).  The capacity only sizes buffers: no kernel of the step reads it.
 
 // The extents of every block for a step at (N, T): TextEnc runs over N text positions, the other networks over T frames,
 // doubled by each transposed convolution.  Rows are packed at this shape from the start of each capacity-sized buffer, so
@@ -1254,6 +1256,61 @@ void train_set_shape(H* h, int N, int T) {
     }
 }
 
+// The shape-dependent workspace for steps up to (N, T): saved activations, attention buffers, gradient ping-pong
+// buffers and the tensor-core operand planes, and every block's pointers into them.  Grows only; what the buffers held is
+// not kept (each step rewrites what it reads).  The arenas -- variables, gradients, Adam moments, the Adam table -- are
+// not touched, so neither the optimiser state nor the gradient arena's address changes.
+void train_alloc_ws(H* h, int N, int T) {
+    auto& tr = h->tr;
+    const dctts_hparams& hp = h->hp;
+    const int B = tr.B, d = hp.d, num = tr.num;
+    size_t pre_f = 0, out_f = 0, g_f = 0, dy_f = 0, wt_f = 0, tca_f = 0, tcb_f = 0;
+    train_set_shape(h, N, T);                                    // the capacity: every buffer below is sized for it
+    for (auto& t : tr.layers) {
+        const LayerDev& l = *t.l;
+        t.ld_out = roundup(l.cout, 4);
+        pre_f += (size_t)t.rows * l.ldw; out_f += (size_t)t.rows * t.ld_out;
+        g_f = std::max(g_f, (size_t)t.rows * std::max(t.ld_out, roundup(l.cin, 4)));
+        dy_f = std::max(dy_f, (size_t)t.rows * l.ldw);
+        wt_f = std::max(wt_f, (size_t)l.size * l.ldw * roundup(l.cin, 4));
+        {   // operand planes of the tensor-core GEMMs: activations / gradients (plain and transposed), packed weights
+            const size_t rows_in = (size_t)B * t.L_in, cmax = (size_t)roundup(std::max(l.cin, l.ldw), 8);
+            tca_f = std::max(tca_f, std::max(rows_in * cmax, (size_t)l.size * B * roundup(l.cin, 8) * roundup(t.L_in, 8)));
+            tcb_f = std::max(tcb_f, std::max((size_t)B * cmax * roundup(t.L_in, 8),
+                                             (size_t)l.size * roundup(std::max(l.cin, l.ldw) + 255, 256) * roundup(std::max(l.cin, l.ldw), 32)));
+        }
+    }
+    tr.pre.ensure(pre_f * sizeof(float)); tr.out.ensure(out_f * sizeof(float));
+    if (num == 1) {
+        tr.emb.ensure((size_t)B * N * hp.e * sizeof(float)); tr.R.ensure((size_t)B * T * 2 * d * sizeof(float));
+        tr.align.ensure((size_t)B * N * T * sizeof(float)); tr.dS.ensure((size_t)B * T * N * sizeof(float));
+        g_f = std::max(g_f, (size_t)B * std::max(N, T) * (size_t)std::max(2 * d, hp.e));
+    }
+    for (auto& g : tr.gbuf) g.ensure(g_f * sizeof(float));
+    tr.dy.ensure(dy_f * sizeof(float)); tr.wT.ensure(wt_f * sizeof(float));
+    tr.tc_a_hi.ensure(tca_f * sizeof(__half)); tr.tc_a_lo.ensure(tca_f * sizeof(__half));
+    tr.tc_b_hi.ensure(tcb_f * sizeof(__half)); tr.tc_b_lo.ensure(tcb_f * sizeof(__half));
+    tr.tc_slots.ensure(2048 * sizeof(unsigned));
+    tr.tc = GemmTcWs{};
+    tr.tc.a_hi = tr.tc_a_hi.as<__half>(); tr.tc.a_lo = tr.tc_a_lo.as<__half>(); tr.tc.a_elems = tca_f;
+    tr.tc.b_hi = tr.tc_b_hi.as<__half>(); tr.tc.b_lo = tr.tc_b_lo.as<__half>(); tr.tc.b_elems = tcb_f;
+    tr.tc.slots = tr.tc_slots.as<unsigned>(); tr.tc.n_slots = 2048;
+    float* pre = tr.pre.as<float>(); float* out = tr.out.as<float>();
+    for (auto& t : tr.layers) {
+        t.pre = pre; pre += (size_t)t.rows * t.l->ldw;
+        t.out = out; out += (size_t)t.rows * t.ld_out;
+    }
+    // inputs: each block reads the previous block's output; the first block of a network reads the embedding (TextEnc), the
+    // mels shifted by one frame (AudioEnc, train.py:51; set per step), R (AudioDec) or the ground-truth mels (SSRN, per step)
+    for (int net = 0; net < (num == 1 ? 3 : 1); ++net)
+        for (int i = tr.first[net] + 1; i <= tr.last[net]; ++i) { tr.layers[i].in = tr.layers[i - 1].out; tr.layers[i].ld_in = tr.layers[i - 1].ld_out; }
+    if (num == 1) {
+        tr.layers[tr.first[0]].in = tr.emb.as<float>(); tr.layers[tr.first[0]].ld_in = hp.e;
+        tr.layers[tr.first[2]].in = tr.R.as<float>(); tr.layers[tr.first[2]].ld_in = 2 * d;
+    }
+    tr.N_cap = N; tr.T_cap = T;
+}
+
 void train_init(H* h, int B, float rate, int num, int T_in) {
     REQUIRE(h->committed, "dctts_train_init: parameters must be committed first");
     REQUIRE(B >= 1 && rate >= 0.f && rate < 1.f && (num == 1 || num == 2) && T_in >= 1, "dctts_train_init: bad arguments");
@@ -1265,11 +1322,9 @@ void train_init(H* h, int B, float rate, int num, int T_in) {
     h->dec.ok = false; h->dec.why = "this handle has been trained: the packed decode stream is stale";
     tr.ready = false;
     const dctts_hparams& hp = h->hp;
-    const int N = hp.max_N, T = T_in, d = hp.d;
     tr.layers.clear(); tr.tensors.clear();
     std::vector<std::vector<LayerDev>*> nets;
     if (num == 1) nets = {&h->textenc, &h->audioenc, &h->audiodec}; else nets = {&h->ssrn};
-    size_t pre_f = 0, out_f = 0, g_f = 0, dy_f = 0, wt_f = 0, tca_f = 0, tcb_f = 0;
     long long n_grad = 0;
     auto reserve = [&](long long n) { long long o = n_grad; n_grad += (n + 3) / 4 * 4; return o; };
     struct Off { long long W, bias, g1, b1, g2, b2; };
@@ -1286,43 +1341,18 @@ void train_init(H* h, int B, float rate, int num, int T_in) {
         tr.last[net] = li - 1;
     }
     tr.B = B; tr.num = num;
-    train_set_shape(h, N, T);                                    // the capacity: every buffer below is sized for it
     for (auto& t : tr.layers) {
         const LayerDev& l = *t.l;
-        t.ld_out = roundup(l.cout, 4);
-        pre_f += (size_t)t.rows * l.ldw; out_f += (size_t)t.rows * t.ld_out;
-        g_f = std::max(g_f, (size_t)t.rows * std::max(t.ld_out, roundup(l.cin, 4)));
-        dy_f = std::max(dy_f, (size_t)t.rows * l.ldw);
-        wt_f = std::max(wt_f, (size_t)l.size * l.ldw * roundup(l.cin, 4));
-        {   // operand planes of the tensor-core GEMMs: activations / gradients (plain and transposed), packed weights
-            const size_t rows_in = (size_t)B * t.L_in, cmax = (size_t)roundup(std::max(l.cin, l.ldw), 8);
-            tca_f = std::max(tca_f, std::max(rows_in * cmax, (size_t)l.size * B * roundup(l.cin, 8) * roundup(t.L_in, 8)));
-            tcb_f = std::max(tcb_f, std::max((size_t)B * cmax * roundup(t.L_in, 8),
-                                             (size_t)l.size * roundup(std::max(l.cin, l.ldw) + 255, 256) * roundup(std::max(l.cin, l.ldw), 32)));
-        }
         Off o{};
         o.W = reserve((long long)l.size * l.cin * l.ldw); o.bias = reserve(l.ldw);
         o.g1 = reserve(l.cout); o.b1 = reserve(l.cout);
         if (l.kind == K_HC) { o.g2 = reserve(l.cout); o.b2 = reserve(l.cout); }
         offs.push_back(o);
     }
-    tr.pre.ensure(pre_f * sizeof(float)); tr.out.ensure(out_f * sizeof(float));
-    if (num == 1) {
-        tr.emb.ensure((size_t)B * N * hp.e * sizeof(float)); tr.R.ensure((size_t)B * T * 2 * d * sizeof(float));
-        tr.align.ensure((size_t)B * N * T * sizeof(float)); tr.dS.ensure((size_t)B * T * N * sizeof(float));
-        g_f = std::max(g_f, (size_t)B * std::max(N, T) * (size_t)std::max(2 * d, hp.e));
-        tr.gts.ensure((size_t)N * T * sizeof(float)); launch_guided_attention(tr.gts.as<float>(), N, T, h->stream);
+    if (num == 1) {                                              // the (max_N, max_T) table whatever the workspace's capacity
+        tr.gts.ensure((size_t)hp.max_N * T_in * sizeof(float)); launch_guided_attention(tr.gts.as<float>(), hp.max_N, T_in, h->stream);
     }
-    for (auto& g : tr.gbuf) g.ensure(g_f * sizeof(float));
-    tr.dy.ensure(dy_f * sizeof(float)); tr.wT.ensure(wt_f * sizeof(float));
     tr.zeros.ensure(4096 * sizeof(float)); CUDA_CHECK(cudaMemset(tr.zeros.p, 0, 4096 * sizeof(float)));
-    tr.tc_a_hi.ensure(tca_f * sizeof(__half)); tr.tc_a_lo.ensure(tca_f * sizeof(__half));
-    tr.tc_b_hi.ensure(tcb_f * sizeof(__half)); tr.tc_b_lo.ensure(tcb_f * sizeof(__half));
-    tr.tc_slots.ensure(2048 * sizeof(unsigned));
-    tr.tc = GemmTcWs{};
-    tr.tc.a_hi = tr.tc_a_hi.as<__half>(); tr.tc.a_lo = tr.tc_a_lo.as<__half>(); tr.tc.a_elems = tca_f;
-    tr.tc.b_hi = tr.tc_b_hi.as<__half>(); tr.tc.b_lo = tr.tc_b_lo.as<__half>(); tr.tc.b_elems = tcb_f;
-    tr.tc.slots = tr.tc_slots.as<unsigned>(); tr.tc.n_slots = 2048;
     tr.sums.ensure(4 * sizeof(double));
     tr.grads.ensure(n_grad * sizeof(float)); tr.mom.ensure(n_grad * sizeof(float)); tr.vel.ensure(n_grad * sizeof(float));
     CUDA_CHECK(cudaMemset(tr.grads.p, 0, n_grad * sizeof(float)));
@@ -1337,11 +1367,8 @@ void train_init(H* h, int B, float rate, int num, int T_in) {
         return G + off;
     };
     if (num == 1) tr.d_table = reg("Text2Mel/TextEnc/embed_1/lookup_table", h->embed_table, table_off, (long long)hp.vocab_size * hp.e);
-    float* pre = tr.pre.as<float>(); float* out = tr.out.as<float>();
     for (size_t i = 0; i < tr.layers.size(); ++i) {
         auto& t = tr.layers[i]; LayerDev& l = *t.l; const Off& o = offs[i];
-        t.pre = pre; pre += (size_t)t.rows * l.ldw;
-        t.out = out; out += (size_t)t.rows * t.ld_out;
         const long long wn = (long long)l.size * l.cin * l.ldw;
         if (l.kind == K_D) {
             t.dW = reg(l.scope + "/conv2d_transpose/kernel", l.W, o.W, wn, 2, l.size, l.cin, l.cout, l.ldw);
@@ -1354,25 +1381,38 @@ void train_init(H* h, int B, float rate, int num, int T_in) {
         t.dg1 = reg(l.scope + n1 + "/gamma", l.g1, o.g1, l.cout); t.db1 = reg(l.scope + n1 + "/beta", l.b1, o.b1, l.cout);
         if (l.kind == K_HC) { t.dg2 = reg(l.scope + "/H2/gamma", l.g2, o.g2, l.cout); t.db2 = reg(l.scope + "/H2/beta", l.b2, o.b2, l.cout); }
     }
-    // inputs: each block reads the previous block's output; the first block of a network reads the embedding (TextEnc), the
-    // mels shifted by one frame (AudioEnc, train.py:51; set per step), R (AudioDec) or the ground-truth mels (SSRN, per step)
-    for (size_t net = 0; net < nets.size(); ++net)
-        for (int i = tr.first[net]; i <= tr.last[net]; ++i) {
-            auto& t = tr.layers[i];
-            if (i > tr.first[net]) { t.in = tr.layers[i - 1].out; t.ld_in = tr.layers[i - 1].ld_out; }
-        }
+    // the first block of AudioEnc (Text2Mel) or of SSRN reads the step's mels: set per step
     if (num == 1) {
-        tr.layers[tr.first[0]].in = tr.emb.as<float>(); tr.layers[tr.first[0]].ld_in = hp.e;
         tr.layers[tr.first[1]].ld_in = hp.n_mels; tr.layers[tr.first[1]].extra_shift = -1; tr.layers[tr.first[1]].need_dgrad = false;
-        tr.layers[tr.first[2]].in = tr.R.as<float>(); tr.layers[tr.first[2]].ld_in = 2 * d;
     } else {
         tr.layers[0].ld_in = hp.n_mels; tr.layers[0].need_dgrad = false;
     }
+    tr.N_cap = tr.T_cap = 0;
+    train_alloc_ws(h, num == 1 ? hp.max_N : 0, T_in);
     tr.entries.ensure(entries.size() * sizeof(AdamEntry));
     CUDA_CHECK(cudaMemcpy(tr.entries.p, entries.data(), entries.size() * sizeof(AdamEntry), cudaMemcpyHostToDevice));
     tr.n_entries = (int)entries.size();
     CUDA_CHECK(cudaStreamSynchronize(h->stream));
     tr.B = B; tr.rate = rate; tr.num = num; tr.T_in = T_in; tr.ready = true;
+}
+
+// Grow the workspace of the network being trained to at least N text positions (Text2Mel only) and T mel frames.  Never
+// shrinks; a no-op when the workspace already fits.  The arenas stay where they are (train_alloc_ws).
+void train_reserve(H* h, int N, int T) {
+    auto& tr = h->tr;
+    REQUIRE(tr.ready, "dctts_train_reserve: call dctts_train_init or dctts_train_init_ssrn first");
+    REQUIRE(N >= 0 && T >= 0, "dctts_train_reserve: bad arguments");
+    const int n = tr.num == 1 ? std::max(N, tr.N_cap) : 0, t = std::max(T, tr.T_cap);
+    if (n == tr.N_cap && t == tr.T_cap) return;
+    CUDA_CHECK(cudaDeviceSynchronize());                         // steps still in flight may read the buffers being replaced
+    const int n0 = tr.N_cap, t0 = tr.T_cap;
+    try {
+        train_alloc_ws(h, n, t);
+    } catch (...) {                                              // out of memory: back to the old capacity, or no training state
+        cudaGetLastError();
+        try { train_alloc_ws(h, n0, t0); } catch (...) { tr.ready = false; cudaGetLastError(); }
+        throw;
+    }
 }
 
 void layer_shifts(const LayerDev& l, int extra, int* shifts) {
@@ -1495,17 +1535,21 @@ void train_read_losses(H* h, float* losses_host, double n_el, double n_att, cuda
     losses_host[0] = losses_host[1] + losses_host[2] + losses_host[3];
 }
 
-// One Text2Mel step on L (B, N) and mels (B, T, n_mels), packed at that shape, N <= hp.max_N and T <= hp.max_T.  The losses
-// are the reference's at this shape (train.py:83-95): means over B T n_mels, the guided-attention sum over the N x T corner of
-// the (max_N, max_T) table divided by B N T.  The softmax sees N keys and TextEnc's SAME padding the edge at N.
+// One Text2Mel step on L (B, N) and mels (B, T, n_mels), packed at that shape, N and T up to the workspace's capacity
+// ((hp.max_N, hp.max_T) unless dctts_train_reserve grew it).  The losses are the reference's at this shape (train.py:83-95):
+// means over B T n_mels, and the guided-attention sum over the n_lim x t_lim corner of the (max_N, max_T) table divided by
+// B n_lim t_lim, n_lim = min(N, max_N), t_lim = min(T, max_T) (the -1 padding of train.py:91 is cropped to the table).  The
+// softmax sees N keys and TextEnc's SAME padding the edge at N.
 void train_forward_backward(H* h, const int* L, int N, const float* mels, int T, int B, uint32_t seed, float* losses_host,
                             cudaStream_t s) {
     auto& tr = h->tr;
     REQUIRE(tr.ready && tr.num == 1 && tr.B == B, "dctts_train_step: call dctts_train_init with this batch size first");
     const dctts_hparams& hp = h->hp;
-    REQUIRE(N >= 1 && N <= hp.max_N && T >= 1 && T <= hp.max_T,
+    REQUIRE(N >= 1 && N <= tr.N_cap && T >= 1 && T <= tr.T_cap,
             "dctts_train_step: N = " + std::to_string(N) + ", T = " + std::to_string(T) + " outside the handle's capacity (1..max_N = " +
-            std::to_string(hp.max_N) + ", 1..max_T = " + std::to_string(hp.max_T) + ")");
+            std::to_string(hp.max_N) + ", 1..max_T = " + std::to_string(hp.max_T) +
+            (tr.N_cap != hp.max_N || tr.T_cap != hp.max_T ? ", reserved " + std::to_string(tr.N_cap) + " x " + std::to_string(tr.T_cap) : "") +
+            "; dctts_train_reserve grows it)");
     const int d = hp.d;
     train_set_shape(h, N, T);
     Launch lc{h, s};
@@ -1533,24 +1577,26 @@ void train_forward_backward(H* h, const int* L, int N, const float* mels, int T,
     AttnBwdArgs ab{};
     ab.gR = gR; ab.Q = Q; ab.ldq = d; ab.K = KV; ab.V = KV + d; ab.ldkv = 2 * d; ab.align = tr.align.as<float>();
     ab.gts = tr.gts.as<float>(); ab.ld_gts = hp.max_T; ab.dS = tr.dS.as<float>(); ab.gQ = tr.gbuf[2].as<float>(); ab.gKV = tr.gbuf[3].as<float>();
-    ab.B = B; ab.T = T; ab.N = N; ab.d = d; ab.att_scale = 1.0f / ((float)B * (float)N * (float)T);
+    const int n_lim = std::min(N, hp.max_N), t_lim = std::min(T, hp.max_T);      // the crop of train.py:91 to the table
+    ab.B = B; ab.T = T; ab.N = N; ab.d = d; ab.n_lim = n_lim; ab.t_lim = t_lim;
+    ab.att_scale = 1.0f / ((float)B * (float)n_lim * (float)t_lim);
     launch_attn_bwd(ab, tr.sums.as<double>(), s); lc.count(3);
     float* free_a = (gR == tr.gbuf[0].as<float>()) ? tr.gbuf[1].as<float>() : tr.gbuf[0].as<float>();
     train_bwd(h, lc, tr.first[1], tr.last[1], B, seed, tr.gbuf[2].as<float>(), free_a);
     float* gEmb = train_bwd(h, lc, tr.first[0], tr.last[0], B, seed, tr.gbuf[3].as<float>(), free_a);
     launch_embed_bwd(L, gEmb, tr.d_table, B * N, hp.e, s); lc.count();
     CUDA_CHECK(cudaGetLastError());
-    train_read_losses(h, losses_host, (double)B * T * hp.n_mels, (double)B * N * T, s);
+    train_read_losses(h, losses_host, (double)B * T * hp.n_mels, (double)B * n_lim * t_lim, s);
 }
 
 // SSRN (num = 2): ground-truth mels (B, T, n_mels) in, L1 + binary divergence against the linear magnitudes (B, 4T, F), means
-// over B 4T F (train.py:100-108); T up to the capacity given to dctts_train_init_ssrn
+// over B 4T F (train.py:100-108); T up to the capacity given to dctts_train_init_ssrn or grown by dctts_train_reserve
 void train_forward_backward_ssrn(H* h, const float* mels, const float* mags, int B, int T, uint32_t seed, float* losses_host,
                                  cudaStream_t s) {
     auto& tr = h->tr;
     REQUIRE(tr.ready && tr.num == 2 && tr.B == B, "dctts_train_step_ssrn: call dctts_train_init_ssrn with this batch size first");
-    REQUIRE(T >= 1 && T <= tr.T_in, "dctts_train_step_ssrn: T = " + std::to_string(T) + " outside the handle's capacity (1.." +
-            std::to_string(tr.T_in) + ", set by dctts_train_init_ssrn)");
+    REQUIRE(T >= 1 && T <= tr.T_cap, "dctts_train_step_ssrn: T = " + std::to_string(T) + " outside the handle's capacity (1.." +
+            std::to_string(tr.T_cap) + ", set by dctts_train_init_ssrn" + (tr.T_cap != tr.T_in ? " and dctts_train_reserve)" : ")"));
     train_set_shape(h, 0, T);
     Launch lc{h, s};
     CUDA_CHECK(cudaMemsetAsync(tr.grads.p, 0, tr.n_grad * sizeof(float), s));
@@ -2186,6 +2232,17 @@ int dctts_train_step(dctts_handle h, const int32_t* L, const float* mels, int32_
 
 int dctts_train_apply(dctts_handle h, int64_t global_step, float lr, void* stream) {
     return guarded(h, [&] { REQUIRE(global_step >= 0, "dctts_train_apply: bad step"); train_apply(h, global_step, lr, S(h, stream)); });
+}
+
+int dctts_train_reserve(dctts_handle h, int32_t N, int32_t T) {
+    return guarded(h, [&] { train_reserve(h, N, T); });
+}
+
+int dctts_train_capacity(dctts_handle h, int32_t* N, int32_t* T) {
+    return guarded(h, [&] {
+        REQUIRE(h->tr.ready && N && T, "dctts_train_capacity: no training state");
+        *N = h->tr.num == 1 ? h->tr.N_cap : 0; *T = h->tr.T_cap;
+    });
 }
 
 int dctts_train_grads(dctts_handle h, float** grads, int64_t* count) {

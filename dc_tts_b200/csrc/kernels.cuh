@@ -194,11 +194,12 @@ struct AttnBwdArgs {
     const float* gR;                   // (B,T,2d) gradient of [ctx ; Q]
     const float* Q; int ldq; const float* K; const float* V; int ldkv;
     const float* align;                // (B,N,T) probabilities of the forward pass
-    const float* gts; int ld_gts;      // guided-attention weights (max_N, max_T), row stride ld_gts; the (N, T) corner is read
+    const float* gts; int ld_gts;      // guided-attention weights (max_N, max_T), row stride ld_gts; the (n_lim, t_lim) corner is read
     float* dS;                         // (B,T,N) scratch
     float* gQ;                         // (B,T,d)
     float* gKV;                        // (B,N,2d)
-    int B, T, N, d; float att_scale;   // att_scale = 1 / (B N T)
+    int B, T, N, d; float att_scale;   // att_scale = 1 / (B n_lim t_lim)
+    int n_lim, t_lim;                  // the guided-attention crop: min(N, max_N), min(T, max_T); keys / frames past it get no term
 };
 struct AdamEntry { float* p; float* g; float* m; float* v; long long n; };
 void launch_train_dropout(float* x, long long rows, int C, int ld, const DropArgs& d, cudaStream_t s);

@@ -288,10 +288,12 @@ void launch_transpose_w(const float* W, float* WT, int ntaps, int K, int N, int 
 
 // ------------------------------------------------------------------------------------ attention backward
 // Forward (networks.py:140-153, training: no window): S = Q K^T / sqrt(d), A = softmax_n(S), ctx = A V, R = [ctx ; Q];
-// loss_att = sum |A gts| / (B N T) (train.py:91-95) at the step's (N, T); gts is the (max_N, max_T) table of
-// utils.guided_attention with row stride ld_gts, of which the -1 padding and mask of train.py:91-95 leave the N x T
-// corner.  One warp per query row (b, t):
-//   dA[n] = dctx . V[n] + sign(A gts) gts[n,t] / (B N T);  dS[n] = A[n] (dA[n] - sum_m A[m] dA[m])
+// loss_att = sum |A gts| / (B n_lim t_lim) (train.py:91-95) at the step's (N, T); gts is the (max_N, max_T) table of
+// utils.guided_attention with row stride ld_gts, of which the -1 padding, crop and mask of train.py:91-95 leave the
+// n_lim x t_lim corner, n_lim = min(N, max_N), t_lim = min(T, max_T).  Keys n >= n_lim and frames t >= t_lim have no
+// guided-attention term (and the table is not read there); they still get the L1 / BCE gradient through the softmax.
+// One warp per query row (b, t):
+//   dA[n] = dctx . V[n] + sign(A gts) gts[n,t] / (B n_lim t_lim) [inside the corner];  dS[n] = A[n] (dA[n] - sum_m A[m] dA[m])
 //   dQ = dR[d:2d] + sum_n dS[n] K[n] / sqrt(d);  dS is kept (B,T,N) for the key-side kernel.
 // d = 256 = 32 lanes x 8.  dA is kept per warp in dynamic shared memory, N floats.
 __global__ void __launch_bounds__(128) attn_bwd_q_kernel(const AttnBwdArgs a) {
@@ -313,7 +315,7 @@ __global__ void __launch_bounds__(128) attn_bwd_q_kernel(const AttnBwdArgs a) {
         for (int i = 0; i < 8; ++i) s = fmaf(dctx[i], __ldg(v + lane * 8 + i), s);
         s = wsum(s);
         const float p = a.align[((size_t)b * a.N + n) * a.T + t];
-        const float g = a.gts[(size_t)n * a.ld_gts + t];
+        const float g = (n < a.n_lim && t < a.t_lim) ? a.gts[(size_t)n * a.ld_gts + t] : 0.f;
         const float pg = p * g;
         s += (pg > 0.f ? g : (pg < 0.f ? -g : 0.f)) * a.att_scale;
         if (lane == 0) da[n] = s;
@@ -359,16 +361,16 @@ __global__ void __launch_bounds__(128) attn_bwd_kv_kernel(const AttnBwdArgs a) {
     for (int i = 0; i < 8; ++i) { o[lane * 8 + i] = dk[i]; o[a.d + lane * 8 + i] = dv[i]; }
 }
 
-// sums[2] += sum |A gts|; align (B, N, T), gts (>= N, ld_gts >= T)
+// sums[2] += sum over the (n_lim, t_lim) corner of |A gts|; align (B, N, T), gts (>= n_lim rows, ld_gts >= t_lim)
 __global__ void attn_loss_kernel(const float* __restrict__ align, const float* __restrict__ gts, int ld_gts, double* __restrict__ sums,
-                                 int B, int N, int T) {
+                                 int B, int N, int T, int n_lim, int t_lim) {
     __shared__ double red[8];
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     double v = 0.0;
     if (i < (long long)B * N * T) {
         const long long nt = i % ((long long)N * T);
         const int n = (int)(nt / T), t = (int)(nt - (long long)n * T);
-        v = fabsf(align[i] * gts[(size_t)n * ld_gts + t]);
+        if (n < n_lim && t < t_lim) v = fabsf(align[i] * gts[(size_t)n * ld_gts + t]);
     }
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
@@ -378,7 +380,10 @@ __global__ void attn_loss_kernel(const float* __restrict__ align, const float* _
 
 void launch_attn_bwd(const AttnBwdArgs& a, double* sums, cudaStream_t s) {
     if (a.d != 256) throw std::runtime_error("attention backward is built for d = 256");
-    if (a.ld_gts < a.T) throw std::runtime_error("attention backward: the guided-attention table is narrower than T");
+    if (a.n_lim < 1 || a.n_lim > a.N || a.t_lim < 1 || a.t_lim > a.T || a.ld_gts < a.t_lim)
+        throw std::runtime_error("attention backward: the guided-attention crop (" + std::to_string(a.n_lim) + ", " +
+                                 std::to_string(a.t_lim) + ") does not fit the step (" + std::to_string(a.N) + ", " +
+                                 std::to_string(a.T) + ") or the table's row stride " + std::to_string(a.ld_gts));
     const size_t smem = (size_t)4 * a.N * sizeof(float);
     if (smem > 48 * 1024) {
         cudaError_t e = cudaFuncSetAttribute(attn_bwd_q_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -389,7 +394,7 @@ void launch_attn_bwd(const AttnBwdArgs& a, double* sums, cudaStream_t s) {
         }
     }
     const long long n = (long long)a.B * a.N * a.T;
-    attn_loss_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a.align, a.gts, a.ld_gts, sums, a.B, a.N, a.T);
+    attn_loss_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a.align, a.gts, a.ld_gts, sums, a.B, a.N, a.T, a.n_lim, a.t_lim);
     attn_bwd_q_kernel<<<(a.B * a.T + 3) / 4, 128, smem, s>>>(a);
     attn_bwd_kv_kernel<<<(a.B * a.N + 3) / 4, 128, 0, s>>>(a);
 }

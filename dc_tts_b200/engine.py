@@ -399,7 +399,8 @@ class Engine:
 
     def train_step(self, L, mels, global_step=0, seed=0, lr=None, apply=True):
         """One Text2Mel optimiser step on L (B, N) int32 / mels (B, T, n_mels) at the batch's own shape -- a bucket padded
-        to its longest member (trainer.bucketed_batches) or the fixed (max_N, max_T) -- up to N = hp.max_N, T = hp.max_T:
+        to its longest member (trainer.bucketed_batches) or the fixed (max_N, max_T) -- up to N = hp.max_N, T = hp.max_T,
+        or the capacity given to train_reserve:
         forward with dropout, losses (train.py:83-99), backward, clip, Adam (train.py:122-132).
         Returns {loss, loss_mels, loss_bd1, loss_att}."""
         L = self._i32(L); mels = self._f32(mels)
@@ -437,6 +438,20 @@ class Engine:
                                                            int(seed) & 0xffffffff, float(self.hp.lr if lr is None else lr),
                                                            1 if apply else 0, out, self._stream()), "dctts_train_step_ssrn")
         return {"loss": out[0], "loss_mags": out[1], "loss_bd2": out[2]}
+
+    def train_reserve(self, N, T):
+        """Grow the training workspace of the network being trained to at least N text positions (Text2Mel; ignored for
+        SSRN) and T mel frames, so that train_step / train_step_ssrn accept batches up to that shape.  The variables, Adam
+        moments and the gradient arena (train_grads' address) are kept.  Never shrinks; synchronises the device when it
+        grows.  Past (max_N, max_T) the guided-attention loss covers the table's corner only (train.py:91-95)."""
+        self._check(self._lib.dctts_train_reserve(self._h, int(N), int(T)), "dctts_train_reserve")
+
+    def train_capacity(self):
+        """(N_cap, T_cap) of the training workspace: (max_N, max_T) after train_init, (0, T) after train_init_ssrn, or what
+        train_reserve grew it to."""
+        n, t = C.c_int32(0), C.c_int32(0)
+        self._check(self._lib.dctts_train_capacity(self._h, C.byref(n), C.byref(t)), "dctts_train_capacity")
+        return n.value, t.value
 
     def train_apply(self, global_step, lr=None):
         self._check(self._lib.dctts_train_apply(self._h, int(global_step), float(self.hp.lr if lr is None else lr), self._stream()),

@@ -43,11 +43,13 @@ _TRAIN = {1: ("loss", "loss_mels", "loss_bd1", "loss_att"), 2: ("loss", "loss_ma
 
 
 class Graph:
-    def __init__(self, num=1, mode="train", engine=None, fused=True, batches=None, num_batch=None, global_step=0):
+    def __init__(self, num=1, mode="train", engine=None, fused=True, batches=None, num_batch=None, global_step=0,
+                 beyond_capacity="skip", capacity=None):
         """mode "synthesize": the inference graph.  mode "train" (the reference default): `num` = 1 trains Text2Mel, 2 SSRN;
         `batches` is the input pipeline, an iterator of (L, mels, mags, ...) tuples -- trainer.bucketed_batches(...) at each
         batch's own shape, or trainer.fixed_size_batches(...).  Batches beyond the capacity (hp.max_N, hp.max_T) are
-        skipped and counted in `skipped_batches`."""
+        skipped and counted in `skipped_batches`, or with `beyond_capacity="grow"` trained after the workspace grows in
+        place (the Adam state is kept); `capacity` = (N, T) reserves a larger workspace once (trainer.Capacity)."""
         if mode not in ("train", "synthesize"):
             raise ValueError("mode: 'train' or 'synthesize' (train.py:22)")
         self.char2idx, self.idx2char = load_vocab()
@@ -64,7 +66,8 @@ class Graph:
             self.num_batch = num_batch                       # train.py:33; only used for the progress bar
             self.global_step_value = int(global_step)
             self.last = {}
-            self.skipped_batches = 0
+            from .trainer import Capacity
+            self._capacity = Capacity(num, getattr(self.engine, "hp", hp), beyond_capacity, capacity)
             self._initialised = False
             for name in ("global_step", "train_op", "lr") + _TRAIN[num]:
                 setattr(self, name, Symbol(self, name))
@@ -94,20 +97,20 @@ class Graph:
 
     def _train_run(self, names):
         """One `sess.run` of the training graph: fetching train_op consumes a batch and applies one update."""
-        from .trainer import over_capacity
         from .utils import learning_rate_decay
         if "train_op" in names:
-            cap = getattr(self.engine, "hp", hp)
+            cap, capa = getattr(self.engine, "hp", hp), self._capacity
             L, mels, mags = next(self.batches)[:3]
-            while over_capacity(self.num, L, mels, cap):          # the workspace is not re-allocated: that would reset Adam
-                self.skipped_batches += 1
+            while not capa.admit(L, mels, lambda *_: None):      # "skip": counted in skipped_batches
                 L, mels, mags = next(self.batches)[:3]
             if not self._initialised:
                 if self.num == 1:
                     self.engine.train_init(len(L))
                 else:
                     self.engine.train_init_ssrn(len(L), cap.max_T)
+                capa.initialised(self.engine)
                 self._initialised = True
+            capa.prepare(self.engine, L, mels, lambda *_: None)
             gs = self.global_step_value
             if self.num == 1:
                 self.last = self.engine.train_step(L, mels, global_step=gs, seed=gs)
@@ -121,6 +124,11 @@ class Graph:
                 raise ValueError("%s: no training step has run yet (fetch it together with train_op)" % k)
             out[k] = np.float32(self.last.get(k, np.nan))
         return out
+
+    @property
+    def skipped_batches(self):
+        """Batches beyond the capacity skipped so far (beyond_capacity="skip")."""
+        return self._capacity.skipped
 
     def run(self, fetches, feed_dict=None, as_numpy=True):
         """`sess.run` equivalent.  Feeding `self.Y` cuts Text2Mel out of the evaluation,

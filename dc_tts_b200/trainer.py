@@ -8,7 +8,9 @@ Batching: `bucketed_batches` restates the reference's length-bucketed, dynamical
 shuffled stream, buckets by text length every 20 characters, a full bucket emits a batch padded to its own longest
 member).  `train` and `Graph(num, mode="train")` take those batches as they are: the CUDA step runs at each batch's own
 (N_b, T_b), up to the capacity (hp.max_N, hp.max_T), and its losses are the reference's at that shape.  A batch beyond
-the capacity is skipped and counted.  `fixed_size_batches` (plain shuffled batches padded to (max_N, max_T), BASELINE
+the capacity is skipped and counted by default (`beyond_capacity="skip"`); with `beyond_capacity="grow"` the workspace
+grows in place to take it, as the reference trains every batch whatever its shape, and the optimiser state is kept
+(`Capacity`).  `fixed_size_batches` (plain shuffled batches padded to (max_N, max_T), BASELINE
 config 5) and `pad_to_fixed` (a bucket padded further to the fixed shapes) remain for fixed-shape training.
 """
 import codecs
@@ -201,12 +203,84 @@ def over_capacity(num, L, mels, cap=hp):
     return mels.shape[1] > cap.max_T or (num == 1 and L.shape[1] > cap.max_N)
 
 
+def _round64(n):
+    return -(-int(n) // 64) * 64
+
+
+class Capacity:
+    """The (N, T) the training workspace holds and what happens to a batch beyond it, for `train` and
+    `Graph(mode="train")`.  It starts at (hp.max_N, hp.max_T), or at `capacity` = (N, T) where that is larger, which is
+    reserved once right after the engine's train_init (a user who knows the corpus's longest text and clip grows the
+    workspace once, up front).  `beyond_capacity`:
+      "skip"  (default) a batch beyond the capacity is skipped and counted: `admit` returns False;
+      "grow"  the workspace grows to the batch's shape, each growing dimension rounded up to a multiple of 64 so that a
+              stream of buckets does not re-allocate at every slightly longer batch; the growth is logged and the batch
+              trained.  Engine.train_reserve keeps the variables, the Adam moments and the gradient arena, so nothing of
+              the optimiser is lost, and data-parallel ranks may grow at different steps.
+    Past (hp.max_N, hp.max_T) the guided-attention loss covers the (max_N, max_T) table's corner only, as train.py:91-95
+    crops it; the mel losses cover the whole batch."""
+
+    def __init__(self, num, cap=hp, beyond_capacity="skip", capacity=None):
+        if beyond_capacity not in ("skip", "grow"):
+            raise ValueError("beyond_capacity: 'skip' or 'grow', got %r" % (beyond_capacity,))
+        self.num, self.mode, self.cap = num, beyond_capacity, cap
+        self.N, self.T = cap.max_N, cap.max_T
+        self.requested = None
+        if capacity is not None:
+            N, T = (int(x) for x in capacity)
+            if N < 1 or T < 1:
+                raise ValueError("capacity: (N, T) >= 1, got %r" % (capacity,))
+            self.requested = (N, T)
+            self.N, self.T = max(self.N, N), max(self.T, T)
+        self.skipped = 0
+
+    def fits(self, L, mels):
+        return mels.shape[1] <= self.T and (self.num != 1 or L.shape[1] <= self.N)
+
+    def _reserve(self, engine):
+        engine.train_reserve(self.N if self.num == 1 else 0, self.T)
+
+    def admit(self, L, mels, log):
+        """False (logged and counted) when the batch is beyond the capacity and beyond_capacity is "skip"."""
+        if self.mode == "grow" or self.fits(L, mels):
+            return True
+        self.skipped += 1
+        if self.requested is None:
+            log("skipped a batch of shape N=%d, T=%d beyond the capacity (max_N=%d, max_T=%d); %d skipped so far"
+                % (L.shape[1], mels.shape[1], self.cap.max_N, self.cap.max_T, self.skipped))
+        else:
+            log("skipped a batch of shape N=%d, T=%d beyond the capacity (N=%d, T=%d); %d skipped so far"
+                % (L.shape[1], mels.shape[1], self.N, self.T, self.skipped))
+        return False
+
+    def initialised(self, engine):
+        """Right after the engine's train_init: reserve the requested capacity."""
+        if self.requested is not None and (self.N, self.T) != (self.cap.max_N, self.cap.max_T):
+            self._reserve(engine)
+
+    def prepare(self, engine, L, mels, log):
+        """Before a step on an admitted batch: grow the workspace when the batch does not fit it."""
+        if self.fits(L, mels):
+            return
+        if self.num == 1 and L.shape[1] > self.N:
+            self.N = _round64(L.shape[1])
+        if mels.shape[1] > self.T:
+            self.T = _round64(mels.shape[1])
+        self._reserve(engine)
+        if self.num == 1:
+            log("grew the training workspace to N=%d, T=%d for a batch of shape N=%d, T=%d"
+                % (self.N, self.T, L.shape[1], mels.shape[1]))
+        else:
+            log("grew the training workspace to T=%d for a batch of T=%d" % (self.T, mels.shape[1]))
+
+
 def train(num, engine, batches, num_iterations=None, logdir=None, global_step=None, save_every=1000, log=print, resume=True,
-          rank=0, world=1, allreduce=None):
+          rank=0, world=1, allreduce=None, beyond_capacity="skip", capacity=None):
     """train.py:137-160 for num = 1 (Text2Mel) or 2 (SSRN).  `batches` yields (L, mels, mags, names, ...): the bucketed
     batches of `bucketed_batches` at their own shapes or fixed-size ones; `engine` is an `Engine` with parameters loaded.
-    The workspace is allocated once for the capacity (hp.max_N, hp.max_T); a batch beyond it is skipped and counted in the
-    log (re-allocating would reset the Adam state).  Like tf.train.Supervisor (train.py:144), a `logdir` that already holds a checkpoint
+    The workspace is allocated for the capacity (hp.max_N, hp.max_T), or `capacity` = (N, T) when that is larger; a batch
+    beyond it is skipped and counted in the log, or with `beyond_capacity="grow"` the workspace grows in place (keeping the
+    Adam state) and the batch is trained (see `Capacity`).  Like tf.train.Supervisor (train.py:144), a `logdir` that already holds a checkpoint
     is RESUMED: variables, Adam slots and the global step come back from it (`resume=False` or an explicit `global_step`
     starts over).  Data parallel (BASELINE config 5, `world` > 1): every rank feeds its own disjoint `batches`, the step
     runs with apply=False, `allreduce` (default dc_tts_b200.parallel.allreduce_mean_) averages the flat gradient arena,
@@ -219,14 +293,11 @@ def train(num, engine, batches, num_iterations=None, logdir=None, global_step=No
     os.makedirs(logdir, exist_ok=True)
     gs = int(global_step or 0)
     cap = getattr(engine, "hp", hp)
+    capa = Capacity(num, cap, beyond_capacity, capacity)
     initialised = False
-    skipped = 0
     for batch in batches:
         L, mels, mags = batch[:3]
-        if over_capacity(num, L, mels, cap):
-            skipped += 1
-            log("skipped a batch of shape N=%d, T=%d beyond the capacity (max_N=%d, max_T=%d); %d skipped so far"
-                % (L.shape[1], mels.shape[1], cap.max_N, cap.max_T, skipped))
+        if not capa.admit(L, mels, log):
             continue
         if not initialised:
             if num == 1:
@@ -238,7 +309,9 @@ def train(num, engine, batches, num_iterations=None, logdir=None, global_step=No
                 if restored is not None:
                     gs = restored
                     log("resumed from %s at global step %d" % (logdir, gs))
+            capa.initialised(engine)
             initialised = True
+        capa.prepare(engine, L, mels, log)
         if world > 1:
             if allreduce is None:
                 from .parallel import allreduce_mean_ as allreduce

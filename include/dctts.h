@@ -206,7 +206,8 @@ int dctts_train_step(dctts_handle h, const int32_t* L, const float* mels, int32_
                      int32_t apply, float* losses_host, void* stream);
 /* The same step on a length-bucketed batch at its own shape (the reference's dynamic_pad=True, data_load.py:122-129):
  * L (B, N) int32 and mels (B, T, n_mels), packed at that shape.  Capacity: 1 <= N <= max_N and 1 <= T <= max_T of the
- * hparams the handle was created with (texts longer than 180 need a handle with a larger max_N; any max_N >= 1 is accepted, and one too large for device
+ * hparams the handle was created with, or more after dctts_train_reserve (texts longer than 180 need a handle with a
+ * larger max_N or a reserve; any max_N >= 1 is accepted, and one too large for device
  * memory fails where its workspace is allocated); B must be
  * the batch size given to dctts_train_init.  A step outside the capacity fails with a message and launches nothing.
  * The losses are the reference's at this shape: means over B T n_mels; the guided-attention sum over the N x T corner of
@@ -225,6 +226,17 @@ int dctts_train_step_ssrn(dctts_handle h, const float* mels, const float* mags, 
                           int32_t apply, float* losses_host, void* stream);
 int dctts_train_step_ssrn_shaped(dctts_handle h, const float* mels, const float* mags, int32_t B, int32_t T, int64_t global_step,
                                  uint32_t seed, float lr, int32_t apply, float* losses_host, void* stream);
+/* Grow the training workspace of the network being trained (the last init call's) to at least N text positions (Text2Mel;
+ * ignored for SSRN) and T mel frames, so that the shaped steps accept 1 <= N <= N_cap and 1 <= T <= T_cap.  Without a
+ * reserve call the capacity is the init call's: (max_N, max_T) for Text2Mel, T for SSRN.  Never shrinks; a no-op when the
+ * workspace already fits; otherwise it synchronises the device and re-allocates only the shape-dependent buffers: the
+ * variables, the gradient arena (and its address, dctts_train_grads) and the Adam moments are kept, so training continues
+ * where it was.  The guided-attention table stays (max_N, max_T): a Text2Mel step past it takes the guided-attention loss
+ * over the min(N, max_N) x min(T, max_T) corner divided by B min(N, max_N) min(T, max_T) (train.py:91-95 pads with -1 and
+ * crops to the table), and keys or frames outside that corner get the mel losses' gradients only.  A failed growth (out of
+ * memory) leaves the old capacity.  dctts_train_capacity reports (N_cap, T_cap); N_cap is 0 for SSRN. */
+int dctts_train_reserve(dctts_handle h, int32_t N, int32_t T);
+int dctts_train_capacity(dctts_handle h, int32_t* N, int32_t* T);
 int dctts_train_grads(dctts_handle h, float** grads, int64_t* count);
 int dctts_train_tensor(dctts_handle h, const char* tf_name, int32_t what, float* host_out, int64_t count);
 /* Inverse of dctts_train_tensor for what = 0 (variable), 2 (Adam m), 3 (Adam v): restores a training state (resume). */

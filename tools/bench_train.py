@@ -1,12 +1,16 @@
 """BASELINE config 5: Text2Mel training step, B = 32 per GPU, fixed N = 180 / T = 210, synthetic batch, dropout on,
 data-parallel over the launched ranks (gradient all-reduce of the flat arena over NCCL).  Prints one JSON line.
-`--shape N,T` steps at a length bucket's own shape instead (the workspace keeps its (max_N, max_T) capacity).
-    python tools/bench_train.py [--steps 10 --warmup 3 --batch 32 --net 1 --shape 180,210]
+`--shape N,T` steps at a length bucket's own shape instead (the workspace keeps its (max_N, max_T) capacity); with
+`--reserve N,T` the workspace is first grown to that capacity (Engine.train_reserve, timed once: "reserve_ms"), so `--shape`
+can go past (max_N, max_T).  The card's name and power limit are part of the JSON line.
+    python tools/bench_train.py [--steps 10 --warmup 3 --batch 32 --net 1 --shape 180,210 --reserve 256,256]
     python -m torch.distributed.run --nproc-per-node N --master-addr 127.0.0.1 tools/bench_train.py"""
 import argparse
 import json
 import os
+import subprocess
 import sys
+import time
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -24,6 +28,7 @@ ap.add_argument("--batch", type=int, default=32)
 ap.add_argument("--probe", type=int, default=0, help="measurement only: 1 = the wgmma GEMMs fetch their operands but issue no MMA (results are garbage)")
 ap.add_argument("--net", type=int, default=1, choices=[1, 2], help="1 = Text2Mel trainer (BASELINE config 5), 2 = SSRN trainer (train.py num=2) at T = 210")
 ap.add_argument("--shape", default="%d,%d" % (hp.max_N, hp.max_T), help="N,T of every step's batch (text positions, mel frames); SSRN uses T")
+ap.add_argument("--reserve", default=None, help="N,T: grow the training workspace to this capacity after init (SSRN uses T)")
 ap.add_argument("--train-tc", type=int, default=7, help="bit mask: 1 forward conv, 2 data gradient, 4 weight gradient on wgmma (default 7 = all), 0 = fp32 CUDA-core kernels")
 a = ap.parse_args()
 N, T = (int(x) for x in a.shape.split(","))
@@ -40,6 +45,23 @@ if a.net == 1:
     eng.train_init(B)
 else:
     eng.train_init_ssrn(B, hp.max_T)
+reserve_ms = None
+if a.reserve:
+    RN, RT = (int(x) for x in a.reserve.split(","))
+    torch.cuda.synchronize()
+    w0 = time.perf_counter()
+    eng.train_reserve(RN, RT)                       # synchronises the device when it grows
+    reserve_ms = (time.perf_counter() - w0) * 1e3
+
+
+def card():
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", str(local)],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        return out or torch.cuda.get_device_name()
+    except (OSError, subprocess.SubprocessError):
+        return torch.cuda.get_device_name() + ", power limit unknown"
+
 L = torch.from_numpy(synthetic_text(B, min(100, N - 1), seed=rank)[:, :N]).cuda()
 mels = torch.from_numpy(np.random.default_rng(rank).uniform(0, 1, (B, T, hp.n_mels)).astype(np.float32)).cuda()
 mags = torch.from_numpy(np.random.default_rng(rank + 100).uniform(0, 1, (B, T * hp.r, 1 + hp.n_fft // 2)).astype(np.float32)).cuda() if a.net == 2 else None
@@ -80,6 +102,7 @@ if rank == 0:
         flops = 3 * 2 * B * T * 93.66e6                                                          # SSRN: 93.7 MMAC per mel frame
     print(json.dumps({"metric": "train_steps_per_sec", "value": 1e3 / ms, "unit": "steps/s", "n_gpus": world, "ms_per_step": ms,
                       "mel_frames_per_sec": world * B * T * 1e3 / ms, "steps": a.steps, "warmup": a.warmup, "shape": {"N": N, "T": T},
+                      "capacity": dict(zip(("N", "T"), eng.train_capacity())), "reserve_ms": reserve_ms, "device": card(),
                       "config": {"workload": ("Text2Mel train step (fwd + bwd + clip + Adam), B=%d per GPU, N=%d, T=%d, dropout %.2f" % (B, N, T, hp.dropout_rate)
                                               if a.net == 1 else
                                               "SSRN train step (train.py num=2: fwd + bwd + clip + Adam), B=%d per GPU, T=%d -> %d frames x 1025 bins, dropout %.2f"

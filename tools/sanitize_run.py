@@ -1,7 +1,9 @@
 """Small workload for compute-sanitizer (memcheck / racecheck / synccheck; SURVEY section 5, VERDICT r1 item 8): one
 block of every wgmma block-kernel variant (two-stage and deeper rings, transposed conv, a narrow conv), the wgmma
 attention, and a few frames of both decode loops with a window move.
-   compute-sanitizer --tool memcheck python tools/sanitize_run.py [what ...]      what: blocks attention decode graph train"""
+   compute-sanitizer --tool memcheck python tools/sanitize_run.py [what ...]      what: blocks attention decode graph train overcap
+"overcap": one Text2Mel step past (max_N, max_T) on a grown workspace per training kernel set (train_tc 7 and 0): the
+guided-attention table is read only inside its (max_N, max_T) corner."""
 import os
 import sys
 
@@ -10,7 +12,7 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 from dc_tts_b200.engine import Engine  # noqa: E402
 from dc_tts_b200.hyperparams import Hyperparams as hp  # noqa: E402
-from dc_tts_b200.params import init_params, synthetic_text  # noqa: E402
+from dc_tts_b200.params import init_params, synthetic_bucket, synthetic_text  # noqa: E402
 
 what = set(sys.argv[1:]) or {"blocks", "attention", "decode", "graph"}
 e = Engine(0)
@@ -49,3 +51,14 @@ if "train" in what:
     mels = rng.uniform(0, 1, (2, hp.max_T, hp.n_mels)).astype(np.float32)
     out = t.train_step(synthetic_text(2, 60, seed=1), mels, global_step=7, seed=1)
     torch.cuda.synchronize(); print("train step ok", out, flush=True)
+if "overcap" in what:
+    for tc in (7, 0):
+        t = Engine(0)
+        t.load_params(init_params(0))
+        t.set_option("train_tc", tc)
+        t.train_init(2)
+        t.train_reserve(256, 256)
+        Lb, mels = synthetic_bucket(2, 200, 240, seed=1)
+        out = t.train_step(Lb, mels, global_step=7, seed=1)
+        torch.cuda.synchronize(); print("over-capacity train step ok, train_tc", tc, out, flush=True)
+        t.close()
