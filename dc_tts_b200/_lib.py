@@ -44,7 +44,8 @@ SIGNATURES = {
                                     C.POINTER(_i32), _p]),
     "dctts_conv_gemm": (C.c_int, [Handle, _i32, _i32, _p, _i32, _i32, _i32, _i32, _p, _i32, _i32, _i32, C.POINTER(_i32), _p,
                                   _i32, _p, _i32, _p]),
-    "dctts_set_vocoder_params": (C.c_int, [Handle, _i32, _i32, C.c_float, C.c_float, C.c_float, C.c_float, _i32]),
+    "dctts_vocoder_stage": (C.c_int, [Handle, _i32, _i32, _i32, _p, _p, _p, C.POINTER(_i32), _p]),
+    "dctts_set_vocoder_params": (C.c_int, [Handle, _i32, _i32, C.c_float, C.c_float, C.c_float, C.c_double, _i32]),
     "dctts_spectrogram2wav": (C.c_int, [Handle, _p, _i32, _i32, _i32, _p, _p, _p]),
     "dctts_get_spectrograms": (C.c_int, [Handle, _p, _i64, _i32, _p, _p, _i32, C.POINTER(_i32), C.POINTER(_i32), _p]),
     "dctts_load_spectrograms_batch": (C.c_int, [Handle, _p, _i32, C.POINTER(_i64), _i32, _i32, _p, _p, _i32, C.POINTER(_i32),

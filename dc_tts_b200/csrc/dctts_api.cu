@@ -151,7 +151,7 @@ struct dctts_handle_s {
     } tr;
 
     // vocoder (Griffin-Lim) state
-    struct { int hop = 275, win = 1102, n_iter = 50; float power = 1.5f, max_db = 100.f, ref_db = 20.f, preemph = 0.97f; } voc;
+    struct { int hop = 275, win = 1102, n_iter = 50; float power = 1.5f, max_db = 100.f, ref_db = 20.f; double preemph = 0.97; } voc;
     DevBuf feat_melw, feat_range, feat_tw, feat_window, feat_wss;   // feature extraction tables (dctts_get_spectrograms)
     DevBuf feat_seg;                                                // per-utterance segment tables of a feature batch
     DevBuf rs_win, rs_tab;                                          // resampling: kaiser_best filter, per-call tables
@@ -1723,7 +1723,7 @@ void feat_batch(H* h, const char* who, const void* wav, int dtype, const int64_t
     a.mag = mag; a.mel = mel; a.mag_rows = r * T_b; a.mel_rows = T_b; a.r = r;
     a.melw = h->feat_melw.as<float>(); a.melrange = h->feat_range.as<int>(); a.tw = h->feat_tw.as<float2>();
     a.window = h->feat_window.as<float>(); a.F = F; a.n_mels = n_mels; a.win = h->voc.win; a.hop = hop;
-    a.preemph = h->voc.preemph; a.ref_db = h->voc.ref_db; a.max_db = h->voc.max_db;
+    a.preemph = (float)h->voc.preemph; a.ref_db = h->voc.ref_db; a.max_db = h->voc.max_db;
     feat_run(a, s);
     h->launches += 1;
     CUDA_CHECK(cudaGetLastError());
@@ -2078,7 +2078,7 @@ int dctts_conv_gemm(dctts_handle h, int32_t impl, int32_t mode, const float* X, 
 }
 
 int dctts_set_vocoder_params(dctts_handle h, int32_t hop_length, int32_t win_length, float power, float max_db,
-                             float ref_db, float preemphasis, int32_t n_iter) {
+                             float ref_db, double preemphasis, int32_t n_iter) {
     return guarded(h, [&] {
         REQUIRE(hop_length >= 1 && win_length >= 1 && win_length <= 2048 && n_iter >= 0, "dctts_set_vocoder_params: bad arguments");
         h->voc.hop = hop_length; h->voc.win = win_length; h->voc.power = power; h->voc.max_db = max_db;
@@ -2086,39 +2086,86 @@ int dctts_set_vocoder_params(dctts_handle h, int32_t hop_length, int32_t win_len
     });
 }
 
+namespace {
+// The handle's vocoder buffers and tables sized for (B, T) and its parameters; the caller sets mag, wav and n_iter.
+VocoderArgs voc_args(H* h, const char* fn, int B, int T, cudaStream_t s) {
+    REQUIRE(B >= 1 && T >= 2, std::string(fn) + ": need B >= 1 and T >= 2 frames, got B = " + std::to_string(B) + ", T = " +
+                              std::to_string(T));
+    REQUIRE(h->F == 1025, std::string(fn) + ": the FFT kernel is built for n_fft = 2048");
+    const int F = h->F, win = h->voc.win, hop = h->voc.hop, Ly = hop * (T - 1), nfr = 1 + Ly / 512;
+    const size_t n = (size_t)B * T * F;
+    h->voc_S.ensure(n * sizeof(float)); h->voc_X.ensure(n * sizeof(float2));
+    h->voc_frames.ensure((size_t)B * T * win * sizeof(float)); h->voc_mse.ensure((size_t)B * nfr * sizeof(float));
+    h->voc_deemph.ensure(voc_deemph_scratch_bytes(B, T, hop));
+    if (h->voc_tables_T != T || h->voc_tables_win != win || h->voc_tables_hop != hop) {
+        h->voc_tw.ensure(2048 * sizeof(float2)); h->voc_window.ensure(win * sizeof(float));
+        h->voc_wss.ensure((size_t)(2048 + hop * (T - 1)) * sizeof(float));
+        voc_make_tables(h->voc_tw.as<float2>(), h->voc_window.as<float>(), h->voc_wss.as<float>(), T, win, hop, s);
+        CUDA_CHECK(cudaGetLastError());
+        h->voc_tables_T = T; h->voc_tables_win = win; h->voc_tables_hop = hop;
+    }
+    VocoderArgs a{};
+    a.S = h->voc_S.as<float>(); a.X = h->voc_X.as<float2>(); a.frames = h->voc_frames.as<float>();
+    a.mse = h->voc_mse.as<float>(); a.tw = h->voc_tw.as<float2>(); a.window = h->voc_window.as<float>();
+    a.wss = h->voc_wss.as<float>(); a.deemph = h->voc_deemph.as<double>(); a.B = B; a.T = T; a.F = F; a.win = win; a.hop = hop;
+    a.n_iter = h->voc.n_iter;
+    a.max_db = h->voc.max_db; a.ref_db = h->voc.ref_db; a.power = h->voc.power; a.preemphasis = h->voc.preemph;
+    return a;
+}
+
+// librosa.effects.trim from the device frame energies a.mse (B, 1 + Ly / 512): frames within 60 dB of the loudest.
+// Synchronises s.
+void voc_trims(const VocoderArgs& a, int32_t* trim_host, cudaStream_t s) {
+    const int Ly = a.hop * (a.T - 1), nfr = 1 + Ly / 512;
+    std::vector<float> mse((size_t)a.B * nfr);
+    CUDA_CHECK(cudaMemcpyAsync(mse.data(), a.mse, mse.size() * sizeof(float), cudaMemcpyDeviceToHost, s));
+    CUDA_CHECK(cudaStreamSynchronize(s));
+    if (trim_host)
+        for (int b = 0; b < a.B; ++b) trim_from_mse(mse.data() + (size_t)b * nfr, nfr, Ly, trim_host + 2 * b);
+}
+}  // namespace
+
 int dctts_spectrogram2wav(dctts_handle h, const float* mag, int32_t B, int32_t T, int32_t n_iter, float* wav,
                           int32_t* trim_host, void* stream) {
     return guarded(h, [&] {
-        REQUIRE(mag && wav && B >= 1 && T >= 2, "dctts_spectrogram2wav: bad arguments");
-        REQUIRE(h->F == 1025, "dctts_spectrogram2wav: the FFT kernel is built for n_fft = 2048");
+        REQUIRE(mag && wav, "dctts_spectrogram2wav: bad arguments");
         cudaStream_t s = S(h, stream);
-        const int F = h->F, win = h->voc.win, hop = h->voc.hop, Ly = hop * (T - 1), nfr = 1 + Ly / 512;
-        const size_t n = (size_t)B * T * F;
-        h->voc_S.ensure(n * sizeof(float)); h->voc_X.ensure(n * sizeof(float2));
-        h->voc_frames.ensure((size_t)B * T * win * sizeof(float)); h->voc_mse.ensure((size_t)B * nfr * sizeof(float));
-        h->voc_deemph.ensure(voc_deemph_scratch_bytes(B, T, hop));
-        if (h->voc_tables_T != T || h->voc_tables_win != win || h->voc_tables_hop != hop) {
-            h->voc_tw.ensure(2048 * sizeof(float2)); h->voc_window.ensure(win * sizeof(float));
-            h->voc_wss.ensure((size_t)(2048 + hop * (T - 1)) * sizeof(float));
-            voc_make_tables(h->voc_tw.as<float2>(), h->voc_window.as<float>(), h->voc_wss.as<float>(), T, win, hop, s);
-            CUDA_CHECK(cudaGetLastError());
-            h->voc_tables_T = T; h->voc_tables_win = win; h->voc_tables_hop = hop;
-        }
-        VocoderArgs a{};
-        a.mag = mag; a.S = h->voc_S.as<float>(); a.X = h->voc_X.as<float2>(); a.frames = h->voc_frames.as<float>();
-        a.wav = wav; a.mse = h->voc_mse.as<float>(); a.tw = h->voc_tw.as<float2>(); a.window = h->voc_window.as<float>();
-        a.wss = h->voc_wss.as<float>(); a.deemph = h->voc_deemph.as<double>(); a.B = B; a.T = T; a.F = F; a.win = win; a.hop = hop;
-        a.n_iter = n_iter < 0 ? h->voc.n_iter : n_iter;
-        a.max_db = h->voc.max_db; a.ref_db = h->voc.ref_db; a.power = h->voc.power; a.preemphasis = h->voc.preemph;
+        VocoderArgs a = voc_args(h, "dctts_spectrogram2wav", B, T, s);
+        a.mag = mag; a.wav = wav;
+        if (n_iter >= 0) a.n_iter = n_iter;
         voc_run(a, s);
         h->launches += voc_launches_per_call(a.n_iter);
         CUDA_CHECK(cudaGetLastError());
-        // librosa.effects.trim: frames whose energy is within 60 dB of the loudest
-        std::vector<float> mse((size_t)B * nfr);
-        CUDA_CHECK(cudaMemcpyAsync(mse.data(), a.mse, mse.size() * sizeof(float), cudaMemcpyDeviceToHost, s));
-        CUDA_CHECK(cudaStreamSynchronize(s));
-        if (trim_host)
-            for (int b = 0; b < B; ++b) trim_from_mse(mse.data() + (size_t)b * nfr, nfr, Ly, trim_host + 2 * b);
+        voc_trims(a, trim_host, s);
+    });
+}
+
+int dctts_vocoder_stage(dctts_handle h, int32_t stage, int32_t B, int32_t T, const void* in, const float* S_in, void* out,
+                        int32_t* trim_host, void* stream) {
+    return guarded(h, [&] {
+        const std::string fn = "dctts_vocoder_stage";
+        REQUIRE(stage >= 0 && stage <= 4, fn + ": stage " + std::to_string(stage) +
+                                          " is not one of 0 prepare, 1 istft, 2 stft_phase, 3 deemph, 4 energies");
+        REQUIRE(in && out, fn + ": in and out are required");
+        REQUIRE(stage != 2 || S_in, fn + ": stage 2 (stft_phase) needs S (B, T, F)");
+        REQUIRE(stage != 3 || in == out, fn + ": stage 3 (deemph) works in place: in must equal out");
+        cudaStream_t s = S(h, stream);
+        VocoderArgs a = voc_args(h, fn.c_str(), B, T, s);
+        static const int launches[5] = {1, 2, 1, 3, 1};
+        switch (stage) {
+            case 0: a.mag = static_cast<const float*>(in); a.X = static_cast<float2*>(out); voc_prepare(a, s); break;
+            case 1: a.X = static_cast<float2*>(const_cast<void*>(in)); a.wav = static_cast<float*>(out); voc_istft(a, s); break;
+            case 2:
+                a.wav = static_cast<float*>(const_cast<void*>(in)); a.S = const_cast<float*>(S_in); a.X = static_cast<float2*>(out);
+                voc_stft_phase(a, s);
+                break;
+            case 3: a.wav = static_cast<float*>(out); voc_deemph(a, s); break;
+            case 4: a.wav = static_cast<float*>(const_cast<void*>(in)); a.mse = static_cast<float*>(out); voc_energies(a, s); break;
+        }
+        h->launches += launches[stage];
+        CUDA_CHECK(cudaGetLastError());
+        if (stage == 4) voc_trims(a, trim_host, s);
+        else CUDA_CHECK(cudaStreamSynchronize(s));
     });
 }
 

@@ -124,9 +124,16 @@ struct VocoderArgs {
     const float2* tw; const float* window; const float* wss;
     double* deemph;                // (B, chunks) float64 states of the de-pre-emphasis recurrence
     int B, T, F, win, hop, n_iter;
-    float max_db, ref_db, power, preemphasis;
+    float max_db, ref_db, power;
+    double preemphasis;            // float64 like the reference's scipy.signal.lfilter([1], [1, -hp.preemphasis], wav)
 };
 void voc_make_tables(float2* tw_dev, float* window_dev, float* wss_dev, int T, int win, int hop, cudaStream_t s);
+// voc_run = voc_prepare, (voc_istft, voc_stft_phase) x n_iter, voc_istft, voc_deemph, voc_energies
+void voc_prepare(const VocoderArgs& a, cudaStream_t s);      // mag -> S, X = S (zero phase); 1 launch
+void voc_istft(const VocoderArgs& a, cudaStream_t s);        // X -> frames -> wav; 2 launches
+void voc_stft_phase(const VocoderArgs& a, cudaStream_t s);   // wav, S -> X; 1 launch
+void voc_deemph(const VocoderArgs& a, cudaStream_t s);       // wav in place, deemph scratch; 3 launches
+void voc_energies(const VocoderArgs& a, cudaStream_t s);     // wav -> mse; 1 launch
 void voc_run(const VocoderArgs& a, cudaStream_t s);
 int voc_launches_per_call(int n_iter);
 size_t voc_deemph_scratch_bytes(int B, int T, int hop);

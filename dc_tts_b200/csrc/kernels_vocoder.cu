@@ -28,6 +28,20 @@ constexpr int VC_H = VC_N / 2;                      // complex FFT length (real-
 
 __device__ __forceinline__ float2 cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
 
+// Index into [0, len) of sample u of np.pad(y, p, mode='reflect') at any pad length p (u < 0 lies in the left pad,
+// u >= len in the right one).  A pad longer than the signal is reflected again and again, so the padded signal is
+// periodic with period 2 (len - 1); numpy repeats the single sample of a signal of length 1.
+__device__ __forceinline__ int reflect_index(int u, int len) {
+    if (len == 1) return 0;
+    const int period = 2 * (len - 1);
+    if (u < 0) u = -u;
+    if (u >= len) {
+        u %= period;
+        if (u >= len) u = period - u;
+    }
+    return u;
+}
+
 // 1024-point complex FFT, Stockham autosort, radix 4, 256 threads, one butterfly per thread per pass.
 // Entry: v[k] = x[tid + 256 k]; exit: v[k] = X[tid + 256 k] (natural order, no scaling).  The first
 // pass reads and the last pass writes registers only; the three passes between go through the two
@@ -148,9 +162,7 @@ __global__ void __launch_bounds__(VC_THREADS) voc_stft_phase_kernel(const float*
     auto sample = [&](int n) -> float {
         const int m = n - lpad;
         if (m < 0 || m >= win) return 0.f;
-        int u = t * hop + n - VC_N / 2;                   // np.pad(y, n_fft//2, mode='reflect')
-        if (u < 0) u = -u;
-        if (u >= Ly) u = 2 * (Ly - 1) - u;
+        const int u = reflect_index(t * hop + n - VC_N / 2, Ly);   // np.pad(y, n_fft//2, mode='reflect')
         return yb[u] * window[m];
     };
     float2 v[4];
@@ -222,20 +234,12 @@ __device__ __forceinline__ float wav_sample(const float* __restrict__ y, long lo
 __device__ __forceinline__ float wav_sample(const int16_t* __restrict__ y, long long i) { return (float)y[i] * (1.0f / 32768.0f); }
 
 // librosa.feature.rmse(y, flen, fhop)**2 of centred frame f (reflect padding) of the signal yb[0, Ly), Ly >= 2.  256
-// threads; the result is valid in thread 0.  A signal shorter than the padding is reflected again and again, as
-// np.pad(mode='reflect') does: the padded signal is periodic with period 2 (Ly - 1).
+// threads; the result is valid in thread 0.
 template <typename In>
 __device__ __forceinline__ float frame_mse(const In* __restrict__ yb, int Ly, int f, int flen, int fhop, float* red) {
-    const int period = 2 * (Ly - 1);
     float acc = 0.f;
     for (int n = threadIdx.x; n < flen; n += 256) {
-        int u = f * fhop + n - flen / 2;
-        if (u < 0) u = -u;
-        if (u >= Ly) {
-            u %= period;
-            if (u >= Ly) u = period - u;
-        }
-        const float v = wav_sample(yb, u);
+        const float v = wav_sample(yb, reflect_index(f * fhop + n - flen / 2, Ly));
         acc = fmaf(v, v, acc);
     }
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
@@ -301,10 +305,7 @@ __global__ void __launch_bounds__(VC_THREADS) feat_stft_mel_kernel(const In* __r
     auto sample = [&](int n) -> float {
         const int m = n - lpad;
         if (m < 0 || m >= win) return 0.f;
-        int u = t * hop + n - VC_N / 2;                   // np.pad(y, n_fft//2, mode='reflect')
-        if (u < 0) u = -u;
-        if (u >= len) u = 2 * (len - 1) - u;
-        u = min(max(u, 0), len - 1);
+        const int u = reflect_index(t * hop + n - VC_N / 2, len);  // np.pad(y, n_fft//2, mode='reflect')
         const float v = (u > 0) ? __fsub_rn(wav_sample(y, u), __fmul_rn(preemph, wav_sample(y, u - 1))) : wav_sample(y, 0);   // utils.py:39
         return v * window[m];
     };
@@ -559,24 +560,44 @@ void resample_run(const void* wav, int dtype, const ResampleUtt* utt, int B, con
 int voc_launches_per_call(int n_iter) { return 1 + 3 * n_iter + 2 + 3 + 1; }
 size_t voc_deemph_scratch_bytes(int B, int T, int hop) { return (size_t)B * ((hop * (T - 1) + DE_LC - 1) / DE_LC) * sizeof(double); }
 
-void voc_run(const VocoderArgs& a, cudaStream_t s) {
-    const int T = a.T, F = a.F, B = a.B, win = a.win, hop = a.hop, Ly = hop * (T - 1), lpad = (VC_N - win) / 2;
-    const long long n = (long long)B * T * F;
+// The stages of voc_run, each a fixed sequence of launches (dctts_vocoder_stage runs them one at a time).
+void voc_prepare(const VocoderArgs& a, cudaStream_t s) {
+    const long long n = (long long)a.B * a.T * a.F;
     voc_prepare_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a.mag, a.S, a.X, n, a.max_db, a.ref_db, a.power);
-    dim3 gframes(T, B), gsamp((Ly + 255) / 256, B);
+}
+
+void voc_istft(const VocoderArgs& a, cudaStream_t s) {
+    const int Ly = a.hop * (a.T - 1), lpad = (VC_N - a.win) / 2;
+    voc_istft_kernel<<<dim3(a.T, a.B), VC_THREADS, 0, s>>>(a.X, a.frames, a.tw, a.window, a.T, a.F, a.win, lpad);
+    voc_ola_kernel<<<dim3((Ly + 255) / 256, a.B), 256, 0, s>>>(a.frames, a.wss, a.wav, a.T, a.win, lpad, a.hop, Ly, 1.17549435e-38f);
+}
+
+void voc_stft_phase(const VocoderArgs& a, cudaStream_t s) {
+    const int Ly = a.hop * (a.T - 1), lpad = (VC_N - a.win) / 2;
+    voc_stft_phase_kernel<<<dim3(a.T, a.B), VC_THREADS, 0, s>>>(a.wav, a.S, a.X, a.tw, a.window, a.T, a.F, a.win, lpad, a.hop, Ly);
+}
+
+void voc_deemph(const VocoderArgs& a, cudaStream_t s) {
+    const int Ly = a.hop * (a.T - 1), nch = (Ly + DE_LC - 1) / DE_LC;
+    const dim3 gch((nch + 63) / 64, a.B);
+    voc_deemph_local_kernel<<<gch, 64, 0, s>>>(a.wav, a.deemph, Ly, nch, a.preemphasis);
+    voc_deemph_carry_kernel<<<(a.B + 31) / 32, 32, 0, s>>>(a.deemph, nch, a.B, a.preemphasis);
+    voc_deemph_apply_kernel<<<gch, 64, 0, s>>>(a.wav, a.deemph, Ly, nch, a.preemphasis);
+}
+
+void voc_energies(const VocoderArgs& a, cudaStream_t s) {
+    const int Ly = a.hop * (a.T - 1), nfr = 1 + Ly / 512;
+    voc_frame_mse_kernel<<<dim3(nfr, a.B), 256, 0, s>>>(a.wav, a.mse, Ly, nfr, 2048, 512);
+}
+
+void voc_run(const VocoderArgs& a, cudaStream_t s) {
+    voc_prepare(a, s);
     for (int it = 0; it <= a.n_iter; ++it) {
-        voc_istft_kernel<<<gframes, VC_THREADS, 0, s>>>(a.X, a.frames, a.tw, a.window, T, F, win, lpad);
-        voc_ola_kernel<<<gsamp, 256, 0, s>>>(a.frames, a.wss, a.wav, T, win, lpad, hop, Ly, 1.17549435e-38f);
-        if (it < a.n_iter)
-            voc_stft_phase_kernel<<<gframes, VC_THREADS, 0, s>>>(a.wav, a.S, a.X, a.tw, a.window, T, F, win, lpad, hop, Ly);
+        voc_istft(a, s);
+        if (it < a.n_iter) voc_stft_phase(a, s);
     }
-    const int nch = (Ly + DE_LC - 1) / DE_LC;
-    const dim3 gch((nch + 63) / 64, B);
-    voc_deemph_local_kernel<<<gch, 64, 0, s>>>(a.wav, a.deemph, Ly, nch, (double)a.preemphasis);
-    voc_deemph_carry_kernel<<<(B + 31) / 32, 32, 0, s>>>(a.deemph, nch, B, (double)a.preemphasis);
-    voc_deemph_apply_kernel<<<gch, 64, 0, s>>>(a.wav, a.deemph, Ly, nch, (double)a.preemphasis);
-    const int nfr = 1 + Ly / 512;
-    voc_frame_mse_kernel<<<dim3(nfr, B), 256, 0, s>>>(a.wav, a.mse, Ly, nfr, 2048, 512);
+    voc_deemph(a, s);
+    voc_energies(a, s);
 }
 
 }  // namespace dctts

@@ -293,6 +293,48 @@ class Engine:
                                                     trim.ctypes.data_as(C.c_void_p), self._stream()), "dctts_spectrogram2wav")
         return wav, trim
 
+    def vocoder_stage(self, stage, x, out, S=None, hop=None, win=None, power=None):
+        """Test aid (include/dctts.h: dctts_vocoder_stage): ONE stage of spectrogram2wav on caller CUDA tensors, with the
+        hyperparameters' vocoder constants except `hop`, `win` and `power` when given.  Ly = hop (T - 1), F = 1025:
+          0 prepare     x = mag (B, T, F) float32                -> out = X (B, T, F) complex64
+          1 istft       x = X (B, T, F) complex64                -> out = wav (B, Ly) float32
+          2 stft_phase  x = wav (B, Ly), S = (B, T, F) float32   -> out = X (B, T, F) complex64
+          3 deemph      x = out = wav (B, Ly), in place
+          4 energies    x = wav (B, Ly)                          -> out = mse (B, 1 + Ly // 512) float32
+        Tensors must be contiguous (they may be views into larger buffers).  Returns the trims (B, 2) int32 numpy for
+        stage 4 (as spectrogram2wav reports them), else out."""
+        h = self.hp
+        hop = int(hop or h.hop_length)
+        win = int(win or h.win_length)
+        power = float(h.power if power is None else power)
+        self._check(self._lib.dctts_set_vocoder_params(self._h, hop, win, power, float(h.max_db), float(h.ref_db),
+                                                       float(h.preemphasis), int(h.n_iter)), "dctts_set_vocoder_params")
+        f32, c64 = torch.float32, torch.complex64
+        B = x.shape[0]
+        if stage in (0, 1):
+            T = x.shape[1]
+        elif stage == 2:
+            if S is None or S.dim() != 3:
+                raise DcttsError("vocoder_stage: stage 2 (stft_phase) needs S (B, T, F)")
+            T = S.shape[1]
+        else:
+            T = x.shape[1] // hop + 1
+        Ly, F = hop * (T - 1), self.F
+        want = {0: [(x, (B, T, F), f32), (out, (B, T, F), c64)],
+                1: [(x, (B, T, F), c64), (out, (B, Ly), f32)],
+                2: [(x, (B, Ly), f32), (S, (B, T, F), f32), (out, (B, T, F), c64)],
+                3: [(x, (B, Ly), f32), (out, (B, Ly), f32)],
+                4: [(x, (B, Ly), f32), (out, (B, 1 + Ly // 512), f32)]}.get(stage, [])
+        for t, shape, dt in want:
+            if tuple(t.shape) != shape or t.dtype != dt or not t.is_cuda or not t.is_contiguous():
+                raise DcttsError("vocoder_stage %d: expected a contiguous CUDA %s tensor of shape %s, got %s %s" %
+                                 (stage, dt, shape, t.dtype, tuple(t.shape)))
+        trim = np.zeros((B, 2), np.int32)
+        self._check(self._lib.dctts_vocoder_stage(self._h, int(stage), B, T, _ptr(x), _ptr(S), _ptr(out),
+                                                  trim.ctypes.data_as(C.POINTER(C.c_int32)), self._stream()),
+                    "dctts_vocoder_stage")
+        return trim if stage == 4 else out
+
     def get_spectrograms(self, wav, sr=None):
         """utils.py:20-65 from a loaded waveform (1-D float32, hp.sr): -> (mel (T, n_mels), mag (T, F)) CUDA tensors and
         the [start, end) sample range librosa.effects.trim keeps."""

@@ -127,9 +127,11 @@ int dctts_synthesize_host(dctts_handle h, const int32_t* L_host, int32_t B,
 
 /* ---- vocoder ("next" row after the path: reference utils.py:67-114) --------------------- */
 /* Signal-processing constants of hyperparams.py:13-24 (defaults = the LJ values: hop 275, win 1102, power 1.5,
- * max_db 100, ref_db 20, preemphasis 0.97, n_iter 50; n_fft is fixed at 2048 = 2*(F-1)). */
+ * max_db 100, ref_db 20, preemphasis 0.97, n_iter 50; n_fft is fixed at 2048 = 2*(F-1)).  preemphasis is float64:
+ * the de-pre-emphasis filter runs with it as scipy.signal.lfilter does; the features' pre-emphasis rounds it to float32
+ * as numpy does for a float32 waveform. */
 int dctts_set_vocoder_params(dctts_handle h, int32_t hop_length, int32_t win_length, float power, float max_db,
-                             float ref_db, float preemphasis, int32_t n_iter);
+                             float ref_db, double preemphasis, int32_t n_iter);
 /* spectrogram2wav (utils.py:67-94) for a batch, entirely on the device: mag (B, T, F) normalised linear
  * magnitudes -> de-normalise, ^power, Griffin-Lim (n_iter x istft/stft with librosa's conventions), de-pre-emphasis.
  * wav (B, hop*(T-1)) DEVICE float32 receives the UNTRIMMED waveform; trim_host (B, 2) HOST int32 receives the
@@ -295,6 +297,18 @@ int dctts_bench_block(dctts_handle h, const char* scope, int32_t B, int32_t L, i
 int dctts_conv_gemm(dctts_handle h, int32_t impl, int32_t mode, const float* X, int32_t ldx, int32_t B, int32_t L, int32_t K,
                     const float* Wd, int32_t ldwd, int32_t N, int32_t ntaps, const int32_t* shifts_host, const float* bias,
                     int32_t accumulate, float* out, int32_t ldo, void* stream);
+/* Test aid: ONE stage of dctts_spectrogram2wav on caller DEVICE tensors, through the launch functions the product calls,
+ * with the handle's vocoder parameters and the tables (twiddles, window, window sum-square) it builds for (T, win, hop).
+ * Ly = hop (T - 1), nfr = 1 + Ly / 512, F = 1025.
+ *   0 prepare:    in = mag (B,T,F) float32            -> out = X (B,T,F) complex64  (S = Re X, zero phase)
+ *   1 istft:      in = X (B,T,F) complex64            -> out = wav (B,Ly) float32
+ *   2 stft_phase: in = wav (B,Ly), S (B,T,F) float32  -> out = X (B,T,F) complex64
+ *   3 deemph:     in = out = wav (B,Ly), in place
+ *   4 energies:   in = wav (B,Ly)                     -> out = mse (B,nfr) float32; trim_host (B,2) HOST int32 (optional)
+ *                 receives the [start, end) ranges dctts_spectrogram2wav would report for this waveform.
+ * Fails with a message on a bad stage or shape.  Synchronises `stream`. */
+int dctts_vocoder_stage(dctts_handle h, int32_t stage, int32_t B, int32_t T, const void* in, const float* S, void* out,
+                        int32_t* trim_host, void* stream);
 /* Raw device memory helpers so that a host without torch can drive the library. */
 int dctts_malloc(dctts_handle h, void** ptr, int64_t bytes);
 int dctts_free(dctts_handle h, void* ptr);
