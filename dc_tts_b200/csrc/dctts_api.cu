@@ -158,6 +158,10 @@ struct dctts_handle_s {
     int feat_sr = 0, feat_win = 0;
     DevBuf voc_S, voc_X, voc_frames, voc_mse, voc_tw, voc_window, voc_wss, voc_deemph;
     int voc_tables_T = 0, voc_tables_win = 0, voc_tables_hop = 0;
+    // co-resident 16-CTA clusters of the 144-column block kernel (the F = 2049 conv1d blocks), -1 until first needed;
+    // when none fits, why those blocks run on the fp32 kernels
+    int tc16_clusters = -1;
+    std::string tc16_why;
 
     // AR decode graph
     cudaGraphExec_t ar_exec = nullptr;
@@ -329,7 +333,15 @@ void pack_tc(H* h, LayerDev& l, const std::vector<float>& W /* [size][cin][ldw] 
         p.half = (l.cout <= 256) ? 32 : 128; p.bn = 2 * p.half; p.ncta = l.cout / p.half;   // decode nets: 8 narrow CTAs per tile
         if (l.cout % p.half) return;
     }
-    if (p.ncta > 8) return;
+    if (p.ncta > 8) {
+        // the F = 2049 conv1d blocks: a 16-CTA cluster of the 144-column kernel, if one can be co-resident on this device
+        if (p.mode != 0 || p.ncta > 16 || p.bn != 144) return;
+        if (h->tc16_clusters < 0) {
+            h->tc16_clusters = conv_ln_tc_max_clusters(16, 144, tc_bk());
+            if (h->tc16_clusters < 1) h->tc16_why = "a 16-CTA cluster of the 144-column block kernel cannot be scheduled on this device";
+        }
+        if (h->tc16_clusters < 1) return;
+    }
     p.Ktot = p.ntaps * cin_pad; p.nrows = p.ncta * p.bn;
     auto wv = [&](int tap, int ci, int row) -> float {
         const int i = row / p.bn, a = row % p.bn;
@@ -1624,6 +1636,14 @@ void train_apply(H* h, long long global_step, float lr, cudaStream_t s) {
     CUDA_CHECK(cudaGetLastError());
 }
 
+// The STFT kernels exist for n_fft 1024, 2048 and 4096 (F = 513, 1025, 2049)
+void require_fft_size(const H* h, const std::string& fn) {
+    const int n_fft = 2 * (h->F - 1);
+    REQUIRE(voc_fft_size_ok(n_fft), fn + ": n_fft = " + std::to_string(n_fft) + " has no STFT kernel (supported: 1024, 2048, 4096)");
+    REQUIRE(h->voc.win <= n_fft, fn + ": win_length " + std::to_string(h->voc.win) + " exceeds n_fft = " + std::to_string(n_fft) +
+                                 " (dctts_set_vocoder_params)");
+}
+
 // librosa.effects.trim(y)[1] from the per-frame mean squares: frames within 60 dB of the loudest one
 void trim_from_mse(const float* m, int nfr, int Ly, int32_t* out) {
     float mx = 0.f;
@@ -1645,10 +1665,11 @@ void feat_tables(H* h, int sample_rate, cudaStream_t s) {
     std::vector<float> w; std::vector<int> range;
     feat_make_mel_basis(sample_rate, h->hp.n_fft, h->hp.n_mels, w, range);
     h->feat_melw.ensure(w.size() * sizeof(float)); h->feat_range.ensure(range.size() * sizeof(int));
-    h->feat_tw.ensure(2048 * sizeof(float2)); h->feat_window.ensure(win * sizeof(float)); h->feat_wss.ensure(2048 * sizeof(float));
+    const int n_fft = 2 * (h->F - 1);
+    h->feat_tw.ensure(n_fft * sizeof(float2)); h->feat_window.ensure(win * sizeof(float)); h->feat_wss.ensure(n_fft * sizeof(float));
     CUDA_CHECK(cudaMemcpyAsync(h->feat_melw.p, w.data(), w.size() * sizeof(float), cudaMemcpyHostToDevice, s));
     CUDA_CHECK(cudaMemcpyAsync(h->feat_range.p, range.data(), range.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-    voc_make_tables(h->feat_tw.as<float2>(), h->feat_window.as<float>(), h->feat_wss.as<float>(), 1, win, hop, s);   // synchronises
+    voc_make_tables(n_fft, h->feat_tw.as<float2>(), h->feat_window.as<float>(), h->feat_wss.as<float>(), 1, win, hop, s);   // synchronises
     h->feat_sr = sample_rate; h->feat_win = win;
 }
 
@@ -1663,7 +1684,7 @@ void feat_batch(H* h, const char* who, const void* wav, int dtype, const int64_t
     const std::string fn(who);
     REQUIRE(wav && offsets && mel && mag && B >= 1 && (dtype == 0 || dtype == 1) && sample_rate > 0 && t_capacity >= 1 && r >= 1,
             fn + ": bad arguments");
-    REQUIRE(h->F == 1025, fn + ": the FFT kernel is built for n_fft = 2048");
+    require_fft_size(h, fn);
     std::vector<FeatSeg> seg(2 * (size_t)(B + 1));
     FeatSeg* mseg = seg.data();                     // whole utterances, frames of the trim energies
     FeatSeg* fseg = seg.data() + B + 1;             // trimmed utterances, STFT frames
@@ -2080,7 +2101,9 @@ int dctts_conv_gemm(dctts_handle h, int32_t impl, int32_t mode, const float* X, 
 int dctts_set_vocoder_params(dctts_handle h, int32_t hop_length, int32_t win_length, float power, float max_db,
                              float ref_db, double preemphasis, int32_t n_iter) {
     return guarded(h, [&] {
-        REQUIRE(hop_length >= 1 && win_length >= 1 && win_length <= 2048 && n_iter >= 0, "dctts_set_vocoder_params: bad arguments");
+        REQUIRE(hop_length >= 1 && win_length >= 1 && n_iter >= 0, "dctts_set_vocoder_params: bad arguments");
+        REQUIRE(win_length <= 2 * (h->F - 1), "dctts_set_vocoder_params: win_length " + std::to_string(win_length) +
+                                              " exceeds n_fft = " + std::to_string(2 * (h->F - 1)));
         h->voc.hop = hop_length; h->voc.win = win_length; h->voc.power = power; h->voc.max_db = max_db;
         h->voc.ref_db = ref_db; h->voc.preemph = preemphasis; h->voc.n_iter = n_iter;
     });
@@ -2091,16 +2114,16 @@ namespace {
 VocoderArgs voc_args(H* h, const char* fn, int B, int T, cudaStream_t s) {
     REQUIRE(B >= 1 && T >= 2, std::string(fn) + ": need B >= 1 and T >= 2 frames, got B = " + std::to_string(B) + ", T = " +
                               std::to_string(T));
-    REQUIRE(h->F == 1025, std::string(fn) + ": the FFT kernel is built for n_fft = 2048");
-    const int F = h->F, win = h->voc.win, hop = h->voc.hop, Ly = hop * (T - 1), nfr = 1 + Ly / 512;
+    require_fft_size(h, fn);
+    const int F = h->F, n_fft = 2 * (F - 1), win = h->voc.win, hop = h->voc.hop, Ly = hop * (T - 1), nfr = 1 + Ly / 512;
     const size_t n = (size_t)B * T * F;
     h->voc_S.ensure(n * sizeof(float)); h->voc_X.ensure(n * sizeof(float2));
     h->voc_frames.ensure((size_t)B * T * win * sizeof(float)); h->voc_mse.ensure((size_t)B * nfr * sizeof(float));
     h->voc_deemph.ensure(voc_deemph_scratch_bytes(B, T, hop));
     if (h->voc_tables_T != T || h->voc_tables_win != win || h->voc_tables_hop != hop) {
-        h->voc_tw.ensure(2048 * sizeof(float2)); h->voc_window.ensure(win * sizeof(float));
-        h->voc_wss.ensure((size_t)(2048 + hop * (T - 1)) * sizeof(float));
-        voc_make_tables(h->voc_tw.as<float2>(), h->voc_window.as<float>(), h->voc_wss.as<float>(), T, win, hop, s);
+        h->voc_tw.ensure(n_fft * sizeof(float2)); h->voc_window.ensure(win * sizeof(float));
+        h->voc_wss.ensure((size_t)(n_fft + hop * (T - 1)) * sizeof(float));
+        voc_make_tables(n_fft, h->voc_tw.as<float2>(), h->voc_window.as<float>(), h->voc_wss.as<float>(), T, win, hop, s);
         CUDA_CHECK(cudaGetLastError());
         h->voc_tables_T = T; h->voc_tables_win = win; h->voc_tables_hop = hop;
     }
@@ -2467,6 +2490,14 @@ int dctts_get_option(dctts_handle h, const char* name, int32_t* value) {
         if (name && std::string(name) == "pdl") { *value = pdl_enabled() ? 1 : 0; return; }
         if (name && std::string(name) == "decode_available") { *value = h->dec.ok ? 1 : 0; return; }
         if (name && std::string(name) == "decode_max_clusters") { *value = h->dec.max_clusters; return; }   // co-resident 16-CTA clusters
+        if (name && std::string(name) == "ssrn_tc_available") {     // every SSRN block has a wgmma kernel (needs committed parameters)
+            REQUIRE(h->committed, "dctts_get_option(ssrn_tc_available): parameters not committed");
+            REQUIRE(h->tc16_why.empty(), "dctts_get_option(ssrn_tc_available): " + h->tc16_why);
+            bool ok = !h->ssrn.empty();
+            for (const auto& l : h->ssrn) ok = ok && l.tc.ok;
+            *value = ok ? 1 : 0;
+            return;
+        }
         int* slot = option_slot(h, name);
         REQUIRE(slot, "dctts_get_option: unknown option");
         *value = *slot;

@@ -127,7 +127,12 @@ struct VocoderArgs {
     float max_db, ref_db, power;
     double preemphasis;            // float64 like the reference's scipy.signal.lfilter([1], [1, -hp.preemphasis], wav)
 };
-void voc_make_tables(float2* tw_dev, float* window_dev, float* wss_dev, int T, int win, int hop, cudaStream_t s);
+// n_fft 1024, 2048 and 4096 have kernel instantiations (F = 1 + n_fft / 2 = 513, 1025, 2049); the launchers take n_fft
+// from F and throw for any other size
+bool voc_fft_size_ok(int n_fft);
+// twiddles tw[k] = exp(-2 pi i k / n_fft) (n_fft entries), the win-tap Hann window, and the window sum-square of T frames
+// (n_fft + hop (T - 1) entries)
+void voc_make_tables(int n_fft, float2* tw_dev, float* window_dev, float* wss_dev, int T, int win, int hop, cudaStream_t s);
 // voc_run = voc_prepare, (voc_istft, voc_stft_phase) x n_iter, voc_istft, voc_deemph, voc_energies
 void voc_prepare(const VocoderArgs& a, cudaStream_t s);      // mag -> S, X = S (zero phase); 1 launch
 void voc_istft(const VocoderArgs& a, cudaStream_t s);        // X -> frames -> wav; 2 launches

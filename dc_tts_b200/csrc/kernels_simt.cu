@@ -606,7 +606,9 @@ void launch_ln_rows(const LnArgs& a, cudaStream_t s) {
     if (a.C <= 256)       launch_kernel(ln_rows_kernel<8>, dim3(grid), dim3(threads), 0, s, a);
     else if (a.C <= 512)  launch_kernel(ln_rows_kernel<16>, dim3(grid), dim3(threads), 0, s, a);
     else if (a.C <= 1024) launch_kernel(ln_rows_kernel<32>, dim3(grid), dim3(threads), 0, s, a);
-    else                  launch_kernel(ln_rows_kernel<33>, dim3(grid), dim3(threads), 0, s, a);   // F = 1025
+    else if (a.C <= 1056) launch_kernel(ln_rows_kernel<33>, dim3(grid), dim3(threads), 0, s, a);   // F = 1025
+    else if (a.C <= 2080) launch_kernel(ln_rows_kernel<65>, dim3(grid), dim3(threads), 0, s, a);   // F = 2049
+    else throw std::runtime_error("ln_rows: " + std::to_string(a.C) + " channels exceed the widest LayerNorm kernel (2080)");
 }
 
 // ------------------------------------------------------------------------------------

@@ -5,9 +5,9 @@
 // cores, and the whole epilogue -- bias, LayerNorm (two of them for hc), relu / sigmoid
 // gate / highway mix -- applied to the accumulator tile.
 //
-//   grid    (ncta, tiles); a thread-block CLUSTER of `ncta` CTAs shares one 128-row tile and
-//           splits the output channels; LayerNorm statistics are combined across the
-//           cluster through distributed shared memory (Chan's parallel mean/M2 merge).
+//   grid    (ncta, tiles); a thread-block CLUSTER of `ncta` CTAs (<= 8; 16 for the 144-column instantiation, the
+//           F = 2049 blocks) shares one 128-row tile and splits the output channels; LayerNorm statistics are
+//           combined across the cluster through distributed shared memory (Chan's parallel mean/M2 merge).
 //   warp 0  TMA producer: per k-block (BK channels of one tap) one {BK x 128 rows} box of
 //           each activation plane -- the tap's time shift is just the box coordinate, and
 //           TMA's out-of-bounds zero fill IS the reference's zero padding -- plus the
@@ -89,6 +89,9 @@ __host__ __device__ inline int tc_ring_bytes(int stages, int stage_bytes, int bn
     const int acc = TC_BM * tc_acc_ld(bn) * 4;
     return ((ring > acc ? ring : acc) + 1023) & ~1023;
 }
+// Largest cluster of an instantiation: 16 CTAs (a non-portable cluster size) for the 144-column one, whose F = 2049 conv1d
+// blocks split 2049 channels over 16 x 144; 8 for the others
+__host__ __device__ constexpr int tc_max_cluster(int bn) { return bn == 144 ? 16 : 8; }
 __host__ __device__ inline int tc_resid_bytes(int resid_tma, int half) { return resid_tma ? 2 * (half / 64) * 16384 : 0; }
 
 // One 128-row tile per CTA, split over two consumer warpgroups (rows 0-63 / 64-127), each holding its 64 x BN accumulator in
@@ -113,6 +116,7 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
     const int rank = (int)cluster_ctarank();                         // channel slice of this CTA
     const int ncta = (int)cluster_nctarank();
     const int nslices = ncta;
+    constexpr int MAXC = tc_max_cluster(BN);                         // cluster size bound: the statistics merge's unroll
     constexpr int bn = BN;                                           // accumulator columns per CTA
     const int half = a.half;                                         // columns per LN half
     constexpr int TC_A_PLANE = TC_BM * TC_BK * 2;                    // bytes of one activation plane tile
@@ -328,16 +332,16 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
             cluster_wait();
             if (r == 0) { dbg_mark(a.dbg, 7, 1); dbg_time(a.dbg, 12); }   // t4: cluster barrier passed
             const uint32_t my_slot = smem_u32(&s_part[r]);
-            float4 pv[8];
+            float4 pv[MAXC];
 #pragma unroll
-            for (int p = 0; p < 8; ++p) pv[p] = (p < nslices) ? ld_cluster_f4(mapa(my_slot, (uint32_t)p)) : make_float4(0.f, 0.f, 0.f, 0.f);
+            for (int p = 0; p < MAXC; ++p) pv[p] = (p < nslices) ? ld_cluster_f4(mapa(my_slot, (uint32_t)p)) : make_float4(0.f, 0.f, 0.f, 0.f);
             float S1 = 0.f, S2 = 0.f;
 #pragma unroll
-            for (int p = 0; p < 8; ++p) if (p < nslices) { S1 += pv[p].x; S2 += pv[p].z; }
+            for (int p = 0; p < MAXC; ++p) if (p < nslices) { S1 += pv[p].x; S2 += pv[p].z; }
             mean1 = S1 / (float)a.C; mean2 = S2 / (float)a.C;
             float M1 = 0.f, M2 = 0.f;
 #pragma unroll
-            for (int p = 0; p < 8; ++p) {
+            for (int p = 0; p < MAXC; ++p) {
                 if (p >= nslices) continue;
                 const float4 v = pv[p];
                 const int np = (a.mode == 0) ? min(max(a.C - p * bn, 0), bn) : half;
@@ -633,7 +637,8 @@ int tc_stages_for(int bn, int bk, int resid_tma, int half) {      // bn = accumu
 }
 
 // the kernel instantiation for (bk, bn): the accumulator widths of the networks' blocks -- 64 (Text2Mel's 256-channel
-// blocks), 80 (the mel output), 144 (the F = 1025 blocks over 8 CTAs), 256 (the 512- and 1024-channel blocks)
+// blocks), 80 (the mel output), 144 (the F = 1025 blocks over 8 CTAs, F = 2049 over 16), 256 (the 512- and 1024-channel
+// blocks)
 typedef void (*ConvLnKernel)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
                              const CUtensorMap, const CUtensorMap, const CUtensorMap, const TcArgs);
 template <int BK>
@@ -648,23 +653,48 @@ static ConvLnKernel conv_ln_kernel_bn(int bn) {
     }
 }
 
-void launch_conv_ln_tc(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& w_hi,
-                       const CUtensorMap& w_lo, const CUtensorMap* io, const TcArgs& a, int ncta, int ctas_y, int bk,
-                       cudaStream_t s) {
-    if (ncta > 8) throw std::runtime_error("conv_ln_tc: unsupported tile (cluster <= 8)");
-    const ConvLnKernel kern = bk == 64 ? conv_ln_kernel_bn<64>(a.bn) : conv_ln_kernel_bn<32>(a.bn);
+// The instantiation for (bk, bn) with its attributes raised on the current device: the shared-memory limit, and for the
+// 144-column one clusters of 16 CTAs
+static ConvLnKernel conv_ln_kernel_ready(int bk, int bn) {
+    const ConvLnKernel kern = bk == 64 ? conv_ln_kernel_bn<64>(bn) : conv_ln_kernel_bn<32>(bn);
     // the attributes are per device and per instantiation: cache them per device, not per process (a second Engine on
     // another GPU of the same process must raise its own limits)
     static bool attr_set_dev[64][8] = {};
     int dev = 0;
     cudaGetDevice(&dev);
-    const int inst = (bk == 64 ? 4 : 0) + (a.bn == 64 ? 0 : a.bn == 80 ? 1 : a.bn == 144 ? 2 : 3);
+    const int inst = (bk == 64 ? 4 : 0) + (bn == 64 ? 0 : bn == 80 ? 1 : bn == 144 ? 2 : 3);
     bool& attr_set = attr_set_dev[dev & 63][inst];
     if (!attr_set) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_MAX_SMEM);
+        if (e == cudaSuccess && tc_max_cluster(bn) > 8) e = cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
         if (e != cudaSuccess) throw std::runtime_error(std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e));
         attr_set = true;
     }
+    return kern;
+}
+
+int conv_ln_tc_max_clusters(int ncta, int bn, int bk) {
+    const ConvLnKernel kern = conv_ln_kernel_ready(bk, bn);
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3((unsigned)ncta, 1, 1);
+    cfg.blockDim = dim3(TC_THREADS, 1, 1);
+    cfg.dynamicSmemBytes = conv_ln_smem(tc_stages_for(bn, bk, 0, bn), bn, bn, 0, bk);
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeClusterDimension;
+    at[0].val.clusterDim.x = (unsigned)ncta; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+    cfg.attrs = at; cfg.numAttrs = 1;
+    int n = 0;
+    if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess) { cudaGetLastError(); return 0; }
+    return n;
+}
+
+void launch_conv_ln_tc(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& w_hi,
+                       const CUtensorMap& w_lo, const CUtensorMap* io, const TcArgs& a, int ncta, int ctas_y, int bk,
+                       cudaStream_t s) {
+    if (ncta > tc_max_cluster(a.bn))
+        throw std::runtime_error("conv_ln_tc: a cluster of " + std::to_string(ncta) + " CTAs at " + std::to_string(a.bn) +
+                                 " columns (16 at 144 columns, else 8 at most)");
+    const ConvLnKernel kern = conv_ln_kernel_ready(bk, a.bn);
     const size_t smem = conv_ln_smem(a.stages, a.bn, a.half, a.resid_tma, bk);
     if (smem > (size_t)TC_MAX_SMEM) throw std::runtime_error("conv_ln_tc: shared memory budget exceeded");
     cudaLaunchConfig_t cfg{};

@@ -66,6 +66,8 @@ void tc_make_map3(CUtensorMap* m, const __half* base, uint64_t d0, uint64_t d1, 
 int tc_stages_for(int bn, int bk, int resid_tma, int half);
 // reduction slab per pipeline stage (fp16 elements): 32 (64B swizzle)
 int tc_bk();
+// co-resident clusters of `ncta` CTAs of the conv1d instantiation with `bn` columns (0: none can be scheduled)
+int conv_ln_tc_max_clusters(int ncta, int bn, int bk);
 // grid = (ncta, tiles); cluster (ncta,1,1)
 void launch_conv_ln_tc(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& w_hi,
                        const CUtensorMap& w_lo, const CUtensorMap* io /* [4]: X hi, X lo, out hi, out lo ({64,128,1} boxes) or null */, const TcArgs& a, int ncta, int ctas_y, int bk, cudaStream_t s);

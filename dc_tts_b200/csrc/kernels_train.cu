@@ -113,8 +113,10 @@ __device__ __forceinline__ void ln_fwd_half(const float* __restrict__ y, int C, 
 constexpr int BWD_WARPS = 8;
 constexpr int BWD_ROWS_PER_WARP = 4;
 
-// grid: ceil(rows / 32) CTAs of 8 warps; dynamic shared memory: (4 C + nconv) floats of column accumulators
-template <int MAXV>
+// grid: ceil(rows / 32) CTAs of 8 warps; dynamic shared memory: (4 C + nconv) floats of column accumulators.
+// HC = false compiles the conv1d branch only (mode 0): the hc branch holds six MAXV arrays, which spill at MAXV = 65,
+// and no hc block is that wide (the F-wide SSRN blocks are conv1d).
+template <int MAXV, bool HC = true>
 __global__ void __launch_bounds__(BWD_WARPS * 32) train_block_bwd_kernel(const BlockBwdArgs a) {
     extern __shared__ float acc[];                 // [dg1 C][db1 C][dg2 C][db2 C][dbias nconv]
     const int C = a.C, nconv = a.mode == 1 ? 2 * C : C;
@@ -131,7 +133,7 @@ __global__ void __launch_bounds__(BWD_WARPS * 32) train_block_bwd_kernel(const B
         float yh1[MAXV], dz1[MAXV], dy1[MAXV];
         float r1;
         ln_fwd_half<MAXV>(y, C, lane, yh1, r1);
-        if (a.mode == 0) {
+        if (!HC || a.mode == 0) {
 #pragma unroll
             for (int i = 0; i < MAXV; ++i) {
                 const int c = lane + 32 * i;
@@ -195,7 +197,9 @@ void launch_train_block_bwd(const BlockBwdArgs& a, cudaStream_t s) {
     else if (a.C <= 512) train_block_bwd_kernel<16><<<grid, BWD_WARPS * 32, smem, s>>>(a);
     else if (a.C <= 1024) train_block_bwd_kernel<32><<<grid, BWD_WARPS * 32, smem, s>>>(a);
     else if (a.C <= 1056) train_block_bwd_kernel<33><<<grid, BWD_WARPS * 32, smem, s>>>(a);     // F = 1025
-    else throw std::runtime_error("train_block_bwd: C > 1056 is not on the path");
+    else if (a.C <= 2080 && a.mode == 0) train_block_bwd_kernel<65, false><<<grid, BWD_WARPS * 32, smem, s>>>(a);   // F = 2049
+    else if (a.C <= 2080) throw std::runtime_error("train_block_bwd: no hc kernel for " + std::to_string(a.C) + " channels (1056 at most)");
+    else throw std::runtime_error("train_block_bwd: " + std::to_string(a.C) + " channels exceed the widest kernel (2080)");
 }
 
 // ------------------------------------------------------------------------------------ weight gradient

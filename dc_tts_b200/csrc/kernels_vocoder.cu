@@ -2,12 +2,12 @@
 // This is the first "next" row of SURVEY.md 8(f): the step right after the synthesis path, serial
 // per-utterance CPU work in the reference (librosa), 51 inverse + 50 forward STFTs per utterance.
 //
-// One CTA per STFT frame; the 2048-point real transform is a 1024-point complex Stockham radix-4 FFT
-// (first and last pass in registers, three through 16 KB of shared memory), the
-// Hann window (1102 non-zero taps, centred in the 2048 frame) and librosa's conventions
-// (center=True reflect padding, division by the summed squared window, n_fft/2 trimmed at both
-// ends) are applied on the fly, so per Griffin-Lim iteration only the (B, T, 1025) complex
-// spectrum, the windowed frames and the waveform touch HBM:
+// One CTA of n_fft / 8 threads per STFT frame; the n_fft-point real transform is an n_fft/2-point complex Stockham FFT
+// (radix-4 passes, plus one radix-2 pass where log2(n_fft/2) is odd; the first pass reads and the last pass writes
+// registers, the others go through 2 x n_fft/2 x 8 B of shared memory), n_fft in {1024, 2048, 4096}.  The Hann window
+// (win <= n_fft non-zero taps, centred in the frame) and librosa's conventions (center=True reflect padding, division by
+// the summed squared window, n_fft/2 trimmed at both ends) are applied on the fly, so per Griffin-Lim iteration only the
+// (B, T, 1 + n_fft/2) complex spectrum, the windowed frames and the waveform touch HBM:
 //   voc_istft_kernel   spectrum row -> Hermitian extension -> IFFT -> x window -> frame buffer
 //   voc_ola_kernel     overlap-add of the <= 5 frames covering a sample, / window sum-square
 //   voc_stft_phase_kernel  reflect-padded frame x window -> FFT -> X = S * est / max(1e-8, |est|)
@@ -17,14 +17,24 @@
 
 #include <algorithm>
 #include <cmath>
+#include <stdexcept>
+#include <string>
+#include <type_traits>
 #include <vector>
 
 namespace dctts {
 
-constexpr int VC_N = 2048;
-constexpr int VC_THREADS = 256;
-
-constexpr int VC_H = VC_N / 2;                      // complex FFT length (real-input packing)
+// N = n_fft; the complex FFT has N / 2 points (real-input packing) and a CTA N / 8 threads, four values each
+template <int N> struct VcSize {
+    static constexpr int H = N / 2;
+    static constexpr int THREADS = N / 8;
+    static constexpr int LOG2H = N == 1024 ? 9 : N == 2048 ? 10 : 11;
+    static constexpr int R4_SMEM = (LOG2H - 1) / 2;     // radix-4 passes that end in shared memory
+    // __launch_bounds__ minimum of voc_istft_kernel: at 512 threads ptxas otherwise caps it at 32 registers and spills;
+    // 0 (no minimum) leaves the smaller sizes as they were
+    static constexpr int ISTFT_MIN_BLOCKS = N == 4096 ? 1 : 0;
+    static_assert(N == 1024 || N == 2048 || N == 4096, "n_fft must be 1024, 2048 or 4096");
+};
 
 __device__ __forceinline__ float2 cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
 
@@ -42,16 +52,21 @@ __device__ __forceinline__ int reflect_index(int u, int len) {
     return u;
 }
 
-// 1024-point complex FFT, Stockham autosort, radix 4, 256 threads, one butterfly per thread per pass.
-// Entry: v[k] = x[tid + 256 k]; exit: v[k] = X[tid + 256 k] (natural order, no scaling).  The first
-// pass reads and the last pass writes registers only; the three passes between go through the two
-// 8 KB ping-pong buffers (one __syncthreads each).  tw[k] = exp(-2 pi i k / 2048), k < 2048.
-template <bool INV>
-__device__ __forceinline__ void fft1024(float2 (&v)[4], float2* s0, float2* s1, const float2* __restrict__ tw) {
+// N/2-point complex FFT, Stockham autosort, N/8 threads, one radix-4 butterfly per thread per pass.
+// Entry: v[k] = x[tid + N/8 k]; exit: v[k] = X[tid + N/8 k] (natural order, no scaling).  The first pass reads
+// registers; every radix-4 pass but a last one of length 4 writes one of the two ping-pong buffers s0 / s1 (one
+// __syncthreads each, s0 first).  When log2(N/2) is even the last radix-4 pass (length 4, unit twiddles) stays in
+// registers; when it is odd a radix-2 pass (length 2) does, on the pairs (v[0], v[2]) and (v[1], v[3]).
+// tw[k] = exp(-2 pi i k / N), k < N.  Returns the buffer that no thread reads after the last barrier (free for the
+// caller at once).
+template <int N, bool INV>
+__device__ __forceinline__ float2* fft_half(float2 (&v)[4], float2* s0, float2* s1, const float2* __restrict__ tw) {
+    constexpr int T = VcSize<N>::THREADS, LOG2H = VcSize<N>::LOG2H;
+    constexpr int LS_LAST = (LOG2H & 1) ? LOG2H - 3 : LOG2H - 2;      // ls of the last radix-4 pass
     const int tid = threadIdx.x;
     float2* buf = s0;
 #pragma unroll
-    for (int ls = 0; ls <= 8; ls += 2) {
+    for (int ls = 0; ls <= LS_LAST; ls += 2) {
         const int str = 1 << ls, q = tid & (str - 1), p = tid >> ls;
         const float2 a = v[0], b = v[1], c = v[2], d = v[3];
         const float2 apc = make_float2(a.x + c.x, a.y + c.y), amc = make_float2(a.x - c.x, a.y - c.y);
@@ -61,7 +76,7 @@ __device__ __forceinline__ void fft1024(float2 (&v)[4], float2* s0, float2* s1, 
         float2 y1 = make_float2(amc.x - jb.x, amc.y - jb.y);
         float2 y2 = make_float2(apc.x - bpd.x, apc.y - bpd.y);
         float2 y3 = make_float2(amc.x + jb.x, amc.y + jb.y);
-        if (ls == 8) { v[0] = y0; v[1] = y1; v[2] = y2; v[3] = y3; break; }                   // n = 4: p = 0, unit twiddles
+        if (!(LOG2H & 1) && ls == LS_LAST) { v[0] = y0; v[1] = y1; v[2] = y2; v[3] = y3; break; }   // n = 4: p = 0, unit twiddles
         const int i1 = 2 * (tid - q);
         float2 w1 = tw[i1], w2 = tw[2 * i1], w3 = tw[3 * i1];
         if (INV) { w1.y = -w1.y; w2.y = -w2.y; w3.y = -w3.y; }
@@ -73,16 +88,23 @@ __device__ __forceinline__ void fft1024(float2 (&v)[4], float2* s0, float2* s1, 
         } else { o[0] = y0; o[str] = y1; o[2 * str] = y2; o[3 * str] = y3; }
         __syncthreads();
 #pragma unroll
-        for (int k = 0; k < 4; ++k) v[k] = buf[tid + 256 * k];
+        for (int k = 0; k < 4; ++k) v[k] = buf[tid + T * k];
         buf = (buf == s0) ? s1 : s0;
     }
+    if (LOG2H & 1) {                                                                             // n = 2: unit twiddles
+        const float2 a = v[0], b = v[1], c = v[2], d = v[3];
+        v[0] = make_float2(a.x + c.x, a.y + c.y); v[2] = make_float2(a.x - c.x, a.y - c.y);
+        v[1] = make_float2(b.x + d.x, b.y + d.y); v[3] = make_float2(b.x - d.x, b.y - d.y);
+    }
+    return (VcSize<N>::R4_SMEM & 1) ? s1 : s0;     // the buffer of the second-to-last shared-memory pass
 }
 
+template <int N>
 __global__ void voc_twiddle_kernel(float2* tw) {
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
-    if (k < VC_N) {
+    if (k < N) {
         double s, c;
-        sincospi(-2.0 * (double)k / (double)VC_N, &s, &c);
+        sincospi(-2.0 * (double)k / (double)N, &s, &c);
         tw[k] = make_float2((float)c, (float)s);
     }
 }
@@ -99,44 +121,47 @@ __global__ void voc_prepare_kernel(const float* __restrict__ mag, float* __restr
 }
 
 // librosa.core.istft, one frame: grid (T, B).  fr: (B, T, win) windowed time-domain frames.
-// The 2048-point Hermitian inverse is a 1024-point complex one: with E/O the spectra of the even/odd
-// samples, X[k] = E[k] + W^k O[k], X[k+1024] = conj(X[1024-k]) = E[k] - W^k O[k]; z = IFFT(E + i O)
+// The N-point Hermitian inverse is an N/2-point complex one: with E/O the spectra of the even/odd
+// samples, X[k] = E[k] + W^k O[k], X[k+N/2] = conj(X[N/2-k]) = E[k] - W^k O[k]; z = IFFT(E + i O)
 // carries x[2n] in its real and x[2n+1] in its imaginary part.
-__global__ void __launch_bounds__(VC_THREADS) voc_istft_kernel(const float2* __restrict__ X, float* __restrict__ fr,
-                                                               const float2* __restrict__ tw, const float* __restrict__ window,
-                                                               int T, int F, int win, int lpad) {
-    __shared__ __align__(16) float2 s0[VC_H];
-    __shared__ __align__(16) float2 s1[VC_H];
+template <int N>
+__global__ void __launch_bounds__(VcSize<N>::THREADS, VcSize<N>::ISTFT_MIN_BLOCKS)
+voc_istft_kernel(const float2* __restrict__ X, float* __restrict__ fr, const float2* __restrict__ tw, const float* __restrict__ window,
+                 int T, int F, int win, int lpad) {
+    constexpr int H = VcSize<N>::H, NT = VcSize<N>::THREADS;
+    __shared__ __align__(16) float2 s0[H];
+    __shared__ __align__(16) float2 s1[H];
     const int t = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
     const float2* x = X + ((size_t)b * T + t) * F;
     float2 v[4];
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-        const int kk = tid + 256 * k;
-        float2 xk = x[kk], xc = x[VC_H - kk];
+        const int kk = tid + NT * k;
+        float2 xk = x[kk], xc = x[H - kk];
         if (kk == 0) { xk.y = 0.f; xc.y = 0.f; }        // ifft(...).real drops the imaginary parts of bins 0 and n_fft/2
         xc.y = -xc.y;
         const float2 e = make_float2(xk.x + xc.x, xk.y + xc.y), d = make_float2(xk.x - xc.x, xk.y - xc.y);
         float2 w = tw[kk]; w.y = -w.y;
         const float2 o = cmul(d, w);
-        v[k] = make_float2(e.x - o.y, e.y + o.x);        // E + i O (the halves are folded into the 1/2048 below)
+        v[k] = make_float2(e.x - o.y, e.y + o.x);        // E + i O (the halves are folded into the 1/N below)
     }
-    fft1024<true>(v, s0, s1, tw);
+    fft_half<N, true>(v, s0, s1, tw);
     float* o = fr + ((size_t)b * T + t) * win;
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-        const int m = 2 * (tid + 256 * k) - lpad;        // frame sample 2n -> position in the window
-        if (m >= 0 && m < win) o[m] = v[k].x * (1.0f / VC_N) * window[m];
-        if (m + 1 >= 0 && m + 1 < win) o[m + 1] = v[k].y * (1.0f / VC_N) * window[m + 1];
+        const int m = 2 * (tid + NT * k) - lpad;         // frame sample 2n -> position in the window
+        if (m >= 0 && m < win) o[m] = v[k].x * (1.0f / N) * window[m];
+        if (m + 1 >= 0 && m + 1 < win) o[m + 1] = v[k].y * (1.0f / N) * window[m + 1];
     }
 }
 
 // overlap-add + window sum-square normalisation + centre trim: y (B, Ly), Ly = hop*(T-1)
+template <int N>
 __global__ void voc_ola_kernel(const float* __restrict__ fr, const float* __restrict__ wss, float* __restrict__ y,
                                int T, int win, int lpad, int hop, int Ly, float tiny) {
     const int sidx = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
     if (sidx >= Ly) return;
-    const int u = sidx + VC_N / 2;                       // index in the un-trimmed signal
+    const int u = sidx + N / 2;                          // index in the un-trimmed signal
     // frames t with lpad <= u - hop*t < lpad + win, in ascending order like librosa's loop
     int t_hi = (u - lpad) / hop;
     int t_lo = (u - lpad - win) / hop + 1;
@@ -150,27 +175,29 @@ __global__ void voc_ola_kernel(const float* __restrict__ fr, const float* __rest
 
 // librosa.core.stft of the current estimate, one frame, fused with the Griffin-Lim phase update
 // (utils.py:101-104): X = S * est / max(1e-8, |est|).  grid (T, B).  Real input packed as
-// z[n] = x[2n] + i x[2n+1]; est[k] = (Z[k] + conj Z[1024-k]) / 2 - i W^k (Z[k] - conj Z[1024-k]) / 2.
-__global__ void __launch_bounds__(VC_THREADS) voc_stft_phase_kernel(const float* __restrict__ y, const float* __restrict__ S,
-                                                                    float2* __restrict__ X, const float2* __restrict__ tw,
-                                                                    const float* __restrict__ window, int T, int F, int win,
-                                                                    int lpad, int hop, int Ly) {
-    __shared__ __align__(16) float2 s0[VC_H];
-    __shared__ __align__(16) float2 s1[VC_H];
+// z[n] = x[2n] + i x[2n+1]; est[k] = (Z[k] + conj Z[N/2-k]) / 2 - i W^k (Z[k] - conj Z[N/2-k]) / 2.
+template <int N>
+__global__ void __launch_bounds__(VcSize<N>::THREADS) voc_stft_phase_kernel(const float* __restrict__ y, const float* __restrict__ S,
+                                                                           float2* __restrict__ X, const float2* __restrict__ tw,
+                                                                           const float* __restrict__ window, int T, int F, int win,
+                                                                           int lpad, int hop, int Ly) {
+    constexpr int H = VcSize<N>::H, NT = VcSize<N>::THREADS;
+    __shared__ __align__(16) float2 s0[H];
+    __shared__ __align__(16) float2 s1[H];
     const int t = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
     const float* yb = y + (size_t)b * Ly;
     auto sample = [&](int n) -> float {
         const int m = n - lpad;
         if (m < 0 || m >= win) return 0.f;
-        const int u = reflect_index(t * hop + n - VC_N / 2, Ly);   // np.pad(y, n_fft//2, mode='reflect')
+        const int u = reflect_index(t * hop + n - N / 2, Ly);      // np.pad(y, n_fft//2, mode='reflect')
         return yb[u] * window[m];
     };
     float2 v[4];
 #pragma unroll
-    for (int k = 0; k < 4; ++k) { const int n = 2 * (tid + 256 * k); v[k] = make_float2(sample(n), sample(n + 1)); }
-    fft1024<false>(v, s0, s1, tw);
+    for (int k = 0; k < 4; ++k) { const int n = 2 * (tid + NT * k); v[k] = make_float2(sample(n), sample(n + 1)); }
+    float2* z = fft_half<N, false>(v, s0, s1, tw);                  // z was last read before the final barrier of the FFT
 #pragma unroll
-    for (int k = 0; k < 4; ++k) s0[tid + 256 * k] = v[k];          // s0 was last read before the final barrier of the FFT
+    for (int k = 0; k < 4; ++k) z[tid + NT * k] = v[k];
     __syncthreads();
     const float* Sb = S + ((size_t)b * T + t) * F;
     float2* x = X + ((size_t)b * T + t) * F;
@@ -181,14 +208,14 @@ __global__ void __launch_bounds__(VC_THREADS) voc_stft_phase_kernel(const float*
     };
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-        const int kk = tid + 256 * k;
+        const int kk = tid + NT * k;
         const float2 zk = v[k];
-        float2 zc = s0[(VC_H - kk) & (VC_H - 1)]; zc.y = -zc.y;
+        float2 zc = z[(H - kk) & (H - 1)]; zc.y = -zc.y;
         const float2 e = make_float2(0.5f * (zk.x + zc.x), 0.5f * (zk.y + zc.y));
         const float2 d = make_float2(0.5f * (zk.x - zc.x), 0.5f * (zk.y - zc.y));
         const float2 o = cmul(make_float2(d.y, -d.x), tw[kk]);     // -i d W^k
         emit(kk, make_float2(e.x + o.x, e.y + o.y));
-        if (kk == 0) emit(VC_H, make_float2(zk.x - zk.y, 0.f));    // bin n_fft/2: E[0] - O[0]
+        if (kk == 0) emit(H, make_float2(zk.x - zk.y, 0.f));       // bin n_fft/2: E[0] - O[0]
     }
 }
 
@@ -287,17 +314,18 @@ __global__ void __launch_bounds__(256) feat_frame_mse_kernel(const In* __restric
 // like numpy), reflect-padded Hann frame, the same real-packed FFT, |X|, the mel filterbank (each mel bin is a
 // contiguous run of FFT bins), 20 log10, normalisation.  Frame t of utterance b writes mag row b * mag_rows + t; frames
 // with t % r == 0 also write mel row b * mel_rows + t / r (load_spectrograms' reduction, utils.py:155-160).
-template <typename In>
-__global__ void __launch_bounds__(VC_THREADS) feat_stft_mel_kernel(const In* __restrict__ wav, const FeatSeg* __restrict__ seg,
-                                                                   int B, float preemph,
-                                                                   float* __restrict__ mag_out, float* __restrict__ mel_out,
-                                                                   int mag_rows, int mel_rows, int r,
-                                                                   const float* __restrict__ melw, const int2* __restrict__ melrange,
-                                                                   const float2* __restrict__ tw, const float* __restrict__ window,
-                                                                   int F, int n_mels, int win, int lpad, int hop, float ref_db,
-                                                                   float max_db) {
-    __shared__ __align__(16) float2 s0[VC_H];
-    __shared__ __align__(16) float2 s1[VC_H];
+template <int N, typename In>
+__global__ void __launch_bounds__(VcSize<N>::THREADS) feat_stft_mel_kernel(const In* __restrict__ wav, const FeatSeg* __restrict__ seg,
+                                                                          int B, float preemph,
+                                                                          float* __restrict__ mag_out, float* __restrict__ mel_out,
+                                                                          int mag_rows, int mel_rows, int r,
+                                                                          const float* __restrict__ melw, const int2* __restrict__ melrange,
+                                                                          const float2* __restrict__ tw, const float* __restrict__ window,
+                                                                          int F, int n_mels, int win, int lpad, int hop, float ref_db,
+                                                                          float max_db) {
+    constexpr int H = VcSize<N>::H, NT = VcSize<N>::THREADS;
+    __shared__ __align__(16) float2 s0[H];
+    __shared__ __align__(16) float2 s1[H];
     const int tid = threadIdx.x, b = feat_segment(seg, B, blockIdx.x);
     const FeatSeg sg = seg[b];
     const int t = blockIdx.x - sg.f0, len = sg.len;
@@ -305,18 +333,18 @@ __global__ void __launch_bounds__(VC_THREADS) feat_stft_mel_kernel(const In* __r
     auto sample = [&](int n) -> float {
         const int m = n - lpad;
         if (m < 0 || m >= win) return 0.f;
-        const int u = reflect_index(t * hop + n - VC_N / 2, len);  // np.pad(y, n_fft//2, mode='reflect')
+        const int u = reflect_index(t * hop + n - N / 2, len);     // np.pad(y, n_fft//2, mode='reflect')
         const float v = (u > 0) ? __fsub_rn(wav_sample(y, u), __fmul_rn(preemph, wav_sample(y, u - 1))) : wav_sample(y, 0);   // utils.py:39
         return v * window[m];
     };
     float2 v[4];
 #pragma unroll
-    for (int k = 0; k < 4; ++k) { const int n = 2 * (tid + 256 * k); v[k] = make_float2(sample(n), sample(n + 1)); }
-    fft1024<false>(v, s0, s1, tw);
+    for (int k = 0; k < 4; ++k) { const int n = 2 * (tid + NT * k); v[k] = make_float2(sample(n), sample(n + 1)); }
+    float2* z = fft_half<N, false>(v, s0, s1, tw);
 #pragma unroll
-    for (int k = 0; k < 4; ++k) s0[tid + 256 * k] = v[k];
+    for (int k = 0; k < 4; ++k) z[tid + NT * k] = v[k];
     __syncthreads();
-    float* lin = reinterpret_cast<float*>(s1);             // |X[k]|, k <= 1024 (s1 was last read inside the FFT)
+    float* lin = reinterpret_cast<float*>(z == s0 ? s1 : s0);   // |X[k]|, k <= N/2 (the other buffer was last read inside the FFT)
     float* mo = mag_out + ((size_t)b * mag_rows + t) * F;
     auto emit = [&](int kk, float2 e) {
         const float a = sqrtf(e.x * e.x + e.y * e.y);
@@ -326,20 +354,20 @@ __global__ void __launch_bounds__(VC_THREADS) feat_stft_mel_kernel(const In* __r
     };
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-        const int kk = tid + 256 * k;
+        const int kk = tid + NT * k;
         const float2 zk = v[k];
-        float2 zc = s0[(VC_H - kk) & (VC_H - 1)]; zc.y = -zc.y;
+        float2 zc = z[(H - kk) & (H - 1)]; zc.y = -zc.y;
         const float2 e = make_float2(0.5f * (zk.x + zc.x), 0.5f * (zk.y + zc.y));
         const float2 d = make_float2(0.5f * (zk.x - zc.x), 0.5f * (zk.y - zc.y));
         const float2 o = cmul(make_float2(d.y, -d.x), tw[kk]);
         emit(kk, make_float2(e.x + o.x, e.y + o.y));
-        if (kk == 0) emit(VC_H, make_float2(zk.x - zk.y, 0.f));
+        if (kk == 0) emit(H, make_float2(zk.x - zk.y, 0.f));
     }
     if (t % r != 0) return;                                // a frame the reduction drops: mag only
     __syncthreads();
     float* mel_row = mel_out + ((size_t)b * mel_rows + t / r) * n_mels;
     const int warp = tid >> 5, lane = tid & 31;
-    for (int m = warp; m < n_mels; m += VC_THREADS / 32) {
+    for (int m = warp; m < n_mels; m += NT / 32) {
         const int2 r = melrange[m];
         const float* w = melw + (size_t)m * F;
         float acc = 0.f;
@@ -353,19 +381,32 @@ __global__ void __launch_bounds__(VC_THREADS) feat_stft_mel_kernel(const In* __r
 }
 
 // ---------------------------------------------------------------------------------------- host
-void voc_make_tables(float2* tw_dev, float* window_dev, float* wss_dev, int T, int win, int hop, cudaStream_t s) {
-    voc_twiddle_kernel<<<(VC_N + 255) / 256, 256, 0, s>>>(tw_dev);
+bool voc_fft_size_ok(int n_fft) { return n_fft == 1024 || n_fft == 2048 || n_fft == 4096; }
+
+// Calls f(std::integral_constant<int, n_fft>): the kernel instantiation for the handle's n_fft
+template <typename Fn>
+static void voc_dispatch(int n_fft, Fn&& f) {
+    switch (n_fft) {
+        case 1024: f(std::integral_constant<int, 1024>{}); break;
+        case 2048: f(std::integral_constant<int, 2048>{}); break;
+        case 4096: f(std::integral_constant<int, 4096>{}); break;
+        default: throw std::runtime_error("vocoder: n_fft = " + std::to_string(n_fft) + " (supported: 1024, 2048, 4096)");
+    }
+}
+
+void voc_make_tables(int n_fft, float2* tw_dev, float* window_dev, float* wss_dev, int T, int win, int hop, cudaStream_t s) {
+    voc_dispatch(n_fft, [&](auto n) { voc_twiddle_kernel<decltype(n)::value><<<(n_fft + 255) / 256, 256, 0, s>>>(tw_dev); });
     // periodic Hann of win taps (scipy get_window('hann', win, fftbins=True)) and librosa's window_sumsquare,
     // accumulated in float32 in frame order like the reference
     std::vector<float> w(win);
     for (int n = 0; n < win; ++n) w[n] = (float)(0.5 - 0.5 * std::cos(2.0 * M_PI * (double)n / (double)win));
-    const int lpad = (VC_N - win) / 2;
-    const int n_tot = VC_N + hop * (T - 1);
+    const int lpad = (n_fft - win) / 2;
+    const int n_tot = n_fft + hop * (T - 1);
     std::vector<float> wss(n_tot, 0.f);
-    std::vector<float> wsq(VC_N, 0.f);
+    std::vector<float> wsq(n_fft, 0.f);
     for (int n = 0; n < win; ++n) { const double d = 0.5 - 0.5 * std::cos(2.0 * M_PI * (double)n / (double)win); wsq[lpad + n] = (float)(d * d); }
     for (int t = 0; t < T; ++t)
-        for (int n = 0; n < VC_N && t * hop + n < n_tot; ++n) wss[t * hop + n] += wsq[n];
+        for (int n = 0; n < n_fft && t * hop + n < n_tot; ++n) wss[t * hop + n] += wsq[n];
     cudaMemcpyAsync(window_dev, w.data(), win * sizeof(float), cudaMemcpyHostToDevice, s);
     cudaMemcpyAsync(wss_dev, wss.data(), n_tot * sizeof(float), cudaMemcpyHostToDevice, s);
     cudaStreamSynchronize(s);
@@ -408,15 +449,18 @@ void feat_frame_mse(const void* wav, int dtype, const FeatSeg* seg, int B, int f
 
 void feat_run(const FeatArgs& a, cudaStream_t s) {
     const int2* range = reinterpret_cast<const int2*>(a.melrange);
-    const int lpad = (VC_N - a.win) / 2;
-    if (a.dtype == 1)
-        feat_stft_mel_kernel<int16_t><<<a.frames, VC_THREADS, 0, s>>>(
-            static_cast<const int16_t*>(a.wav), a.seg, a.B, a.preemph, a.mag, a.mel, a.mag_rows, a.mel_rows, a.r, a.melw, range,
-            a.tw, a.window, a.F, a.n_mels, a.win, lpad, a.hop, a.ref_db, a.max_db);
-    else
-        feat_stft_mel_kernel<float><<<a.frames, VC_THREADS, 0, s>>>(
-            static_cast<const float*>(a.wav), a.seg, a.B, a.preemph, a.mag, a.mel, a.mag_rows, a.mel_rows, a.r, a.melw, range,
-            a.tw, a.window, a.F, a.n_mels, a.win, lpad, a.hop, a.ref_db, a.max_db);
+    voc_dispatch(2 * (a.F - 1), [&](auto n) {
+        constexpr int N = decltype(n)::value;
+        const int lpad = (N - a.win) / 2;
+        if (a.dtype == 1)
+            feat_stft_mel_kernel<N, int16_t><<<a.frames, VcSize<N>::THREADS, 0, s>>>(
+                static_cast<const int16_t*>(a.wav), a.seg, a.B, a.preemph, a.mag, a.mel, a.mag_rows, a.mel_rows, a.r, a.melw, range,
+                a.tw, a.window, a.F, a.n_mels, a.win, lpad, a.hop, a.ref_db, a.max_db);
+        else
+            feat_stft_mel_kernel<N, float><<<a.frames, VcSize<N>::THREADS, 0, s>>>(
+                static_cast<const float*>(a.wav), a.seg, a.B, a.preemph, a.mag, a.mel, a.mag_rows, a.mel_rows, a.r, a.melw, range,
+                a.tw, a.window, a.F, a.n_mels, a.win, lpad, a.hop, a.ref_db, a.max_db);
+    });
 }
 
 // ---------------------------------------------------------------------------------------- resampling
@@ -567,14 +611,22 @@ void voc_prepare(const VocoderArgs& a, cudaStream_t s) {
 }
 
 void voc_istft(const VocoderArgs& a, cudaStream_t s) {
-    const int Ly = a.hop * (a.T - 1), lpad = (VC_N - a.win) / 2;
-    voc_istft_kernel<<<dim3(a.T, a.B), VC_THREADS, 0, s>>>(a.X, a.frames, a.tw, a.window, a.T, a.F, a.win, lpad);
-    voc_ola_kernel<<<dim3((Ly + 255) / 256, a.B), 256, 0, s>>>(a.frames, a.wss, a.wav, a.T, a.win, lpad, a.hop, Ly, 1.17549435e-38f);
+    voc_dispatch(2 * (a.F - 1), [&](auto n) {
+        constexpr int N = decltype(n)::value;
+        const int Ly = a.hop * (a.T - 1), lpad = (N - a.win) / 2;
+        voc_istft_kernel<N><<<dim3(a.T, a.B), VcSize<N>::THREADS, 0, s>>>(a.X, a.frames, a.tw, a.window, a.T, a.F, a.win, lpad);
+        voc_ola_kernel<N><<<dim3((Ly + 255) / 256, a.B), 256, 0, s>>>(a.frames, a.wss, a.wav, a.T, a.win, lpad, a.hop, Ly,
+                                                                     1.17549435e-38f);
+    });
 }
 
 void voc_stft_phase(const VocoderArgs& a, cudaStream_t s) {
-    const int Ly = a.hop * (a.T - 1), lpad = (VC_N - a.win) / 2;
-    voc_stft_phase_kernel<<<dim3(a.T, a.B), VC_THREADS, 0, s>>>(a.wav, a.S, a.X, a.tw, a.window, a.T, a.F, a.win, lpad, a.hop, Ly);
+    voc_dispatch(2 * (a.F - 1), [&](auto n) {
+        constexpr int N = decltype(n)::value;
+        const int Ly = a.hop * (a.T - 1), lpad = (N - a.win) / 2;
+        voc_stft_phase_kernel<N><<<dim3(a.T, a.B), VcSize<N>::THREADS, 0, s>>>(a.wav, a.S, a.X, a.tw, a.window, a.T, a.F, a.win,
+                                                                              lpad, a.hop, Ly);
+    });
 }
 
 void voc_deemph(const VocoderArgs& a, cudaStream_t s) {

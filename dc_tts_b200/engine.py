@@ -295,7 +295,7 @@ class Engine:
 
     def vocoder_stage(self, stage, x, out, S=None, hop=None, win=None, power=None):
         """Test aid (include/dctts.h: dctts_vocoder_stage): ONE stage of spectrogram2wav on caller CUDA tensors, with the
-        hyperparameters' vocoder constants except `hop`, `win` and `power` when given.  Ly = hop (T - 1), F = 1025:
+        hyperparameters' vocoder constants except `hop`, `win` and `power` when given.  Ly = hop (T - 1), F = 1 + n_fft/2:
           0 prepare     x = mag (B, T, F) float32                -> out = X (B, T, F) complex64
           1 istft       x = X (B, T, F) complex64                -> out = wav (B, Ly) float32
           2 stft_phase  x = wav (B, Ly), S = (B, T, F) float32   -> out = X (B, T, F) complex64

@@ -2,8 +2,8 @@
 `spectrogram2wav(mag)`, `griffin_lim(spectrogram)`, `invert_spectrogram(spectrogram)`.
 
 The reference runs librosa's stft / istft on the CPU, 50 + 51 times per utterance; here the whole
-Griffin-Lim loop runs on the GPU (csrc/kernels_vocoder.cu: one CTA per STFT frame, a 2048-point FFT
-in shared memory) behind `dctts_spectrogram2wav`.  This is the first "next" row of SURVEY.md 8(f), not part
+Griffin-Lim loop runs on the GPU (csrc/kernels_vocoder.cu: one CTA per STFT frame, an n_fft-point FFT
+in shared memory, n_fft 1024, 2048 or 4096) behind `dctts_spectrogram2wav`.  This is the first "next" row of SURVEY.md 8(f), not part
 of the Text2Mel + SSRN hot path.  Feature extraction (`get_spectrograms`, `load_spectrograms`,
 utils.py:20-65,147-162) runs on the GPU too (`dctts_get_spectrograms` / `dctts_load_spectrograms_batch`: trim,
 pre-emphasis, STFT, mel filterbank, dB, normalisation in two kernels per call, for one utterance or a whole bucket);

@@ -37,7 +37,7 @@ typedef struct dctts_hparams {
     int32_t d;                   /* hp.d = 256  */
     int32_t c;                   /* hp.c = 512  */
     int32_t n_mels;              /* hp.n_mels = 80 */
-    int32_t n_fft;               /* hp.n_fft = 2048 -> F = 1 + n_fft/2 */
+    int32_t n_fft;               /* hp.n_fft = 2048 -> F = 1 + n_fft/2; the STFT kernels exist for 1024, 2048, 4096 */
     int32_t max_N;               /* hp.max_N = 180 */
     int32_t max_T;               /* hp.max_T = 210 */
     int32_t attention_win_size;  /* hp.attention_win_size = 3 */
@@ -127,7 +127,8 @@ int dctts_synthesize_host(dctts_handle h, const int32_t* L_host, int32_t B,
 
 /* ---- vocoder ("next" row after the path: reference utils.py:67-114) --------------------- */
 /* Signal-processing constants of hyperparams.py:13-24 (defaults = the LJ values: hop 275, win 1102, power 1.5,
- * max_db 100, ref_db 20, preemphasis 0.97, n_iter 50; n_fft is fixed at 2048 = 2*(F-1)).  preemphasis is float64:
+ * max_db 100, ref_db 20, preemphasis 0.97, n_iter 50; n_fft = 2*(F-1) of the handle: 1024, 2048 or 4096, and
+ * win_length <= n_fft, else the call fails).  preemphasis is float64:
  * the de-pre-emphasis filter runs with it as scipy.signal.lfilter does; the features' pre-emphasis rounds it to float32
  * as numpy does for a float32 waveform. */
 int dctts_set_vocoder_params(dctts_handle h, int32_t hop_length, int32_t win_length, float power, float max_db,
@@ -267,8 +268,10 @@ int dctts_set_tensor_path(dctts_handle h, int32_t mode);
  *   "decode_force_prepass" 0/1: measurement / test switch of the persistent decode (default 0): every utterance takes the
  *                  receptive-field recompute at every frame j >= 1, as if its attention window had moved (the worst case)
  *   "train_tc" 0..7: training GEMMs on wgmma, bit mask 1 forward conv (+ wgmma attention), 2 data gradient, 4 weight gradient
- * dctts_get_option also answers "decode_available" (1 when this handle / device can run the persistent decode) and
- * "decode_max_clusters" (16-CTA clusters of the decode kernel that are co-resident on this device). */
+ * dctts_get_option also answers "decode_available" (1 when this handle / device can run the persistent decode),
+ * "decode_max_clusters" (16-CTA clusters of the decode kernel that are co-resident on this device) and, once the
+ * parameters are committed, "ssrn_tc_available" (1 when every SSRN block has a wgmma kernel, the F-wide ones included:
+ * at F = 2049 they need a 16-CTA cluster; when none can be scheduled on the device the call fails and says so). */
 int dctts_set_option(dctts_handle h, const char* name, int32_t value);
 int dctts_get_option(dctts_handle h, const char* name, int32_t* value);
 /* Of the last dctts_text2mel_generate on the persistent decode path: frames in which a cluster had to recompute the
@@ -299,7 +302,7 @@ int dctts_conv_gemm(dctts_handle h, int32_t impl, int32_t mode, const float* X, 
                     int32_t accumulate, float* out, int32_t ldo, void* stream);
 /* Test aid: ONE stage of dctts_spectrogram2wav on caller DEVICE tensors, through the launch functions the product calls,
  * with the handle's vocoder parameters and the tables (twiddles, window, window sum-square) it builds for (T, win, hop).
- * Ly = hop (T - 1), nfr = 1 + Ly / 512, F = 1025.
+ * Ly = hop (T - 1), nfr = 1 + Ly / 512, F = 1 + n_fft / 2.
  *   0 prepare:    in = mag (B,T,F) float32            -> out = X (B,T,F) complex64  (S = Re X, zero phase)
  *   1 istft:      in = X (B,T,F) complex64            -> out = wav (B,Ly) float32
  *   2 stft_phase: in = wav (B,Ly), S (B,T,F) float32  -> out = X (B,T,F) complex64
