@@ -457,7 +457,7 @@ void pack_decode(H* h) {
         if (K % L.krows || L.krows % 8 || kr8 * L.ns > DEC_REG_F || kr8 % (8 * sg) || (L.prow > 1 && kr8 % 16)) {
             D.why = "persistent decode: chunk geometry"; return;
         }
-        if (L.prow > 1 && (L.prow - 1) + (l.size - 1) * l.rate > 96) { D.why = "persistent decode: receptive field too tall"; return; }
+        if (L.prow > 1 && (L.prow - 1) + (l.size - 1) * l.rate > DEC_PL_PAD) { D.why = "persistent decode: receptive field too tall"; return; }
         L.ch0 = nch;
         for (int k0 = 0; k0 < K; k0 += L.krows) {
             if (nch >= DEC_MAXCH) { D.why = "persistent decode: too many weight chunks"; return; }
@@ -1074,7 +1074,7 @@ bool decode_cluster(H* h, int B, int steps, cudaStream_t s) {
     P.p_hist = ib.p_hist; P.p_final = D.pfinal.as<int>(); P.stats = D.stats.as<int>();
     P.prof = nullptr;
     P.force_prepass = h->opt.decode_force_prepass != 0;
-    if (h->opt.decode_prof) { D.prof.ensure(16 * sizeof(long long)); CUDA_CHECK(cudaMemsetAsync(D.prof.p, 0, 16 * sizeof(long long), s)); P.prof = D.prof.as<long long>(); }
+    if (h->opt.decode_prof) { D.prof.ensure(DEC_NPROF * sizeof(long long)); CUDA_CHECK(cudaMemsetAsync(D.prof.p, 0, DEC_NPROF * sizeof(long long), s)); P.prof = D.prof.as<long long>(); }
     P.B = B;
     {   // utterances per cluster: the fewest that let every cluster be co-resident (a second wave doubles the time)
         const int mc = std::max(1, D.max_clusters);
@@ -2524,14 +2524,13 @@ int dctts_decode_stats(dctts_handle h, int32_t* moved_frames, int32_t* moved_utt
 }
 
 // SM-clock lap timers of the last persistent decode run with option decode_prof = 1 (cluster 0, CTA rank 0, thread 0):
-// cycles[0..13] = block start / stream wait / GEMV / slot release / gather / cluster barrier / LayerNorm / mix / attention /
-// recompute attention / recompute GEMM / recompute LayerNorm / recompute barriers / frame bookkeeping.
+// the buckets are listed in include/dctts.h.
 int dctts_decode_profile(dctts_handle h, int64_t* cycles, int32_t n) {
     return guarded(h, [&] {
-        REQUIRE(cycles && n >= 1 && n <= 16, "dctts_decode_profile: bad arguments");
+        REQUIRE(cycles && n >= 1 && n <= DEC_NPROF, "dctts_decode_profile: bad arguments");
         REQUIRE(h->dec.prof.p, "dctts_decode_profile: no profiled decode has run (set option decode_prof)");
         CUDA_CHECK(cudaDeviceSynchronize());
-        long long v[16];
+        long long v[DEC_NPROF];
         CUDA_CHECK(cudaMemcpy(v, h->dec.prof.p, sizeof(v), cudaMemcpyDeviceToHost));
         for (int i = 0; i < n; ++i) cycles[i] = v[i];
     });

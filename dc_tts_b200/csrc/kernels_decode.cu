@@ -25,7 +25,8 @@
 //     give.  When it moves, a PRE-PASS refreshes the rows t < j of its AudioDec receptive field
 //     (84/82/76/58/4/2 rows of C_1, HC_2..HC_6) under the new window -- attention one warp per row, a
 //     wgmma GEMM per utterance (split-fp16 planes staged per 16-channel slab in the no-swizzle K-major
-//     layout, the three taps being the same slab read through shifted descriptors), pre-LN rows through
+//     layout, each slab fetched once per cluster and multicast to its 16 CTAs, the three taps being the
+//     same slab read through shifted descriptors), pre-LN rows through
 //     an L2 scratch, LayerNorm one warp per row over the whole cluster -- and the ordinary one-row pass
 //     then runs for every utterance.  The pre-pass consumes the same weight chunks a second time: the
 //     stream is "virtual" (frame, segment, chunk) and both the consumer and the refill cursor walk it.
@@ -38,6 +39,7 @@
 
 #include <cuda_fp16.h>
 #include <atomic>
+#include <cstddef>
 #include <math.h>
 
 namespace dctts {
@@ -48,10 +50,15 @@ namespace {
 constexpr int NC = DEC_NC, GMAX = DEC_GMAX, NT = DEC_THREADS, NWARP = NT / 32;
 constexpr int XLD = 768;                       // row pitch of the input vectors: [tap0 | tap1 | current]
 constexpr int PLD = GMAX * 32 + 16;            // pitch between the ranks' slices in `pre` (16 floats of bank skew)
-constexpr int TC_RA = 96;                      // pre-pass: rows per k8 group of an A slab plane (<= 96 source rows per utterance)
+constexpr int TC_RA = DEC_PL_PAD;              // pre-pass: rows per k8 group of an A slab plane (source rows per utterance, pack_decode)
 constexpr int TC_APLANE = 2 * TC_RA * 16;      // bytes of one plane of one 16-channel slab (2 k8 groups)
 constexpr int TC_ASTAGE = 2 * TC_APLANE;       // hi + lo planes
-constexpr int TC_NSTG = 3;                     // A slab stages
+constexpr int TC_NSTG = 6;                     // A slab stages: five slabs in flight while one is multiplied
+constexpr int gcd_c(int a, int b) { return b == 0 ? a : gcd_c(b, a % b); }
+constexpr unsigned TC_QCYC = NC / gcd_c(NC, TC_NSTG) * TC_NSTG;   // slabs between two stagings of one stage by one CTA
+constexpr int TC_PR = 24;                      // packed tile (pyr_tc_packed): rows per k8 group of a tap image (>= GMAX * 4)
+constexpr int TC_PTAP = 2 * 2 * TC_PR * 16;    // bytes of one tap image (hi + lo planes, 2 k8 groups)
+static_assert(3 * TC_PTAP <= TC_ASTAGE, "packed tap images inside a stage");
 static_assert(GMAX * NT >= 1024, "red: LayerNorm parameters of the pre-pass");
 static_assert(TC_RA == DEC_PL_PAD, "pl_c1 rows are staged as whole slabs");
 
@@ -60,7 +67,8 @@ struct Smem {
     float red[GMAX][NT];                // per-frame path: partial sums per warp; pre-pass: LayerNorm parameters of the block
     float xin[2][GMAX][XLD];
     union {                             // never live together: between the cluster barriers that enclose the pre-pass no peer
-                                        // sends pre-LN slices, so the pre-pass stages A here
+                                        // sends pre-LN slices, so the pre-pass stages A here (and the peers' multicast
+                                        // slabs land here only between those barriers)
         float pre[2][NC][PLD];
         unsigned char tca[TC_NSTG][TC_ASTAGE];   // (the MMAs read up to 128 + 54 rows past a slab start: outv / prm follow)
     };
@@ -76,16 +84,23 @@ struct Smem {
                                         // constant bank those indexed loads missed the (instruction-shared) constant cache
     int p_cur[GMAX], p_prev[GMAX], p_next[GMAX], moved[GMAX];
     int fmoved[2];
-    long long prof[16], prof_last;
+    long long prof[DEC_NPROF], prof_last;
 };
 
 static_assert(sizeof(Smem) + 128 <= 232448, "decode kernel: shared memory budget (227 KB per CTA)");
-static_assert(sizeof(float) * 2 * NC * PLD >= TC_NSTG * TC_ASTAGE, "A stages inside pre");
+// An A descriptor reads 64 rows per live M half from its k8 group: up to TC_RA + 128 rows from a group that holds TC_RA
+// (tap shift <= TC_RA, pack_decode), i.e. up to 128 rows of 16 bytes past the end of the last stage.  Those rows are thrown
+// away but must be shared memory of this kernel.
+static_assert(offsetof(Smem, tca) + sizeof(Smem::tca) + 128 * 16 <= sizeof(Smem), "A tile reads past the stages");
 
 // lap timer (option decode_prof): thread 0 attributes the cycles since the previous lap to bucket i
 #define LAP(i) do { if constexpr (PROF) { if (threadIdx.x == 0) { const long long now_ = clock64(); S.prof[i] += now_ - S.prof_last; S.prof_last = now_; } } } while (0)
 enum { LP_START = 0, LP_WAIT = 1, LP_GEMV = 2, LP_RELEASE = 3, LP_GATHER = 4, LP_CBAR = 5, LP_LN = 6, LP_MIX = 7, LP_ATT = 8,
-       LP_PYR_ATT = 9, LP_PYR_GEMM = 10, LP_PYR_LN = 11, LP_PYR_BAR = 12, LP_FRAME = 13 };
+       LP_PYR_ATT = 9, LP_PYR_WTS = 10, LP_PYR_TABLE = 11, LP_PYR_STAGE = 12, LP_PYR_DRAIN = 13, LP_PYR_REFILL = 14,
+       LP_PYR_LN = 15, LP_PYR_BAR = 16, LP_FRAME = 17,
+       // the MMA warpgroup's own laps (thread 128, pyr_mma_rows): they overlap thread 0's
+       LP_WG_AWAIT = 18, LP_WG_MMA = 19, LP_WG_EPI = 20, LP_COUNT };
+static_assert(LP_COUNT <= DEC_NPROF, "lap buckets");
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
@@ -109,6 +124,12 @@ template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile(
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, unsigned long long* bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  :: "r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
+}
+// the same, multicast: the bytes land at the same CTA-relative offset in every CTA of `mask`, each completing on its own
+// mbarrier at the offset of `bar`
+__device__ __forceinline__ void bulk_g2s_mc(void* dst, const void* src, uint32_t bytes, unsigned long long* bar, uint16_t mask) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;"
+                 :: "r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)), "h"(mask) : "memory");
 }
 // local shared memory -> a peer CTA's shared memory, completing on the PEER's mbarrier
 __device__ __forceinline__ void bulk_s2peer(uint32_t dst_cluster, const void* src, uint32_t bytes, uint32_t bar_cluster) {
@@ -529,7 +550,7 @@ __device__ __forceinline__ void pre_row_of(const PreRows& r, int m, int& g, int&
 __device__ __forceinline__ int pre_off_of(const PreRows& r, int g) { return r.n * __popc(r.mask & ((1u << g) - 1u)); }
 // address of W[k][n] (k = row within the layer's K) inside the ring; the layer's chunks occupy consecutive slots from pos0
 // ---- the pre-pass GEMM on the tensor cores (wgmma) ---------------------------------------------------------------------
-// One utterance, <= 96 source rows.  A = the source rows as split-fp16 planes (hi = fp16(x), lo = fp16(x - hi)), staged per
+// One utterance, <= TC_RA source rows.  A = the source rows as split-fp16 planes (hi = fp16(x), lo = fp16(x - hi)), staged per
 // 16-channel slab in the NO-SWIZZLE K-major core-matrix layout [k8][row][8 halfs]: rows are consecutive 16-byte chunks, so
 // the three taps of the dilated conv are the SAME slab read through descriptors whose start address is shifted by
 // tap * rate rows -- staged once, multiplied three times.  B = this CTA's weight columns, pre-packed in the same layout
@@ -554,29 +575,42 @@ __device__ __forceinline__ void pyr_tc_table(const DecParams& P, Smem& S, int li
 // The shape is compile-time -- NS weight columns, NTAPS taps, MH live row halves of 64 (MH = 1 when every output row is below
 // 64: the other half would multiply rows that are thrown away) -- so that the products of one slab are ONE straight
 // fence -> MMAs -> commit sequence.  (With a run-time tap loop ptxas serialised every wgmma: C7520.)  One slab stays in
-// flight: slab ks is issued before the wait for slab ks - 1, whose stage is released only after that wait.
-template <int NS, int NTAPS, int MH>
-__device__ __forceinline__ void pyr_mma_rows(const DecParams& P, Smem& S, int li, unsigned& use, int& stg, int n_out, int rank,
+// flight: slab ks is issued before the wait for slab ks - 1, whose stage is released only after that wait.  Slabs are
+// numbered through the launch from q0 (see pyr_tc_utt); the release of slab q goes to the CTA that stages slab q + TC_NSTG.
+// A layout of a stage: PACKED = false, one utterance's window of source rows, tap t read from row t * rate of it;
+// PACKED = true, one image per tap of the rows that tap reads for all moved utterances (pyr_tc_packed).
+template <bool PROF, int NS, int NTAPS, int MH, bool PACKED>
+__device__ __forceinline__ void pyr_mma_rows(const DecParams& P, Smem& S, int li, unsigned q0, int n_out, int rank,
                                              float* scr_rows) {
     const DecLayer& l = P.L[li];
     const int nslab = l.cin / 16, lane = threadIdx.x & 31, w4 = (threadIdx.x >> 5) & 3;
     const bool leader = (threadIdx.x & 127) == 0;
+    long long t_prof = 0;                                             // lap timers of this warpgroup (thread 128)
+    auto wlap = [&](int i) {
+        if constexpr (PROF) { if (leader) { const long long now = clock64(); if (i >= 0) S.prof[i] += now - t_prof; t_prof = now; } }
+    };
+    wlap(-1);
     unsigned char* As = &S.tca[0][0];
-    const uint64_t dA0 = gmma_desc_noswz(0, TC_RA * 16, 128), dB0 = gmma_desc_noswz(0, (uint32_t)NS * 16, 128);
-    const uint32_t a_base = (smem_u32(As) & 0x3FFFFu) >> 4, b_lo = (uint32_t)NS * 2, tap_step = (uint32_t)l.rate;
+    const uint64_t dA0 = gmma_desc_noswz(0, (PACKED ? TC_PR : TC_RA) * 16, 128), dB0 = gmma_desc_noswz(0, (uint32_t)NS * 16, 128);
+    const uint32_t a_base = (smem_u32(As) & 0x3FFFFu) >> 4, b_lo = (uint32_t)NS * 2;
+    const uint32_t tap_step = PACKED ? (uint32_t)(TC_PTAP >> 4) : (uint32_t)l.rate;
+    constexpr uint32_t a_lo = (PACKED ? 2 * TC_PR * 16 : TC_APLANE) >> 4;
     float acc[MH][NS / 2];
 #pragma unroll
     for (int m = 0; m < MH; ++m)
 #pragma unroll
         for (int i = 0; i < NS / 2; ++i) acc[m][i] = 0.f;
-    int prev = 0;                                                     // stage of the slab still in flight
+    auto release = [&](unsigned q) { mbar_arrive_remote(bar64(&S.sbar[q % TC_NSTG]), (q + TC_NSTG) % NC); };
+    unsigned q = q0;
 #pragma unroll 1
-    for (int ks = 0; ks < nslab; ++ks) {
+    for (int ks = 0; ks < nslab; ++ks, ++q) {
         uint32_t bt[NTAPS];
 #pragma unroll
         for (int tap = 0; tap < NTAPS; ++tap) bt[tap] = S.tc_baddr[tap * nslab + ks];
-        const uint32_t aa = a_base + (uint32_t)stg * (TC_ASTAGE >> 4);
-        mbar_wait(bar64(&S.abar[stg]), use & 1u);                     // the slab is staged (its bulk copies completed)
+        const unsigned stg = q % TC_NSTG;
+        const uint32_t aa = a_base + stg * (TC_ASTAGE >> 4);
+        mbar_wait(bar64(&S.abar[stg]), (q / TC_NSTG) & 1u);          // the slab is staged (its bulk copies completed)
+        wlap(LP_WG_AWAIT);
         wg_fence();
 #pragma unroll
         for (int tap = 0; tap < NTAPS; ++tap) {
@@ -584,7 +618,7 @@ __device__ __forceinline__ void pyr_mma_rows(const DecParams& P, Smem& S, int li
 #pragma unroll
             for (int m = 0; m < MH; ++m) {                            // rows 64 m .. 64 m + 63: 64 rows of 16 bytes further
                 const uint32_t a = aa + (uint32_t)tap * tap_step + 64u * m;
-                const uint64_t da_hi = dA0 | a, da_lo = dA0 | (a + (TC_APLANE >> 4));
+                const uint64_t da_hi = dA0 | a, da_lo = dA0 | (a + a_lo);
                 wgmma_f16<NS / 16>(acc[m], da_hi, db_hi, (ks | tap) != 0);
                 wgmma_f16<NS / 16>(acc[m], da_hi, db_lo, 1u);
                 wgmma_f16<NS / 16>(acc[m], da_lo, db_hi, 1u);
@@ -592,14 +626,14 @@ __device__ __forceinline__ void pyr_mma_rows(const DecParams& P, Smem& S, int li
         }
         wg_commit();
         wg_wait<1>();                                                 // slab ks - 1 is multiplied: its stage may be refilled
-        if (ks > 0 && leader) mbar_arrive(bar64(&S.sbar[prev]));
-        prev = stg;
-        if (++stg == TC_NSTG) { stg = 0; ++use; }
+        if (ks > 0 && leader) release(q - 1);
+        wlap(LP_WG_MMA);
     }
     wg_wait<0>();
 #pragma unroll
     for (int m = 0; m < MH; ++m) wg_fence_regs(acc[m]);
-    if (leader) mbar_arrive(bar64(&S.sbar[prev]));
+    if (leader) release(q - 1);
+    wlap(LP_WG_MMA);
     const float inv = P.inv_scale[li];
     const float* bs = P.bias[li];
 #pragma unroll
@@ -619,55 +653,111 @@ __device__ __forceinline__ void pyr_mma_rows(const DecParams& P, Smem& S, int li
                                                                      fmaf(acc[m][i * 4 + 2 * h + 1], inv, bq.y));
             }
         }
+    wlap(LP_WG_EPI);
 }
 
-// The slab pipeline has no block barrier.  Thread 0 stages slab q into stage s with bulk copies completing on abar[s];
-// warpgroup 1 waits for abar[s], issues the split-fp16 products of every tap and releases the stage through sbar[s], which
-// thread 0 waits for before it overwrites it.  Slabs are numbered through the whole launch (st.tcq): slab q lives in stage
-// q % TC_NSTG and is that stage's (q / TC_NSTG)-th use, which gives every wait its phase parity without any shared counter.
+// The slab pipeline has no block barrier, and every slab is fetched from L2 once per cluster: every CTA needs the whole K
+// of the same source rows for its own output columns, so slab q is staged by ONE CTA, rank q % NC, with bulk copies
+// multicast to the same stage of all NC CTAs, each completing on that CTA's own abar[s].  Slabs are numbered through the
+// whole launch (st.tcq, the same in every CTA: the moved mask is computed identically everywhere): slab q lives in stage
+// s = q % TC_NSTG and is that stage's (q / TC_NSTG)-th use, which gives every wait its phase parity without a shared counter.
+//   * Thread 0 of every CTA arms abar[s] for slab q (expected bytes) once its previous slab in that stage has landed, so
+//     the arming opens the right phase; the multicast may land before the arming (the transaction count then runs negative
+//     until it).
+//   * Stage s may be overwritten with slab q once every CTA's MMA warpgroup has multiplied slab q - TC_NSTG.  Those NC
+//     releases go to sbar[s] of the CTA that stages slab q, and to no other CTA: sbar[s] of CTA r then counts releases of
+//     the slabs q - TC_NSTG with q = r mod NC and q = s mod TC_NSTG only, one every TC_QCYC slabs, and the slab after
+//     cannot be released before this CTA has staged the slab in between -- so no release is ever counted in the wrong
+//     phase, and the phase of slab q's wait is (q - TC_NSTG) / TC_QCYC.
 // Source of the slabs: the plane history of the block's input (rows t_lo - halo .. t_lo + n_out - 1 of utterance b: four
 // runs of n_src rows, the zero rows in front of t = 0 included), or for the first AudioDec block the cluster's plane
 // scratch of the recomputed rows, `c1` (a whole stage per slab).
+template <bool PROF>
 __device__ __forceinline__ void pyr_tc_utt(const DecParams& P, Smem& S, int li, unsigned q0, int b, int t_lo, int n_out,
                                         int rank, float* scr_rows, const __half* c1) {
     const DecLayer& l = P.L[li];
     const int tid = threadIdx.x, warp = tid >> 5;
-    unsigned use = q0 / TC_NSTG;
-    int stg = (int)(q0 - use * TC_NSTG);
     if (tid == 0) {
-        const int halo = (l.ntaps - 1) * l.rate, n_src = n_out + halo;   // <= 96 (pack_decode)
+        const int halo = (l.ntaps - 1) * l.rate, n_src = n_out + halo;   // <= TC_RA (pack_decode)
         const int nslab = l.cin / 16;
         const size_t run = (size_t)P.pl_rows * 8;                     // halfs between the four (plane, k8) runs of a slab
         const __half* src = c1 ? c1 : P.pl_hist[li] + pl_idx(nslab, P.pl_rows, b, 0, t_lo - halo);
         const size_t sstep = c1 ? (size_t)TC_ASTAGE / 2 : 4 * run;    // halfs per slab
         const uint32_t rb = (uint32_t)n_src * 16;
+        const uint16_t all = (uint16_t)((1u << NC) - 1u);
         fence_proxy_async_global();
+        unsigned q = q0;
 #pragma unroll 1
-        for (int ks = 0; ks < nslab; ++ks, src += sstep) {
-            if (use > 0) mbar_wait(bar64(&S.sbar[stg]), (use - 1) & 1u);   // the MMAs that read this stage are done
+        for (int ks = 0; ks < nslab; ++ks, src += sstep, ++q) {
+            const unsigned stg = q % TC_NSTG, use = q / TC_NSTG;
+            if (use > 0) mbar_wait(bar64(&S.abar[stg]), (use - 1) & 1u);   // this CTA's previous slab in the stage has landed
+            mbar_expect_tx(bar64(&S.abar[stg]), c1 ? (uint32_t)TC_ASTAGE : 4 * rb);
+            if (q % NC != (unsigned)rank) continue;
+            if (use > 0) mbar_wait(bar64(&S.sbar[stg]), ((q - TC_NSTG) / TC_QCYC) & 1u);   // every CTA has multiplied slab q - TC_NSTG
             unsigned char* dst = &S.tca[stg][0];
             if (c1) {
-                mbar_expect_tx(bar64(&S.abar[stg]), TC_ASTAGE);
-                bulk_g2s(dst, src, TC_ASTAGE, &S.abar[stg]);
+                bulk_g2s_mc(dst, src, TC_ASTAGE, &S.abar[stg], all);
             } else {
-                mbar_expect_tx(bar64(&S.abar[stg]), 4 * rb);
 #pragma unroll
                 for (int r = 0; r < 4; ++r)                           // (plane, k8 group) = (r >> 1, r & 1)
-                    bulk_g2s(dst + (r >> 1) * TC_APLANE + (r & 1) * (TC_RA * 16), src + r * run, rb, &S.abar[stg]);
+                    bulk_g2s_mc(dst + (r >> 1) * TC_APLANE + (r & 1) * (TC_RA * 16), src + r * run, rb, &S.abar[stg], all);
             }
-            if (++stg == TC_NSTG) { stg = 0; ++use; }
         }
     } else if (warp >= 4) {                                           // shapes checked by pack_decode: hc 32 columns x 3 taps, conv 16 x 1
         if (l.ns == 32) {
-            if (n_out > 64) pyr_mma_rows<32, 3, 2>(P, S, li, use, stg, n_out, rank, scr_rows);
-            else pyr_mma_rows<32, 3, 1>(P, S, li, use, stg, n_out, rank, scr_rows);
+            if (n_out > 64) pyr_mma_rows<PROF, 32, 3, 2, false>(P, S, li, q0, n_out, rank, scr_rows);
+            else pyr_mma_rows<PROF, 32, 3, 1, false>(P, S, li, q0, n_out, rank, scr_rows);
         } else {
-            if (n_out > 64) pyr_mma_rows<16, 1, 2>(P, S, li, use, stg, n_out, rank, scr_rows);
-            else pyr_mma_rows<16, 1, 1>(P, S, li, use, stg, n_out, rank, scr_rows);
+            if (n_out > 64) pyr_mma_rows<PROF, 16, 1, 2, false>(P, S, li, q0, n_out, rank, scr_rows);
+            else pyr_mma_rows<PROF, 16, 1, 1, false>(P, S, li, q0, n_out, rank, scr_rows);
         }
     }
     // no block barrier: thread 0 goes on to the next utterance's slabs while this one's rows are stored (the stage
     // mbarriers order them); the caller synchronises once after the block's last utterance
+}
+
+// The short blocks (n <= 4 refreshed rows per utterance: HC_5, HC_6) as ONE M = 64 tile for all moved utterances of the
+// frame: tile row m = k * n + i is row i of the k-th moved utterance, which is also its scratch row.  A dilated tap of a
+// window would need the whole 2 * rate + n row window per utterance, so each slab is staged as one image per tap instead,
+// holding only the rows that tap reads ([tap][plane][k8 group][TC_PR rows][8 halfs]; rows t_lo - halo + tap * rate ..
+// + n - 1 of every moved utterance).  Every tile row sees the same k sequence on the same bytes as in its own tile, and
+// rows >= k * n are thrown away.  Staging, multicast and release as in pyr_tc_utt.
+template <bool PROF>
+__device__ __forceinline__ void pyr_tc_packed(const DecParams& P, Smem& S, int li, unsigned q0, int b0, const PreRows& rl,
+                                           int rank, float* scr) {
+    const DecLayer& l = P.L[li];
+    const int tid = threadIdx.x, warp = tid >> 5;
+    if (tid == 0) {
+        const int halo = (l.ntaps - 1) * l.rate, nslab = l.cin / 16, nu = __popc(rl.mask);
+        const size_t run = (size_t)P.pl_rows * 8;                     // halfs between the four (plane, k8) runs of a slab
+        const uint32_t rb = (uint32_t)rl.n * 16;
+        const uint16_t all = (uint16_t)((1u << NC) - 1u);
+        fence_proxy_async_global();
+        unsigned q = q0;
+#pragma unroll 1
+        for (int ks = 0; ks < nslab; ++ks, ++q) {
+            const unsigned stg = q % TC_NSTG, use = q / TC_NSTG;
+            if (use > 0) mbar_wait(bar64(&S.abar[stg]), (use - 1) & 1u);   // this CTA's previous slab in the stage has landed
+            mbar_expect_tx(bar64(&S.abar[stg]), (uint32_t)(3 * 4 * nu) * rb);
+            if (q % NC != (unsigned)rank) continue;
+            if (use > 0) mbar_wait(bar64(&S.sbar[stg]), ((q - TC_NSTG) / TC_QCYC) & 1u);   // every CTA has multiplied slab q - TC_NSTG
+            unsigned char* dst = &S.tca[stg][0];
+            unsigned mk = rl.mask;
+#pragma unroll 1
+            for (int k = 0; k < nu; ++k, mk &= mk - 1) {
+                const int g = __ffs(mk) - 1;
+                const __half* src = P.pl_hist[li] + pl_idx(nslab, P.pl_rows, b0 + g, ks * 16, rl.t_lo - halo);
+#pragma unroll 1
+                for (int tap = 0; tap < 3; ++tap)
+#pragma unroll
+                    for (int r = 0; r < 4; ++r)                       // (plane, k8 group) = (r >> 1, r & 1)
+                        bulk_g2s_mc(dst + tap * TC_PTAP + r * (TC_PR * 16) + k * rb, src + (size_t)tap * l.rate * 8 + r * run, rb,
+                                    &S.abar[stg], all);
+            }
+        }
+    } else if (warp >= 4) {                                           // hc blocks only (pack_decode: 32 columns x 3 taps)
+        pyr_mma_rows<PROF, 32, 3, 1, true>(P, S, li, q0, rl.total, rank, scr);
+    }
 }
 
 // LayerNorm / gate / highway mix of the refreshed rows: one warp per row over the whole cluster (parameters in S.red)
@@ -763,25 +853,32 @@ __device__ __forceinline__ Stream prepass(const DecParams& P, Smem& S, Stream st
                     if (lane < NWARP) mbar_wait(bar64(&S.fullw[pp % DEC_NSLOT][lane]), (pp / DEC_NSLOT) & 1u);
                 }
                 __syncwarp();
+                LAP(LP_PYR_WTS);
                 const PreRows rl = pre_rows(S, G, j, l.prow);
                 if (rl.n > 0) {
                     pyr_tc_table(P, S, lp, st.pos);
                     __syncthreads();
-                    for (int g = 0; g < G; ++g) {
+                    LAP(LP_PYR_TABLE);
+                    if (l.ns == 32 && (l.prow - 1) * GMAX <= TC_PR) {   // short block: one tile for all moved utterances
+                        pyr_tc_packed<PROF>(P, S, lp, st.tcq, b0, rl, rank, scr);
+                        st.tcq += l.cin / 16;
+                    } else for (int g = 0; g < G; ++g) {
                         if (!((rl.mask >> g) & 1u)) continue;
                         float* rows = scr + (size_t)pre_off_of(rl, g) * 512;
-                        pyr_tc_utt(P, S, lp, st.tcq, b0 + g, rl.t_lo, rl.n, rank, rows, lp == P.n_enc ? c1s + (size_t)g * c1_utt : nullptr);
+                        pyr_tc_utt<PROF>(P, S, lp, st.tcq, b0 + g, rl.t_lo, rl.n, rank, rows, lp == P.n_enc ? c1s + (size_t)g * c1_utt : nullptr);
                         st.tcq += l.cin / 16;
                     }
+                    LAP(LP_PYR_STAGE);
                 }
                 __syncthreads();                          // every warp is done with every region of these chunks
+                LAP(LP_PYR_DRAIN);
                 for (int c = 0; c < l.nch; ++c) {
                     if (lane == 0) { fence_proxy_async_smem(); stream_issue(P, S, st, st.prod, (int)(st.pos % DEC_NSLOT), warp); }
                     stream_advance(P, S, st);
                 }
                 for (int i = tid; i < 256; i += NT)       // this block's LayerNorm parameters for pyr_ln
                     *reinterpret_cast<float4*>(&S.red[0][0] + i * 4) = __ldg(reinterpret_cast<const float4*>(P.lnp[lp]) + i);
-                LAP(LP_PYR_GEMM);
+                LAP(LP_PYR_REFILL);
                 cluster_sync_all();
                 LAP(LP_PYR_BAR);
                 pyr_ln(P, S, lp, b0, rl, rank, scr);
@@ -817,14 +914,14 @@ decode_cluster_kernel(const __grid_constant__ DecParams Pc) {
         for (int s = 0; s < DEC_NSLOT; ++s)
             for (int w = 0; w < NWARP; ++w) mbar_init(bar64(&S.fullw[s][w]), 1);
         mbar_init(bar64(&S.gbar[0]), 1); mbar_init(bar64(&S.gbar[1]), 1);
-        for (int i = 0; i < TC_NSTG; ++i) { mbar_init(bar64(&S.sbar[i]), 1); mbar_init(bar64(&S.abar[i]), 1); }
+        for (int i = 0; i < TC_NSTG; ++i) { mbar_init(bar64(&S.sbar[i]), NC); mbar_init(bar64(&S.abar[i]), 1); }
         fence_mbar_init();
     }
     for (int i = tid; i < 2 * GMAX * XLD; i += NT) (&S.xin[0][0][0])[i] = 0.f;
     for (int i = tid; i < 2 * NC * PLD; i += NT) (&S.pre[0][0][0])[i] = 0.f;
     if (tid < GMAX) { S.p_cur[tid] = 0; S.p_prev[tid] = 0; S.p_next[tid] = 0; S.moved[tid] = 0; }
     if (tid < 2) S.fmoved[tid] = 0;
-    if (tid < 16) S.prof[tid] = 0;
+    if (tid < DEC_NPROF) S.prof[tid] = 0;
     if (tid == 0) { S.n_moved_frames = 0; S.n_moved_utt = 0; }
     __syncthreads();
 
@@ -886,7 +983,7 @@ decode_cluster_kernel(const __grid_constant__ DecParams Pc) {
     }
     if (rank == 0 && tid < G) P.p_final[b0 + tid] = S.p_cur[tid];
     if (rank == 0 && tid == 0 && P.stats) { P.stats[2 * cluster] = S.n_moved_frames; P.stats[2 * cluster + 1] = S.n_moved_utt; }
-    if (PROF && P.prof && cluster == 0 && rank == 0 && tid < 16) P.prof[tid] = S.prof[tid];
+    if (PROF && P.prof && cluster == 0 && rank == 0 && tid < DEC_NPROF) P.prof[tid] = S.prof[tid];
     cp_async_wait<0>();
     cluster_sync_all();                                   // no CTA exits while a peer may still write into its shared memory
 }

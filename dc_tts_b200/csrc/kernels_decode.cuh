@@ -18,7 +18,8 @@ constexpr int DEC_SLOT_F = 8 * DEC_REG_F;   // 48 KB per slot
 constexpr int DEC_MAXL = 24;        // 13 AudioEnc + 11 AudioDec blocks
 constexpr int DEC_MAXCH = 48;       // weight chunks per frame
 constexpr int DEC_PRM_F = 1024 + 64;   // per-layer parameter block: gamma1 | beta1 | gamma2 | beta2 (256 each) | bias slice
-constexpr int DEC_PL_PAD = 96;      // zero rows in front of t = 0 in the split-fp16 plane histories (>= the tallest source window)
+constexpr int DEC_PL_PAD = 88;      // zero rows in front of t = 0 in the split-fp16 plane histories (>= the tallest source window: 84 rows)
+constexpr int DEC_NPROF = 24;       // lap-timer buckets (option decode_prof; dctts_decode_profile lists them)
 
 struct DecLayer {
     int kind;        // 0 conv1d (LN, optional relu), 1 hc (two LNs, sigmoid gate, highway mix)
@@ -58,7 +59,7 @@ struct DecParams {
     int* p_final;                      // (B) window after the last step
     float inv_scale[DEC_MAXL];         // 1 / (power-of-two scale of the block's split-fp16 weight planes), tensor-core pre-pass
     int* stats;                        // [clusters][2]: frames with a window move, utterance-frames recomputed
-    long long* prof;                   // optional [16] SM-clock lap timers of cluster 0 / rank 0 (option decode_prof), else nullptr
+    long long* prof;                   // optional [DEC_NPROF] SM-clock lap timers of cluster 0 / rank 0 (option decode_prof), else nullptr
     int nl, n_enc, nch, nch_enc, pyr_ch0, pyr_ch1, stream_len;   // pyr_ch0..pyr_ch1: chunks of the AudioDec blocks with prow > 1
     int B, G, T, N, d, n_mels, win_size, steps;
     int force_prepass;                 // option decode_force_prepass: every utterance recomputes at every frame j >= 1

@@ -188,6 +188,11 @@ __device__ __forceinline__ uint32_t mapa(uint32_t smem_addr, uint32_t rank);
 __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
     asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" :: "r"(mapa(smem_u32(bar), rank)) : "memory");
 }
+// the same with release semantics at CTA scope only: the caller's MMAs, whose reads it announces, have completed
+// (wgmma.wait_group), and cluster scope would make every arrive wait for the thread's earlier global stores
+__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t rank) {
+    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" :: "r"(mapa(smem_u32(bar), rank)) : "memory");
+}
 // named barrier of `n` threads (ids 1..15; 0 is __syncthreads)
 __device__ __forceinline__ void named_sync(int id, int n) { asm volatile("bar.sync %0, %1;" :: "r"(id), "r"(n) : "memory"); }
 

@@ -123,10 +123,11 @@ class Engine:
 
     def decode_profile(self):
         """Lap timers (SM cycles) of the last persistent decode run with option decode_prof = 1; see include/dctts.h."""
-        v = (C.c_int64 * 14)()
-        self._check(self._lib.dctts_decode_profile(self._h, v, 14), "dctts_decode_profile")
         names = ["start", "stream_wait", "gemv", "release", "gather", "cluster_barrier", "layernorm", "mix", "attention",
-                 "re_attention", "re_gemm", "re_layernorm", "re_barriers", "frame"]
+                 "re_attention", "re_weights", "re_table", "re_stage", "re_drain", "re_refill", "re_layernorm", "re_barriers",
+                 "frame", "wg_a_wait", "wg_mma", "wg_epilogue"]
+        v = (C.c_int64 * len(names))()
+        self._check(self._lib.dctts_decode_profile(self._h, v, len(names)), "dctts_decode_profile")
         return dict(zip(names, [int(x) for x in v]))
 
     def reserve(self, batch):

@@ -279,8 +279,12 @@ int dctts_get_option(dctts_handle h, const char* name, int32_t* value);
  * clusters launched.  Synchronises the device. */
 int dctts_decode_stats(dctts_handle h, int32_t* moved_frames, int32_t* moved_utterance_frames, int32_t* clusters);
 /* SM-clock lap timers (cycles) of the last persistent decode run with option "decode_prof" = 1: cluster 0, CTA rank 0.
- * Buckets: 0 block start, 1 weight-stream wait, 2 GEMV, 3 slot release, 4 all-gather, 5 cluster barrier, 6 LayerNorm, 7 mix,
- * 8 attention, 9 recompute attention, 10 recompute GEMM, 11 recompute LayerNorm, 12 recompute barriers, 13 frame bookkeeping. */
+ * n <= 24.  Buckets of thread 0, which together cover the kernel: 0 block start, 1 weight-stream wait, 2 GEMV, 3 slot release,
+ * 4 all-gather, 5 cluster barrier, 6 LayerNorm, 7 mix, 8 attention, 9 recompute attention; the recompute GEMM as 10 waiting
+ * for the block's weight chunks, 11 descriptor table, 12 issuing the A slabs, 13 draining the MMAs and epilogue stores,
+ * 14 weight refill and LayerNorm parameters; 15 recompute LayerNorm, 16 recompute barriers, 17 frame bookkeeping.
+ * Buckets of the recompute's MMA warpgroup (thread 128), which overlap the above: 18 waiting for A slabs, 19 issuing the MMAs
+ * and waiting for the slab before, 20 epilogue stores. */
 int dctts_decode_profile(dctts_handle h, int64_t* cycles, int32_t n);
 /* Measurement aid for bench.py's roofline leg: runs the block `scope` on a synthetic
  * (B,L,Cin) input `warmup`+`iters` times and returns the mean device time of each of its
