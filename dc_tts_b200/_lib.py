@@ -58,6 +58,8 @@ SIGNATURES = {
     "dctts_train_step": (C.c_int, [Handle, _p, _p, _i32, _i64, C.c_uint32, C.c_float, _i32, C.POINTER(C.c_float), _p]),
     "dctts_train_step_shaped": (C.c_int, [Handle, _p, _i32, _p, _i32, _i32, _i64, C.c_uint32, C.c_float, _i32, C.POINTER(C.c_float), _p]),
     "dctts_train_apply": (C.c_int, [Handle, _i64, C.c_float, _p]),
+    "dctts_train_eval": (C.c_int, [Handle, _p, _i32, _p, _i32, _i32, C.c_uint32, _p, _p, C.POINTER(C.c_float), _p]),
+    "dctts_train_eval_ssrn": (C.c_int, [Handle, _p, _p, _i32, _i32, C.c_uint32, _p, C.POINTER(C.c_float), _p]),
     "dctts_train_init_ssrn": (C.c_int, [Handle, _i32, _i32, C.c_float]),
     "dctts_train_step_ssrn": (C.c_int, [Handle, _p, _p, _i32, _i64, C.c_uint32, C.c_float, _i32, C.POINTER(C.c_float), _p]),
     "dctts_train_step_ssrn_shaped": (C.c_int, [Handle, _p, _p, _i32, _i32, _i64, C.c_uint32, C.c_float, _i32, C.POINTER(C.c_float), _p]),

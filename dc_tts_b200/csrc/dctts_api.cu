@@ -1552,9 +1552,14 @@ void train_read_losses(H* h, float* losses_host, double n_el, double n_att, cuda
 // means over B T n_mels, and the guided-attention sum over the n_lim x t_lim corner of the (max_N, max_T) table divided by
 // B n_lim t_lim, n_lim = min(N, max_N), t_lim = min(T, max_T) (the -1 padding of train.py:91 is cropped to the table).  The
 // softmax sees N keys and TextEnc's SAME padding the edge at N.
-void train_forward_backward(H* h, const int* L, int N, const float* mels, int T, int B, uint32_t seed, float* losses_host,
-                            cudaStream_t s) {
+//
+// The forward half, shared by the step and dctts_train_eval: the shape checks (before any launch), the forward with the
+// step's dropout mask, the attention on the kernel set train_tc selects, and the mel losses into sums[0..1] (their gradient
+// into gbuf[0]).  It writes the workspace, the loss sums and the abs-max slots (which every step clears again first), never
+// the variables, the gradient arena or the Adam moments.
+void train_forward(H* h, Launch& lc, const int* L, int N, const float* mels, int T, int B, uint32_t seed) {
     auto& tr = h->tr;
+    cudaStream_t s = lc.s;
     REQUIRE(tr.ready && tr.num == 1 && tr.B == B, "dctts_train_step: call dctts_train_init with this batch size first");
     const dctts_hparams& hp = h->hp;
     REQUIRE(N >= 1 && N <= tr.N_cap && T >= 1 && T <= tr.T_cap,
@@ -1564,8 +1569,6 @@ void train_forward_backward(H* h, const int* L, int N, const float* mels, int T,
             "; dctts_train_reserve grows it)");
     const int d = hp.d;
     train_set_shape(h, N, T);
-    Launch lc{h, s};
-    CUDA_CHECK(cudaMemsetAsync(tr.grads.p, 0, tr.n_grad * sizeof(float), s));
     CUDA_CHECK(cudaMemsetAsync(tr.sums.p, 0, 4 * sizeof(double), s));
     gemm_tc_begin_step(tr.tc, s); tr.tc.probe = h->opt.train_probe;
     tr.layers[tr.first[1]].in = mels;
@@ -1585,6 +1588,18 @@ void train_forward_backward(H* h, const int* L, int N, const float* mels, int T,
     const auto& lastl = tr.layers[tr.last[2]];
     launch_train_loss(lastl.out, lastl.ld_out, mels, tr.gbuf[0].as<float>(), lastl.ld_out, tr.sums.as<double>(), (long long)B * T, hp.n_mels, s);
     lc.count();
+}
+
+void train_forward_backward(H* h, const int* L, int N, const float* mels, int T, int B, uint32_t seed, float* losses_host,
+                            cudaStream_t s) {
+    auto& tr = h->tr;
+    const dctts_hparams& hp = h->hp;
+    const int d = hp.d;
+    Launch lc{h, s};
+    train_forward(h, lc, L, N, mels, T, B, seed);
+    CUDA_CHECK(cudaMemsetAsync(tr.grads.p, 0, tr.n_grad * sizeof(float), s));
+    const float* KV = tr.layers[tr.last[0]].out;
+    const float* Q = tr.layers[tr.last[1]].out;
     float* gR = train_bwd(h, lc, tr.first[2], tr.last[2], B, seed, tr.gbuf[0].as<float>(), tr.gbuf[1].as<float>());
     AttnBwdArgs ab{};
     ab.gR = gR; ab.Q = Q; ab.ldq = d; ab.K = KV; ab.V = KV + d; ab.ldkv = 2 * d; ab.align = tr.align.as<float>();
@@ -1601,17 +1616,36 @@ void train_forward_backward(H* h, const int* L, int N, const float* mels, int T,
     train_read_losses(h, losses_host, (double)B * T * hp.n_mels, (double)B * n_lim * t_lim, s);
 }
 
-// SSRN (num = 2): ground-truth mels (B, T, n_mels) in, L1 + binary divergence against the linear magnitudes (B, 4T, F), means
-// over B 4T F (train.py:100-108); T up to the capacity given to dctts_train_init_ssrn or grown by dctts_train_reserve
-void train_forward_backward_ssrn(H* h, const float* mels, const float* mags, int B, int T, uint32_t seed, float* losses_host,
-                                 cudaStream_t s) {
+// An evaluation of the Text2Mel training graph without an update (what the reference's sess.run(g.alignments) or
+// sess.run(g.merged) computes on a batch): train_forward, then the guided-attention sum alone, and copies of
+// Y = sigmoid(logits) (B, T, n_mels) and the alignments (B, N, T) into the caller's device buffers when they are given.
+void train_eval(H* h, const int* L, int N, const float* mels, int T, int B, uint32_t seed, float* Y_out, float* align_out,
+                float* losses_host, cudaStream_t s) {
     auto& tr = h->tr;
+    const dctts_hparams& hp = h->hp;
+    Launch lc{h, s};
+    train_forward(h, lc, L, N, mels, T, B, seed);
+    const int n_lim = std::min(N, hp.max_N), t_lim = std::min(T, hp.max_T);
+    launch_attn_loss(tr.align.as<float>(), tr.gts.as<float>(), hp.max_T, tr.sums.as<double>(), B, N, T, n_lim, t_lim, s); lc.count();
+    if (Y_out) {
+        const auto& lastl = tr.layers[tr.last[2]];
+        launch_sigmoid_rows(lastl.out, lastl.ld_out, Y_out, (long long)B * T, hp.n_mels, s); lc.count();
+    }
+    if (align_out) CUDA_CHECK(cudaMemcpyAsync(align_out, tr.align.p, (size_t)B * N * T * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    CUDA_CHECK(cudaGetLastError());
+    train_read_losses(h, losses_host, (double)B * T * hp.n_mels, (double)B * n_lim * t_lim, s);
+}
+
+// SSRN (num = 2): ground-truth mels (B, T, n_mels) in, L1 + binary divergence against the linear magnitudes (B, 4T, F), means
+// over B 4T F (train.py:100-108); T up to the capacity given to dctts_train_init_ssrn or grown by dctts_train_reserve.
+// The forward half, shared by the step and dctts_train_eval_ssrn (same contract as train_forward).
+void train_forward_ssrn(H* h, Launch& lc, const float* mels, const float* mags, int B, int T, uint32_t seed) {
+    auto& tr = h->tr;
+    cudaStream_t s = lc.s;
     REQUIRE(tr.ready && tr.num == 2 && tr.B == B, "dctts_train_step_ssrn: call dctts_train_init_ssrn with this batch size first");
     REQUIRE(T >= 1 && T <= tr.T_cap, "dctts_train_step_ssrn: T = " + std::to_string(T) + " outside the handle's capacity (1.." +
             std::to_string(tr.T_cap) + ", set by dctts_train_init_ssrn" + (tr.T_cap != tr.T_in ? " and dctts_train_reserve)" : ")"));
     train_set_shape(h, 0, T);
-    Launch lc{h, s};
-    CUDA_CHECK(cudaMemsetAsync(tr.grads.p, 0, tr.n_grad * sizeof(float), s));
     CUDA_CHECK(cudaMemsetAsync(tr.sums.p, 0, 4 * sizeof(double), s));
     gemm_tc_begin_step(tr.tc, s); tr.tc.probe = h->opt.train_probe;
     tr.layers[0].in = mels;
@@ -1619,7 +1653,29 @@ void train_forward_backward_ssrn(H* h, const float* mels, const float* mags, int
     train_fwd(h, lc, 0, last, B, seed);
     const auto& ll = tr.layers[last];
     launch_train_loss(ll.out, ll.ld_out, mags, tr.gbuf[0].as<float>(), ll.ld_out, tr.sums.as<double>(), ll.rows, ll.l->cout, s); lc.count();
+}
+
+void train_forward_backward_ssrn(H* h, const float* mels, const float* mags, int B, int T, uint32_t seed, float* losses_host,
+                                 cudaStream_t s) {
+    auto& tr = h->tr;
+    Launch lc{h, s};
+    train_forward_ssrn(h, lc, mels, mags, B, T, seed);
+    CUDA_CHECK(cudaMemsetAsync(tr.grads.p, 0, tr.n_grad * sizeof(float), s));
+    const int last = (int)tr.layers.size() - 1;
     train_bwd(h, lc, 0, last, B, seed, tr.gbuf[0].as<float>(), tr.gbuf[1].as<float>());
+    CUDA_CHECK(cudaGetLastError());
+    const auto& ll = tr.layers[last];
+    train_read_losses(h, losses_host, (double)ll.rows * ll.l->cout, 0.0, s);
+}
+
+// The SSRN counterpart of train_eval: Z = sigmoid(logits) (B, 4T, F) packed from the last block's padded rows
+void train_eval_ssrn(H* h, const float* mels, const float* mags, int B, int T, uint32_t seed, float* Z_out, float* losses_host,
+                     cudaStream_t s) {
+    auto& tr = h->tr;
+    Launch lc{h, s};
+    train_forward_ssrn(h, lc, mels, mags, B, T, seed);
+    const auto& ll = tr.layers.back();
+    if (Z_out) { launch_sigmoid_rows(ll.out, ll.ld_out, Z_out, ll.rows, ll.l->cout, s); lc.count(); }
     CUDA_CHECK(cudaGetLastError());
     train_read_losses(h, losses_host, (double)ll.rows * ll.l->cout, 0.0, s);
 }
@@ -2298,6 +2354,22 @@ int dctts_train_step_shaped(dctts_handle h, const int32_t* L, int32_t N, const f
 int dctts_train_step(dctts_handle h, const int32_t* L, const float* mels, int32_t B, int64_t global_step, uint32_t seed, float lr,
                      int32_t apply, float* losses_host, void* stream) {
     return dctts_train_step_shaped(h, L, h ? h->hp.max_N : 0, mels, h ? h->hp.max_T : 0, B, global_step, seed, lr, apply, losses_host, stream);
+}
+
+int dctts_train_eval(dctts_handle h, const int32_t* L, int32_t N, const float* mels, int32_t T, int32_t B, uint32_t seed,
+                     float* Y_out, float* align_out, float* losses_host, void* stream) {
+    return guarded(h, [&] {
+        REQUIRE(L && mels && B >= 1, "dctts_train_eval: bad arguments");
+        train_eval(h, reinterpret_cast<const int*>(L), N, mels, T, B, seed, Y_out, align_out, losses_host, S(h, stream));
+    });
+}
+
+int dctts_train_eval_ssrn(dctts_handle h, const float* mels, const float* mags, int32_t B, int32_t T, uint32_t seed, float* Z_out,
+                          float* losses_host, void* stream) {
+    return guarded(h, [&] {
+        REQUIRE(mels && mags && B >= 1, "dctts_train_eval_ssrn: bad arguments");
+        train_eval_ssrn(h, mels, mags, B, T, seed, Z_out, losses_host, S(h, stream));
+    });
 }
 
 int dctts_train_apply(dctts_handle h, int64_t global_step, float lr, void* stream) {

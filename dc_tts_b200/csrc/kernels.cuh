@@ -221,6 +221,11 @@ void launch_train_block_bwd(const BlockBwdArgs& a, cudaStream_t s);
 void launch_conv_wgrad(WgradArgs a, cudaStream_t s);
 void launch_transpose_w(const float* W, float* WT, int ntaps, int K, int N, int ldw, int Kp, cudaStream_t s);
 void launch_attn_bwd(const AttnBwdArgs& a, double* sums, cudaStream_t s);
+// the guided-attention sum alone (the first kernel of launch_attn_bwd): sums[2] += sum over the (n_lim, t_lim) corner of |A gts|
+void launch_attn_loss(const float* align, const float* gts, int ld_gts, double* sums, int B, int N, int T, int n_lim, int t_lim,
+                      cudaStream_t s);
+// out (rows, C) dense = sigmoid(x), x (rows, C) with leading dimension ldx
+void launch_sigmoid_rows(const float* x, int ldx, float* out, long long rows, int C, cudaStream_t s);
 void launch_guided_attention(float* W, int N, int T, cudaStream_t s);
 void launch_embed_bwd(const int* ids, const float* g, float* dtable, int rows, int e, cudaStream_t s);
 void launch_adam(const AdamEntry* entries_dev, int n_entries, float lr_t, float beta1, float beta2, float eps, cudaStream_t s);

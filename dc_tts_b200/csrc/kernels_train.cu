@@ -72,6 +72,19 @@ void launch_train_loss(const float* logits, int ldl, const float* target, float*
     train_loss_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(logits, ldl, target, dlogits, ldg, sums, n, C);
 }
 
+// Y = sigmoid(logits) packed from the ld-pitched last block (train.py:68,72), for an evaluation of the training graph
+__global__ void sigmoid_rows_kernel(const float* __restrict__ x, int ldx, float* __restrict__ out, long long n, int C) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const long long row = i / C;
+    out[i] = 1.0f / (1.0f + expf(-x[row * ldx + (i - row * C)]));
+}
+
+void launch_sigmoid_rows(const float* x, int ldx, float* out, long long rows, int C, cudaStream_t s) {
+    const long long n = rows * C;
+    sigmoid_rows_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(x, ldx, out, n, C);
+}
+
 // ------------------------------------------------------------------------------------ block backward
 __device__ __forceinline__ float wsum(float v) {
 #pragma unroll
@@ -382,6 +395,12 @@ __global__ void attn_loss_kernel(const float* __restrict__ align, const float* _
     if (threadIdx.x == 0) { double s = 0.0; for (int k = 0; k < 8; ++k) s += red[k]; atomicAdd(&sums[2], s); }
 }
 
+void launch_attn_loss(const float* align, const float* gts, int ld_gts, double* sums, int B, int N, int T, int n_lim, int t_lim,
+                      cudaStream_t s) {
+    const long long n = (long long)B * N * T;
+    attn_loss_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(align, gts, ld_gts, sums, B, N, T, n_lim, t_lim);
+}
+
 void launch_attn_bwd(const AttnBwdArgs& a, double* sums, cudaStream_t s) {
     if (a.d != 256) throw std::runtime_error("attention backward is built for d = 256");
     if (a.n_lim < 1 || a.n_lim > a.N || a.t_lim < 1 || a.t_lim > a.T || a.ld_gts < a.t_lim)
@@ -397,8 +416,7 @@ void launch_attn_bwd(const AttnBwdArgs& a, double* sums, cudaStream_t s) {
                                      " bytes of shared memory per block, more than the device allows");
         }
     }
-    const long long n = (long long)a.B * a.N * a.T;
-    attn_loss_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a.align, a.gts, a.ld_gts, sums, a.B, a.N, a.T, a.n_lim, a.t_lim);
+    launch_attn_loss(a.align, a.gts, a.ld_gts, sums, a.B, a.N, a.T, a.n_lim, a.t_lim, s);
     attn_bwd_q_kernel<<<(a.B * a.T + 3) / 4, 128, smem, s>>>(a);
     attn_bwd_kv_kernel<<<(a.B * a.N + 3) / 4, 128, 0, s>>>(a);
 }

@@ -482,6 +482,50 @@ class Engine:
                                                            1 if apply else 0, out, self._stream()), "dctts_train_step_ssrn")
         return {"loss": out[0], "loss_mags": out[1], "loss_bd2": out[2]}
 
+    def train_eval(self, L, mels, seed=0, want=("Y", "alignments")):
+        """The Text2Mel training graph evaluated on one batch without an update -- the reference's sess.run(g.alignments)
+        or sess.run(g.merged) (train.py:100-104,156): the step's forward with its dropout mask at `seed`, and its losses at
+        the batch's shape.  Same shapes as train_step.  The variables, Adam moments and the gradient arena are untouched.
+        Returns ({loss, loss_mels, loss_bd1, loss_att}, {name: CUDA tensor}) for the names in `want`: "Y" (B, T, n_mels)
+        and "alignments" (B, N, T)."""
+        L = self._i32(L); mels = self._f32(mels)
+        if L.dim() != 2:
+            raise DcttsError("train_eval: L must be (B, N), got shape %s" % (tuple(L.shape),))
+        B, N = L.shape
+        if mels.dim() != 3 or mels.shape[0] != B or mels.shape[2] != self.hp.n_mels:
+            raise DcttsError("train_eval: mels must be (B=%d, T, n_mels=%d), got shape %s" % (B, self.hp.n_mels, tuple(mels.shape)))
+        unknown = set(want) - {"Y", "alignments"}
+        if unknown:
+            raise DcttsError("train_eval: can return Y and alignments, not %s" % sorted(unknown))
+        T = mels.shape[1]
+        tensors = {}
+        if "Y" in want:
+            tensors["Y"] = self._empty(B, T, self.hp.n_mels)
+        if "alignments" in want:
+            tensors["alignments"] = self._empty(B, N, T)
+        out = (C.c_float * 4)()
+        self._check(self._lib.dctts_train_eval(self._h, _ptr(L), N, _ptr(mels), T, B, int(seed) & 0xffffffff, _ptr(tensors.get("Y")),
+                                               _ptr(tensors.get("alignments")), out, self._stream()), "dctts_train_eval")
+        return {"loss": out[0], "loss_mels": out[1], "loss_bd1": out[2], "loss_att": out[3]}, tensors
+
+    def train_eval_ssrn(self, mels, mags, seed=0, want=("Z",)):
+        """The SSRN counterpart of train_eval (train.py:115-118): returns ({loss, loss_mags, loss_bd2}, {"Z": (B, 4T, F)})."""
+        mels = self._f32(mels); mags = self._f32(mags)
+        if mels.dim() != 3 or mels.shape[2] != self.hp.n_mels:
+            raise DcttsError("train_eval_ssrn: mels must be (B, T, n_mels=%d), got shape %s" % (self.hp.n_mels, tuple(mels.shape)))
+        B, T = mels.shape[0], mels.shape[1]
+        if tuple(mags.shape) != (B, self.hp.r * T, self.F):
+            raise DcttsError("train_eval_ssrn: mags must be (B, %d T, F) = %s for mels %s, got %s"
+                             % (self.hp.r, (B, self.hp.r * T, self.F), tuple(mels.shape), tuple(mags.shape)))
+        unknown = set(want) - {"Z"}
+        if unknown:
+            raise DcttsError("train_eval_ssrn: can return Z, not %s" % sorted(unknown))
+        tensors = {"Z": self._empty(B, self.hp.r * T, self.F)} if "Z" in want else {}
+        out = (C.c_float * 4)()
+        self._check(self._lib.dctts_train_eval_ssrn(self._h, _ptr(mels), _ptr(mags), B, T, int(seed) & 0xffffffff,
+                                                    _ptr(tensors.get("Z")), out, self._stream()), "dctts_train_eval_ssrn")
+        return {"loss": out[0], "loss_mags": out[1], "loss_bd2": out[2]}, tensors
+
     def train_reserve(self, N, T):
         """Grow the training workspace of the network being trained to at least N text positions (Text2Mel; ignored for
         SSRN) and T mel frames, so that train_step / train_step_ssrn accept batches up to that shape.  The variables, Adam

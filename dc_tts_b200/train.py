@@ -13,7 +13,11 @@ losses and `train_op` are fetchable with `Session.run` exactly as train.py:148 d
 g.train_op])`): fetching `train_op` takes the next batch of the input pipeline (data_load.get_batch -> here an iterator of
 (L, mels, mags, ...) batches, dc_tts_b200/trainer.py) and runs ONE optimiser step -- forward with dropout, the losses of
 train.py:83-113, backward, clipping, Adam with the Noam rate (train.py:120-131) -- through `Engine.train_step` /
-`train_step_ssrn`.  Plots and summaries (train.py:100-104,116-119,154-157) are out of scope.
+`train_step_ssrn`.  Fetching `alignments` or `Y` (num = 1), `Z` (num = 2) or `merged` WITHOUT train_op evaluates the
+training graph on the next batch of the pipeline, as TF's queue dequeues one for any run: the forward with dropout and
+its losses, no update, global_step unchanged (`Engine.train_eval`); `merged` is the serialized Summary of train.py's
+summaries (train.py:100-104,115-118,123; dc_tts_b200/summary.py).  trainer.train(..., summaries=True) writes them and
+the alignment plots of train.py:154-157 to logdir.
 """
 import numpy as np
 import torch
@@ -40,6 +44,7 @@ _FUSED_OK = {"Y", "max_attentions", "alignments", "global_step"}
 
 
 _TRAIN = {1: ("loss", "loss_mels", "loss_bd1", "loss_att"), 2: ("loss", "loss_mags", "loss_bd2")}
+_TRAIN_EVAL = {1: ("alignments", "Y", "merged"), 2: ("Z", "merged")}
 
 
 class Graph:
@@ -69,7 +74,7 @@ class Graph:
             from .trainer import Capacity
             self._capacity = Capacity(num, getattr(self.engine, "hp", hp), beyond_capacity, capacity)
             self._initialised = False
-            for name in ("global_step", "train_op", "lr") + _TRAIN[num]:
+            for name in ("global_step", "train_op", "lr") + _TRAIN[num] + _TRAIN_EVAL[num]:
                 setattr(self, name, Symbol(self, name))
             return
         self.global_step_value = 0          # `gs/global_step` (train.py:79-80); no checkpoint offline
@@ -98,7 +103,12 @@ class Graph:
     def _train_run(self, names):
         """One `sess.run` of the training graph: fetching train_op consumes a batch and applies one update."""
         from .utils import learning_rate_decay
-        if "train_op" in names:
+        evals = [n for n in names if n in _TRAIN_EVAL[self.num]]
+        if evals and "train_op" in names:
+            raise ValueError("%s cannot be fetched together with train_op: fetch it in a run of its own, as train.py:156 does"
+                             % ", ".join(evals))
+        out, losses = {}, self.last
+        if "train_op" in names or evals:
             cap, capa = getattr(self.engine, "hp", hp), self._capacity
             L, mels, mags = next(self.batches)[:3]
             while not capa.admit(L, mels, lambda *_: None):      # "skip": counted in skipped_batches
@@ -112,17 +122,23 @@ class Graph:
                 self._initialised = True
             capa.prepare(self.engine, L, mels, lambda *_: None)
             gs = self.global_step_value
+        if evals:
+            from .trainer import evaluate
+            losses, t, merged = evaluate(self.num, self.engine, L, mels, mags, gs, alignments="alignments" in evals)
+            out.update({k: v.cpu().numpy() for k, v in t.items()}, merged=merged)
+        elif "train_op" in names:
             if self.num == 1:
                 self.last = self.engine.train_step(L, mels, global_step=gs, seed=gs)
             else:
                 self.last = self.engine.train_step_ssrn(mels, mags, global_step=gs, seed=gs)
+            losses = self.last
             self.global_step_value = gs + 1                   # apply_gradients(global_step=...) increments (train.py:131)
-        out = {"train_op": None, "global_step": np.int64(self.global_step_value),
-               "lr": np.float32(learning_rate_decay(hp.lr, self.global_step_value))}
-        for k in _TRAIN[self.num]:
-            if k in names and k not in self.last:
+        out.update({"train_op": None, "global_step": np.int64(self.global_step_value),
+                    "lr": np.float32(learning_rate_decay(hp.lr, self.global_step_value))})
+        for k in _TRAIN[self.num]:                            # with an evaluation: the evaluated batch's losses
+            if k in names and k not in losses:
                 raise ValueError("%s: no training step has run yet (fetch it together with train_op)" % k)
-            out[k] = np.float32(self.last.get(k, np.nan))
+            out[k] = np.float32(losses.get(k, np.nan))
         return out
 
     @property

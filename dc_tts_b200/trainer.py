@@ -15,6 +15,7 @@ config 5) and `pad_to_fixed` (a bucket padded further to the fixed shapes) remai
 """
 import codecs
 import os
+import time
 
 import numpy as np
 
@@ -274,8 +275,29 @@ class Capacity:
             log("grew the training workspace to T=%d for a batch of T=%d" % (self.T, mels.shape[1]))
 
 
+# The dropout seed of evaluations of the training graph (summaries, alignment plots).  Steps use the global step, times the
+# world size plus the rank in data-parallel runs, which stays far below it.
+EVAL_SEED = 0xffffffff
+
+
+def evaluate(num, engine, L, mels, mags, global_step, alignments=False):
+    """One forward-only evaluation of the training graph on a batch, with dropout and no update (Engine.train_eval /
+    train_eval_ssrn): returns (losses, CUDA tensors Y [+ alignments] or Z, the merged Summary bytes of train.py's
+    summaries with lr at `global_step`)."""
+    from .summary import train_summary
+    from .utils import learning_rate_decay
+    if num == 1:
+        losses, t = engine.train_eval(L, mels, seed=EVAL_SEED, want=("Y", "alignments") if alignments else ("Y",))
+        target, out = mels, t["Y"]
+    else:
+        losses, t = engine.train_eval_ssrn(mels, mags, seed=EVAL_SEED)
+        target, out = mags, t["Z"]
+    host = lambda x: x[:1].cpu().numpy() if hasattr(x, "cpu") else np.asarray(x[:1])
+    return losses, t, train_summary(num, losses, host(target), host(out), learning_rate_decay(hp.lr, global_step))
+
+
 def train(num, engine, batches, num_iterations=None, logdir=None, global_step=None, save_every=1000, log=print, resume=True,
-          rank=0, world=1, allreduce=None, beyond_capacity="skip", capacity=None):
+          rank=0, world=1, allreduce=None, beyond_capacity="skip", capacity=None, summaries=False, summary_secs=120):
     """train.py:137-160 for num = 1 (Text2Mel) or 2 (SSRN).  `batches` yields (L, mels, mags, names, ...): the bucketed
     batches of `bucketed_batches` at their own shapes or fixed-size ones; `engine` is an `Engine` with parameters loaded.
     The workspace is allocated for the capacity (hp.max_N, hp.max_T), or `capacity` = (N, T) when that is larger; a batch
@@ -285,7 +307,14 @@ def train(num, engine, batches, num_iterations=None, logdir=None, global_step=No
     starts over).  Data parallel (BASELINE config 5, `world` > 1): every rank feeds its own disjoint `batches`, the step
     runs with apply=False, `allreduce` (default dc_tts_b200.parallel.allreduce_mean_) averages the flat gradient arena,
     every rank applies the identical Adam update, dropout masks differ per rank (seed = gs * world + rank) and only rank 0
-    writes checkpoints.  Returns the final global step."""
+    writes checkpoints.
+
+    `summaries=True` adds what the reference's Supervisor and train.py:154-157 write, on rank 0: every `summary_secs`
+    seconds of wall clock (0: after every step), at a step boundary, the next batch of `batches` is evaluated without an
+    update (`evaluate`) and one event with train.py's merged summaries, `lr` and `global_step/sec` goes to a new
+    `events.out.tfevents.*` file in `logdir`; at every checkpoint of Text2Mel the next batch is evaluated and its first
+    alignment written as `alignment_{NNN}k.png` (utils.plot_alignment).  Evaluations consume batches as TF's queue does.
+    Returns the final global step."""
     if num not in (1, 2):
         raise ValueError("num: 1 for Text2Mel, 2 for SSRN (train.py:139)")
     num_iterations = hp.num_iterations if num_iterations is None else num_iterations
@@ -295,10 +324,28 @@ def train(num, engine, batches, num_iterations=None, logdir=None, global_step=No
     cap = getattr(engine, "hp", hp)
     capa = Capacity(num, cap, beyond_capacity, capacity)
     initialised = False
-    for batch in batches:
+    batches = iter(batches)
+    writer = None
+
+    def next_admitted():
+        for b in batches:
+            if capa.admit(b[0], b[1], log):
+                return b
+        return None
+
+    def evaluate_next(alignments=False):
+        """`evaluate` on the next admitted batch, or None when the input pipeline is exhausted."""
+        b = next_admitted()
+        if b is None:
+            return None
+        capa.prepare(engine, b[0], b[1], log)
+        return evaluate(num, engine, b[0], b[1], b[2], gs, alignments)
+
+    while True:
+        batch = next_admitted()
+        if batch is None:
+            break
         L, mels, mags = batch[:3]
-        if not capa.admit(L, mels, log):
-            continue
         if not initialised:
             if num == 1:
                 engine.train_init(len(L))
@@ -311,6 +358,10 @@ def train(num, engine, batches, num_iterations=None, logdir=None, global_step=No
                     log("resumed from %s at global step %d" % (logdir, gs))
             capa.initialised(engine)
             initialised = True
+            if summaries and rank == 0:
+                from .summary import FileWriter, merge, scalar
+                writer = FileWriter(logdir)
+                last_t, last_gs = time.time(), gs
         capa.prepare(engine, L, mels, log)
         if world > 1:
             if allreduce is None:
@@ -330,6 +381,21 @@ def train(num, engine, batches, num_iterations=None, logdir=None, global_step=No
         if gs % save_every == 0 and rank == 0:    # train.py:151-152
             engine.save_checkpoint(checkpoint_name(logdir, gs), gs, "Text2Mel" if num == 1 else "SSRN")
             log("step %d  %s" % (gs, "  ".join("%s %.4f" % kv for kv in sorted(losses.items()))))
+            if writer is not None and num == 1:   # train.py:154-157
+                ev = evaluate_next(alignments=True)
+                if ev is not None:
+                    from .utils import plot_alignment
+                    plot_alignment(ev[1]["alignments"][0].cpu().numpy(), str(gs // 1000).zfill(3) + "k", logdir)
+        if writer is not None and time.time() - last_t >= summary_secs:
+            ev = evaluate_next()
+            now = time.time()
+            if ev is not None:
+                rate = (gs - last_gs) / max(now - last_t, 1e-9)
+                writer.add_summary(merge(ev[2], scalar("global_step/sec", rate)), gs)
+                writer.flush()
+            last_t, last_gs = now, gs
         if gs > num_iterations:                   # train.py:160
             break
+    if writer is not None:
+        writer.close()
     return gs

@@ -10,8 +10,8 @@ pre-emphasis, STFT, mel filterbank, dB, normalisation in two kernels per call, f
 `librosa.load` is replaced by scipy's WAV reader,
 and with `resample=True` a file at another sample rate is resampled to hp.sr on the GPU as librosa.load(fpath, sr=hp.sr)
 does (`dctts_resample_batch`: librosa 0.6 / resampy 'kaiser_best'); without it such a file is refused, so a corpus at an
-unexpected rate is never converted silently.  Other file formats, plotting and the training helpers
-of the reference's utils.py stay out of scope.
+unexpected rate is never converted silently.  `plot_alignment` writes its PNG without matplotlib (no title, axes or
+colorbar).  Other file formats and the remaining training helpers of the reference's utils.py stay out of scope.
 """
 import os
 
@@ -166,6 +166,42 @@ def guided_attention(g=0.2):
     n = np.arange(hp.max_N, dtype=np.float64)[:, None] / float(hp.max_N)
     t = np.arange(hp.max_T, dtype=np.float64)[None, :] / float(hp.max_T)
     return (1.0 - np.exp(-(t - n) ** 2 / (2.0 * g * g))).astype(np.float32)
+
+
+# 256-entry viridis table from a published degree-6 polynomial fit of matplotlib's viridis (per channel, t in [0, 1])
+_VIRIDIS_FIT = np.array([[0.2777273272234177, 0.005407344544966578, 0.3340998053353061],
+                         [0.1050930431085774, 1.404613529898575, 1.384590162594685],
+                         [-0.3308618287255563, 0.214847559468213, 0.09509516302823659],
+                         [-4.634230498983486, -5.799100973351585, -19.33244095627987],
+                         [6.228269936347081, 14.17993336680509, 56.69055260068105],
+                         [4.776384997670288, -13.74514537774601, -65.35303263337234],
+                         [-5.435455855934631, 4.645852612178535, 26.3124352495832]])
+
+
+def _viridis():
+    t = np.linspace(0.0, 1.0, 256)[:, None]
+    rgb = sum(c[None, :] * t ** k for k, c in enumerate(_VIRIDIS_FIT))
+    return np.round(np.clip(rgb, 0, 1) * 255).astype(np.uint8)
+
+
+def plot_alignment(alignment, gs, dir=hp.logdir):
+    """utils.py:116-132: writes `{dir}/alignment_{gs}.png` of an (N, T) alignment -- N rows, T columns, row 0 at the top
+    as imshow draws it, scaled from its min to its max through a 256-entry viridis table and enlarged by an integer factor
+    (at least 400 pixels on the shorter side, at most 4 times).  No title, axes or colorbar (matplotlib is not used).
+    Returns the path."""
+    from .summary import png
+    os.makedirs(dir, exist_ok=True)
+    a = np.asarray(alignment, np.float64)
+    if a.ndim != 2:
+        raise ValueError("plot_alignment: alignment must be (N, T), got shape %s" % (a.shape,))
+    lo, hi = np.nanmin(a), np.nanmax(a)
+    idx = np.zeros(a.shape, np.int64) if not hi > lo else np.clip(np.floor((a - lo) / (hi - lo) * 255.0 + 0.5), 0, 255).astype(np.int64)
+    k = max(1, min(4, -(-400 // max(1, min(a.shape)))))
+    px = np.repeat(np.repeat(_viridis()[idx], k, axis=0), k, axis=1)
+    path = os.path.join(dir, "alignment_{}.png".format(gs))
+    with open(path, "wb") as f:
+        f.write(png(px))
+    return path
 
 
 def learning_rate_decay(init_lr, global_step, warmup_steps=4000.):

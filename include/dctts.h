@@ -219,6 +219,20 @@ int dctts_train_step(dctts_handle h, const int32_t* L, const float* mels, int32_
 int dctts_train_step_shaped(dctts_handle h, const int32_t* L, int32_t N, const float* mels, int32_t T, int32_t B, int64_t global_step,
                             uint32_t seed, float lr, int32_t apply, float* losses_host, void* stream);
 int dctts_train_apply(dctts_handle h, int64_t global_step, float lr, void* stream);
+/* A forward-only evaluation of the Text2Mel training graph on one batch: what the reference computes for
+ * sess.run(g.alignments) or sess.run(g.merged) (train.py:100-104,156) -- the step's forward at (N, T) with its dropout mask at
+ * `seed`, on the kernel set "train_tc" selects, and the step's losses at that shape into losses_host = {total, mels L1,
+ * binary divergence, guided attention} (optional; reading them synchronises).  Y_out (B, T, n_mels) = sigmoid(logits) and
+ * align_out (B, N, T), DEVICE pointers, are written when non-NULL.  It accepts exactly the shapes dctts_train_step_shaped
+ * accepts and fails, before launching anything, with its message outside them.  It writes neither the variables, the
+ * gradient arena (dctts_train_grads: an eval between a step with apply = 0 and dctts_train_apply leaves it as it was) nor
+ * the Adam moments, so a step after an eval is the step without it. */
+int dctts_train_eval(dctts_handle h, const int32_t* L, int32_t N, const float* mels, int32_t T, int32_t B, uint32_t seed,
+                     float* Y_out, float* align_out, float* losses_host, void* stream);
+/* The SSRN counterpart (train.py:115-118): Z_out (B, 4T, F) = sigmoid(logits), DEVICE, optional; losses_host = {total,
+ * mags L1, binary divergence}; the shapes of dctts_train_step_ssrn_shaped; the same state contract. */
+int dctts_train_eval_ssrn(dctts_handle h, const float* mels, const float* mags, int32_t B, int32_t T, uint32_t seed, float* Z_out,
+                          float* losses_host, void* stream);
 /* The SSRN trainer (train.py num = 2: SSRN on the GROUND-TRUTH mels :69-72, losses :100-108, same optimiser): mels
  * (B, T, n_mels), mags (B, 4T, 1 + n_fft/2) DEVICE pointers; losses_host = {total, mags L1, binary divergence, 0}.
  * A handle trains one of the two networks at a time (the init call selects which).  The T given to dctts_train_init_ssrn

@@ -2,8 +2,9 @@
 data-parallel over the launched ranks (gradient all-reduce of the flat arena over NCCL).  Prints one JSON line.
 `--shape N,T` steps at a length bucket's own shape instead (the workspace keeps its (max_N, max_T) capacity); with
 `--reserve N,T` the workspace is first grown to that capacity (Engine.train_reserve, timed once: "reserve_ms"), so `--shape`
-can go past (max_N, max_T).  The card's name and power limit are part of the JSON line.
-    python tools/bench_train.py [--steps 10 --warmup 3 --batch 32 --net 1 --shape 180,210 --reserve 256,256]
+can go past (max_N, max_T).  `--eval` also times the forward-only evaluation of the training graph on the same batch
+(what summaries and alignment plots cost: "eval_ms").  The card's name and power limit are part of the JSON line.
+    python tools/bench_train.py [--steps 10 --warmup 3 --batch 32 --net 1 --shape 180,210 --reserve 256,256 --eval]
     python -m torch.distributed.run --nproc-per-node N --master-addr 127.0.0.1 tools/bench_train.py"""
 import argparse
 import json
@@ -29,6 +30,7 @@ ap.add_argument("--probe", type=int, default=0, help="measurement only: 1 = the 
 ap.add_argument("--net", type=int, default=1, choices=[1, 2], help="1 = Text2Mel trainer (BASELINE config 5), 2 = SSRN trainer (train.py num=2) at T = 210")
 ap.add_argument("--shape", default="%d,%d" % (hp.max_N, hp.max_T), help="N,T of every step's batch (text positions, mel frames); SSRN uses T")
 ap.add_argument("--reserve", default=None, help="N,T: grow the training workspace to this capacity after init (SSRN uses T)")
+ap.add_argument("--eval", action="store_true", help="also time Engine.train_eval / train_eval_ssrn (forward only, no update) on the same batch: eval_ms")
 ap.add_argument("--train-tc", type=int, default=7, help="bit mask: 1 forward conv, 2 data gradient, 4 weight gradient on wgmma (default 7 = all), 0 = fp32 CUDA-core kernels")
 a = ap.parse_args()
 N, T = (int(x) for x in a.shape.split(","))
@@ -95,6 +97,19 @@ torch.cuda.synchronize()
 ms = torch.tensor([t0.elapsed_time(t1) / a.steps], device="cuda")
 if world > 1:
     dist.all_reduce(ms, op=dist.ReduceOp.MAX)
+eval_ms = None
+if a.eval:                                          # the forward-only evaluation of the same batch (summaries, alignment plots)
+    def evaluate():
+        return eng.train_eval_ssrn(mels, mags, seed=0xffffffff) if a.net == 2 else eng.train_eval(L, mels, seed=0xffffffff)
+    for _ in range(a.warmup):
+        evaluate()
+    torch.cuda.synchronize()
+    t0.record()
+    for _ in range(a.steps):
+        evaluate()
+    t1.record()
+    torch.cuda.synchronize()
+    eval_ms = t0.elapsed_time(t1) / a.steps
 if rank == 0:
     ms = float(ms)
     flops = 3 * 2 * B * (N * 17.10e6 + T * (4.08e6 + 2.71e6 + 0.09e6))                    # SURVEY 8(d) config 5: fwd MACs x 2 x 3
@@ -110,6 +125,7 @@ if rank == 0:
                                  "parallelism": "dp%d (all-reduce of %d gradients)" % (world, grads.numel())},
                       "dtype": ("f32 tensors; GEMMs as split-fp16 x3 on wgmma, fp32 accumulate" if a.train_tc else "f32 (CUDA-core kernels)"), "data": "synthetic",
                       "achieved_tflops": world * flops / (ms * 1e-3) / 1e12, "gpu_launches_per_step": (eng.launch_count() - n0) // a.steps,
-                      "loss_first": first["loss"], "loss_last": last["loss"]}))
+                      "loss_first": first["loss"], "loss_last": last["loss"],
+                      "eval_ms": eval_ms, "eval_over_step": None if eval_ms is None else eval_ms / ms}))
 if world > 1:
     dist.destroy_process_group()
