@@ -189,10 +189,13 @@ struct dctts_handle_s {
     struct {
         bool ok = false;          // stream packed, geometry supported, 16-CTA clusters schedulable
         DecParams tab{};          // layer / chunk tables (+ parameter pointers); per-call fields filled by text2mel_generate
-        DevBuf wstream, lnp, scr, stats, pfinal, prof, pl;
+        DevBuf wstream, lnp, scr, stats, pfinal, prof, pl, frames;
         int max_clusters = 0;
         std::string why;          // why not ok
         int last_moved_frames = -1, last_moved_utt = -1, last_clusters = 0;
+        int last_frames = -1;     // frames the last generation executed, summed over clusters (-1: none yet)
+        bool frames_pending = false;   // last_frames is still in `frames` (per cluster) on the device
+
     } dec;
 
     ~dctts_handle_s() {
@@ -201,7 +204,7 @@ struct dctts_handle_s {
         for (DevBuf* b : {&tr.pre, &tr.out, &tr.emb, &tr.R, &tr.align, &tr.dS, &tr.gbuf[0], &tr.gbuf[1], &tr.gbuf[2], &tr.gbuf[3], &tr.dy,
                           &tr.wT, &tr.zeros, &tr.gts, &tr.sums, &tr.ids, &tr.grads, &tr.mom, &tr.vel, &tr.entries, &tr.tc_a_hi, &tr.tc_a_lo, &tr.tc_b_hi,
                           &tr.tc_b_lo, &tr.tc_slots}) b->release();
-        dec.prof.release(); dec.wstream.release(); dec.lnp.release(); dec.scr.release(); dec.stats.release(); dec.pfinal.release(); dec.pl.release();
+        dec.prof.release(); dec.wstream.release(); dec.lnp.release(); dec.scr.release(); dec.stats.release(); dec.pfinal.release(); dec.pl.release(); dec.frames.release();
         tickets.release(); scratch.release(); act0.release(); act1.release(); kv.release(); ybuf.release();
         rbuf.release(); ad_sig.release(); ibuf.release(); lbuf.release(); zbuf.release();
         for (auto& b : plane) b.release();
@@ -612,6 +615,26 @@ size_t decode_plane_halfs(H* h, int B, __half* base = nullptr, DecParams* set = 
     return off;
 }
 
+// The last persistent decode's per-cluster counters (dec.stats, dec.frames) summed on the host.  Called when they are
+// read, and before ensure_ws reallocates their buffers.
+void settle_decode_counts(H* h) {
+    auto& D = h->dec;
+    if (D.last_clusters > 0 && (D.last_moved_frames < 0 || D.frames_pending)) CUDA_CHECK(cudaDeviceSynchronize());
+    if (D.last_clusters > 0 && D.last_moved_frames < 0) {
+        std::vector<int> st(2 * (size_t)D.last_clusters);
+        CUDA_CHECK(cudaMemcpy(st.data(), D.stats.p, st.size() * sizeof(int), cudaMemcpyDeviceToHost));
+        D.last_moved_frames = 0; D.last_moved_utt = 0;
+        for (int c = 0; c < D.last_clusters; ++c) { D.last_moved_frames += st[2 * c]; D.last_moved_utt += st[2 * c + 1]; }
+    }
+    if (D.frames_pending) {
+        std::vector<int> fr((size_t)D.last_clusters);
+        CUDA_CHECK(cudaMemcpy(fr.data(), D.frames.p, fr.size() * sizeof(int), cudaMemcpyDeviceToHost));
+        D.last_frames = 0;
+        for (int f : fr) D.last_frames += f;
+        D.frames_pending = false;
+    }
+}
+
 void ensure_ws(H* h, int B) {
     if (B <= h->ws_B) return;
     const dctts_hparams& hp = h->hp;
@@ -620,6 +643,7 @@ void ensure_ws(H* h, int B) {
     // invalidate anything that baked pointers
     if (h->ar_exec) { CUDA_CHECK(cudaStreamSynchronize(h->stream)); cudaGraphExecDestroy(h->ar_exec); h->ar_exec = nullptr; h->ar_B = 0; }
     CUDA_CHECK(cudaDeviceSynchronize());
+    settle_decode_counts(h);                              // the counter buffers below may move
     const size_t ld_scr = (size_t)roundup(std::max(std::max(4 * hp.c, F), 4 * d), 4);
     h->scratch.ensure(std::max(rows_ssrn * ld_scr * sizeof(float), (size_t)64 << 20));
     const size_t ld_act = (size_t)roundup(std::max(std::max(2 * hp.c, F), 2 * d), 4);
@@ -649,6 +673,7 @@ void ensure_ws(H* h, int B) {
     CUDA_CHECK(cudaMemset(h->dec.pl.p, 0, h->dec.pl.bytes));     // the DEC_PL_PAD rows in front of t = 0 stay zero
     h->dec.stats.ensure((size_t)2 * B * sizeof(int));
     h->dec.pfinal.ensure((size_t)B * sizeof(int));
+    h->dec.frames.ensure((size_t)B * sizeof(int));
     h->ws_B = B;
 }
 
@@ -1057,8 +1082,11 @@ void build_ar_graph(H* h, int B) {
     h->ar_B = B;
 }
 
+// End of utterance for dctts_text2mel_generate_until: device stop positions (B), tail frames, device lengths out (B)
+struct Until { const int* stop_pos; int tail; int* lengths; };
+
 // The whole AR loop as one persistent launch (kernels_decode.cu).  Returns false when this handle / device cannot run it.
-bool decode_cluster(H* h, int B, int steps, cudaStream_t s) {
+bool decode_cluster(H* h, int B, int steps, cudaStream_t s, const Until* u) {
     auto& D = h->dec;
     if (!D.ok || h->opt.decode_mode != 1) return false;
     const dctts_hparams& hp = h->hp;
@@ -1074,7 +1102,12 @@ bool decode_cluster(H* h, int B, int steps, cudaStream_t s) {
     P.p_hist = ib.p_hist; P.p_final = D.pfinal.as<int>(); P.stats = D.stats.as<int>();
     P.prof = nullptr;
     P.force_prepass = h->opt.decode_force_prepass != 0;
-    if (h->opt.decode_prof) { D.prof.ensure(DEC_NPROF * sizeof(long long)); CUDA_CHECK(cudaMemsetAsync(D.prof.p, 0, DEC_NPROF * sizeof(long long), s)); P.prof = D.prof.as<long long>(); }
+    P.stop_pos = nullptr; P.lengths = nullptr; P.frames = nullptr; P.tail = 0;
+    if (u) {
+        // the stream bound is lowered at a frame's attention; the refill cursor must then still be inside that frame
+        REQUIRE(P.nch - P.nch_enc >= DEC_NSLOT, "decode: fewer AudioDec weight chunks per frame than ring slots");
+        P.stop_pos = u->stop_pos; P.lengths = u->lengths; P.frames = D.frames.as<int>(); P.tail = u->tail;
+    } else if (h->opt.decode_prof) { D.prof.ensure(DEC_NPROF * sizeof(long long)); CUDA_CHECK(cudaMemsetAsync(D.prof.p, 0, DEC_NPROF * sizeof(long long), s)); P.prof = D.prof.as<long long>(); }
     P.B = B;
     {   // utterances per cluster: the fewest that let every cluster be co-resident (a second wave doubles the time)
         const int mc = std::max(1, D.max_clusters);
@@ -1095,11 +1128,13 @@ bool decode_cluster(H* h, int B, int steps, cudaStream_t s) {
     }
     h->launches += 1;
     D.last_clusters = n_clusters; D.last_moved_frames = -1;
+    D.frames_pending = u != nullptr;
+    D.last_frames = u ? -1 : n_clusters * steps;
     return true;
 }
 
 void text2mel_generate(H* h, const int* L, int B, int steps, float* Y, int* prev_hist,
-                       long long* maxatt, float* align, cudaStream_t s) {
+                       long long* maxatt, float* align, cudaStream_t s, const Until* u = nullptr) {
     const dctts_hparams& hp = h->hp;
     const int T = hp.max_T, N = hp.max_N, d = hp.d;
     if (steps <= 0 || steps > T) steps = T;
@@ -1111,7 +1146,8 @@ void text2mel_generate(H* h, const int* L, int B, int steps, float* Y, int* prev
     run_textenc(lc, L, B, h->kv.as<float>());
     CUDA_CHECK(cudaMemsetAsync(h->ybuf.p, 0, (size_t)B * T * hp.n_mels * sizeof(float), s));
     CUDA_CHECK(cudaMemsetAsync(h->ibuf.p, 0, (size_t)(4 + 3 * h->ws_B + (size_t)h->ws_B * T) * sizeof(int), s));
-    if (cluster && decode_cluster(h, B, steps, s)) {
+    bool persistent = cluster && decode_cluster(h, B, steps, s, u);
+    if (persistent) {
         // the whole loop ran as one launch
     } else {
         if (cluster) { CUDA_CHECK(cudaStreamSynchronize(s)); build_ar_graph(h, B); }
@@ -1119,12 +1155,19 @@ void text2mel_generate(H* h, const int* L, int B, int steps, float* Y, int* prev
             CUDA_CHECK(cudaGraphLaunch(h->ar_exec, s));
             h->launches += h->ar_nodes;
         }
+        h->dec.frames_pending = false; h->dec.last_frames = steps;
     }
     if (Y) CUDA_CHECK(cudaMemcpyAsync(Y, h->ybuf.p, (size_t)B * T * hp.n_mels * sizeof(float),
                                       cudaMemcpyDeviceToDevice, s));
     if (prev_hist) CUDA_CHECK(cudaMemcpy2DAsync(prev_hist, (size_t)T * sizeof(int), ib.p_hist,
                                                 (size_t)T * sizeof(int), (size_t)T * sizeof(int), B,
                                                 cudaMemcpyDeviceToDevice, s));
+    if (u) {
+        // the persistent kernel wrote the lengths; after the graph-per-frame loop (all frames) they come from the window
+        // history by the same rule.  The loop is causal, so rows below a length are those of the full-length run.
+        launch_until_finish(u->stop_pos, u->tail, steps, T, hp.n_mels, ib.p_hist, !persistent, u->lengths, Y, prev_hist, B, s);
+        lc.count();
+    }
     if (maxatt || align) {
         // what the LAST sess.run (j = steps-1) returns: every row under that step's window.
         // p_hist[:, steps-1] is that window; gather it into p_prev.
@@ -1999,6 +2042,17 @@ int dctts_text2mel_generate(dctts_handle h, const int32_t* L, int32_t B, int32_t
     });
 }
 
+int dctts_text2mel_generate_until(dctts_handle h, const int32_t* L, int32_t B, int32_t steps, const int32_t* stop_pos,
+                                  int32_t tail, float* Y, int32_t* prev_hist, int32_t* lengths, void* stream) {
+    return guarded(h, [&] {
+        REQUIRE(h->committed, "parameters not committed");
+        REQUIRE(B >= 1 && L && stop_pos && Y && lengths, "dctts_text2mel_generate_until: bad arguments");
+        REQUIRE(tail >= 0, "dctts_text2mel_generate_until: tail must be >= 0");
+        const Until u{stop_pos, std::min<int>(tail, h->hp.max_T), lengths};
+        text2mel_generate(h, L, B, steps, Y, prev_hist, nullptr, nullptr, S(h, stream), &u);
+    });
+}
+
 int dctts_synthesize_host(dctts_handle h, const int32_t* L_host, int32_t B, float* Y_host, float* Z_host) {
     return guarded(h, [&] {
         REQUIRE(h->committed, "parameters not committed");
@@ -2562,6 +2616,12 @@ int dctts_get_option(dctts_handle h, const char* name, int32_t* value) {
         if (name && std::string(name) == "pdl") { *value = pdl_enabled() ? 1 : 0; return; }
         if (name && std::string(name) == "decode_available") { *value = h->dec.ok ? 1 : 0; return; }
         if (name && std::string(name) == "decode_max_clusters") { *value = h->dec.max_clusters; return; }   // co-resident 16-CTA clusters
+        if (name && std::string(name) == "decode_last_frames") {     // frames the last generation executed, summed over clusters
+            REQUIRE(h->dec.last_frames >= 0 || h->dec.frames_pending, "dctts_get_option(decode_last_frames): no generation has run");
+            settle_decode_counts(h);
+            *value = h->dec.last_frames;
+            return;
+        }
         if (name && std::string(name) == "ssrn_tc_available") {     // every SSRN block has a wgmma kernel (needs committed parameters)
             REQUIRE(h->committed, "dctts_get_option(ssrn_tc_available): parameters not committed");
             REQUIRE(h->tc16_why.empty(), "dctts_get_option(ssrn_tc_available): " + h->tc16_why);
@@ -2582,13 +2642,7 @@ int dctts_decode_stats(dctts_handle h, int32_t* moved_frames, int32_t* moved_utt
     return guarded(h, [&] {
         auto& D = h->dec;
         REQUIRE(D.last_clusters > 0, "dctts_decode_stats: no persistent decode has run on this handle");
-        if (D.last_moved_frames < 0) {
-            std::vector<int> st(2 * (size_t)D.last_clusters);
-            CUDA_CHECK(cudaDeviceSynchronize());
-            CUDA_CHECK(cudaMemcpy(st.data(), D.stats.p, st.size() * sizeof(int), cudaMemcpyDeviceToHost));
-            D.last_moved_frames = 0; D.last_moved_utt = 0;
-            for (int c = 0; c < D.last_clusters; ++c) { D.last_moved_frames += st[2 * c]; D.last_moved_utt += st[2 * c + 1]; }
-        }
+        settle_decode_counts(h);
         if (moved_frames) *moved_frames = D.last_moved_frames;
         if (moved_utterance_frames) *moved_utterance_frames = D.last_moved_utt;
         if (clusters) *clusters = D.last_clusters;

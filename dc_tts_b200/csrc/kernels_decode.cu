@@ -85,6 +85,7 @@ struct Smem {
     int p_cur[GMAX], p_prev[GMAX], p_next[GMAX], moved[GMAX];
     int fmoved[2];
     long long prof[DEC_NPROF], prof_last;
+    int stop[GMAX], ulen[GMAX], f_end;  // decode_until_kernel: stop positions, lengths (-1 while unknown), frames to execute
 };
 
 static_assert(sizeof(Smem) + 128 <= 232448, "decode kernel: shared memory budget (227 KB per CTA)");
@@ -189,9 +190,12 @@ struct Stream {
     unsigned pos;               // number of chunks consumed so far
     unsigned tcq;               // pre-pass: slabs staged so far (mbarrier phase parities)
 };
-// one lane of warp `warp`: load the warp's rows of chunk `u` into its region of `slot`
+// one lane of warp `warp`: load the warp's rows of chunk `u` into its region of `slot`.  STOP: the cluster executes S.f_end
+// frames; S.f_end is lowered at a frame's attention, before the AudioDec refills that carry the cursor into the next frame,
+// so no copy of a frame that will not run is ever issued and none is in flight when the cluster exits.
+template <bool STOP>
 __device__ __forceinline__ void stream_issue(const DecParams& P, Smem& S, const Stream& st, const Cur& u, int slot, int warp) {
-    if (u.f >= P.steps) return;
+    if (u.f >= (STOP ? S.f_end : P.steps)) return;
     const DecChunk& ch = P.C[u.c];
     const uint32_t bytes = (uint32_t)ch.nfl4 * 2u;                   // nfl * 4 bytes / 8 warps
     mbar_expect_tx(bar64(&S.fullw[slot][warp]), bytes);
@@ -202,9 +206,10 @@ __device__ __forceinline__ void stream_advance(const DecParams& P, const Smem& S
     cur_next(P, S, st.prod); st.pos++;
 }
 // the calling warp has read its region of the current chunk: refill it with its rows of the chunk 3 ahead
+template <bool STOP>
 __device__ __forceinline__ void warp_release(const DecParams& P, Smem& S, Stream& st, int warp, int lane) {
     __syncwarp();                                                     // every lane's loads of the region have returned (their FMAs have issued)
-    if (lane == 0) stream_issue(P, S, st, st.prod, (int)(st.pos % DEC_NSLOT), warp);
+    if (lane == 0) stream_issue<STOP>(P, S, st, st.prod, (int)(st.pos % DEC_NSLOT), warp);
     stream_advance(P, S, st);
 }
 
@@ -312,7 +317,7 @@ __device__ __forceinline__ void gemv_warp32(const float* __restrict__ wreg, cons
 // ---- one block on ONE row per utterance -------------------------------------------------------------------
 // in: S.xin[cb][g] = [taps | current row] of the block's input, S.prm[li&1] = its parameters (both prefetched).
 // out: S.xin[cb^1][g][next_off ..] = the block's output row; this CTA's channel slice appended to the output history.
-template <bool PROF, int GT>
+template <bool PROF, int GT, bool STOP>
 __device__ __forceinline__ int layer_row(const DecParams& P, Smem& S, Stream& st, int li, int j, int b0, int G, int rank, int cb, unsigned& lcount) {
     const DecLayer& l = P.L[li];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -346,7 +351,7 @@ __device__ __forceinline__ int layer_row(const DecParams& P, Smem& S, Stream& st
             const int kr8 = ch.krows >> 3;
             gemv_warp32<GT>(&S.ring[slot][warp][0], &S.xin[cb][0][ch.k0 + warp * kr8], kr8, pe, po);
             LAP(LP_GEMV);
-            warp_release(P, S, st, warp, lane);
+            warp_release<STOP>(P, S, st, warp, lane);
             LAP(LP_RELEASE);
         }
 #pragma unroll
@@ -368,7 +373,7 @@ __device__ __forceinline__ int layer_row(const DecParams& P, Smem& S, Stream& st
             const int kr8 = ch.krows >> 3;
             gemv_warp<GT>(&S.ring[slot][warp][0], &S.xin[cb][0][ch.k0 + warp * kr8], kr8, l.ns, acc);
             LAP(LP_GEMV);
-            warp_release(P, S, st, warp, lane);
+            warp_release<STOP>(P, S, st, warp, lane);
             LAP(LP_RELEASE);
         }
 #pragma unroll
@@ -814,7 +819,7 @@ __device__ __forceinline__ void pyr_ln(const DecParams& P, Smem& S, int li, int 
 
 // ---- the pre-pass.  Inlined: a wgmma pipeline must not cross a call boundary -- with the pre-pass out of line ptxas
 // serialised every MMA in it (C7510).  The stream cursors go in and come back by value; everything else lives in shared memory.
-template <bool PROF>
+template <bool PROF, bool STOP>
 __device__ __forceinline__ Stream prepass(const DecParams& P, Smem& S, Stream st, int j, int b0, int G, int rank, float* scr,
                                           __half* c1s) {
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -873,7 +878,7 @@ __device__ __forceinline__ Stream prepass(const DecParams& P, Smem& S, Stream st
                 __syncthreads();                          // every warp is done with every region of these chunks
                 LAP(LP_PYR_DRAIN);
                 for (int c = 0; c < l.nch; ++c) {
-                    if (lane == 0) { fence_proxy_async_smem(); stream_issue(P, S, st, st.prod, (int)(st.pos % DEC_NSLOT), warp); }
+                    if (lane == 0) { fence_proxy_async_smem(); stream_issue<STOP>(P, S, st, st.prod, (int)(st.pos % DEC_NSLOT), warp); }
                     stream_advance(P, S, st);
                 }
                 for (int i = tid; i < 256; i += NT)       // this block's LayerNorm parameters for pyr_ln
@@ -890,9 +895,11 @@ __device__ __forceinline__ Stream prepass(const DecParams& P, Smem& S, Stream st
             return st;
 }
 
-template <bool PROF, int GT>
-__global__ void __cluster_dims__(DEC_NC, 1, 1) __launch_bounds__(DEC_THREADS, 1)
-decode_cluster_kernel(const __grid_constant__ DecParams Pc) {
+// The kernel body.  STOP (decode_until_kernel): after frame j's attention every CTA applies the end-of-utterance rule to
+// S.p_next -- computed identically in every CTA -- so all 16 CTAs leave the frame loop after the same frame, with no
+// extra communication, and go through the ordinary epilogue.
+template <bool PROF, int GT, bool STOP>
+__device__ __forceinline__ void decode_body(const DecParams& Pc) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     Smem& S = *reinterpret_cast<Smem*>(smem_raw);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -923,13 +930,17 @@ decode_cluster_kernel(const __grid_constant__ DecParams Pc) {
     if (tid < 2) S.fmoved[tid] = 0;
     if (tid < DEC_NPROF) S.prof[tid] = 0;
     if (tid == 0) { S.n_moved_frames = 0; S.n_moved_utt = 0; }
+    if constexpr (STOP) {                                 // slots past the cluster's utterances count as ended at frame 0
+        if (tid < GMAX) { S.stop[tid] = tid < G ? P.stop_pos[b0 + tid] : -1; S.ulen[tid] = tid < G ? -1 : 0; }
+        if (tid == 0) S.f_end = P.steps;
+    }
     __syncthreads();
 
     Stream st;
     st.base = P.wstream + (size_t)rank * P.stream_len;
     st.prod = Cur{0, 0, 0}; st.pos = 0; st.tcq = 0;
     for (int s = 0; s < DEC_NSLOT; ++s) {                // the first chunks are AudioEnc chunks of frame 0 (nch_enc > DEC_NSLOT)
-        if (lane == 0) stream_issue(P, S, st, st.prod, s, warp);
+        if (lane == 0) stream_issue<STOP>(P, S, st, st.prod, s, warp);
         cur_next(P, S, st.prod);
     }
     prefetch_params(P, S, 0, rank);
@@ -940,6 +951,7 @@ decode_cluster_kernel(const __grid_constant__ DecParams Pc) {
     unsigned lcount = 0;
     __syncthreads();
     if (tid == 0) S.prof_last = clock64();
+    int frames = P.steps;
     for (int j = 0; j < P.steps; ++j) {
         if (tid < GMAX) S.moved[tid] = (tid < G && j > 0 && (P.force_prepass || S.p_cur[tid] != S.p_prev[tid])) ? 1 : 0;
         if (tid == 0) {
@@ -969,10 +981,26 @@ decode_cluster_kernel(const __grid_constant__ DecParams Pc) {
         }
         cb ^= 1;
         LAP(LP_ATT);
+        if constexpr (STOP) {
+            // argmax of row j = S.p_next.  Utterance g ends at min(steps, j + 1 + tail) once it reaches its stop position;
+            // when every utterance has a length the cluster executes the longest.  S.f_end >= j + 1 here, and the refill
+            // cursor is still inside frame j (the AudioDec chunks of a frame outnumber the ring slots: checked by the host),
+            // so lowering the bound now keeps every chunk of frame f_end unissued.  The next block barrier (layer_row's
+            // first, or the pre-pass's cluster barrier) publishes it before any refill.
+            __syncthreads();
+            if (tid == 0) {
+                int fe = 0;
+                for (int g = 0; g < GMAX; ++g) {
+                    if (S.ulen[g] < 0 && S.stop[g] >= 0 && S.p_next[g] >= S.stop[g]) S.ulen[g] = min(P.steps, j + 1 + P.tail);
+                    fe = (fe < 0 || S.ulen[g] < 0) ? -1 : max(fe, S.ulen[g]);
+                }
+                if (fe >= 0) S.f_end = fe;
+            }
+        }
 
-        if (any_moved) st = prepass<PROF>(P, S, st, j, b0, G, rank, scr, c1s);
+        if (any_moved) st = prepass<PROF, STOP>(P, S, st, j, b0, G, rank, scr, c1s);
         }   // li == n_enc
-        cb = layer_row<PROF, GT>(P, S, st, li, j, b0, G, rank, cb, lcount);
+        cb = layer_row<PROF, GT, STOP>(P, S, st, li, j, b0, G, rank, cb, lcount);
         }   // blocks
 
         __syncthreads();
@@ -980,6 +1008,13 @@ decode_cluster_kernel(const __grid_constant__ DecParams Pc) {
         fence_proxy_async_global();                       // this frame's plane rows: read by bulk copies in later frames
         cluster_sync_all();                               // this frame's history rows are visible to the whole cluster
         LAP(LP_FRAME);
+        if constexpr (STOP) {                             // S.f_end is the same in every CTA: the whole cluster leaves here
+            if (j + 1 >= S.f_end) { frames = j + 1; break; }
+        }
+    }
+    if constexpr (STOP) {
+        if (rank == 0 && tid < G) P.lengths[b0 + tid] = S.ulen[tid] < 0 ? P.steps : S.ulen[tid];
+        if (rank == 0 && tid == 0) P.frames[cluster] = frames;
     }
     if (rank == 0 && tid < G) P.p_final[b0 + tid] = S.p_cur[tid];
     if (rank == 0 && tid == 0 && P.stats) { P.stats[2 * cluster] = S.n_moved_frames; P.stats[2 * cluster + 1] = S.n_moved_utt; }
@@ -988,11 +1023,28 @@ decode_cluster_kernel(const __grid_constant__ DecParams Pc) {
     cluster_sync_all();                                   // no CTA exits while a peer may still write into its shared memory
 }
 
+template <bool PROF, int GT>
+__global__ void __cluster_dims__(DEC_NC, 1, 1) __launch_bounds__(DEC_THREADS, 1)
+decode_cluster_kernel(const __grid_constant__ DecParams Pc) { decode_body<PROF, GT, false>(Pc); }
+
+// the same loop ending each utterance at its text (DecParams::stop_pos); a separate kernel, so that the frame loop of
+// decode_cluster_kernel is the one it always was
+template <int GT>
+__global__ void __cluster_dims__(DEC_NC, 1, 1) __launch_bounds__(DEC_THREADS, 1)
+decode_until_kernel(const __grid_constant__ DecParams Pc) { decode_body<false, GT, true>(Pc); }
+
 size_t decode_smem_bytes() { return sizeof(Smem) + 128; }
 
 using DecKernel = void (*)(DecParams);
-// one instantiation per (lap timers, utterances per cluster); exactly one of them runs in a launch
-static DecKernel decode_kernel_of(bool prof, int G) {
+// one instantiation per (lap timers, utterances per cluster) and per utterance count with a stop; exactly one runs in a launch
+static DecKernel decode_kernel_of(bool prof, int G, bool stop = false) {
+    if (stop) switch (G) {
+        case 1: return decode_until_kernel<1>;
+        case 2: return decode_until_kernel<2>;
+        case 3: return decode_until_kernel<3>;
+        case 4: return decode_until_kernel<4>;
+        default: return decode_until_kernel<5>;
+    }
     switch (G) {
         case 1: return prof ? decode_cluster_kernel<true, 1> : decode_cluster_kernel<false, 1>;
         case 2: return prof ? decode_cluster_kernel<true, 2> : decode_cluster_kernel<false, 2>;
@@ -1010,8 +1062,8 @@ static cudaError_t decode_prepare() {
     if (e != cudaSuccess) return e;
     if (dev >= 0 && dev < 64 && done[dev].load(std::memory_order_acquire)) return cudaSuccess;
     for (int G = 1; G <= DEC_GMAX; ++G)
-        for (int prof = 0; prof < 2; ++prof) {
-            DecKernel k = decode_kernel_of(prof != 0, G);
+        for (int v = 0; v < 3; ++v) {                     // decode_cluster_kernel without / with lap timers, decode_until_kernel
+            DecKernel k = decode_kernel_of(v == 1, G, v == 2);
             e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)decode_smem_bytes());
             if (e != cudaSuccess) return e;
             e = cudaFuncSetAttribute(k, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
@@ -1040,7 +1092,36 @@ cudaError_t launch_decode_cluster(const DecParams& p, int n_clusters, cudaStream
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(n_clusters * DEC_NC); cfg.blockDim = dim3(DEC_THREADS); cfg.dynamicSmemBytes = decode_smem_bytes(); cfg.stream = s;
     cfg.attrs = nullptr; cfg.numAttrs = 0;               // cluster dims are compiled in (__cluster_dims__)
-    return cudaLaunchKernelEx(&cfg, decode_kernel_of(p.prof != nullptr, p.G), p);
+    return cudaLaunchKernelEx(&cfg, decode_kernel_of(p.prof != nullptr, p.G, p.stop_pos != nullptr), p);
+}
+
+__global__ void until_finish_kernel(const int* __restrict__ stop_pos, int tail, int steps, int T, int n_mels,
+                                    const int* __restrict__ p_hist, int derive, int* lengths, float* Y, int* prev_hist) {
+    const int b = blockIdx.x;
+    __shared__ int len;
+    if (threadIdx.x == 0) {
+        if (derive) {
+            // argmax of row j = the window of frame j + 1.  The last row is not needed: reaching the stop there gives
+            // min(steps, steps + tail) = steps, the length of never reaching it.
+            int n = steps;
+            const int sp = stop_pos[b];
+            for (int j = 0; sp >= 0 && j + 1 < steps; ++j) {
+                if (p_hist[(size_t)b * T + j + 1] >= sp) { n = min(steps, j + 1 + tail); break; }
+            }
+            lengths[b] = n;
+        }
+        len = lengths[b];
+    }
+    __syncthreads();
+    if (Y)
+        for (int i = len * n_mels + (int)threadIdx.x; i < T * n_mels; i += blockDim.x) Y[(size_t)b * T * n_mels + i] = 0.f;
+    if (prev_hist)
+        for (int t = len + (int)threadIdx.x; t < T; t += blockDim.x) prev_hist[(size_t)b * T + t] = -1;
+}
+
+void launch_until_finish(const int* stop_pos, int tail, int steps, int T, int n_mels, const int* p_hist, bool derive,
+                         int* lengths, float* Y, int* prev_hist, int B, cudaStream_t s) {
+    until_finish_kernel<<<B, 256, 0, s>>>(stop_pos, tail, steps, T, n_mels, p_hist, derive ? 1 : 0, lengths, Y, prev_hist);
 }
 
 }  // namespace dctts

@@ -63,12 +63,25 @@ struct DecParams {
     int nl, n_enc, nch, nch_enc, pyr_ch0, pyr_ch1, stream_len;   // pyr_ch0..pyr_ch1: chunks of the AudioDec blocks with prow > 1
     int B, G, T, N, d, n_mels, win_size, steps;
     int force_prepass;                 // option decode_force_prepass: every utterance recomputes at every frame j >= 1
+    // End of utterance (decode_until_kernel only; nullptr / unused in decode_cluster_kernel): utterance b ends `tail` frames
+    // after the first frame whose attention argmax reaches stop_pos[b] (< 0: never); a cluster leaves the frame loop once
+    // all its utterances have ended.
+    const int* stop_pos;               // (B)
+    int* lengths;                      // (B) out: frames of each utterance
+    int* frames;                       // [clusters] out: frames the cluster executed
+    int tail;
 };
 static_assert(sizeof(DecParams) <= 4000, "DecParams must fit the kernel parameter space");
 
 size_t decode_smem_bytes();
-// returns cudaSuccess or the launch / attribute error (the caller decides whether to fall back)
+// returns cudaSuccess or the launch / attribute error (the caller decides whether to fall back).
+// p.stop_pos != nullptr runs decode_until_kernel (end of utterance, no lap timers).
 cudaError_t launch_decode_cluster(const DecParams& p, int n_clusters, cudaStream_t s);
+// Rows past each utterance's length: Y (B, T, n_mels) rows 0, prev_hist (B, T) rows -1 (either may be nullptr).  With
+// `derive`, lengths[b] is first computed from the window history p_hist (B, T) of a run of `steps` frames by the rule
+// decode_until_kernel applies in its frame loop.
+void launch_until_finish(const int* stop_pos, int tail, int steps, int T, int n_mels, const int* p_hist, bool derive,
+                         int* lengths, float* Y, int* prev_hist, int B, cudaStream_t s);
 // 0 when a 16-CTA cluster with this shared-memory footprint cannot be scheduled on the current device
 int decode_max_active_clusters();
 

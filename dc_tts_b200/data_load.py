@@ -26,6 +26,32 @@ def text_normalize(text):
     return re.sub("[ ]+", " ", text)
 
 
+def eos_positions(texts):
+    """(B, N) ids -> (B,) int32: the index of the first EOS id ("E", which load_data appends to every text), -1 for a row
+    without one.  The default stop position of Engine.text2mel_generate_until."""
+    t = np.asarray(texts)
+    hit = t == hp.vocab.index("E")
+    return np.where(hit.any(axis=1), hit.argmax(axis=1), -1).astype(np.int32)
+
+
+def utterance_lengths(max_attentions, stop_pos, tail=0, steps=None):
+    """The end-of-utterance rule on a window history.  max_attentions (B, >= steps): the attention argmax of every frame
+    (row j is the window of frame j + 1).  Utterance b ends at min(steps, j* + 1 + tail), j* being the first frame
+    j < steps whose argmax is >= stop_pos[b], or at `steps` when there is none or stop_pos[b] < 0."""
+    m = np.asarray(max_attentions)
+    steps = m.shape[1] if steps is None else int(steps)
+    if tail < 0:
+        raise ValueError("tail must be >= 0")
+    out = np.full(m.shape[0], steps, np.int32)
+    for b, sp in enumerate(np.asarray(stop_pos).reshape(-1)):
+        if sp < 0:
+            continue
+        hit = np.nonzero(m[b, :steps] >= sp)[0]
+        if hit.size:
+            out[b] = min(steps, int(hit[0]) + 1 + int(tail))
+    return out
+
+
 def load_data(mode="synthesize", path=None):
     """data_load.py:79-86: sentences file (first line is a header and is dropped, the
     leading "N. " of each line is removed) -> int32 ids (num_sentences, max_N), each

@@ -277,6 +277,38 @@ class Engine:
                                                       _ptr(A), self._stream()), "dctts_text2mel_generate")
         return Y, P, M, A
 
+    def text2mel_generate_until(self, L, stop_pos=None, tail=0, steps=0):
+        """text2mel_generate with an end for each utterance (include/dctts.h: dctts_text2mel_generate_until): utterance b
+        ends `tail` frames after the first frame whose attention argmax reaches stop_pos[b] (< 0: never).  stop_pos=None:
+        the EOS positions of L (data_load.eos_positions).  Returns (Y, P, lengths): Y rows >= lengths[b] are 0, P rows
+        >= lengths[b] are -1, and the rows below are those of text2mel_generate, bit for bit; lengths is an int32 CUDA
+        tensor.  The utterances are decoded in the order of their stop positions, so that the utterances sharing a decode
+        cluster end at similar frames; the outputs are in the caller's order."""
+        from .data_load import eos_positions
+        if tail < 0:
+            raise DcttsError("text2mel_generate_until: tail must be >= 0")
+        L = self._i32(L)
+        B = L.shape[0]
+        sp = eos_positions(L.cpu().numpy()) if stop_pos is None else \
+            np.asarray(stop_pos.cpu() if isinstance(stop_pos, torch.Tensor) else stop_pos, np.int64).reshape(-1)
+        if sp.shape[0] != B:
+            raise DcttsError("text2mel_generate_until: %d stop positions for %d utterances" % (sp.shape[0], B))
+        order = np.argsort(np.where(sp < 0, np.iinfo(np.int32).max, sp), kind="stable")
+        perm = None if np.array_equal(order, np.arange(B)) else torch.as_tensor(order, device=self.device)
+        Ls = L if perm is None else L.index_select(0, perm).contiguous()
+        sps = self._i32(sp[order])
+        Y = self._empty(B, self.hp.max_T, self.hp.n_mels)
+        P = self._empty(B, self.hp.max_T, dtype=torch.int32)
+        n = self._empty(B, dtype=torch.int32)
+        self._check(self._lib.dctts_text2mel_generate_until(self._h, _ptr(Ls), B, int(steps), _ptr(sps), int(tail), _ptr(Y),
+                                                            _ptr(P), _ptr(n), self._stream()),
+                    "dctts_text2mel_generate_until")
+        if perm is None:
+            return Y, P, n
+        Yc, Pc, nc = torch.empty_like(Y), torch.empty_like(P), torch.empty_like(n)
+        Yc[perm], Pc[perm], nc[perm] = Y, P, n
+        return Yc, Pc, nc
+
     def spectrogram2wav(self, mag, n_iter=-1):
         """utils.py:67-94 for a batch: mag (B, T, F) in [0,1] -> (untrimmed wav (B, hop*(T-1)) CUDA tensor,
         trim (B, 2) int32 numpy [start, end) as librosa.effects.trim would keep)."""

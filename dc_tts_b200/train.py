@@ -188,6 +188,11 @@ class Graph:
         Y, P, _, _ = self.engine.text2mel_generate(L, steps)
         return Y, P
 
+    def generate_until_eos(self, L, tail=0):
+        """generate() with each utterance ending `tail` frames after its attention reaches the EOS id of its text:
+        returns (Y, prev_max_attentions history, lengths), rows past an utterance's length 0 / -1 (Engine.text2mel_generate_until)."""
+        return self.engine.text2mel_generate_until(L, tail=tail)
+
 
 class Session:
     """Minimal stand-in for tf.Session used as `with Session() as sess: sess.run(...)`."""

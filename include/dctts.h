@@ -119,6 +119,16 @@ int dctts_text2mel_forward(dctts_handle h, const int32_t* L, const float* mels,
 int dctts_text2mel_generate(dctts_handle h, const int32_t* L, int32_t B, int32_t steps,
                             float* Y, int32_t* prev_hist,
                             int64_t* max_attentions, float* alignments, void* stream);
+/* dctts_text2mel_generate with an end for each utterance.  Utterance b ends at
+ *   len[b] = min(steps, j* + 1 + tail),  j* = the first frame whose attention argmax reaches stop_pos[b],
+ * or at `steps` when no frame does (or stop_pos[b] < 0).  stop_pos and lengths (B) int32 are device pointers; tail >= 0.
+ * Y rows < len[b] and prev_hist rows < len[b] are those of dctts_text2mel_generate on the same batch, bit for bit; Y rows
+ * >= len[b] are 0 and prev_hist rows >= len[b] are -1 (prev_hist may be NULL).  On the persistent decode path a cluster
+ * of utterances stops once all of them have ended (dctts_get_option "decode_last_frames": frames executed, summed over
+ * clusters); the graph-per-frame loop (decode_mode 0) runs every frame and then applies the same rule. */
+int dctts_text2mel_generate_until(dctts_handle h, const int32_t* L, int32_t B, int32_t steps,
+                                  const int32_t* stop_pos, int32_t tail, float* Y, int32_t* prev_hist,
+                                  int32_t* lengths, void* stream);
 /* synthesize.py:45-57 end to end with HOST buffers: copies L_host in, runs
  * dctts_text2mel_generate + dctts_ssrn, copies Y_host (B,max_T,n_mels; may be NULL) and
  * Z_host (B,4*max_T,F) out, and synchronises.  Host buffers should be pinned for speed. */
@@ -285,7 +295,9 @@ int dctts_set_tensor_path(dctts_handle h, int32_t mode);
  * dctts_get_option also answers "decode_available" (1 when this handle / device can run the persistent decode),
  * "decode_max_clusters" (16-CTA clusters of the decode kernel that are co-resident on this device) and, once the
  * parameters are committed, "ssrn_tc_available" (1 when every SSRN block has a wgmma kernel, the F-wide ones included:
- * at F = 2049 they need a 16-CTA cluster; when none can be scheduled on the device the call fails and says so). */
+ * at F = 2049 they need a 16-CTA cluster; when none can be scheduled on the device the call fails and says so), and
+ * "decode_last_frames": frames the last generation executed, summed over the persistent decode's clusters (the
+ * graph-per-frame loop: its step count); synchronises the device. */
 int dctts_set_option(dctts_handle h, const char* name, int32_t value);
 int dctts_get_option(dctts_handle h, const char* name, int32_t* value);
 /* Of the last dctts_text2mel_generate on the persistent decode path: frames in which a cluster had to recompute the
