@@ -4,7 +4,7 @@ Each network in /root/reference/networks.py is a straight-line chain of three bl
 kinds (modules.py): `C` = conv1d (+LN +act), `HC` = highway conv, `D` = stride-2
 transposed conv (+LN).  This module states those chains as data so that the host
 wrappers, the parameter store, the oracle tests and the C library's own table
-(csrc/dctts_nets.cu) can be cross-checked against one another.
+(csrc/api_params.cu `build_tables`) can be cross-checked against one another.
 
 Scope names follow the running counter `i` of the reference (e.g. networks.py:23-68).
 """

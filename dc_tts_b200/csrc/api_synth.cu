@@ -1,0 +1,957 @@
+// api_synth.cu -- synthesis: workspace, block runners, chains, attention, the AR decode and the op-level entry points.
+// Reference mapping:
+//   block semantics ......... modules.py:91-141 (conv1d), :143-197 (hc), :199-247 (conv1d_transpose)
+//   graph wiring / shift .... train.py:48-68, :74-77
+//   autoregressive loop ..... synthesize.py:45-57
+#include "api_internal.cuh"
+
+namespace {
+
+// ---------------------------------------------------------------------------- workspace
+// Persistent decode, split-fp16 planes of the recompute's inputs (kernels_decode.cuh: pl_hist, pl_c1), in halfs:
+// the input history of every receptive-field block after the first ((DEC_PL_PAD + T) rows per utterance), then one
+// DEC_PL_PAD-row stage image per slab of the first block's input for every utterance slot of every cluster.
+// `set` (optional) receives the pointers.
+size_t decode_plane_halfs(H* h, int B, __half* base = nullptr, DecParams* set = nullptr) {
+    const int T = h->hp.max_T;
+    const std::vector<int> rows = audiodec_rows(h->audiodec, T);
+    size_t off = 0;
+    for (size_t i = 1; i < rows.size() && rows[i] > 1; ++i) {
+        if (set) set->pl_hist[set->n_enc + i] = base + off;
+        off += (size_t)B * h->audiodec[i].cin * 2 * (DEC_PL_PAD + T);
+    }
+    if (set) { set->pl_c1 = base + off; set->pl_rows = DEC_PL_PAD + T; }
+    if (!h->audiodec.empty()) off += (size_t)(B + DEC_GMAX) * h->audiodec[0].cin * 2 * DEC_PL_PAD;
+    return off;
+}
+
+}  // namespace
+
+// The last persistent decode's per-cluster counters (dec.stats, dec.frames) summed on the host.  Called when they are
+// read, and before ensure_ws reallocates their buffers.
+void dctts::api::settle_decode_counts(H* h) {
+    auto& D = h->dec;
+    if (D.last_clusters > 0 && (D.last_moved_frames < 0 || D.frames_pending)) CUDA_CHECK(cudaDeviceSynchronize());
+    if (D.last_clusters > 0 && D.last_moved_frames < 0) {
+        std::vector<int> st(2 * (size_t)D.last_clusters);
+        CUDA_CHECK(cudaMemcpy(st.data(), D.stats.p, st.size() * sizeof(int), cudaMemcpyDeviceToHost));
+        D.last_moved_frames = 0; D.last_moved_utt = 0;
+        for (int c = 0; c < D.last_clusters; ++c) { D.last_moved_frames += st[2 * c]; D.last_moved_utt += st[2 * c + 1]; }
+    }
+    if (D.frames_pending) {
+        std::vector<int> fr((size_t)D.last_clusters);
+        CUDA_CHECK(cudaMemcpy(fr.data(), D.frames.p, fr.size() * sizeof(int), cudaMemcpyDeviceToHost));
+        D.last_frames = 0;
+        for (int f : fr) D.last_frames += f;
+        D.frames_pending = false;
+    }
+}
+
+// The one place the captured AR step is destroyed; each caller synchronises first as its own ordering needs.
+void dctts::api::drop_ar_graph(H* h) {
+    if (h->ar_exec) { cudaGraphExecDestroy(h->ar_exec); h->ar_exec = nullptr; h->ar_B = 0; }
+}
+
+namespace {
+
+void ensure_ws(H* h, int B) {
+    if (B <= h->ws_B) return;
+    const dctts_hparams& hp = h->hp;
+    const int T = hp.max_T, N = hp.max_N, d = hp.d, F = h->F;
+    const size_t rows_ssrn = (size_t)B * T * hp.r;
+    // invalidate anything that baked pointers
+    if (h->ar_exec) CUDA_CHECK(cudaStreamSynchronize(h->stream));
+    drop_ar_graph(h);
+    CUDA_CHECK(cudaDeviceSynchronize());
+    settle_decode_counts(h);                              // the counter buffers below may move
+    const size_t ld_scr = (size_t)roundup(std::max(std::max(4 * hp.c, F), 4 * d), 4);
+    h->scratch.ensure(std::max(rows_ssrn * ld_scr * sizeof(float), (size_t)64 << 20));
+    const size_t ld_act = (size_t)roundup(std::max(std::max(2 * hp.c, F), 2 * d), 4);
+    h->act0.ensure(rows_ssrn * ld_act * sizeof(float));
+    h->act1.ensure(rows_ssrn * ld_act * sizeof(float));
+    h->kv.ensure((size_t)B * N * 2 * d * sizeof(float));
+    h->ybuf.ensure((size_t)B * T * hp.n_mels * sizeof(float));
+    h->rbuf.ensure((size_t)B * T * 2 * d * sizeof(float));
+    h->ad_sig.ensure((size_t)B * T * hp.n_mels * sizeof(float));
+    h->ae_out.resize(h->audioenc.size());
+    for (size_t i = 0; i < h->audioenc.size(); ++i)
+        h->ae_out[i].ensure((size_t)B * T * h->audioenc[i].cout * sizeof(float));
+    h->ad_out.resize(h->audiodec.size());
+    for (size_t i = 0; i < h->audiodec.size(); ++i)
+        h->ad_out[i].ensure((size_t)B * T * h->audiodec[i].cout * sizeof(float));
+    h->ibuf.ensure((size_t)(4 + 3 * B + (size_t)B * T) * sizeof(int));
+    h->lbuf.ensure((size_t)B * N * sizeof(int));
+    for (auto& pb : h->plane) pb.ensure(rows_ssrn * (size_t)roundup(std::max(std::max(2 * hp.c, F), 2 * d), 8) * sizeof(__half));
+    h->in_inv.ensure((size_t)B * sizeof(float));
+    for (int i = 0; i < 10; ++i) {
+        const size_t bytes = (size_t)B * T * (i < 2 ? 2 * d : d) * sizeof(__half);
+        h->arpl[i].ensure(bytes);
+        CUDA_CHECK(cudaMemset(h->arpl[i].p, 0, h->arpl[i].bytes));
+    }
+    h->dec.scr.ensure((size_t)(B + DEC_GMAX) * 85 * 512 * sizeof(float));
+    h->dec.pl.ensure(decode_plane_halfs(h, B) * sizeof(__half));
+    CUDA_CHECK(cudaMemset(h->dec.pl.p, 0, h->dec.pl.bytes));     // the DEC_PL_PAD rows in front of t = 0 stay zero
+    h->dec.stats.ensure((size_t)2 * B * sizeof(int));
+    h->dec.pfinal.ensure((size_t)B * sizeof(int));
+    h->dec.frames.ensure((size_t)B * sizeof(int));
+    h->ws_B = B;
+}
+
+void ensure_scratch(H* h, size_t bytes);
+struct IntBufs { int *j, *p_cur, *p_next, *p_prev, *p_hist; };
+IntBufs ints(H* h) {
+    int* base = h->ibuf.as<int>();
+    IntBufs r;
+    r.j = base; r.p_cur = base + 4; r.p_next = r.p_cur + h->ws_B; r.p_prev = r.p_next + h->ws_B;
+    r.p_hist = r.p_prev + h->ws_B;
+    return r;
+}
+
+// ---------------------------------------------------------------------------- block runners
+
+// conv (+bias) into scratch, then the LN / highway epilogue.  `extra_shift` moves every tap
+// (AudioEnc's first block reads the mel buffer one frame back: train.py:51).
+void run_block(Launch& lc, const LayerDev& l, int rate, bool causal, int act,
+               const float* X, int ldx, RowWin win, float* out, int ldo, float* out2, int ldo2,
+               int extra_shift = 0) {
+    H* h = lc.h;
+    REQUIRE(l.kind != K_D, "run_block: transposed conv must use run_deconv");
+    ConvArgs c{};
+    c.X = X; c.ldx = ldx; c.Y = h->scratch.as<float>(); c.ldy = l.ldw; c.bias = l.bias;
+    c.K = l.cin; c.N = l.nconv; c.ldw = l.ldw;
+    c.ntaps = l.size;
+    const int tot = (l.size - 1) * rate;
+    const int left = causal ? tot : tot / 2;
+    for (int j = 0; j < l.size; ++j) {
+        c.taps[j].W = l.W + (size_t)j * l.cin * l.ldw;
+        c.taps[j].shift = j * rate - left + extra_shift;
+    }
+    c.win = win; c.Lout = win.L; c.ostride = 1; c.ooff = 0;
+    LnArgs n{};
+    n.Y = c.Y; n.ldy = l.ldw; n.g1 = l.g1; n.b1 = l.b1; n.g2 = l.g2; n.b2 = l.b2;
+    n.X = X; n.ldx = ldx; n.out = out; n.ldo = ldo; n.out2 = out2; n.ldo2 = ldo2;
+    n.C = l.cout; n.mode = (l.kind == K_HC) ? 1 : 0; n.act = act; n.win = win;
+    // option fused_ln (experiment): GEMM and LN epilogue in one launch, the last CTAs of each 16-row block
+    // waiting on an arrival counter.  Parity-green but SLOWER than two graph nodes (B=1: 220 vs 187 us per
+    // decode step, B=32: 339 vs 303): a kernel boundary inside a CUDA graph costs less than the
+    // ticket / spin / L2 round trips that replace it.
+    if (h->opt.fused_ln && h->tickets.p && conv_gemm_ln_fusable(c, n)) {
+        launch_conv_gemm_ln(c, n, h->tickets.as<int>(), lc.s, h->scratch.bytes); lc.count();
+        return;
+    }
+    GemmOut go = launch_conv_gemm(c, lc.s, h->scratch.bytes); lc.count();
+    n.nparts = go.nparts; n.compact = go.compact; n.part_stride = go.part_stride;
+    launch_ln_rows(n, lc.s); lc.count();
+}
+
+// stride-2 transposed conv (modules.py:232-239): out[2t] = W0 x[t] + W2 x[t-1], out[2t+1] = W1 x[t].
+void run_deconv(Launch& lc, const LayerDev& l, const float* X, int ldx, int B, int L, float* out, int ldo) {
+    H* h = lc.h;
+    ConvArgs c{};
+    c.X = X; c.ldx = ldx; c.Y = h->scratch.as<float>(); c.ldy = l.ldw; c.bias = l.bias;
+    c.K = l.cin; c.N = l.nconv; c.ldw = l.ldw;
+    c.win = RowWin{B, L, L, nullptr}; c.Lout = 2 * L; c.ostride = 2;
+    const size_t tapsz = (size_t)l.cin * l.ldw;
+    c.ntaps = 2; c.taps[0] = ConvTap{l.W + 0 * tapsz, 0}; c.taps[1] = ConvTap{l.W + 2 * tapsz, -1}; c.ooff = 0;
+    launch_conv_gemm(c, lc.s, h->scratch.bytes, false); lc.count();
+    c.ntaps = 1; c.taps[0] = ConvTap{l.W + 1 * tapsz, 0}; c.ooff = 1;
+    launch_conv_gemm(c, lc.s, h->scratch.bytes, false); lc.count();
+    LnArgs n{};
+    n.Y = c.Y; n.ldy = l.ldw; n.g1 = l.g1; n.b1 = l.b1; n.out = out; n.ldo = ldo;
+    n.C = l.cout; n.mode = 0; n.act = 0; n.win = RowWin{B, 2 * L, 2 * L, nullptr};
+    launch_ln_rows(n, lc.s); lc.count();
+}
+
+bool chain_tc_ok(H* h, const std::vector<LayerDev>& net);
+void run_chain_tc_planes(Launch& lc, const std::vector<LayerDev>& net, Planes cur, int which, int B, int L,
+                         float* out, float* out_sig, int first_extra_shift, const float* in_inv);
+void run_chain_full_tc(Launch& lc, const std::vector<LayerDev>& net, const float* X, int ldx, int B, int L,
+                       float* out, float* out_sig);
+
+// A whole chain over full sequences, ping-ponging act0/act1; the last block writes
+// `out` (dense, ld = its cout) and optionally sigmoid(out) into out_sig.
+void run_chain_full(Launch& lc, const std::vector<LayerDev>& net, const float* X, int ldx, int B, int L,
+                    float* out, float* out_sig) {
+    H* h = lc.h;
+    if (chain_tc_ok(h, net) && (out || out_sig)) { run_chain_full_tc(lc, net, X, ldx, B, L, out, out_sig); return; }
+    const float* cur = X; int ld = ldx; int len = L;
+    float* bufs[2] = {h->act0.as<float>(), h->act1.as<float>()};
+    int which = 0;
+    for (size_t i = 0; i < net.size(); ++i) {
+        const LayerDev& l = net[i];
+        const bool last = (i + 1 == net.size());
+        float* dst = last ? out : bufs[which];
+        const int ldo = last ? l.cout : roundup(l.cout, 4);
+        if (last && !dst) { dst = bufs[which]; }            // logits not requested: park them
+        if (l.kind == K_D) {
+            run_deconv(lc, l, cur, ld, B, len, dst, ldo);
+            len *= 2;
+        } else {
+            run_block(lc, l, l.rate, l.causal, l.act, cur, ld, RowWin{B, len, len, nullptr}, dst, ldo,
+                      last ? out_sig : nullptr, l.cout);
+        }
+        cur = dst; ld = ldo; which ^= 1;
+    }
+}
+
+Planes ws_planes(H* h, int which, int C) {
+    Planes p; p.hi = h->plane[2 * which].as<__half>(); p.lo = h->plane[2 * which + 1].as<__half>(); p.ld = roundup(C, 8);
+    return p;
+}
+
+// One reference block as ONE wgmma kernel (kernels_tc.cu).  X are the split planes of the
+// (B, L, cin) input; the output goes to planes and/or fp32 tensors.
+void run_block_tc(Launch& lc, const LayerDev& l, int rate, bool causal, int act, Planes X, RowWin win,
+                  int TT, int TB, int tiles_t, Planes out, float* out_f32, int ld_f32, float* sig_f32, int ld_sig,
+                  Planes sig, int extra_shift = 0, const float* in_inv = nullptr) {
+    const LayerDev::TcPack& p = l.tc;
+    REQUIRE(p.ok, "tensor-core path not available for this block");
+    // the highway residual is read from the input planes unscaled; scaled input planes only reach conv1d blocks
+    REQUIRE(!in_inv || p.mode != 1, "hc block with scaled input planes");
+    TcArgs a{};
+    a.bias = l.bias; a.g1 = l.g1; a.b1 = l.b1; a.g2 = (p.mode == 1) ? l.g2 : l.g1; a.b2 = (p.mode == 1) ? l.b2 : l.b1;
+    a.mode = p.mode; a.act = act; a.C = l.cout; a.bn = p.bn; a.half = p.half; a.inv_scale = p.inv_scale; a.in_inv = in_inv;
+    const int tiles = ((win.B + TB - 1) / TB) * tiles_t;
+    // Option tc_occ2 = 0 (default): the ring holds as many stages as shared memory allows (three for a 256-column hc block,
+    // four for a 256-column conv1d, six at 144 columns); 1 gives launches wider than the device a two-stage ring.  The kernel
+    // runs one CTA per SM either way.  With one k-block of MMAs in flight the deeper ring is faster: on an H100 SXM (400 W
+    // limit) SSRN at B = 32, T = 210 took 13.9 ms per pass against 18.9 ms with two stages.
+    H* h = lc.h;
+    const bool occ2 = h->opt.tc_occ2 != 0 && !win.jptr && TT == 128 && TB == 1 && tiles * p.ncta >= h->num_sms;
+    const int bk = tc_bk();
+    a.ntaps = p.ntaps; a.kb_per_tap = p.kb_per_tap * (64 / bk);
+    if (p.mode == 2) { a.shifts[0] = 0; a.shifts[1] = -1; }
+    else {
+        const int tot = (l.size - 1) * rate, left = causal ? tot : tot / 2;
+        for (int j = 0; j < l.size; ++j) a.shifts[j] = j * rate - left + extra_shift;
+    }
+    a.TT = TT; a.TB = TB; a.tiles_t = tiles_t; a.ntiles = tiles; a.win = win;
+    a.X = X; a.out = out; a.out_f32 = out_f32; a.ld_f32 = ld_f32; a.sig_f32 = sig_f32; a.ld_sig = ld_sig; a.sig = sig;
+    // the A tile is identical in all CTAs of the cluster: fetch it once (TMA multicast) when the
+    // tile is 128 consecutive time rows, each CTA contributing 128/ncta of them
+    const bool no_mcast = h->opt.tc_mcast == 0;
+    a.mcast = (!no_mcast && p.ncta > 1 && TT == 128 && TB == 1) ? 1 : 0;
+    const int box_rows = a.mcast ? TT / p.ncta : TT;
+    CUtensorMap mAh, mAl;
+    tc_make_act_map(&mAh, X.hi, l.cin, X.ld, win.L, win.B, box_rows, TB, bk);
+    tc_make_act_map(&mAl, X.lo, l.cin, X.ld, win.L, win.B, box_rows, TB, bk);
+    // option tc_debug: progress markers in host-mapped memory, dumped after a synchronising launch
+    const bool debug = h->opt.tc_debug != 0;
+    static int* dbg_host = nullptr;
+    if (debug) {
+        if (!dbg_host) CUDA_CHECK(cudaHostAlloc(&dbg_host, 16 * 64 * sizeof(int), cudaHostAllocMapped));
+        memset(dbg_host, 0, 16 * 64 * sizeof(int));
+        CUDA_CHECK(cudaHostGetDevicePointer(&a.dbg, dbg_host, 0));
+    }
+    const CUtensorMap mWh = p.mWhi, mWl = p.mWlo;
+    // hc on full sequences: the residual tile comes in by TMA and the output planes leave by TMA (staged in the
+    // same shared-memory tile), instead of row-scattered 32-byte loads / stores from the epilogue threads
+    const bool no_rtma = h->opt.tc_resid_tma == 0;
+    CUtensorMap io[4];
+    a.resid_tma = 0;
+    a.out_tma = 0;
+    if (!no_rtma && p.mode == 1 && TT == 128 && TB == 1 && (a.half % 64) == 0) {
+        a.resid_tma = 1;
+        // TMA stores only on full sequences: in the decode window the tile starts at a negative time coordinate
+        // (measured: the launch traps), and there the few output rows are cheap to store directly
+        a.out_tma = (out.hi && !win.jptr) ? 1 : 0;
+        tc_make_act_map(&io[0], X.hi, l.cin, X.ld, win.L, win.B, 128, 1, 64);
+        tc_make_act_map(&io[1], X.lo, l.cin, X.ld, win.L, win.B, 128, 1, 64);
+        if (a.out_tma) {
+            tc_make_act_map(&io[2], out.hi, l.cout, out.ld, win.L, win.B, 128, 1, 64);
+            tc_make_act_map(&io[3], out.lo, l.cout, out.ld, win.L, win.B, 128, 1, 64);
+        } else { io[2] = io[0]; io[3] = io[1]; }
+    }
+    // decode-window launches and launches that fill the machine: two stages (more CTAs in flight on a wide grid,
+    // fewer idle bytes on a short reduction); otherwise as many as shared memory holds
+    a.stages = std::min((occ2 || win.jptr) ? 2 : tc_stages_for(p.bn, bk, a.resid_tma, a.half), std::max(1, a.ntaps * a.kb_per_tap));
+    if (debug)
+        fprintf(stderr, "[tc] %s mode=%d ncta=%d bn=%d half=%d stages=%d nkb=%d tiles=%d TT=%d TB=%d L=%d B=%d\n", l.scope.c_str(),
+                a.mode, p.ncta, a.bn, a.half, a.stages, a.ntaps * a.kb_per_tap, tiles, TT, TB, win.L, win.B);
+    launch_conv_ln_tc(mAh, mAl, mWh, mWl, a.resid_tma ? io : nullptr, a, p.ncta, tiles, bk, lc.s); lc.count();
+    if (debug) {
+        cudaError_t e = cudaStreamSynchronize(lc.s);
+        for (int c = 0; c < std::min(16, p.ncta * tiles); ++c)
+            fprintf(stderr, "[tc]  cta %2d: start=%d tmem=0x%x nkb=%d tma=%d mma=%d acc_ready=%d published=%d combined=%d\n", c,
+                    dbg_host[64 * c], dbg_host[64 * c + 1], dbg_host[64 * c + 2], dbg_host[64 * c + 3], dbg_host[64 * c + 4],
+                    dbg_host[64 * c + 5], dbg_host[64 * c + 6], dbg_host[64 * c + 7]);
+        {
+            const int* d0 = dbg_host;      // SM-clock deltas of CTA 0
+            auto dt = [&](int a_, int b_) { return (d0[b_] - d0[a_]) & 0x7fffffff; };
+            fprintf(stderr, "[tc]  cta 0 cycles: setup %d | main loop %d | sweeps1+2 %d | cluster barrier %d | sweep3+stores %d | teardown %d | total %d\n",
+                    dt(8, 9), dt(9, 10), dt(10, 11), dt(11, 12), dt(12, 13), dt(13, 14), dt(8, 14));
+        }
+        if (e != cudaSuccess) throw std::runtime_error(std::string("conv_ln_tc failed: ") + cudaGetErrorString(e));
+    }
+}
+
+bool chain_tc_ok(H* h, const std::vector<LayerDev>& net) {
+    if (h->tensor_path != 1) return false;
+    for (auto& l : net) if (!l.tc.ok) return false;
+    return true;
+}
+
+// Whole chain on the tensor-core path, starting from split planes `cur` (buffer index `which`
+// of the ping-pong pair, or -1 for an external buffer): ... -> fp32 out (+ sigmoid).
+// in_inv: inverse per-utterance scales of `cur` (launch_f32_to_planes_scaled), or null.
+void run_chain_tc_planes(Launch& lc, const std::vector<LayerDev>& net, Planes cur, int which, int B, int L,
+                         float* out, float* out_sig, int first_extra_shift, const float* in_inv) {
+    H* h = lc.h;
+    int len = L;
+    int nxt = (which == 0) ? 1 : 0;
+    for (size_t i = 0; i < net.size(); ++i) {
+        const LayerDev& l = net[i];
+        const bool last = (i + 1 == net.size());
+        Planes dst = last ? Planes{} : ws_planes(h, nxt, l.cout);
+        run_block_tc(lc, l, l.rate, l.causal, l.act, cur, RowWin{B, len, len, nullptr}, 128, 1, (len + 127) / 128,
+                     dst, last ? out : nullptr, l.cout, last ? out_sig : nullptr, l.cout, Planes{},
+                     i == 0 ? first_extra_shift : 0, i == 0 ? in_inv : nullptr);
+        if (l.kind == K_D) len *= 2;
+        cur = dst; nxt ^= 1;
+    }
+}
+
+// (B) device floats for the inverse input scales; grows (after a device sync) for an op-level call beyond the workspace
+float* input_inv_scales(H* h, int B) {
+    if (h->in_inv.bytes < (size_t)B * sizeof(float)) {
+        CUDA_CHECK(cudaDeviceSynchronize());
+        h->in_inv.ensure((size_t)B * sizeof(float));
+    }
+    return h->in_inv.as<float>();
+}
+
+// The fp32 (B, L, l.cin) input of block l -> its split planes, the way the chains carry that block's input: the first
+// block of AudioEnc, AudioDec and SSRN reads audio-level data (mels, R), which silence puts at 1e-8 and below, so its
+// planes get a power-of-two scale per utterance (the inverses are returned for the block's epilogue).  Every other
+// block reads a LayerNorm output, O(1) per row, or an embedding row, whose magnitude is the committed table's: unscaled
+// planes (null).  The op-level entry points follow the same rule, so a network composed block by block computes
+// exactly what its chain computes.
+const float* block_input_planes(Launch& lc, const LayerDev& l, const float* x, int ldx, Planes p, int B, int L) {
+    H* h = lc.h;
+    const bool net_input = (!h->audioenc.empty() && &l == &h->audioenc[0]) || (!h->audiodec.empty() && &l == &h->audiodec[0]) ||
+                           (!h->ssrn.empty() && &l == &h->ssrn[0]);
+    if (!net_input) {
+        launch_f32_to_planes(x, ldx, p, (long long)B * L, l.cin, lc.s); lc.count();
+        return nullptr;
+    }
+    float* in_inv = input_inv_scales(h, B);
+    launch_f32_to_planes_scaled(x, ldx, p, B, L, l.cin, in_inv, lc.s); lc.count();
+    return in_inv;
+}
+
+// fp32 in -> planes -> chain
+void run_chain_full_tc(Launch& lc, const std::vector<LayerDev>& net, const float* X, int ldx, int B, int L,
+                       float* out, float* out_sig) {
+    H* h = lc.h;
+    Planes cur = ws_planes(h, 0, net[0].cin);
+    const float* in_inv = block_input_planes(lc, net[0], X, ldx, cur, B, L);
+    run_chain_tc_planes(lc, net, cur, 0, B, L, out, out_sig, 0, in_inv);
+}
+
+}  // namespace
+
+void dctts::api::run_attention(Launch& lc, const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
+                               RowWin win, int N, const int* pma, float* R, float* align, long long* maxatt,
+                               int* p_next, int* p_hist, Planes Rpl) {
+    H* h = lc.h;
+    REQUIRE(h->hp.d <= 256, "attention: d exceeds 256");
+    AttnArgs a{};
+    a.Q = Q; a.ldq = ldq; a.K = K; a.ldk = ldk; a.V = V; a.ldv = ldv;
+    a.r_hi = Rpl.hi; a.r_lo = Rpl.lo; a.ldr_h = Rpl.ld;
+    a.Rout = R; a.ldr = 2 * h->hp.d; a.align = align; a.maxatt = maxatt; a.pma = pma;
+    a.p_next = p_next; a.p_hist = p_hist; a.N = N; a.d = h->hp.d; a.win_size = h->hp.attention_win_size;
+    a.win = win;
+    launch_attention(a, lc.s); lc.count();
+}
+
+// Full-sequence attention on the tensor cores (kernels_attn_tc.cu): dense or with the monotonic
+// window.  Q, K, V are fp32 device tensors; their split planes are built here.
+void dctts::api::run_attention_tc(Launch& lc, const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv, int B, int T,
+                                  int N, const int* pma, float* R, float* align, long long* maxatt, Planes Rpl) {
+    H* h = lc.h;
+    const int d = h->hp.d, NP = attn_tc_padded_keys(N);
+    const size_t need[3] = {(size_t)B * T * d * sizeof(__half), (size_t)B * N * d * sizeof(__half), (size_t)B * d * NP * sizeof(__half)};
+    for (int i = 0; i < 6; ++i)
+        if (h->attpl[i].bytes < need[i / 2]) { CUDA_CHECK(cudaDeviceSynchronize()); h->attpl[i].ensure(need[i / 2]); }
+    Planes qp, kp, vp;
+    qp.hi = h->attpl[0].as<__half>(); qp.lo = h->attpl[1].as<__half>(); qp.ld = d;
+    kp.hi = h->attpl[2].as<__half>(); kp.lo = h->attpl[3].as<__half>(); kp.ld = d;
+    vp.hi = h->attpl[4].as<__half>(); vp.lo = h->attpl[5].as<__half>(); vp.ld = NP;
+    // Q is AudioEnc's last highway output, h1 * LN(.) + (1 - h1) * x: O(1) per row whatever the mels' level, so its planes
+    // need no scale (a network input is scaled before AudioEnc's first block instead)
+    launch_f32_to_planes(Q, ldq, qp, (long long)B * T, d, lc.s); lc.count();
+    launch_attn_kv_planes(K, ldk, V, ldv, kp, vp, B, N, d, lc.s); lc.count();
+    AttnTcArgs a{};
+    a.Q = Q; a.ldq = ldq; a.R = R; a.ldr = 2 * d; a.Rpl = Rpl; a.align = align; a.maxatt = maxatt; a.pma = pma;
+    a.T = T; a.N = N; a.d = d; a.win_size = h->hp.attention_win_size; a.scale = 1.0f / std::sqrt((float)d);
+    launch_attention_tc(qp, kp, vp, a, B, lc.s); lc.count();
+}
+
+// Receptive-field pyramid of AudioDec for ONE new frame (SURVEY.md App. A / Q1): number of
+// trailing rows each block must (re)compute at every AR step.
+std::vector<int> dctts::api::audiodec_rows(const std::vector<LayerDev>& net, int T) {
+    std::vector<int> rows(net.size(), 1);
+    int need = 1;   // rows of this layer's OUTPUT needed
+    for (int i = (int)net.size() - 1; i >= 0; --i) {
+        rows[i] = std::min(need, T);
+        need += (net[i].size - 1) * net[i].rate;    // rows of its input needed
+    }
+    return rows;
+}
+
+namespace {
+
+bool attention_tc_ok(H* h) { return h->tensor_path == 1 && h->hp.d == 256; }
+
+void run_textenc(Launch& lc, const int* L, int B, float* kv_out /* (B,N,2d) */) {
+    H* h = lc.h;
+    const int N = h->hp.max_N;
+    float* emb = h->act1.as<float>();
+    // park the embedding at the far end of act1 so the ping-pong (which starts on act0) never
+    // overwrites it before the first block has consumed it
+    launch_embed(L, h->embed_table, emb, B * N, h->hp.e, lc.s); lc.count();
+    // first block reads act1 and writes act0, and so on
+    run_chain_full(lc, h->textenc, emb, h->hp.e, B, N, kv_out, nullptr);
+}
+
+// One AR step (synthesize.py:48-54 restated incrementally, exact w.r.t. the reference's
+// full recompute): AudioEnc row j, attention over the AudioDec receptive field under the
+// CURRENT window, AudioDec pyramid, Y[j] = sigmoid(logits[j]), p <- argmax of row j, j <- j+1.
+void run_ar_step(Launch& lc, int B) {
+    H* h = lc.h;
+    const dctts_hparams& hp = h->hp;
+    const int T = hp.max_T, N = hp.max_N, d = hp.d;
+    IntBufs ib = ints(h);
+    // AudioEnc: one new row per utterance; first block reads Y[j-1] (train.py:51)
+    const float* cur = h->ybuf.as<float>(); int ld = hp.n_mels;
+    for (size_t i = 0; i < h->audioenc.size(); ++i) {
+        const LayerDev& l = h->audioenc[i];
+        float* dst = h->ae_out[i].as<float>();
+        run_block(lc, l, l.rate, l.causal, l.act, cur, ld, RowWin{B, T, 1, ib.j}, dst, l.cout, nullptr, 0,
+                  i == 0 ? -1 : 0);
+        cur = dst; ld = l.cout;
+    }
+    const float* Q = cur;
+    std::vector<int> rows = audiodec_rows(h->audiodec, T);
+    const int att_rows = std::min(T, rows[0] + (h->audiodec[0].size - 1) * h->audiodec[0].rate);
+    const float* K = h->kv.as<float>();
+    // Large batches run the wide part of the AudioDec pyramid (85..59 rows per utterance) on the
+    // tensor cores, one 128-row tile per utterance ending at row j; the narrow tail and the
+    // one-row AudioEnc stay on the latency-oriented fp32 kernels.
+    auto on_tc = [&](size_t i) { return h->tensor_path == 1 && B >= 8 && i < 4 && rows[i] >= 32 && h->audiodec[i].tc.ok; };
+    auto ar_planes = [&](int idx, int C) {
+        Planes p; p.hi = h->arpl[2 * idx].as<__half>(); p.lo = h->arpl[2 * idx + 1].as<__half>(); p.ld = C; return p;
+    };
+    Planes Rpl = on_tc(0) ? ar_planes(0, 2 * d) : Planes{};
+    run_attention(lc, Q, d, K, 2 * d, K + d, 2 * d, RowWin{B, T, att_rows, ib.j}, N, ib.p_cur,
+                  h->rbuf.as<float>(), nullptr, nullptr, ib.p_next, ib.p_hist, Rpl);
+    cur = h->rbuf.as<float>(); ld = 2 * d;
+    Planes cur_pl = Rpl;
+    for (size_t i = 0; i < h->audiodec.size(); ++i) {
+        const LayerDev& l = h->audiodec[i];
+        const bool last = (i + 1 == h->audiodec.size());
+        float* dst = h->ad_out[i].as<float>();
+        if (on_tc(i)) {
+            const bool next_tc = (i + 1 < h->audiodec.size()) && on_tc(i + 1);
+            Planes outp = next_tc ? ar_planes((int)i + 1, l.cout) : Planes{};
+            run_block_tc(lc, l, l.rate, l.causal, l.act, cur_pl, RowWin{B, T, rows[i], ib.j}, 128, 1, 1, outp,
+                         next_tc ? nullptr : dst, l.cout, nullptr, 0, Planes{});
+            cur_pl = outp;
+        } else {
+            run_block(lc, l, l.rate, l.causal, l.act, cur, ld, RowWin{B, T, rows[i], ib.j}, dst, l.cout,
+                      last ? h->ybuf.as<float>() : nullptr, hp.n_mels);
+        }
+        cur = dst; ld = l.cout;
+    }
+    launch_ar_advance(ib.p_cur, ib.p_next, ib.j, B, lc.s); lc.count();
+    // keep the window used by this step for the optional final alignment pass
+}
+
+void build_ar_graph(H* h, int B) {
+    if (h->ar_exec && h->ar_B == B) return;
+    drop_ar_graph(h);
+    CUDA_CHECK(cudaStreamSynchronize(h->stream));
+    cudaGraph_t graph = nullptr;
+    int64_t before = h->launches;
+    CUDA_CHECK(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
+    try {
+        Launch lc{h, h->stream};
+        run_ar_step(lc, B);
+    } catch (...) {
+        cudaStreamEndCapture(h->stream, &graph);
+        if (graph) cudaGraphDestroy(graph);
+        h->launches = before;
+        throw;
+    }
+    CUDA_CHECK(cudaStreamEndCapture(h->stream, &graph));
+    h->ar_nodes = h->launches - before;
+    h->launches = before;
+    cudaError_t e = cudaGraphInstantiate(&h->ar_exec, graph, 0);
+    cudaGraphDestroy(graph);
+    CUDA_CHECK(e);
+    CUDA_CHECK(cudaGetLastError());
+    h->ar_B = B;
+}
+
+// End of utterance for dctts_text2mel_generate_until: device stop positions (B), tail frames, device lengths out (B)
+struct Until { const int* stop_pos; int tail; int* lengths; };
+
+// The whole AR loop as one persistent launch (kernels_decode.cu).  Returns false when this handle / device cannot run it.
+bool decode_cluster(H* h, int B, int steps, cudaStream_t s, const Until* u) {
+    auto& D = h->dec;
+    if (!D.ok || h->opt.decode_mode != 1) return false;
+    const dctts_hparams& hp = h->hp;
+    IntBufs ib = ints(h);
+    DecParams P = D.tab;
+    for (int li = 0; li < P.nl; ++li) {
+        const bool enc = li < P.n_enc;
+        P.out_hist[li] = enc ? h->ae_out[li].as<float>() : h->ad_out[li - P.n_enc].as<float>();
+        P.in_hist[li] = li == 0 ? nullptr : (li == P.n_enc ? h->rbuf.as<float>() : P.out_hist[li - 1]);
+    }
+    P.kv = h->kv.as<float>(); P.ybuf = h->ybuf.as<float>(); P.rbuf = h->rbuf.as<float>(); P.pre_scr = D.scr.as<float>();
+    decode_plane_halfs(h, h->ws_B, D.pl.as<__half>(), &P);
+    P.p_hist = ib.p_hist; P.p_final = D.pfinal.as<int>(); P.stats = D.stats.as<int>();
+    P.prof = nullptr;
+    P.force_prepass = h->opt.decode_force_prepass != 0;
+    P.stop_pos = nullptr; P.lengths = nullptr; P.frames = nullptr; P.tail = 0;
+    if (u) {
+        // the stream bound is lowered at a frame's attention; the refill cursor must then still be inside that frame
+        REQUIRE(P.nch - P.nch_enc >= DEC_NSLOT, "decode: fewer AudioDec weight chunks per frame than ring slots");
+        P.stop_pos = u->stop_pos; P.lengths = u->lengths; P.frames = D.frames.as<int>(); P.tail = u->tail;
+    } else if (h->opt.decode_prof) { D.prof.ensure(DEC_NPROF * sizeof(long long)); CUDA_CHECK(cudaMemsetAsync(D.prof.p, 0, DEC_NPROF * sizeof(long long), s)); P.prof = D.prof.as<long long>(); }
+    P.B = B;
+    {   // utterances per cluster: the fewest that let every cluster be co-resident (a second wave doubles the time)
+        const int mc = std::max(1, D.max_clusters);
+        int G = 1;
+        while (G < DEC_GMAX && (B + G - 1) / G > mc) ++G;
+        P.G = G;
+    }
+    P.T = hp.max_T; P.N = hp.max_N; P.d = hp.d; P.n_mels = hp.n_mels;
+    P.win_size = hp.attention_win_size; P.steps = steps;
+    const int n_clusters = (B + P.G - 1) / P.G;
+    cudaError_t e = launch_decode_cluster(P, n_clusters, s);
+    if (e != cudaSuccess) {
+        // a device on which the 16-CTA cluster cannot be placed after all: remember it and let the caller take the
+        // graph-per-frame loop (another GPU path, not a CPU fallback)
+        cudaGetLastError();
+        D.ok = false; D.why = std::string("decode_cluster_kernel launch failed: ") + cudaGetErrorString(e);
+        return false;
+    }
+    h->launches += 1;
+    D.last_clusters = n_clusters; D.last_moved_frames = -1;
+    D.frames_pending = u != nullptr;
+    D.last_frames = u ? -1 : n_clusters * steps;
+    return true;
+}
+
+void text2mel_generate(H* h, const int* L, int B, int steps, float* Y, int* prev_hist,
+                       long long* maxatt, float* align, cudaStream_t s, const Until* u = nullptr) {
+    const dctts_hparams& hp = h->hp;
+    const int T = hp.max_T, N = hp.max_N, d = hp.d;
+    if (steps <= 0 || steps > T) steps = T;
+    ensure_ws(h, B);
+    const bool cluster = h->dec.ok && h->opt.decode_mode == 1;
+    if (!cluster) build_ar_graph(h, B);
+    IntBufs ib = ints(h);
+    Launch lc{h, s};
+    run_textenc(lc, L, B, h->kv.as<float>());
+    CUDA_CHECK(cudaMemsetAsync(h->ybuf.p, 0, (size_t)B * T * hp.n_mels * sizeof(float), s));
+    CUDA_CHECK(cudaMemsetAsync(h->ibuf.p, 0, (size_t)(4 + 3 * h->ws_B + (size_t)h->ws_B * T) * sizeof(int), s));
+    bool persistent = cluster && decode_cluster(h, B, steps, s, u);
+    if (persistent) {
+        // the whole loop ran as one launch
+    } else {
+        if (cluster) { CUDA_CHECK(cudaStreamSynchronize(s)); build_ar_graph(h, B); }
+        for (int j = 0; j < steps; ++j) {
+            CUDA_CHECK(cudaGraphLaunch(h->ar_exec, s));
+            h->launches += h->ar_nodes;
+        }
+        h->dec.frames_pending = false; h->dec.last_frames = steps;
+    }
+    if (Y) CUDA_CHECK(cudaMemcpyAsync(Y, h->ybuf.p, (size_t)B * T * hp.n_mels * sizeof(float),
+                                      cudaMemcpyDeviceToDevice, s));
+    if (prev_hist) CUDA_CHECK(cudaMemcpy2DAsync(prev_hist, (size_t)T * sizeof(int), ib.p_hist,
+                                                (size_t)T * sizeof(int), (size_t)T * sizeof(int), B,
+                                                cudaMemcpyDeviceToDevice, s));
+    if (u) {
+        // the persistent kernel wrote the lengths; after the graph-per-frame loop (all frames) they come from the window
+        // history by the same rule.  The loop is causal, so rows below a length are those of the full-length run.
+        launch_until_finish(u->stop_pos, u->tail, steps, T, hp.n_mels, ib.p_hist, !persistent, u->lengths, Y, prev_hist, B, s);
+        lc.count();
+    }
+    if (maxatt || align) {
+        // what the LAST sess.run (j = steps-1) returns: every row under that step's window.
+        // p_hist[:, steps-1] is that window; gather it into p_prev.
+        CUDA_CHECK(cudaMemcpy2DAsync(ib.p_prev, sizeof(int), ib.p_hist + (steps - 1), (size_t)T * sizeof(int),
+                                     sizeof(int), B, cudaMemcpyDeviceToDevice, s));
+        const float* K = h->kv.as<float>();
+        run_attention(lc, h->ae_out.back().as<float>(), d, K, 2 * d, K + d, 2 * d, RowWin{B, T, T, nullptr}, N,
+                      ib.p_prev, h->rbuf.as<float>(), align, maxatt, nullptr, nullptr);
+    }
+}
+
+void text2mel_forward(H* h, const int* L, const float* mels, const int* pma, int B, float* Y,
+                      long long* maxatt, float* align, cudaStream_t s) {
+    const dctts_hparams& hp = h->hp;
+    const int T = hp.max_T, N = hp.max_N, d = hp.d;
+    ensure_ws(h, B);
+    Launch lc{h, s};
+    run_textenc(lc, L, B, h->kv.as<float>());
+    const float* K = h->kv.as<float>();
+    if (chain_tc_ok(h, h->audioenc) && chain_tc_ok(h, h->audiodec)) {
+        // tensor-core path: every block over all B*T rows as one wgmma kernel
+        Planes mp = ws_planes(h, 0, hp.n_mels);
+        const float* in_inv = block_input_planes(lc, h->audioenc[0], mels, hp.n_mels, mp, B, T);
+        float* Q = h->ae_out.back().as<float>();
+        run_chain_tc_planes(lc, h->audioenc, mp, 0, B, T, Q, nullptr, -1, in_inv);  // shift: train.py:51
+        Planes Rpl; Rpl.hi = h->arpl[0].as<__half>(); Rpl.lo = h->arpl[1].as<__half>(); Rpl.ld = 2 * d;
+        if (attention_tc_ok(h))
+            run_attention_tc(lc, Q, d, K, 2 * d, K + d, 2 * d, B, T, N, pma, h->rbuf.as<float>(), align, maxatt, Rpl);
+        else
+            run_attention(lc, Q, d, K, 2 * d, K + d, 2 * d, RowWin{B, T, T, nullptr}, N, pma, h->rbuf.as<float>(),
+                          align, maxatt, nullptr, nullptr, Rpl);
+        run_chain_tc_planes(lc, h->audiodec, Rpl, -1, B, T, h->ad_out.back().as<float>(), Y, 0, nullptr);
+        return;
+    }
+    // AudioEnc over all rows, reading mels shifted by one frame (train.py:51)
+    const float* cur = mels; int ld = hp.n_mels;
+    for (size_t i = 0; i < h->audioenc.size(); ++i) {
+        const LayerDev& l = h->audioenc[i];
+        float* dst = h->ae_out[i].as<float>();
+        run_block(lc, l, l.rate, l.causal, l.act, cur, ld, RowWin{B, T, T, nullptr}, dst, l.cout, nullptr, 0,
+                  i == 0 ? -1 : 0);
+        cur = dst; ld = l.cout;
+    }
+    run_attention(lc, cur, d, K, 2 * d, K + d, 2 * d, RowWin{B, T, T, nullptr}, N, pma, h->rbuf.as<float>(),
+                  align, maxatt, nullptr, nullptr);
+    cur = h->rbuf.as<float>(); ld = 2 * d;
+    for (size_t i = 0; i < h->audiodec.size(); ++i) {
+        const LayerDev& l = h->audiodec[i];
+        const bool last = (i + 1 == h->audiodec.size());
+        float* dst = h->ad_out[i].as<float>();
+        run_block(lc, l, l.rate, l.causal, l.act, cur, ld, RowWin{B, T, T, nullptr}, dst, l.cout,
+                  last ? Y : nullptr, hp.n_mels);
+        cur = dst; ld = l.cout;
+    }
+}
+
+// Op-level entry (modules.py signatures): fp32 in, fp32 out, on whichever path is selected.
+void run_block_op(Launch& lc, const LayerDev& l, int rate, bool causal, int act, const float* x, int B, int L, float* out) {
+    H* h = lc.h;
+    const int Lout = (l.kind == K_D) ? 2 * L : L;
+    if (h->tensor_path == 1 && l.tc.ok) {
+        const size_t need = (size_t)B * L * roundup(l.cin, 8) * sizeof(__half);
+        if (h->plane[0].bytes < need || h->plane[1].bytes < need) {
+            CUDA_CHECK(cudaDeviceSynchronize());
+            h->plane[0].ensure(need); h->plane[1].ensure(need);
+        }
+        Planes X = ws_planes(h, 0, l.cin);
+        const float* in_inv = block_input_planes(lc, l, x, l.cin, X, B, L);
+        run_block_tc(lc, l, rate, causal, act, X, RowWin{B, L, L, nullptr}, 128, 1, (L + 127) / 128, Planes{}, out, l.cout,
+                     nullptr, 0, Planes{}, 0, in_inv);
+        return;
+    }
+    ensure_scratch(h, (size_t)B * Lout * l.ldw * sizeof(float));
+    if (l.kind == K_D) run_deconv(lc, l, x, l.cin, B, L, out, l.cout);
+    else run_block(lc, l, rate, causal, act, x, l.cin, RowWin{B, L, L, nullptr}, out, l.cout, nullptr, 0);
+}
+
+LayerDev* find_layer(H* h, const char* scope, int kind) {
+    REQUIRE(h->committed, "parameters not committed");
+    auto it = h->by_scope.find(scope ? scope : "");
+    if (it == h->by_scope.end()) throw std::runtime_error(std::string("unknown scope: ") + (scope ? scope : "(null)"));
+    if (it->second->kind != kind) throw std::runtime_error(std::string("scope has a different block kind: ") + scope);
+    return it->second;
+}
+
+// Grow the pre-LN scratch for an op-level call; a reallocation invalidates the AR graph,
+// which has the old pointer baked in.
+void ensure_scratch(H* h, size_t bytes) {
+    bytes = std::max(bytes, (size_t)64 << 20);     // room for the skinny GEMM's split-K partials
+    if (bytes <= h->scratch.bytes) return;
+    CUDA_CHECK(cudaDeviceSynchronize());
+    drop_ar_graph(h);
+    h->scratch.ensure(bytes);
+}
+
+}  // namespace
+
+extern "C" {
+
+int dctts_embed(dctts_handle h, const char* scope, const int32_t* ids, int32_t B, int32_t N, float* out, void* stream) {
+    return guarded(h, [&] {
+        REQUIRE(h->committed, "parameters not committed");
+        auto it = h->dev_vec.find(std::string(scope ? scope : "") + "/lookup_table");
+        REQUIRE(it != h->dev_vec.end(), "dctts_embed: unknown scope");
+        launch_embed(ids, it->second, out, B * N, h->hp.e, S(h, stream)); h->launches++;
+    });
+}
+
+int dctts_normalize(dctts_handle h, const char* scope, const float* x, int64_t rows, int32_t C, float* out, void* stream) {
+    return guarded(h, [&] {
+        REQUIRE(h->committed, "parameters not committed");
+        auto g = h->dev_vec.find(std::string(scope ? scope : "") + "/gamma");
+        auto b = h->dev_vec.find(std::string(scope ? scope : "") + "/beta");
+        REQUIRE(g != h->dev_vec.end() && b != h->dev_vec.end(), "dctts_normalize: unknown scope");
+        REQUIRE(C >= 1 && C <= 1056 && rows < (1ll << 31), "dctts_normalize: unsupported width");
+        LnArgs n{};
+        n.Y = x; n.ldy = C; n.g1 = g->second; n.b1 = b->second; n.out = out; n.ldo = C; n.C = C;
+        n.mode = 0; n.act = 0; n.win = RowWin{1, (int)rows, (int)rows, nullptr};
+        launch_ln_rows(n, S(h, stream)); h->launches++;
+    });
+}
+
+int dctts_conv1d(dctts_handle h, const char* scope, const float* x, int32_t B, int32_t L, int32_t rate,
+                 int32_t causal, int32_t act, float* out, void* stream) {
+    return guarded(h, [&] {
+        LayerDev* l = find_layer(h, scope, K_C);
+        REQUIRE(B >= 1 && L >= 1 && rate >= 1, "dctts_conv1d: bad sizes");
+        Launch lc{h, S(h, stream)};
+        run_block_op(lc, *l, rate, causal != 0, act, x, B, L, out);
+    });
+}
+
+int dctts_hc(dctts_handle h, const char* scope, const float* x, int32_t B, int32_t L, int32_t rate,
+             int32_t causal, float* out, void* stream) {
+    return guarded(h, [&] {
+        LayerDev* l = find_layer(h, scope, K_HC);
+        REQUIRE(B >= 1 && L >= 1 && rate >= 1, "dctts_hc: bad sizes");
+        Launch lc{h, S(h, stream)};
+        run_block_op(lc, *l, rate, causal != 0, 0, x, B, L, out);
+    });
+}
+
+int dctts_conv1d_transpose(dctts_handle h, const char* scope, const float* x, int32_t B, int32_t L, float* out, void* stream) {
+    return guarded(h, [&] {
+        LayerDev* l = find_layer(h, scope, K_D);
+        REQUIRE(B >= 1 && L >= 1, "dctts_conv1d_transpose: bad sizes");
+        Launch lc{h, S(h, stream)};
+        run_block_op(lc, *l, 1, false, 0, x, B, L, out);
+    });
+}
+
+int dctts_textenc(dctts_handle h, const int32_t* L, int32_t B, float* K, float* V, void* stream) {
+    return guarded(h, [&] {
+        REQUIRE(h->committed, "parameters not committed");
+        REQUIRE(B >= 1 && L && K && V, "dctts_textenc: bad arguments");
+        ensure_ws(h, B);
+        cudaStream_t s = S(h, stream);
+        Launch lc{h, s};
+        run_textenc(lc, L, B, h->kv.as<float>());
+        const int N = h->hp.max_N, d = h->hp.d;
+        const size_t w = (size_t)d * sizeof(float);
+        CUDA_CHECK(cudaMemcpy2DAsync(K, w, h->kv.as<float>(), 2 * w, w, (size_t)B * N, cudaMemcpyDeviceToDevice, s));
+        CUDA_CHECK(cudaMemcpy2DAsync(V, w, h->kv.as<float>() + d, 2 * w, w, (size_t)B * N, cudaMemcpyDeviceToDevice, s));
+    });
+}
+
+int dctts_audioenc(dctts_handle h, const float* Sin, int32_t B, int32_t T, float* Q, void* stream) {
+    return guarded(h, [&] {
+        REQUIRE(h->committed, "parameters not committed");
+        REQUIRE(B >= 1 && T >= 1 && T <= h->hp.max_T && Sin && Q, "dctts_audioenc: bad arguments (T must be <= max_T)");
+        ensure_ws(h, B);
+        Launch lc{h, S(h, stream)};
+        run_chain_full(lc, h->audioenc, Sin, h->hp.n_mels, B, T, Q, nullptr);
+    });
+}
+
+int dctts_attention(dctts_handle h, const float* Q, const float* K, const float* V, int32_t B, int32_t T, int32_t N,
+                    int32_t monotonic, const int32_t* pma, float* R, float* alignments, int64_t* max_attentions,
+                    void* stream) {
+    return guarded(h, [&] {
+        REQUIRE(B >= 1 && T >= 1 && N >= 1 && Q && K && V && R, "dctts_attention: bad arguments");
+        REQUIRE(!monotonic || pma, "dctts_attention: monotonic attention needs prev_max_attentions");
+        Launch lc{h, S(h, stream)};
+        const int d = h->hp.d;
+        if (attention_tc_ok(h))
+            run_attention_tc(lc, Q, d, K, d, V, d, B, T, N, monotonic ? pma : nullptr, R, alignments,
+                             reinterpret_cast<long long*>(max_attentions), Planes{});
+        else
+            run_attention(lc, Q, d, K, d, V, d, RowWin{B, T, T, nullptr}, N, monotonic ? pma : nullptr, R, alignments,
+                          reinterpret_cast<long long*>(max_attentions), nullptr, nullptr);
+    });
+}
+
+int dctts_audiodec(dctts_handle h, const float* R, int32_t B, int32_t T, float* Y_logits, float* Y, void* stream) {
+    return guarded(h, [&] {
+        REQUIRE(h->committed, "parameters not committed");
+        REQUIRE(B >= 1 && T >= 1 && T <= h->hp.max_T && R && Y, "dctts_audiodec: bad arguments (T must be <= max_T)");
+        ensure_ws(h, B);
+        Launch lc{h, S(h, stream)};
+        run_chain_full(lc, h->audiodec, R, 2 * h->hp.d, B, T, Y_logits, Y);
+    });
+}
+
+int dctts_ssrn(dctts_handle h, const float* Y, int32_t B, int32_t T, float* Z_logits, float* Z, void* stream) {
+    return guarded(h, [&] {
+        REQUIRE(h->committed, "parameters not committed");
+        REQUIRE(B >= 1 && T >= 1 && T <= h->hp.max_T && Y && Z, "dctts_ssrn: bad arguments (T must be <= max_T)");
+        ensure_ws(h, B);
+        Launch lc{h, S(h, stream)};
+        run_chain_full(lc, h->ssrn, Y, h->hp.n_mels, B, T, Z_logits, Z);
+    });
+}
+
+int dctts_text2mel_forward(dctts_handle h, const int32_t* L, const float* mels, const int32_t* pma, int32_t B,
+                           float* Y, int64_t* max_attentions, float* alignments, void* stream) {
+    return guarded(h, [&] {
+        REQUIRE(h->committed, "parameters not committed");
+        REQUIRE(B >= 1 && L && mels && pma && Y, "dctts_text2mel_forward: bad arguments");
+        text2mel_forward(h, L, mels, pma, B, Y, reinterpret_cast<long long*>(max_attentions), alignments, S(h, stream));
+    });
+}
+
+int dctts_text2mel_generate(dctts_handle h, const int32_t* L, int32_t B, int32_t steps, float* Y, int32_t* prev_hist,
+                            int64_t* max_attentions, float* alignments, void* stream) {
+    return guarded(h, [&] {
+        REQUIRE(h->committed, "parameters not committed");
+        REQUIRE(B >= 1 && L, "dctts_text2mel_generate: bad arguments");
+        text2mel_generate(h, L, B, steps, Y, prev_hist, reinterpret_cast<long long*>(max_attentions), alignments,
+                          S(h, stream));
+    });
+}
+
+int dctts_text2mel_generate_until(dctts_handle h, const int32_t* L, int32_t B, int32_t steps, const int32_t* stop_pos,
+                                  int32_t tail, float* Y, int32_t* prev_hist, int32_t* lengths, void* stream) {
+    return guarded(h, [&] {
+        REQUIRE(h->committed, "parameters not committed");
+        REQUIRE(B >= 1 && L && stop_pos && Y && lengths, "dctts_text2mel_generate_until: bad arguments");
+        REQUIRE(tail >= 0, "dctts_text2mel_generate_until: tail must be >= 0");
+        const Until u{stop_pos, std::min<int>(tail, h->hp.max_T), lengths};
+        text2mel_generate(h, L, B, steps, Y, prev_hist, nullptr, nullptr, S(h, stream), &u);
+    });
+}
+
+int dctts_synthesize_host(dctts_handle h, const int32_t* L_host, int32_t B, float* Y_host, float* Z_host) {
+    return guarded(h, [&] {
+        REQUIRE(h->committed, "parameters not committed");
+        REQUIRE(B >= 1 && L_host && Z_host, "dctts_synthesize_host: bad arguments");
+        const dctts_hparams& hp = h->hp;
+        const int T = hp.max_T, N = hp.max_N;
+        ensure_ws(h, B);
+        const size_t zbytes = (size_t)B * T * hp.r * h->F * sizeof(float);
+        h->zbuf.ensure(zbytes);
+        cudaStream_t s = h->stream;
+        CUDA_CHECK(cudaMemcpyAsync(h->lbuf.p, L_host, (size_t)B * N * sizeof(int), cudaMemcpyHostToDevice, s));
+        text2mel_generate(h, h->lbuf.as<int>(), B, T, nullptr, nullptr, nullptr, nullptr, s);
+        if (Y_host) CUDA_CHECK(cudaMemcpyAsync(Y_host, h->ybuf.p, (size_t)B * T * hp.n_mels * sizeof(float), cudaMemcpyDeviceToHost, s));
+        // SSRN in utterance chunks; the device->host copy of chunk i (copy stream) runs under the SSRN of chunk i+1.
+        // Z is 3.5 MB per utterance: at PCIe rates the copy of a 32-utterance batch is as long as its SSRN.
+        if (!h->copy_stream) {
+            CUDA_CHECK(cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking));
+            for (auto& e : h->chunk_done) CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+        }
+        // chunk ends: quarters of the batch (B >= 16) with the LAST quarter split again -- only the last chunk's copy is exposed,
+        // and a chunk costs the SSRN a partly filled wave (measured ~0.55 ms per extra chunk at B = 32), so more, smaller chunks
+        // at the front would cost more than they hide
+        int ends[8], nchunk = 0;
+        if (B >= 16) { for (int c = 1; c <= 3; ++c) ends[nchunk++] = (int)((long long)B * c / 4); ends[nchunk++] = (int)((long long)B * 7 / 8); ends[nchunk++] = B; }
+        else if (B >= 4) { ends[nchunk++] = B / 2; ends[nchunk++] = B; }
+        else ends[nchunk++] = B;
+        const size_t zrow = (size_t)T * hp.r * h->F;
+        Launch lc{h, s};
+        int b0 = 0;
+        for (int c = 0; c < nchunk; ++c) {
+            const int b1 = ends[c];
+            if (b1 <= b0) continue;
+            float* zc = h->zbuf.as<float>() + (size_t)b0 * zrow;
+            run_chain_full(lc, h->ssrn, h->ybuf.as<float>() + (size_t)b0 * T * hp.n_mels, hp.n_mels, b1 - b0, T, nullptr, zc);
+            CUDA_CHECK(cudaEventRecord(h->chunk_done[c], s));
+            CUDA_CHECK(cudaStreamWaitEvent(h->copy_stream, h->chunk_done[c], 0));
+            CUDA_CHECK(cudaMemcpyAsync(Z_host + (size_t)b0 * zrow, zc, (size_t)(b1 - b0) * zrow * sizeof(float),
+                                       cudaMemcpyDeviceToHost, h->copy_stream));
+            b0 = b1;
+        }
+        CUDA_CHECK(cudaStreamSynchronize(h->copy_stream));
+        CUDA_CHECK(cudaStreamSynchronize(s));
+    });
+}
+
+int dctts_bench_block(dctts_handle h, const char* scope, int32_t B, int32_t L, int32_t iters, int32_t warmup,
+                      float* ms_per_kernel, int32_t* n_kernels, void* stream) {
+    return guarded(h, [&] {
+        REQUIRE(h->committed, "parameters not committed");
+        REQUIRE(scope && B >= 1 && L >= 1 && iters >= 1 && ms_per_kernel && n_kernels, "dctts_bench_block: bad arguments");
+        auto it = h->by_scope.find(scope);
+        REQUIRE(it != h->by_scope.end(), "dctts_bench_block: unknown scope");
+        const LayerDev& l = *it->second;
+        const int Lout = (l.kind == K_D) ? 2 * L : L;
+        DevBuf x, y;
+        x.ensure((size_t)B * L * l.cin * sizeof(float));
+        y.ensure((size_t)B * Lout * l.cout * sizeof(float));
+        cudaStream_t s = S(h, stream);
+        CUDA_CHECK(cudaMemsetAsync(x.p, 0x3c, x.bytes, s));      // 0x3c3c3c3c = 0.0115 as float
+        std::vector<cudaEvent_t> evs;
+        std::vector<double> acc;
+        int nk = 0;
+        for (int i = 0; i < warmup + iters; ++i) {
+            Launch lc{h, s};
+            evs.clear();
+            if (i >= warmup) {
+                lc.evs = &evs;
+                cudaEvent_t e0; CUDA_CHECK(cudaEventCreate(&e0)); CUDA_CHECK(cudaEventRecord(e0, s)); evs.push_back(e0);
+            }
+            run_block_op(lc, l, l.rate, l.causal, l.act, x.as<float>(), B, L, y.as<float>());
+            if (i >= warmup) {
+                CUDA_CHECK(cudaStreamSynchronize(s));
+                nk = (int)evs.size() - 1;
+                if (acc.empty()) acc.assign(nk, 0.0);
+                for (int k = 0; k < nk; ++k) {
+                    float ms = 0.f;
+                    CUDA_CHECK(cudaEventElapsedTime(&ms, evs[k], evs[k + 1]));
+                    acc[k] += ms;
+                }
+                for (auto e : evs) cudaEventDestroy(e);
+            }
+        }
+        REQUIRE(nk <= 8, "dctts_bench_block: too many kernels");
+        for (int k = 0; k < nk; ++k) ms_per_kernel[k] = (float)(acc[k] / iters);
+        *n_kernels = nk;
+        CUDA_CHECK(cudaStreamSynchronize(s));
+    });
+}
+
+int dctts_reserve(dctts_handle h, int32_t max_batch) {
+    return guarded(h, [&] { REQUIRE(max_batch >= 1, "dctts_reserve: bad batch"); ensure_ws(h, max_batch); });
+}
+
+int dctts_set_tensor_path(dctts_handle h, int32_t mode) {
+    return guarded(h, [&] {
+        REQUIRE(mode == 0 || mode == 1, "dctts_set_tensor_path: mode must be 0 or 1");
+        REQUIRE(!(h->tr.ready && mode == 1), "dctts_set_tensor_path: this handle has been trained -- its packed fp16 weight planes "
+                "are stale; load the trained variables (dctts_train_tensor) into a new handle for the wgmma kernel set");
+        if (mode != h->tensor_path && h->ar_exec) {      // the captured AR step depends on the mode
+            CUDA_CHECK(cudaDeviceSynchronize());
+            drop_ar_graph(h);
+        }
+        h->tensor_path = mode;
+    });
+}
+
+// Of the last dctts_text2mel_generate on the persistent decode path: frames in which at least one utterance of a cluster
+// moved its attention window (summed over clusters), utterance-frames whose receptive field was recomputed, clusters used.
+int dctts_decode_stats(dctts_handle h, int32_t* moved_frames, int32_t* moved_utterance_frames, int32_t* clusters) {
+    return guarded(h, [&] {
+        auto& D = h->dec;
+        REQUIRE(D.last_clusters > 0, "dctts_decode_stats: no persistent decode has run on this handle");
+        settle_decode_counts(h);
+        if (moved_frames) *moved_frames = D.last_moved_frames;
+        if (moved_utterance_frames) *moved_utterance_frames = D.last_moved_utt;
+        if (clusters) *clusters = D.last_clusters;
+    });
+}
+
+// SM-clock lap timers of the last persistent decode run with option decode_prof = 1 (cluster 0, CTA rank 0, thread 0):
+// the buckets are listed in include/dctts.h.
+int dctts_decode_profile(dctts_handle h, int64_t* cycles, int32_t n) {
+    return guarded(h, [&] {
+        REQUIRE(cycles && n >= 1 && n <= DEC_NPROF, "dctts_decode_profile: bad arguments");
+        REQUIRE(h->dec.prof.p, "dctts_decode_profile: no profiled decode has run (set option decode_prof)");
+        CUDA_CHECK(cudaDeviceSynchronize());
+        long long v[DEC_NPROF];
+        CUDA_CHECK(cudaMemcpy(v, h->dec.prof.p, sizeof(v), cudaMemcpyDeviceToHost));
+        for (int i = 0; i < n; ++i) cycles[i] = v[i];
+    });
+}
+
+}  // extern "C"

@@ -309,6 +309,14 @@ class Engine:
         Yc[perm], Pc[perm], nc[perm] = Y, P, n
         return Yc, Pc, nc
 
+    def _set_vocoder_params(self, hop=None, win=None, power=None):
+        """The hyperparameters' vocoder constants on the handle, with `hop`, `win` and `power` instead when given."""
+        h = self.hp
+        self._check(self._lib.dctts_set_vocoder_params(self._h, int(hop or h.hop_length), int(win or h.win_length),
+                                                       float(h.power if power is None else power), float(h.max_db),
+                                                       float(h.ref_db), float(h.preemphasis), int(h.n_iter)),
+                    "dctts_set_vocoder_params")
+
     def spectrogram2wav(self, mag, n_iter=-1):
         """utils.py:67-94 for a batch: mag (B, T, F) in [0,1] -> (untrimmed wav (B, hop*(T-1)) CUDA tensor,
         trim (B, 2) int32 numpy [start, end) as librosa.effects.trim would keep)."""
@@ -317,9 +325,7 @@ class Engine:
             mag = mag[None]
         B, T, F = mag.shape
         h = self.hp
-        self._check(self._lib.dctts_set_vocoder_params(self._h, h.hop_length, h.win_length, float(h.power), float(h.max_db),
-                                                       float(h.ref_db), float(h.preemphasis), int(h.n_iter)),
-                    "dctts_set_vocoder_params")
+        self._set_vocoder_params()
         wav = self._empty(B, h.hop_length * (T - 1))
         trim = np.zeros((B, 2), np.int32)
         self._check(self._lib.dctts_spectrogram2wav(self._h, _ptr(mag), B, T, int(n_iter), _ptr(wav),
@@ -336,12 +342,8 @@ class Engine:
           4 energies    x = wav (B, Ly)                          -> out = mse (B, 1 + Ly // 512) float32
         Tensors must be contiguous (they may be views into larger buffers).  Returns the trims (B, 2) int32 numpy for
         stage 4 (as spectrogram2wav reports them), else out."""
-        h = self.hp
-        hop = int(hop or h.hop_length)
-        win = int(win or h.win_length)
-        power = float(h.power if power is None else power)
-        self._check(self._lib.dctts_set_vocoder_params(self._h, hop, win, power, float(h.max_db), float(h.ref_db),
-                                                       float(h.preemphasis), int(h.n_iter)), "dctts_set_vocoder_params")
+        hop = int(hop or self.hp.hop_length)
+        self._set_vocoder_params(hop, win, power)
         f32, c64 = torch.float32, torch.complex64
         B = x.shape[0]
         if stage in (0, 1):
@@ -374,9 +376,7 @@ class Engine:
         h = self.hp
         wav = self._f32(wav).reshape(-1)
         n = wav.numel()
-        self._check(self._lib.dctts_set_vocoder_params(self._h, h.hop_length, h.win_length, float(h.power), float(h.max_db),
-                                                       float(h.ref_db), float(h.preemphasis), int(h.n_iter)),
-                    "dctts_set_vocoder_params")
+        self._set_vocoder_params()
         cap = 1 + n // h.hop_length
         mel = self._empty(cap, h.n_mels)
         mag = self._empty(cap, self.F)
@@ -448,9 +448,7 @@ class Engine:
             wav, dtype = self._rs_out, 0
         if t_capacity is None:
             t_capacity = max(-(-(1 + int(n) // h.hop_length) // h.r) for n in np.diff(offsets))
-        self._check(self._lib.dctts_set_vocoder_params(self._h, h.hop_length, h.win_length, float(h.power), float(h.max_db),
-                                                       float(h.ref_db), float(h.preemphasis), int(h.n_iter)),
-                    "dctts_set_vocoder_params")
+        self._set_vocoder_params()
         mel = self._empty(B * t_capacity * h.n_mels)
         mag = self._empty(B * t_capacity * h.r * self.F)
         t = np.zeros(B, np.int32)
@@ -472,18 +470,33 @@ class Engine:
         rate = self.hp.dropout_rate if dropout_rate is None else dropout_rate
         self._check(self._lib.dctts_train_init(self._h, int(B), float(rate)), "dctts_train_init")
 
+    def _text_mels(self, who, L, mels):
+        L = self._i32(L); mels = self._f32(mels)
+        if L.dim() != 2:
+            raise DcttsError("%s: L must be (B, N), got shape %s" % (who, tuple(L.shape)))
+        B = L.shape[0]
+        if mels.dim() != 3 or mels.shape[0] != B or mels.shape[2] != self.hp.n_mels:
+            raise DcttsError("%s: mels must be (B=%d, T, n_mels=%d), got shape %s" % (who, B, self.hp.n_mels, tuple(mels.shape)))
+        return L, mels
+
+    def _mels_mags(self, who, mels, mags):
+        mels = self._f32(mels); mags = self._f32(mags)
+        if mels.dim() != 3 or mels.shape[2] != self.hp.n_mels:
+            raise DcttsError("%s: mels must be (B, T, n_mels=%d), got shape %s" % (who, self.hp.n_mels, tuple(mels.shape)))
+        B, T = mels.shape[0], mels.shape[1]
+        if tuple(mags.shape) != (B, self.hp.r * T, self.F):
+            raise DcttsError("%s: mags must be (B, %d T, F) = %s for mels %s, got %s"
+                             % (who, self.hp.r, (B, self.hp.r * T, self.F), tuple(mels.shape), tuple(mags.shape)))
+        return mels, mags
+
     def train_step(self, L, mels, global_step=0, seed=0, lr=None, apply=True):
         """One Text2Mel optimiser step on L (B, N) int32 / mels (B, T, n_mels) at the batch's own shape -- a bucket padded
         to its longest member (trainer.bucketed_batches) or the fixed (max_N, max_T) -- up to N = hp.max_N, T = hp.max_T,
         or the capacity given to train_reserve:
         forward with dropout, losses (train.py:83-99), backward, clip, Adam (train.py:122-132).
         Returns {loss, loss_mels, loss_bd1, loss_att}."""
-        L = self._i32(L); mels = self._f32(mels)
-        if L.dim() != 2:
-            raise DcttsError("train_step: L must be (B, N), got shape %s" % (tuple(L.shape),))
+        L, mels = self._text_mels("train_step", L, mels)
         B, N = L.shape
-        if mels.dim() != 3 or mels.shape[0] != B or mels.shape[2] != self.hp.n_mels:
-            raise DcttsError("train_step: mels must be (B=%d, T, n_mels=%d), got shape %s" % (B, self.hp.n_mels, tuple(mels.shape)))
         out = (C.c_float * 4)()
         self._check(self._lib.dctts_train_step_shaped(self._h, _ptr(L), N, _ptr(mels), mels.shape[1], B, int(global_step),
                                                       int(seed) & 0xffffffff, float(self.hp.lr if lr is None else lr),
@@ -501,13 +514,8 @@ class Engine:
     def train_step_ssrn(self, mels, mags, global_step=0, seed=0, lr=None, apply=True):
         """One SSRN optimiser step on ground-truth mels (B, T, n_mels) / mags (B, 4T, F) at the batch's own T, up to the
         capacity of train_init_ssrn (train.py:69-72,100-108,122-132)."""
-        mels = self._f32(mels); mags = self._f32(mags)
-        if mels.dim() != 3 or mels.shape[2] != self.hp.n_mels:
-            raise DcttsError("train_step_ssrn: mels must be (B, T, n_mels=%d), got shape %s" % (self.hp.n_mels, tuple(mels.shape)))
+        mels, mags = self._mels_mags("train_step_ssrn", mels, mags)
         B, T = mels.shape[0], mels.shape[1]
-        if tuple(mags.shape) != (B, self.hp.r * T, self.F):
-            raise DcttsError("train_step_ssrn: mags must be (B, %d T, F) = %s for mels %s, got %s"
-                             % (self.hp.r, (B, self.hp.r * T, self.F), tuple(mels.shape), tuple(mags.shape)))
         out = (C.c_float * 4)()
         self._check(self._lib.dctts_train_step_ssrn_shaped(self._h, _ptr(mels), _ptr(mags), B, T, int(global_step),
                                                            int(seed) & 0xffffffff, float(self.hp.lr if lr is None else lr),
@@ -520,12 +528,8 @@ class Engine:
         the batch's shape.  Same shapes as train_step.  The variables, Adam moments and the gradient arena are untouched.
         Returns ({loss, loss_mels, loss_bd1, loss_att}, {name: CUDA tensor}) for the names in `want`: "Y" (B, T, n_mels)
         and "alignments" (B, N, T)."""
-        L = self._i32(L); mels = self._f32(mels)
-        if L.dim() != 2:
-            raise DcttsError("train_eval: L must be (B, N), got shape %s" % (tuple(L.shape),))
+        L, mels = self._text_mels("train_eval", L, mels)
         B, N = L.shape
-        if mels.dim() != 3 or mels.shape[0] != B or mels.shape[2] != self.hp.n_mels:
-            raise DcttsError("train_eval: mels must be (B=%d, T, n_mels=%d), got shape %s" % (B, self.hp.n_mels, tuple(mels.shape)))
         unknown = set(want) - {"Y", "alignments"}
         if unknown:
             raise DcttsError("train_eval: can return Y and alignments, not %s" % sorted(unknown))
@@ -542,13 +546,8 @@ class Engine:
 
     def train_eval_ssrn(self, mels, mags, seed=0, want=("Z",)):
         """The SSRN counterpart of train_eval (train.py:115-118): returns ({loss, loss_mags, loss_bd2}, {"Z": (B, 4T, F)})."""
-        mels = self._f32(mels); mags = self._f32(mags)
-        if mels.dim() != 3 or mels.shape[2] != self.hp.n_mels:
-            raise DcttsError("train_eval_ssrn: mels must be (B, T, n_mels=%d), got shape %s" % (self.hp.n_mels, tuple(mels.shape)))
+        mels, mags = self._mels_mags("train_eval_ssrn", mels, mags)
         B, T = mels.shape[0], mels.shape[1]
-        if tuple(mags.shape) != (B, self.hp.r * T, self.F):
-            raise DcttsError("train_eval_ssrn: mags must be (B, %d T, F) = %s for mels %s, got %s"
-                             % (self.hp.r, (B, self.hp.r * T, self.F), tuple(mels.shape), tuple(mags.shape)))
         unknown = set(want) - {"Z"}
         if unknown:
             raise DcttsError("train_eval_ssrn: can return Z, not %s" % sorted(unknown))

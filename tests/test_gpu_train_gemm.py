@@ -1,6 +1,6 @@
 """The conv-GEMMs of the training step, one launch at a time (dctts_conv_gemm), against float64, on both kernel sets.
 
-Each block of the two trainers issues a forward conv, a data gradient and a weight gradient (dctts_api.cu train_fwd /
+Each block of the two trainers issues a forward conv, a data gradient and a weight gradient (api_train.cu train_fwd /
 train_bwd); the transposed-conv blocks of SSRN issue three weight-gradient and two data-gradient launches on the
 (B*L, 2*ldw) view of their gradient.  The cases below are generated from `arch`, deduplicated, and every one runs on the
 fp32 CUDA-core kernels (impl 0) and, where the step can use them, the wgmma split-fp16 kernels (impl 1).
@@ -56,7 +56,7 @@ def ref_wgrad(X, dY, shifts):
 
 
 def layer_shifts(l, extra=0):
-    """Source-row offsets of the taps of a conv block (dctts_api.cu layer_shifts)."""
+    """Source-row offsets of the taps of a conv block (api_train.cu layer_shifts)."""
     tot = (l.size - 1) * l.rate
     left = tot if l.pad == "CAUSAL" else tot // 2
     return tuple(j * l.rate - left + extra for j in range(l.size))

@@ -29,7 +29,7 @@ def rup(x, m):
 
 
 def block_table(F):
-    """(scope, kind, cin, cout, taps, L factor over T) of every SSRN block, as build_tables lays them out (dctts_api.cu)."""
+    """(scope, kind, cin, cout, taps, L factor over T) of every SSRN block, as build_tables lays them out (api_params.cu)."""
     c = hp.c
     t = [("SSRN/C_1", "C", hp.n_mels, c, 1, 1), ("SSRN/HC_2", "HC", c, c, 3, 1), ("SSRN/HC_3", "HC", c, c, 3, 1),
          ("SSRN/D_4", "D", c, c, 3, 1), ("SSRN/HC_5", "HC", c, c, 3, 2), ("SSRN/HC_6", "HC", c, c, 3, 2),
@@ -44,7 +44,7 @@ def block_table(F):
 
 
 def tile_cols(kind, cout):
-    """Accumulator columns over the cluster (pack_tc in dctts_api.cu)."""
+    """Accumulator columns over the cluster (pack_tc in api_params.cu)."""
     if kind == "C":
         maxbn = 64 if (cout <= 256 and cout % 64 == 0) else 256
         n = 1
