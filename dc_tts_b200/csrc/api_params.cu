@@ -1,6 +1,7 @@
 // api_params.cu -- layer tables; parameter staging, split-fp16 packing and the persistent decode's weight stream.
 // Reference mapping: layer tables networks.py:23-68 (TextEnc), :81-124 (AudioEnc), :166-209 (AudioDec), :223-290 (SSRN)
 #include "api_internal.cuh"
+#include "numerics.cuh"
 
 namespace {
 
@@ -101,8 +102,7 @@ float* upload_vec(H* h, const std::string& name, int n, int padded) {
 // Split-fp16 packing for the wgmma kernel (kernels_tc.cu).  Rows are accumulator columns in
 // cluster-slice order (CTA i owns rows [i*bn, (i+1)*bn); for hc / transposed conv its first
 // `half` rows are the first LN half, the rest the second), columns are k = tap*cin_pad + ci.
-// Weights are multiplied by a power of two that brings max|W| into [2^10, 2^11) so that the
-// low plane stays in fp16's normal range; the kernel multiplies the accumulator back.
+// Weights are multiplied by weight_scale (numerics.cuh); the kernel multiplies the accumulator back.
 void pack_tc(H* h, LayerDev& l, const std::vector<float>& W /* [size][cin][ldw] */) {
     LayerDev::TcPack& p = l.tc;
     const int cin_pad = roundup(l.cin, 64);
@@ -143,18 +143,14 @@ void pack_tc(H* h, LayerDev& l, const std::vector<float>& W /* [size][cin][ldw] 
     for (int tap = 0; tap < p.ntaps; ++tap)
         for (int ci = 0; ci < l.cin; ++ci)
             for (int row = 0; row < p.nrows; ++row) maxabs = std::max(maxabs, std::fabs(wv(tap, ci, row)));
-    float scale = 1.f;
-    if (maxabs > 0.f) { int e; std::frexp(maxabs, &e); scale = std::ldexp(1.f, 11 - e); }   // maxabs*scale in [2^10, 2^11)
+    const float scale = weight_scale(maxabs);
     p.inv_scale = 1.f / scale;
     std::vector<__half> hi((size_t)p.nrows * p.Ktot, __float2half_rn(0.f)), lo(hi);
     for (int row = 0; row < p.nrows; ++row)
         for (int tap = 0; tap < p.ntaps; ++tap)
             for (int ci = 0; ci < l.cin; ++ci) {
-                const float v = wv(tap, ci, row) * scale;
-                const __half hv = __float2half_rn(v);
                 const size_t idx = (size_t)row * p.Ktot + (size_t)tap * cin_pad + ci;
-                hi[idx] = hv;
-                lo[idx] = __float2half_rn(v - __half2float(hv));
+                split_f16(wv(tap, ci, row) * scale, hi[idx], lo[idx]);
             }
     p.Whi = upload(h, hi);
     p.Wlo = upload(h, lo);
@@ -276,9 +272,7 @@ void pack_decode(H* h) {
         if (L.prow <= 1) continue;
         float maxabs = 0.f;
         for (size_t i = 0; i < l.hostW.size(); ++i) maxabs = std::max(maxabs, std::fabs(l.hostW[i]));
-        float scale = 1.f;
-        if (maxabs > 0.f) { int e; std::frexp(maxabs, &e); scale = std::ldexp(1.f, 11 - e); }
-        P.inv_scale[li] = 1.f / scale;
+        P.inv_scale[li] = 1.f / weight_scale(maxabs);
     }
     for (int r = 0; r < DEC_NC; ++r)
         for (int li = 0; li < P.nl; ++li) {
@@ -319,11 +313,9 @@ void pack_decode(H* h) {
                     for (int n = 0; n < L.ns; ++n) {
                         const int col = column(n);
                         const float v = (col >= 0 && ci < l.cin) ? wrow[col] * scale : 0.f;
-                        const __half hv = __float2half_rn(v);
                         const size_t base = (size_t)slab * 32 * L.ns;                  // halfs per slab = 2 planes * 2 groups * ns * 8
                         const size_t idx = ((size_t)grp * L.ns + n) * 8 + e8;
-                        d16[base + idx] = hv;
-                        d16[base + (size_t)2 * L.ns * 8 + idx] = __float2half_rn(v - __half2float(hv));
+                        split_f16(v, d16[base + idx], d16[base + (size_t)2 * L.ns * 8 + idx]);
                     }
                 }
             }

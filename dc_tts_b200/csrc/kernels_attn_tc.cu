@@ -22,6 +22,7 @@
 // the P block (16 KB), and a 6-stage ring of 16 KB stages carrying K slabs (64 keys x 64
 // channels) and, in pass 3, V^T chunks (64 channels x 64 keys), both as hi | lo.
 #include "kernels_tc.cuh"
+#include "numerics.cuh"
 #include "tc_ptx.cuh"
 
 #include <algorithm>
@@ -230,11 +231,11 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap mapQ_hi, const __grid_co
                     p2[e] = p;
                 }
                 if (live) {
-                    const __half h0 = __float2half_rn(p2[0]), h1 = __float2half_rn(p2[1]);
-                    const __half l0 = __float2half_rn(p2[0] - __half2float(h0)), l1 = __float2half_rn(p2[1] - __half2float(h1));
+                    __half2 h, l;
+                    split_f16x2(make_float2(p2[0], p2[1]), h, l);
                     const int off = r * 128 + ((i ^ (r & 7)) << 4) + 4 * (lane & 3);
-                    *reinterpret_cast<__half2*>(p_hi + off) = __halves2half2(h0, h1);
-                    *reinterpret_cast<__half2*>(p_lo + off) = __halves2half2(l0, l1);
+                    *reinterpret_cast<__half2*>(p_hi + off) = h;
+                    *reinterpret_cast<__half2*>(p_lo + off) = l;
                 }
             }
         }
@@ -296,14 +297,10 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap mapQ_hi, const __grid_co
                 *reinterpret_cast<float2*>(a.R + row * a.ldr + c) = v;
                 *reinterpret_cast<float2*>(a.R + row * a.ldr + AT_D + c) = q;
                 if (a.Rpl.hi) {
-                    const __half vh0 = __float2half_rn(v.x), vh1 = __float2half_rn(v.y);
-                    const __half qh0 = __float2half_rn(q.x), qh1 = __float2half_rn(q.y);
                     __half* dh = a.Rpl.hi + row * a.Rpl.ld;
                     __half* dl = a.Rpl.lo + row * a.Rpl.ld;
-                    *reinterpret_cast<__half2*>(dh + c) = __halves2half2(vh0, vh1);
-                    *reinterpret_cast<__half2*>(dl + c) = __halves2half2(__float2half_rn(v.x - __half2float(vh0)), __float2half_rn(v.y - __half2float(vh1)));
-                    *reinterpret_cast<__half2*>(dh + AT_D + c) = __halves2half2(qh0, qh1);
-                    *reinterpret_cast<__half2*>(dl + AT_D + c) = __halves2half2(__float2half_rn(q.x - __half2float(qh0)), __float2half_rn(q.y - __half2float(qh1)));
+                    split_f16x2(v, *reinterpret_cast<__half2*>(dh + c), *reinterpret_cast<__half2*>(dl + c));
+                    split_f16x2(q, *reinterpret_cast<__half2*>(dh + AT_D + c), *reinterpret_cast<__half2*>(dl + AT_D + c));
                 }
             }
     }
@@ -321,14 +318,8 @@ __global__ void attn_kv_planes_kernel(const float* __restrict__ K, int ldk, cons
         const int b = (int)(i / ((long long)d * NP));
         float kv = 0.f, vv = 0.f;
         if (n < N) { kv = K[((size_t)b * N + n) * ldk + c]; vv = V[((size_t)b * N + n) * ldv + c]; }
-        if (n < N) {
-            __half h = __float2half_rn(kv);
-            kp.hi[((size_t)b * N + n) * kp.ld + c] = h;
-            kp.lo[((size_t)b * N + n) * kp.ld + c] = __float2half_rn(kv - __half2float(h));
-        }
-        __half h = __float2half_rn(vv);
-        vtp.hi[((size_t)b * d + c) * vtp.ld + n] = h;                 // keys >= N are written as zeros
-        vtp.lo[((size_t)b * d + c) * vtp.ld + n] = __float2half_rn(vv - __half2float(h));
+        if (n < N) split_f16(kv, kp.hi[((size_t)b * N + n) * kp.ld + c], kp.lo[((size_t)b * N + n) * kp.ld + c]);
+        split_f16(vv, vtp.hi[((size_t)b * d + c) * vtp.ld + n], vtp.lo[((size_t)b * d + c) * vtp.ld + n]);   // keys >= N: zeros
     }
 }
 

@@ -35,6 +35,7 @@
 // end) are executed by all threads of all CTAs in uniform control flow: every branch that contains
 // one depends only on the attention windows, which every CTA computes identically.
 #include "kernels_decode.cuh"
+#include "numerics.cuh"
 #include "tc_ptx.cuh"
 
 #include <cuda_fp16.h>
@@ -103,15 +104,9 @@ enum { LP_START = 0, LP_WAIT = 1, LP_GEMV = 2, LP_RELEASE = 3, LP_GATHER = 4, LP
        LP_WG_AWAIT = 18, LP_WG_MMA = 19, LP_WG_EPI = 20, LP_COUNT };
 static_assert(LP_COUNT <= DEC_NPROF, "lap buckets");
 
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
 // NOTE on `__noinline__` in this file: there is none.  With 227 KB of shared memory per CTA the L1 data cache is ~0 KB, so every
 // stack access (ABI spills of a non-inlined call, a dynamically indexed local array) is an L2 round trip of ~500 cycles: the
 // first three versions of this kernel spent 60 % of their time there (ptxas must report a 0-byte stack frame).
-__device__ __forceinline__ float sigmoid_acc(float x) { return 1.0f / (1.0f + expf(-x)); }
 // the per-frame path: ex2.approx + rcp (2 ulp each; far inside the 1e-3 budget, half the instructions)
 __device__ __forceinline__ float sigmoid_fast(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
 
@@ -141,31 +136,10 @@ __device__ __forceinline__ void cluster_sync_all() { cluster_arrive(); cluster_w
 // generic-proxy global stores (the plane histories) -> visible to later bulk copies (async proxy) once a barrier orders them
 __device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
 
-// ---- split-fp16 plane histories (DecParams::pl_hist): hi = fp16(x), lo = fp16(x - hi) ----------------------------------
+// ---- split-fp16 plane histories (DecParams::pl_hist, numerics.cuh) ------------------------------------------------------
 // index (in halfs) of channel c of row t of utterance b in the hi plane; the lo plane follows at + 2 * rows * 8
 __device__ __forceinline__ size_t pl_idx(int nslab, int rows, int b, int c, int t) {
     return ((size_t)(b * nslab + (c >> 4)) * 4 + ((c >> 3) & 1)) * (size_t)rows * 8 + (size_t)(t + DEC_PL_PAD) * 8 + (c & 7);
-}
-__device__ __forceinline__ void split_h(float v, __half& hi, __half& lo) {
-    hi = __float2half_rn(v);
-    lo = __float2half_rn(v - __half2float(hi));
-}
-// eight consecutive channels -> 16 bytes of the hi plane at p, 16 bytes of the lo plane TC_APLANE bytes further (a stage image)
-__device__ __forceinline__ void store_split8(__half* p, const float (&v)[8]) {
-    __align__(16) __half hi[8];
-    __align__(16) __half lo[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) split_h(v[i], hi[i], lo[i]);
-    *reinterpret_cast<uint4*>(p) = *reinterpret_cast<const uint4*>(hi);
-    *reinterpret_cast<uint4*>(p + TC_APLANE / 2) = *reinterpret_cast<const uint4*>(lo);
-}
-// four consecutive channels (c % 4 == 0) of one row
-__device__ __forceinline__ void pl_store4(__half* pl, size_t idx, size_t lo_off, float a, float b, float c, float d) {
-    __align__(8) __half hi[4];
-    __align__(8) __half lo[4];
-    split_h(a, hi[0], lo[0]); split_h(b, hi[1], lo[1]); split_h(c, hi[2], lo[2]); split_h(d, hi[3], lo[3]);
-    *reinterpret_cast<uint2*>(pl + idx) = *reinterpret_cast<const uint2*>(hi);
-    *reinterpret_cast<uint2*>(pl + idx + lo_off) = *reinterpret_cast<const uint2*>(lo);
 }
 // two independent fp32 FMAs on (x, y) pairs
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
@@ -466,7 +440,7 @@ __device__ __forceinline__ int layer_row(const DecParams& P, Smem& S, Stream& st
                     oh[row * C + c] = o[g];
                     if (pl) {
                         const size_t ix = pl_idx(C >> 4, P.pl_rows, b0 + g, c, j);
-                        split_h(o[g], pl[ix], pl[ix + pl_lo]);
+                        split_f16(o[g], pl[ix], pl[ix + pl_lo]);
                     }
                 }
                 if (last) {                                           // Y = sigmoid(logits), networks.py:210; next frame's AudioEnc input
@@ -809,8 +783,10 @@ __device__ __forceinline__ void pyr_ln(const DecParams& P, Smem& S, int li, int 
         *reinterpret_cast<float4*>(orow + 128 + lane * 4) = make_float4(o[4], o[5], o[6], o[7]);
         if (__half* pl = P.pl_hist[li + 1]) {                        // the next block's recompute reads these rows as planes
             const size_t lo = (size_t)P.pl_rows * 16;
-            pl_store4(pl, pl_idx(16, P.pl_rows, b0 + g, lane * 4, t), lo, o[0], o[1], o[2], o[3]);
-            pl_store4(pl, pl_idx(16, P.pl_rows, b0 + g, 128 + lane * 4, t), lo, o[4], o[5], o[6], o[7]);
+            __half* p = pl + pl_idx(16, P.pl_rows, b0 + g, lane * 4, t);           // four consecutive channels of one row
+            split_store_f16<4>(o, p, p + lo);
+            p = pl + pl_idx(16, P.pl_rows, b0 + g, 128 + lane * 4, t);
+            split_store_f16<4>(o + 4, p, p + lo);
         }
     }
 }
@@ -844,8 +820,9 @@ __device__ __forceinline__ Stream prepass(const DecParams& P, Smem& S, Stream st
                 // the same row as the first AudioDec block's A operand: slab-major planes, row t - t_lo of utterance g's stage
                 // images (lane holds channels lane * 8 .. + 8 of [ctx | q]: slab lane / 2 (+ d / 16), k8 group lane % 2)
                 __half* cs = c1s + (size_t)g * c1_utt + (size_t)(lane >> 1) * (TC_ASTAGE / 2) + (lane & 1) * (TC_RA * 8) + (t - ra.t_lo) * 8;
-                store_split8(cs, ctx);
-                store_split8(cs + (size_t)(P.d >> 4) * (TC_ASTAGE / 2), qv);
+                split_store_f16<8>(ctx, cs, cs + TC_APLANE / 2);              // the lo plane: TC_APLANE bytes further
+                __half* cq = cs + (size_t)(P.d >> 4) * (TC_ASTAGE / 2);
+                split_store_f16<8>(qv, cq, cq + TC_APLANE / 2);
             }
             fence_proxy_async_global();                   // the plane rows are read by bulk copies after the barrier
             cluster_sync_all();

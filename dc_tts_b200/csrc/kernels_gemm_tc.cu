@@ -6,11 +6,9 @@
 //   weight gradient        (mode 1):  dW[tap][k][n] += sum_b sum_t X[b, t+shift_tap, k] dY[b,t,n]
 //
 // fp32 operands cannot feed the tensor cores directly, and bf16 / single fp16 operands miss the gradient-parity budget, so every
-// operand is first written as two fp16 planes hi = fp16(s x), lo = fp16(s x - hi) with a per-tensor power-of-two scale s
-// (the largest magnitude lands in [2^13, 2^14): gradients of 1e-7 and weights of 1e-2 both use fp16's normal range), and
-// each k-step issues hi*hi + hi*lo + lo*hi into one fp32 accumulator -- the scheme of the synthesis
-// kernels (kernels_tc.cuh).  The planes are laid out so that BOTH operands of all three GEMMs are K-major tiles that TMA
-// delivers in the 64-byte swizzle, the reduction index being contiguous:
+// operand is first written as split-fp16 planes with a per-tensor scale (numerics.cuh: the format and slot_scale).  The planes
+// are laid out so that BOTH operands of all three GEMMs are K-major tiles that TMA delivers in the 64-byte swizzle, the
+// reduction index being contiguous:
 //   mode 0: A = activation planes (B, L, C) box {32 ch, 128 t, 1 b}: the conv tap is the box's time coordinate and TMA's
 //           zero fill is the zero padding;  B = weight planes [n][tap * Kp + k].
 //   mode 1: A = TRANSPOSED activation planes (tap, B, C, L) box {32 t, 128 k, 1 b} (one pre-shifted copy per tap), B = transposed
@@ -21,6 +19,7 @@
 // shared memory (over the drained ring) and store it one row per thread, each warpgroup half of the columns.
 #include "kernels.cuh"
 #include "kernels_tc.cuh"
+#include "numerics.cuh"
 #include "tc_ptx.cuh"
 
 #include <algorithm>
@@ -36,15 +35,6 @@ constexpr int G_BM = 128, G_BK = 32, G_THREADS = 384, G_MAX_STAGES = 4;
 constexpr int G_SW = G_BK * 2;                         // bytes per tile row = swizzle span (64)
 constexpr int G_APLANE = G_BM * G_SW;                  // one plane of the A tile (8 KB)
 constexpr int G_AUX = 256;
-
-// power-of-two scale of a tensor whose largest magnitude sits in the slot (float bits): max * s in [2^13, 2^14)
-__device__ __forceinline__ float slot_scale(const unsigned* slot) {
-    const float m = __uint_as_float(*slot);
-    if (!(m > 0.f) || !(m < 3.0e38f)) return 1.0f;
-    int e = 127 + 13 - ilogbf(m);
-    e = e < 1 ? 1 : (e > 254 ? 254 : e);
-    return __uint_as_float((unsigned)e << 23);
-}
 
 struct GemmTcArgs {
     int mode;                 // 0: rows x channels conv GEMM, 1: weight gradient
@@ -277,11 +267,6 @@ void launch_absmax(const float* x, int ld, long long rows, int C, unsigned* slot
     else absmax_kernel<false><<<grid, 256, 0, s>>>(x, ld, rows, C, slot);
 }
 
-__device__ __forceinline__ void split_half(float v, __half& h, __half& l) {
-    h = __float2half_rn(v);
-    l = __float2half_rn(v - __half2float(h));
-}
-
 // (rows, C) fp32 -> planes (rows, ldp), columns >= C zero; one thread per 8 columns (one 16-byte store per plane)
 __global__ void to_planes_kernel(const float* __restrict__ x, int ld, long long rows, int C, __half* __restrict__ hi,
                                  __half* __restrict__ lo, int ldp, const unsigned* slot, int vec) {
@@ -300,12 +285,9 @@ __global__ void to_planes_kernel(const float* __restrict__ x, int ld, long long 
 #pragma unroll
         for (int e = 0; e < 8; ++e) v[e] = (c + e < C) ? p[e] : 0.f;
     }
-    __align__(16) __half h[8];
-    __align__(16) __half l[8];
 #pragma unroll
-    for (int e = 0; e < 8; ++e) split_half(v[e] * s, h[e], l[e]);
-    *reinterpret_cast<uint4*>(hi + r * ldp + c) = *reinterpret_cast<const uint4*>(h);
-    *reinterpret_cast<uint4*>(lo + r * ldp + c) = *reinterpret_cast<const uint4*>(l);
+    for (int e = 0; e < 8; ++e) v[e] *= s;
+    split_store_f16<8>(v, hi + r * ldp + c, lo + r * ldp + c);
 }
 void launch_to_planes(const float* x, int ld, long long rows, int C, __half* hi, __half* lo, int ldp, const unsigned* slot, cudaStream_t s) {
     const int vec = ((ld & 3) == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0) ? 1 : 0;
@@ -333,8 +315,8 @@ __global__ void to_planes_t_kernel(const float* __restrict__ x, int ld, int B, i
         const int c = c0 + i, t = t0 + 2 * threadIdx.x;
         if (c < C && t < ldt) {                        // ldt is a multiple of 8 and t even: the pair stays inside the row
             __half h0, l0, h1, l1;
-            split_half(tile[2 * threadIdx.x][i], h0, l0);
-            split_half(tile[2 * threadIdx.x + 1][i], h1, l1);
+            split_f16(tile[2 * threadIdx.x][i], h0, l0);
+            split_f16(tile[2 * threadIdx.x + 1][i], h1, l1);
             const size_t o = (((size_t)j * B + b) * C + c) * ldt + t;
             *reinterpret_cast<__half2*>(hi + o) = __halves2half2(h0, h1);
             *reinterpret_cast<__half2*>(lo + o) = __halves2half2(l0, l1);
@@ -369,10 +351,8 @@ __global__ void w_to_planes_kernel(WTaps taps, int K, int N, int ldw, __half* __
     for (int i = threadIdx.y; i < 32; i += blockDim.y) {
         const int n = n0 + i, k = k0 + threadIdx.x;
         if (n < Nrows && k < Kp2) {
-            __half h, l;
-            split_half(tile[threadIdx.x][i], h, l);
             const size_t o = (size_t)n * Ktot + (size_t)tp * Kp2 + k;
-            hi[o] = h; lo[o] = l;
+            split_f16(tile[threadIdx.x][i], hi[o], lo[o]);
         }
     }
 }

@@ -8,6 +8,7 @@
 // small-M autoregressive decode (weight-bandwidth / latency bound) and are the
 // reference the tensor-core kernels (kernels_tc.cu) are validated against.
 #include "kernels.cuh"
+#include "numerics.cuh"
 #include <math.h>
 
 #include <stdexcept>
@@ -370,13 +371,6 @@ void launch_conv_gemm_ln(const ConvArgs& a, LnArgs n, int* tickets, cudaStream_t
 // Row-wise LayerNorm / highway epilogue: one warp per output row, values in registers,
 // two-pass mean/variance (biased, eps 1e-12: tf.contrib.layers.layer_norm).
 // ------------------------------------------------------------------------------------
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-__device__ __forceinline__ float sigmoidf_acc(float x) { return 1.0f / (1.0f + expf(-x)); }
-
 template <int MAXV>
 __device__ __forceinline__ void ln_stats(const float (&v)[MAXV], int C, int lane, float& mean, float& inv) {
     float s = 0.f;
@@ -448,7 +442,7 @@ __global__ void __launch_bounds__(256) ln_rows_kernel(const LnArgs a) {
                 float z = (v1[i] - mean1) * inv1 * __ldg(a.g1 + c) + __ldg(a.b1 + c);
                 if (a.act == 1) z = fmaxf(z, 0.f);
                 o[c] = z * keep_mul((uint32_t)(row * C + c), a.drop);
-                if (o2) o2[c] = sigmoidf_acc(z);
+                if (o2) o2[c] = sigmoid_acc(z);
             }
         }
     } else {
@@ -462,7 +456,7 @@ __global__ void __launch_bounds__(256) ln_rows_kernel(const LnArgs a) {
         for (int i = 0; i < MAXV; ++i) {
             int c = lane + 32 * i;
             if (c < C) {
-                float h1 = sigmoidf_acc((v1[i] - mean1) * inv1 * __ldg(a.g1 + c) + __ldg(a.b1 + c));
+                float h1 = sigmoid_acc((v1[i] - mean1) * inv1 * __ldg(a.g1 + c) + __ldg(a.b1 + c));
                 float h2 = (v2[i] - mean2) * inv2 * __ldg(a.g2 + c) + __ldg(a.b2 + c);
                 o[c] = (h1 * h2 + (1.0f - h1) * x[c]) * keep_mul((uint32_t)(row * C + c), a.drop);
             }
@@ -521,7 +515,7 @@ __global__ void __launch_bounds__(128) ln_row_cta_kernel(const LnArgs a) {
                 float z = (u ? d1 : d0) * inv1 * __ldg(a.g1 + c) + __ldg(a.b1 + c);
                 if (a.act == 1) z = fmaxf(z, 0.f);
                 o[c] = z * keep_mul((uint32_t)(row * C + c), a.drop);
-                if (o2) o2[c] = sigmoidf_acc(z);
+                if (o2) o2[c] = sigmoid_acc(z);
             }
         }
     } else {
@@ -534,7 +528,7 @@ __global__ void __launch_bounds__(128) ln_row_cta_kernel(const LnArgs a) {
         for (int u = 0; u < 2; ++u) {
             const int c = u ? c1 : c0;
             if (c < C) {
-                const float h1 = sigmoidf_acc((u ? d1 : d0) * inv1 * __ldg(a.g1 + c) + __ldg(a.b1 + c));
+                const float h1 = sigmoid_acc((u ? d1 : d0) * inv1 * __ldg(a.g1 + c) + __ldg(a.b1 + c));
                 const float h2 = (u ? e1 : e0) * inv2 * __ldg(a.g2 + c) + __ldg(a.b2 + c);
                 o[c] = h1 * h2 + (1.0f - h1) * x[c];
             }
@@ -579,14 +573,14 @@ __device__ void ln_row_256(const LnArgs& a, int rix, float* sm) {
             float z = d * inv1 * __ldg(a.g1 + c) + __ldg(a.b1 + c);
             if (a.act == 1) z = fmaxf(z, 0.f);
             a.out[row * a.ldo + c] = z;
-            if (a.out2) a.out2[row * a.ldo2 + c] = sigmoidf_acc(z);
+            if (a.out2) a.out2[row * a.ldo2 + c] = sigmoid_acc(z);
         }
     } else {
         const float mean2 = block_sum_256(ok ? w : 0.f, sm, warp, lane) / fC;
         const float e = ok ? w - mean2 : 0.f;
         const float inv2 = 1.0f / sqrtf(block_sum_256(e * e, sm, warp, lane) / fC + 1e-12f);
         if (ok) {
-            const float h1 = sigmoidf_acc(d * inv1 * __ldg(a.g1 + c) + __ldg(a.b1 + c));
+            const float h1 = sigmoid_acc(d * inv1 * __ldg(a.g1 + c) + __ldg(a.b1 + c));
             const float h2 = e * inv2 * __ldg(a.g2 + c) + __ldg(a.b2 + c);
             a.out[row * a.ldo + c] = h1 * h2 + (1.0f - h1) * a.X[row * a.ldx + c];
         }
@@ -705,10 +699,8 @@ __global__ void __launch_bounds__(ATT_WARPS * 32) attention_kernel(const AttnArg
 #pragma unroll
         for (int i = 0; i < 8; ++i)
             if (lane * 8 + i < d) {
-                __half h = __float2half_rn(ctx[i]);
-                rh[lane * 8 + i] = h; rl[lane * 8 + i] = __float2half_rn(ctx[i] - __half2float(h));
-                h = __float2half_rn(qv[i]);
-                rh[d + lane * 8 + i] = h; rl[d + lane * 8 + i] = __float2half_rn(qv[i] - __half2float(h));
+                split_f16(ctx[i], rh[lane * 8 + i], rl[lane * 8 + i]);
+                split_f16(qv[i], rh[d + lane * 8 + i], rl[d + lane * 8 + i]);
             }
     }
     if (a.align) {

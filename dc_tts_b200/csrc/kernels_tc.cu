@@ -19,6 +19,7 @@
 //   warpgroup 1  epilogue: thread == row, so LN reductions are thread-local; one
 //           statistics sweep and one normalise+store sweep over the tile.
 #include "kernels_tc.cuh"
+#include "numerics.cuh"
 #include "tc_ptx.cuh"
 
 #include <cstdlib>
@@ -35,8 +36,6 @@ constexpr int TC_MAX_STAGES = 8;
 constexpr int TC_AUX_BYTES = 256 /*barriers*/ + 3 * 512 * 4 /*bias,gamma,beta*/ + 128 * 16 /*this CTA's LN partials*/;
 constexpr int TC_MAX_SMEM = 227 * 1024;
 
-__device__ __forceinline__ float sigmoid_acc(float x) { return 1.0f / (1.0f + expf(-x)); }
-
 // Optional progress markers into host-mapped memory (survive a trapped launch): dbg[64*cta + slot].
 __device__ __forceinline__ void dbg_mark(int* dbg, int slot, int v) {
     if (dbg) {
@@ -49,33 +48,15 @@ __device__ __forceinline__ void dbg_time(int* dbg, int slot) {
     if (dbg) dbg_mark(dbg, slot, (int)(clock64() & 0x7fffffff));
 }
 
-__device__ __forceinline__ void split_store16(const float (&o)[16], __half* hi, __half* lo) {
-    __align__(16) __half h[16];
-    __align__(16) __half l[16];
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-        h[i] = __float2half_rn(o[i]);
-        l[i] = __float2half_rn(o[i] - __half2float(h[i]));
-    }
-    reinterpret_cast<uint4*>(hi)[0] = reinterpret_cast<const uint4*>(h)[0];
-    reinterpret_cast<uint4*>(hi)[1] = reinterpret_cast<const uint4*>(h)[1];
-    reinterpret_cast<uint4*>(lo)[0] = reinterpret_cast<const uint4*>(l)[0];
-    reinterpret_cast<uint4*>(lo)[1] = reinterpret_cast<const uint4*>(l)[1];
-}
-
 __device__ __forceinline__ void store_planes(const Planes& p, size_t row, int col, int C, const float (&o)[16]) {
     __half* hi = p.hi + row * p.ld + col;
     __half* lo = p.lo + row * p.ld + col;
     if (col + 16 <= p.ld) {
-        split_store16(o, hi, lo);
+        split_store_f16<16>(o, hi, lo);
     } else {
 #pragma unroll
         for (int i = 0; i < 16; ++i)
-            if (col + i < C) {
-                __half h = __float2half_rn(o[i]);
-                hi[i] = h;
-                lo[i] = __float2half_rn(o[i] - __half2float(h));
-            }
+            if (col + i < C) split_f16(o[i], hi[i], lo[i]);
     }
 }
 
@@ -418,7 +399,7 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
                         float z1 = (fmaf(v1[i], inv_s, s_bias[c + i]) - mean1) * rstd1 * s_gam[c + i] + s_bet[c + i];
                         float z2 = (fmaf(v2[i], inv_s, s_bias[half + c + i]) - mean2) * rstd2 * s_gam[half + c + i] + s_bet[half + c + i];
                         float h1 = sigmoid_acc(z1);
-                        float x = __half2float(xh[i]) + __half2float(xl[i]);
+                        float x = join_f16(xh[i], xl[i]);
                         o[i] = h1 * z2 + (1.0f - h1) * x;
                     }
                     if (a.out_tma) {
@@ -426,7 +407,7 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
                         __align__(16) __half oh[16];
                         __align__(16) __half ol[16];
 #pragma unroll
-                        for (int i = 0; i < 16; ++i) { oh[i] = __float2half_rn(o[i]); ol[i] = __float2half_rn(o[i] - __half2float(oh[i])); }
+                        for (int i = 0; i < 16; ++i) split_f16(o[i], oh[i], ol[i]);
                         *reinterpret_cast<uint4*>(sh + k0) = reinterpret_cast<const uint4*>(oh)[0];
                         *reinterpret_cast<uint4*>(sh + k1) = reinterpret_cast<const uint4*>(oh)[1];
                         *reinterpret_cast<uint4*>(sl + k0) = reinterpret_cast<const uint4*>(ol)[0];
@@ -496,21 +477,16 @@ __global__ void f32_to_planes_kernel(const float* __restrict__ x, int ldx, Plane
     long long total = rows * C;
     if (i >= total) return;
     long long r = i / C; int c = (int)(i - r * C);
-    float v = x[r * ldx + c];
-    __half h = __float2half_rn(v);
-    p.hi[r * p.ld + c] = h;
-    p.lo[r * p.ld + c] = __float2half_rn(v - __half2float(h));
+    split_f16(x[r * ldx + c], p.hi[r * p.ld + c], p.lo[r * p.ld + c]);
 }
 __global__ void planes_to_f32_kernel(Planes p, float* __restrict__ y, int ldy, long long rows, int C) {
     long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     long long total = rows * C;
     if (i >= total) return;
     long long r = i / C; int c = (int)(i - r * C);
-    y[r * ldy + c] = __half2float(p.hi[r * p.ld + c]) + __half2float(p.lo[r * p.ld + c]);
+    y[r * ldy + c] = join_f16(p.hi[r * p.ld + c], p.lo[r * p.ld + c]);
 }
-// One CTA per utterance: abs-max of its L x C inputs -> s = 2^k with max * s in [2^14, 2^15) (1 for an all-zero or
-// non-finite utterance), then hi = fp16(s x), lo = fp16(s x - hi).  s x is exact in fp32, so s only moves the values into
-// fp16's normal range: unscaled, 1e-8 flushes to zero and 1e-6 .. 1e-4 keep a few bits.
+// One CTA per utterance: abs-max of its L x C inputs -> s = utterance_scale(max), then the planes of s x.
 constexpr int PLANES_SCALED_THREADS = 512;
 __global__ void __launch_bounds__(PLANES_SCALED_THREADS)
 f32_to_planes_scaled_kernel(const float* __restrict__ x, int ldx, Planes p, int L, int C, float* __restrict__ in_inv) {
@@ -529,12 +505,7 @@ f32_to_planes_scaled_kernel(const float* __restrict__ x, int ldx, Planes p, int 
     __syncthreads();
     if (threadIdx.x == 0) {
         for (int w = 1; w < (int)(blockDim.x >> 5); ++w) m = fmaxf(m, s_red[w]);
-        float sc = 1.f;
-        if (m > 0.f && isfinite(m)) {
-            int e;
-            frexpf(m, &e);                                     // m in [2^(e-1), 2^e)
-            sc = ldexpf(1.f, min(15 - e, 100));                // 1/s stays a normal float
-        }
+        const float sc = utterance_scale(m);
         s_scale = sc;
         in_inv[b] = 1.f / sc;
     }
@@ -543,10 +514,7 @@ f32_to_planes_scaled_kernel(const float* __restrict__ x, int ldx, Planes p, int 
     const size_t row0 = (size_t)b * L;
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
         const int r = i / C, c = i - r * C;
-        const float v = xb[(size_t)r * ldx + c] * sc;
-        const __half h = __float2half_rn(v);
-        p.hi[(row0 + r) * p.ld + c] = h;
-        p.lo[(row0 + r) * p.ld + c] = __float2half_rn(v - __half2float(h));
+        split_f16(xb[(size_t)r * ldx + c] * sc, p.hi[(row0 + r) * p.ld + c], p.lo[(row0 + r) * p.ld + c]);
     }
 }
 void launch_f32_to_planes(const float* x, int ldx, Planes p, long long rows, int C, cudaStream_t s) {

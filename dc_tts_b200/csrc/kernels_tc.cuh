@@ -1,13 +1,7 @@
 // kernels_tc.cuh -- interface of the wgmma fused conv + LayerNorm / highway kernels.
 //
-// Activation format on the tensor-core path ("split planes"): every fp32 activation x is
-// held as two fp16 tensors hi = fp16(x), lo = fp16(x - hi) (22 significand bits together,
-// 4 bytes per element like fp32).  The audio-level input of AudioEnc, AudioDec and SSRN is
-// first multiplied by a power-of-two scale per utterance (launch_f32_to_planes_scaled),
-// undone in the first block's epilogue; hidden activations are LayerNorm outputs, O(1) per
-// row, and unscaled.
-// A conv-GEMM is three wgmma passes per k-step: hi*Whi + hi*Wlo + lo*Whi accumulated in
-// fp32 registers -- fp32-grade results on the fp16 tensor pipe.  Single-pass fp16/tf32 operands miss the 1e-3 parity budget (DESIGN.md).
+// Activations on the tensor-core path are split-fp16 planes (numerics.cuh).  The audio-level input of AudioEnc, AudioDec
+// and SSRN is scaled per utterance (launch_f32_to_planes_scaled), undone in the first block's epilogue.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -91,8 +85,8 @@ void launch_attn_kv_planes(const float* K, int ldk, const float* V, int ldv, Pla
 void launch_attention_tc(const Planes& Q, const Planes& K, const Planes& Vt, const AttnTcArgs& a, int B, cudaStream_t s);
 
 void launch_f32_to_planes(const float* x, int ldx, Planes p, long long rows, int C, cudaStream_t s);
-// (B, L, C) fp32 -> planes of s_b x with one power-of-two scale s_b per utterance (max |x_b| s_b in [2^14, 2^15)), so
-// that quiet inputs (silence at 1e-8) keep fp16's normal range; in_inv[b] = 1 / s_b for TcArgs::in_inv.  No host sync.
+// (B, L, C) fp32 -> planes of s_b x with s_b = utterance_scale(max |x_b|) (numerics.cuh); in_inv[b] = 1 / s_b for
+// TcArgs::in_inv.  No host sync.
 void launch_f32_to_planes_scaled(const float* x, int ldx, Planes p, int B, int L, int C, float* in_inv, cudaStream_t s);
 void launch_planes_to_f32(Planes p, float* y, int ldy, long long rows, int C, cudaStream_t s);
 

@@ -13,6 +13,7 @@
 //   attn_bwd_q_kernel / attn_bwd_kv_kernel   softmax attention backward incl. the guided-attention term
 //   embed_bwd_kernel, adam_kernel
 #include "kernels.cuh"
+#include "numerics.cuh"
 
 #include <cmath>
 
@@ -48,7 +49,7 @@ __global__ void train_loss_kernel(const float* __restrict__ logits, int ldl, con
         const long long row = i / C;
         const int c = (int)(i - row * C);
         const float x = logits[row * ldl + c], m = target[i];
-        const float y = 1.0f / (1.0f + expf(-x));
+        const float y = sigmoid_acc(x);
         const float d = y - m;
         l1 = fabsf(d);
         bce = fmaxf(x, 0.f) - x * m + log1pf(expf(-fabsf(x)));
@@ -77,7 +78,7 @@ __global__ void sigmoid_rows_kernel(const float* __restrict__ x, int ldx, float*
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const long long row = i / C;
-    out[i] = 1.0f / (1.0f + expf(-x[row * ldx + (i - row * C)]));
+    out[i] = sigmoid_acc(x[row * ldx + (i - row * C)]);
 }
 
 void launch_sigmoid_rows(const float* x, int ldx, float* out, long long rows, int C, cudaStream_t s) {
@@ -86,12 +87,6 @@ void launch_sigmoid_rows(const float* x, int ldx, float* out, long long rows, in
 }
 
 // ------------------------------------------------------------------------------------ block backward
-__device__ __forceinline__ float wsum(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
 // LayerNorm backward for one half held in registers.  yhat = (y - mean) rstd, z = yhat g + b.
 //   dy = rstd (dyh - mean(dyh) - yhat mean(dyh yhat)),  dyh = dz g
 template <int MAXV>
@@ -104,7 +99,7 @@ __device__ __forceinline__ void ln_bwd_half(const float (&yhat)[MAXV], const flo
         if (c < C) { const float t = dz[i] * __ldg(gam + c); dy[i] = t; s1 += t; s2 = fmaf(t, yhat[i], s2); }
         else dy[i] = 0.f;
     }
-    s1 = wsum(s1) / (float)C; s2 = wsum(s2) / (float)C;
+    s1 = warp_sum(s1) / (float)C; s2 = warp_sum(s2) / (float)C;
 #pragma unroll
     for (int i = 0; i < MAXV; ++i) dy[i] = rstd * (dy[i] - s1 - yhat[i] * s2);
 }
@@ -114,11 +109,11 @@ __device__ __forceinline__ void ln_fwd_half(const float* __restrict__ y, int C, 
     float s = 0.f;
 #pragma unroll
     for (int i = 0; i < MAXV; ++i) { const int c = lane + 32 * i; yhat[i] = c < C ? y[c] : 0.f; s += yhat[i]; }
-    const float mean = wsum(s) / (float)C;
+    const float mean = warp_sum(s) / (float)C;
     float q = 0.f;
 #pragma unroll
     for (int i = 0; i < MAXV; ++i) { const int c = lane + 32 * i; const float d = c < C ? yhat[i] - mean : 0.f; yhat[i] = d; q = fmaf(d, d, q); }
-    rstd = 1.0f / sqrtf(wsum(q) / (float)C + 1e-12f);
+    rstd = 1.0f / sqrtf(warp_sum(q) / (float)C + 1e-12f);
 #pragma unroll
     for (int i = 0; i < MAXV; ++i) yhat[i] *= rstd;
 }
@@ -174,7 +169,7 @@ __global__ void __launch_bounds__(BWD_WARPS * 32) train_block_bwd_kernel(const B
                 float d1 = 0.f, d2 = 0.f;
                 if (c < C) {
                     const float g = go[c] * keep_mul((uint32_t)(row * C + c), a.drop);
-                    const float h1 = 1.0f / (1.0f + expf(-(yh1[i] * __ldg(a.g1 + c) + __ldg(a.b1 + c))));
+                    const float h1 = sigmoid_acc(yh1[i] * __ldg(a.g1 + c) + __ldg(a.b1 + c));
                     const float h2 = yh2[i] * __ldg(a.g2 + c) + __ldg(a.b2 + c);
                     d1 = g * (h2 - x[c]) * h1 * (1.0f - h1);
                     d2 = g * h1;
@@ -330,7 +325,7 @@ __global__ void __launch_bounds__(128) attn_bwd_q_kernel(const AttnBwdArgs a) {
         float s = 0.f;
 #pragma unroll
         for (int i = 0; i < 8; ++i) s = fmaf(dctx[i], __ldg(v + lane * 8 + i), s);
-        s = wsum(s);
+        s = warp_sum(s);
         const float p = a.align[((size_t)b * a.N + n) * a.T + t];
         const float g = (n < a.n_lim && t < a.t_lim) ? a.gts[(size_t)n * a.ld_gts + t] : 0.f;
         const float pg = p * g;
