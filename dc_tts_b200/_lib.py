@@ -37,6 +37,7 @@ SIGNATURES = {
     "dctts_attention": (C.c_int, [Handle, _p, _p, _p, _i32, _i32, _i32, _i32, _p, _p, _p, _p, _p]),
     "dctts_audiodec": (C.c_int, [Handle, _p, _i32, _i32, _p, _p, _p]),
     "dctts_ssrn": (C.c_int, [Handle, _p, _i32, _i32, _p, _p, _p]),
+    "dctts_ssrn_ragged": (C.c_int, [Handle, _p, _i32, _i32, _p, _p, _p, _p]),
     "dctts_text2mel_forward": (C.c_int, [Handle, _p, _p, _p, _i32, _p, _p, _p, _p]),
     "dctts_text2mel_generate": (C.c_int, [Handle, _p, _i32, _i32, _p, _p, _p, _p, _p]),
     "dctts_text2mel_generate_until": (C.c_int, [Handle, _p, _i32, _i32, _p, _i32, _p, _p, _p, _p]),
@@ -48,6 +49,7 @@ SIGNATURES = {
     "dctts_vocoder_stage": (C.c_int, [Handle, _i32, _i32, _i32, _p, _p, _p, C.POINTER(_i32), _p]),
     "dctts_set_vocoder_params": (C.c_int, [Handle, _i32, _i32, C.c_float, C.c_float, C.c_float, C.c_double, _i32]),
     "dctts_spectrogram2wav": (C.c_int, [Handle, _p, _i32, _i32, _i32, _p, _p, _p]),
+    "dctts_spectrogram2wav_ragged": (C.c_int, [Handle, _p, _i32, _i32, _p, _i32, _p, _p, _p]),
     "dctts_get_spectrograms": (C.c_int, [Handle, _p, _i64, _i32, _p, _p, _i32, C.POINTER(_i32), C.POINTER(_i32), _p]),
     "dctts_load_spectrograms_batch": (C.c_int, [Handle, _p, _i32, C.POINTER(_i64), _i32, _i32, _p, _p, _i32, C.POINTER(_i32),
                                                 C.POINTER(_i32), C.POINTER(_i32), _p]),

@@ -129,29 +129,34 @@ VocoderArgs voc_args(H* h, const char* fn, int B, int T, cudaStream_t s) {
     h->voc_deemph.ensure(voc_deemph_scratch_bytes(B, T, hop));
     if (h->voc_tables_T != T || h->voc_tables_win != win || h->voc_tables_hop != hop) {
         h->voc_tw.ensure(n_fft * sizeof(float2)); h->voc_window.ensure(win * sizeof(float));
-        h->voc_wss.ensure((size_t)(n_fft + hop * (T - 1)) * sizeof(float));
-        voc_make_tables(n_fft, h->voc_tw.as<float2>(), h->voc_window.as<float>(), h->voc_wss.as<float>(), T, win, hop, s);
+        h->voc_wss.ensure((size_t)(n_fft + hop * (T - 1)) * sizeof(float)); h->voc_wsq.ensure(n_fft * sizeof(float));
+        voc_make_tables(n_fft, h->voc_tw.as<float2>(), h->voc_window.as<float>(), h->voc_wss.as<float>(), T, win, hop, s,
+                        h->voc_wsq.as<float>());
         CUDA_CHECK(cudaGetLastError());
         h->voc_tables_T = T; h->voc_tables_win = win; h->voc_tables_hop = hop;
     }
     VocoderArgs a{};
     a.S = h->voc_S.as<float>(); a.X = h->voc_X.as<float2>(); a.frames = h->voc_frames.as<float>();
     a.mse = h->voc_mse.as<float>(); a.tw = h->voc_tw.as<float2>(); a.window = h->voc_window.as<float>();
-    a.wss = h->voc_wss.as<float>(); a.deemph = h->voc_deemph.as<double>(); a.B = B; a.T = T; a.F = F; a.win = win; a.hop = hop;
+    a.wss = h->voc_wss.as<float>(); a.wsq = h->voc_wsq.as<float>(); a.deemph = h->voc_deemph.as<double>(); a.B = B; a.T = T; a.F = F; a.win = win; a.hop = hop;
     a.n_iter = h->voc.n_iter;
     a.max_db = h->voc.max_db; a.ref_db = h->voc.ref_db; a.power = h->voc.power; a.preemphasis = h->voc.preemph;
     return a;
 }
 
 // librosa.effects.trim from the device frame energies a.mse (B, 1 + Ly / 512): frames within 60 dB of the loudest.
-// Synchronises s.
-void voc_trims(const VocoderArgs& a, int32_t* trim_host, cudaStream_t s) {
+// T_host (optional): the frame count of each utterance of a ragged call, whose energies cover its own 1 + Ly_b / 512
+// frames.  Synchronises s.
+void voc_trims(const VocoderArgs& a, int32_t* trim_host, cudaStream_t s, const int32_t* T_host = nullptr) {
     const int Ly = a.hop * (a.T - 1), nfr = 1 + Ly / 512;
     std::vector<float> mse((size_t)a.B * nfr);
     CUDA_CHECK(cudaMemcpyAsync(mse.data(), a.mse, mse.size() * sizeof(float), cudaMemcpyDeviceToHost, s));
     CUDA_CHECK(cudaStreamSynchronize(s));
     if (trim_host)
-        for (int b = 0; b < a.B; ++b) trim_from_mse(mse.data() + (size_t)b * nfr, nfr, Ly, trim_host + 2 * b);
+        for (int b = 0; b < a.B; ++b) {
+            const int Lyb = T_host ? a.hop * (T_host[b] - 1) : Ly;
+            trim_from_mse(mse.data() + (size_t)b * nfr, 1 + Lyb / 512, Lyb, trim_host + 2 * b);
+        }
 }
 
 }  // namespace
@@ -181,6 +186,28 @@ int dctts_spectrogram2wav(dctts_handle h, const float* mag, int32_t B, int32_t T
         h->launches += voc_launches_per_call(a.n_iter);
         CUDA_CHECK(cudaGetLastError());
         voc_trims(a, trim_host, s);
+    });
+}
+
+int dctts_spectrogram2wav_ragged(dctts_handle h, const float* mag, int32_t B, int32_t T, const int32_t* lengths_host,
+                                 int32_t n_iter, float* wav, int32_t* trim_host, void* stream) {
+    return guarded(h, [&] {
+        const std::string fn = "dctts_spectrogram2wav_ragged";
+        REQUIRE(mag && wav && lengths_host, fn + ": bad arguments");
+        for (int b = 0; b < B; ++b)
+            REQUIRE(lengths_host[b] >= 2 && lengths_host[b] <= T, fn + ": utterance " + std::to_string(b) + " has " +
+                                                                  std::to_string(lengths_host[b]) + " frames (need 2 to T = " +
+                                                                  std::to_string(T) + ")");
+        cudaStream_t s = S(h, stream);
+        VocoderArgs a = voc_args(h, fn.c_str(), B, T, s);
+        h->voc_len.ensure((size_t)B * sizeof(int));
+        CUDA_CHECK(cudaMemcpyAsync(h->voc_len.p, lengths_host, (size_t)B * sizeof(int), cudaMemcpyHostToDevice, s));
+        a.mag = mag; a.wav = wav; a.lengths = h->voc_len.as<int>();
+        if (n_iter >= 0) a.n_iter = n_iter;
+        voc_run(a, s);
+        h->launches += voc_launches_per_call(a.n_iter);
+        CUDA_CHECK(cudaGetLastError());
+        voc_trims(a, trim_host, s, lengths_host);
     });
 }
 

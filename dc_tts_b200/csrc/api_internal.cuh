@@ -161,6 +161,7 @@ struct dctts_handle_s {
     DevBuf rs_win, rs_tab;                                          // resampling: kaiser_best filter, per-call tables
     int feat_sr = 0, feat_win = 0;
     DevBuf voc_S, voc_X, voc_frames, voc_mse, voc_tw, voc_window, voc_wss, voc_deemph;
+    DevBuf voc_wsq, voc_len;                      // squared window row (n_fft), per-utterance frame counts (ragged call)
     int voc_tables_T = 0, voc_tables_win = 0, voc_tables_hop = 0;
     // co-resident 16-CTA clusters of the 144-column block kernel (the F = 2049 conv1d blocks), -1 until first needed;
     // when none fits, why those blocks run on the fp32 kernels

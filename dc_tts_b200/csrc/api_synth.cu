@@ -164,16 +164,39 @@ void run_deconv(Launch& lc, const LayerDev& l, const float* X, int ldx, int B, i
 
 bool chain_tc_ok(H* h, const std::vector<LayerDev>& net);
 void run_chain_tc_planes(Launch& lc, const std::vector<LayerDev>& net, Planes cur, int which, int B, int L,
-                         float* out, float* out_sig, int first_extra_shift, const float* in_inv);
+                         float* out, float* out_sig, int first_extra_shift, const float* in_inv, const int* lengths = nullptr);
 void run_chain_full_tc(Launch& lc, const std::vector<LayerDev>& net, const float* X, int ldx, int B, int L,
-                       float* out, float* out_sig);
+                       float* out, float* out_sig, const int* lengths = nullptr);
 
 // A whole chain over full sequences, ping-ponging act0/act1; the last block writes
 // `out` (dense, ld = its cout) and optionally sigmoid(out) into out_sig.
+// lengths (device, optional; 1 <= lengths[b] <= L): each utterance's output rows [0, lengths[b] Lout / L) are what the chain
+// computes for that utterance alone at L = lengths[b], and its rows past them are zeros.  On the wgmma path that is one
+// launch per block over the batch.  The fp32 path's GEMM schedule depends on a launch's row count (split-K below 257 rows,
+// tiled above), so one launch over the batch cannot reproduce it: there the lengths are read back and the chain runs once
+// per utterance.
 void run_chain_full(Launch& lc, const std::vector<LayerDev>& net, const float* X, int ldx, int B, int L,
-                    float* out, float* out_sig) {
+                    float* out, float* out_sig, const int* lengths = nullptr) {
     H* h = lc.h;
-    if (chain_tc_ok(h, net) && (out || out_sig)) { run_chain_full_tc(lc, net, X, ldx, B, L, out, out_sig); return; }
+    if (chain_tc_ok(h, net) && (out || out_sig)) { run_chain_full_tc(lc, net, X, ldx, B, L, out, out_sig, lengths); return; }
+    if (lengths) {
+        std::vector<int> n((size_t)B);
+        CUDA_CHECK(cudaMemcpyAsync(n.data(), lengths, n.size() * sizeof(int), cudaMemcpyDeviceToHost, lc.s));
+        CUDA_CHECK(cudaStreamSynchronize(lc.s));
+        int up = 1;                                        // output rows per input row
+        for (auto& l : net) if (l.kind == K_D) up *= 2;
+        const int Lout = L * up, C = net.back().cout;
+        for (int b = 0; b < B; ++b)
+            REQUIRE(n[b] >= 1 && n[b] <= L, "utterance " + std::to_string(b) + ": length " + std::to_string(n[b]) +
+                                                " outside [1, " + std::to_string(L) + "]");
+        for (int b = 0; b < B; ++b) {
+            const size_t o = (size_t)b * Lout * C, live = (size_t)n[b] * up * C, dead = (size_t)Lout * C - live;
+            run_chain_full(lc, net, X + (size_t)b * L * ldx, ldx, 1, n[b], out ? out + o : nullptr, out_sig ? out_sig + o : nullptr);
+            if (dead && out) CUDA_CHECK(cudaMemsetAsync(out + o + live, 0, dead * sizeof(float), lc.s));
+            if (dead && out_sig) CUDA_CHECK(cudaMemsetAsync(out_sig + o + live, 0, dead * sizeof(float), lc.s));
+        }
+        return;
+    }
     const float* cur = X; int ld = ldx; int len = L;
     float* bufs[2] = {h->act0.as<float>(), h->act1.as<float>()};
     int which = 0;
@@ -203,7 +226,7 @@ Planes ws_planes(H* h, int which, int C) {
 // (B, L, cin) input; the output goes to planes and/or fp32 tensors.
 void run_block_tc(Launch& lc, const LayerDev& l, int rate, bool causal, int act, Planes X, RowWin win,
                   int TT, int TB, int tiles_t, Planes out, float* out_f32, int ld_f32, float* sig_f32, int ld_sig,
-                  Planes sig, int extra_shift = 0, const float* in_inv = nullptr) {
+                  Planes sig, int extra_shift = 0, const float* in_inv = nullptr, const int* lengths = nullptr, int len_shift = 0) {
     const LayerDev::TcPack& p = l.tc;
     REQUIRE(p.ok, "tensor-core path not available for this block");
     // the highway residual is read from the input planes unscaled; scaled input planes only reach conv1d blocks
@@ -227,6 +250,7 @@ void run_block_tc(Launch& lc, const LayerDev& l, int rate, bool causal, int act,
     }
     a.TT = TT; a.TB = TB; a.tiles_t = tiles_t; a.ntiles = tiles; a.win = win;
     a.X = X; a.out = out; a.out_f32 = out_f32; a.ld_f32 = ld_f32; a.sig_f32 = sig_f32; a.ld_sig = ld_sig; a.sig = sig;
+    a.lengths = lengths; a.len_shift = len_shift;
     // the A tile is identical in all CTAs of the cluster: fetch it once (TMA multicast) when the
     // tile is 128 consecutive time rows, each CTA contributing 128/ncta of them
     const bool no_mcast = h->opt.tc_mcast == 0;
@@ -293,11 +317,12 @@ bool chain_tc_ok(H* h, const std::vector<LayerDev>& net) {
 
 // Whole chain on the tensor-core path, starting from split planes `cur` (buffer index `which`
 // of the ping-pong pair, or -1 for an external buffer): ... -> fp32 out (+ sigmoid).
-// in_inv: inverse per-utterance scales of `cur` (launch_f32_to_planes_scaled), or null.
+// in_inv: inverse per-utterance scales of `cur` (launch_f32_to_planes_scaled), or null.  lengths: per-utterance lengths
+// at L (device), or null; every block stores its rows past them as zeros (run_chain_full).
 void run_chain_tc_planes(Launch& lc, const std::vector<LayerDev>& net, Planes cur, int which, int B, int L,
-                         float* out, float* out_sig, int first_extra_shift, const float* in_inv) {
+                         float* out, float* out_sig, int first_extra_shift, const float* in_inv, const int* lengths) {
     H* h = lc.h;
-    int len = L;
+    int len = L, len_shift = 0;
     int nxt = (which == 0) ? 1 : 0;
     for (size_t i = 0; i < net.size(); ++i) {
         const LayerDev& l = net[i];
@@ -305,8 +330,8 @@ void run_chain_tc_planes(Launch& lc, const std::vector<LayerDev>& net, Planes cu
         Planes dst = last ? Planes{} : ws_planes(h, nxt, l.cout);
         run_block_tc(lc, l, l.rate, l.causal, l.act, cur, RowWin{B, len, len, nullptr}, 128, 1, (len + 127) / 128,
                      dst, last ? out : nullptr, l.cout, last ? out_sig : nullptr, l.cout, Planes{},
-                     i == 0 ? first_extra_shift : 0, i == 0 ? in_inv : nullptr);
-        if (l.kind == K_D) len *= 2;
+                     i == 0 ? first_extra_shift : 0, i == 0 ? in_inv : nullptr, lengths, len_shift);
+        if (l.kind == K_D) { len *= 2; ++len_shift; }
         cur = dst; nxt ^= 1;
     }
 }
@@ -326,26 +351,29 @@ float* input_inv_scales(H* h, int B) {
 // block reads a LayerNorm output, O(1) per row, or an embedding row, whose magnitude is the committed table's: unscaled
 // planes (null).  The op-level entry points follow the same rule, so a network composed block by block computes
 // exactly what its chain computes.
-const float* block_input_planes(Launch& lc, const LayerDev& l, const float* x, int ldx, Planes p, int B, int L) {
+// lengths (device, optional, network inputs only): utterance b's rows past lengths[b] are not read and become zero planes.
+const float* block_input_planes(Launch& lc, const LayerDev& l, const float* x, int ldx, Planes p, int B, int L,
+                                const int* lengths = nullptr) {
     H* h = lc.h;
     const bool net_input = (!h->audioenc.empty() && &l == &h->audioenc[0]) || (!h->audiodec.empty() && &l == &h->audiodec[0]) ||
                            (!h->ssrn.empty() && &l == &h->ssrn[0]);
     if (!net_input) {
+        REQUIRE(!lengths, "block_input_planes: per-utterance lengths on a hidden block's input");
         launch_f32_to_planes(x, ldx, p, (long long)B * L, l.cin, lc.s); lc.count();
         return nullptr;
     }
     float* in_inv = input_inv_scales(h, B);
-    launch_f32_to_planes_scaled(x, ldx, p, B, L, l.cin, in_inv, lc.s); lc.count();
+    launch_f32_to_planes_scaled(x, ldx, p, B, L, l.cin, in_inv, lc.s, lengths); lc.count();
     return in_inv;
 }
 
 // fp32 in -> planes -> chain
 void run_chain_full_tc(Launch& lc, const std::vector<LayerDev>& net, const float* X, int ldx, int B, int L,
-                       float* out, float* out_sig) {
+                       float* out, float* out_sig, const int* lengths) {
     H* h = lc.h;
     Planes cur = ws_planes(h, 0, net[0].cin);
-    const float* in_inv = block_input_planes(lc, net[0], X, ldx, cur, B, L);
-    run_chain_tc_planes(lc, net, cur, 0, B, L, out, out_sig, 0, in_inv);
+    const float* in_inv = block_input_planes(lc, net[0], X, ldx, cur, B, L, lengths);
+    run_chain_tc_planes(lc, net, cur, 0, B, L, out, out_sig, 0, in_inv, lengths);
 }
 
 }  // namespace
@@ -789,6 +817,18 @@ int dctts_ssrn(dctts_handle h, const float* Y, int32_t B, int32_t T, float* Z_lo
         ensure_ws(h, B);
         Launch lc{h, S(h, stream)};
         run_chain_full(lc, h->ssrn, Y, h->hp.n_mels, B, T, Z_logits, Z);
+    });
+}
+
+int dctts_ssrn_ragged(dctts_handle h, const float* Y, int32_t B, int32_t T, const int32_t* lengths, float* Z_logits, float* Z,
+                      void* stream) {
+    return guarded(h, [&] {
+        REQUIRE(h->committed, "parameters not committed");
+        REQUIRE(B >= 1 && T >= 1 && T <= h->hp.max_T && Y && Z && lengths,
+                "dctts_ssrn_ragged: bad arguments (T must be <= max_T, lengths non-null)");
+        ensure_ws(h, B);
+        Launch lc{h, S(h, stream)};
+        run_chain_full(lc, h->ssrn, Y, h->hp.n_mels, B, T, Z_logits, Z, lengths);
     });
 }
 

@@ -124,15 +124,20 @@ struct VocoderArgs {
     const float2* tw; const float* window; const float* wss;
     double* deemph;                // (B, chunks) float64 states of the de-pre-emphasis recurrence
     int B, T, F, win, hop, n_iter;
+    // ragged call: (B) DEVICE frame counts, 2 <= lengths[b] <= T; utterance b is computed as a call at T = lengths[b] alone
+    // (its mag rows past it are not read, its samples past hop (lengths[b] - 1) are 0).  Null: every utterance has T.
+    const int* lengths;
+    const float* wsq;              // (n_fft) squared window centred in the frame: window sum-square past wss's valid range
     float max_db, ref_db, power;
     double preemphasis;            // float64 like the reference's scipy.signal.lfilter([1], [1, -hp.preemphasis], wav)
 };
 // n_fft 1024, 2048 and 4096 have kernel instantiations (F = 1 + n_fft / 2 = 513, 1025, 2049); the launchers take n_fft
 // from F and throw for any other size
 bool voc_fft_size_ok(int n_fft);
-// twiddles tw[k] = exp(-2 pi i k / n_fft) (n_fft entries), the win-tap Hann window, and the window sum-square of T frames
-// (n_fft + hop (T - 1) entries)
-void voc_make_tables(int n_fft, float2* tw_dev, float* window_dev, float* wss_dev, int T, int win, int hop, cudaStream_t s);
+// twiddles tw[k] = exp(-2 pi i k / n_fft) (n_fft entries), the win-tap Hann window, the window sum-square of T frames
+// (n_fft + hop (T - 1) entries) and, when wsq_dev is given, the squared window it sums (n_fft entries)
+void voc_make_tables(int n_fft, float2* tw_dev, float* window_dev, float* wss_dev, int T, int win, int hop, cudaStream_t s,
+                     float* wsq_dev = nullptr);
 // voc_run = voc_prepare, (voc_istft, voc_stft_phase) x n_iter, voc_istft, voc_deemph, voc_energies
 void voc_prepare(const VocoderArgs& a, cudaStream_t s);      // mag -> S, X = S (zero phase); 1 launch
 void voc_istft(const VocoderArgs& a, cudaStream_t s);        // X -> frames -> wav; 2 launches

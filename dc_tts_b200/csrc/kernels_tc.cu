@@ -267,6 +267,10 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
 
         const int b = b0s + bi, t = t0s + ti;
         const bool row_ok = (b < a.win.B) && (t >= t_lo) && (t <= t_end) && (t < L);
+        // ragged launch: a row at or past its utterance's length (in this block's input rows) is stored as zeros, so that the
+        // next block's taps read there what TMA's zero fill gives a launch over the utterance alone
+        const bool live = !(a.lengths && b < a.win.B) ||
+                          t < (min(max(__ldg(a.lengths + b), 0), L >> a.len_shift) << a.len_shift);
         // a row reads input rows of its own utterance only, so one input scale per row; both scales are powers of two
         const float in_s = (a.in_inv && b < a.win.B) ? __ldg(a.in_inv + b) : 1.f;
         const float inv_s = a.inv_scale * in_s;
@@ -348,7 +352,7 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
                     for (int i = 0; i < 16; ++i) {
                         float z = (fmaf(v[i], inv_s, s_bias[c + i]) - mean1) * rstd1 * s_gam[c + i] + s_bet[c + i];
                         if (a.act == 1) z = fmaxf(z, 0.f);
-                        o[i] = (c + i < n1) ? z : 0.f;
+                        o[i] = (c + i < n1 && live) ? z : 0.f;
                     }
                     if (row_ok && a.out.hi) store_planes(a.out, row, col, a.C, o);
                     if (row_ok && a.out_f32) {
@@ -358,7 +362,7 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
                     }
                     if (a.sig_f32 || a.sig.hi) {
 #pragma unroll
-                        for (int i = 0; i < 16; ++i) o[i] = (c + i < n1) ? sigmoid_acc(o[i]) : 0.f;
+                        for (int i = 0; i < 16; ++i) o[i] = (c + i < n1 && live) ? sigmoid_acc(o[i]) : 0.f;
                         if (row_ok && a.sig.hi) store_planes(a.sig, row, col, a.C, o);
                         if (row_ok && a.sig_f32) {
                             float* p = a.sig_f32 + row * a.ld_sig + col;
@@ -400,7 +404,7 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
                         float z2 = (fmaf(v2[i], inv_s, s_bias[half + c + i]) - mean2) * rstd2 * s_gam[half + c + i] + s_bet[half + c + i];
                         float h1 = sigmoid_acc(z1);
                         float x = join_f16(xh[i], xl[i]);
-                        o[i] = h1 * z2 + (1.0f - h1) * x;
+                        o[i] = live ? h1 * z2 + (1.0f - h1) * x : 0.f;
                     }
                     if (a.out_tma) {
                         // stage the output planes in place of the residual just consumed (same swizzled slots)
@@ -445,7 +449,7 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
 #pragma unroll
                         for (int i = 0; i < 16; ++i) {
                             const int ac = hsel * half + c + i;
-                            o[i] = (fmaf(v[i], inv_s, s_bias[ac]) - mean) * rstd * s_gam[ac] + s_bet[ac];
+                            o[i] = live ? (fmaf(v[i], inv_s, s_bias[ac]) - mean) * rstd * s_gam[ac] + s_bet[ac] : 0.f;
                         }
                         if (row_ok && a.out.hi) store_planes(a.out, row_e + hsel, col, a.C, o);
                         if (row_ok && a.out_f32) {
@@ -486,16 +490,20 @@ __global__ void planes_to_f32_kernel(Planes p, float* __restrict__ y, int ldy, l
     long long r = i / C; int c = (int)(i - r * C);
     y[r * ldy + c] = join_f16(p.hi[r * p.ld + c], p.lo[r * p.ld + c]);
 }
-// One CTA per utterance: abs-max of its L x C inputs -> s = utterance_scale(max), then the planes of s x.
+// One CTA per utterance: abs-max of its L x C inputs -> s = utterance_scale(max), then the planes of s x.  With lengths,
+// only the utterance's first lengths[b] rows (clamped to [0, L]) are read; its rows past them become zero planes, which is
+// what the TMA zero fill gives a call over those rows alone.
 constexpr int PLANES_SCALED_THREADS = 512;
 __global__ void __launch_bounds__(PLANES_SCALED_THREADS)
-f32_to_planes_scaled_kernel(const float* __restrict__ x, int ldx, Planes p, int L, int C, float* __restrict__ in_inv) {
+f32_to_planes_scaled_kernel(const float* __restrict__ x, int ldx, Planes p, int L, int C, float* __restrict__ in_inv,
+                            const int* __restrict__ lengths) {
     __shared__ float s_red[PLANES_SCALED_THREADS / 32];
     __shared__ float s_scale;
     const int b = blockIdx.x, n = L * C;
+    const int nlive = lengths ? min(max(__ldg(lengths + b), 0), L) * C : n;
     const float* xb = x + (size_t)b * L * ldx;
     float m = 0.f;
-    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    for (int i = threadIdx.x; i < nlive; i += blockDim.x) {
         const int r = i / C, c = i - r * C;
         m = fmaxf(m, fabsf(xb[(size_t)r * ldx + c]));
     }
@@ -514,16 +522,17 @@ f32_to_planes_scaled_kernel(const float* __restrict__ x, int ldx, Planes p, int 
     const size_t row0 = (size_t)b * L;
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
         const int r = i / C, c = i - r * C;
-        split_f16(xb[(size_t)r * ldx + c] * sc, p.hi[(row0 + r) * p.ld + c], p.lo[(row0 + r) * p.ld + c]);
+        split_f16(i < nlive ? xb[(size_t)r * ldx + c] * sc : 0.f, p.hi[(row0 + r) * p.ld + c], p.lo[(row0 + r) * p.ld + c]);
     }
 }
 void launch_f32_to_planes(const float* x, int ldx, Planes p, long long rows, int C, cudaStream_t s) {
     long long n = rows * C;
     if (n > 0) f32_to_planes_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(x, ldx, p, rows, C);
 }
-void launch_f32_to_planes_scaled(const float* x, int ldx, Planes p, int B, int L, int C, float* in_inv, cudaStream_t s) {
+void launch_f32_to_planes_scaled(const float* x, int ldx, Planes p, int B, int L, int C, float* in_inv, cudaStream_t s,
+                                 const int* lengths) {
     if (B > 0 && (long long)L * C > 0x7fffffffLL) throw std::runtime_error("f32_to_planes_scaled: L x C exceeds 2^31");
-    if (B > 0) f32_to_planes_scaled_kernel<<<(unsigned)B, PLANES_SCALED_THREADS, 0, s>>>(x, ldx, p, L, C, in_inv);
+    if (B > 0) f32_to_planes_scaled_kernel<<<(unsigned)B, PLANES_SCALED_THREADS, 0, s>>>(x, ldx, p, L, C, in_inv, lengths);
 }
 void launch_planes_to_f32(Planes p, float* y, int ldy, long long rows, int C, cudaStream_t s) {
     long long n = rows * C;

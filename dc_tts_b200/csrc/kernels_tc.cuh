@@ -44,7 +44,10 @@ struct TcArgs {
     float* out_f32; int ld_f32;    // fp32 output (may be null)
     float* sig_f32; int ld_sig;    // fp32 sigmoid(output) (mode 0, may be null)
     Planes sig;                    // split planes of sigmoid(output) (mode 0, may be null)
-    int* dbg;                      // optional host-mapped progress markers (debugging), else null
+    // per-utterance lengths (ragged SSRN): utterance b's rows t >= lengths[b] << len_shift (input rows; mode 2 writes both
+    // output rows 2t and 2t+1) are stored as zeros.  Null: every row of the launch is live.
+    const int* lengths; int len_shift;
+    int* dbg;                     // optional host-mapped progress markers (debugging), else null
 };
 
 // Encodes the rank-3 (C, L, B) activation map with a {bk, TT, TB} box; bk = 64 -> 128-byte swizzle, 32 -> 64-byte.
@@ -86,8 +89,10 @@ void launch_attention_tc(const Planes& Q, const Planes& K, const Planes& Vt, con
 
 void launch_f32_to_planes(const float* x, int ldx, Planes p, long long rows, int C, cudaStream_t s);
 // (B, L, C) fp32 -> planes of s_b x with s_b = utterance_scale(max |x_b|) (numerics.cuh); in_inv[b] = 1 / s_b for
-// TcArgs::in_inv.  No host sync.
-void launch_f32_to_planes_scaled(const float* x, int ldx, Planes p, int B, int L, int C, float* in_inv, cudaStream_t s);
+// TcArgs::in_inv.  No host sync.  lengths (device, optional): only utterance b's rows t < lengths[b] are read (the scale is
+// their abs-max), its rows past them become zero planes.
+void launch_f32_to_planes_scaled(const float* x, int ldx, Planes p, int B, int L, int C, float* in_inv, cudaStream_t s,
+                                 const int* lengths = nullptr);
 void launch_planes_to_f32(Planes p, float* y, int ldy, long long rows, int C, cudaStream_t s);
 
 }  // namespace dctts

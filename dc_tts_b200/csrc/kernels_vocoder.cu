@@ -36,6 +36,11 @@ template <int N> struct VcSize {
     static_assert(N == 1024 || N == 2048 || N == 4096, "n_fft must be 1024, 2048 or 4096");
 };
 
+// Frames of utterance b: lengths[b] in a ragged call (clamped to [2, T]; the host checks the range), else T
+__device__ __forceinline__ int voc_frames_of(const int* __restrict__ lengths, int b, int T) {
+    return lengths ? min(max(__ldg(lengths + b), 2), T) : T;
+}
+
 __device__ __forceinline__ float2 cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
 
 // Index into [0, len) of sample u of np.pad(y, p, mode='reflect') at any pad length p (u < 0 lies in the left pad,
@@ -111,9 +116,13 @@ __global__ void voc_twiddle_kernel(float2* tw) {
 
 // utils.py:78-85: amplitude target S = (10 ^ ((clip(z,0,1)*max_db - max_db + ref_db) * 0.05)) ^ power; X <- S (zero phase)
 __global__ void voc_prepare_kernel(const float* __restrict__ mag, float* __restrict__ S, float2* __restrict__ X, long long n,
-                                   float max_db, float ref_db, float power) {
+                                   float max_db, float ref_db, float power, const int* __restrict__ lengths, int T, int F) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    if (lengths) {                                       // rows past the utterance's frames: not read, zero
+        const long long row = i / F;
+        if ((int)(row % T) >= voc_frames_of(lengths, (int)(row / T), T)) { S[i] = 0.f; X[i] = make_float2(0.f, 0.f); return; }
+    }
     float m = fminf(fmaxf(mag[i], 0.f), 1.f) * max_db - max_db + ref_db;
     float v = powf(powf(10.0f, m * 0.05f), power);
     S[i] = v;
@@ -127,11 +136,12 @@ __global__ void voc_prepare_kernel(const float* __restrict__ mag, float* __restr
 template <int N>
 __global__ void __launch_bounds__(VcSize<N>::THREADS, VcSize<N>::ISTFT_MIN_BLOCKS)
 voc_istft_kernel(const float2* __restrict__ X, float* __restrict__ fr, const float2* __restrict__ tw, const float* __restrict__ window,
-                 int T, int F, int win, int lpad) {
+                 int T, int F, int win, int lpad, const int* __restrict__ lengths) {
     constexpr int H = VcSize<N>::H, NT = VcSize<N>::THREADS;
     __shared__ __align__(16) float2 s0[H];
     __shared__ __align__(16) float2 s1[H];
     const int t = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
+    if (t >= voc_frames_of(lengths, b, T)) return;       // whole CTA
     const float2* x = X + ((size_t)b * T + t) * F;
     float2 v[4];
 #pragma unroll
@@ -155,21 +165,36 @@ voc_istft_kernel(const float2* __restrict__ X, float* __restrict__ fr, const flo
     }
 }
 
-// overlap-add + window sum-square normalisation + centre trim: y (B, Ly), Ly = hop*(T-1)
+// overlap-add + window sum-square normalisation + centre trim: y (B, Ly), Ly = hop*(T-1).  Ragged call: utterance b has
+// Tb frames and Ly_b = hop*(Tb-1) samples, the rest of its row is 0.  The table wss (T frames) equals the sum-square of Tb
+// frames below Tb*hop + lpad (the later frames add zeros of the squared window there, which is exact); above it the
+// sum is formed here from wsq, over frames < Tb in ascending order in float32 like voc_make_tables.
 template <int N>
 __global__ void voc_ola_kernel(const float* __restrict__ fr, const float* __restrict__ wss, float* __restrict__ y,
-                               int T, int win, int lpad, int hop, int Ly, float tiny) {
+                               int T, int win, int lpad, int hop, int Ly, float tiny, const int* __restrict__ lengths,
+                               const float* __restrict__ wsq) {
     const int sidx = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
     if (sidx >= Ly) return;
+    const int Tb = voc_frames_of(lengths, b, T);
+    if (sidx >= hop * (Tb - 1)) { y[(size_t)b * Ly + sidx] = 0.f; return; }
     const int u = sidx + N / 2;                          // index in the un-trimmed signal
     // frames t with lpad <= u - hop*t < lpad + win, in ascending order like librosa's loop
     int t_hi = (u - lpad) / hop;
     int t_lo = (u - lpad - win) / hop + 1;
     if (u - lpad - win < 0) t_lo = 0;
-    t_hi = min(t_hi, T - 1);
+    t_hi = min(t_hi, Tb - 1);
     float acc = 0.f;
     for (int t = max(t_lo, 0); t <= t_hi; ++t) acc += fr[((size_t)b * T + t) * win + (u - hop * t - lpad)];
-    const float w = wss[u];
+    float w;
+    if (Tb == T || u < Tb * hop + lpad) {
+        w = wss[u];
+    } else {
+        w = 0.f;
+        for (int t = max(0, (u - N) / hop); t < Tb; ++t) {
+            const int n = u - t * hop;
+            if (n >= 0 && n < N) w += wsq[n];
+        }
+    }
     y[(size_t)b * Ly + sidx] = (w > tiny) ? acc / w : acc;
 }
 
@@ -180,16 +205,18 @@ template <int N>
 __global__ void __launch_bounds__(VcSize<N>::THREADS) voc_stft_phase_kernel(const float* __restrict__ y, const float* __restrict__ S,
                                                                            float2* __restrict__ X, const float2* __restrict__ tw,
                                                                            const float* __restrict__ window, int T, int F, int win,
-                                                                           int lpad, int hop, int Ly) {
+                                                                           int lpad, int hop, int Ly, const int* __restrict__ lengths) {
     constexpr int H = VcSize<N>::H, NT = VcSize<N>::THREADS;
     __shared__ __align__(16) float2 s0[H];
     __shared__ __align__(16) float2 s1[H];
     const int t = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
+    const int Tb = voc_frames_of(lengths, b, T), Lyb = hop * (Tb - 1);
+    if (t >= Tb) return;                                            // whole CTA
     const float* yb = y + (size_t)b * Ly;
     auto sample = [&](int n) -> float {
         const int m = n - lpad;
         if (m < 0 || m >= win) return 0.f;
-        const int u = reflect_index(t * hop + n - N / 2, Ly);      // np.pad(y, n_fft//2, mode='reflect')
+        const int u = reflect_index(t * hop + n - N / 2, Lyb);     // np.pad(y, n_fft//2, mode='reflect')
         return yb[u] * window[m];
     };
     float2 v[4];
@@ -227,31 +254,42 @@ __global__ void __launch_bounds__(VcSize<N>::THREADS) voc_stft_phase_kernel(cons
 // evaluation by float64 rounding only.  (One thread per utterance walking all samples took 5-13 ms.)
 constexpr int DE_LC = 512;
 
-__global__ void voc_deemph_local_kernel(const float* __restrict__ y, double* __restrict__ ends, int Ly, int nch, double c) {
+// Ragged call: utterance b's chunks cover its Ly_b = hop (T_b - 1) samples only.
+__device__ __forceinline__ int voc_samples_of(const int* __restrict__ lengths, int b, int T, int hop) {
+    return hop * (voc_frames_of(lengths, b, T) - 1);
+}
+
+__global__ void voc_deemph_local_kernel(const float* __restrict__ y, double* __restrict__ ends, int Ly, int nch, double c,
+                                        const int* __restrict__ lengths, int T, int hop) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
-    if (j >= nch) return;
+    const int Lyb = lengths ? voc_samples_of(lengths, b, T, hop) : Ly;
+    if (j >= (Lyb + DE_LC - 1) / DE_LC) return;
     const float* p = y + (size_t)b * Ly + (size_t)j * DE_LC;
-    const int n = min(DE_LC, Ly - j * DE_LC);
+    const int n = min(DE_LC, Lyb - j * DE_LC);
     double acc = 0.0;
     for (int i = 0; i < n; ++i) acc = (double)p[i] + c * acc;
     ends[(size_t)b * nch + j] = acc;
 }
 
-__global__ void voc_deemph_carry_kernel(double* __restrict__ ends, int nch, int B, double c) {
+__global__ void voc_deemph_carry_kernel(double* __restrict__ ends, int nch, int B, double c, const int* __restrict__ lengths, int T,
+                                        int hop) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= B) return;
     double cl = 1.0;
     for (int i = 0; i < DE_LC; ++i) cl *= c;
     double* e = ends + (size_t)b * nch;
     double carry = 0.0;
-    for (int j = 0; j < nch; ++j) { const double local = e[j]; e[j] = carry; carry = local + cl * carry; }
+    const int nchb = lengths ? (voc_samples_of(lengths, b, T, hop) + DE_LC - 1) / DE_LC : nch;
+    for (int j = 0; j < nchb; ++j) { const double local = e[j]; e[j] = carry; carry = local + cl * carry; }
 }
 
-__global__ void voc_deemph_apply_kernel(float* __restrict__ y, const double* __restrict__ carry, int Ly, int nch, double c) {
+__global__ void voc_deemph_apply_kernel(float* __restrict__ y, const double* __restrict__ carry, int Ly, int nch, double c,
+                                        const int* __restrict__ lengths, int T, int hop) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
-    if (j >= nch) return;
+    const int Lyb = lengths ? voc_samples_of(lengths, b, T, hop) : Ly;
+    if (j >= (Lyb + DE_LC - 1) / DE_LC) return;
     float* p = y + (size_t)b * Ly + (size_t)j * DE_LC;
-    const int n = min(DE_LC, Ly - j * DE_LC);
+    const int n = min(DE_LC, Lyb - j * DE_LC);
     double acc = carry[(size_t)b * nch + j];
     for (int i = 0; i < n; ++i) { acc = (double)p[i] + c * acc; p[i] = (float)acc; }
 }
@@ -279,10 +317,13 @@ __device__ __forceinline__ float frame_mse(const In* __restrict__ yb, int Ly, in
 }
 
 // frame energies of B equally long signals: mse (B, nfr), grid (nfr, B)
+// (ragged call: utterance b's 1 + Ly_b / fhop frames over its Ly_b samples; the other CTAs of its row leave)
 __global__ void __launch_bounds__(256) voc_frame_mse_kernel(const float* __restrict__ y, float* __restrict__ mse, int Ly, int nfr,
-                                                           int flen, int fhop) {
+                                                           int flen, int fhop, const int* __restrict__ lengths, int T, int hop) {
     __shared__ float red[8];
-    const float m = frame_mse(y + (size_t)blockIdx.y * Ly, Ly, blockIdx.x, flen, fhop, red);
+    const int Lyb = lengths ? voc_samples_of(lengths, blockIdx.y, T, hop) : Ly;
+    if ((int)blockIdx.x >= 1 + Lyb / fhop) return;                  // whole CTA
+    const float m = frame_mse(y + (size_t)blockIdx.y * Ly, Lyb, blockIdx.x, flen, fhop, red);
     if (threadIdx.x == 0) mse[(size_t)blockIdx.y * nfr + blockIdx.x] = m;
 }
 
@@ -394,7 +435,8 @@ static void voc_dispatch(int n_fft, Fn&& f) {
     }
 }
 
-void voc_make_tables(int n_fft, float2* tw_dev, float* window_dev, float* wss_dev, int T, int win, int hop, cudaStream_t s) {
+void voc_make_tables(int n_fft, float2* tw_dev, float* window_dev, float* wss_dev, int T, int win, int hop, cudaStream_t s,
+                     float* wsq_dev) {
     voc_dispatch(n_fft, [&](auto n) { voc_twiddle_kernel<decltype(n)::value><<<(n_fft + 255) / 256, 256, 0, s>>>(tw_dev); });
     // periodic Hann of win taps (scipy get_window('hann', win, fftbins=True)) and librosa's window_sumsquare,
     // accumulated in float32 in frame order like the reference
@@ -409,6 +451,7 @@ void voc_make_tables(int n_fft, float2* tw_dev, float* window_dev, float* wss_de
         for (int n = 0; n < n_fft && t * hop + n < n_tot; ++n) wss[t * hop + n] += wsq[n];
     cudaMemcpyAsync(window_dev, w.data(), win * sizeof(float), cudaMemcpyHostToDevice, s);
     cudaMemcpyAsync(wss_dev, wss.data(), n_tot * sizeof(float), cudaMemcpyHostToDevice, s);
+    if (wsq_dev) cudaMemcpyAsync(wsq_dev, wsq.data(), n_fft * sizeof(float), cudaMemcpyHostToDevice, s);
     cudaStreamSynchronize(s);
 }
 
@@ -607,16 +650,18 @@ size_t voc_deemph_scratch_bytes(int B, int T, int hop) { return (size_t)B * ((ho
 // The stages of voc_run, each a fixed sequence of launches (dctts_vocoder_stage runs them one at a time).
 void voc_prepare(const VocoderArgs& a, cudaStream_t s) {
     const long long n = (long long)a.B * a.T * a.F;
-    voc_prepare_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a.mag, a.S, a.X, n, a.max_db, a.ref_db, a.power);
+    voc_prepare_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a.mag, a.S, a.X, n, a.max_db, a.ref_db, a.power, a.lengths,
+                                                                   a.T, a.F);
 }
 
 void voc_istft(const VocoderArgs& a, cudaStream_t s) {
     voc_dispatch(2 * (a.F - 1), [&](auto n) {
         constexpr int N = decltype(n)::value;
         const int Ly = a.hop * (a.T - 1), lpad = (N - a.win) / 2;
-        voc_istft_kernel<N><<<dim3(a.T, a.B), VcSize<N>::THREADS, 0, s>>>(a.X, a.frames, a.tw, a.window, a.T, a.F, a.win, lpad);
+        voc_istft_kernel<N><<<dim3(a.T, a.B), VcSize<N>::THREADS, 0, s>>>(a.X, a.frames, a.tw, a.window, a.T, a.F, a.win, lpad,
+                                                                              a.lengths);
         voc_ola_kernel<N><<<dim3((Ly + 255) / 256, a.B), 256, 0, s>>>(a.frames, a.wss, a.wav, a.T, a.win, lpad, a.hop, Ly,
-                                                                     1.17549435e-38f);
+                                                                     1.17549435e-38f, a.lengths, a.wsq);
     });
 }
 
@@ -625,21 +670,21 @@ void voc_stft_phase(const VocoderArgs& a, cudaStream_t s) {
         constexpr int N = decltype(n)::value;
         const int Ly = a.hop * (a.T - 1), lpad = (N - a.win) / 2;
         voc_stft_phase_kernel<N><<<dim3(a.T, a.B), VcSize<N>::THREADS, 0, s>>>(a.wav, a.S, a.X, a.tw, a.window, a.T, a.F, a.win,
-                                                                              lpad, a.hop, Ly);
+                                                                              lpad, a.hop, Ly, a.lengths);
     });
 }
 
 void voc_deemph(const VocoderArgs& a, cudaStream_t s) {
     const int Ly = a.hop * (a.T - 1), nch = (Ly + DE_LC - 1) / DE_LC;
     const dim3 gch((nch + 63) / 64, a.B);
-    voc_deemph_local_kernel<<<gch, 64, 0, s>>>(a.wav, a.deemph, Ly, nch, a.preemphasis);
-    voc_deemph_carry_kernel<<<(a.B + 31) / 32, 32, 0, s>>>(a.deemph, nch, a.B, a.preemphasis);
-    voc_deemph_apply_kernel<<<gch, 64, 0, s>>>(a.wav, a.deemph, Ly, nch, a.preemphasis);
+    voc_deemph_local_kernel<<<gch, 64, 0, s>>>(a.wav, a.deemph, Ly, nch, a.preemphasis, a.lengths, a.T, a.hop);
+    voc_deemph_carry_kernel<<<(a.B + 31) / 32, 32, 0, s>>>(a.deemph, nch, a.B, a.preemphasis, a.lengths, a.T, a.hop);
+    voc_deemph_apply_kernel<<<gch, 64, 0, s>>>(a.wav, a.deemph, Ly, nch, a.preemphasis, a.lengths, a.T, a.hop);
 }
 
 void voc_energies(const VocoderArgs& a, cudaStream_t s) {
     const int Ly = a.hop * (a.T - 1), nfr = 1 + Ly / 512;
-    voc_frame_mse_kernel<<<dim3(nfr, a.B), 256, 0, s>>>(a.wav, a.mse, Ly, nfr, 2048, 512);
+    voc_frame_mse_kernel<<<dim3(nfr, a.B), 256, 0, s>>>(a.wav, a.mse, Ly, nfr, 2048, 512, a.lengths, a.T, a.hop);
 }
 
 void voc_run(const VocoderArgs& a, cudaStream_t s) {

@@ -240,17 +240,33 @@ class Engine:
         self._check(self._lib.dctts_audiodec(self._h, _ptr(R), B, T, _ptr(logits), _ptr(Y), self._stream()), "dctts_audiodec")
         return logits, Y
 
-    def ssrn(self, Y, want_logits=True, out=None):
-        """`out`: optional preallocated contiguous (B, 4T, F) float32 CUDA tensor (e.g. a slice of a gather buffer)."""
+    def ssrn(self, Y, want_logits=True, out=None, lengths=None):
+        """`out`: optional preallocated contiguous (B, 4T, F) float32 CUDA tensor (e.g. a slice of a gather buffer).
+        `lengths`: optional (B,) mel frames per utterance, 1 <= lengths[b] <= T (include/dctts.h: dctts_ssrn_ragged):
+        rows < 4 lengths[b] of Z and the logits are what this call gives for Y[b:b+1, :lengths[b]] alone, bit for bit, rows
+        past them are 0, and Y rows >= lengths[b] are never read.  The range is checked on the host (one small copy)."""
         Y = self._f32(Y)
         B, T, _ = Y.shape
         if out is not None:
             if tuple(out.shape) != (B, T * self.hp.r, self.F) or out.dtype != torch.float32 or not out.is_contiguous() \
                     or out.device != self.device:
                 raise DcttsError("ssrn: `out` must be a contiguous float32 (B, 4T, F) tensor on this engine's device")
+        n = None
+        if lengths is not None:
+            n = self._i32(lengths).reshape(-1)
+            nh = n.cpu().numpy()
+            if nh.shape[0] != B:
+                raise DcttsError("ssrn: %d lengths for %d utterances" % (nh.shape[0], B))
+            bad = np.flatnonzero((nh < 1) | (nh > T))
+            if bad.size:
+                raise DcttsError("ssrn: utterance %d has length %d outside [1, %d]" % (bad[0], nh[bad[0]], T))
         Z = out if out is not None else self._empty(B, T * self.hp.r, self.F)
         logits = self._empty(B, T * self.hp.r, self.F) if want_logits else None
-        self._check(self._lib.dctts_ssrn(self._h, _ptr(Y), B, T, _ptr(logits), _ptr(Z), self._stream()), "dctts_ssrn")
+        if n is None:
+            self._check(self._lib.dctts_ssrn(self._h, _ptr(Y), B, T, _ptr(logits), _ptr(Z), self._stream()), "dctts_ssrn")
+        else:
+            self._check(self._lib.dctts_ssrn_ragged(self._h, _ptr(Y), B, T, _ptr(n), _ptr(logits), _ptr(Z), self._stream()),
+                        "dctts_ssrn_ragged")
         return logits, Z
 
     # ------------------------------------------------------------------ graph level
@@ -317,9 +333,12 @@ class Engine:
                                                        float(h.ref_db), float(h.preemphasis), int(h.n_iter)),
                     "dctts_set_vocoder_params")
 
-    def spectrogram2wav(self, mag, n_iter=-1):
+    def spectrogram2wav(self, mag, n_iter=-1, lengths=None):
         """utils.py:67-94 for a batch: mag (B, T, F) in [0,1] -> (untrimmed wav (B, hop*(T-1)) CUDA tensor,
-        trim (B, 2) int32 numpy [start, end) as librosa.effects.trim would keep)."""
+        trim (B, 2) int32 numpy [start, end) as librosa.effects.trim would keep).
+        `lengths`: optional (B,) magnitude frames per utterance, 2 <= lengths[b] <= T (include/dctts.h:
+        dctts_spectrogram2wav_ragged): wav[b, :hop*(lengths[b]-1)] and trim[b] are what this call gives for
+        mag[b:b+1, :lengths[b]] alone, bit for bit, the rest of wav[b] is 0, and mag rows past lengths[b] are never read."""
         mag = self._f32(mag)
         if mag.dim() == 2:
             mag = mag[None]
@@ -328,8 +347,17 @@ class Engine:
         self._set_vocoder_params()
         wav = self._empty(B, h.hop_length * (T - 1))
         trim = np.zeros((B, 2), np.int32)
-        self._check(self._lib.dctts_spectrogram2wav(self._h, _ptr(mag), B, T, int(n_iter), _ptr(wav),
-                                                    trim.ctypes.data_as(C.c_void_p), self._stream()), "dctts_spectrogram2wav")
+        if lengths is None:
+            self._check(self._lib.dctts_spectrogram2wav(self._h, _ptr(mag), B, T, int(n_iter), _ptr(wav),
+                                                        trim.ctypes.data_as(C.c_void_p), self._stream()), "dctts_spectrogram2wav")
+            return wav, trim
+        n = np.ascontiguousarray(np.asarray(lengths.cpu() if isinstance(lengths, torch.Tensor) else lengths).reshape(-1),
+                                 dtype=np.int32)
+        if n.shape[0] != B:
+            raise DcttsError("spectrogram2wav: %d lengths for %d utterances" % (n.shape[0], B))
+        self._check(self._lib.dctts_spectrogram2wav_ragged(self._h, _ptr(mag), B, T, n.ctypes.data_as(C.c_void_p), int(n_iter),
+                                                           _ptr(wav), trim.ctypes.data_as(C.c_void_p), self._stream()),
+                    "dctts_spectrogram2wav_ragged")
         return wav, trim
 
     def vocoder_stage(self, stage, x, out, S=None, hop=None, win=None, power=None):

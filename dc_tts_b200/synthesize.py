@@ -20,11 +20,17 @@ from .params import init_params
 from .train import Graph, Session
 
 
-def synthesize(params=None, sentences=None, fast=True, write=True, seed=0, vocoder=True, allow_random_init=False):
+def synthesize(params=None, sentences=None, fast=True, write=True, seed=0, vocoder=True, allow_random_init=False,
+               until_eos=False, tail=0):
     """`params`: a name -> array dict to use instead of the checkpoints.  Without it the latest checkpoints of
     hp.logdir-1 (Text2Mel) and hp.logdir-2 (SSRN) are restored, and a missing one RAISES like the reference's
     `saver.restore(sess, None)` does (synthesize.py:33,39) -- seeded random weights are used only when the caller asks
-    for them (`allow_random_init=True`, benchmarks and smoke tests) or has already loaded parameters into the engine."""
+    for them (`allow_random_init=True`, benchmarks and smoke tests) or has already loaded parameters into the engine.
+
+    `until_eos=True`: each utterance ends `tail` frames after its attention reaches the EOS of its text
+    (Graph.generate_until_eos).  SSRN and the vocoder then run once each over the batch at its longest length, with a
+    length per utterance: each wav is Griffin-Lim of that utterance's r * length magnitude frames.  Y and Z rows past each
+    length are 0."""
     # Load data
     L = load_data("synthesize", sentences)
 
@@ -53,7 +59,16 @@ def synthesize(params=None, sentences=None, fast=True, write=True, seed=0, vocod
                 raise FileNotFoundError("no checkpoint under %s (reference: Saver.restore(sess, None) fails); pass params=..., "
                                         "or allow_random_init=True for seeded random weights" % " and ".join(missing))
 
-        if fast:
+        lengths = None
+        if until_eos:
+            Y, _, n = g.generate_until_eos(L, tail=tail)
+            lengths = n.cpu().numpy()
+            Tmax = int(lengths.max())
+            # SSRN at the batch's longest length; rows past each utterance's length come back as 0
+            _, Zd = g.engine.ssrn(Y[:, :Tmax], want_logits=False, lengths=n)
+            Z = np.zeros((len(L), hp.r * hp.max_T, Zd.shape[2]), np.float32)
+            Z[:, :hp.r * Tmax] = Zd.cpu().numpy()
+        elif fast:
             # the whole loop on the device (CUDA-graph replay), identical results
             Y, _ = g.generate(L)
         else:
@@ -67,8 +82,9 @@ def synthesize(params=None, sentences=None, fast=True, write=True, seed=0, vocod
                 Y[:, j, :] = _Y[:, j, :]
                 prev_max_attentions = _max_attentions[:, j]
 
-        # Get magnitude (synthesize.py:57)
-        Z = sess.run(g.Z, {g.Y: Y})
+        if lengths is None:
+            # Get magnitude (synthesize.py:57)
+            Z = sess.run(g.Z, {g.Y: Y})
 
     # Generate wav files (synthesize.py:60-64): Griffin-Lim on the GPU for the whole batch
     if write:
@@ -77,11 +93,18 @@ def synthesize(params=None, sentences=None, fast=True, write=True, seed=0, vocod
         if vocoder:
             from scipy.io.wavfile import write as write_wav
             from .utils import spectrograms2wavs
-            for i, wav in enumerate(spectrograms2wavs(Z)):
+            if lengths is None:
+                wavs = spectrograms2wavs(Z)
+            else:
+                # one call at the batch's longest length, each utterance on its own magnitude frames
+                wavs = spectrograms2wavs(Z[:, :hp.r * int(lengths.max())], lengths=hp.r * lengths)
+            for i, wav in enumerate(wavs):
                 print("Working on file", i + 1)
                 write_wav(os.path.join(hp.sampledir, "{}.wav".format(i + 1)), hp.sr, wav)
         else:
             for i, mag in enumerate(Z):
+                if lengths is not None:
+                    mag = mag[:hp.r * int(lengths[i])]
                 np.save(os.path.join(hp.sampledir, "{}.mag.npy".format(i + 1)), mag)
     return (Y.cpu().numpy() if hasattr(Y, "cpu") else Y), Z
 

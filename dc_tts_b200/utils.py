@@ -28,9 +28,10 @@ def spectrogram2wav(mag):
     return wav[0, s:e].cpu().numpy().astype(np.float32)
 
 
-def spectrograms2wavs(mags):
-    """Batched form: (B, T, F) -> list of trimmed wavs (one device pass for the whole batch)."""
-    wav, trim = get_engine().spectrogram2wav(mags)
+def spectrograms2wavs(mags, lengths=None):
+    """Batched form: (B, T, F) -> list of trimmed wavs (one device pass for the whole batch).  `lengths`: optional (B,)
+    magnitude frames per utterance; wav b is then spectrogram2wav(mags[b, :lengths[b]]), bit for bit."""
+    wav, trim = get_engine().spectrogram2wav(mags, lengths=lengths)
     wav = wav.cpu().numpy()
     return [wav[b, int(trim[b, 0]):int(trim[b, 1])].astype(np.float32) for b in range(wav.shape[0])]
 

@@ -100,6 +100,15 @@ int dctts_audiodec(dctts_handle h, const float* R, int32_t B, int32_t T,
 /* SSRN (networks.py:214-292): Y (B,T,n_mels) -> Z_logits, Z (B,4T,F). Z_logits may be NULL. */
 int dctts_ssrn(dctts_handle h, const float* Y, int32_t B, int32_t T,
                float* Z_logits, float* Z, void* stream);
+/* SSRN with a length per utterance.  lengths: (B) int32 DEVICE mel frames, 1 <= lengths[b] <= T (as
+ * dctts_text2mel_generate_until writes them).  For each b, Z[b, :4 lengths[b]] and Z_logits[b, :4 lengths[b]] are
+ * dctts_ssrn of Y[b:b+1, :lengths[b]] alone on the same kernel set, bit for bit; their rows past that are 0 (Z too).
+ * Rows >= lengths[b] of Y are never read.  On the wgmma path (dctts_set_tensor_path 1) it is one launch per block over
+ * the batch and no host sync; a length outside the range is clamped to [0, T] and no row outside the utterance's
+ * [0, T) / [0, 4T) is touched.  On the fp32 path the lengths are copied to the host (a sync), a length outside the range
+ * fails the call, and the chain runs once per utterance: that path's GEMM schedule depends on a launch's row count. */
+int dctts_ssrn_ragged(dctts_handle h, const float* Y, int32_t B, int32_t T, const int32_t* lengths,
+                      float* Z_logits, float* Z, void* stream);
 
 /* ---- graph-level (reference train.py Graph, synthesize.py loop) ------------------ */
 /* One sess.run of the synthesize graph (train.py:48-68 fetched at synthesize.py:48-52):
@@ -150,6 +159,12 @@ int dctts_set_vocoder_params(dctts_handle h, int32_t hop_length, int32_t win_len
  * Synchronises `stream` before returning (trim_host is written by the host). */
 int dctts_spectrogram2wav(dctts_handle h, const float* mag, int32_t B, int32_t T, int32_t n_iter, float* wav,
                           int32_t* trim_host, void* stream);
+/* dctts_spectrogram2wav with a frame count per utterance, in one call at T.  lengths_host: (B) HOST int32 magnitude
+ * frames, 2 <= lengths_host[b] <= T; a count outside that range fails the call, naming the utterance, before any
+ * launch.  For each b, wav[b, :hop (T_b - 1)] and trim_host[b] are those of dctts_spectrogram2wav on mag[b:b+1, :T_b]
+ * alone, bit for bit; wav[b] past that is 0.  Mag rows >= T_b are never read.  Synchronises `stream`. */
+int dctts_spectrogram2wav_ragged(dctts_handle h, const float* mag, int32_t B, int32_t T, const int32_t* lengths_host,
+                                 int32_t n_iter, float* wav, int32_t* trim_host, void* stream);
 
 /* Feature extraction (next row, SURVEY 8f-4): get_spectrograms -- utils.py:20-65 -- for ONE utterance from the
  * loaded waveform on: trim (librosa.effects.trim), pre-emphasis, STFT, |.|, mel filterbank

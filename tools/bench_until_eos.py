@@ -1,5 +1,9 @@
 """Time generation with each utterance ending at its text (Engine.text2mel_generate_until) against the full-length
 generation, B = 32, the two alternated in one run, CUDA events, and report the frames the decode clusters executed.
+Then the stages after it with the same lengths, each variant alternated with the others:
+  SSRN      full at max_T frames | one ragged call at the batch's longest length | one call per utterance
+  vocoder   one call over the batch at r max_T frames | one ragged call at r x the longest | one call per utterance
+  chain     generate + SSRN + vocoder at full length | generate_until + ragged SSRN + ragged vocoder
 
 SYNTHETIC LENGTHS: no trained model is available, and the seeded weights move the attention window on only ~15 % of
 frames, so the EOS id is rarely reached.  The script instead sets each utterance's stop position from a full run's
@@ -77,3 +81,53 @@ frames_full = e.get_option("decode_last_frames")
 for k, v in res.items():
     print("%-16s %s ms (median %.2f)" % (k, " ".join("%.2f" % x for x in v), float(np.median(v))), flush=True)
 print("frames executed, summed over clusters: full %d, until %d" % (frames_full, frames_until), flush=True)
+
+
+# ---- the stages after generation, with the same lengths ----
+Y, _, n_dev = e.text2mel_generate_until(L, stop_pos=sp)
+n_host = n_dev.cpu().numpy()
+Yf = e.text2mel_generate(L)[0]
+Zf = e.ssrn(Yf, want_logits=False)[1]
+Zr = e.ssrn(Y[:, :T_eff], want_logits=False, lengths=n_dev)[1]
+
+
+def ssrn_each():
+    for b, k in enumerate(n_host):
+        e.ssrn(Y[b:b + 1, :k], want_logits=False)
+
+
+def vocoder_each(Z):
+    for b, k in enumerate(n_host):
+        e.spectrogram2wav(Z[b:b + 1, :hp.r * k])
+
+
+def chain_full():
+    Yc = e.text2mel_generate(L)[0]
+    e.spectrogram2wav(e.ssrn(Yc, want_logits=False)[1])
+
+
+def chain_until():
+    Yc, _, nc = e.text2mel_generate_until(L, stop_pos=sp)
+    Zc = e.ssrn(Yc[:, :T_eff], want_logits=False, lengths=nc)[1]
+    e.spectrogram2wav(Zc, lengths=hp.r * nc.cpu().numpy())
+
+
+stages = {
+    "ssrn full %d" % hp.max_T: lambda: e.ssrn(Yf, want_logits=False),
+    "ssrn ragged %d" % T_eff: lambda: e.ssrn(Y[:, :T_eff], want_logits=False, lengths=n_dev),
+    "ssrn per utt": ssrn_each,
+    "vocoder full %d" % (hp.r * hp.max_T): lambda: e.spectrogram2wav(Zf),
+    "vocoder ragged %d" % (hp.r * T_eff): lambda: e.spectrogram2wav(Zr, lengths=hp.r * n_host),
+    "vocoder per utt": lambda: vocoder_each(Zr),
+    "chain full": chain_full,
+    "chain until": chain_until,
+}
+for fn in stages.values():
+    fn()
+torch.cuda.synchronize()
+res = {k: [] for k in stages}
+for rep in range(a.reps):
+    for k, fn in stages.items():
+        res[k].append(timed(fn))
+for k, v in res.items():
+    print("%-20s %s ms (median %.2f)" % (k, " ".join("%.2f" % x for x in v), float(np.median(v))), flush=True)
