@@ -50,6 +50,8 @@ SIGNATURES = {
     "dctts_set_vocoder_params": (C.c_int, [Handle, _i32, _i32, C.c_float, C.c_float, C.c_float, C.c_double, _i32]),
     "dctts_spectrogram2wav": (C.c_int, [Handle, _p, _i32, _i32, _i32, _p, _p, _p]),
     "dctts_spectrogram2wav_ragged": (C.c_int, [Handle, _p, _i32, _i32, _p, _i32, _p, _p, _p]),
+    "dctts_spectrogram2wav_momentum": (C.c_int, [Handle, _p, _i32, _i32, _p, _i32, C.c_double, _p, _p, _p, _p]),
+    "dctts_vocoder_momentum_step": (C.c_int, [Handle, _i32, _i32, _p, _p, _p, _p, C.c_double, _p, _p]),
     "dctts_get_spectrograms": (C.c_int, [Handle, _p, _i64, _i32, _p, _p, _i32, C.POINTER(_i32), C.POINTER(_i32), _p]),
     "dctts_load_spectrograms_batch": (C.c_int, [Handle, _p, _i32, C.POINTER(_i64), _i32, _i32, _p, _p, _i32, C.POINTER(_i32),
                                                 C.POINTER(_i32), C.POINTER(_i32), _p]),

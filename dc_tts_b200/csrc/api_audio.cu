@@ -159,6 +159,22 @@ void voc_trims(const VocoderArgs& a, int32_t* trim_host, cudaStream_t s, const i
         }
 }
 
+// A ragged call's frame counts: 2 <= lengths_host[b] <= T, else the call fails naming the utterance, before any launch
+void require_frame_counts(const std::string& fn, const int32_t* lengths_host, int B, int T) {
+    for (int b = 0; b < B; ++b)
+        REQUIRE(lengths_host[b] >= 2 && lengths_host[b] <= T, fn + ": utterance " + std::to_string(b) + " has " +
+                                                              std::to_string(lengths_host[b]) + " frames (need 2 to T = " +
+                                                              std::to_string(T) + ")");
+}
+
+// The fast Griffin-Lim weight alpha = momentum / (1 + momentum), formed in float64 and rounded to float32 as numpy does
+// when it multiplies a complex64 array by a Python float
+float momentum_alpha(const std::string& fn, double momentum) {
+    REQUIRE(std::isfinite(momentum) && momentum >= 0.0,
+            fn + ": momentum must be finite and >= 0, got " + std::to_string(momentum));
+    return (float)(momentum / (1.0 + momentum));
+}
+
 }  // namespace
 
 extern "C" {
@@ -194,10 +210,7 @@ int dctts_spectrogram2wav_ragged(dctts_handle h, const float* mag, int32_t B, in
     return guarded(h, [&] {
         const std::string fn = "dctts_spectrogram2wav_ragged";
         REQUIRE(mag && wav && lengths_host, fn + ": bad arguments");
-        for (int b = 0; b < B; ++b)
-            REQUIRE(lengths_host[b] >= 2 && lengths_host[b] <= T, fn + ": utterance " + std::to_string(b) + " has " +
-                                                                  std::to_string(lengths_host[b]) + " frames (need 2 to T = " +
-                                                                  std::to_string(T) + ")");
+        require_frame_counts(fn, lengths_host, B, T);
         cudaStream_t s = S(h, stream);
         VocoderArgs a = voc_args(h, fn.c_str(), B, T, s);
         h->voc_len.ensure((size_t)B * sizeof(int));
@@ -208,6 +221,57 @@ int dctts_spectrogram2wav_ragged(dctts_handle h, const float* mag, int32_t B, in
         h->launches += voc_launches_per_call(a.n_iter);
         CUDA_CHECK(cudaGetLastError());
         voc_trims(a, trim_host, s, lengths_host);
+    });
+}
+
+int dctts_spectrogram2wav_momentum(dctts_handle h, const float* mag, int32_t B, int32_t T, const int32_t* lengths_host,
+                                   int32_t n_iter, double momentum, float* wav, int32_t* trim_host, double* convergence,
+                                   void* stream) {
+    return guarded(h, [&] {
+        const std::string fn = "dctts_spectrogram2wav_momentum";
+        REQUIRE(mag && wav, fn + ": bad arguments");
+        const float alpha = momentum_alpha(fn, momentum);
+        if (lengths_host) require_frame_counts(fn, lengths_host, B, T);
+        cudaStream_t s = S(h, stream);
+        VocoderArgs a = voc_args(h, fn.c_str(), B, T, s);
+        a.mag = mag; a.wav = wav;
+        if (n_iter >= 0) a.n_iter = n_iter;
+        if (lengths_host) {
+            h->voc_len.ensure((size_t)B * sizeof(int));
+            CUDA_CHECK(cudaMemcpyAsync(h->voc_len.p, lengths_host, (size_t)B * sizeof(int), cudaMemcpyHostToDevice, s));
+            a.lengths = h->voc_len.as<int>();
+        }
+        if (alpha != 0.f) {                 // est_{-1} = 0; a momentum that rounds to alpha = 0 is the plain update
+            const size_t n = (size_t)B * T * a.F * sizeof(float2);
+            h->voc_E.ensure(n);
+            CUDA_CHECK(cudaMemsetAsync(h->voc_E.p, 0, n, s));
+            a.E = h->voc_E.as<float2>(); a.alpha = alpha;
+        }
+        if (convergence) {
+            h->voc_part.ensure((size_t)(a.n_iter + 1) * B * T * sizeof(float));
+            a.part = h->voc_part.as<float>(); a.conv = convergence;
+        }
+        voc_run(a, s);
+        h->launches += voc_launches_per_call(a.n_iter, convergence != nullptr);
+        CUDA_CHECK(cudaGetLastError());
+        voc_trims(a, trim_host, s, lengths_host);
+    });
+}
+
+int dctts_vocoder_momentum_step(dctts_handle h, int32_t B, int32_t T, const float* wav, const float* S_in, void* E, void* X,
+                                double momentum, float* partials, void* stream) {
+    return guarded(h, [&] {
+        const std::string fn = "dctts_vocoder_momentum_step";
+        REQUIRE(wav && S_in && E && X, fn + ": wav, S, E and X are required");
+        const float alpha = momentum_alpha(fn, momentum);
+        cudaStream_t s = S(h, stream);
+        VocoderArgs a = voc_args(h, fn.c_str(), B, T, s);
+        a.wav = const_cast<float*>(wav); a.S = const_cast<float*>(S_in); a.X = static_cast<float2*>(X);
+        a.E = static_cast<float2*>(E); a.alpha = alpha; a.part = partials;
+        voc_stft_phase(a, s);
+        h->launches += 1;
+        CUDA_CHECK(cudaGetLastError());
+        CUDA_CHECK(cudaStreamSynchronize(s));
     });
 }
 

@@ -162,6 +162,7 @@ struct dctts_handle_s {
     int feat_sr = 0, feat_win = 0;
     DevBuf voc_S, voc_X, voc_frames, voc_mse, voc_tw, voc_window, voc_wss, voc_deemph;
     DevBuf voc_wsq, voc_len;                      // squared window row (n_fft), per-utterance frame counts (ragged call)
+    DevBuf voc_E, voc_part;                       // fast Griffin-Lim: previous raw estimate (B, T, F), convergence partials
     int voc_tables_T = 0, voc_tables_win = 0, voc_tables_hop = 0;
     // co-resident 16-CTA clusters of the 144-column block kernel (the F = 2049 conv1d blocks), -1 until first needed;
     // when none fits, why those blocks run on the fp32 kernels

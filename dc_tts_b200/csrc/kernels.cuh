@@ -130,6 +130,14 @@ struct VocoderArgs {
     const float* wsq;              // (n_fft) squared window centred in the frame: window sum-square past wss's valid range
     float max_db, ref_db, power;
     double preemphasis;            // float64 like the reference's scipy.signal.lfilter([1], [1, -hp.preemphasis], wav)
+    // fast Griffin-Lim: E (B, T, F) the previous iteration's raw STFT estimate (zero before the first), updated in place;
+    // alpha = momentum / (1 + momentum) rounded to float32.  Null E: the plain update.
+    float2* E;
+    float alpha;
+    // spectral convergence: part (n_iter + 1, B, T) per-frame sums of (S - |est|)^2, conv (B, n_iter + 1) DEVICE float64.
+    // Null part: no convergence, and no extra STFT of the final waveform.
+    float* part;
+    double* conv;
 };
 // n_fft 1024, 2048 and 4096 have kernel instantiations (F = 1 + n_fft / 2 = 513, 1025, 2049); the launchers take n_fft
 // from F and throw for any other size
@@ -138,14 +146,17 @@ bool voc_fft_size_ok(int n_fft);
 // (n_fft + hop (T - 1) entries) and, when wsq_dev is given, the squared window it sums (n_fft entries)
 void voc_make_tables(int n_fft, float2* tw_dev, float* window_dev, float* wss_dev, int T, int win, int hop, cudaStream_t s,
                      float* wsq_dev = nullptr);
-// voc_run = voc_prepare, (voc_istft, voc_stft_phase) x n_iter, voc_istft, voc_deemph, voc_energies
+// voc_run = voc_prepare, (voc_istft, voc_stft_phase) x n_iter, voc_istft, [voc_stft_phase, voc_convergence when part is
+// set], voc_deemph, voc_energies
 void voc_prepare(const VocoderArgs& a, cudaStream_t s);      // mag -> S, X = S (zero phase); 1 launch
 void voc_istft(const VocoderArgs& a, cudaStream_t s);        // X -> frames -> wav; 2 launches
-void voc_stft_phase(const VocoderArgs& a, cudaStream_t s);   // wav, S -> X; 1 launch
+// wav, S (, E) -> X (, E); with part, iteration it's per-frame partials to part + it B T; 1 launch
+void voc_stft_phase(const VocoderArgs& a, cudaStream_t s, int it = 0);
+void voc_convergence(const VocoderArgs& a, cudaStream_t s);  // S, part -> conv; 1 launch
 void voc_deemph(const VocoderArgs& a, cudaStream_t s);       // wav in place, deemph scratch; 3 launches
 void voc_energies(const VocoderArgs& a, cudaStream_t s);     // wav -> mse; 1 launch
 void voc_run(const VocoderArgs& a, cudaStream_t s);
-int voc_launches_per_call(int n_iter);
+int voc_launches_per_call(int n_iter, bool convergence = false);
 size_t voc_deemph_scratch_bytes(int B, int T, int hop);
 // feature extraction (reference utils.py:20-65,147-162) for a ragged batch of utterances packed back to back
 struct FeatSeg {

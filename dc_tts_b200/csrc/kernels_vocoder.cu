@@ -10,10 +10,12 @@
 // (B, T, 1 + n_fft/2) complex spectrum, the windowed frames and the waveform touch HBM:
 //   voc_istft_kernel   spectrum row -> Hermitian extension -> IFFT -> x window -> frame buffer
 //   voc_ola_kernel     overlap-add of the <= 5 frames covering a sample, / window sum-square
-//   voc_stft_phase_kernel  reflect-padded frame x window -> FFT -> X = S * est / max(1e-8, |est|)
+//   voc_stft_phase_kernel  reflect-padded frame x window -> FFT -> X = S * est / max(1e-8, |est|) (or the fast
+//                          Griffin-Lim update, and the frame's spectral-convergence partial)
 // plus de-normalisation (power law), the de-pre-emphasis IIR (float64 like scipy.signal.lfilter)
 // and the frame energies librosa.effects.trim thresholds.
 #include "kernels.cuh"
+#include "numerics.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -201,11 +203,16 @@ __global__ void voc_ola_kernel(const float* __restrict__ fr, const float* __rest
 // librosa.core.stft of the current estimate, one frame, fused with the Griffin-Lim phase update
 // (utils.py:101-104): X = S * est / max(1e-8, |est|).  grid (T, B).  Real input packed as
 // z[n] = x[2n] + i x[2n+1]; est[k] = (Z[k] + conj Z[N/2-k]) / 2 - i W^k (Z[k] - conj Z[N/2-k]) / 2.
-template <int N>
+// MOM (fast Griffin-Lim): E (B, T, F) holds the previous iteration's raw estimate; the thread of bin k reads E[k], writes
+// est[k] over it and updates with c = est - alpha E[k] (a float32 product, then a float32 difference, as numpy forms it for
+// complex64): X = S * c / max(1e-8, |c|).  CONV: the frame's sum_k (S - |est|)^2 goes to part[b * T + t], summed in a fixed
+// order (each thread's bins in ascending order, a warp butterfly, then the warp sums in ascending order; no atomics).
+template <int N, bool MOM, bool CONV>
 __global__ void __launch_bounds__(VcSize<N>::THREADS) voc_stft_phase_kernel(const float* __restrict__ y, const float* __restrict__ S,
                                                                            float2* __restrict__ X, const float2* __restrict__ tw,
                                                                            const float* __restrict__ window, int T, int F, int win,
-                                                                           int lpad, int hop, int Ly, const int* __restrict__ lengths) {
+                                                                           int lpad, int hop, int Ly, const int* __restrict__ lengths,
+                                                                           float2* __restrict__ E, float alpha, float* __restrict__ part) {
     constexpr int H = VcSize<N>::H, NT = VcSize<N>::THREADS;
     __shared__ __align__(16) float2 s0[H];
     __shared__ __align__(16) float2 s1[H];
@@ -222,16 +229,46 @@ __global__ void __launch_bounds__(VcSize<N>::THREADS) voc_stft_phase_kernel(cons
     float2 v[4];
 #pragma unroll
     for (int k = 0; k < 4; ++k) { const int n = 2 * (tid + NT * k); v[k] = make_float2(sample(n), sample(n + 1)); }
+    float2* eb = MOM ? E + ((size_t)b * T + t) * F : nullptr;
+    // MOM / CONV: this thread's S and previous estimates (index 4: bin n_fft/2, thread 0) are fetched before the FFT, so
+    // that their latency hides behind it
+    float sv[5] = {};
+    float2 pv[5] = {};
+    if constexpr (MOM || CONV) {
+        const float* Sp = S + ((size_t)b * T + t) * F;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            sv[k] = Sp[tid + NT * k];
+            if constexpr (MOM) pv[k] = eb[tid + NT * k];
+        }
+        if (tid == 0) {
+            sv[4] = Sp[H];
+            if constexpr (MOM) pv[4] = eb[H];
+        }
+    }
     float2* z = fft_half<N, false>(v, s0, s1, tw);                  // z was last read before the final barrier of the FFT
 #pragma unroll
     for (int k = 0; k < 4; ++k) z[tid + NT * k] = v[k];
     __syncthreads();
     const float* Sb = S + ((size_t)b * T + t) * F;
     float2* x = X + ((size_t)b * T + t) * F;
-    auto emit = [&](int kk, float2 e) {
-        const float mag = fmaxf(1e-8f, sqrtf(e.x * e.x + e.y * e.y));
-        const float a = Sb[kk];
-        x[kk] = make_float2(a * (e.x / mag), a * (e.y / mag));
+    float dev = 0.f;                                                // CONV: this thread's sum of (S - |est|)^2
+    auto emit = [&](int kk, float2 e, int slot) {
+        if constexpr (MOM || CONV) {
+            const float a = sv[slot];
+            if constexpr (CONV) { const float d = a - sqrtf(e.x * e.x + e.y * e.y); dev = fmaf(d, d, dev); }
+            if constexpr (MOM) {
+                const float2 p = pv[slot];
+                eb[kk] = e;
+                e = make_float2(__fsub_rn(e.x, __fmul_rn(alpha, p.x)), __fsub_rn(e.y, __fmul_rn(alpha, p.y)));
+            }
+            const float mag = fmaxf(1e-8f, sqrtf(e.x * e.x + e.y * e.y));
+            x[kk] = make_float2(a * (e.x / mag), a * (e.y / mag));
+        } else {
+            const float mag = fmaxf(1e-8f, sqrtf(e.x * e.x + e.y * e.y));
+            const float a = Sb[kk];
+            x[kk] = make_float2(a * (e.x / mag), a * (e.y / mag));
+        }
     };
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
@@ -241,8 +278,46 @@ __global__ void __launch_bounds__(VcSize<N>::THREADS) voc_stft_phase_kernel(cons
         const float2 e = make_float2(0.5f * (zk.x + zc.x), 0.5f * (zk.y + zc.y));
         const float2 d = make_float2(0.5f * (zk.x - zc.x), 0.5f * (zk.y - zc.y));
         const float2 o = cmul(make_float2(d.y, -d.x), tw[kk]);     // -i d W^k
-        emit(kk, make_float2(e.x + o.x, e.y + o.y));
-        if (kk == 0) emit(H, make_float2(zk.x - zk.y, 0.f));       // bin n_fft/2: E[0] - O[0]
+        emit(kk, make_float2(e.x + o.x, e.y + o.y), k);
+        if (kk == 0) emit(H, make_float2(zk.x - zk.y, 0.f), 4);    // bin n_fft/2: E[0] - O[0]
+    }
+    if constexpr (CONV) {
+        dev = warp_sum(dev);
+        float* red = reinterpret_cast<float*>(z == s0 ? s1 : s0);  // last read inside the FFT, before the barrier above
+        if ((tid & 31) == 0) red[tid >> 5] = dev;
+        __syncthreads();
+        if (tid == 0) {
+            float sum = 0.f;
+            for (int w = 0; w < NT / 32; ++w) sum += red[w];
+            part[(size_t)b * T + t] = sum;
+        }
+    }
+}
+
+// Spectral convergence ||S - |est_i||| / ||S|| of utterance b for i < n_hist: conv (B, n_hist) float64.  part (n_hist, B, T)
+// holds the per-frame sums of voc_stft_phase_kernel<N, *, true>; frames t < T_b are summed in ascending order in float64.
+// sum S^2 over the utterance's rows is formed once, in float64, each thread over a fixed stride, then a fixed tree.
+// grid B, 256 threads.
+__global__ void __launch_bounds__(256) voc_convergence_kernel(const float* __restrict__ S, const float* __restrict__ part,
+                                                              double* __restrict__ conv, int B, int T, int F, int n_hist,
+                                                              const int* __restrict__ lengths) {
+    __shared__ double red[256];
+    const int b = blockIdx.x, tid = threadIdx.x, Tb = voc_frames_of(lengths, b, T);
+    const float* Sb = S + (size_t)b * T * F;
+    double acc = 0.0;
+    for (long long i = tid; i < (long long)Tb * F; i += 256) { const double v = Sb[i]; acc += v * v; }
+    red[tid] = acc;
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+        if (tid < o) red[tid] += red[tid + o];
+        __syncthreads();
+    }
+    const double norm = sqrt(red[0]);
+    for (int i = tid; i < n_hist; i += 256) {
+        const float* p = part + ((size_t)i * B + b) * T;
+        double num = 0.0;
+        for (int t = 0; t < Tb; ++t) num += (double)p[t];
+        conv[(size_t)b * n_hist + i] = sqrt(num) / norm;
     }
 }
 
@@ -644,7 +719,7 @@ void resample_run(const void* wav, int dtype, const ResampleUtt* utt, int B, con
         resample_kernel<float><<<grid, 256, 0, s>>>(static_cast<const float*>(wav), utt, B, seg, win, out, total);
 }
 
-int voc_launches_per_call(int n_iter) { return 1 + 3 * n_iter + 2 + 3 + 1; }
+int voc_launches_per_call(int n_iter, bool convergence) { return 1 + 3 * n_iter + 2 + 3 + 1 + (convergence ? 2 : 0); }
 size_t voc_deemph_scratch_bytes(int B, int T, int hop) { return (size_t)B * ((hop * (T - 1) + DE_LC - 1) / DE_LC) * sizeof(double); }
 
 // The stages of voc_run, each a fixed sequence of launches (dctts_vocoder_stage runs them one at a time).
@@ -665,13 +740,25 @@ void voc_istft(const VocoderArgs& a, cudaStream_t s) {
     });
 }
 
-void voc_stft_phase(const VocoderArgs& a, cudaStream_t s) {
+void voc_stft_phase(const VocoderArgs& a, cudaStream_t s, int it) {
+    float* part = a.part ? a.part + (size_t)it * a.B * a.T : nullptr;
     voc_dispatch(2 * (a.F - 1), [&](auto n) {
         constexpr int N = decltype(n)::value;
         const int Ly = a.hop * (a.T - 1), lpad = (N - a.win) / 2;
-        voc_stft_phase_kernel<N><<<dim3(a.T, a.B), VcSize<N>::THREADS, 0, s>>>(a.wav, a.S, a.X, a.tw, a.window, a.T, a.F, a.win,
-                                                                              lpad, a.hop, Ly, a.lengths);
+        auto launch = [&](auto kern) {
+            kern<<<dim3(a.T, a.B), VcSize<N>::THREADS, 0, s>>>(a.wav, a.S, a.X, a.tw, a.window, a.T, a.F, a.win, lpad, a.hop, Ly,
+                                                               a.lengths, a.E, a.alpha, part);
+        };
+        if (a.E) {
+            if (part) launch(voc_stft_phase_kernel<N, true, true>); else launch(voc_stft_phase_kernel<N, true, false>);
+        } else {
+            if (part) launch(voc_stft_phase_kernel<N, false, true>); else launch(voc_stft_phase_kernel<N, false, false>);
+        }
     });
+}
+
+void voc_convergence(const VocoderArgs& a, cudaStream_t s) {
+    voc_convergence_kernel<<<a.B, 256, 0, s>>>(a.S, a.part, a.conv, a.B, a.T, a.F, a.n_iter + 1, a.lengths);
 }
 
 void voc_deemph(const VocoderArgs& a, cudaStream_t s) {
@@ -691,7 +778,13 @@ void voc_run(const VocoderArgs& a, cudaStream_t s) {
     voc_prepare(a, s);
     for (int it = 0; it <= a.n_iter; ++it) {
         voc_istft(a, s);
-        if (it < a.n_iter) voc_stft_phase(a, s);
+        if (it < a.n_iter) voc_stft_phase(a, s, it);
+    }
+    if (a.part) {                       // est_{n_iter}: one more STFT of the final waveform (X is free now, E is not needed)
+        VocoderArgs f = a;
+        f.E = nullptr;
+        voc_stft_phase(f, s, a.n_iter);
+        voc_convergence(a, s);
     }
     voc_deemph(a, s);
     voc_energies(a, s);

@@ -5,6 +5,7 @@ the C-ABI (include/dctts.h).  This object plays the role of the reference's
 `tf.Session` + restored variables (/root/reference/synthesize.py:28-41).
 """
 import ctypes as C
+import warnings
 
 import numpy as np
 import torch
@@ -333,12 +334,16 @@ class Engine:
                                                        float(h.ref_db), float(h.preemphasis), int(h.n_iter)),
                     "dctts_set_vocoder_params")
 
-    def spectrogram2wav(self, mag, n_iter=-1, lengths=None):
+    def spectrogram2wav(self, mag, n_iter=-1, lengths=None, momentum=0.0, convergence=False):
         """utils.py:67-94 for a batch: mag (B, T, F) in [0,1] -> (untrimmed wav (B, hop*(T-1)) CUDA tensor,
         trim (B, 2) int32 numpy [start, end) as librosa.effects.trim would keep).
         `lengths`: optional (B,) magnitude frames per utterance, 2 <= lengths[b] <= T (include/dctts.h:
         dctts_spectrogram2wav_ragged): wav[b, :hop*(lengths[b]-1)] and trim[b] are what this call gives for
-        mag[b:b+1, :lengths[b]] alone, bit for bit, the rest of wav[b] is 0, and mag rows past lengths[b] are never read."""
+        mag[b:b+1, :lengths[b]] alone, bit for bit, the rest of wav[b] is 0, and mag rows past lengths[b] are never read.
+        `momentum`: the fast Griffin-Lim update of librosa's griffinlim(momentum=...) (dctts_spectrogram2wav_momentum);
+        0 is the reference's plain update.  Above 1 it warns, as librosa does; a negative one is refused.
+        `convergence=True` also returns the spectral convergence ||S - |STFT(x_i)||| / ||S|| of every iteration i = 0 ..
+        n_iter, (B, n_iter + 1) float64 CUDA tensor, as a third value."""
         mag = self._f32(mag)
         if mag.dim() == 2:
             mag = mag[None]
@@ -347,18 +352,50 @@ class Engine:
         self._set_vocoder_params()
         wav = self._empty(B, h.hop_length * (T - 1))
         trim = np.zeros((B, 2), np.int32)
-        if lengths is None:
+        n = None
+        if lengths is not None:
+            n = np.ascontiguousarray(np.asarray(lengths.cpu() if isinstance(lengths, torch.Tensor) else lengths).reshape(-1),
+                                     dtype=np.int32)
+            if n.shape[0] != B:
+                raise DcttsError("spectrogram2wav: %d lengths for %d utterances" % (n.shape[0], B))
+        momentum = float(momentum)
+        if momentum != 0.0 or convergence:
+            if momentum > 1:
+                warnings.warn("Griffin-Lim with momentum=%g > 1 can be unstable. Proceed with caution!" % momentum,
+                              stacklevel=2)
+            iters = h.n_iter if n_iter < 0 else int(n_iter)
+            conv = self._empty(B, iters + 1, dtype=torch.float64) if convergence else None
+            self._check(self._lib.dctts_spectrogram2wav_momentum(
+                self._h, _ptr(mag), B, T, None if n is None else n.ctypes.data_as(C.c_void_p), iters, momentum, _ptr(wav),
+                trim.ctypes.data_as(C.c_void_p), _ptr(conv), self._stream()), "dctts_spectrogram2wav_momentum")
+            return (wav, trim, conv) if convergence else (wav, trim)
+        if n is None:
             self._check(self._lib.dctts_spectrogram2wav(self._h, _ptr(mag), B, T, int(n_iter), _ptr(wav),
                                                         trim.ctypes.data_as(C.c_void_p), self._stream()), "dctts_spectrogram2wav")
             return wav, trim
-        n = np.ascontiguousarray(np.asarray(lengths.cpu() if isinstance(lengths, torch.Tensor) else lengths).reshape(-1),
-                                 dtype=np.int32)
-        if n.shape[0] != B:
-            raise DcttsError("spectrogram2wav: %d lengths for %d utterances" % (n.shape[0], B))
         self._check(self._lib.dctts_spectrogram2wav_ragged(self._h, _ptr(mag), B, T, n.ctypes.data_as(C.c_void_p), int(n_iter),
                                                            _ptr(wav), trim.ctypes.data_as(C.c_void_p), self._stream()),
                     "dctts_spectrogram2wav_ragged")
         return wav, trim
+
+    def vocoder_momentum_step(self, wav, S, E, X, momentum, partials=None, hop=None, win=None):
+        """Test aid (include/dctts.h: dctts_vocoder_momentum_step): ONE fast Griffin-Lim phase step on caller CUDA tensors.
+        wav (B, Ly) and S (B, T, F) float32 in; E (B, T, F) complex64 holds est_{i-1} on entry and est_i on return;
+        X (B, T, F) complex64 out; partials: optional (B, T) float32 out, each frame's sum (S - |est_i|)^2."""
+        hop = int(hop or self.hp.hop_length)
+        self._set_vocoder_params(hop, win)
+        B, T = S.shape[0], S.shape[1]
+        want = [(wav, (B, hop * (T - 1)), torch.float32), (S, (B, T, self.F), torch.float32),
+                (E, (B, T, self.F), torch.complex64), (X, (B, T, self.F), torch.complex64)]
+        if partials is not None:
+            want.append((partials, (B, T), torch.float32))
+        for t, shape, dt in want:
+            if tuple(t.shape) != shape or t.dtype != dt or not t.is_cuda or not t.is_contiguous():
+                raise DcttsError("vocoder_momentum_step: expected a contiguous CUDA %s tensor of shape %s, got %s %s" %
+                                 (dt, shape, t.dtype, tuple(t.shape)))
+        self._check(self._lib.dctts_vocoder_momentum_step(self._h, B, T, _ptr(wav), _ptr(S), _ptr(E), _ptr(X), float(momentum),
+                                                          _ptr(partials), self._stream()), "dctts_vocoder_momentum_step")
+        return X
 
     def vocoder_stage(self, stage, x, out, S=None, hop=None, win=None, power=None):
         """Test aid (include/dctts.h: dctts_vocoder_stage): ONE stage of spectrogram2wav on caller CUDA tensors, with the

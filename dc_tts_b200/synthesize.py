@@ -21,7 +21,7 @@ from .train import Graph, Session
 
 
 def synthesize(params=None, sentences=None, fast=True, write=True, seed=0, vocoder=True, allow_random_init=False,
-               until_eos=False, tail=0):
+               until_eos=False, tail=0, momentum=0.0):
     """`params`: a name -> array dict to use instead of the checkpoints.  Without it the latest checkpoints of
     hp.logdir-1 (Text2Mel) and hp.logdir-2 (SSRN) are restored, and a missing one RAISES like the reference's
     `saver.restore(sess, None)` does (synthesize.py:33,39) -- seeded random weights are used only when the caller asks
@@ -30,7 +30,10 @@ def synthesize(params=None, sentences=None, fast=True, write=True, seed=0, vocod
     `until_eos=True`: each utterance ends `tail` frames after its attention reaches the EOS of its text
     (Graph.generate_until_eos).  SSRN and the vocoder then run once each over the batch at its longest length, with a
     length per utterance: each wav is Griffin-Lim of that utterance's r * length magnitude frames.  Y and Z rows past each
-    length are 0."""
+    length are 0.
+
+    `momentum`: the vocoder's fast Griffin-Lim update (librosa's griffinlim(momentum=...)); 0 is the reference's plain
+    Griffin-Lim."""
     # Load data
     L = load_data("synthesize", sentences)
 
@@ -94,10 +97,10 @@ def synthesize(params=None, sentences=None, fast=True, write=True, seed=0, vocod
             from scipy.io.wavfile import write as write_wav
             from .utils import spectrograms2wavs
             if lengths is None:
-                wavs = spectrograms2wavs(Z)
+                wavs = spectrograms2wavs(Z, momentum=momentum)
             else:
                 # one call at the batch's longest length, each utterance on its own magnitude frames
-                wavs = spectrograms2wavs(Z[:, :hp.r * int(lengths.max())], lengths=hp.r * lengths)
+                wavs = spectrograms2wavs(Z[:, :hp.r * int(lengths.max())], lengths=hp.r * lengths, momentum=momentum)
             for i, wav in enumerate(wavs):
                 print("Working on file", i + 1)
                 write_wav(os.path.join(hp.sampledir, "{}.wav".format(i + 1)), hp.sr, wav)

@@ -21,17 +21,19 @@ from .engine import get_engine
 from .hyperparams import Hyperparams as hp
 
 
-def spectrogram2wav(mag):
-    """utils.py:67-94.  mag: (T, 1+n_fft//2) normalised magnitudes -> trimmed float32 wav (numpy)."""
-    wav, trim = get_engine().spectrogram2wav(np.asarray(mag, np.float32)[None])
+def spectrogram2wav(mag, momentum=0.0):
+    """utils.py:67-94.  mag: (T, 1+n_fft//2) normalised magnitudes -> trimmed float32 wav (numpy).  `momentum`: the
+    fast Griffin-Lim update (librosa's griffinlim(momentum=...)); 0 is the reference's plain Griffin-Lim."""
+    wav, trim = get_engine().spectrogram2wav(np.asarray(mag, np.float32)[None], momentum=momentum)
     s, e = int(trim[0, 0]), int(trim[0, 1])
     return wav[0, s:e].cpu().numpy().astype(np.float32)
 
 
-def spectrograms2wavs(mags, lengths=None):
+def spectrograms2wavs(mags, lengths=None, momentum=0.0):
     """Batched form: (B, T, F) -> list of trimmed wavs (one device pass for the whole batch).  `lengths`: optional (B,)
-    magnitude frames per utterance; wav b is then spectrogram2wav(mags[b, :lengths[b]]), bit for bit."""
-    wav, trim = get_engine().spectrogram2wav(mags, lengths=lengths)
+    magnitude frames per utterance; wav b is then spectrogram2wav(mags[b, :lengths[b]]), bit for bit.  `momentum` as
+    for spectrogram2wav."""
+    wav, trim = get_engine().spectrogram2wav(mags, lengths=lengths, momentum=momentum)
     wav = wav.cpu().numpy()
     return [wav[b, int(trim[b, 0]):int(trim[b, 1])].astype(np.float32) for b in range(wav.shape[0])]
 

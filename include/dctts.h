@@ -165,6 +165,18 @@ int dctts_spectrogram2wav(dctts_handle h, const float* mag, int32_t B, int32_t T
  * alone, bit for bit; wav[b] past that is 0.  Mag rows >= T_b are never read.  Synchronises `stream`. */
 int dctts_spectrogram2wav_ragged(dctts_handle h, const float* mag, int32_t B, int32_t T, const int32_t* lengths_host,
                                  int32_t n_iter, float* wav, int32_t* trim_host, void* stream);
+/* dctts_spectrogram2wav / _ragged with the fast Griffin-Lim update (Perraudin, Balazs and Sondergaard 2013; librosa's
+ * griffinlim(momentum=...)) and an optional per-iteration spectral convergence.  With alpha = momentum / (1 + momentum)
+ * (float64, rounded to float32) and est_i = stft(istft(X_i)), est_{-1} = 0: c = est_i - alpha est_{i-1},
+ * X_{i+1} = S c / max(1e-8, |c|); zero initial phase.  momentum must be finite and >= 0, else the call fails with a
+ * message.  lengths_host: NULL, or (B) HOST frame counts as for dctts_spectrogram2wav_ragged.  convergence: NULL, or
+ * (B, n_iter + 1) DEVICE float64 receiving ||S - |est_i||| / ||S|| over each utterance's frames, entry n_iter from one
+ * more STFT of the final waveform (before de-emphasis).  At momentum 0 the waveform and trims equal
+ * dctts_spectrogram2wav (lengths_host NULL) or dctts_spectrogram2wav_ragged, bit for bit, with or without convergence.
+ * Synchronises `stream`. */
+int dctts_spectrogram2wav_momentum(dctts_handle h, const float* mag, int32_t B, int32_t T, const int32_t* lengths_host,
+                                   int32_t n_iter, double momentum, float* wav, int32_t* trim_host, double* convergence,
+                                   void* stream);
 
 /* Feature extraction (next row, SURVEY 8f-4): get_spectrograms -- utils.py:20-65 -- for ONE utterance from the
  * loaded waveform on: trim (librosa.effects.trim), pre-emphasis, STFT, |.|, mel filterbank
@@ -357,6 +369,13 @@ int dctts_conv_gemm(dctts_handle h, int32_t impl, int32_t mode, const float* X, 
  * Fails with a message on a bad stage or shape.  Synchronises `stream`. */
 int dctts_vocoder_stage(dctts_handle h, int32_t stage, int32_t B, int32_t T, const void* in, const float* S, void* out,
                         int32_t* trim_host, void* stream);
+/* Test aid: ONE fast Griffin-Lim phase step of dctts_spectrogram2wav_momentum on caller DEVICE tensors, through the
+ * same launch function, like dctts_vocoder_stage 2: in = wav (B,Ly) float32 and S (B,T,F) float32; E (B,T,F) complex64
+ * holds est_{i-1} on entry and est_i on return; X (B,T,F) complex64 receives S c / max(1e-8, |c|).  partials: NULL, or
+ * (B,T) float32 receiving each frame's sum_k (S - |est_i|)^2.  Always runs the momentum kernel (at momentum 0,
+ * c = est_i - 0 est_{i-1}).  Fails with a message on a bad momentum.  Synchronises `stream`. */
+int dctts_vocoder_momentum_step(dctts_handle h, int32_t B, int32_t T, const float* wav, const float* S, void* E, void* X,
+                                double momentum, float* partials, void* stream);
 /* Raw device memory helpers so that a host without torch can drive the library. */
 int dctts_malloc(dctts_handle h, void** ptr, int64_t bytes);
 int dctts_free(dctts_handle h, void* ptr);
