@@ -175,6 +175,37 @@ float momentum_alpha(const std::string& fn, double momentum) {
     return (float)(momentum / (1.0 + momentum));
 }
 
+// The three spectrogram2wav entry points: Griffin-Lim on mag (B, T, F) into wav, with the fast Griffin-Lim update when
+// momentum rounds to a non-zero alpha, per-utterance frame counts when lengths_host is given and the spectral
+// convergence of every iteration when convergence is given.  fn names the entry point in every error message.
+void griffin_lim(H* h, const char* fn, const float* mag, int B, int T, const int32_t* lengths_host, int n_iter,
+                 double momentum, float* wav, int32_t* trim_host, double* convergence, cudaStream_t s) {
+    const float alpha = momentum_alpha(fn, momentum);
+    if (lengths_host) require_frame_counts(fn, lengths_host, B, T);
+    VocoderArgs a = voc_args(h, fn, B, T, s);
+    a.mag = mag; a.wav = wav;
+    if (n_iter >= 0) a.n_iter = n_iter;
+    if (lengths_host) {
+        h->voc_len.ensure((size_t)B * sizeof(int));
+        CUDA_CHECK(cudaMemcpyAsync(h->voc_len.p, lengths_host, (size_t)B * sizeof(int), cudaMemcpyHostToDevice, s));
+        a.lengths = h->voc_len.as<int>();
+    }
+    if (alpha != 0.f) {                 // est_{-1} = 0; a momentum that rounds to alpha = 0 is the plain update
+        const size_t n = (size_t)B * T * a.F * sizeof(float2);
+        h->voc_E.ensure(n);
+        CUDA_CHECK(cudaMemsetAsync(h->voc_E.p, 0, n, s));
+        a.E = h->voc_E.as<float2>(); a.alpha = alpha;
+    }
+    if (convergence) {
+        h->voc_part.ensure((size_t)(a.n_iter + 1) * B * T * sizeof(float));
+        a.part = h->voc_part.as<float>(); a.conv = convergence;
+    }
+    voc_run(a, s);
+    h->launches += voc_launches_per_call(a.n_iter, convergence != nullptr);
+    CUDA_CHECK(cudaGetLastError());
+    voc_trims(a, trim_host, s, lengths_host);
+}
+
 }  // namespace
 
 extern "C" {
@@ -193,34 +224,18 @@ int dctts_set_vocoder_params(dctts_handle h, int32_t hop_length, int32_t win_len
 int dctts_spectrogram2wav(dctts_handle h, const float* mag, int32_t B, int32_t T, int32_t n_iter, float* wav,
                           int32_t* trim_host, void* stream) {
     return guarded(h, [&] {
-        REQUIRE(mag && wav, "dctts_spectrogram2wav: bad arguments");
-        cudaStream_t s = S(h, stream);
-        VocoderArgs a = voc_args(h, "dctts_spectrogram2wav", B, T, s);
-        a.mag = mag; a.wav = wav;
-        if (n_iter >= 0) a.n_iter = n_iter;
-        voc_run(a, s);
-        h->launches += voc_launches_per_call(a.n_iter);
-        CUDA_CHECK(cudaGetLastError());
-        voc_trims(a, trim_host, s);
+        const char* fn = "dctts_spectrogram2wav";
+        REQUIRE(mag && wav, std::string(fn) + ": bad arguments");
+        griffin_lim(h, fn, mag, B, T, nullptr, n_iter, 0.0, wav, trim_host, nullptr, S(h, stream));
     });
 }
 
 int dctts_spectrogram2wav_ragged(dctts_handle h, const float* mag, int32_t B, int32_t T, const int32_t* lengths_host,
                                  int32_t n_iter, float* wav, int32_t* trim_host, void* stream) {
     return guarded(h, [&] {
-        const std::string fn = "dctts_spectrogram2wav_ragged";
-        REQUIRE(mag && wav && lengths_host, fn + ": bad arguments");
-        require_frame_counts(fn, lengths_host, B, T);
-        cudaStream_t s = S(h, stream);
-        VocoderArgs a = voc_args(h, fn.c_str(), B, T, s);
-        h->voc_len.ensure((size_t)B * sizeof(int));
-        CUDA_CHECK(cudaMemcpyAsync(h->voc_len.p, lengths_host, (size_t)B * sizeof(int), cudaMemcpyHostToDevice, s));
-        a.mag = mag; a.wav = wav; a.lengths = h->voc_len.as<int>();
-        if (n_iter >= 0) a.n_iter = n_iter;
-        voc_run(a, s);
-        h->launches += voc_launches_per_call(a.n_iter);
-        CUDA_CHECK(cudaGetLastError());
-        voc_trims(a, trim_host, s, lengths_host);
+        const char* fn = "dctts_spectrogram2wav_ragged";
+        REQUIRE(mag && wav && lengths_host, std::string(fn) + ": bad arguments");
+        griffin_lim(h, fn, mag, B, T, lengths_host, n_iter, 0.0, wav, trim_host, nullptr, S(h, stream));
     });
 }
 
@@ -228,33 +243,9 @@ int dctts_spectrogram2wav_momentum(dctts_handle h, const float* mag, int32_t B, 
                                    int32_t n_iter, double momentum, float* wav, int32_t* trim_host, double* convergence,
                                    void* stream) {
     return guarded(h, [&] {
-        const std::string fn = "dctts_spectrogram2wav_momentum";
-        REQUIRE(mag && wav, fn + ": bad arguments");
-        const float alpha = momentum_alpha(fn, momentum);
-        if (lengths_host) require_frame_counts(fn, lengths_host, B, T);
-        cudaStream_t s = S(h, stream);
-        VocoderArgs a = voc_args(h, fn.c_str(), B, T, s);
-        a.mag = mag; a.wav = wav;
-        if (n_iter >= 0) a.n_iter = n_iter;
-        if (lengths_host) {
-            h->voc_len.ensure((size_t)B * sizeof(int));
-            CUDA_CHECK(cudaMemcpyAsync(h->voc_len.p, lengths_host, (size_t)B * sizeof(int), cudaMemcpyHostToDevice, s));
-            a.lengths = h->voc_len.as<int>();
-        }
-        if (alpha != 0.f) {                 // est_{-1} = 0; a momentum that rounds to alpha = 0 is the plain update
-            const size_t n = (size_t)B * T * a.F * sizeof(float2);
-            h->voc_E.ensure(n);
-            CUDA_CHECK(cudaMemsetAsync(h->voc_E.p, 0, n, s));
-            a.E = h->voc_E.as<float2>(); a.alpha = alpha;
-        }
-        if (convergence) {
-            h->voc_part.ensure((size_t)(a.n_iter + 1) * B * T * sizeof(float));
-            a.part = h->voc_part.as<float>(); a.conv = convergence;
-        }
-        voc_run(a, s);
-        h->launches += voc_launches_per_call(a.n_iter, convergence != nullptr);
-        CUDA_CHECK(cudaGetLastError());
-        voc_trims(a, trim_host, s, lengths_host);
+        const char* fn = "dctts_spectrogram2wav_momentum";
+        REQUIRE(mag && wav, std::string(fn) + ": bad arguments");
+        griffin_lim(h, fn, mag, B, T, lengths_host, n_iter, momentum, wav, trim_host, convergence, S(h, stream));
     });
 }
 

@@ -23,6 +23,14 @@ def _ptr(t):
     return C.c_void_p(0) if t is None else C.c_void_p(t.data_ptr())
 
 
+def _require_tensors(who, want):
+    """Each (tensor, shape, dtype) of `want` is a contiguous CUDA tensor of that shape and dtype, else DcttsError."""
+    for t, shape, dt in want:
+        if tuple(t.shape) != shape or t.dtype != dt or not t.is_cuda or not t.is_contiguous():
+            raise DcttsError("%s: expected a contiguous CUDA %s tensor of shape %s, got %s %s" %
+                             (who, dt, shape, t.dtype, tuple(t.shape)))
+
+
 class Engine:
     def __init__(self, device=0, hparams=hp):
         self._lib = _lib.load()
@@ -336,12 +344,13 @@ class Engine:
 
     def spectrogram2wav(self, mag, n_iter=-1, lengths=None, momentum=0.0, convergence=False):
         """utils.py:67-94 for a batch: mag (B, T, F) in [0,1] -> (untrimmed wav (B, hop*(T-1)) CUDA tensor,
-        trim (B, 2) int32 numpy [start, end) as librosa.effects.trim would keep).
-        `lengths`: optional (B,) magnitude frames per utterance, 2 <= lengths[b] <= T (include/dctts.h:
-        dctts_spectrogram2wav_ragged): wav[b, :hop*(lengths[b]-1)] and trim[b] are what this call gives for
-        mag[b:b+1, :lengths[b]] alone, bit for bit, the rest of wav[b] is 0, and mag rows past lengths[b] are never read.
-        `momentum`: the fast Griffin-Lim update of librosa's griffinlim(momentum=...) (dctts_spectrogram2wav_momentum);
-        0 is the reference's plain update.  Above 1 it warns, as librosa does; a negative one is refused.
+        trim (B, 2) int32 numpy [start, end) as librosa.effects.trim would keep).  Every call goes through
+        dctts_spectrogram2wav_momentum (include/dctts.h), so its errors name that entry point.
+        `lengths`: optional (B,) magnitude frames per utterance, 2 <= lengths[b] <= T: wav[b, :hop*(lengths[b]-1)] and
+        trim[b] are what this call gives for mag[b:b+1, :lengths[b]] alone, bit for bit, the rest of wav[b] is 0, and mag
+        rows past lengths[b] are never read.
+        `momentum`: the fast Griffin-Lim update of librosa's griffinlim(momentum=...); 0 is the reference's plain update.
+        Above 1 it warns, as librosa does; a negative one is refused.
         `convergence=True` also returns the spectral convergence ||S - |STFT(x_i)||| / ||S|| of every iteration i = 0 ..
         n_iter, (B, n_iter + 1) float64 CUDA tensor, as a third value."""
         mag = self._f32(mag)
@@ -359,24 +368,14 @@ class Engine:
             if n.shape[0] != B:
                 raise DcttsError("spectrogram2wav: %d lengths for %d utterances" % (n.shape[0], B))
         momentum = float(momentum)
-        if momentum != 0.0 or convergence:
-            if momentum > 1:
-                warnings.warn("Griffin-Lim with momentum=%g > 1 can be unstable. Proceed with caution!" % momentum,
-                              stacklevel=2)
-            iters = h.n_iter if n_iter < 0 else int(n_iter)
-            conv = self._empty(B, iters + 1, dtype=torch.float64) if convergence else None
-            self._check(self._lib.dctts_spectrogram2wav_momentum(
-                self._h, _ptr(mag), B, T, None if n is None else n.ctypes.data_as(C.c_void_p), iters, momentum, _ptr(wav),
-                trim.ctypes.data_as(C.c_void_p), _ptr(conv), self._stream()), "dctts_spectrogram2wav_momentum")
-            return (wav, trim, conv) if convergence else (wav, trim)
-        if n is None:
-            self._check(self._lib.dctts_spectrogram2wav(self._h, _ptr(mag), B, T, int(n_iter), _ptr(wav),
-                                                        trim.ctypes.data_as(C.c_void_p), self._stream()), "dctts_spectrogram2wav")
-            return wav, trim
-        self._check(self._lib.dctts_spectrogram2wav_ragged(self._h, _ptr(mag), B, T, n.ctypes.data_as(C.c_void_p), int(n_iter),
-                                                           _ptr(wav), trim.ctypes.data_as(C.c_void_p), self._stream()),
-                    "dctts_spectrogram2wav_ragged")
-        return wav, trim
+        if momentum > 1:
+            warnings.warn("Griffin-Lim with momentum=%g > 1 can be unstable. Proceed with caution!" % momentum, stacklevel=2)
+        iters = h.n_iter if n_iter < 0 else int(n_iter)
+        conv = self._empty(B, iters + 1, dtype=torch.float64) if convergence else None
+        self._check(self._lib.dctts_spectrogram2wav_momentum(
+            self._h, _ptr(mag), B, T, None if n is None else n.ctypes.data_as(C.c_void_p), iters, momentum, _ptr(wav),
+            trim.ctypes.data_as(C.c_void_p), _ptr(conv), self._stream()), "dctts_spectrogram2wav_momentum")
+        return (wav, trim, conv) if convergence else (wav, trim)
 
     def vocoder_momentum_step(self, wav, S, E, X, momentum, partials=None, hop=None, win=None):
         """Test aid (include/dctts.h: dctts_vocoder_momentum_step): ONE fast Griffin-Lim phase step on caller CUDA tensors.
@@ -389,10 +388,7 @@ class Engine:
                 (E, (B, T, self.F), torch.complex64), (X, (B, T, self.F), torch.complex64)]
         if partials is not None:
             want.append((partials, (B, T), torch.float32))
-        for t, shape, dt in want:
-            if tuple(t.shape) != shape or t.dtype != dt or not t.is_cuda or not t.is_contiguous():
-                raise DcttsError("vocoder_momentum_step: expected a contiguous CUDA %s tensor of shape %s, got %s %s" %
-                                 (dt, shape, t.dtype, tuple(t.shape)))
+        _require_tensors("vocoder_momentum_step", want)
         self._check(self._lib.dctts_vocoder_momentum_step(self._h, B, T, _ptr(wav), _ptr(S), _ptr(E), _ptr(X), float(momentum),
                                                           _ptr(partials), self._stream()), "dctts_vocoder_momentum_step")
         return X
@@ -425,10 +421,7 @@ class Engine:
                 2: [(x, (B, Ly), f32), (S, (B, T, F), f32), (out, (B, T, F), c64)],
                 3: [(x, (B, Ly), f32), (out, (B, Ly), f32)],
                 4: [(x, (B, Ly), f32), (out, (B, 1 + Ly // 512), f32)]}.get(stage, [])
-        for t, shape, dt in want:
-            if tuple(t.shape) != shape or t.dtype != dt or not t.is_cuda or not t.is_contiguous():
-                raise DcttsError("vocoder_stage %d: expected a contiguous CUDA %s tensor of shape %s, got %s %s" %
-                                 (stage, dt, shape, t.dtype, tuple(t.shape)))
+        _require_tensors("vocoder_stage %d" % stage, want)
         trim = np.zeros((B, 2), np.int32)
         self._check(self._lib.dctts_vocoder_stage(self._h, int(stage), B, T, _ptr(x), _ptr(S), _ptr(out),
                                                   trim.ctypes.data_as(C.POINTER(C.c_int32)), self._stream()),

@@ -38,20 +38,24 @@ def spectrograms2wavs(mags, lengths=None, momentum=0.0):
     return [wav[b, int(trim[b, 0]):int(trim[b, 1])].astype(np.float32) for b in range(wav.shape[0])]
 
 
-def griffin_lim(spectrogram):
-    """utils.py:96-107.  spectrogram: (1+n_fft//2, t) amplitude (already ** hp.power) -> waveform."""
-    S = np.asarray(spectrogram, np.float32).T
+def _vocode_amplitude(S, n_iter, clip):
+    """The device vocoder on an amplitude S (t, 1+n_fft//2), already ** hp.power, without its de-emphasis.  `clip`:
+    clip the normalised magnitude to [0, 1], else refuse one outside it."""
     # undo the de-normalisation the device entry point applies: S = (10 ^ ((z*max_db - max_db + ref_db)/20)) ^ power
     z = (20.0 * np.log10(np.maximum(S, 1e-30) ** (1.0 / hp.power)) + hp.max_db - hp.ref_db) / hp.max_db
-    if z.min() < 0 or z.max() > 1:
+    if not clip and (z.min() < 0 or z.max() > 1):
         raise ValueError("griffin_lim: amplitude outside the range spectrogram2wav can produce")
-    e = get_engine()
-    wav, _ = e.spectrogram2wav(z[None].astype(np.float32))
+    wav, _ = get_engine().spectrogram2wav(np.clip(z, 0, 1)[None].astype(np.float32), n_iter=n_iter)
     # spectrogram2wav also de-pre-emphasises; Griffin-Lim alone does not: invert y[n] = x[n] + c y[n-1]
     y = wav[0].cpu().numpy().astype(np.float64)
     x = y.copy()
     x[1:] -= hp.preemphasis * y[:-1]
     return x.astype(np.float32)
+
+
+def griffin_lim(spectrogram):
+    """utils.py:96-107.  spectrogram: (1+n_fft//2, t) amplitude (already ** hp.power) -> waveform."""
+    return _vocode_amplitude(np.asarray(spectrogram, np.float32).T, -1, clip=False)
 
 
 def invert_spectrogram(spectrogram):
@@ -60,13 +64,7 @@ def invert_spectrogram(spectrogram):
     if np.iscomplexobj(S):
         raise NotImplementedError("invert_spectrogram: only zero-phase (real) input is exposed; the complex "
                                   "iterations run inside dctts_spectrogram2wav")
-    z = (20.0 * np.log10(np.maximum(S.T, 1e-30) ** (1.0 / hp.power)) + hp.max_db - hp.ref_db) / hp.max_db
-    e = get_engine()
-    wav, _ = e.spectrogram2wav(np.clip(z, 0, 1)[None].astype(np.float32), n_iter=0)
-    y = wav[0].cpu().numpy().astype(np.float64)
-    x = y.copy()
-    x[1:] -= hp.preemphasis * y[:-1]
-    return x.astype(np.float32)
+    return _vocode_amplitude(S.T, 0, clip=True)
 
 
 def _read_wav(fpath):

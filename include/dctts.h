@@ -156,13 +156,15 @@ int dctts_set_vocoder_params(dctts_handle h, int32_t hop_length, int32_t win_len
  * magnitudes -> de-normalise, ^power, Griffin-Lim (n_iter x istft/stft with librosa's conventions), de-pre-emphasis.
  * wav (B, hop*(T-1)) DEVICE float32 receives the UNTRIMMED waveform; trim_host (B, 2) HOST int32 receives the
  * [start, end) sample range librosa.effects.trim (top_db 60) would keep.  n_iter < 0 means the configured value.
- * Synchronises `stream` before returning (trim_host is written by the host). */
+ * Synchronises `stream` before returning (trim_host is written by the host).  This is dctts_spectrogram2wav_momentum
+ * with lengths_host NULL and momentum 0. */
 int dctts_spectrogram2wav(dctts_handle h, const float* mag, int32_t B, int32_t T, int32_t n_iter, float* wav,
                           int32_t* trim_host, void* stream);
 /* dctts_spectrogram2wav with a frame count per utterance, in one call at T.  lengths_host: (B) HOST int32 magnitude
  * frames, 2 <= lengths_host[b] <= T; a count outside that range fails the call, naming the utterance, before any
  * launch.  For each b, wav[b, :hop (T_b - 1)] and trim_host[b] are those of dctts_spectrogram2wav on mag[b:b+1, :T_b]
- * alone, bit for bit; wav[b] past that is 0.  Mag rows >= T_b are never read.  Synchronises `stream`. */
+ * alone, bit for bit; wav[b] past that is 0.  Mag rows >= T_b are never read.  Synchronises `stream`.  This is
+ * dctts_spectrogram2wav_momentum with momentum 0 (lengths_host is required here). */
 int dctts_spectrogram2wav_ragged(dctts_handle h, const float* mag, int32_t B, int32_t T, const int32_t* lengths_host,
                                  int32_t n_iter, float* wav, int32_t* trim_host, void* stream);
 /* dctts_spectrogram2wav / _ragged with the fast Griffin-Lim update (Perraudin, Balazs and Sondergaard 2013; librosa's

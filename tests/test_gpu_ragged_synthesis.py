@@ -42,8 +42,9 @@ _SINGLE = {}
 
 
 def _single(e, path, Y, b, n):
-    """SSRN of utterance b alone at its own length (cached per kernel set)."""
-    key = (id(e), path, b, n)
+    """SSRN of utterance b alone at its own length (cached per engine and kernel set; the key holds the engine itself, as
+    an engine built after another was closed may get its id)."""
+    key = (e, path, b, n)
     if key not in _SINGLE:
         lg, Z = e.ssrn(Y[b:b + 1, :n])
         _SINGLE[key] = (lg[0].cpu(), Z[0].cpu())
@@ -207,7 +208,7 @@ _VSINGLE = {}
 
 
 def _voc_single(e, mags, b, k, n_iter):
-    key = (id(e), b, k, n_iter)
+    key = (e, b, k, n_iter)                 # the engine itself, as for _single
     if key not in _VSINGLE:
         wav, trim = e.spectrogram2wav(mags[b:b + 1, :k], n_iter=n_iter)
         _VSINGLE[key] = (wav[0].cpu(), trim[0].copy())

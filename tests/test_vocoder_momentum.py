@@ -1,49 +1,15 @@
 """Fast Griffin-Lim in the oracle (tests/ref_fast_griffin_lim.py): momentum 0 is the reference's Griffin-Lim bit
 for bit, and on the magnitudes of real-looking signals momentum 0.99 converges further in 50 iterations than plain
 Griffin-Lim does, measured by the spectral convergence ||S - |STFT(x)||| / ||S||.  The GPU half is
-test_gpu_vocoder_momentum.py; it takes its signals from here."""
+test_gpu_vocoder_momentum.py; both take their signals from tests/ref_vocoder_stages.py."""
 import numpy as np
 import pytest
 
 from dc_tts_b200.hyperparams import Hyperparams as hp
-from oracle import ref_features as rf
 from oracle import ref_vocoder as rv
 
 import ref_fast_griffin_lim as fg
-
-SIGNALS = ("vibrato", "chirp", "bursts")
-POWERS = (1.0, 1.5)
-
-
-def signal(kind, seconds=1.0, seed=0):
-    """Seeded synthetic waveforms at hp.sr: a harmonic tone with vibrato, a linear chirp, noise bursts."""
-    rng = np.random.default_rng(seed)
-    n = int(seconds * hp.sr)
-    t = np.arange(n) / hp.sr
-    if kind == "vibrato":
-        f0 = 140.0 + 8.0 * np.sin(2 * np.pi * 5.5 * t)
-        ph = 2 * np.pi * np.cumsum(f0) / hp.sr
-        y = sum(0.3 / h * np.sin(h * ph) for h in range(1, 9)) * (0.6 + 0.4 * np.sin(2 * np.pi * 2 * t))
-    elif kind == "chirp":
-        y = 0.5 * np.sin(2 * np.pi * (200.0 * t + 0.5 * 3000.0 * t * t / seconds))
-    else:
-        y = 0.02 * rng.standard_normal(n)
-        for start in rng.uniform(0, seconds - 0.12, 6):
-            i = int(start * hp.sr)
-            m = int(0.1 * hp.sr)
-            y[i:i + m] += 0.4 * rng.standard_normal(m) * np.hanning(m)
-    return np.clip(y, -1, 1).astype(np.float32)
-
-
-def magnitude(kind):
-    """The normalised linear magnitude (T, 1 + n_fft / 2) of signal `kind`, as the reference's get_spectrograms gives it."""
-    return rf.get_spectrograms(signal(kind))[1]
-
-
-def amplitude(mag, power, dtype=np.float32):
-    """utils.py:78-85 at `power`: (F, T) amplitude target S of a (T, F) normalised magnitude."""
-    m = (np.clip(mag.T, 0, 1) * hp.max_db) - hp.max_db + hp.ref_db
-    return (np.power(10.0, m * 0.05) ** power).astype(dtype)
+from ref_vocoder_stages import POWERS, SIGNALS, amplitude, magnitude
 
 
 def test_momentum_zero_is_griffin_lim_bit_for_bit():

@@ -1,9 +1,9 @@
 """Time the Griffin-Lim vocoder with and without momentum, and measure what momentum gains in spectral convergence.
 
 B = 32 utterances of 840 magnitude frames (10.5 s at 22.05 kHz), n_iter = 50; three variants alternated in one run,
-CUDA events around `--iters` calls each:
-  plain          Engine.spectrogram2wav(mag)                              (dctts_spectrogram2wav)
-  momentum       Engine.spectrogram2wav(mag, momentum=0.99)               (dctts_spectrogram2wav_momentum)
+CUDA events around `--iters` calls each, all three through dctts_spectrogram2wav_momentum:
+  plain          Engine.spectrogram2wav(mag)                              (momentum 0: the plain update)
+  momentum       Engine.spectrogram2wav(mag, momentum=0.99)
   momentum+conv  Engine.spectrogram2wav(mag, momentum=0.99, convergence=True)
 The magnitudes are the on-device features (Engine.get_spectrograms) of seeded synthetic signals: harmonic tones with
 vibrato, chirps and noise bursts, cycled over the batch.  Then, from the convergence histories of plain Griffin-Lim and of
