@@ -302,7 +302,7 @@ void run_block_tc(Launch& lc, const LayerDev& l, int rate, bool causal, int act,
         {
             const int* d0 = dbg_host;      // SM-clock deltas of CTA 0
             auto dt = [&](int a_, int b_) { return (d0[b_] - d0[a_]) & 0x7fffffff; };
-            fprintf(stderr, "[tc]  cta 0 cycles: setup %d | main loop %d | sweeps1+2 %d | cluster barrier %d | sweep3+stores %d | teardown %d | total %d\n",
+            fprintf(stderr, "[tc]  cta 0 cycles: setup %d | main loop %d | statistics %d | cluster barrier %d | normalise+stores %d | teardown %d | total %d\n",
                     dt(8, 9), dt(9, 10), dt(10, 11), dt(11, 12), dt(12, 13), dt(13, 14), dt(8, 14));
         }
         if (e != cudaSuccess) throw std::runtime_error(std::string("conv_ln_tc failed: ") + cudaGetErrorString(e));

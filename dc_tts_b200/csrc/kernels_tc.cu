@@ -14,10 +14,9 @@
 //           {BK x bn} box of each weight plane, swizzled, mbarrier pipelined.
 //   warpgroups 1, 2  wgmma (M=64 each, N=bn: one instruction over the CTA's whole width, K=16):
 //           hi*Whi + hi*Wlo + lo*Whi per k-step into fp32 register accumulators, one k-block
-//           in flight while the next is issued; then the accumulators go to shared memory as
-//           one 128 x bn tile.
-//   warpgroup 1  epilogue: thread == row, so LN reductions are thread-local; one
-//           statistics sweep and one normalise+store sweep over the tile.
+//           in flight while the next is issued; then each warpgroup runs the epilogue of its
+//           64 rows on its accumulator fragment: LN statistics as per-thread partial sums
+//           completed over the quad that holds a row, then normalise + store.
 #include "kernels_tc.cuh"
 #include "numerics.cuh"
 #include "tc_ptx.cuh"
@@ -48,28 +47,99 @@ __device__ __forceinline__ void dbg_time(int* dbg, int slot) {
     if (dbg) dbg_mark(dbg, slot, (int)(clock64() & 0x7fffffff));
 }
 
-__device__ __forceinline__ void store_planes(const Planes& p, size_t row, int col, int C, const float (&o)[16]) {
-    __half* hi = p.hi + row * p.ld + col;
-    __half* lo = p.lo + row * p.ld + col;
-    if (col + 16 <= p.ld) {
-        split_store_f16<16>(o, hi, lo);
-    } else {
+// The epilogue works on the m64nBN accumulator fragment (tc_ptx.cuh) in registers: the thread at (warp w4 of its
+// warpgroup, lane) holds rows w4 * 16 + lane / 4 (h = 0) and that + 8 (h = 1) of its warpgroup's 64, and in each 8-column
+// group q the columns 8q + 2j + {0, 1}, j = lane & 3, at v[4q + 2h + {0, 1}].  A row is spread over the 4 lanes of a quad.
+
+// Shifted sums of columns [0, n) of groups [G0, G0 + NG) of fragment row h, completed over the quad: s = their sum, m2 =
+// the sum of squared deviations from their mean.  The deviations are taken about the row's first column of the range, so
+// that m2 = Q - S^2 / n does not cancel.  The order of the sums depends on the column layout only, never on the tile.
+template <int G0, int NG, int R>
+__device__ __forceinline__ void row_stats(const float (&v)[R], int h, int j, int n, float& s, float& m2) {
+    const float piv = __shfl_sync(0xffffffffu, v[4 * G0 + 2 * h], (threadIdx.x & 31) & ~3);
+    float S = 0.f, Q = 0.f;
 #pragma unroll
-        for (int i = 0; i < 16; ++i)
-            if (col + i < C) split_f16(o[i], hi[i], lo[i]);
+    for (int k = 0; k < NG; ++k)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+            if (8 * k + 2 * j + e < n) { const float d = v[4 * (G0 + k) + 2 * h + e] - piv; S += d; Q = fmaf(d, d, Q); }
+#pragma unroll
+    for (int m = 1; m < 4; m <<= 1) { S += __shfl_xor_sync(0xffffffffu, S, m); Q += __shfl_xor_sync(0xffffffffu, Q, m); }
+    s = piv * (float)n + S;
+    m2 = fmaxf(Q - S * S / (float)max(n, 1), 0.f);
+}
+
+// 4 x 4 transpose over a quad: on entry lane j holds x[k] = part j of group k, on exit x[k] = part k of group j
+__device__ __forceinline__ void quad_transpose(uint32_t (&x)[4], int j) {
+#pragma unroll
+    for (int m = 2; m > 0; m >>= 1) {
+        const bool up = (j & m) != 0;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            if (k & m) continue;
+            const uint32_t r = __shfl_xor_sync(0xffffffffu, up ? x[k] : x[k ^ m], m);
+            if (up) x[k] = r; else x[k ^ m] = r;
+        }
     }
 }
 
-// Shared memory: [ring of `stages` stages | after the main loop: the 128 x (bn + 4) fp32 accumulator tile] [residual /
-// output staging tile (hc with resid_tma)] [barriers, epilogue vectors, LN partials].  The accumulator tile reuses the ring:
-// it is written only once every k-block has been multiplied, and every multicast box aimed at this CTA has landed by then
-// (each one completes on a full barrier that the consumers waited for).
-__host__ __device__ inline int tc_acc_ld(int bn) { return bn + 4; }                  // row pitch: float4 rows hit distinct banks
-__host__ __device__ inline int tc_ring_bytes(int stages, int stage_bytes, int bn) {
-    const int ring = stages * stage_bytes;                                             // each wgmma reads exactly bn weight rows
-    const int acc = TC_BM * tc_acc_ld(bn) * 4;
-    return ((ring > acc ? ring : acc) + 1023) & ~1023;
+__device__ __forceinline__ uint32_t h2_bits(__half2 v) { return *reinterpret_cast<uint32_t*>(&v); }
+
+// Groups [G0, G0 + NG) of fragment row h -> split planes, columns col0 .. col0 + 8 NG of output row `row` (stored if ok).
+// Every four groups are transposed over the quad so that each lane stores 8 consecutive columns, 16 bytes per plane, and a
+// quad 64 contiguous bytes.  A group at or past the row pitch is not stored; columns past C inside it hold zeros.  All lanes
+// call it (the transpose shuffles), whatever their row's ok.
+template <int G0, int NG, int R>
+__device__ __forceinline__ void store_planes_frag(const Planes& p, size_t row, int col0, const float (&v)[R], int h, int j,
+                                                  bool ok) {
+    __half* hi = p.hi + row * p.ld;
+    __half* lo = p.lo + row * p.ld;
+#pragma unroll
+    for (int k = 0; k + 4 <= NG; k += 4) {
+        uint32_t xh[4], xl[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int q = G0 + k + i;
+            __half2 a, b;
+            split_f16x2(make_float2(v[4 * q + 2 * h], v[4 * q + 2 * h + 1]), a, b);
+            xh[i] = h2_bits(a); xl[i] = h2_bits(b);
+        }
+        quad_transpose(xh, j);
+        quad_transpose(xl, j);
+        const int col = col0 + 8 * (k + j);
+        if (ok && col + 8 <= p.ld) {
+            *reinterpret_cast<uint4*>(hi + col) = make_uint4(xh[0], xh[1], xh[2], xh[3]);
+            *reinterpret_cast<uint4*>(lo + col) = make_uint4(xl[0], xl[1], xl[2], xl[3]);
+        }
+    }
+#pragma unroll
+    for (int k = NG & ~3; k < NG; ++k) {                                  // groups past the last four: 4 bytes per plane
+        const int q = G0 + k, col = col0 + 8 * k + 2 * j;
+        __half2 a, b;
+        split_f16x2(make_float2(v[4 * q + 2 * h], v[4 * q + 2 * h + 1]), a, b);
+        if (ok && col + 2 <= p.ld) { *reinterpret_cast<__half2*>(hi + col) = a; *reinterpret_cast<__half2*>(lo + col) = b; }
+    }
 }
+
+// Columns [0, n) of groups [G0, G0 + NG) of fragment row h -> fp32 row `dst` from column col0: a quad writes 8 consecutive
+// floats per group, 8-byte stores where the address allows and scalar ones otherwise.  That is one 32-byte sector only
+// where the row and col0 are 32-byte aligned; the networks' fp32 outputs (80 and 1025 floats per row) mostly are not,
+// so there a group spans two sectors.
+template <int G0, int NG, int R>
+__device__ __forceinline__ void store_f32_frag(float* dst, int col0, int n, const float (&v)[R], int h, int j) {
+#pragma unroll
+    for (int k = 0; k < NG; ++k) {
+        const int c = 8 * k + 2 * j;
+        const float x0 = v[4 * (G0 + k) + 2 * h], x1 = v[4 * (G0 + k) + 2 * h + 1];
+        float* d = dst + col0 + c;
+        if (c + 1 < n && (reinterpret_cast<uintptr_t>(d) & 7) == 0) *reinterpret_cast<float2*>(d) = make_float2(x0, x1);
+        else { if (c < n) d[0] = x0; if (c + 1 < n) d[1] = x1; }
+    }
+}
+
+// Shared memory: [ring of `stages` stages] [residual / output staging tile (hc with resid_tma)] [barriers, epilogue
+// vectors, LN partials]
+__host__ __device__ inline int tc_ring_bytes(int stages, int stage_bytes) { return (stages * stage_bytes + 1023) & ~1023; }
 // Largest cluster of an instantiation: 16 CTAs (a non-portable cluster size) for the 144-column one, whose F = 2049 conv1d
 // blocks split 2049 channels over 16 x 144; 8 for the others
 __host__ __device__ constexpr int tc_max_cluster(int bn) { return bn == 144 ? 16 : 8; }
@@ -87,19 +157,20 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
                   const __grid_constant__ CUtensorMap mapO_hi, const __grid_constant__ CUtensorMap mapO_lo,
                   const TcArgs a) {
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    // aligned by an offset from smem_raw (not through an integer), so that the compiler keeps shared-memory loads
+    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     pdl_launch_dependents();          // PDL: let the next kernel's CTAs be scheduled behind this one
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int wg = threadIdx.x >> 7;                                 // 0: producer warpgroup, 1 / 2: consumers of rows 0-63 / 64-127
-    const bool epi = wg == 1;                                        // the first consumer warpgroup also runs the epilogue
     if (threadIdx.x == 0) dbg_time(a.dbg, 8);                        // t0: kernel entry
     const int rank = (int)cluster_ctarank();                         // channel slice of this CTA
     const int ncta = (int)cluster_nctarank();
     const int nslices = ncta;
     constexpr int MAXC = tc_max_cluster(BN);                         // cluster size bound: the statistics merge's unroll
     constexpr int bn = BN;                                           // accumulator columns per CTA
-    const int half = a.half;                                         // columns per LN half
+    const int half = a.half;                                         // columns per LN half (mode 0: bn)
+    constexpr int HALF = BN / 2, NG = BN / 8, HG = BN / 16;          // modes 1, 2: columns of one LN half; 8-column groups
     constexpr int TC_A_PLANE = TC_BM * TC_BK * 2;                    // bytes of one activation plane tile
     constexpr int SW = TC_BK * 2;                                    // swizzle span = row bytes (128 or 64)
     constexpr int b_plane = bn * SW;                                 // bytes of one weight plane tile
@@ -107,10 +178,8 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
     constexpr int stage_bytes = A_BYTES + 2 * b_plane;
     const int stages = a.stages;
     const int nkb = a.ntaps * a.kb_per_tap;
-    const int acc_ld = tc_acc_ld(bn);
 
-    float* s_acc = reinterpret_cast<float*>(smem);
-    uint8_t* rs = smem + tc_ring_bytes(stages, stage_bytes, bn);   // residual / output staging tile
+    uint8_t* rs = smem + tc_ring_bytes(stages, stage_bytes);      // residual / output staging tile
     uint8_t* aux = rs + tc_resid_bytes(a.resid_tma, half);
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(aux);              // [stages]
     uint64_t* empty_bar = full_bar + TC_MAX_STAGES;                      // [stages]
@@ -165,9 +234,12 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
     const uint16_t cta_mask = (uint16_t)((1u << ncta) - 1u);
     const int slice_rows = TC_BM / ncta;
 
-    if (warp == 0) {
+    if (wg == 0) {
         // =========================== TMA producer ===========================
-        if (lane == 0) {
+        // its registers go to the consumers, whose epilogue holds the whole fragment: 128 x 40 + 256 x 232 = 64,512
+        // registers, what __launch_bounds__(384, 1) gives the CTA
+        setmaxnreg_dec<40>();
+        if (warp == 0 && lane == 0) {
             for (int kb = 0; kb < nkb; ++kb) {
                 const int s = kb % stages;
                 const uint32_t ph = (uint32_t)(kb / stages) & 1u;
@@ -201,8 +273,9 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
             }
         }
         __syncwarp();
-    } else if (wg >= 1) {
+    } else {
         // =========================== wgmma consumers ===========================
+        setmaxnreg_inc<232>();
         const int mh = wg - 1;                                           // row half of the tile
         float acc[BN / 2];                                               // m64nBN fragment (tc_ptx.cuh)
 #pragma unroll
@@ -236,237 +309,211 @@ conv_ln_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_cons
         }
         wg_wait<0>();                                                    // the last k-block (its stage is never refilled)
         wg_fence_regs(acc);
-        if (threadIdx.x == 128) dbg_mark(a.dbg, 4, nkb);
-        named_sync(1, 256);                                              // both halves done reading the ring
-        {
-            const int w4 = (threadIdx.x >> 5) & 3;
-            const int r0 = mh * 64 + w4 * 16 + (lane >> 2);
+        if (threadIdx.x == 128) { dbg_mark(a.dbg, 4, nkb); dbg_mark(a.dbg, 5, 1); dbg_time(a.dbg, 10); }   // t2: main loop over
+
+        // =========================== epilogue on the fragment: both warpgroups, 64 rows each ===========================
+        const int j = lane & 3;
+        const int rt = mh * 64 + (warp & 3) * 16 + (lane >> 2);          // tile rows rt (h = 0) and rt + 8 (h = 1)
+        int bb[2], tt[2];
+        bool ok[2], live[2];
+        float inv_s[2];
 #pragma unroll
-            for (int q = 0; q < BN / 8; ++q) {
-                const int col = q * 8 + 2 * (lane & 3);
-                *reinterpret_cast<float2*>(s_acc + (size_t)r0 * acc_ld + col) = make_float2(acc[q * 4], acc[q * 4 + 1]);
-                *reinterpret_cast<float2*>(s_acc + (size_t)(r0 + 8) * acc_ld + col) = make_float2(acc[q * 4 + 2], acc[q * 4 + 3]);
+        for (int h = 0; h < 2; ++h) {
+            const int r = rt + 8 * h, bi = r / a.TT;
+            const int b = b0s + bi, t = t0s + r - bi * a.TT;
+            bb[h] = b; tt[h] = t;
+            ok[h] = (b < a.win.B) && (t >= t_lo) && (t <= t_end) && (t < L);
+            // ragged launch: a row at or past its utterance's length (in this block's input rows) is stored as zeros, so
+            // that the next block's taps read there what TMA's zero fill gives a launch over the utterance alone
+            live[h] = !(a.lengths && b < a.win.B) || t < (min(max(__ldg(a.lengths + b), 0), L >> a.len_shift) << a.len_shift);
+            // a row reads input rows of its own utterance only, so one input scale per row; both scales are powers of two
+            inv_s[h] = a.inv_scale * ((a.in_inv && b < a.win.B) ? __ldg(a.in_inv + b) : 1.f);
+        }
+#pragma unroll
+        for (int q = 0; q < NG; ++q) {
+            const float2 bi2 = *reinterpret_cast<const float2*>(s_bias + 8 * q + 2 * j);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                acc[4 * q + 2 * h] = fmaf(acc[4 * q + 2 * h], inv_s[h], bi2.x);
+                acc[4 * q + 2 * h + 1] = fmaf(acc[4 * q + 2 * h + 1], inv_s[h], bi2.y);
             }
         }
-        named_sync(1, 256);                                              // accumulator tile complete in shared memory
-    }
-    if (epi) {
-        // =========================== epilogue: thread == tile row ===========================
-        const int r = threadIdx.x - 128;
-        const float* arow = s_acc + (size_t)r * acc_ld;
-        auto ld16 = [&](int c, float (&v)[16]) {
-#pragma unroll
-            for (int i = 0; i < 16; i += 4) {
-                const float4 x = *reinterpret_cast<const float4*>(arow + c + i);
-                v[i] = x.x; v[i + 1] = x.y; v[i + 2] = x.z; v[i + 3] = x.w;
-            }
-        };
-        const int bi = r / a.TT, ti = r - bi * a.TT;
-        const int n1 = (a.mode == 0) ? min(max(a.C - rank * bn, 0), bn) : half;
-        if (r == 0) { dbg_mark(a.dbg, 5, 1); dbg_time(a.dbg, 10); }       // t2: accumulator complete (main loop over)
+        const int n1 = (a.mode == 0) ? min(max(a.C - rank * bn, 0), bn) : HALF;
 
-        const int b = b0s + bi, t = t0s + ti;
-        const bool row_ok = (b < a.win.B) && (t >= t_lo) && (t <= t_end) && (t < L);
-        // ragged launch: a row at or past its utterance's length (in this block's input rows) is stored as zeros, so that the
-        // next block's taps read there what TMA's zero fill gives a launch over the utterance alone
-        const bool live = !(a.lengths && b < a.win.B) ||
-                          t < (min(max(__ldg(a.lengths + b), 0), L >> a.len_shift) << a.len_shift);
-        // a row reads input rows of its own utterance only, so one input scale per row; both scales are powers of two
-        const float in_s = (a.in_inv && b < a.win.B) ? __ldg(a.in_inv + b) : 1.f;
-        const float inv_s = a.inv_scale * in_s;
-
-        // ONE statistics sweep: shifted sums about a pivot taken from the row itself, so that M2 = Q - S^2/n does not cancel
-        float s1, s2 = 0.f, q1, q2 = 0.f, m1, m2 = 0.f;
-        {
-            float piv = 0.f, S = 0.f, Q = 0.f;
-            for (int c = 0; c < n1; c += 16) {
-                float v[16];
-                ld16(c, v);
-                if (c == 0) piv = fmaf(v[0], inv_s, s_bias[0]);
+        float s1[2], q1[2], s2[2] = {0.f, 0.f}, q2[2] = {0.f, 0.f};
 #pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                    const int cc = c + i;
-                    if (cc < n1) { const float d = fmaf(v[i], inv_s, s_bias[cc]) - piv; S += d; Q = fmaf(d, d, Q); }
-                }
-            }
-            const float n = (float)max(n1, 1);
-            s1 = piv * (float)n1 + S; m1 = n1 > 0 ? s1 / n : 0.f; q1 = fmaxf(Q - S * S / n, 0.f);
-        }
-        if (a.mode != 0) {
-            float piv = 0.f, S = 0.f, Q = 0.f;
-            for (int c = 0; c < half; c += 16) {
-                float v[16];
-                ld16(half + c, v);
-                if (c == 0) piv = fmaf(v[0], inv_s, s_bias[half]);
-#pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                    const int cc = c + i;
-                    if (cc < half) { const float d = fmaf(v[i], inv_s, s_bias[half + cc]) - piv; S += d; Q = fmaf(d, d, Q); }
-                }
-            }
-            s2 = piv * (float)half + S; m2 = s2 / (float)half; q2 = fmaxf(Q - S * S / (float)half, 0.f);
+        for (int h = 0; h < 2; ++h) {
+            if (a.mode == 0) row_stats<0, NG>(acc, h, j, n1, s1[h], q1[h]);
+            else { row_stats<0, HG>(acc, h, j, HALF, s1[h], q1[h]); row_stats<HG, HG>(acc, h, j, HALF, s2[h], q2[h]); }
         }
         // combine over the cluster
-        float mean1, rstd1, mean2 = 0.f, rstd2 = 0.f;
+        float mean1[2], rstd1[2], mean2[2] = {0.f, 0.f}, rstd2[2] = {0.f, 0.f};
         if (ncta > 1) {
             // each CTA publishes its partials in its OWN shared memory; after the cluster barrier every CTA reads
             // the slices' partials through distributed shared memory
-            s_part[r] = make_float4(s1, q1, s2, q2);
-            if (r == 0) { dbg_mark(a.dbg, 6, 1); dbg_time(a.dbg, 11); }   // t3: statistics sweep done, partials published
+            if (j == 0) {
+                s_part[rt] = make_float4(s1[0], q1[0], s2[0], q2[0]);
+                s_part[rt + 8] = make_float4(s1[1], q1[1], s2[1], q2[1]);
+            }
+            if (threadIdx.x == 128) { dbg_mark(a.dbg, 6, 1); dbg_time(a.dbg, 11); }   // t3: statistics done, partials published
             cluster_arrive();                                              // phase 2: partials published
             cluster_wait();
-            if (r == 0) { dbg_mark(a.dbg, 7, 1); dbg_time(a.dbg, 12); }   // t4: cluster barrier passed
-            const uint32_t my_slot = smem_u32(&s_part[r]);
-            float4 pv[MAXC];
+            if (threadIdx.x == 128) { dbg_mark(a.dbg, 7, 1); dbg_time(a.dbg, 12); }   // t4: cluster barrier passed
 #pragma unroll
-            for (int p = 0; p < MAXC; ++p) pv[p] = (p < nslices) ? ld_cluster_f4(mapa(my_slot, (uint32_t)p)) : make_float4(0.f, 0.f, 0.f, 0.f);
-            float S1 = 0.f, S2 = 0.f;
+            for (int h = 0; h < 2; ++h) {
+                const uint32_t my_slot = smem_u32(&s_part[rt + 8 * h]);
+                float4 pv[MAXC];
 #pragma unroll
-            for (int p = 0; p < MAXC; ++p) if (p < nslices) { S1 += pv[p].x; S2 += pv[p].z; }
-            mean1 = S1 / (float)a.C; mean2 = S2 / (float)a.C;
-            float M1 = 0.f, M2 = 0.f;
+                for (int p = 0; p < MAXC; ++p) pv[p] = (p < nslices) ? ld_cluster_f4(mapa(my_slot, (uint32_t)p)) : make_float4(0.f, 0.f, 0.f, 0.f);
+                float S1 = 0.f, S2 = 0.f;
 #pragma unroll
-            for (int p = 0; p < MAXC; ++p) {
-                if (p >= nslices) continue;
-                const float4 v = pv[p];
-                const int np = (a.mode == 0) ? min(max(a.C - p * bn, 0), bn) : half;
-                if (np > 0) { float d = v.x / (float)np - mean1; M1 += v.y + (float)np * d * d; }
-                if (a.mode != 0) { float d = v.z / (float)half - mean2; M2 += v.w + (float)half * d * d; }
+                for (int p = 0; p < MAXC; ++p) if (p < nslices) { S1 += pv[p].x; S2 += pv[p].z; }
+                mean1[h] = S1 / (float)a.C; mean2[h] = S2 / (float)a.C;
+                float M1 = 0.f, M2 = 0.f;
+#pragma unroll
+                for (int p = 0; p < MAXC; ++p) {
+                    if (p >= nslices) continue;
+                    const float4 v = pv[p];
+                    const int np = (a.mode == 0) ? min(max(a.C - p * bn, 0), bn) : HALF;
+                    if (np > 0) { float d = v.x / (float)np - mean1[h]; M1 += v.y + (float)np * d * d; }
+                    if (a.mode != 0) { float d = v.z / (float)HALF - mean2[h]; M2 += v.w + (float)HALF * d * d; }
+                }
+                rstd1[h] = 1.0f / sqrtf(M1 / (float)a.C + 1e-12f);
+                rstd2[h] = 1.0f / sqrtf(M2 / (float)a.C + 1e-12f);
             }
-            rstd1 = 1.0f / sqrtf(M1 / (float)a.C + 1e-12f);
-            rstd2 = 1.0f / sqrtf(M2 / (float)a.C + 1e-12f);
         } else {
-            mean1 = m1; rstd1 = 1.0f / sqrtf(q1 / (float)a.C + 1e-12f);
-            mean2 = m2; rstd2 = 1.0f / sqrtf(q2 / (float)a.C + 1e-12f);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                mean1[h] = n1 > 0 ? s1[h] / (float)max(n1, 1) : 0.f; rstd1[h] = 1.0f / sqrtf(q1[h] / (float)a.C + 1e-12f);
+                mean2[h] = s2[h] / (float)HALF; rstd2[h] = 1.0f / sqrtf(q2[h] / (float)a.C + 1e-12f);
+            }
         }
 
-        // sweep 2: normalise, activate, mix, store
-        {
-            if (a.mode == 0) {
-                const size_t row = (size_t)b * L + t;
-                for (int c = 0; c < n1; c += 16) {
-                    float v[16], o[16];
-                    ld16(c, v);
-                    const int col = rank * bn + c;
+        // normalise, activate, mix, store
+        if (a.mode == 0) {
 #pragma unroll
-                    for (int i = 0; i < 16; ++i) {
-                        float z = (fmaf(v[i], inv_s, s_bias[c + i]) - mean1) * rstd1 * s_gam[c + i] + s_bet[c + i];
+            for (int q = 0; q < NG; ++q)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int c = 8 * q + 2 * j + e;
+                        float z = (acc[4 * q + 2 * h + e] - mean1[h]) * rstd1[h] * s_gam[c] + s_bet[c];
                         if (a.act == 1) z = fmaxf(z, 0.f);
-                        o[i] = (c + i < n1 && live) ? z : 0.f;
+                        acc[4 * q + 2 * h + e] = (c < n1 && live[h]) ? z : 0.f;
                     }
-                    if (row_ok && a.out.hi) store_planes(a.out, row, col, a.C, o);
-                    if (row_ok && a.out_f32) {
-                        float* p = a.out_f32 + row * a.ld_f32 + col;
+            const int col0 = rank * bn;
 #pragma unroll
-                        for (int i = 0; i < 16; ++i) if (c + i < n1) p[i] = o[i];
-                    }
-                    if (a.sig_f32 || a.sig.hi) {
+            for (int h = 0; h < 2; ++h) {
+                const size_t row = (size_t)bb[h] * L + tt[h];
+                if (a.out.hi) store_planes_frag<0, NG>(a.out, row, col0, acc, h, j, ok[h]);
+                if (ok[h] && a.out_f32) store_f32_frag<0, NG>(a.out_f32 + row * a.ld_f32, col0, n1, acc, h, j);
+            }
+            if (a.sig_f32 || a.sig.hi) {
 #pragma unroll
-                        for (int i = 0; i < 16; ++i) o[i] = (c + i < n1 && live) ? sigmoid_acc(o[i]) : 0.f;
-                        if (row_ok && a.sig.hi) store_planes(a.sig, row, col, a.C, o);
-                        if (row_ok && a.sig_f32) {
-                            float* p = a.sig_f32 + row * a.ld_sig + col;
+                for (int h = 0; h < 2; ++h)
 #pragma unroll
-                            for (int i = 0; i < 16; ++i) if (c + i < n1) p[i] = o[i];
+                    for (int q = 0; q < NG; ++q)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int c = 8 * q + 2 * j + e;
+                            acc[4 * q + 2 * h + e] = (c < n1 && live[h]) ? sigmoid_acc(acc[4 * q + 2 * h + e]) : 0.f;
                         }
-                    }
-                }
-            } else if (a.mode == 1) {
-                const size_t row = (size_t)b * L + t;
-                // residual / output staging tile: [plane][box of 64 ch][128 rows][128 B], 128B swizzle
-                const int nbox = half / 64;
-                if (a.resid_tma) mbar_wait(resid_bar, 0);
-                for (int c = 0; c < half; c += 16) {
-                    float v1[16], v2[16], o[16];
-                    const int col = rank * half + c;
-                    // highway residual: 16 channels of both planes (2 x 32 B)
-                    __align__(16) __half xh[16] = {};
-                    __align__(16) __half xl[16] = {};
-                    uint8_t* sh = rs + (c >> 6) * 16384 + r * 128;              // this row inside box c/64 (hi plane)
-                    uint8_t* sl = sh + nbox * 16384;
-                    const int k0 = (((c & 63) >> 3) ^ (r & 7)) << 4, k1 = ((((c & 63) >> 3) + 1) ^ (r & 7)) << 4;
-                    if (a.resid_tma) {
-                        reinterpret_cast<uint4*>(xh)[0] = *reinterpret_cast<const uint4*>(sh + k0);
-                        reinterpret_cast<uint4*>(xh)[1] = *reinterpret_cast<const uint4*>(sh + k1);
-                        reinterpret_cast<uint4*>(xl)[0] = *reinterpret_cast<const uint4*>(sl + k0);
-                        reinterpret_cast<uint4*>(xl)[1] = *reinterpret_cast<const uint4*>(sl + k1);
-                    } else if (row_ok) {
-                        const uint4* ph = reinterpret_cast<const uint4*>(a.X.hi + row * a.X.ld + col);
-                        const uint4* pl = reinterpret_cast<const uint4*>(a.X.lo + row * a.X.ld + col);
-                        reinterpret_cast<uint4*>(xh)[0] = __ldg(ph); reinterpret_cast<uint4*>(xh)[1] = __ldg(ph + 1);
-                        reinterpret_cast<uint4*>(xl)[0] = __ldg(pl); reinterpret_cast<uint4*>(xl)[1] = __ldg(pl + 1);
-                    }
-                    ld16(c, v1);
-                    ld16(half + c, v2);
 #pragma unroll
-                    for (int i = 0; i < 16; ++i) {
-                        float z1 = (fmaf(v1[i], inv_s, s_bias[c + i]) - mean1) * rstd1 * s_gam[c + i] + s_bet[c + i];
-                        float z2 = (fmaf(v2[i], inv_s, s_bias[half + c + i]) - mean2) * rstd2 * s_gam[half + c + i] + s_bet[half + c + i];
-                        float h1 = sigmoid_acc(z1);
-                        float x = join_f16(xh[i], xl[i]);
-                        o[i] = live ? h1 * z2 + (1.0f - h1) * x : 0.f;
+                for (int h = 0; h < 2; ++h) {
+                    const size_t row = (size_t)bb[h] * L + tt[h];
+                    if (a.sig.hi) store_planes_frag<0, NG>(a.sig, row, col0, acc, h, j, ok[h]);
+                    if (ok[h] && a.sig_f32) store_f32_frag<0, NG>(a.sig_f32 + row * a.ld_sig, col0, n1, acc, h, j);
+                }
+            }
+        } else if (a.mode == 1) {
+            // residual / output staging tile: [plane][box of 64 ch][128 rows][128 B], 128B swizzle; the pair of columns a
+            // thread holds in a row is 4 bytes of one 16-byte chunk, and the 8 rows of a warp's access hit 8 distinct chunks
+            const int nbox = HALF / 64;
+            if (a.resid_tma) mbar_wait(resid_bar, 0);
+#pragma unroll
+            for (int q = 0; q < HG; ++q) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int r = rt + 8 * h;
+                    const size_t row = (size_t)bb[h] * L + tt[h];
+                    const int c = 8 * q + 2 * j;
+                    uint8_t* sh = rs + (q >> 3) * 16384 + r * 128 + ((((q & 7) ^ (r & 7)) << 4) | (4 * j));
+                    uint8_t* sl = sh + nbox * 16384;
+                    __half2 xh = __float2half2_rn(0.f), xl = xh;
+                    if (a.resid_tma) {
+                        xh = *reinterpret_cast<const __half2*>(sh);
+                        xl = *reinterpret_cast<const __half2*>(sl);
+                    } else if (ok[h]) {
+                        xh = __ldg(reinterpret_cast<const __half2*>(a.X.hi + row * a.X.ld + rank * HALF + c));
+                        xl = __ldg(reinterpret_cast<const __half2*>(a.X.lo + row * a.X.ld + rank * HALF + c));
+                    }
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const float z1 = (acc[4 * q + 2 * h + e] - mean1[h]) * rstd1[h] * s_gam[c + e] + s_bet[c + e];
+                        const float z2 = (acc[4 * (q + HG) + 2 * h + e] - mean2[h]) * rstd2[h] * s_gam[HALF + c + e] + s_bet[HALF + c + e];
+                        const float h1 = sigmoid_acc(z1);
+                        const float x = e ? join_f16(__high2half(xh), __high2half(xl)) : join_f16(__low2half(xh), __low2half(xl));
+                        acc[4 * q + 2 * h + e] = live[h] ? h1 * z2 + (1.0f - h1) * x : 0.f;
                     }
                     if (a.out_tma) {
                         // stage the output planes in place of the residual just consumed (same swizzled slots)
-                        __align__(16) __half oh[16];
-                        __align__(16) __half ol[16];
-#pragma unroll
-                        for (int i = 0; i < 16; ++i) split_f16(o[i], oh[i], ol[i]);
-                        *reinterpret_cast<uint4*>(sh + k0) = reinterpret_cast<const uint4*>(oh)[0];
-                        *reinterpret_cast<uint4*>(sh + k1) = reinterpret_cast<const uint4*>(oh)[1];
-                        *reinterpret_cast<uint4*>(sl + k0) = reinterpret_cast<const uint4*>(ol)[0];
-                        *reinterpret_cast<uint4*>(sl + k1) = reinterpret_cast<const uint4*>(ol)[1];
-                    } else if (row_ok && a.out.hi) {
-                        store_planes(a.out, row, col, a.C, o);
-                    }
-                    if (row_ok && a.out_f32) {
-                        float* p = a.out_f32 + row * a.ld_f32 + col;
-#pragma unroll
-                        for (int i = 0; i < 16; ++i) p[i] = o[i];
-                    }
-                }
-                if (a.out_tma) {
-                    // whole tile staged: one thread hands it to the TMA engine (rows past the end are clipped)
-                    fence_proxy_async_smem();
-                    named_sync(2, 128);                                          // the epilogue warpgroup only
-                    if (r == 0) {
-                        for (int i = 0; i < nbox; ++i) {
-                            tma_store_3d(&mapO_hi, rs + i * 16384, rank * half + i * 64, t0s, b0s);
-                            tma_store_3d(&mapO_lo, rs + (nbox + i) * 16384, rank * half + i * 64, t0s, b0s);
-                        }
-                        tma_store_commit_and_wait();
-                    }
-                }
-            } else {
-                // transposed conv: first half -> output row 2t, second half -> row 2t+1 (modules.py:232-241)
-                const size_t row_e = (size_t)b * (2 * L) + 2 * (size_t)t;
-                for (int hsel = 0; hsel < 2; ++hsel) {
-                    const float mean = hsel ? mean2 : mean1, rstd = hsel ? rstd2 : rstd1;
-                    for (int c = 0; c < half; c += 16) {
-                        float v[16], o[16];
-                        ld16(hsel * half + c, v);
-                        const int col = rank * half + c;
-#pragma unroll
-                        for (int i = 0; i < 16; ++i) {
-                            const int ac = hsel * half + c + i;
-                            o[i] = live ? (fmaf(v[i], inv_s, s_bias[ac]) - mean) * rstd * s_gam[ac] + s_bet[ac] : 0.f;
-                        }
-                        if (row_ok && a.out.hi) store_planes(a.out, row_e + hsel, col, a.C, o);
-                        if (row_ok && a.out_f32) {
-                            float* p = a.out_f32 + (row_e + hsel) * a.ld_f32 + col;
-#pragma unroll
-                            for (int i = 0; i < 16; ++i) p[i] = o[i];
-                        }
+                        __half2 oh, ol;
+                        split_f16x2(make_float2(acc[4 * q + 2 * h], acc[4 * q + 2 * h + 1]), oh, ol);
+                        *reinterpret_cast<__half2*>(sh) = oh;
+                        *reinterpret_cast<__half2*>(sl) = ol;
                     }
                 }
             }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const size_t row = (size_t)bb[h] * L + tt[h];
+                if (!a.out_tma && a.out.hi) store_planes_frag<0, HG>(a.out, row, rank * HALF, acc, h, j, ok[h]);
+                if (ok[h] && a.out_f32) store_f32_frag<0, HG>(a.out_f32 + row * a.ld_f32, rank * HALF, HALF, acc, h, j);
+            }
+            if (a.out_tma) {
+                // whole tile staged: one thread hands it to the TMA engine (rows past the end are clipped)
+                fence_proxy_async_smem();
+                named_sync(1, 256);                                          // both consumer warpgroups
+                if (threadIdx.x == 128) {
+                    for (int i = 0; i < nbox; ++i) {
+                        tma_store_3d(&mapO_hi, rs + i * 16384, rank * HALF + i * 64, t0s, b0s);
+                        tma_store_3d(&mapO_lo, rs + (nbox + i) * 16384, rank * HALF + i * 64, t0s, b0s);
+                    }
+                    tma_store_commit_and_wait();
+                }
+            }
+        } else {
+            // transposed conv: first half -> output row 2t, second half -> row 2t+1 (modules.py:232-241)
+#pragma unroll
+            for (int q = 0; q < NG; ++q)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int c = 8 * q + 2 * j + e;
+                        const float mean = q < HG ? mean1[h] : mean2[h], rstd = q < HG ? rstd1[h] : rstd2[h];
+                        acc[4 * q + 2 * h + e] = live[h] ? (acc[4 * q + 2 * h + e] - mean) * rstd * s_gam[c] + s_bet[c] : 0.f;
+                    }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const size_t row_e = (size_t)bb[h] * (2 * L) + 2 * (size_t)tt[h];
+                if (a.out.hi) {
+                    store_planes_frag<0, HG>(a.out, row_e, rank * HALF, acc, h, j, ok[h]);
+                    store_planes_frag<HG, HG>(a.out, row_e + 1, rank * HALF, acc, h, j, ok[h]);
+                }
+                if (ok[h] && a.out_f32) {
+                    store_f32_frag<0, HG>(a.out_f32 + row_e * a.ld_f32, rank * HALF, HALF, acc, h, j);
+                    store_f32_frag<HG, HG>(a.out_f32 + (row_e + 1) * a.ld_f32, rank * HALF, HALF, acc, h, j);
+                }
+            }
         }
-        if (r == 0) dbg_time(a.dbg, 13);                                  // t5: stores issued
+        if (threadIdx.x == 128) dbg_time(a.dbg, 13);                      // t5: stores issued
     }
 
-    // ---- teardown: the other warps match the epilogue's cluster barrier phase ----
+    // ---- teardown: the producer warpgroup matches the consumers' cluster barrier phase ----
     if (ncta > 1) {
-        if (!epi) { cluster_arrive(); cluster_wait(); }
+        if (wg == 0) { cluster_arrive(); cluster_wait(); }
         cluster_arrive();                     // last phase: nobody reads my shared memory any more
         cluster_wait();
     }
@@ -597,14 +644,14 @@ void tc_make_w_map(CUtensorMap* m, const __half* base, int Ktot, int Nrows, int 
 }
 
 int tc_bk() {
-    // 32-wide slabs (64-byte swizzle): the fp32 accumulator tile of a 256-column block (130 KB) and the highway residual tile
-    // (64 KB) leave room for two or more 48 KB stages, where 64-wide stages would fit only one
+    // 32-wide slabs (64-byte swizzle): beside the highway residual tile (64 KB) of a 256-column block there is room for three
+    // 48 KB stages, where 64-wide stages (96 KB) would fit only one
     return 32;
 }
 
 static size_t conv_ln_smem(int stages, int bn, int half, int resid_tma, int bk) {
     const int stage = 2 * TC_BM * bk * 2 + 2 * bn * bk * 2;
-    return (size_t)tc_ring_bytes(stages, stage, bn) + tc_resid_bytes(resid_tma, half) + TC_AUX_BYTES + 1024;
+    return (size_t)tc_ring_bytes(stages, stage) + tc_resid_bytes(resid_tma, half) + TC_AUX_BYTES + 1024;
 }
 
 int tc_stages_for(int bn, int bk, int resid_tma, int half) {      // bn = accumulator columns per CTA
@@ -671,6 +718,7 @@ void launch_conv_ln_tc(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const C
     if (ncta > tc_max_cluster(a.bn))
         throw std::runtime_error("conv_ln_tc: a cluster of " + std::to_string(ncta) + " CTAs at " + std::to_string(a.bn) +
                                  " columns (16 at 144 columns, else 8 at most)");
+    if (a.mode != 0 && 2 * a.half != a.bn) throw std::runtime_error("conv_ln_tc: hc and transposed blocks hold two halves of bn / 2 columns");
     const ConvLnKernel kern = conv_ln_kernel_ready(bk, a.bn);
     const size_t smem = conv_ln_smem(a.stages, a.bn, a.half, a.resid_tma, bk);
     if (smem > (size_t)TC_MAX_SMEM) throw std::runtime_error("conv_ln_tc: shared memory budget exceeded");
