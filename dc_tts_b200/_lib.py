@@ -73,6 +73,7 @@ SIGNATURES = {
     "dctts_train_grads": (C.c_int, [Handle, C.POINTER(_p), C.POINTER(_i64)]),
     "dctts_train_tensor": (C.c_int, [Handle, C.c_char_p, _i32, _p, _i64]),
     "dctts_train_set_tensor": (C.c_int, [Handle, C.c_char_p, _i32, _p, _i64]),
+    "dctts_refresh_synthesis": (C.c_int, [Handle, _p]),
     "dctts_reserve": (C.c_int, [Handle, _i32]),
     "dctts_launch_count": (_i64, [Handle]),
     "dctts_crc32c": (C.c_uint32, [C.c_uint32, _p, _i64]),

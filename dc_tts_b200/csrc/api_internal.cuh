@@ -53,7 +53,6 @@ struct LayerDev {
     int act = 0;
     int nconv = 0, ldw = 0;
     float* W = nullptr;      // [size][cin][ldw]
-    std::vector<float> hostW;   // same, kept on the host until the decode stream is packed (AudioEnc / AudioDec only)
     float* bias = nullptr;   // [ldw]
     float *g1 = nullptr, *b1 = nullptr, *g2 = nullptr, *b2 = nullptr;
     // tensor-core path: split-fp16 K-major weight planes [ncta*bn][ntaps*cin_pad], pre-scaled
@@ -114,6 +113,10 @@ struct dctts_handle_s {
     std::map<std::string, float*> dev_vec;    // every committed variable (flat copy) by TF name
     std::deque<DevBuf> param_bufs;            // every committed parameter plane; a deque keeps the pointers that tensor maps and DecParams hold
     float* embed_table = nullptr;
+    DevBuf pack_max;              // weight packing (kernels_pack.cu): every layer's max |W| (float bits)
+    // the variables changed since the planes and the decode stream were packed (mark_synthesis_stale): synthesis runs on
+    // the fp32 kernels with the graph-per-frame decode until dctts_refresh_synthesis packs them again
+    bool synth_stale = false;
 
     // workspace (sized for ws_B utterances)
     int ws_B = 0;
@@ -194,6 +197,9 @@ struct dctts_handle_s {
     // persistent decode (kernels_decode.cu)
     struct {
         bool ok = false;          // stream packed, geometry supported, 16-CTA clusters schedulable
+        bool tables_ok = false;   // geometry supported: the tables are built and the stream allocated
+        bool commit_ok = false;   // ok / why as commit left them: what a refresh restores
+        std::string commit_why;
         DecParams tab{};          // layer / chunk tables (+ parameter pointers); per-call fields filled by text2mel_generate
         DevBuf wstream, lnp, scr, stats, pfinal, prof, pl, frames;
         int max_clusters = 0;
@@ -254,6 +260,8 @@ inline cudaStream_t S(dctts_handle, void* s) { return reinterpret_cast<cudaStrea
 
 // ---------------------------------------------------------------------------- called across stages
 void build_tables(H* h);                                                          // api_params.cu
+void pack_weights(H* h, cudaStream_t s);
+void mark_synthesis_stale(H* h);
 std::vector<int> audiodec_rows(const std::vector<LayerDev>& net, int T);          // api_synth.cu
 void settle_decode_counts(H* h);
 void drop_ar_graph(H* h);

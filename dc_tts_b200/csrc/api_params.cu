@@ -1,4 +1,5 @@
-// api_params.cu -- layer tables; parameter staging, split-fp16 packing and the persistent decode's weight stream.
+// api_params.cu -- layer tables; parameter staging and commit; the geometry of the split-fp16 planes and of the persistent
+// decode's weight stream, and their packing on the device (kernels_pack.cu).
 // Reference mapping: layer tables networks.py:23-68 (TextEnc), :81-124 (AudioEnc), :166-209 (AudioDec), :223-290 (SSRN)
 #include "api_internal.cuh"
 #include "numerics.cuh"
@@ -99,11 +100,11 @@ float* upload_vec(H* h, const std::string& name, int n, int padded) {
     return d;
 }
 
-// Split-fp16 packing for the wgmma kernel (kernels_tc.cu).  Rows are accumulator columns in
-// cluster-slice order (CTA i owns rows [i*bn, (i+1)*bn); for hc / transposed conv its first
-// `half` rows are the first LN half, the rest the second), columns are k = tap*cin_pad + ci.
-// Weights are multiplied by weight_scale (numerics.cuh); the kernel multiplies the accumulator back.
-void pack_tc(H* h, LayerDev& l, const std::vector<float>& W /* [size][cin][ldw] */) {
+// Split-fp16 planes for the wgmma kernel (kernels_tc.cu): the geometry, the two planes and their tensor maps.  Rows are
+// accumulator columns in cluster-slice order (CTA i owns rows [i*bn, (i+1)*bn); for hc / transposed conv its first
+// `half` rows are the first LN half, the rest the second), columns are k = tap*cin_pad + ci.  pack_weights fills them
+// with the weights multiplied by weight_scale (numerics.cuh); the kernel multiplies the accumulator back.
+void tc_tables(H* h, LayerDev& l) {
     LayerDev::TcPack& p = l.tc;
     const int cin_pad = roundup(l.cin, 64);
     p.kb_per_tap = cin_pad / 64;
@@ -129,31 +130,11 @@ void pack_tc(H* h, LayerDev& l, const std::vector<float>& W /* [size][cin][ldw] 
         if (h->tc16_clusters < 1) return;
     }
     p.Ktot = p.ntaps * cin_pad; p.nrows = p.ncta * p.bn;
-    auto wv = [&](int tap, int ci, int row) -> float {
-        const int i = row / p.bn, a = row % p.bn;
-        if (p.mode == 0) return row < l.cout ? W[((size_t)tap * l.cin + ci) * l.ldw + row] : 0.f;
-        const bool second = a >= p.half;
-        const int col = i * p.half + (a % p.half);
-        if (p.mode == 1) return W[((size_t)tap * l.cin + ci) * l.ldw + (second ? l.cout + col : col)];
-        // transposed conv: k-tap 0 reads x[t] (W0 -> even rows, W1 -> odd rows), k-tap 1 reads x[t-1] (W2 -> even rows)
-        if (tap == 0) return W[((size_t)(second ? 1 : 0) * l.cin + ci) * l.ldw + col];
-        return second ? 0.f : W[((size_t)2 * l.cin + ci) * l.ldw + col];
-    };
-    float maxabs = 0.f;
-    for (int tap = 0; tap < p.ntaps; ++tap)
-        for (int ci = 0; ci < l.cin; ++ci)
-            for (int row = 0; row < p.nrows; ++row) maxabs = std::max(maxabs, std::fabs(wv(tap, ci, row)));
-    const float scale = weight_scale(maxabs);
-    p.inv_scale = 1.f / scale;
-    std::vector<__half> hi((size_t)p.nrows * p.Ktot, __float2half_rn(0.f)), lo(hi);
-    for (int row = 0; row < p.nrows; ++row)
-        for (int tap = 0; tap < p.ntaps; ++tap)
-            for (int ci = 0; ci < l.cin; ++ci) {
-                const size_t idx = (size_t)row * p.Ktot + (size_t)tap * cin_pad + ci;
-                split_f16(wv(tap, ci, row) * scale, hi[idx], lo[idx]);
-            }
-    p.Whi = upload(h, hi);
-    p.Wlo = upload(h, lo);
+    const size_t bytes = (size_t)p.nrows * p.Ktot * sizeof(__half);
+    DevBuf& hi = h->param_bufs.emplace_back();
+    DevBuf& lo = h->param_bufs.emplace_back();
+    hi.ensure(bytes); lo.ensure(bytes);
+    p.Whi = hi.as<__half>(); p.Wlo = lo.as<__half>();
     tc_make_w_map(&p.mWhi, p.Whi, p.Ktot, p.nrows, p.bn, tc_bk());
     tc_make_w_map(&p.mWlo, p.Wlo, p.Ktot, p.nrows, p.bn, tc_bk());
     p.ok = true;
@@ -180,8 +161,7 @@ void commit_layer(H* h, LayerDev& l) {
         h->n_params += (int64_t)k * cin * nconv;
     }
     l.W = upload(h, W);
-    if (l.scope.compare(0, 14, "Text2Mel/Audio") == 0) l.hostW = W;
-    pack_tc(h, l, W);
+    tc_tables(h, l);
     if (l.kind == K_HC) {
         l.g1 = upload_vec(h, l.scope + "/H1/gamma", l.cout, l.cout);
         l.b1 = upload_vec(h, l.scope + "/H1/beta", l.cout, l.cout);
@@ -198,10 +178,10 @@ void commit_layer(H* h, LayerDev& l) {
 // Stream of rank r = for every block of AudioEnc then AudioDec, for every tap, for every chunk of <= 4096 floats:
 // the block's weight columns owned by rank r ([k/4][column][4]).  hc blocks: columns [0, cs) are the gate
 // channels r*cs.., [cs, 2cs) the info channels of the same index (modules.py:188-193); conv blocks: cs columns
-// (+ zero columns up to a multiple of 4).
-void pack_decode(H* h) {
+// (+ zero columns up to a multiple of 4).  The tables depend on the shapes only; pack_weights writes the stream.
+void decode_tables(H* h) {
     auto& D = h->dec;
-    D.ok = false;
+    D.ok = false; D.tables_ok = false;
     const dctts_hparams& hp = h->hp;
     const int d = hp.d;
     if (d != 256) { D.why = "persistent decode needs d = 256"; return; }
@@ -264,80 +244,24 @@ void pack_decode(H* h) {
         for (int c = L.ch0; c < L.ch0 + L.nch; ++c) { P.C[c].off16 = off; off += L.krows * L.ns; }
     }
     P.stream_len = off;
-    // streams: chunk = 8 warp regions, region w = rows [w*kr8, (w+1)*kr8) as [k/4][column][4] (32-column slices: pair-split, below)
-    std::vector<float> st((size_t)DEC_NC * off, 0.f);
-    for (int li = 0; li < P.nl; ++li) {                              // power-of-two scale per receptive-field block (as pack_tc)
-        const LayerDev& l = *nets[li]; const DecLayer& L = P.L[li];
-        P.inv_scale[li] = 1.f;
-        if (L.prow <= 1) continue;
-        float maxabs = 0.f;
-        for (size_t i = 0; i < l.hostW.size(); ++i) maxabs = std::max(maxabs, std::fabs(l.hostW[i]));
-        P.inv_scale[li] = 1.f / weight_scale(maxabs);
-    }
-    for (int r = 0; r < DEC_NC; ++r)
-        for (int li = 0; li < P.nl; ++li) {
-            const LayerDev& l = *nets[li]; const DecLayer& L = P.L[li];
-            REQUIRE(!l.hostW.empty(), "persistent decode: host weights missing");
-            const int cinp = roundup(l.cin, 128), kr8 = L.krows / 8;
-            auto column = [&](int n) -> int {
-                if (L.kind) return n < L.cs ? r * L.cs + n : l.cout + r * L.cs + (n - L.cs);
-                return n < L.cs ? r * L.cs + n : -1;
-            };
-            for (int c = L.ch0; c < L.ch0 + L.nch; ++c) {
-                const DecChunk& ch = P.C[c];
-                float* dst = st.data() + (size_t)r * off + ch.off;
-                for (int kc = 0; kc < ch.krows; ++kc) {
-                    const int k = ch.k0 + kc, tap = k / cinp, ci = k % cinp;
-                    if (ci >= l.cin) continue;
-                    const int w = kc / kr8, kk = kc % kr8;
-                    const float* wrow = l.hostW.data() + ((size_t)tap * l.cin + ci) * l.ldw;
-                    for (int n = 0; n < L.ns; ++n) {
-                        const int col = column(n);
-                        if (col < 0) continue;
-                        // 32-column slices: pair-split layout per 8-k block [column parity][k-group][column pair][4 k]
-                        // (gemv_warp32); narrower slices: [k/4][column][4]
-                        const size_t idx = L.ns == 32 ? (size_t)(kk / 8) * 256 + ((size_t)((n & 1) * 2 + (kk / 4) % 2) * 16 + (n >> 1)) * 4 + (kk % 4)
-                                                      : ((size_t)(kk / 4) * L.ns + n) * 4 + (kk % 4);
-                        dst[(size_t)w * kr8 * L.ns + idx] = wrow[col];
-                    }
-                }
-                if (L.prow <= 1) continue;
-                // the same rows as MMA slabs of 16 k: [plane hi | lo][k8 group][column][8 halfs], 16*ns floats per slab, in k order
-                // (slab s of the chunk sits at float offset s*16*ns: region w of the chunk = slabs [w*spr, (w+1)*spr))
-                __half* d16 = reinterpret_cast<__half*>(st.data() + (size_t)r * off + ch.off16);
-                const float scale = 1.f / P.inv_scale[li];
-                for (int kc = 0; kc < ch.krows; ++kc) {
-                    const int k = ch.k0 + kc, tap = k / cinp, ci = k % cinp;
-                    const int slab = kc / 16, k16 = kc % 16, grp = k16 / 8, e8 = k16 % 8;
-                    const float* wrow = l.hostW.data() + ((size_t)tap * l.cin + ci) * l.ldw;
-                    for (int n = 0; n < L.ns; ++n) {
-                        const int col = column(n);
-                        const float v = (col >= 0 && ci < l.cin) ? wrow[col] * scale : 0.f;
-                        const size_t base = (size_t)slab * 32 * L.ns;                  // halfs per slab = 2 planes * 2 groups * ns * 8
-                        const size_t idx = ((size_t)grp * L.ns + n) * 8 + e8;
-                        split_f16(v, d16[base + idx], d16[base + (size_t)2 * L.ns * 8 + idx]);
-                    }
-                }
-            }
-        }
-    D.wstream.ensure(st.size() * sizeof(float));
-    CUDA_CHECK(cudaMemcpy(D.wstream.p, st.data(), st.size() * sizeof(float), cudaMemcpyHostToDevice));
-    // LayerNorm parameters [layer][gamma1 | beta1 | gamma2 | beta2][256]
+    D.wstream.ensure((size_t)DEC_NC * off * sizeof(float));
+    P.wstream = D.wstream.as<float>();
+    // LayerNorm parameters [layer][gamma1 | beta1 | gamma2 | beta2][256]; pack_weights copies them in
     D.lnp.ensure((size_t)P.nl * 1024 * sizeof(float));
     CUDA_CHECK(cudaMemset(D.lnp.p, 0, D.lnp.bytes));
-    for (int li = 0; li < P.nl; ++li) {
-        const LayerDev& l = *nets[li];
-        float* base = D.lnp.as<float>() + (size_t)li * 1024;
-        const float* src[4] = {l.g1, l.b1, l.kind == K_HC ? l.g2 : nullptr, l.kind == K_HC ? l.b2 : nullptr};
-        for (int q = 0; q < 4; ++q)
-            if (src[q]) CUDA_CHECK(cudaMemcpy(base + q * 256, src[q], (size_t)l.cout * sizeof(float), cudaMemcpyDeviceToDevice));
-        P.lnp[li] = base; P.bias[li] = l.bias;
-    }
-    P.wstream = D.wstream.as<float>();
-    for (auto* lp : nets) { lp->hostW.clear(); lp->hostW.shrink_to_fit(); }
+    for (int li = 0; li < P.nl; ++li) { P.lnp[li] = D.lnp.as<float>() + (size_t)li * 1024; P.bias[li] = nets[li]->bias; }
+    D.tables_ok = true;
     D.max_clusters = decode_max_active_clusters();
     if (D.max_clusters < 1) { D.why = "persistent decode: a 16-CTA cluster with " + std::to_string(decode_smem_bytes()) + " B of shared memory cannot be scheduled"; return; }
     D.ok = true; D.why.clear();
+}
+
+// every layer, in the order of the abs-max table: TextEnc, AudioEnc, AudioDec, SSRN
+std::vector<LayerDev*> all_layers(H* h) {
+    std::vector<LayerDev*> v;
+    for (auto* vec : {&h->textenc, &h->audioenc, &h->audiodec, &h->ssrn})
+        for (auto& l : *vec) v.push_back(&l);
+    return v;
 }
 
 void commit_params(H* h) {
@@ -362,12 +286,63 @@ void commit_params(H* h) {
         }
         throw std::runtime_error("staged variable count does not match the path's variable set");
     }
-    pack_decode(h);
+    decode_tables(h);
+    h->dec.commit_ok = h->dec.ok; h->dec.commit_why = h->dec.why;
+    pack_weights(h, nullptr);
     h->staged.clear();
     h->committed = true;
 }
 
 }  // namespace
+
+// The wgmma planes of every block that has them and the persistent decode's weight stream and LayerNorm parameters,
+// packed on the device from the layers' fp32 variables as they are now (kernels_pack.cu).  One abs-max reduction over
+// every layer, read back, gives the power-of-two scales the host tables hold (LayerDev::TcPack::inv_scale,
+// DecParams::inv_scale).  Writes nothing but those planes, that stream and the abs-max slots; synchronises `s`.
+void dctts::api::pack_weights(H* h, cudaStream_t s) {
+    const std::vector<LayerDev*> layers = all_layers(h);
+    const int n = (int)layers.size();
+    REQUIRE(n <= PACK_MAXL, "pack_weights: more layers than one abs-max launch takes");
+    PackMaxTable t{};
+    for (int i = 0; i < n; ++i) { t.W[i] = layers[i]->W; t.n[i] = (long long)layers[i]->size * layers[i]->cin * layers[i]->ldw; }
+    t.count = n;
+    CUDA_CHECK(cudaMemsetAsync(h->pack_max.p, 0, (size_t)n * sizeof(unsigned), s));
+    launch_weight_absmax(t, h->pack_max.as<unsigned>(), s);
+    std::vector<float> maxabs((size_t)n);
+    CUDA_CHECK(cudaMemcpyAsync(maxabs.data(), h->pack_max.p, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, s));
+    CUDA_CHECK(cudaStreamSynchronize(s));
+    for (int i = 0; i < n; ++i) {
+        LayerDev& l = *layers[i];
+        LayerDev::TcPack& p = l.tc;
+        if (!p.ok) continue;
+        const float scale = weight_scale(maxabs[i]);
+        p.inv_scale = 1.f / scale;
+        launch_pack_tc(TcPackArgs{l.W, p.Whi, p.Wlo, p.mode, l.cin, l.cout, l.ldw, roundup(l.cin, 64), p.Ktot, p.nrows, p.bn,
+                                  p.half, scale}, s);
+    }
+    auto& D = h->dec;
+    if (D.tables_ok) {
+        DecParams& P = D.tab;
+        const int first = (int)h->textenc.size();                 // AudioEnc's first block in `layers`
+        CUDA_CHECK(cudaMemsetAsync(D.wstream.p, 0, (size_t)DEC_NC * P.stream_len * sizeof(float), s));
+        for (int li = 0; li < P.nl; ++li) {
+            const LayerDev& l = *layers[first + li];
+            const DecLayer& L = P.L[li];
+            // power-of-two scale of the receptive-field blocks' MMA slabs, as for the block planes
+            P.inv_scale[li] = L.prow > 1 ? 1.f / weight_scale(maxabs[first + li]) : 1.f;
+            const int cinp = roundup(l.cin, 128);
+            launch_pack_decode(DecPackArgs{l.W, D.wstream.as<float>(), P.stream_len, L.kind, l.cin, l.cout, l.ldw, cinp, l.size * cinp,
+                                           L.krows, L.ns, L.cs, P.C[L.ch0].off, P.C[L.ch0].off16,
+                                           L.prow > 1 ? 1.f / P.inv_scale[li] : 0.f}, s);
+            const float* src[4] = {l.g1, l.b1, l.kind == K_HC ? l.g2 : nullptr, l.kind == K_HC ? l.b2 : nullptr};
+            for (int q = 0; q < 4; ++q)
+                if (src[q]) CUDA_CHECK(cudaMemcpyAsync(D.lnp.as<float>() + (size_t)li * 1024 + q * 256, src[q], (size_t)l.cout * sizeof(float),
+                                                        cudaMemcpyDeviceToDevice, s));
+        }
+    }
+    CUDA_CHECK(cudaGetLastError());
+    CUDA_CHECK(cudaStreamSynchronize(s));
+}
 
 extern "C" {
 
@@ -386,5 +361,18 @@ int dctts_set_param(dctts_handle h, const char* tf_name, const float* data, cons
 int dctts_commit_params(dctts_handle h) { return guarded(h, [&] { commit_params(h); }); }
 
 int64_t dctts_num_params(dctts_handle h) { return (h && h->committed) ? h->n_params : -1; }
+
+int dctts_refresh_synthesis(dctts_handle h, void* stream) {
+    return guarded(h, [&] {
+        REQUIRE(h->committed, "dctts_refresh_synthesis: parameters not committed");
+        if (!h->synth_stale) return;
+        pack_weights(h, S(h, stream));
+        CUDA_CHECK(cudaDeviceSynchronize());          // a replay of the captured AR step may still be in flight on another stream
+        drop_ar_graph(h);
+        h->tensor_path = 1;
+        h->dec.ok = h->dec.commit_ok; h->dec.why = h->dec.commit_why;
+        h->synth_stale = false;
+    });
+}
 
 }  // extern "C"

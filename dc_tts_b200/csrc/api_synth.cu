@@ -958,7 +958,7 @@ int dctts_reserve(dctts_handle h, int32_t max_batch) {
 int dctts_set_tensor_path(dctts_handle h, int32_t mode) {
     return guarded(h, [&] {
         REQUIRE(mode == 0 || mode == 1, "dctts_set_tensor_path: mode must be 0 or 1");
-        REQUIRE(!(h->tr.ready && mode == 1), "dctts_set_tensor_path: this handle has been trained -- its packed fp16 weight planes "
+        REQUIRE(!(h->synth_stale && mode == 1), "dctts_set_tensor_path: this handle has been trained -- its packed fp16 weight planes "
                 "are stale; load the trained variables (dctts_train_tensor) into a new handle for the wgmma kernel set");
         if (mode != h->tensor_path && h->ar_exec) {      // the captured AR step depends on the mode
             CUDA_CHECK(cudaDeviceSynchronize());

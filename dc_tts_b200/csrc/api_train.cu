@@ -90,9 +90,7 @@ void train_init(H* h, int B, float rate, int num, int T_in) {
     auto& tr = h->tr;
     if (tr.ready && tr.B == B && tr.num == num && tr.T_in == T_in) { tr.rate = rate; return; }
     CUDA_CHECK(cudaDeviceSynchronize());
-    drop_ar_graph(h);
-    h->tensor_path = 0;            // the optimiser updates the fp32 weights only: this handle stops using the packed fp16 planes
-    h->dec.ok = false; h->dec.why = "this handle has been trained: the packed decode stream is stale";
+    mark_synthesis_stale(h);
     tr.ready = false;
     const dctts_hparams& hp = h->hp;
     tr.layers.clear(); tr.tensors.clear();
@@ -444,6 +442,7 @@ void train_eval_ssrn(H* h, const float* mels, const float* mags, int B, int T, u
 void train_apply(H* h, long long global_step, float lr, cudaStream_t s) {
     auto& tr = h->tr;
     REQUIRE(tr.ready, "dctts_train_apply: no training state");
+    mark_synthesis_stale(h);
     const double beta1 = 0.9, beta2 = 0.999, warm = 4000.0;
     const double step = (double)(global_step + 1);
     const double lr_now = (double)(lr > 0.f ? lr : 0.001f) * std::sqrt(warm) * std::min(step * std::pow(warm, -1.5), 1.0 / std::sqrt(step));   // utils.py:141-145
@@ -461,6 +460,19 @@ size_t device_index(const H::TrainTensor& t, long long i) {
 }
 
 }  // namespace
+
+// The one place a handle's synthesis is switched off its packed weights: every entry point that writes a variable calls
+// it (dctts_train_init, the optimiser update of dctts_train_step / dctts_train_step_ssrn / dctts_train_apply,
+// dctts_train_set_tensor of a variable).  The optimiser updates the fp32 weights only, so until dctts_refresh_synthesis
+// packs them again synthesis runs on the fp32 kernel set and the graph-per-frame decode, and dctts_set_tensor_path(1) is
+// refused.  Cheap when the handle is stale already; otherwise it synchronises the device once to drop the captured AR step.
+void dctts::api::mark_synthesis_stale(H* h) {
+    if (h->synth_stale) return;
+    if (h->ar_exec) { CUDA_CHECK(cudaDeviceSynchronize()); drop_ar_graph(h); }
+    h->tensor_path = 0;
+    h->dec.ok = false; h->dec.why = "this handle has been trained: the packed decode stream is stale";
+    h->synth_stale = true;
+}
 
 extern "C" {
 
@@ -635,6 +647,7 @@ int dctts_train_set_tensor(dctts_handle h, const char* tf_name, int32_t what, co
         REQUIRE(count == logical, "dctts_train_set_tensor: element count mismatch");
         float* dst = what == 0 ? t.p : what == 2 ? t.m : t.v;
         CUDA_CHECK(cudaDeviceSynchronize());
+        if (what == 0) mark_synthesis_stale(h);
         if (t.layout == 0) {
             CUDA_CHECK(cudaMemcpy(dst, host_in, (size_t)count * sizeof(float), cudaMemcpyHostToDevice));
             return;

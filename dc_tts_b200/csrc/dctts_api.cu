@@ -49,6 +49,7 @@ int dctts_create(const dctts_hparams* hp, int device, dctts_handle* out) {
         build_tables(h.get());
         h->tickets.ensure(64 * sizeof(int));
         CUDA_CHECK(cudaMemset(h->tickets.p, 0, 64 * sizeof(int)));
+        h->pack_max.ensure(PACK_MAXL * sizeof(unsigned));
         *out = h.release();
         return 0;
     } catch (const std::exception& e) {

@@ -260,6 +260,23 @@ int launch_conv_gemm_tc(const ConvArgs& c, GemmTcWs& ws, cudaStream_t s, GemmTcS
 bool conv_wgrad_tc_ok(const WgradArgs& w, int B, const GemmTcWs& ws);
 int launch_conv_wgrad_tc(const WgradArgs& w, int B, GemmTcWs& ws, cudaStream_t s, GemmTcSlots* io = nullptr);
 
+// ---- weight packers (kernels_pack.cu): fp32 W [tap][cin][ldw] -> wgmma planes and the persistent decode's stream ----
+constexpr int PACK_MAXL = 64;  // layers of one abs-max launch (the four networks have 54)
+struct PackMaxTable { const float* W[PACK_MAXL]; long long n[PACK_MAXL]; int count; };
+// maxbits_dev[e] = float bits of max |W| over the n[e] floats at W[e]; the caller zeroes maxbits_dev first
+void launch_weight_absmax(const PackMaxTable& t, unsigned* maxbits_dev, cudaStream_t s);
+struct TcPackArgs {           // LayerDev::TcPack's geometry; hi / lo: [nrows][Ktot]; W pre-multiplied by scale
+    const float* W; __half* hi; __half* lo;
+    int mode, cin, cout, ldw, cin_pad, Ktot, nrows, bn, half; float scale;
+};
+void launch_pack_tc(const TcPackArgs& a, cudaStream_t s);
+struct DecPackArgs {          // one decode block: K = ntaps * cinp k rows in chunks of krows at rank float offsets off (fp32) / off16 (slabs)
+    const float* W; float* stream; int stream_len;
+    int kind, cin, cout, ldw, cinp, K, krows, ns, cs, off, off16;
+    float scale;              // > 0: also the split-fp16 MMA slabs of a receptive-field block, W pre-multiplied by scale
+};
+void launch_pack_decode(const DecPackArgs& a, cudaStream_t s);
+
 // scratch_bytes bounds the split-K partial buffer of the skinny path
 GemmOut launch_conv_gemm(const ConvArgs& a, cudaStream_t s, size_t scratch_bytes, bool allow_skinny = true);
 void launch_ln_rows(const LnArgs& a, cudaStream_t s);

@@ -51,7 +51,7 @@ namespace {
 constexpr int NC = DEC_NC, GMAX = DEC_GMAX, NT = DEC_THREADS, NWARP = NT / 32;
 constexpr int XLD = 768;                       // row pitch of the input vectors: [tap0 | tap1 | current]
 constexpr int PLD = GMAX * 32 + 16;            // pitch between the ranks' slices in `pre` (16 floats of bank skew)
-constexpr int TC_RA = DEC_PL_PAD;              // pre-pass: rows per k8 group of an A slab plane (source rows per utterance, pack_decode)
+constexpr int TC_RA = DEC_PL_PAD;              // pre-pass: rows per k8 group of an A slab plane (source rows per utterance, decode_tables)
 constexpr int TC_APLANE = 2 * TC_RA * 16;      // bytes of one plane of one 16-channel slab (2 k8 groups)
 constexpr int TC_ASTAGE = 2 * TC_APLANE;       // hi + lo planes
 constexpr int TC_NSTG = 6;                     // A slab stages: five slabs in flight while one is multiplied
@@ -91,7 +91,7 @@ struct Smem {
 
 static_assert(sizeof(Smem) + 128 <= 232448, "decode kernel: shared memory budget (227 KB per CTA)");
 // An A descriptor reads 64 rows per live M half from its k8 group: up to TC_RA + 128 rows from a group that holds TC_RA
-// (tap shift <= TC_RA, pack_decode), i.e. up to 128 rows of 16 bytes past the end of the last stage.  Those rows are thrown
+// (tap shift <= TC_RA, decode_tables), i.e. up to 128 rows of 16 bytes past the end of the last stage.  Those rows are thrown
 // away but must be shared memory of this kernel.
 static_assert(offsetof(Smem, tca) + sizeof(Smem::tca) + 128 * 16 <= sizeof(Smem), "A tile reads past the stages");
 
@@ -204,7 +204,7 @@ __device__ __forceinline__ void prefetch_params(const DecParams& P, Smem& S, int
     }
 }
 // taps (all but the last) of block li at frame j: rows j - (ntaps-1-tap)*rate of its input history -> xin[buf][g][tap*256..]
-// (multi-tap blocks have 256 input channels and 3 taps: pack_decode checks it)
+// (multi-tap blocks have 256 input channels and 3 taps: decode_tables checks it)
 __device__ __forceinline__ void prefetch_taps(const DecParams& P, Smem& S, int li, int j, int b0, int G, int buf) {
     const DecLayer& l = P.L[li];
     if (l.ntaps != 3 || !P.in_hist[li]) return;
@@ -260,7 +260,7 @@ __device__ __forceinline__ void gemv_warp(const float* __restrict__ wreg, const 
 // The loop above is bound by shared-memory wavefronts: per 8 k a warp reads 8 wavefronts of weights and 2 x GT broadcast
 // loads of the activations (every lane wants the same 8 k of x).  Here a lane owns TWO columns (2cp, 2cp+1) and HALF of the k
 // (kh = lane >> 4 takes k-group 2j + kh), so a step needs ONE activation load per utterance (two addresses per warp, one
-// wavefront) for the same number of FMAs: 8 + GT wavefronts instead of 8 + 2 GT.  Weight layout per 8-k block (1 KB, pack_decode):
+// wavefront) for the same number of FMAs: 8 + GT wavefronts instead of 8 + 2 GT.  Weight layout per 8-k block (1 KB, kernels_pack.cu):
 // [column parity][k-group kh][column pair cp][4 k], so both weight loads of a warp are 512 contiguous bytes.  Partial sums of
 // the two k-halves are added with one shuffle per accumulator after the last chunk.
 template <int GT>
@@ -657,7 +657,7 @@ __device__ __forceinline__ void pyr_tc_utt(const DecParams& P, Smem& S, int li, 
     const DecLayer& l = P.L[li];
     const int tid = threadIdx.x, warp = tid >> 5;
     if (tid == 0) {
-        const int halo = (l.ntaps - 1) * l.rate, n_src = n_out + halo;   // <= TC_RA (pack_decode)
+        const int halo = (l.ntaps - 1) * l.rate, n_src = n_out + halo;   // <= TC_RA (decode_tables)
         const int nslab = l.cin / 16;
         const size_t run = (size_t)P.pl_rows * 8;                     // halfs between the four (plane, k8) runs of a slab
         const __half* src = c1 ? c1 : P.pl_hist[li] + pl_idx(nslab, P.pl_rows, b, 0, t_lo - halo);
@@ -682,7 +682,7 @@ __device__ __forceinline__ void pyr_tc_utt(const DecParams& P, Smem& S, int li, 
                     bulk_g2s_mc(dst + (r >> 1) * TC_APLANE + (r & 1) * (TC_RA * 16), src + r * run, rb, &S.abar[stg], all);
             }
         }
-    } else if (warp >= 4) {                                           // shapes checked by pack_decode: hc 32 columns x 3 taps, conv 16 x 1
+    } else if (warp >= 4) {                                           // shapes checked by decode_tables: hc 32 columns x 3 taps, conv 16 x 1
         if (l.ns == 32) {
             if (n_out > 64) pyr_mma_rows<PROF, 32, 3, 2, false>(P, S, li, q0, n_out, rank, scr_rows);
             else pyr_mma_rows<PROF, 32, 3, 1, false>(P, S, li, q0, n_out, rank, scr_rows);
@@ -734,7 +734,7 @@ __device__ __forceinline__ void pyr_tc_packed(const DecParams& P, Smem& S, int l
                                     &S.abar[stg], all);
             }
         }
-    } else if (warp >= 4) {                                           // hc blocks only (pack_decode: 32 columns x 3 taps)
+    } else if (warp >= 4) {                                           // hc blocks only (decode_tables: 32 columns x 3 taps)
         pyr_mma_rows<PROF, 32, 3, 1, true>(P, S, li, q0, rl.total, rank, scr);
     }
 }

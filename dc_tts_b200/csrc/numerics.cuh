@@ -1,5 +1,5 @@
 // numerics.cuh -- the kernels' shared arithmetic: the split-fp16 operand format, its power-of-two scales, the warp sum and
-// the accurate sigmoid.  Every kernel and both host weight packers use these definitions; none restates them.
+// the accurate sigmoid.  Every kernel, the weight packers included, uses these definitions; none restates them.
 //
 // Split-fp16 operands ("split planes"): every fp32 value x that feeds the fp16 tensor cores is held as two fp16 tensors
 // hi = fp16(s x), lo = fp16(s x - hi) (22 significand bits together, 4 bytes per element like fp32) with a power-of-two
@@ -47,8 +47,9 @@ __device__ __forceinline__ void split_store_f16(const float* v, __half* hi, __ha
 }
 
 // ---- the scales s, one rule per kind of operand ----
-// Weights of the block kernels and of the persistent decode's pre-pass (host packers): max|W| s in [2^10, 2^11), so that
-// the lo plane stays in fp16's normal range; the kernel multiplies the accumulator by 1 / s.
+// Weights of the block kernels and of the persistent decode's pre-pass (kernels_pack.cu; the host computes s from the
+// device abs-max): max|W| s in [2^10, 2^11), so that the lo plane stays in fp16's normal range; the kernel multiplies the
+// accumulator by 1 / s.
 inline float weight_scale(float maxabs) {
     float s = 1.f;
     if (maxabs > 0.f) { int e; std::frexp(maxabs, &e); s = std::ldexp(1.f, 11 - e); }

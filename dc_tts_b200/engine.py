@@ -661,6 +661,14 @@ class Engine:
         self._check(self._lib.dctts_train_set_tensor(self._h, name.encode(), {"param": 0, "m": 2, "v": 3}[what],
                                                      a.ctypes.data_as(C.c_void_p), a.size), "dctts_train_set_tensor(%s)" % name)
 
+    def refresh_synthesis(self):
+        """Synthesise from the variables being trained (include/dctts.h: dctts_refresh_synthesis): packs the wgmma weight
+        planes and the persistent decode's weight stream again on the device, so that this handle computes what a fresh
+        handle loaded with the same variables computes, on the same kernels.  Training state is untouched; the next update
+        (train_step with apply, train_apply, train_set_tensor of a variable, restore_training) makes the packing stale
+        again.  A no-op when nothing changed since the last packing."""
+        self._check(self._lib.dctts_refresh_synthesis(self._h, self._stream()), "dctts_refresh_synthesis")
+
     def restore_training(self, logdir, scope="Text2Mel"):
         """What tf.train.Supervisor does when `logdir` already holds a checkpoint (train.py:144): every variable of the
         network being trained, its Adam slots (`<name>/Adam`, `<name>/Adam_1`) and `gs/global_step` come back from the

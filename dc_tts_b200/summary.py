@@ -6,6 +6,8 @@ Records use TFRecord framing: uint64 length, masked CRC-32C of the length, the d
 CRC-32C and its mask are checkpoint.py's, which reads TF's tensor bundles).  `read_events` parses such a file back and
 verifies every checksum.
 
+`audio` (the trainer's samples) is written from the same recollection of TF 1.x's Summary protobuf, also unchecked.
+
 `image` follows TF 1.x's image summary op for float input, as recalled (not checked against TF): min and max over the
 finite pixels; if min >= 0 the pixels are scaled by 255 / max, otherwise by 127 / max|x| and offset by 128 (a scale of 0
 when that maximum is below 1e-6); the result is truncated to uint8, non-finite pixels become 255; 8-bit grayscale PNG.
@@ -91,6 +93,24 @@ def image(tag, array, max_outputs=3):
     return out
 
 
+def wav_bytes(wav, sample_rate):
+    """A mono 16-bit PCM WAV file of float samples in [-1, 1] (clipped, scaled by 32767 and rounded)."""
+    pcm = np.round(np.clip(np.asarray(wav, np.float32), -1.0, 1.0) * 32767.0).astype("<i2").tobytes()
+    fmt = struct.pack("<HHIIHH", 1, 1, int(sample_rate), 2 * int(sample_rate), 2, 16)
+    return (b"RIFF" + struct.pack("<I", 36 + len(pcm)) + b"WAVE" + b"fmt " + struct.pack("<I", len(fmt)) + fmt +
+            b"data" + struct.pack("<I", len(pcm)) + pcm)
+
+
+def audio(tag, wav, sample_rate):
+    """Serialized `Summary` with one audio clip, tagged `<tag>/audio/0` as tf.summary.audio(tag, ..., max_outputs=1) names
+    it: Value.audio (field 6) = {sample_rate, num_channels 1, length_frames, 16-bit PCM WAV bytes (wav_bytes),
+    content_type "audio/wav"}.  Written from the TF 1.x protobuf definitions as recalled, not checked against TF."""
+    n = int(np.asarray(wav).shape[0])
+    body = (_fixed32_field(1, sample_rate) + _proto_varint_field(2, 1) + _proto_varint_field(3, n) +
+            _proto_bytes_field(4, wav_bytes(wav, sample_rate)) + _proto_bytes_field(5, b"audio/wav"))
+    return _value(tag + "/audio/0", _proto_bytes_field(6, body))
+
+
 def merge(*summaries):
     """tf.summary.merge: the values of several serialized Summaries in one (protobuf messages concatenate)."""
     return b"".join(summaries)
@@ -147,7 +167,8 @@ class FileWriter:
 
 
 def parse_summary(buf):
-    """Summary bytes -> [(tag, float) for scalars or (tag, {height, width, colorspace, png}) for images]."""
+    """Summary bytes -> [(tag, float) for scalars, (tag, {height, width, colorspace, png}) for images or
+    (tag, {sample_rate, num_channels, length_frames, wav, content_type}) for audio]."""
     out = []
     for field, _, val in _proto_fields(buf):
         if field != 1:
@@ -161,6 +182,11 @@ def parse_summary(buf):
             elif f == 4:
                 img = {1: "height", 2: "width", 3: "colorspace", 4: "png"}
                 v = {img[k]: y for k, _, y in _proto_fields(x) if k in img}
+            elif f == 6:
+                au = {1: "sample_rate", 2: "num_channels", 3: "length_frames", 4: "wav", 5: "content_type"}
+                v = {au[k]: y for k, _, y in _proto_fields(x) if k in au}
+                if "sample_rate" in v:
+                    v["sample_rate"] = struct.unpack("<f", struct.pack("<I", v["sample_rate"]))[0]
         out.append((tag, v))
     return out
 

@@ -296,8 +296,64 @@ def evaluate(num, engine, L, mels, mags, global_step, alignments=False):
     return losses, t, train_summary(num, losses, host(target), host(out), learning_rate_decay(hp.lr, global_step))
 
 
+def sample_texts(samples):
+    """`samples` -> (B, max_N) int32 ids through data_load.load_data("synthesize", ...): the path of a sentences file in
+    harvard_sentences.txt's format (a header line, then "N. sentence" lines), or a list of sentences."""
+    import tempfile
+    from .data_load import load_data
+    if isinstance(samples, (str, os.PathLike)):
+        return load_data("synthesize", os.fspath(samples))
+    samples = list(samples)
+    if not samples:
+        raise ValueError("samples: no sentences")
+    with tempfile.TemporaryDirectory() as d:
+        path = os.path.join(d, "samples.txt")
+        with codecs.open(path, "w", "utf-8") as f:
+            f.write("samples\n" + "".join("%d. %s\n" % (i + 1, t.replace("\n", " ")) for i, t in enumerate(samples)))
+        return load_data("synthesize", path)
+
+
+def write_samples(engine, texts, logdir, global_step, writer=None):
+    """What the model being trained says when it runs free, for the checkpoint at `global_step`: the engine's synthesis is
+    refreshed from its current variables (Engine.refresh_synthesis), `texts` (B, max_N) are decoded until their EOS
+    (Engine.text2mel_generate_until), SSRN runs on each utterance's own frames and Griffin-Lim turns them into
+    `samples_{NNN}k/{i}.wav` (i from 1) in `logdir`, beside `samples_{NNN}k/alignment_{i}.png`: the attention window of
+    every frame (the decode's argmax history, max_N x length).  Text2Mel and SSRN are the weights the engine holds: one of
+    them is being trained, the other is as it was loaded.  With a `writer` (summary.FileWriter) one event at
+    `global_step` holds an audio summary per sample (`samples/{i}/audio/0`), the mean length in frames
+    (`samples/length_frames`) and the share of samples that stopped at their text's end before max_T frames
+    (`samples/eos_reached`).  Returns (wavs, lengths in mel frames)."""
+    from scipy.io.wavfile import write as write_wav
+    from .data_load import eos_positions
+    from .utils import plot_alignment, spectrograms2wavs
+    h = engine.hp
+    engine.refresh_synthesis()
+    Y, P, n = engine.text2mel_generate_until(texts)
+    lengths = n.cpu().numpy()
+    Tmax = int(lengths.max())
+    _, Z = engine.ssrn(Y[:, :Tmax], want_logits=False, lengths=n)
+    wavs = spectrograms2wavs(Z, lengths=h.r * lengths, engine=engine)
+    out = os.path.join(logdir, "samples_" + str(global_step // 1000).zfill(3) + "k")
+    os.makedirs(out, exist_ok=True)
+    P = P.cpu().numpy()
+    for i, wav in enumerate(wavs):
+        write_wav(os.path.join(out, "{}.wav".format(i + 1)), h.sr, wav)
+        path = np.zeros((h.max_N, int(lengths[i])), np.float32)
+        path[P[i, :lengths[i]], np.arange(lengths[i])] = 1.0
+        plot_alignment(path, i + 1, out)
+    if writer is not None:
+        from .summary import audio, merge, scalar
+        stopped = np.mean((lengths < h.max_T) & (eos_positions(np.asarray(texts)) >= 0))
+        writer.add_summary(merge(*[audio("samples/%d" % (i + 1), w, h.sr) for i, w in enumerate(wavs)],
+                                 scalar("samples/length_frames", float(lengths.mean())), scalar("samples/eos_reached", stopped)),
+                           global_step)
+        writer.flush()
+    return wavs, lengths
+
+
 def train(num, engine, batches, num_iterations=None, logdir=None, global_step=None, save_every=1000, log=print, resume=True,
-          rank=0, world=1, allreduce=None, beyond_capacity="skip", capacity=None, summaries=False, summary_secs=120):
+          rank=0, world=1, allreduce=None, beyond_capacity="skip", capacity=None, summaries=False, summary_secs=120,
+          samples=None):
     """train.py:137-160 for num = 1 (Text2Mel) or 2 (SSRN).  `batches` yields (L, mels, mags, names, ...): the bucketed
     batches of `bucketed_batches` at their own shapes or fixed-size ones; `engine` is an `Engine` with parameters loaded.
     The workspace is allocated for the capacity (hp.max_N, hp.max_T), or `capacity` = (N, T) when that is larger; a batch
@@ -314,6 +370,12 @@ def train(num, engine, batches, num_iterations=None, logdir=None, global_step=No
     update (`evaluate`) and one event with train.py's merged summaries, `lr` and `global_step/sec` goes to a new
     `events.out.tfevents.*` file in `logdir`; at every checkpoint of Text2Mel the next batch is evaluated and its first
     alignment written as `alignment_{NNN}k.png` (utils.plot_alignment).  Evaluations consume batches as TF's queue does.
+
+    `samples` (default None: off): sentences -- a list, or a file in harvard_sentences.txt's format -- that rank 0 synthesises
+    at every checkpoint from the weights being trained (`write_samples`: wavs and window-path plots in
+    `samples_{NNN}k/`, and with `summaries` an event with their audio).  The network not being trained is the one the
+    engine holds: for num = 1, SSRN as loaded (e.g. restored from logdir-2; random SSRN weights still give the mels'
+    lengths and a rough sound); for num = 2, Text2Mel as loaded.  It consumes no batch.
     Returns the final global step."""
     if num not in (1, 2):
         raise ValueError("num: 1 for Text2Mel, 2 for SSRN (train.py:139)")
@@ -326,6 +388,7 @@ def train(num, engine, batches, num_iterations=None, logdir=None, global_step=No
     initialised = False
     batches = iter(batches)
     writer = None
+    texts = sample_texts(samples) if samples is not None and rank == 0 else None
 
     def next_admitted():
         for b in batches:
@@ -386,6 +449,8 @@ def train(num, engine, batches, num_iterations=None, logdir=None, global_step=No
                 if ev is not None:
                     from .utils import plot_alignment
                     plot_alignment(ev[1]["alignments"][0].cpu().numpy(), str(gs // 1000).zfill(3) + "k", logdir)
+            if texts is not None:
+                write_samples(engine, texts, logdir, gs, writer)
         if writer is not None and time.time() - last_t >= summary_secs:
             ev = evaluate_next()
             now = time.time()

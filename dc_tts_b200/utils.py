@@ -29,11 +29,11 @@ def spectrogram2wav(mag, momentum=0.0):
     return wav[0, s:e].cpu().numpy().astype(np.float32)
 
 
-def spectrograms2wavs(mags, lengths=None, momentum=0.0):
+def spectrograms2wavs(mags, lengths=None, momentum=0.0, engine=None):
     """Batched form: (B, T, F) -> list of trimmed wavs (one device pass for the whole batch).  `lengths`: optional (B,)
     magnitude frames per utterance; wav b is then spectrogram2wav(mags[b, :lengths[b]]), bit for bit.  `momentum` as
-    for spectrogram2wav."""
-    wav, trim = get_engine().spectrogram2wav(mags, lengths=lengths, momentum=momentum)
+    for spectrogram2wav.  `engine`: the Engine to run on (default: the process-wide one)."""
+    wav, trim = (engine or get_engine()).spectrogram2wav(mags, lengths=lengths, momentum=momentum)
     wav = wav.cpu().numpy()
     return [wav[b, int(trim[b, 0]):int(trim[b, 1])].astype(np.float32) for b in range(wav.shape[0])]
 

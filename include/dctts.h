@@ -237,7 +237,8 @@ int32_t dctts_resample_time_register(int64_t n_out, int32_t sr_in, int32_t sr_ou
  * pointers.  All tensors are float32; the three GEMMs of every block (forward conv, data gradient, weight gradient) run on
  * wgmma as split-fp16 x3 with per-tensor power-of-two scales (option "train_tc", default 7; 0 = the float32 CUDA-core
  * kernels).  dctts_train_init allocates the saved activations and the gradient / Adam arenas and switches the handle's
- * SYNTHESIS entry points to the fp32 kernel set (the optimiser updates the fp32 weights only, the packed planes go stale).
+ * SYNTHESIS entry points to the fp32 kernel set (the optimiser updates the fp32 weights only, the packed planes go stale;
+ * dctts_refresh_synthesis packs them again).
  * Dropout uses a stateless hash of (element, block index, seed) -- TF's random stream cannot be reproduced.
  * losses_host (optional): {total, mels L1, binary divergence, guided attention}; reading them synchronises.
  * apply = 0 leaves the gradients in the arena (dctts_train_grads: one flat device buffer, what a data-parallel job
@@ -297,6 +298,17 @@ int dctts_train_grads(dctts_handle h, float** grads, int64_t* count);
 int dctts_train_tensor(dctts_handle h, const char* tf_name, int32_t what, float* host_out, int64_t count);
 /* Inverse of dctts_train_tensor for what = 0 (variable), 2 (Adam m), 3 (Adam v): restores a training state (resume). */
 int dctts_train_set_tensor(dctts_handle h, const char* tf_name, int32_t what, const float* host_in, int64_t count);
+/* Synthesis from the variables being trained.  Every call that writes a variable -- dctts_train_init, a step with apply = 1,
+ * dctts_train_apply, dctts_train_set_tensor with what = 0 -- leaves the handle's packed weights stale: synthesis runs on the
+ * fp32 kernel set with the graph-per-frame decode, and dctts_set_tensor_path(1) fails.  This call packs the wgmma weight
+ * planes, the persistent decode's weight stream and its LayerNorm parameters again on the device from the variables as
+ * they are, so that afterwards the handle selects its kernels and computes exactly what a freshly committed handle
+ * holding the same variables would: tensor path 1, the persistent decode where it can be placed (the captured AR step is
+ * dropped).  It writes none of the variables, the Adam moments, the gradient arena or the training workspace, and a step
+ * with apply = 0 or an evaluation (dctts_train_eval*) keeps it in force.  A no-op on a handle whose packed weights are
+ * current (one never trained, or refreshed since its last update).  Synchronises `stream` and the device; costs one
+ * abs-max reduction, one small device-to-host copy and one pass over the weights. */
+int dctts_refresh_synthesis(dctts_handle h, void* stream);
 
 /* ---- utilities ----------------------------------------------------------------- */
 /* Pre-size the workspace (otherwise grown lazily on first use) for batches up to B. */
