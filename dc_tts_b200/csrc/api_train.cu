@@ -349,6 +349,19 @@ void train_forward(H* h, Launch& lc, const int* L, int N, const float* mels, int
     lc.count();
 }
 
+// The attention backward's arguments: gR (B,T,2d) = the gradient of [ctx ; Q], Q (B,T,d), KV (B,N,2d) = [K | V], align
+// (B,N,T), the guided-attention table gts (row stride ld_gts) and its (n_lim, t_lim) corner, dS (B,T,N) scratch, gQ (B,T,d),
+// gKV (B,N,2d).  The guided-attention loss is sum |A gts| / (B n_lim t_lim) (train.py:91-95).
+AttnBwdArgs attn_bwd_args(const float* gR, const float* Q, const float* KV, const float* align, const float* gts, int ld_gts,
+                          float* dS, float* gQ, float* gKV, int B, int T, int N, int d, int n_lim, int t_lim) {
+    AttnBwdArgs ab{};
+    ab.gR = gR; ab.Q = Q; ab.ldq = d; ab.K = KV; ab.V = KV + d; ab.ldkv = 2 * d; ab.align = align;
+    ab.gts = gts; ab.ld_gts = ld_gts; ab.dS = dS; ab.gQ = gQ; ab.gKV = gKV;
+    ab.B = B; ab.T = T; ab.N = N; ab.d = d; ab.n_lim = n_lim; ab.t_lim = t_lim;
+    ab.att_scale = 1.0f / ((float)B * (float)n_lim * (float)t_lim);
+    return ab;
+}
+
 void train_forward_backward(H* h, const int* L, int N, const float* mels, int T, int B, uint32_t seed, float* losses_host,
                             cudaStream_t s) {
     auto& tr = h->tr;
@@ -360,12 +373,9 @@ void train_forward_backward(H* h, const int* L, int N, const float* mels, int T,
     const float* KV = tr.layers[tr.last[0]].out;
     const float* Q = tr.layers[tr.last[1]].out;
     float* gR = train_bwd(h, lc, tr.first[2], tr.last[2], B, seed, tr.gbuf[0].as<float>(), tr.gbuf[1].as<float>());
-    AttnBwdArgs ab{};
-    ab.gR = gR; ab.Q = Q; ab.ldq = d; ab.K = KV; ab.V = KV + d; ab.ldkv = 2 * d; ab.align = tr.align.as<float>();
-    ab.gts = tr.gts.as<float>(); ab.ld_gts = hp.max_T; ab.dS = tr.dS.as<float>(); ab.gQ = tr.gbuf[2].as<float>(); ab.gKV = tr.gbuf[3].as<float>();
     const int n_lim = std::min(N, hp.max_N), t_lim = std::min(T, hp.max_T);      // the crop of train.py:91 to the table
-    ab.B = B; ab.T = T; ab.N = N; ab.d = d; ab.n_lim = n_lim; ab.t_lim = t_lim;
-    ab.att_scale = 1.0f / ((float)B * (float)n_lim * (float)t_lim);
+    const AttnBwdArgs ab = attn_bwd_args(gR, Q, KV, tr.align.as<float>(), tr.gts.as<float>(), hp.max_T, tr.dS.as<float>(),
+                                         tr.gbuf[2].as<float>(), tr.gbuf[3].as<float>(), B, T, N, d, n_lim, t_lim);
     launch_attn_bwd(ab, tr.sums.as<double>(), s); lc.count(3);
     float* free_a = (gR == tr.gbuf[0].as<float>()) ? tr.gbuf[1].as<float>() : tr.gbuf[0].as<float>();
     train_bwd(h, lc, tr.first[1], tr.last[1], B, seed, tr.gbuf[2].as<float>(), free_a);
@@ -535,6 +545,63 @@ int dctts_conv_gemm(dctts_handle h, int32_t impl, int32_t mode, const float* X, 
         h->launches += launches;
         CUDA_CHECK(cudaGetLastError());
         CUDA_CHECK(cudaStreamSynchronize(s));      // before the workspace is freed
+    });
+}
+
+int dctts_block_bwd(dctts_handle h, int32_t mode, int32_t act, int64_t rows, int32_t C, const float* pre, int32_t ldy,
+                    const float* gout, int32_t ldg, const float* X, int32_t ldx, const float* ln, float dropout_rate, int32_t layer,
+                    uint32_t seed, float* dy, float* gin, float* dparams, void* stream) {
+    return guarded(h, [&] {
+        REQUIRE(mode == 0 || mode == 1, "dctts_block_bwd: mode must be 0 (conv1d / transposed conv) or 1 (highway)");
+        REQUIRE(act == 0 || act == 1, "dctts_block_bwd: act must be 0 (none) or 1 (ReLU)");
+        REQUIRE(rows >= 1 && C >= 1 && layer >= 0 && dropout_rate >= 0.f && dropout_rate < 1.f, "dctts_block_bwd: bad arguments");
+        const int nconv = mode == 1 ? 2 * C : C;
+        REQUIRE(pre && gout && ln && dy && dparams && (mode == 0 || (X && gin)),
+                "dctts_block_bwd: pre, gout, ln, dy, dparams (and X, gin for a highway block) are required");
+        REQUIRE(ldy >= nconv && ldg >= C && (mode == 0 || ldx >= C), "dctts_block_bwd: a pitch is narrower than its tensor's width");
+        cudaStream_t s = S(h, stream);
+        BlockBwdArgs a{};
+        a.pre = pre; a.ldy = ldy; a.gout = gout; a.ldg = ldg; a.X = X; a.ldx = ldx;
+        a.g1 = ln; a.b1 = ln + C; a.g2 = ln + 2 * C; a.b2 = ln + 3 * C; a.dy = dy; a.gin = gin;
+        a.dg1 = dparams; a.db1 = dparams + C; a.dg2 = dparams + 2 * C; a.db2 = dparams + 3 * C; a.dbias = dparams + 4 * C;
+        a.rows = rows; a.C = C; a.mode = mode; a.act = act;
+        a.drop = drop_args(dropout_rate, layer, seed);
+        launch_train_block_bwd(a, s);              // refuses a width no kernel instantiation covers before launching
+        h->launches += 1;
+        CUDA_CHECK(cudaGetLastError());
+        CUDA_CHECK(cudaStreamSynchronize(s));
+    });
+}
+
+int dctts_attn_bwd(dctts_handle h, const float* gR, const float* Q, const float* KV, const float* align, const float* gts,
+                   int32_t ld_gts, int32_t B, int32_t T, int32_t N, int32_t n_lim, int32_t t_lim, float* gQ, float* gKV, double* sums,
+                   void* stream) {
+    DevBuf dS;                                      // the call's own dS scratch, freed on every exit
+    return guarded(h, [&] {
+        REQUIRE(gR && Q && KV && align && gts && gQ && gKV && sums && B >= 1 && T >= 1 && N >= 1, "dctts_attn_bwd: bad arguments");
+        AttnBwdArgs a = attn_bwd_args(gR, Q, KV, align, gts, ld_gts, nullptr, gQ, gKV, B, T, N, h->hp.d, n_lim, t_lim);
+        check_attn_bwd(a);                         // d and the crop, before the scratch is allocated
+        dS.ensure((size_t)B * T * N * sizeof(float));
+        a.dS = dS.as<float>();
+        cudaStream_t s = S(h, stream);
+        launch_attn_bwd(a, sums, s);
+        h->launches += 3;
+        CUDA_CHECK(cudaGetLastError());
+        CUDA_CHECK(cudaStreamSynchronize(s));      // before the scratch is freed
+    });
+}
+
+int dctts_train_loss(dctts_handle h, const float* logits, int32_t ldl, const float* target, int64_t rows, int32_t C, float* dlogits,
+                     int32_t ldg, float* Y, double* sums, void* stream) {
+    return guarded(h, [&] {
+        REQUIRE(logits && target && dlogits && sums && rows >= 1 && C >= 1, "dctts_train_loss: bad arguments");
+        REQUIRE(ldl >= C && ldg >= C, "dctts_train_loss: a pitch is narrower than its tensor's width");
+        cudaStream_t s = S(h, stream);
+        launch_train_loss(logits, ldl, target, dlogits, ldg, sums, rows, C, s);
+        h->launches += 1;
+        if (Y) { launch_sigmoid_rows(logits, ldl, Y, rows, C, s); h->launches += 1; }
+        CUDA_CHECK(cudaGetLastError());
+        CUDA_CHECK(cudaStreamSynchronize(s));
     });
 }
 

@@ -237,6 +237,8 @@ void launch_train_block_bwd(const BlockBwdArgs& a, cudaStream_t s);
 void launch_conv_wgrad(WgradArgs a, cudaStream_t s);
 void launch_transpose_w(const float* W, float* WT, int ntaps, int K, int N, int ldw, int Kp, cudaStream_t s);
 void launch_attn_bwd(const AttnBwdArgs& a, double* sums, cudaStream_t s);
+// what launch_attn_bwd refuses before it launches anything: d != 256, a crop outside (N, T) or wider than the table's stride
+void check_attn_bwd(const AttnBwdArgs& a);
 // the guided-attention sum alone (the first kernel of launch_attn_bwd): sums[2] += sum over the (n_lim, t_lim) corner of |A gts|
 void launch_attn_loss(const float* align, const float* gts, int ld_gts, double* sums, int B, int N, int T, int n_lim, int t_lim,
                       cudaStream_t s);

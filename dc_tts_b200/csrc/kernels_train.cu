@@ -218,7 +218,7 @@ __global__ void __launch_bounds__(256) conv_wgrad_kernel(const WgradArgs a) {
     const int tid = threadIdx.x;
     const int n0 = blockIdx.x * 64, k0 = blockIdx.y * 64;
     const int tap = blockIdx.z / a.nsplit, split = blockIdx.z - tap * a.nsplit;
-    const int shift = a.shifts[tap];
+    const int shift = tap == 0 ? a.shifts[0] : tap == 1 ? a.shifts[1] : a.shifts[2];   // a dynamic index would copy the params to the stack
     const long long r_begin = (long long)split * a.rows_per_split, r_end = min((long long)a.rows, r_begin + a.rows_per_split);
     const int tx = tid & 15, ty = tid >> 4;               // 16 x 16 threads, 4 x 4 outputs each
     const int lr = tid >> 4, lq = (tid & 15) * 4;         // loader: row lr (0..15), 4 consecutive columns at lq
@@ -396,12 +396,16 @@ void launch_attn_loss(const float* align, const float* gts, int ld_gts, double* 
     attn_loss_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(align, gts, ld_gts, sums, B, N, T, n_lim, t_lim);
 }
 
-void launch_attn_bwd(const AttnBwdArgs& a, double* sums, cudaStream_t s) {
+void check_attn_bwd(const AttnBwdArgs& a) {
     if (a.d != 256) throw std::runtime_error("attention backward is built for d = 256");
     if (a.n_lim < 1 || a.n_lim > a.N || a.t_lim < 1 || a.t_lim > a.T || a.ld_gts < a.t_lim)
         throw std::runtime_error("attention backward: the guided-attention crop (" + std::to_string(a.n_lim) + ", " +
                                  std::to_string(a.t_lim) + ") does not fit the step (" + std::to_string(a.N) + ", " +
                                  std::to_string(a.T) + ") or the table's row stride " + std::to_string(a.ld_gts));
+}
+
+void launch_attn_bwd(const AttnBwdArgs& a, double* sums, cudaStream_t s) {
+    check_attn_bwd(a);
     const size_t smem = (size_t)4 * a.N * sizeof(float);
     if (smem > 48 * 1024) {
         cudaError_t e = cudaFuncSetAttribute(attn_bwd_q_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -440,7 +444,8 @@ void launch_embed_bwd(const int* ids, const float* g, float* dtable, int rows, i
 }
 
 // ------------------------------------------------------------------------------------ optimiser
-// train.py:122-132: clip to [-1, 1], tf.train.AdamOptimizer (bias correction folded into lr_t by the host)
+// train.py:122-132: clip to [-1, 1], tf.train.AdamOptimizer (bias correction folded into lr_t by the host).  fmaxf returns
+// its non-NaN operand, so a NaN gradient element clips to -1 (tests/test_gpu_train_kernels.py pins it; DESIGN.md 8e).
 __global__ void adam_kernel(const AdamEntry* __restrict__ entries, int n_entries, float lr_t, float beta1, float beta2, float eps) {
     const AdamEntry e = entries[blockIdx.y];
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < e.n; i += (long long)gridDim.x * blockDim.x) {

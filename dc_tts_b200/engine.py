@@ -170,6 +170,83 @@ class Engine:
                                               out.stride(1), self._stream()), "dctts_conv_gemm")
         return out
 
+    @staticmethod
+    def _pitched(who, ts, rows):
+        """Each tensor of `ts` is a CUDA float32 view of `rows` rows with a unit inner stride, its rows evenly pitched (the
+        pitch is the row stride); returns the pitches."""
+        if not all(t.is_cuda and t.dtype == torch.float32 and t.stride(-1) == 1 for t in ts):
+            raise DcttsError("%s: CUDA float32 tensors with a unit inner stride expected" % who)
+        pitches = []
+        for t in ts:
+            lead = t.shape[:-1]
+            n = 1
+            for s in lead:
+                n *= s
+            ld = t.stride(-2) if t.dim() >= 2 else t.shape[-1]
+            even = all(t.stride(i) == t.stride(i + 1) * t.shape[i + 1] for i in range(t.dim() - 2))
+            if n != rows or not even:
+                raise DcttsError("%s: rows of a tensor are not evenly pitched, or not %d of them" % (who, rows))
+            pitches.append(ld)
+        return pitches
+
+    def block_bwd(self, mode, act, C, pre, gout, ln, dy, dparams, X=None, gin=None, dropout_rate=0.0, layer=0, seed=0):
+        """Test aid (include/dctts.h: dctts_block_bwd): the dropout / activation / highway / LayerNorm backward of one block,
+        one launch.  pre, dy (rows, >= nconv); gout (rows, >= C); X, gin (rows, >= C) for mode 1 (highway); ln (4, C) =
+        g1 | b1 | g2 | b2 contiguous; dparams (4 C + nconv) contiguous, added onto.  Leading dims are flattened into rows;
+        the pitches are the views' row strides."""
+        nconv = 2 * C if mode == 1 else C
+        if mode == 1 and (X is None or gin is None):
+            raise DcttsError("block_bwd: a highway block (mode 1) needs X and gin")
+        rows = 1
+        for s in pre.shape[:-1]:
+            rows *= s
+        ts = [pre, gout, dy] + ([X, gin] if mode == 1 else [])
+        if any(t.shape[-1] < w for t, w in zip(ts, (nconv, C, nconv, C, C))):
+            raise DcttsError("block_bwd: pre and dy need %d columns, gout, X and gin %d" % (nconv, C))
+        lds = self._pitched("block_bwd", ts, rows)
+        if gout.stride(-2) != lds[1] or (mode == 1 and gin.stride(-2) != lds[1]):
+            raise DcttsError("block_bwd: gout and gin share one pitch")
+        if dy.stride(-2) != lds[0]:
+            raise DcttsError("block_bwd: pre and dy share one pitch")
+        _require_tensors("block_bwd", [(ln, (4, C), torch.float32), (dparams, (4 * C + nconv,), torch.float32)])
+        self._check(self._lib.dctts_block_bwd(self._h, int(mode), int(act), rows, int(C), _ptr(pre), lds[0], _ptr(gout), lds[1],
+                                              _ptr(X), lds[3] if mode == 1 else 0, _ptr(ln), float(dropout_rate), int(layer),
+                                              int(seed) & 0xffffffff, _ptr(dy), _ptr(gin), _ptr(dparams), self._stream()),
+                    "dctts_block_bwd")
+        return dy
+
+    def attn_bwd(self, gR, Q, KV, align, gts, n_lim, t_lim, gQ, gKV, sums):
+        """Test aid (include/dctts.h: dctts_attn_bwd): the attention backward of the Text2Mel step.  gR (B, T, 2d), Q (B, T, d),
+        KV (B, N, 2d), align (B, N, T), gQ (B, T, d), gKV (B, N, 2d) contiguous; gts (>= n_lim, ld_gts) with a unit inner
+        stride, its row stride the table's; sums (3,) float64, sums[2] added onto."""
+        B, T, N, d = align.shape[0], align.shape[2], align.shape[1], self.hp.d
+        f32 = torch.float32
+        _require_tensors("attn_bwd", [(gR, (B, T, 2 * d), f32), (Q, (B, T, d), f32), (KV, (B, N, 2 * d), f32),
+                                      (align, (B, N, T), f32), (gQ, (B, T, d), f32), (gKV, (B, N, 2 * d), f32),
+                                      (sums, (3,), torch.float64)])
+        if gts.dim() != 2 or gts.shape[0] < n_lim or gts.shape[1] < t_lim:
+            raise DcttsError("attn_bwd: gts must be 2-D with at least n_lim = %d rows and t_lim = %d columns, got %s"
+                             % (n_lim, t_lim, tuple(gts.shape)))
+        ld_gts = self._pitched("attn_bwd", [gts], gts.shape[0])[0]
+        self._check(self._lib.dctts_attn_bwd(self._h, _ptr(gR), _ptr(Q), _ptr(KV), _ptr(align), _ptr(gts), ld_gts, B, T, N,
+                                             int(n_lim), int(t_lim), _ptr(gQ), _ptr(gKV), _ptr(sums), self._stream()),
+                    "dctts_attn_bwd")
+        return gQ, gKV
+
+    def train_loss(self, logits, target, dlogits, sums, Y=None):
+        """Test aid (include/dctts.h: dctts_train_loss): L1 + BCE on sigmoid(logits) against target, and the logits'
+        gradient.  logits, dlogits (rows, >= C) views with a unit inner stride (the pitches are their row strides); target
+        and Y (rows, C) contiguous; sums (2,) float64, added onto."""
+        rows, C = target.shape
+        if logits.shape[-1] < C or dlogits.shape[-1] < C:
+            raise DcttsError("train_loss: logits and dlogits need %d columns" % C)
+        ldl, ldg = self._pitched("train_loss", [logits, dlogits], rows)
+        want = [(target, (rows, C), torch.float32), (sums, (2,), torch.float64)] + ([(Y, (rows, C), torch.float32)] if Y is not None else [])
+        _require_tensors("train_loss", want)
+        self._check(self._lib.dctts_train_loss(self._h, _ptr(logits), ldl, _ptr(target), rows, C, _ptr(dlogits), ldg, _ptr(Y),
+                                               _ptr(sums), self._stream()), "dctts_train_loss")
+        return dlogits
+
     def launch_count(self):
         return int(self._lib.dctts_launch_count(self._h))
 

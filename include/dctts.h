@@ -371,6 +371,42 @@ int dctts_bench_block(dctts_handle h, const char* scope, int32_t B, int32_t L, i
 int dctts_conv_gemm(dctts_handle h, int32_t impl, int32_t mode, const float* X, int32_t ldx, int32_t B, int32_t L, int32_t K,
                     const float* Wd, int32_t ldwd, int32_t N, int32_t ntaps, const int32_t* shifts_host, const float* bias,
                     int32_t accumulate, float* out, int32_t ldo, void* stream);
+/* Test aid: the backward of ONE block's dropout / activation / highway gate / LayerNorm on caller DEVICE tensors, through the
+ * launch function the training step calls (one launch); the training state is not touched.
+ *   mode 0: conv1d or transposed conv, out = dropout(act(LN(pre[:, 0:C]; g1, b1))), act 0 none / 1 ReLU (mask z > 0);
+ *   mode 1: highway, out = dropout(h1 h2 + (1 - h1) x), h1 = sigmoid(LN(pre[:, 0:C]; g1, b1)), h2 = LN(pre[:, C:2C]; g2, b2);
+ *   LayerNorm: biased variance, eps 1e-12.  nconv = C (mode 0) or 2C (mode 1).
+ * pre (rows, ldy >= nconv) the pre-LN conv output; gout (rows, ldg >= C) the gradient of out; X (rows, ldx >= C) the
+ * block input (mode 1; NULL otherwise); ln (4, C) = g1 | b1 | g2 | b2 (g2, b2 unused in mode 0).  The dropout mask is the
+ * step's: element (row, c) is kept iff its hash of (row C + c, layer, seed) clears dropout_rate, kept values scaled by
+ * 1 / (1 - dropout_rate); rate 0 keeps everything.
+ * Out: dy (rows, ldy) the gradient of pre (columns [0, nconv)); gin (rows, ldg, mode 1) the highway part g (1 - h1) of the
+ * input gradient; dparams (4C + nconv) floats ADDED onto: dg1 | db1 | dg2 | db2 | dbias (dg2, db2 untouched in mode 0).
+ * Pad columns are neither read nor written.  Fails with a message, launching nothing, on a bad mode, act, rate or pitch,
+ * a highway block wider than 1056 channels or any block wider than 2080.  Synchronises `stream`. */
+int dctts_block_bwd(dctts_handle h, int32_t mode, int32_t act, int64_t rows, int32_t C, const float* pre, int32_t ldy,
+                    const float* gout, int32_t ldg, const float* X, int32_t ldx, const float* ln, float dropout_rate, int32_t layer,
+                    uint32_t seed, float* dy, float* gin, float* dparams, void* stream);
+/* Test aid: the attention backward of the Text2Mel training step (three launches: guided-attention sum, query side, key side)
+ * on caller DEVICE tensors, through the launch function the step calls, with the handle's d (the kernels need d = 256).
+ * gR (B,T,2d) the gradient of R = [ctx ; Q]; Q (B,T,d); KV (B,N,2d) = [K | V]; align (B,N,T) the forward's softmax over
+ * n; gts the guided-attention weights, >= n_lim rows of stride ld_gts >= t_lim, of which the (n_lim, t_lim) corner is read.
+ * With S = Q K^T / sqrt(d), A = align (used as given), loss = sum_corner |A gts| / (B n_lim t_lim):
+ *   gQ (B,T,d) = gR[:, :, d:2d] + dS K / sqrt(d);  gKV (B,N,2d) = [dS^T Q / sqrt(d) | A dctx];  sums[2] += sum_corner |A gts|
+ * with dA = dctx V^T + sign(A gts) gts / (B n_lim t_lim) inside the corner, dS = A (dA - sum_n A dA).  sums: 3 doubles, only
+ * sums[2] is written.  The call owns the (B,T,N) dS scratch.  Fails with a message, launching nothing, when d != 256, the
+ * crop does not fit (1 <= n_lim <= N, 1 <= t_lim <= T, t_lim <= ld_gts) or N keys need more shared memory than the device
+ * allows.  Synchronises `stream`. */
+int dctts_attn_bwd(dctts_handle h, const float* gR, const float* Q, const float* KV, const float* align, const float* gts,
+                   int32_t ld_gts, int32_t B, int32_t T, int32_t N, int32_t n_lim, int32_t t_lim, float* gQ, float* gKV, double* sums,
+                   void* stream);
+/* Test aid: the mel / magnitude losses of the training step on caller DEVICE tensors, through the launch functions the step
+ * calls.  logits (rows, ldl >= C), target (rows, C) dense, n = rows C, y = sigmoid(logits):
+ *   sums[0] += sum |y - target|,  sums[1] += sum BCE(logits, target),  dlogits (rows, ldg >= C) = (sign(y - t) y (1 - y) + y - t) / n
+ * and, when Y is not NULL, Y (rows, C) dense = y (a second launch, the one the training-graph evaluation makes).  Pad
+ * columns are neither read nor written.  Fails with a message on a bad shape or pitch.  Synchronises `stream`. */
+int dctts_train_loss(dctts_handle h, const float* logits, int32_t ldl, const float* target, int64_t rows, int32_t C, float* dlogits,
+                     int32_t ldg, float* Y, double* sums, void* stream);
 /* Test aid: ONE stage of dctts_spectrogram2wav on caller DEVICE tensors, through the launch functions the product calls,
  * with the handle's vocoder parameters and the tables (twiddles, window, window sum-square) it builds for (T, win, hop).
  * Ly = hop (T - 1), nfr = 1 + Ly / 512, F = 1 + n_fft / 2.
