@@ -14,12 +14,14 @@
 //     multiplies: it waits on its own mbarrier, and refills its own 6 KB region the moment it has read
 //     it -- the chunk loop has no block-wide synchronisation at all.
 //   * per block: GEMV of the slice on fp32 FMA (exact fp32 arithmetic, as the reference), one block
-//     barrier for the cross-warp reduction, the pre-LN slice goes to every peer with ONE bulk copy
-//     per peer through distributed shared memory, completing on the peer's mbarrier (no hardware
-//     cluster barrier on this path); every CTA then normalises the whole rows redundantly (LayerNorm
-//     statistics one warp per (utterance, half), gate / highway mix one thread per channel), so the next
-//     block's input is in local shared memory.  Dilated taps come from the per-layer history in HBM/L2, prefetched one
-//     block ahead with cp.async; each CTA appends its channel slice of the new row.
+//     barrier for the cross-warp reduction; the threads that finish the slice's values store them from
+//     registers into every peer with st.async through distributed shared memory, together with the
+//     LayerNorm statistics of the slice's channels, completing on the peer's mbarrier (no hardware
+//     cluster barrier on this path); every CTA then merges the 16 slices' statistics and normalises the
+//     whole rows redundantly (gate / highway mix one thread per channel), so the next block's input is
+//     in local shared memory.  Two block barriers per block.  Dilated taps come from the per-layer
+//     history in HBM/L2, prefetched one block ahead with cp.async while the peers' slices are in
+//     flight; each CTA appends its channel slice of the new row.
 //   * Quirk Q1 (SURVEY 3.1): the reference recomputes R under the CURRENT window every step.  While
 //     the window of an utterance does not move, the cached rows are exactly what a recompute would
 //     give.  When it moves, a PRE-PASS refreshes the rows t < j of its AudioDec receptive field
@@ -51,6 +53,7 @@ namespace {
 constexpr int NC = DEC_NC, GMAX = DEC_GMAX, NT = DEC_THREADS, NWARP = NT / 32;
 constexpr int XLD = 768;                       // row pitch of the input vectors: [tap0 | tap1 | current]
 constexpr int PLD = GMAX * 32 + 16;            // pitch between the ranks' slices in `pre` (16 floats of bank skew)
+constexpr int PPD = 2 * NC + 4;                // pitch of one (utterance, LN half) in `part`: NC x (mean, M2), 4 floats of bank skew
 constexpr int TC_RA = DEC_PL_PAD;              // pre-pass: rows per k8 group of an A slab plane (source rows per utterance, decode_tables)
 constexpr int TC_APLANE = 2 * TC_RA * 16;      // bytes of one plane of one 16-channel slab (2 k8 groups)
 constexpr int TC_ASTAGE = 2 * TC_APLANE;       // hi + lo planes
@@ -70,15 +73,16 @@ struct Smem {
     union {                             // never live together: between the cluster barriers that enclose the pre-pass no peer
                                         // sends pre-LN slices, so the pre-pass stages A here (and the peers' multicast
                                         // slabs land here only between those barriers)
-        float pre[2][NC][PLD];
-        unsigned char tca[TC_NSTG][TC_ASTAGE];   // (the MMAs read up to 128 + 54 rows past a slab start: outv / prm follow)
+        struct {
+            float pre[2][NC][PLD];
+            float part[2][GMAX * 2][PPD];   // every rank's LayerNorm partials (mean, M2) per (utterance, LN half)
+        };
+        unsigned char tca[TC_NSTG][TC_ASTAGE];   // (the MMAs read up to 128 + 54 rows past a slab start: prm follows)
     };
-    float outv[2][GMAX * 32];
     float prm[2][DEC_PRM_F];
     unsigned long long fullw[DEC_NSLOT][NWARP];
     unsigned long long gbar[2];
     unsigned long long sbar[TC_NSTG], abar[TC_NSTG];   // pre-pass: slab stage free / slab stage filled
-    float stat[GMAX][2][2];             // per utterance and LN half: mean, 1/sqrt(var + eps)
     uint32_t tc_baddr[96];              // pre-pass: descriptor start field of every weight slab of the current block
     int n_moved_frames, n_moved_utt;
     DecParams P;                        // the kernel's parameter block: indexed per block / chunk on the critical path; in the
@@ -94,6 +98,8 @@ static_assert(sizeof(Smem) + 128 <= 232448, "decode kernel: shared memory budget
 // (tap shift <= TC_RA, decode_tables), i.e. up to 128 rows of 16 bytes past the end of the last stage.  Those rows are thrown
 // away but must be shared memory of this kernel.
 static_assert(offsetof(Smem, tca) + sizeof(Smem::tca) + 128 * 16 <= sizeof(Smem), "A tile reads past the stages");
+static_assert(offsetof(Smem, pre) % 16 == 0 && (PLD * 4) % 16 == 0, "pre: 16-byte st.async targets");
+static_assert(offsetof(Smem, part) % 16 == 0 && (PPD * 4) % 16 == 0, "part: float4 loads of the merge");
 
 // lap timer (option decode_prof): thread 0 attributes the cycles since the previous lap to bucket i
 #define LAP(i) do { if constexpr (PROF) { if (threadIdx.x == 0) { const long long now_ = clock64(); S.prof[i] += now_ - S.prof_last; S.prof_last = now_; } } } while (0)
@@ -101,7 +107,9 @@ enum { LP_START = 0, LP_WAIT = 1, LP_GEMV = 2, LP_RELEASE = 3, LP_GATHER = 4, LP
        LP_PYR_ATT = 9, LP_PYR_WTS = 10, LP_PYR_TABLE = 11, LP_PYR_STAGE = 12, LP_PYR_DRAIN = 13, LP_PYR_REFILL = 14,
        LP_PYR_LN = 15, LP_PYR_BAR = 16, LP_FRAME = 17,
        // the MMA warpgroup's own laps (thread 128, pyr_mma_rows): they overlap thread 0's
-       LP_WG_AWAIT = 18, LP_WG_MMA = 19, LP_WG_EPI = 20, LP_COUNT };
+       LP_WG_AWAIT = 18, LP_WG_MMA = 19, LP_WG_EPI = 20,
+       // thread 0 again: issuing the next block's parameter and tap prefetch, between its slice stores and the gather wait
+       LP_PREFETCH = 21, LP_COUNT };
 static_assert(LP_COUNT <= DEC_NPROF, "lap buckets");
 
 // NOTE on `__noinline__` in this file: there is none.  With 227 KB of shared memory per CTA the L1 data cache is ~0 KB, so every
@@ -126,11 +134,6 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
 __device__ __forceinline__ void bulk_g2s_mc(void* dst, const void* src, uint32_t bytes, unsigned long long* bar, uint16_t mask) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;"
                  :: "r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)), "h"(mask) : "memory");
-}
-// local shared memory -> a peer CTA's shared memory, completing on the PEER's mbarrier
-__device__ __forceinline__ void bulk_s2peer(uint32_t dst_cluster, const void* src, uint32_t bytes, uint32_t bar_cluster) {
-    asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 :: "r"(dst_cluster), "r"(smem_u32(src)), "r"(bytes), "r"(bar_cluster) : "memory");
 }
 __device__ __forceinline__ void cluster_sync_all() { cluster_arrive(); cluster_wait(); }
 // generic-proxy global stores (the plane histories) -> visible to later bulk copies (async proxy) once a barrier orders them
@@ -299,18 +302,13 @@ __device__ __forceinline__ int layer_row(const DecParams& P, Smem& S, Stream& st
     const int nl_next = last ? 0 : li + 1;
     const int pb = (int)(lcount & 1u);
     const uint32_t gpar = (lcount >> 1) & 1u;
-    const uint32_t gbytes = (uint32_t)(GT * l.ns * 4);
+    const int nh = l.kind + 1;                                      // LayerNorm halves (hc: gate, info)
+    // bytes every rank sends to every rank: its pre-LN slice, and a (mean, M2) LayerNorm partial per (utterance, half)
+    const uint32_t gbytes = (uint32_t)(GT * l.ns * 4), pbytes = (uint32_t)(GT * nh * 8);
 
-    cp_async_wait<0>();                     // this block's taps and parameters (issued one block ago)
-    __syncthreads();                        // ... and every warp has finished the previous block
-    if (tid == 0) mbar_expect_tx(bar64(&S.gbar[pb]), NC * gbytes);
-    // prefetch for the following block: its taps are rows of earlier frames, already in the history
-    if (!last || j + 1 < P.steps) {
-        prefetch_params(P, S, nl_next, rank);
-        // the following block's input vector lives in xin[cb^1]; the attention writes the whole AudioDec C_1 input itself
-        if (nl_next != P.n_enc) prefetch_taps(P, S, nl_next, last ? j + 1 : j, b0, G, cb ^ 1);
-    }
-    cp_async_commit();
+    cp_async_wait<0>();                     // this block's taps and parameters (issued during the previous block)
+    __syncthreads();                        // barrier 1: every warp has finished the previous block (its mix wrote our input)
+    if (tid == 0) mbar_expect_tx(bar64(&S.gbar[pb]), NC * (gbytes + pbytes));
     LAP(LP_START);
 
     if (l.ns == 32) {
@@ -353,57 +351,115 @@ __device__ __forceinline__ int layer_row(const DecParams& P, Smem& S, Stream& st
 #pragma unroll
         for (int g = 0; g < GT; ++g) S.red[g][tid] = acc[g];
     }
-    __syncthreads();
-    // final sums of the slice (one thread per value) -> staging -> one bulk copy per peer (all-gather through distributed
-    // shared memory).  With one utterance the values fit one warp, which then issues the copies without a second block barrier.
+    __syncthreads();                        // barrier 2: every warp's partial sums are in S.red
+    // All-gather from registers: thread (g, n) finishes value n of utterance g of the slice (same order as always: bias, even
+    // and odd warp partials, their sum), and the slice goes to every rank's S.pre[pb][rank] with st.async, four consecutive
+    // columns per store, completing on that rank's gbar[pb].  With it, each LayerNorm half of the slice (16 channels in 16
+    // consecutive lanes; 5 channels in 8 lanes for the n_mels-wide last block) ships its own statistics, pivoted on its first
+    // channel: mean m_r and M2_r = sum (x - m_r)^2, computed as sum d^2 - (sum d) m' with d = x - pivot, m' = mean d.
+    //
+    // Reuse of S.pre[pb] / S.part[pb] (pb = block count mod 2): a rank stores block l + 2's slice only after the GEMV of
+    // l + 2, which needs block l + 1's output, i.e. after its gbar wait of block l + 1, which needs OUR slice of l + 1; we
+    // send that only past barrier 1 of l + 1, which every one of our threads reaches after its last read of block l's
+    // values and partials (statistics merge and mix).  So nothing of l + 2 lands while block l is read.
+    // gbar[pb] parity: the phase of block l completes with our arrive (expect_tx, past barrier 1 of l) and all 16 slices of
+    // l.  A rank's bytes of l + 2 may land before our arrive of l + 2 (the tx count goes negative, the phase cannot complete
+    // without the arrive) but not before the phase of l has completed: they follow our slice of l + 1, which we send after
+    // our gbar wait of l.  Each phase therefore counts exactly one block's bytes, and the wait parity is (count / 2) & 1.
     const int lgns = (l.ns == 32) ? 5 : (l.ns == 16 ? 4 : 3);
+    const int cs = l.cs;
     {
         const int nvals = GT << lgns, ng = NT >> lgns;
-        float* ov = S.outv[pb];
-        if (tid < nvals) {
-            const float* bs = S.prm[li & 1] + 1024;
+        if ((tid & ~31) < nvals) {                                   // warp-uniform: the shuffles below need whole warps
             const int g = tid >> lgns, n = tid & (l.ns - 1);
-            const float* rp = &S.red[g][n];
-            float s0 = bs[n], s1 = 0.f;
+            float v = 0.f;
+            if (tid < nvals) {
+                const float* bs = S.prm[li & 1] + 1024;
+                const float* rp = &S.red[g][n];
+                float s0 = bs[n], s1 = 0.f;
 #pragma unroll 4
-            for (int q = 0; q < ng; q += 2) { s0 += rp[q << lgns]; s1 += rp[(q + 1) << lgns]; }
-            ov[tid] = s0 + s1;
-            fence_proxy_async_smem();
+                for (int q = 0; q < ng; q += 2) { s0 += rp[q << lgns]; s1 += rp[(q + 1) << lgns]; }
+                v = s0 + s1;
+            }
+            const int W = (l.ns == 8) ? 8 : 16, w = lane & (W - 1);  // lanes of one (utterance, half); w = its column
+            const float piv = __shfl_sync(0xffffffffu, v, lane & ~(W - 1));
+            const float d = (w < cs) ? v - piv : 0.f;                // a constant half gives d = 0: mean = pivot, M2 = 0 exactly
+            float s1 = d, s2 = d * d;
+#pragma unroll
+            for (int o = 1; o < 8; o <<= 1) { s1 += __shfl_xor_sync(0xffffffffu, s1, o); s2 += __shfl_xor_sync(0xffffffffu, s2, o); }
+            if (W == 16) { s1 += __shfl_xor_sync(0xffffffffu, s1, 8); s2 += __shfl_xor_sync(0xffffffffu, s2, 8); }
+            const float md = s1 * ((cs == 16) ? (1.0f / 16.0f) : __frcp_rn((float)cs));
+            const float mr = piv + md, m2 = fmaxf(fmaf(-s1, md, s2), 0.f);
+            const int q0 = lane & ~3;
+            const float4 v4 = make_float4(__shfl_sync(0xffffffffu, v, q0), __shfl_sync(0xffffffffu, v, q0 + 1),
+                                          __shfl_sync(0xffffffffu, v, q0 + 2), __shfl_sync(0xffffffffu, v, q0 + 3));
+            if (tid < nvals) {
+                const uint32_t bar = smem_u32(&S.gbar[pb]);
+                const uint32_t vdst = smem_u32(&S.pre[pb][rank][(g << lgns) + (n & ~3)]);
+                const int hf = (l.ns == 32) ? (n >> 4) : 0;
+                const uint32_t pdst = smem_u32(&S.part[pb][2 * g + hf][2 * rank]);
+                // the 4 lanes of a quad hold the same 4 values: each stores them to 4 of the 16 ranks
+#pragma unroll
+                for (int i = 0; i < NC / 4; ++i) {
+                    const uint32_t r = (uint32_t)((lane & 3) + 4 * i);
+                    st_async_v4(mapa(vdst, r), v4, mapa(bar, r));
+                }
+                for (int r = w; r < NC; r += W) st_async_v2(mapa(pdst, (uint32_t)r), mr, m2, mapa(bar, (uint32_t)r));
+            }
         }
-        if (GT > 1) __syncthreads(); else __syncwarp();
-        if (tid < NC)
-            bulk_s2peer(mapa(smem_u32(&S.pre[pb][rank][0]), (uint32_t)tid), ov, gbytes, mapa(smem_u32(&S.gbar[pb]), (uint32_t)tid));
     }
     LAP(LP_GATHER);
-    mbar_wait(bar64(&S.gbar[pb]), gpar);
+    // prefetch for the following block, issued while the peers' slices are in flight: its taps are rows of earlier frames,
+    // already in the history.  prm[nl_next & 1] was last read by the previous block's mix, and the taps go to xin[cb^1][g][0,
+    // 512), which this block's mix does not write (it writes from next_off on) and nobody reads before barrier 1 of the next block.
+    if (!last || j + 1 < P.steps) {
+        prefetch_params(P, S, nl_next, rank);
+        // the following block's input vector lives in xin[cb^1]; the attention writes the whole AudioDec C_1 input itself
+        if (nl_next != P.n_enc) prefetch_taps(P, S, nl_next, last ? j + 1 : j, b0, G, cb ^ 1);
+    }
+    cp_async_commit();
+    LAP(LP_PREFETCH);
+    mbar_wait_cluster(bar64(&S.gbar[pb]), gpar);
     LAP(LP_CBAR);
-    // LayerNorm statistics: one warp per (utterance, half), pivoted single pass (pivot = channel 0: a constant row gives exactly 0,
-    // quirk Q4); then gate / highway mix one thread per channel.  Redundantly in every CTA: the next block's input is local.
+    // LayerNorm statistics from the 16 ranks' partials (Chan's merge, every rank having the same cs channels of a half):
+    // mean = m_0 + sum_r (m_r - m_0) / 16, M2 = sum_r M2_r + cs sum_r (m_r - mean)^2.  Relative to rank 0's mean, so equal
+    // partial means -- a constant row -- give exactly zero variance (quirk Q4).  Lane 2g + hf of EVERY warp merges (g, hf) and
+    // the warp's lanes read the results by shuffle: no block barrier.  Then gate / highway mix one thread per channel.
+    // Redundantly in every CTA: the next block's input is local.
     {
-        const int C = l.cout, cs = l.cs, nh = l.kind + 1;
+        const int C = l.cout;
         const float rC = (C == 256) ? (1.0f / 256.0f) : __frcp_rn((float)C);
+        float mu = 0.f, rs = 0.f;
+        if (lane < 2 * GT && (lane & 1) < nh) {
+            const float* pp = &S.part[pb][lane][0];
+            float4 a[NC / 2];                                         // (m, M2) of ranks 2i and 2i + 1
+#pragma unroll
+            for (int i = 0; i < NC / 2; ++i) a[i] = *reinterpret_cast<const float4*>(pp + 4 * i);
+            const float m0 = a[0].x;
+            float sd0 = 0.f, sd1 = 0.f;                               // even and odd ranks: two independent chains
+#pragma unroll
+            for (int i = 0; i < NC / 2; ++i) { sd0 += a[i].x - m0; sd1 += a[i].z - m0; }
+            mu = m0 + (sd0 + sd1) * (1.0f / NC);
+            float q0 = 0.f, q1 = 0.f, e0 = 0.f, e1 = 0.f;
+#pragma unroll
+            for (int i = 0; i < NC / 2; ++i) {
+                const float d0 = a[i].x - mu, d1 = a[i].z - mu;
+                q0 += a[i].y; q1 += a[i].w;
+                e0 = fmaf(d0, d0, e0); e1 = fmaf(d1, d1, e1);
+            }
+            rs = rsqrtf(fmaxf(fmaf((float)cs, e0 + e1, q0 + q1) * rC, 0.f) + 1e-12f);
+        }
+        float mean[GT][2], rstd[GT][2];
+#pragma unroll
+        for (int g = 0; g < GT; ++g)
+#pragma unroll
+            for (int hf = 0; hf < 2; ++hf) {
+                mean[g][hf] = __shfl_sync(0xffffffffu, mu, 2 * g + hf);
+                rstd[g][hf] = __shfl_sync(0xffffffffu, rs, 2 * g + hf);
+            }
+        LAP(LP_LN);
         // channel c lives in the slice of rank c / cs at column c % cs (cs = 16, or 5 for the n_mels-wide last block)
         auto pre_off = [&](int c) { const int rk = (cs == 16) ? (c >> 4) : ((c * 205) >> 10); return rk * PLD + (c - rk * cs); };
-        for (int pr = warp; pr < GT * nh; pr += NWARP) {
-            const int g = (nh == 2) ? (pr >> 1) : pr, hf = (nh == 2) ? (pr & 1) : 0;
-            const float* base = &S.pre[pb][0][(g << lgns) + hf * cs];
-            const float piv = base[0];
-            float sv = 0.f, qv = 0.f;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const int c = lane + 32 * i;
-                if (c < C) { const float d = base[pre_off(c)] - piv; sv += d; qv = fmaf(d, d, qv); }
-            }
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) { sv += __shfl_xor_sync(0xffffffffu, sv, o); qv += __shfl_xor_sync(0xffffffffu, qv, o); }
-            if (lane == 0) {
-                const float m = sv * rC;
-                S.stat[g][hf][0] = piv + m;
-                S.stat[g][hf][1] = rsqrtf(fmaxf(qv * rC - m * m, 0.f) + 1e-12f);
-            }
-        }
-        __syncthreads();
-        LAP(LP_LN);
         const float* prm = S.prm[li & 1];
         const int cur_off = (l.ntaps - 1) * 256;
         const int next_off = (last || li + 1 == P.n_enc) ? 0 : (P.L[li + 1].ntaps - 1) * 256;
@@ -419,13 +475,13 @@ __device__ __forceinline__ int layer_row(const DecParams& P, Smem& S, Stream& st
 #pragma unroll
             for (int g = 0; g < GT; ++g) {
                 const float* pr = &S.pre[pb][0][g << lgns];
-                o[g] = (pr[po] - S.stat[g][0][0]) * S.stat[g][0][1] * g1 + b1;
+                o[g] = (pr[po] - mean[g][0]) * rstd[g][0] * g1 + b1;
             }
             if (l.kind == 1) {
 #pragma unroll
                 for (int g = 0; g < GT; ++g) {
                     const float* pr = &S.pre[pb][0][g << lgns];
-                    const float h2 = (pr[po + cs] - S.stat[g][1][0]) * S.stat[g][1][1] * g2 + b2;
+                    const float h2 = (pr[po + cs] - mean[g][1]) * rstd[g][1] * g2 + b2;
                     const float h1 = sigmoid_fast(o[g]);
                     o[g] = h1 * h2 + (1.0f - h1) * S.xin[cb][g][cur_off + c];
                 }

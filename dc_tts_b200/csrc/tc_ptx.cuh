@@ -41,6 +41,33 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     while (!mbar_try_wait(bar, parity))
         if (clock64() - t0 > 4000000000ll) __trap();
 }
+// The same wait with acquire semantics at CLUSTER scope: for a phase completed by other CTAs' st.async, whose complete_tx
+// releases their stores at cluster scope.
+__device__ __forceinline__ bool mbar_try_wait_cluster(uint64_t* bar, uint32_t parity) {
+    uint32_t ok;
+    asm volatile(
+        "{\n\t.reg .pred P;\n\t"
+        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 P, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, P;\n\t}"
+        : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
+    return ok != 0;
+}
+__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
+    if (mbar_try_wait_cluster(bar, parity)) return;
+    const long long t0 = clock64();
+    while (!mbar_try_wait_cluster(bar, parity))
+        if (clock64() - t0 > 4000000000ll) __trap();
+}
+// st.async: registers -> shared memory of a CTA of the cluster (dst and bar are shared::cluster addresses, from mapa), the
+// bytes completing as transaction count on that CTA's mbarrier `bar` (which must live in the same CTA as dst)
+__device__ __forceinline__ void st_async_v4(uint32_t dst, float4 v, uint32_t bar) {
+    asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v4.f32 [%0], {%1, %2, %3, %4}, [%5];"
+                 :: "r"(dst), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "r"(bar) : "memory");
+}
+__device__ __forceinline__ void st_async_v2(uint32_t dst, float a, float b, uint32_t bar) {
+    asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v2.f32 [%0], {%1, %2}, [%3];"
+                 :: "r"(dst), "f"(a), "f"(b), "r"(bar) : "memory");
+}
 
 // ---- TMA ----------------------------------------------------------------------------------
 __device__ __forceinline__ void prefetch_tmap(const void* tmap) {

@@ -134,7 +134,7 @@ class Engine:
         """Lap timers (SM cycles) of the last persistent decode run with option decode_prof = 1; see include/dctts.h."""
         names = ["start", "stream_wait", "gemv", "release", "gather", "cluster_barrier", "layernorm", "mix", "attention",
                  "re_attention", "re_weights", "re_table", "re_stage", "re_drain", "re_refill", "re_layernorm", "re_barriers",
-                 "frame", "wg_a_wait", "wg_mma", "wg_epilogue"]
+                 "frame", "wg_a_wait", "wg_mma", "wg_epilogue", "prefetch"]
         v = (C.c_int64 * len(names))()
         self._check(self._lib.dctts_decode_profile(self._h, v, len(names)), "dctts_decode_profile")
         return dict(zip(names, [int(x) for x in v]))

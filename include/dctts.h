@@ -349,7 +349,9 @@ int dctts_decode_stats(dctts_handle h, int32_t* moved_frames, int32_t* moved_utt
  * n <= 24.  Buckets of thread 0, which together cover the kernel: 0 block start, 1 weight-stream wait, 2 GEMV, 3 slot release,
  * 4 all-gather, 5 cluster barrier, 6 LayerNorm, 7 mix, 8 attention, 9 recompute attention; the recompute GEMM as 10 waiting
  * for the block's weight chunks, 11 descriptor table, 12 issuing the A slabs, 13 draining the MMAs and epilogue stores,
- * 14 weight refill and LayerNorm parameters; 15 recompute LayerNorm, 16 recompute barriers, 17 frame bookkeeping.
+ * 14 weight refill and LayerNorm parameters; 15 recompute LayerNorm, 16 recompute barriers, 17 frame bookkeeping;
+ * 21 issuing the next block's parameter and tap prefetch.  In the one-row pass, 4 is finishing the slice and storing it
+ * to every CTA, 5 waiting for the other CTAs' slices, 6 merging their LayerNorm statistics.
  * Buckets of the recompute's MMA warpgroup (thread 128), which overlap the above: 18 waiting for A slabs, 19 issuing the MMAs
  * and waiting for the slab before, 20 epilogue stores. */
 int dctts_decode_profile(dctts_handle h, int64_t* cycles, int32_t n);
