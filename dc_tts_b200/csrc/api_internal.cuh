@@ -154,6 +154,8 @@ struct dctts_handle_s {
         long long n_grad = 0; int n_entries = 0; float* d_table = nullptr;
         DevBuf tc_a_hi, tc_a_lo, tc_b_hi, tc_b_lo, tc_slots;    // operand planes of the wgmma training GEMMs (kernels_gemm_tc.cu)
         GemmTcWs tc;
+        // ordered sums (option train_deterministic): partials of the largest launch at the capacity, allocated while the option is on
+        DevBuf ord_part, ord_dpart; size_t ord_floats = 0; OrderedWs ord;
         int first[3] = {0, 0, 0}, last[3] = {0, 0, 0};         // layer index ranges: TextEnc, AudioEnc, AudioDec
     } tr;
 
@@ -192,6 +194,7 @@ struct dctts_handle_s {
         int decode_mode = 1;      // 1 = persistent cluster kernel (kernels_decode.cu), 0 = one CUDA graph per frame (round-1 path)
         int train_probe = 0;      // measurement only (tools/bench_train.py --probe): the training GEMMs fetch their operands but issue no MMA
         int train_tc = 7;         // training GEMMs on wgmma, bit mask: 1 forward conv, 2 data gradient, 4 weight gradient; 0 = fp32 CUDA-core kernels
+        int train_deterministic = 0;   // 1: the training step's sums in a fixed order (kernels_ordered.cu): a seeded run repeats bit for bit
     } opt;
 
     // persistent decode (kernels_decode.cu)

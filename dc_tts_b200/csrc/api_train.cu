@@ -37,10 +37,23 @@ void train_alloc_ws(H* h, int N, int T) {
     auto& tr = h->tr;
     const dctts_hparams& hp = h->hp;
     const int B = tr.B, d = hp.d, num = tr.num;
-    size_t pre_f = 0, out_f = 0, g_f = 0, dy_f = 0, wt_f = 0, tca_f = 0, tcb_f = 0;
+    size_t pre_f = 0, out_f = 0, g_f = 0, dy_f = 0, wt_f = 0, tca_f = 0, tcb_f = 0, ord_f = 0;
     train_set_shape(h, N, T);                                    // the capacity: every buffer below is sized for it
     for (auto& t : tr.layers) {
         const LayerDev& l = *t.l;
+        {   // the ordered mode's partials: the block backward and the weight gradient on either kernel set, whose split
+            // counts grow with the rows, so the capacity bounds every step
+            ord_f = std::max(ord_f, block_bwd_ordered_floats(t.rows, l.cout, l.kind == K_HC ? 1 : 0));
+            WgradArgs w{};
+            w.K = l.cin;
+            if (l.kind == K_D) {
+                w.rows = (long long)B * t.L_in; w.L = t.L_in; w.N = l.cout; w.ntaps = 1;
+                ord_f = std::max(ord_f, conv_wgrad_ordered_floats(w));
+            } else {
+                w.rows = t.rows; w.L = t.L_in; w.N = l.nconv; w.ntaps = l.size;
+                ord_f = std::max({ord_f, conv_wgrad_ordered_floats(w), conv_wgrad_tc_ordered_floats(w, B)});
+            }
+        }
         t.ld_out = roundup(l.cout, 4);
         pre_f += (size_t)t.rows * l.ldw; out_f += (size_t)t.rows * t.ld_out;
         g_f = std::max(g_f, (size_t)t.rows * std::max(t.ld_out, roundup(l.cin, 4)));
@@ -81,7 +94,31 @@ void train_alloc_ws(H* h, int N, int T) {
         tr.layers[tr.first[0]].in = tr.emb.as<float>(); tr.layers[tr.first[0]].ld_in = hp.e;
         tr.layers[tr.first[2]].in = tr.R.as<float>(); tr.layers[tr.first[2]].ld_in = 2 * d;
     }
+    tr.ord_floats = ord_f;
+    if (h->opt.train_deterministic) { tr.ord_part.ensure(ord_f * sizeof(float)); tr.ord_dpart.ensure(ORD_LOSS_PARTS * sizeof(double)); }
     tr.N_cap = N; tr.T_cap = T;
+}
+
+// The ordered mode's workspace when the option is on (allocated at the first step that needs it), else nullptr: the default
+// kernels.  It outlives the step, like the rest of the shape-dependent workspace.
+const OrderedWs* train_ordered(H* h) {
+    auto& tr = h->tr;
+    if (!h->opt.train_deterministic) return nullptr;
+    tr.ord_part.ensure(std::max<size_t>(tr.ord_floats, 1) * sizeof(float));
+    tr.ord_dpart.ensure(ORD_LOSS_PARTS * sizeof(double));
+    tr.ord.part = tr.ord_part.as<float>(); tr.ord.part_elems = tr.ord_floats;
+    tr.ord.dpart = tr.ord_dpart.as<double>(); tr.ord.dpart_elems = ORD_LOSS_PARTS;
+    return &tr.ord;
+}
+
+// The same for one launch of a test aid (dctts_conv_gemm, dctts_block_bwd, dctts_attn_bwd, dctts_train_loss): `floats`
+// partial floats and the loss partials in the call's own buffers
+const OrderedWs* call_ordered(H* h, DevBuf& part, DevBuf& dpart, size_t floats, OrderedWs& o) {
+    if (!h->opt.train_deterministic) return nullptr;
+    part.ensure(std::max<size_t>(floats, 1) * sizeof(float));
+    dpart.ensure(ORD_LOSS_PARTS * sizeof(double));
+    o.part = part.as<float>(); o.part_elems = floats; o.dpart = dpart.as<double>(); o.dpart_elems = ORD_LOSS_PARTS;
+    return &o;
 }
 
 void train_init(H* h, int B, float rate, int num, int T_in) {
@@ -241,6 +278,7 @@ float* train_bwd(H* h, Launch& lc, int first, int last, int B, uint32_t seed, fl
     auto& tr = h->tr;
     cudaStream_t s = lc.s;
     float* dy = tr.dy.as<float>(); float* wT = tr.wT.as<float>();
+    const OrderedWs* ord = train_ordered(h);
     for (int i = last; i >= first; --i) {
         auto& t = tr.layers[i]; const LayerDev& l = *t.l;
         const int cin_p = roundup(l.cin, 4);
@@ -250,7 +288,7 @@ float* train_bwd(H* h, Launch& lc, int first, int last, int B, uint32_t seed, fl
         a.dg1 = t.dg1; a.db1 = t.db1; a.dg2 = t.dg2; a.db2 = t.db2; a.dbias = t.dbias;
         a.rows = t.rows; a.C = l.cout; a.mode = l.kind == K_HC ? 1 : 0; a.act = l.kind == K_D ? 0 : l.act;
         a.drop = drop_args(tr.rate, t.li, seed);
-        launch_train_block_bwd(a, s); lc.count();
+        lc.count(launch_train_block_bwd(a, s, ord));
         if (t.need_dgrad) {
             if (cin_p != l.cin) CUDA_CHECK(cudaMemsetAsync(wT, 0, (size_t)l.size * l.ldw * cin_p * sizeof(float), s));   // zero pad columns
             launch_transpose_w(l.W, wT, l.size, l.cin, l.ldw, l.ldw, cin_p, s); lc.count();
@@ -266,9 +304,9 @@ float* train_bwd(H* h, Launch& lc, int first, int last, int B, uint32_t seed, fl
             // forward: out[2t] = W0 x[t] + W2 x[t-1], out[2t+1] = W1 x[t]
             const size_t tapsz = (size_t)l.cin * l.ldw;
             w.rows = (long long)B * t.L_in; w.ldy = 2 * l.ldw; w.N = l.cout; w.ntaps = 1;
-            w.dy = dy;         w.dW = t.dW + 0 * tapsz; w.shifts[0] = 0;  launch_conv_wgrad(w, s); lc.count();
-            w.dy = dy;         w.dW = t.dW + 2 * tapsz; w.shifts[0] = -1; launch_conv_wgrad(w, s); lc.count();
-            w.dy = dy + l.ldw; w.dW = t.dW + 1 * tapsz; w.shifts[0] = 0;  launch_conv_wgrad(w, s); lc.count();
+            w.dy = dy;         w.dW = t.dW + 0 * tapsz; w.shifts[0] = 0;  lc.count(launch_conv_wgrad(w, s, ord));
+            w.dy = dy;         w.dW = t.dW + 2 * tapsz; w.shifts[0] = -1; lc.count(launch_conv_wgrad(w, s, ord));
+            w.dy = dy + l.ldw; w.dW = t.dW + 1 * tapsz; w.shifts[0] = 0;  lc.count(launch_conv_wgrad(w, s, ord));
             if (!t.need_dgrad) continue;
             // dx[u] = dyE[u] W0^T + dyE[u+1] W2^T + dyO[u] W1^T
             c.K = l.cout;
@@ -280,8 +318,8 @@ float* train_bwd(H* h, Launch& lc, int first, int last, int B, uint32_t seed, fl
             w.rows = t.rows; w.dy = dy; w.ldy = l.ldw; w.dW = t.dW; w.N = l.nconv; w.ntaps = l.size;
             layer_shifts(l, t.extra_shift, w.shifts);
             GemmTcSlots gs{t.tc_slots.x, nullptr};                   // X's abs-max is known from the forward; dy's is computed once, for both gradients
-            if ((h->opt.train_tc & 4) && conv_wgrad_tc_ok(w, B, tr.tc)) lc.count(launch_conv_wgrad_tc(w, B, tr.tc, s, &gs));
-            else { launch_conv_wgrad(w, s); lc.count(); }
+            if ((h->opt.train_tc & 4) && conv_wgrad_tc_ok(w, B, tr.tc)) lc.count(launch_conv_wgrad_tc(w, B, tr.tc, s, &gs, ord));
+            else lc.count(launch_conv_wgrad(w, s, ord));
             if (!t.need_dgrad) continue;
             c.X = dy; c.ldx = l.ldw; c.ntaps = l.size;
             for (int j = 0; j < l.size; ++j) { c.taps[j].W = wT + (size_t)j * tsz; c.taps[j].shift = -w.shifts[j]; }
@@ -345,8 +383,8 @@ void train_forward(H* h, Launch& lc, const int* L, int N, const float* mels, int
                       nullptr, nullptr, nullptr);
     train_fwd(h, lc, tr.first[2], tr.last[2], B, seed);
     const auto& lastl = tr.layers[tr.last[2]];
-    launch_train_loss(lastl.out, lastl.ld_out, mels, tr.gbuf[0].as<float>(), lastl.ld_out, tr.sums.as<double>(), (long long)B * T, hp.n_mels, s);
-    lc.count();
+    lc.count(launch_train_loss(lastl.out, lastl.ld_out, mels, tr.gbuf[0].as<float>(), lastl.ld_out, tr.sums.as<double>(), (long long)B * T,
+                               hp.n_mels, s, train_ordered(h)));
 }
 
 // The attention backward's arguments: gR (B,T,2d) = the gradient of [ctx ; Q], Q (B,T,d), KV (B,N,2d) = [K | V], align
@@ -376,11 +414,11 @@ void train_forward_backward(H* h, const int* L, int N, const float* mels, int T,
     const int n_lim = std::min(N, hp.max_N), t_lim = std::min(T, hp.max_T);      // the crop of train.py:91 to the table
     const AttnBwdArgs ab = attn_bwd_args(gR, Q, KV, tr.align.as<float>(), tr.gts.as<float>(), hp.max_T, tr.dS.as<float>(),
                                          tr.gbuf[2].as<float>(), tr.gbuf[3].as<float>(), B, T, N, d, n_lim, t_lim);
-    launch_attn_bwd(ab, tr.sums.as<double>(), s); lc.count(3);
+    lc.count(launch_attn_bwd(ab, tr.sums.as<double>(), s, train_ordered(h)));
     float* free_a = (gR == tr.gbuf[0].as<float>()) ? tr.gbuf[1].as<float>() : tr.gbuf[0].as<float>();
     train_bwd(h, lc, tr.first[1], tr.last[1], B, seed, tr.gbuf[2].as<float>(), free_a);
     float* gEmb = train_bwd(h, lc, tr.first[0], tr.last[0], B, seed, tr.gbuf[3].as<float>(), free_a);
-    launch_embed_bwd(L, gEmb, tr.d_table, B * N, hp.e, s); lc.count();
+    lc.count(launch_embed_bwd(L, gEmb, tr.d_table, B * N, hp.e, hp.vocab_size, s, train_ordered(h)));
     CUDA_CHECK(cudaGetLastError());
     train_read_losses(h, losses_host, (double)B * T * hp.n_mels, (double)B * n_lim * t_lim, s);
 }
@@ -395,7 +433,8 @@ void train_eval(H* h, const int* L, int N, const float* mels, int T, int B, uint
     Launch lc{h, s};
     train_forward(h, lc, L, N, mels, T, B, seed);
     const int n_lim = std::min(N, hp.max_N), t_lim = std::min(T, hp.max_T);
-    launch_attn_loss(tr.align.as<float>(), tr.gts.as<float>(), hp.max_T, tr.sums.as<double>(), B, N, T, n_lim, t_lim, s); lc.count();
+    lc.count(launch_attn_loss(tr.align.as<float>(), tr.gts.as<float>(), hp.max_T, tr.sums.as<double>(), B, N, T, n_lim, t_lim, s,
+                              train_ordered(h)));
     if (Y_out) {
         const auto& lastl = tr.layers[tr.last[2]];
         launch_sigmoid_rows(lastl.out, lastl.ld_out, Y_out, (long long)B * T, hp.n_mels, s); lc.count();
@@ -421,7 +460,8 @@ void train_forward_ssrn(H* h, Launch& lc, const float* mels, const float* mags, 
     const int last = (int)tr.layers.size() - 1;
     train_fwd(h, lc, 0, last, B, seed);
     const auto& ll = tr.layers[last];
-    launch_train_loss(ll.out, ll.ld_out, mags, tr.gbuf[0].as<float>(), ll.ld_out, tr.sums.as<double>(), ll.rows, ll.l->cout, s); lc.count();
+    lc.count(launch_train_loss(ll.out, ll.ld_out, mags, tr.gbuf[0].as<float>(), ll.ld_out, tr.sums.as<double>(), ll.rows, ll.l->cout, s,
+                               train_ordered(h)));
 }
 
 void train_forward_backward_ssrn(H* h, const float* mels, const float* mags, int B, int T, uint32_t seed, float* losses_host,
@@ -490,6 +530,7 @@ int dctts_conv_gemm(dctts_handle h, int32_t impl, int32_t mode, const float* X, 
                     const float* Wd, int32_t ldwd, int32_t N, int32_t ntaps, const int32_t* shifts_host, const float* bias,
                     int32_t accumulate, float* out, int32_t ldo, void* stream) {
     DevBuf bufs[5];                                 // the call's own wgmma workspace, freed on every exit
+    DevBuf ord_part, ord_dpart;                     // and its ordered-mode partials (option train_deterministic)
     return guarded(h, [&] {
         REQUIRE(impl == 0 || impl == 1, "dctts_conv_gemm: impl must be 0 (fp32 CUDA cores) or 1 (wgmma)");
         REQUIRE(mode == 0 || mode == 1, "dctts_conv_gemm: mode must be 0 (conv) or 1 (weight gradient)");
@@ -536,10 +577,12 @@ int dctts_conv_gemm(dctts_handle h, int32_t impl, int32_t mode, const float* X, 
             w.X = X; w.ldx = ldx; w.dy = Wd; w.ldy = ldwd; w.dW = out; w.ldw = ldo;
             w.rows = (long long)B * L; w.L = L; w.K = K; w.N = N; w.ntaps = ntaps;
             for (int j = 0; j < ntaps; ++j) w.shifts[j] = shifts_host[j];
-            if (impl == 0) launch_conv_wgrad(w, s);
+            OrderedWs o;
+            const OrderedWs* ord = call_ordered(h, ord_part, ord_dpart, impl == 0 ? conv_wgrad_ordered_floats(w) : conv_wgrad_tc_ordered_floats(w, B), o);
+            if (impl == 0) launches = launch_conv_wgrad(w, s, ord);
             else {
                 REQUIRE(conv_wgrad_tc_ok(w, B, ws), "dctts_conv_gemm: conv_wgrad_tc_ok does not hold for this call");
-                launches = launch_conv_wgrad_tc(w, B, ws, s);
+                launches = launch_conv_wgrad_tc(w, B, ws, s, nullptr, ord);
             }
         }
         h->launches += launches;
@@ -551,6 +594,7 @@ int dctts_conv_gemm(dctts_handle h, int32_t impl, int32_t mode, const float* X, 
 int dctts_block_bwd(dctts_handle h, int32_t mode, int32_t act, int64_t rows, int32_t C, const float* pre, int32_t ldy,
                     const float* gout, int32_t ldg, const float* X, int32_t ldx, const float* ln, float dropout_rate, int32_t layer,
                     uint32_t seed, float* dy, float* gin, float* dparams, void* stream) {
+    DevBuf ord_part, ord_dpart;                     // the call's ordered-mode partials (option train_deterministic)
     return guarded(h, [&] {
         REQUIRE(mode == 0 || mode == 1, "dctts_block_bwd: mode must be 0 (conv1d / transposed conv) or 1 (highway)");
         REQUIRE(act == 0 || act == 1, "dctts_block_bwd: act must be 0 (none) or 1 (ReLU)");
@@ -566,8 +610,9 @@ int dctts_block_bwd(dctts_handle h, int32_t mode, int32_t act, int64_t rows, int
         a.dg1 = dparams; a.db1 = dparams + C; a.dg2 = dparams + 2 * C; a.db2 = dparams + 3 * C; a.dbias = dparams + 4 * C;
         a.rows = rows; a.C = C; a.mode = mode; a.act = act;
         a.drop = drop_args(dropout_rate, layer, seed);
-        launch_train_block_bwd(a, s);              // refuses a width no kernel instantiation covers before launching
-        h->launches += 1;
+        OrderedWs o;
+        const OrderedWs* ord = call_ordered(h, ord_part, ord_dpart, block_bwd_ordered_floats(rows, C, mode), o);
+        h->launches += launch_train_block_bwd(a, s, ord);   // refuses a width no kernel instantiation covers before launching
         CUDA_CHECK(cudaGetLastError());
         CUDA_CHECK(cudaStreamSynchronize(s));
     });
@@ -577,6 +622,7 @@ int dctts_attn_bwd(dctts_handle h, const float* gR, const float* Q, const float*
                    int32_t ld_gts, int32_t B, int32_t T, int32_t N, int32_t n_lim, int32_t t_lim, float* gQ, float* gKV, double* sums,
                    void* stream) {
     DevBuf dS;                                      // the call's own dS scratch, freed on every exit
+    DevBuf ord_part, ord_dpart;                     // and its ordered-mode partials (option train_deterministic)
     return guarded(h, [&] {
         REQUIRE(gR && Q && KV && align && gts && gQ && gKV && sums && B >= 1 && T >= 1 && N >= 1, "dctts_attn_bwd: bad arguments");
         AttnBwdArgs a = attn_bwd_args(gR, Q, KV, align, gts, ld_gts, nullptr, gQ, gKV, B, T, N, h->hp.d, n_lim, t_lim);
@@ -584,8 +630,8 @@ int dctts_attn_bwd(dctts_handle h, const float* gR, const float* Q, const float*
         dS.ensure((size_t)B * T * N * sizeof(float));
         a.dS = dS.as<float>();
         cudaStream_t s = S(h, stream);
-        launch_attn_bwd(a, sums, s);
-        h->launches += 3;
+        OrderedWs o;
+        h->launches += launch_attn_bwd(a, sums, s, call_ordered(h, ord_part, ord_dpart, 0, o));
         CUDA_CHECK(cudaGetLastError());
         CUDA_CHECK(cudaStreamSynchronize(s));      // before the scratch is freed
     });
@@ -593,12 +639,13 @@ int dctts_attn_bwd(dctts_handle h, const float* gR, const float* Q, const float*
 
 int dctts_train_loss(dctts_handle h, const float* logits, int32_t ldl, const float* target, int64_t rows, int32_t C, float* dlogits,
                      int32_t ldg, float* Y, double* sums, void* stream) {
+    DevBuf ord_part, ord_dpart;                     // the call's ordered-mode partials (option train_deterministic)
     return guarded(h, [&] {
         REQUIRE(logits && target && dlogits && sums && rows >= 1 && C >= 1, "dctts_train_loss: bad arguments");
         REQUIRE(ldl >= C && ldg >= C, "dctts_train_loss: a pitch is narrower than its tensor's width");
         cudaStream_t s = S(h, stream);
-        launch_train_loss(logits, ldl, target, dlogits, ldg, sums, rows, C, s);
-        h->launches += 1;
+        OrderedWs o;
+        h->launches += launch_train_loss(logits, ldl, target, dlogits, ldg, sums, rows, C, s, call_ordered(h, ord_part, ord_dpart, 0, o));
         if (Y) { launch_sigmoid_rows(logits, ldl, Y, rows, C, s); h->launches += 1; }
         CUDA_CHECK(cudaGetLastError());
         CUDA_CHECK(cudaStreamSynchronize(s));

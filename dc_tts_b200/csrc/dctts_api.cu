@@ -15,6 +15,7 @@ const Option kOptions[] = {
     {"fused_ln", &H::Options::fused_ln, 2},       {"decode_mode", &H::Options::decode_mode, 2},
     {"decode_prof", &H::Options::decode_prof, 2}, {"decode_force_prepass", &H::Options::decode_force_prepass, 2},
     {"train_tc", &H::Options::train_tc, 7},       {"train_probe", &H::Options::train_probe, 2},
+    {"train_deterministic", &H::Options::train_deterministic, 1},
 };
 
 const Option* find_option(const char* name) {

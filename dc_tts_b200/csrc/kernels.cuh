@@ -230,23 +230,54 @@ struct AttnBwdArgs {
     int n_lim, t_lim;                  // the guided-attention crop: min(N, max_N), min(T, max_T); keys / frames past it get no term
 };
 struct AdamEntry { float* p; float* g; float* m; float* v; long long n; };
+// Ordered sums (option "train_deterministic", kernels_ordered.cu): a launcher given an OrderedWs writes every partial sum to
+// `part` / `dpart` with plain stores in a fixed layout, then one ordered reduction adds the partials in a fixed order and
+// does the single read-modify-write of the destination -- no float atomics, and no split count read from the device.
+// Without one (nullptr) the launchers run the default kernels, which add with float atomics.  Every summing launcher
+// returns the number of kernels it launched.
+struct OrderedWs {
+    float* part = nullptr; size_t part_elems = 0;      // weight-gradient and block-backward partials
+    double* dpart = nullptr; size_t dpart_elems = 0;   // loss partials (ORD_LOSS_PARTS x 2)
+};
+constexpr int ORD_LOSS_CTAS = 1024;                    // fixed grid of the ordered loss kernels: at most this many partial rows
+constexpr size_t ORD_LOSS_PARTS = 2 * ORD_LOSS_CTAS;   // doubles of OrderedWs::dpart
+// floats of OrderedWs::part the ordered path of each launcher needs (0: it adds each element once and needs none)
+size_t block_bwd_ordered_floats(long long rows, int C, int mode);
+size_t conv_wgrad_ordered_floats(const WgradArgs& w);
+size_t conv_wgrad_tc_ordered_floats(const WgradArgs& w, int B);
+int conv_wgrad_ordered_splits(const WgradArgs& w);    // row splits of the fp32 weight gradient in the ordered mode
 void launch_train_dropout(float* x, long long rows, int C, int ld, const DropArgs& d, cudaStream_t s);
-void launch_train_loss(const float* logits, int ldl, const float* target, float* dlogits, int ldg, double* sums, long long rows, int C,
-                       cudaStream_t s);
-void launch_train_block_bwd(const BlockBwdArgs& a, cudaStream_t s);
-void launch_conv_wgrad(WgradArgs a, cudaStream_t s);
+int launch_train_loss(const float* logits, int ldl, const float* target, float* dlogits, int ldg, double* sums, long long rows, int C,
+                      cudaStream_t s, const OrderedWs* ord = nullptr);
+int launch_train_block_bwd(const BlockBwdArgs& a, cudaStream_t s, const OrderedWs* ord = nullptr);
+int launch_conv_wgrad(WgradArgs a, cudaStream_t s, const OrderedWs* ord = nullptr);
 void launch_transpose_w(const float* W, float* WT, int ntaps, int K, int N, int ldw, int Kp, cudaStream_t s);
-void launch_attn_bwd(const AttnBwdArgs& a, double* sums, cudaStream_t s);
+int launch_attn_bwd(const AttnBwdArgs& a, double* sums, cudaStream_t s, const OrderedWs* ord = nullptr);
 // what launch_attn_bwd refuses before it launches anything: d != 256, a crop outside (N, T) or wider than the table's stride
 void check_attn_bwd(const AttnBwdArgs& a);
-// the guided-attention sum alone (the first kernel of launch_attn_bwd): sums[2] += sum over the (n_lim, t_lim) corner of |A gts|
-void launch_attn_loss(const float* align, const float* gts, int ld_gts, double* sums, int B, int N, int T, int n_lim, int t_lim,
-                      cudaStream_t s);
+// the guided-attention sum alone (the first kernel(s) of launch_attn_bwd): sums[2] += sum over the (n_lim, t_lim) corner of |A gts|
+int launch_attn_loss(const float* align, const float* gts, int ld_gts, double* sums, int B, int N, int T, int n_lim, int t_lim,
+                     cudaStream_t s, const OrderedWs* ord = nullptr);
 // out (rows, C) dense = sigmoid(x), x (rows, C) with leading dimension ldx
 void launch_sigmoid_rows(const float* x, int ldx, float* out, long long rows, int C, cudaStream_t s);
 void launch_guided_attention(float* W, int N, int T, cudaStream_t s);
-void launch_embed_bwd(const int* ids, const float* g, float* dtable, int rows, int e, cudaStream_t s);
+// dtable[id] += g[row] for every row with ids[row] = id in [1, vocab) (row 0 of the table gets no gradient)
+int launch_embed_bwd(const int* ids, const float* g, float* dtable, int rows, int e, int vocab, cudaStream_t s,
+                     const OrderedWs* ord = nullptr);
 void launch_adam(const AdamEntry* entries_dev, int n_entries, float lr_t, float beta1, float beta2, float eps, cudaStream_t s);
+// the ordered kernels behind the launchers above (kernels_ordered.cu)
+template <int MAXV, bool HC> int launch_train_block_bwd_ordered(const BlockBwdArgs& a, const OrderedWs& o, cudaStream_t s);
+int launch_conv_wgrad_ordered(const WgradArgs& a, const OrderedWs& o, cudaStream_t s);     // a.nsplit, a.rows_per_split set
+int launch_train_loss_ordered(const float* logits, int ldl, const float* target, float* dlogits, int ldg, double* sums, long long rows,
+                              int C, const OrderedWs& o, cudaStream_t s);
+int launch_attn_loss_ordered(const float* align, const float* gts, int ld_gts, double* sums, int B, int N, int T, int n_lim, int t_lim,
+                             const OrderedWs& o, cudaStream_t s);
+int launch_embed_bwd_ordered(const int* ids, const float* g, float* dtable, int rows, int e, int vocab, cudaStream_t s);
+// dst += the sum over p of part[p][0, width), split into up to 5 destinations: column col0 + i of a segment goes to
+// dst[(i / n) ld + i % n] when i % n < w (partial rows padded past a destination row's w columns skip the padding)
+struct ColSeg { void* dst = nullptr; long long col0 = 0; int n = 1, w = 1, ld = 1; };
+struct ColSegs { int nseg = 0; ColSeg s[5]; };
+template <typename T> void launch_ordered_colsum(const T* part, long long nparts, long long width, const ColSegs& sg, cudaStream_t s);
 
 // ---- the training GEMMs on wgmma (kernels_gemm_tc.cu): drop-ins for launch_conv_gemm (tiled path) / launch_conv_wgrad ----
 struct GemmTcWs {
@@ -260,7 +291,7 @@ bool conv_gemm_tc_ok(const ConvArgs& c, const GemmTcWs& ws);
 struct GemmTcSlots { unsigned* x = nullptr; unsigned* w = nullptr; };   // in: abs-max already known (same tensor converted earlier this step); out: the slots used
 int launch_conv_gemm_tc(const ConvArgs& c, GemmTcWs& ws, cudaStream_t s, GemmTcSlots* io = nullptr);
 bool conv_wgrad_tc_ok(const WgradArgs& w, int B, const GemmTcWs& ws);
-int launch_conv_wgrad_tc(const WgradArgs& w, int B, GemmTcWs& ws, cudaStream_t s, GemmTcSlots* io = nullptr);
+int launch_conv_wgrad_tc(const WgradArgs& w, int B, GemmTcWs& ws, cudaStream_t s, GemmTcSlots* io = nullptr, const OrderedWs* ord = nullptr);
 
 // ---- weight packers (kernels_pack.cu): fp32 W [tap][cin][ldw] -> wgmma planes and the persistent decode's stream ----
 constexpr int PACK_MAXL = 64;  // layers of one abs-max launch (the four networks have 54)

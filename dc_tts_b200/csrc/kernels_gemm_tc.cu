@@ -13,7 +13,8 @@
 //           zero fill is the zero padding;  B = weight planes [n][tap * Kp + k].
 //   mode 1: A = TRANSPOSED activation planes (tap, B, C, L) box {32 t, 128 k, 1 b} (one pre-shifted copy per tap), B = transposed
 //           gradient planes (B, N, L) box {32 t, bn n, 1 b}; the reduction runs over (b, t-block), split over CTAs, and the
-//           partial tiles are added to dW with vector reductions (red.global.add.v4.f32).
+//           partial tiles are added to dW with vector reductions (red.global.add.v4.f32) -- or, in the ordered mode
+//           (kernels_ordered.cu), stored to part[split][tap][K][ldp] and added up in split order by the ordered reduction.
 // One 128 x bn accumulator tile per CTA (bn <= 256), 32-wide slabs, up to four pipeline stages.  Warp 0 = TMA producer,
 // warpgroups 1 and 2 = wgmma consumers of rows 0-63 / 64-127 (fp32 register accumulators), which then write the tile to
 // shared memory (over the drained ring) and store it one row per thread, each warpgroup half of the columns.
@@ -48,6 +49,7 @@ struct GemmTcArgs {
     int tblocks, nb_per_split, B, ksplit, K;
     float* dW; int ldw; long long tap_stride;
     const unsigned* slot_a; const unsigned* slot_b;
+    float* part; int ldp;     // mode 1, ordered: the split tiles go to part (null: added to dW)
     int probe;                // measurement only: 1 = the operands are fetched but no MMA is issued and nothing is stored
 };
 
@@ -59,6 +61,9 @@ __host__ __device__ inline int g_ring_bytes(int stages, int bn) {
     return ((ring > acc ? ring : acc) + 1023) & ~1023;
 }
 
+// PART: mode 1 in the ordered mode, the split tiles stored to a.part (a separate instantiation, so that the default
+// kernel's code is not touched by it)
+template <bool PART>
 __global__ void __launch_bounds__(G_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constant__ CUtensorMap mapA_lo,
                const __grid_constant__ CUtensorMap mapB_hi, const __grid_constant__ CUtensorMap mapB_lo, const GemmTcArgs a) {
@@ -203,7 +208,17 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA_hi, const __grid_constan
         }
     } else {
         const int k = m0 + r;
-        if (k < a.K) {
+        if (PART && k < a.K) {
+            const int split = blockIdx.z - tap * a.ksplit, ntaps = gridDim.z / a.ksplit;
+            float* prow = a.part + (((size_t)split * ntaps + tap) * a.K + k) * a.ldp;
+            for (int c = c_beg; c < c_end; c += 4) {
+                const int n = n0 + c;
+                if (n < a.ldp) {
+                    const float4 v = *reinterpret_cast<const float4*>(arow + c);
+                    *reinterpret_cast<float4*>(prow + n) = make_float4(v.x * inv, v.y * inv, v.z * inv, v.w * inv);
+                }
+            }
+        } else if (!PART && k < a.K) {
             float* wrow = a.dW + (size_t)tap * a.tap_stride + (size_t)k * a.ldw;
             for (int c = c_beg; c < c_end; c += 4) {
                 const int n = n0 + c;
@@ -364,7 +379,8 @@ void prepare_gemm_kernel() {
     int dev = 0;
     cudaGetDevice(&dev);
     if (done[dev & 63]) return;
-    cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) throw std::runtime_error(std::string("cudaFuncSetAttribute(gemm_tc_kernel): ") + cudaGetErrorString(e));
     done[dev & 63] = true;
 }
@@ -377,7 +393,8 @@ void launch_gemm(const CUtensorMap m[4], GemmTcArgs& a, dim3 grid, cudaStream_t 
     a.stages = G_MAX_STAGES;
     while (a.stages > 2 && (size_t)g_ring_bytes(a.stages, a.bn) + G_AUX + 1024 > (size_t)227 * 1024) --a.stages;
     const size_t smem = (size_t)g_ring_bytes(a.stages, a.bn) + G_AUX + 1024;
-    gemm_tc_kernel<<<grid, G_THREADS, smem, s>>>(m[0], m[1], m[2], m[3], a);
+    if (a.part) gemm_tc_kernel<true><<<grid, G_THREADS, smem, s>>>(m[0], m[1], m[2], m[3], a);
+    else gemm_tc_kernel<false><<<grid, G_THREADS, smem, s>>>(m[0], m[1], m[2], m[3], a);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) throw std::runtime_error(std::string("gemm_tc_kernel launch: ") + cudaGetErrorString(e));
 }
@@ -447,9 +464,29 @@ bool conv_wgrad_tc_ok(const WgradArgs& w, int B, const GemmTcWs& ws) {
     return (size_t)w.ntaps * B * w.K * ldt <= ws.a_elems && (size_t)B * w.N * ldt <= ws.b_elems;
 }
 
+// The split over the batch: about `target` CTAs in all, each split a whole number of batch elements, none empty
+static void wgrad_tc_split(int B, int base, int target, int& ksplit, int& nb_per_split) {
+    const int k = std::max(1, std::min(B, (target + base - 1) / base));
+    nb_per_split = (B + k - 1) / k;
+    ksplit = (B + nb_per_split - 1) / nb_per_split;
+}
+
+// The ordered mode's fixed target: two CTAs per SM of a 132-SM H100 SXM, a constant so that the split -- and with it the
+// order of the sums -- does not depend on the device
+constexpr int G_ORDERED_CTAS = 264;
+
+static int wgrad_tc_base(const WgradArgs& w) { return ((w.N + pick_bn(w.N) - 1) / pick_bn(w.N)) * ((w.K + G_BM - 1) / G_BM) * w.ntaps; }
+
+size_t conv_wgrad_tc_ordered_floats(const WgradArgs& w, int B) {
+    int ksplit, nb;
+    wgrad_tc_split(B, wgrad_tc_base(w), G_ORDERED_CTAS, ksplit, nb);
+    return ksplit > 1 ? (size_t)ksplit * w.ntaps * w.K * roundup_i(w.N, 4) : 0;
+}
+
 // dW[tap][k][n] += sum_rows X[b, t + shift_tap, k] dy[b, t, n] -- same contract as launch_conv_wgrad (taps contiguous:
-// dW + tap * K * ldw).  io: x = slot of X, w = slot of dy (see above).  Returns the number of kernels launched.
-int launch_conv_wgrad_tc(const WgradArgs& w, int B, GemmTcWs& ws, cudaStream_t s, GemmTcSlots* io) {
+// dW + tap * K * ldw).  io: x = slot of X, w = slot of dy (see above).  ord: the ordered mode (kernels.cuh: OrderedWs).
+// Returns the number of kernels launched.
+int launch_conv_wgrad_tc(const WgradArgs& w, int B, GemmTcWs& ws, cudaStream_t s, GemmTcSlots* io, const OrderedWs* ord) {
     const int L = w.L, ldt = roundup_i(L, 8);
     int launches = 3;
     unsigned* sa = io ? io->x : nullptr;
@@ -470,15 +507,32 @@ int launch_conv_wgrad_tc(const WgradArgs& w, int B, GemmTcWs& ws, cudaStream_t s
     GemmTcArgs a{};
     a.mode = 1; a.bn = bn; a.N = w.N; a.K = w.K; a.B = B; a.tblocks = (L + G_BK - 1) / G_BK;
     const int base = n_tiles * k_tiles * w.ntaps;
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    int ksplit = std::max(1, std::min(B, (2 * sms + base - 1) / base));
-    a.nb_per_split = (B + ksplit - 1) / ksplit;
-    a.ksplit = (B + a.nb_per_split - 1) / a.nb_per_split;          // no empty split
+    int target = G_ORDERED_CTAS;
+    if (!ord) {
+        int dev = 0, sms = 132;
+        cudaGetDevice(&dev);
+        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+        target = 2 * sms;
+    }
+    wgrad_tc_split(B, base, target, a.ksplit, a.nb_per_split);
     a.dW = w.dW; a.ldw = w.ldw; a.tap_stride = (long long)w.K * w.ldw;
     a.slot_a = sa; a.slot_b = sb; a.probe = ws.probe;
+    // one split adds each element once: no order to fix.  The ingest probe stores nothing, so it has nothing to reduce.
+    if (ord && a.ksplit > 1 && !ws.probe) {
+        a.ldp = roundup_i(w.N, 4);
+        const size_t need = (size_t)a.ksplit * w.ntaps * w.K * a.ldp;
+        if (need > ord->part_elems)
+            throw std::runtime_error("gemm_tc weight gradient: the ordered reduction needs " + std::to_string(need) +
+                                     " partial floats, the workspace holds " + std::to_string(ord->part_elems));
+        a.part = ord->part;
+    }
     launch_gemm(m, a, dim3((unsigned)n_tiles, (unsigned)k_tiles, (unsigned)(w.ntaps * a.ksplit)), s);
+    if (a.part) {
+        ColSegs sg;
+        sg.nseg = 1; sg.s[0] = ColSeg{w.dW, 0, a.ldp, w.N, w.ldw};
+        launch_ordered_colsum<float>(a.part, a.ksplit, (long long)w.ntaps * w.K * a.ldp, sg, s);
+        ++launches;
+    }
     if (io) { io->x = sa; io->w = sb; }
     return launches;
 }

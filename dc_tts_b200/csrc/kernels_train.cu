@@ -12,7 +12,10 @@
 //                            negated shifts (conv_gemm_tiled, accumulate flag for the highway residual)
 //   attn_bwd_q_kernel / attn_bwd_kv_kernel   softmax attention backward incl. the guided-attention term
 //   embed_bwd_kernel, adam_kernel
+// The launchers of the summing kernels take an optional OrderedWs: with it they run the ordered kernels of
+// kernels_ordered.cu instead (option "train_deterministic"), and return the number of kernels launched either way.
 #include "kernels.cuh"
+#include "kernels_train.cuh"
 #include "numerics.cuh"
 
 #include <cmath>
@@ -46,15 +49,9 @@ __global__ void train_loss_kernel(const float* __restrict__ logits, int ldl, con
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     double l1 = 0.0, bce = 0.0;
     if (i < n) {
-        const long long row = i / C;
-        const int c = (int)(i - row * C);
-        const float x = logits[row * ldl + c], m = target[i];
-        const float y = sigmoid_acc(x);
-        const float d = y - m;
-        l1 = fabsf(d);
-        bce = fmaxf(x, 0.f) - x * m + log1pf(expf(-fabsf(x)));
-        const float sg = d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f);
-        dlogits[row * ldg + c] = (sg * y * (1.0f - y) + d) / (float)n;
+        float e1, e2;
+        loss_element(logits, ldl, target, dlogits, ldg, i, n, C, e1, e2);
+        l1 = e1; bce = e2;
     }
     for (int o = 16; o > 0; o >>= 1) { l1 += __shfl_xor_sync(0xffffffffu, l1, o); bce += __shfl_xor_sync(0xffffffffu, bce, o); }
     const int w = threadIdx.x >> 5;
@@ -67,10 +64,12 @@ __global__ void train_loss_kernel(const float* __restrict__ logits, int ldl, con
     }
 }
 
-void launch_train_loss(const float* logits, int ldl, const float* target, float* dlogits, int ldg, double* sums, long long rows, int C,
-                       cudaStream_t s) {
+int launch_train_loss(const float* logits, int ldl, const float* target, float* dlogits, int ldg, double* sums, long long rows, int C,
+                      cudaStream_t s, const OrderedWs* ord) {
+    if (ord) return launch_train_loss_ordered(logits, ldl, target, dlogits, ldg, sums, rows, C, *ord, s);
     const long long n = rows * C;
     train_loss_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(logits, ldl, target, dlogits, ldg, sums, n, C);
+    return 1;
 }
 
 // Y = sigmoid(logits) packed from the ld-pitched last block (train.py:68,72), for an evaluation of the training graph
@@ -87,39 +86,7 @@ void launch_sigmoid_rows(const float* x, int ldx, float* out, long long rows, in
 }
 
 // ------------------------------------------------------------------------------------ block backward
-// LayerNorm backward for one half held in registers.  yhat = (y - mean) rstd, z = yhat g + b.
-//   dy = rstd (dyh - mean(dyh) - yhat mean(dyh yhat)),  dyh = dz g
-template <int MAXV>
-__device__ __forceinline__ void ln_bwd_half(const float (&yhat)[MAXV], const float (&dz)[MAXV], const float* __restrict__ gam,
-                                            int C, int lane, float rstd, float (&dy)[MAXV]) {
-    float s1 = 0.f, s2 = 0.f;
-#pragma unroll
-    for (int i = 0; i < MAXV; ++i) {
-        const int c = lane + 32 * i;
-        if (c < C) { const float t = dz[i] * __ldg(gam + c); dy[i] = t; s1 += t; s2 = fmaf(t, yhat[i], s2); }
-        else dy[i] = 0.f;
-    }
-    s1 = warp_sum(s1) / (float)C; s2 = warp_sum(s2) / (float)C;
-#pragma unroll
-    for (int i = 0; i < MAXV; ++i) dy[i] = rstd * (dy[i] - s1 - yhat[i] * s2);
-}
-
-template <int MAXV>
-__device__ __forceinline__ void ln_fwd_half(const float* __restrict__ y, int C, int lane, float (&yhat)[MAXV], float& rstd) {
-    float s = 0.f;
-#pragma unroll
-    for (int i = 0; i < MAXV; ++i) { const int c = lane + 32 * i; yhat[i] = c < C ? y[c] : 0.f; s += yhat[i]; }
-    const float mean = warp_sum(s) / (float)C;
-    float q = 0.f;
-#pragma unroll
-    for (int i = 0; i < MAXV; ++i) { const int c = lane + 32 * i; const float d = c < C ? yhat[i] - mean : 0.f; yhat[i] = d; q = fmaf(d, d, q); }
-    rstd = 1.0f / sqrtf(warp_sum(q) / (float)C + 1e-12f);
-#pragma unroll
-    for (int i = 0; i < MAXV; ++i) yhat[i] *= rstd;
-}
-
-constexpr int BWD_WARPS = 8;
-constexpr int BWD_ROWS_PER_WARP = 4;
+// ln_fwd_half / ln_bwd_half, BWD_WARPS, BWD_ROWS_PER_WARP: kernels_train.cuh
 
 // grid: ceil(rows / 32) CTAs of 8 warps; dynamic shared memory: (4 C + nconv) floats of column accumulators.
 // HC = false compiles the conv1d branch only (mode 0): the hc branch holds six MAXV arrays, which spill at MAXV = 65,
@@ -196,16 +163,23 @@ __global__ void __launch_bounds__(BWD_WARPS * 32) train_block_bwd_kernel(const B
     for (int i = threadIdx.x; i < nconv; i += blockDim.x) atomicAdd(a.dbias + i, dbs[i]);
 }
 
-void launch_train_block_bwd(const BlockBwdArgs& a, cudaStream_t s) {
+template <int MAXV, bool HC = true>
+int block_bwd(const BlockBwdArgs& a, cudaStream_t s, const OrderedWs* ord) {
+    if (ord) return launch_train_block_bwd_ordered<MAXV, HC>(a, *ord, s);
     const int rows_per_cta = BWD_WARPS * BWD_ROWS_PER_WARP;
     const unsigned grid = (unsigned)((a.rows + rows_per_cta - 1) / rows_per_cta);
     const size_t smem = (size_t)(4 * a.C + (a.mode == 1 ? 2 * a.C : a.C)) * sizeof(float);
-    if (a.C <= 128)      train_block_bwd_kernel<4><<<grid, BWD_WARPS * 32, smem, s>>>(a);
-    else if (a.C <= 256) train_block_bwd_kernel<8><<<grid, BWD_WARPS * 32, smem, s>>>(a);
-    else if (a.C <= 512) train_block_bwd_kernel<16><<<grid, BWD_WARPS * 32, smem, s>>>(a);
-    else if (a.C <= 1024) train_block_bwd_kernel<32><<<grid, BWD_WARPS * 32, smem, s>>>(a);
-    else if (a.C <= 1056) train_block_bwd_kernel<33><<<grid, BWD_WARPS * 32, smem, s>>>(a);     // F = 1025
-    else if (a.C <= 2080 && a.mode == 0) train_block_bwd_kernel<65, false><<<grid, BWD_WARPS * 32, smem, s>>>(a);   // F = 2049
+    train_block_bwd_kernel<MAXV, HC><<<grid, BWD_WARPS * 32, smem, s>>>(a);
+    return 1;
+}
+
+int launch_train_block_bwd(const BlockBwdArgs& a, cudaStream_t s, const OrderedWs* ord) {
+    if (a.C <= 128)      return block_bwd<4>(a, s, ord);
+    else if (a.C <= 256) return block_bwd<8>(a, s, ord);
+    else if (a.C <= 512) return block_bwd<16>(a, s, ord);
+    else if (a.C <= 1024) return block_bwd<32>(a, s, ord);
+    else if (a.C <= 1056) return block_bwd<33>(a, s, ord);                       // F = 1025
+    else if (a.C <= 2080 && a.mode == 0) return block_bwd<65, false>(a, s, ord);  // F = 2049
     else if (a.C <= 2080) throw std::runtime_error("train_block_bwd: no hc kernel for " + std::to_string(a.C) + " channels (1056 at most)");
     else throw std::runtime_error("train_block_bwd: " + std::to_string(a.C) + " channels exceed the widest kernel (2080)");
 }
@@ -220,41 +194,9 @@ __global__ void __launch_bounds__(256) conv_wgrad_kernel(const WgradArgs a) {
     const int tap = blockIdx.z / a.nsplit, split = blockIdx.z - tap * a.nsplit;
     const int shift = tap == 0 ? a.shifts[0] : tap == 1 ? a.shifts[1] : a.shifts[2];   // a dynamic index would copy the params to the stack
     const long long r_begin = (long long)split * a.rows_per_split, r_end = min((long long)a.rows, r_begin + a.rows_per_split);
-    const int tx = tid & 15, ty = tid >> 4;               // 16 x 16 threads, 4 x 4 outputs each
-    const int lr = tid >> 4, lq = (tid & 15) * 4;         // loader: row lr (0..15), 4 consecutive columns at lq
+    const int tx = tid & 15, ty = tid >> 4;
     float acc[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-    for (long long r0 = r_begin; r0 < r_end; r0 += 16) {
-        const long long row = r0 + lr;
-        float4 xv = make_float4(0.f, 0.f, 0.f, 0.f), dv = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (row < r_end) {
-            const int b = (int)(row / a.L), t = (int)(row - (long long)b * a.L), ts = t + shift;
-            const int k = k0 + lq, n = n0 + lq;
-            if (ts >= 0 && ts < a.L && k < a.K) {
-                const float* p = a.X + ((size_t)b * a.L + ts) * a.ldx + k;
-                if (k + 3 < a.K) xv = __ldg(reinterpret_cast<const float4*>(p));
-                else { xv.x = p[0]; if (k + 1 < a.K) xv.y = p[1]; if (k + 2 < a.K) xv.z = p[2]; }
-            }
-            if (n < a.N) dv = __ldg(reinterpret_cast<const float4*>(a.dy + row * a.ldy + n));     // N, ldy multiples of 4
-        }
-        __syncthreads();
-        *reinterpret_cast<float4*>(&Xs[lr][lq]) = xv;
-        *reinterpret_cast<float4*>(&Ds[lr][lq]) = dv;
-        __syncthreads();
-#pragma unroll
-        for (int r = 0; r < 16; ++r) {
-            const float4 xa = *reinterpret_cast<const float4*>(&Xs[r][ty * 4]);
-            const float4 db = *reinterpret_cast<const float4*>(&Ds[r][tx * 4]);
-            const float av[4] = {xa.x, xa.y, xa.z, xa.w}, bv[4] = {db.x, db.y, db.z, db.w};
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-#pragma unroll
-                for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
-        }
-    }
+    wgrad_tile(a, n0, k0, shift, r_begin, r_end, Xs, Ds, acc);
     float* W = a.dW + (size_t)tap * a.K * a.ldw;
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
@@ -268,11 +210,13 @@ __global__ void __launch_bounds__(256) conv_wgrad_kernel(const WgradArgs a) {
     }
 }
 
-void launch_conv_wgrad(WgradArgs a, cudaStream_t s) {
-    a.nsplit = (int)std::max<long long>(1, std::min<long long>(64, a.rows / 512));
+int launch_conv_wgrad(WgradArgs a, cudaStream_t s, const OrderedWs* ord) {
+    a.nsplit = ord ? conv_wgrad_ordered_splits(a) : (int)std::max<long long>(1, std::min<long long>(64, a.rows / 512));
     a.rows_per_split = (int)(((a.rows + a.nsplit - 1) / a.nsplit + 15) / 16 * 16);
+    if (ord && a.nsplit > 1) return launch_conv_wgrad_ordered(a, *ord, s);        // one split adds each element once: no order to fix
     dim3 grid((a.N + 63) / 64, (a.K + 63) / 64, a.ntaps * a.nsplit);
     conv_wgrad_kernel<<<grid, 256, 0, s>>>(a);
+    return 1;
 }
 
 // W[tap][K][ldw] -> WT[tap][N][Kp]   (N rows = columns of W taken, Kp >= K the padded row length; pad columns untouched)
@@ -390,10 +334,12 @@ __global__ void attn_loss_kernel(const float* __restrict__ align, const float* _
     if (threadIdx.x == 0) { double s = 0.0; for (int k = 0; k < 8; ++k) s += red[k]; atomicAdd(&sums[2], s); }
 }
 
-void launch_attn_loss(const float* align, const float* gts, int ld_gts, double* sums, int B, int N, int T, int n_lim, int t_lim,
-                      cudaStream_t s) {
+int launch_attn_loss(const float* align, const float* gts, int ld_gts, double* sums, int B, int N, int T, int n_lim, int t_lim,
+                     cudaStream_t s, const OrderedWs* ord) {
+    if (ord) return launch_attn_loss_ordered(align, gts, ld_gts, sums, B, N, T, n_lim, t_lim, *ord, s);
     const long long n = (long long)B * N * T;
     attn_loss_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(align, gts, ld_gts, sums, B, N, T, n_lim, t_lim);
+    return 1;
 }
 
 void check_attn_bwd(const AttnBwdArgs& a) {
@@ -404,7 +350,7 @@ void check_attn_bwd(const AttnBwdArgs& a) {
                                  std::to_string(a.T) + ") or the table's row stride " + std::to_string(a.ld_gts));
 }
 
-void launch_attn_bwd(const AttnBwdArgs& a, double* sums, cudaStream_t s) {
+int launch_attn_bwd(const AttnBwdArgs& a, double* sums, cudaStream_t s, const OrderedWs* ord) {
     check_attn_bwd(a);
     const size_t smem = (size_t)4 * a.N * sizeof(float);
     if (smem > 48 * 1024) {
@@ -415,9 +361,10 @@ void launch_attn_bwd(const AttnBwdArgs& a, double* sums, cudaStream_t s) {
                                      " bytes of shared memory per block, more than the device allows");
         }
     }
-    launch_attn_loss(a.align, a.gts, a.ld_gts, sums, a.B, a.N, a.T, a.n_lim, a.t_lim, s);
+    const int launches = launch_attn_loss(a.align, a.gts, a.ld_gts, sums, a.B, a.N, a.T, a.n_lim, a.t_lim, s, ord);
     attn_bwd_q_kernel<<<(a.B * a.T + 3) / 4, 128, smem, s>>>(a);
     attn_bwd_kv_kernel<<<(a.B * a.N + 3) / 4, 128, 0, s>>>(a);
+    return launches + 2;
 }
 
 // utils.py:134-140
@@ -439,8 +386,10 @@ __global__ void embed_bwd_kernel(const int* __restrict__ ids, const float* __res
     if (id <= 0) return;
     for (int c = threadIdx.x; c < e; c += blockDim.x) atomicAdd(dtable + (size_t)id * e + c, g[(size_t)row * e + c]);
 }
-void launch_embed_bwd(const int* ids, const float* g, float* dtable, int rows, int e, cudaStream_t s) {
+int launch_embed_bwd(const int* ids, const float* g, float* dtable, int rows, int e, int vocab, cudaStream_t s, const OrderedWs* ord) {
+    if (ord) return launch_embed_bwd_ordered(ids, g, dtable, rows, e, vocab, s);
     embed_bwd_kernel<<<rows, 128, 0, s>>>(ids, g, dtable, rows, e);
+    return 1;
 }
 
 // ------------------------------------------------------------------------------------ optimiser

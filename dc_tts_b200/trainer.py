@@ -353,7 +353,7 @@ def write_samples(engine, texts, logdir, global_step, writer=None):
 
 def train(num, engine, batches, num_iterations=None, logdir=None, global_step=None, save_every=1000, log=print, resume=True,
           rank=0, world=1, allreduce=None, beyond_capacity="skip", capacity=None, summaries=False, summary_secs=120,
-          samples=None):
+          samples=None, deterministic=None):
     """train.py:137-160 for num = 1 (Text2Mel) or 2 (SSRN).  `batches` yields (L, mels, mags, names, ...): the bucketed
     batches of `bucketed_batches` at their own shapes or fixed-size ones; `engine` is an `Engine` with parameters loaded.
     The workspace is allocated for the capacity (hp.max_N, hp.max_T), or `capacity` = (N, T) when that is larger; a batch
@@ -376,9 +376,16 @@ def train(num, engine, batches, num_iterations=None, logdir=None, global_step=No
     `samples_{NNN}k/`, and with `summaries` an event with their audio).  The network not being trained is the one the
     engine holds: for num = 1, SSRN as loaded (e.g. restored from logdir-2; random SSRN weights still give the mels'
     lengths and a rough sound); for num = 2, Text2Mel as loaded.  It consumes no batch.
+    `deterministic=True` sets the engine's option "train_deterministic" (include/dctts.h): every sum of the step runs in a
+    fixed order, so a run with the same seed, data and hyper-parameters repeats bit for bit, and a run resumed from a
+    checkpoint writes the bundles of the run that never stopped.  Each rank's gradient arena is deterministic; the order of
+    the cross-rank all-reduce belongs to torch.distributed.  `deterministic=False` sets the option to 0 (the default
+    kernels); None (the default) leaves the engine's option as it is, which is 0 unless the caller set it.
     Returns the final global step."""
     if num not in (1, 2):
         raise ValueError("num: 1 for Text2Mel, 2 for SSRN (train.py:139)")
+    if deterministic is not None:
+        engine.set_option("train_deterministic", 1 if deterministic else 0)
     num_iterations = hp.num_iterations if num_iterations is None else num_iterations
     logdir = logdir or (hp.logdir + "-" + str(num))
     os.makedirs(logdir, exist_ok=True)

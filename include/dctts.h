@@ -255,7 +255,17 @@ int dctts_train_step(dctts_handle h, const int32_t* L, const float* mels, int32_
  * the batch size given to dctts_train_init.  A step outside the capacity fails with a message and launches nothing.
  * The losses are the reference's at this shape: means over B T n_mels; the guided-attention sum over the N x T corner of
  * the (max_N, max_T) weight table divided by B N T (train.py:91-95).  The softmax runs over the N keys and TextEnc's SAME
- * padding sees the edge of the tensor at N.  dctts_train_step is this call at (max_N, max_T). */
+ * padding sees the edge of the tensor at N.  dctts_train_step is this call at (max_N, max_T).
+ * Determinism: by default the weight, LayerNorm, bias and embedding gradients and the loss sums are added with float
+ * atomics, so two identical steps may differ in the last bits.  With the option "train_deterministic" = 1 every sum runs in
+ * a fixed order, and dctts_train_step(_shaped), dctts_train_step_ssrn(_shaped), dctts_train_apply and
+ * dctts_train_eval(_ssrn) write the same bits -- variables, Adam m and v, the gradient arena, losses_host, and the
+ * evaluations' Y, Z and alignments -- whenever they get the same variables, Adam moments, global step, batch (same shape),
+ * seed, lr, dropout rate, batch size and "train_tc" kernel set, whatever the workspace capacity (dctts_train_reserve),
+ * whatever ran on the handle before (evaluations, synthesis, dctts_refresh_synthesis, a step with apply = 0 followed by
+ * dctts_train_apply) and on whichever handle.  No split count of this mode is read from the device.  Not promised: equal
+ * bits between kernel sets, or with the default mode.  The mode's partial sums live in the training workspace (allocated
+ * at its first step, kept across dctts_train_reserve). */
 int dctts_train_step_shaped(dctts_handle h, const int32_t* L, int32_t N, const float* mels, int32_t T, int32_t B, int64_t global_step,
                             uint32_t seed, float lr, int32_t apply, float* losses_host, void* stream);
 int dctts_train_apply(dctts_handle h, int64_t global_step, float lr, void* stream);
@@ -333,6 +343,8 @@ int dctts_set_tensor_path(dctts_handle h, int32_t mode);
  *   "decode_force_prepass" 0/1: measurement / test switch of the persistent decode (default 0): every utterance takes the
  *                  receptive-field recompute at every frame j >= 1, as if its attention window had moved (the worst case)
  *   "train_tc" 0..7: training GEMMs on wgmma, bit mask 1 forward conv (+ wgmma attention), 2 data gradient, 4 weight gradient
+ *   "train_deterministic" 0/1 (default 0): the training step's sums in a fixed order, so that a seeded run repeats bit for
+ *                  bit (see dctts_train_step_shaped); it may change between steps and does not affect synthesis
  * dctts_get_option also answers "decode_available" (1 when this handle / device can run the persistent decode),
  * "decode_max_clusters" (16-CTA clusters of the decode kernel that are co-resident on this device) and, once the
  * parameters are committed, "ssrn_tc_available" (1 when every SSRN block has a wgmma kernel, the F-wide ones included:

@@ -4,7 +4,8 @@ data-parallel over the launched ranks (gradient all-reduce of the flat arena ove
 `--reserve N,T` the workspace is first grown to that capacity (Engine.train_reserve, timed once: "reserve_ms"), so `--shape`
 can go past (max_N, max_T).  `--eval` also times the forward-only evaluation of the training graph on the same batch
 (what summaries and alignment plots cost: "eval_ms").  The card's name and power limit are part of the JSON line.
-    python tools/bench_train.py [--steps 10 --warmup 3 --batch 32 --net 1 --shape 180,210 --reserve 256,256 --eval]
+`--deterministic` runs the step with the option "train_deterministic" (its sums in a fixed order).
+    python tools/bench_train.py [--steps 10 --warmup 3 --batch 32 --net 1 --shape 180,210 --reserve 256,256 --eval --deterministic]
     python -m torch.distributed.run --nproc-per-node N --master-addr 127.0.0.1 tools/bench_train.py"""
 import argparse
 import json
@@ -32,6 +33,7 @@ ap.add_argument("--shape", default="%d,%d" % (hp.max_N, hp.max_T), help="N,T of 
 ap.add_argument("--reserve", default=None, help="N,T: grow the training workspace to this capacity after init (SSRN uses T)")
 ap.add_argument("--eval", action="store_true", help="also time Engine.train_eval / train_eval_ssrn (forward only, no update) on the same batch: eval_ms")
 ap.add_argument("--train-tc", type=int, default=7, help="bit mask: 1 forward conv, 2 data gradient, 4 weight gradient on wgmma (default 7 = all), 0 = fp32 CUDA-core kernels")
+ap.add_argument("--deterministic", action="store_true", help="option train_deterministic: the step's sums in a fixed order (bit-reproducible)")
 a = ap.parse_args()
 N, T = (int(x) for x in a.shape.split(","))
 rank, world, local = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
@@ -43,6 +45,7 @@ eng.load_params(init_params(0))
 B = a.batch
 eng.set_option("train_tc", a.train_tc)
 eng.set_option("train_probe", a.probe)
+eng.set_option("train_deterministic", 1 if a.deterministic else 0)
 if a.net == 1:
     eng.train_init(B)
 else:
@@ -123,7 +126,7 @@ if rank == 0:
                                               "SSRN train step (train.py num=2: fwd + bwd + clip + Adam), B=%d per GPU, T=%d -> %d frames x 1025 bins, dropout %.2f"
                                               % (B, T, T * hp.r, hp.dropout_rate)),
                                  "parallelism": "dp%d (all-reduce of %d gradients)" % (world, grads.numel())},
-                      "dtype": ("f32 tensors; GEMMs as split-fp16 x3 on wgmma, fp32 accumulate" if a.train_tc else "f32 (CUDA-core kernels)"), "data": "synthetic",
+                      "dtype": ("f32 tensors; GEMMs as split-fp16 x3 on wgmma, fp32 accumulate" if a.train_tc else "f32 (CUDA-core kernels)"), "data": "synthetic", "deterministic": a.deterministic,
                       "achieved_tflops": world * flops / (ms * 1e-3) / 1e12, "gpu_launches_per_step": (eng.launch_count() - n0) // a.steps,
                       "loss_first": first["loss"], "loss_last": last["loss"],
                       "eval_ms": eval_ms, "eval_over_step": None if eval_ms is None else eval_ms / ms}))
