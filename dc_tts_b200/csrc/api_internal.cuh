@@ -129,6 +129,10 @@ struct dctts_handle_s {
     std::vector<DevBuf> ad_out;   // AudioDec per-layer outputs (B, T, d | n_mels)
     DevBuf ad_sig;                // scratch for sigmoid(logits) in full-graph mode
     DevBuf ibuf;                  // ints: j, p_cur[B], p_next[B], p_prev[B], p_hist[B*T]
+    DevBuf pathbuf;               // ints of a decode along a window path: lengths[B], path[B*T], argmax[B*T]
+    int* path_pinned = nullptr;   // pinned staging of pathbuf's lengths and path, reused once path_uploaded has fired
+    size_t path_pinned_n = 0;     // ints
+    cudaEvent_t path_uploaded = nullptr;
     DevBuf lbuf;                  // (B, N) ids staging for the host entry point
     DevBuf zbuf;                  // (B, 4T, F) staging for the host entry point
     DevBuf plane[4];              // tensor-core path activations: {hi,lo} x ping-pong, rows x 1032 fp16
@@ -177,6 +181,7 @@ struct dctts_handle_s {
     // AR decode graph
     cudaGraphExec_t ar_exec = nullptr;
     int ar_B = 0;
+    bool ar_path = false;         // the captured step advances along pathbuf instead of to its own argmax
     int64_t ar_nodes = 0;
 
     int tensor_path = 1;          // wgmma blocks wherever they apply; 0 forces the fp32 CUDA-core kernels
@@ -217,6 +222,8 @@ struct dctts_handle_s {
     ~dctts_handle_s() {
         if (ar_exec) cudaGraphExecDestroy(ar_exec);
         if (copy_stream) { cudaStreamDestroy(copy_stream); for (auto e : chunk_done) if (e) cudaEventDestroy(e); }
+        if (path_uploaded) { cudaEventSynchronize(path_uploaded); cudaEventDestroy(path_uploaded); }
+        if (path_pinned) cudaFreeHost(path_pinned);
         if (stream) cudaStreamDestroy(stream);
     }
 };

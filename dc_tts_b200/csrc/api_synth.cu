@@ -80,6 +80,7 @@ void ensure_ws(H* h, int B) {
     for (size_t i = 0; i < h->audiodec.size(); ++i)
         h->ad_out[i].ensure((size_t)B * T * h->audiodec[i].cout * sizeof(float));
     h->ibuf.ensure((size_t)(4 + 3 * B + (size_t)B * T) * sizeof(int));
+    h->pathbuf.ensure((size_t)(B + 2 * (size_t)B * T) * sizeof(int));
     h->lbuf.ensure((size_t)B * N * sizeof(int));
     for (auto& pb : h->plane) pb.ensure(rows_ssrn * (size_t)roundup(std::max(std::max(2 * hp.c, F), 2 * d), 8) * sizeof(__half));
     h->in_inv.ensure((size_t)B * sizeof(float));
@@ -445,7 +446,8 @@ void run_textenc(Launch& lc, const int* L, int B, float* kv_out /* (B,N,2d) */) 
 // One AR step (synthesize.py:48-54 restated incrementally, exact w.r.t. the reference's
 // full recompute): AudioEnc row j, attention over the AudioDec receptive field under the
 // CURRENT window, AudioDec pyramid, Y[j] = sigmoid(logits[j]), p <- argmax of row j, j <- j+1.
-void run_ar_step(Launch& lc, int B) {
+// `path`: p <- the workspace's window path at j+1 instead, the argmax of row j recorded (h->pathbuf).
+void run_ar_step(Launch& lc, int B, bool path) {
     H* h = lc.h;
     const dctts_hparams& hp = h->hp;
     const int T = hp.max_T, N = hp.max_N, d = hp.d;
@@ -491,12 +493,18 @@ void run_ar_step(Launch& lc, int B) {
         }
         cur = dst; ld = l.cout;
     }
-    launch_ar_advance(ib.p_cur, ib.p_next, ib.j, B, lc.s); lc.count();
+    if (path) {
+        int* pb = h->pathbuf.as<int>() + h->ws_B;
+        launch_ar_advance_path(ib.p_cur, ib.p_next, ib.j, pb, pb + (size_t)h->ws_B * T, B, T, lc.s);
+    } else {
+        launch_ar_advance(ib.p_cur, ib.p_next, ib.j, B, lc.s);
+    }
+    lc.count();
     // keep the window used by this step for the optional final alignment pass
 }
 
-void build_ar_graph(H* h, int B) {
-    if (h->ar_exec && h->ar_B == B) return;
+void build_ar_graph(H* h, int B, bool path = false) {
+    if (h->ar_exec && h->ar_B == B && h->ar_path == path) return;
     drop_ar_graph(h);
     CUDA_CHECK(cudaStreamSynchronize(h->stream));
     cudaGraph_t graph = nullptr;
@@ -504,7 +512,7 @@ void build_ar_graph(H* h, int B) {
     CUDA_CHECK(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
     try {
         Launch lc{h, h->stream};
-        run_ar_step(lc, B);
+        run_ar_step(lc, B, path);
     } catch (...) {
         cudaStreamEndCapture(h->stream, &graph);
         if (graph) cudaGraphDestroy(graph);
@@ -519,13 +527,21 @@ void build_ar_graph(H* h, int B) {
     CUDA_CHECK(e);
     CUDA_CHECK(cudaGetLastError());
     h->ar_B = B;
+    h->ar_path = path;
 }
 
 // End of utterance for dctts_text2mel_generate_until: device stop positions (B), tail frames, device lengths out (B)
 struct Until { const int* stop_pos; int tail; int* lengths; };
+// Decode along a window path (dctts_text2mel_generate_path), all in h->pathbuf: lengths (B), path (B, T) padded past
+// each length with its last window, the argmax of every frame (B, T)
+struct PathRun { const int* lengths; const int* path; int* amax; };
+PathRun path_run(H* h) {
+    int* pb = h->pathbuf.as<int>();
+    return PathRun{pb, pb + h->ws_B, pb + h->ws_B + (size_t)h->ws_B * h->hp.max_T};
+}
 
 // The whole AR loop as one persistent launch (kernels_decode.cu).  Returns false when this handle / device cannot run it.
-bool decode_cluster(H* h, int B, int steps, cudaStream_t s, const Until* u) {
+bool decode_cluster(H* h, int B, int steps, cudaStream_t s, const Until* u, const PathRun* pr = nullptr) {
     auto& D = h->dec;
     if (!D.ok || h->opt.decode_mode != 1) return false;
     const dctts_hparams& hp = h->hp;
@@ -546,6 +562,8 @@ bool decode_cluster(H* h, int B, int steps, cudaStream_t s, const Until* u) {
         // the stream bound is lowered at a frame's attention; the refill cursor must then still be inside that frame
         REQUIRE(P.nch - P.nch_enc >= DEC_NSLOT, "decode: fewer AudioDec weight chunks per frame than ring slots");
         P.stop_pos = u->stop_pos; P.lengths = u->lengths; P.frames = D.frames.as<int>(); P.tail = u->tail;
+    } else if (pr) {
+        P.lengths = const_cast<int*>(pr->lengths); P.frames = D.frames.as<int>();
     } else if (h->opt.decode_prof) { D.prof.ensure(DEC_NPROF * sizeof(long long)); CUDA_CHECK(cudaMemsetAsync(D.prof.p, 0, DEC_NPROF * sizeof(long long), s)); P.prof = D.prof.as<long long>(); }
     P.B = B;
     {   // utterances per cluster: the fewest that let every cluster be co-resident (a second wave doubles the time)
@@ -557,7 +575,7 @@ bool decode_cluster(H* h, int B, int steps, cudaStream_t s, const Until* u) {
     P.T = hp.max_T; P.N = hp.max_N; P.d = hp.d; P.n_mels = hp.n_mels;
     P.win_size = hp.attention_win_size; P.steps = steps;
     const int n_clusters = (B + P.G - 1) / P.G;
-    cudaError_t e = launch_decode_cluster(P, n_clusters, s);
+    cudaError_t e = pr ? launch_decode_path(P, pr->path, pr->amax, n_clusters, s) : launch_decode_cluster(P, n_clusters, s);
     if (e != cudaSuccess) {
         // a device on which the 16-CTA cluster cannot be placed after all: remember it and let the caller take the
         // graph-per-frame loop (another GPU path, not a CPU fallback)
@@ -567,29 +585,32 @@ bool decode_cluster(H* h, int B, int steps, cudaStream_t s, const Until* u) {
     }
     h->launches += 1;
     D.last_clusters = n_clusters; D.last_moved_frames = -1;
-    D.frames_pending = u != nullptr;
-    D.last_frames = u ? -1 : n_clusters * steps;
+    D.frames_pending = u != nullptr || pr != nullptr;
+    D.last_frames = D.frames_pending ? -1 : n_clusters * steps;
     return true;
 }
 
+// `pr`: the workspace's path (path_run) is already uploaded; the windows follow it
 void text2mel_generate(H* h, const int* L, int B, int steps, float* Y, int* prev_hist,
-                       long long* maxatt, float* align, cudaStream_t s, const Until* u = nullptr) {
+                       long long* maxatt, float* align, cudaStream_t s, const Until* u = nullptr, const PathRun* pr = nullptr) {
     const dctts_hparams& hp = h->hp;
     const int T = hp.max_T, N = hp.max_N, d = hp.d;
     if (steps <= 0 || steps > T) steps = T;
     ensure_ws(h, B);
     const bool cluster = h->dec.ok && h->opt.decode_mode == 1;
-    if (!cluster) build_ar_graph(h, B);
+    if (!cluster) build_ar_graph(h, B, pr != nullptr);
     IntBufs ib = ints(h);
     Launch lc{h, s};
     run_textenc(lc, L, B, h->kv.as<float>());
     CUDA_CHECK(cudaMemsetAsync(h->ybuf.p, 0, (size_t)B * T * hp.n_mels * sizeof(float), s));
     CUDA_CHECK(cudaMemsetAsync(h->ibuf.p, 0, (size_t)(4 + 3 * h->ws_B + (size_t)h->ws_B * T) * sizeof(int), s));
-    bool persistent = cluster && decode_cluster(h, B, steps, s, u);
+    if (pr) CUDA_CHECK(cudaMemcpy2DAsync(ib.p_cur, sizeof(int), pr->path, (size_t)T * sizeof(int), sizeof(int), B,
+                                         cudaMemcpyDeviceToDevice, s));   // the window of frame 0
+    bool persistent = cluster && decode_cluster(h, B, steps, s, u, pr);
     if (persistent) {
         // the whole loop ran as one launch
     } else {
-        if (cluster) { CUDA_CHECK(cudaStreamSynchronize(s)); build_ar_graph(h, B); }
+        if (cluster) { CUDA_CHECK(cudaStreamSynchronize(s)); build_ar_graph(h, B, pr != nullptr); }
         for (int j = 0; j < steps; ++j) {
             CUDA_CHECK(cudaGraphLaunch(h->ar_exec, s));
             h->launches += h->ar_nodes;
@@ -859,6 +880,84 @@ int dctts_text2mel_generate_until(dctts_handle h, const int32_t* L, int32_t B, i
         REQUIRE(tail >= 0, "dctts_text2mel_generate_until: tail must be >= 0");
         const Until u{stop_pos, std::min<int>(tail, h->hp.max_T), lengths};
         text2mel_generate(h, L, B, steps, Y, prev_hist, nullptr, nullptr, S(h, stream), &u);
+    });
+}
+
+namespace {
+
+// dctts_text2mel_generate_path with the path (B, steps) and the lengths (B) in host memory.  They are checked before
+// anything is launched, then staged in pinned memory and uploaded with one asynchronous copy; the only wait is for the
+// previous call's upload out of the same staging buffer, so the host keeps queueing while earlier decodes run.
+void generate_path(H* h, const int* L, int B, int steps, const int* p, const int* n, float* Y, int* prev_hist,
+                   int* argmax_hist, cudaStream_t s) {
+    const dctts_hparams& hp = h->hp;
+    const int T = hp.max_T, N = hp.max_N;
+    for (int b = 0; b < B; ++b) {
+        const int nb = n[b];
+        if (nb < 1 || nb > steps)
+            throw std::runtime_error("dctts_text2mel_generate_path: utterance " + std::to_string(b) + " has length " +
+                                     std::to_string(nb) + " outside [1, " + std::to_string(steps) + "]");
+        for (int j = 0; j < nb; ++j) {
+            const int w = p[(size_t)b * steps + j];
+            if (w < 0 || w >= N)
+                throw std::runtime_error("dctts_text2mel_generate_path: utterance " + std::to_string(b) + " has window " +
+                                         std::to_string(w) + " at frame " + std::to_string(j) + " outside [0, " +
+                                         std::to_string(N) + ")");
+        }
+    }
+    ensure_ws(h, B);
+    const PathRun pr = path_run(h);
+    const size_t n_up = (size_t)h->ws_B + (size_t)B * T;      // pathbuf's lengths, then the first B path rows
+    if (!h->path_uploaded) CUDA_CHECK(cudaEventCreateWithFlags(&h->path_uploaded, cudaEventDisableTiming));
+    CUDA_CHECK(cudaEventSynchronize(h->path_uploaded));          // the staging buffer is free again
+    if (h->path_pinned_n < n_up) {
+        if (h->path_pinned) { CUDA_CHECK(cudaFreeHost(h->path_pinned)); h->path_pinned = nullptr; h->path_pinned_n = 0; }
+        CUDA_CHECK(cudaMallocHost(&h->path_pinned, n_up * sizeof(int)));
+        h->path_pinned_n = n_up;
+    }
+    int* st = h->path_pinned;
+    std::copy(n, n + B, st);
+    for (int b = 0; b < B; ++b)
+        for (int j = 0; j < T; ++j)     // past the length: the last window, so no frame there moves it
+            st[h->ws_B + (size_t)b * T + j] = p[(size_t)b * steps + std::min(j, n[b] - 1)];
+    CUDA_CHECK(cudaMemcpyAsync(const_cast<int*>(pr.lengths), st, n_up * sizeof(int), cudaMemcpyHostToDevice, s));
+    CUDA_CHECK(cudaEventRecord(h->path_uploaded, s));
+    text2mel_generate(h, L, B, steps, Y, prev_hist, nullptr, nullptr, s, nullptr, &pr);
+    // rows at and past each length: 0 in Y, -1 in the histories
+    int* len = const_cast<int*>(pr.lengths);
+    launch_until_finish(nullptr, 0, steps, T, hp.n_mels, nullptr, false, len, Y, prev_hist, B, s);
+    if (argmax_hist) {
+        CUDA_CHECK(cudaMemcpyAsync(argmax_hist, pr.amax, (size_t)B * T * sizeof(int), cudaMemcpyDeviceToDevice, s));
+        launch_until_finish(nullptr, 0, steps, T, hp.n_mels, nullptr, false, len, nullptr, argmax_hist, B, s);
+    }
+}
+
+}  // namespace
+
+int dctts_text2mel_generate_path(dctts_handle h, const int32_t* L, int32_t B, int32_t steps, const int32_t* path,
+                                 const int32_t* lengths, float* Y, int32_t* prev_hist, int32_t* argmax_hist, void* stream) {
+    return guarded(h, [&] {
+        REQUIRE(h->committed, "parameters not committed");
+        REQUIRE(B >= 1 && L && path && lengths && Y, "dctts_text2mel_generate_path: bad arguments");
+        REQUIRE(steps >= 1 && steps <= h->hp.max_T, "dctts_text2mel_generate_path: steps must be in [1, max_T]");
+        cudaStream_t s = S(h, stream);
+        // the path and the lengths are checked on the host: read them back (this waits for the stream)
+        std::vector<int> n((size_t)B), p((size_t)B * steps);
+        CUDA_CHECK(cudaMemcpyAsync(n.data(), lengths, n.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
+        CUDA_CHECK(cudaMemcpyAsync(p.data(), path, p.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
+        CUDA_CHECK(cudaStreamSynchronize(s));
+        generate_path(h, L, B, steps, p.data(), n.data(), Y, prev_hist, argmax_hist, s);
+    });
+}
+
+int dctts_text2mel_generate_path_host(dctts_handle h, const int32_t* L, int32_t B, int32_t steps, const int32_t* path_host,
+                                      const int32_t* lengths_host, float* Y, int32_t* prev_hist, int32_t* argmax_hist,
+                                      void* stream) {
+    return guarded(h, [&] {
+        REQUIRE(h->committed, "parameters not committed");
+        REQUIRE(B >= 1 && L && path_host && lengths_host && Y, "dctts_text2mel_generate_path_host: bad arguments");
+        REQUIRE(steps >= 1 && steps <= h->hp.max_T, "dctts_text2mel_generate_path_host: steps must be in [1, max_T]");
+        generate_path(h, L, B, steps, path_host, lengths_host, Y, prev_hist, argmax_hist, S(h, stream));
     });
 }
 

@@ -319,6 +319,7 @@ void launch_attention(const AttnArgs& a, cudaStream_t s);
 void launch_embed(const int* ids, const float* table, float* out, int rows, int e, cudaStream_t s);
 // p_cur = p_next; j += 1  (end of an AR step)
 void launch_ar_advance(int* p_cur, const int* p_next, int* j, int B, cudaStream_t s);
+void launch_ar_advance_path(int* p_cur, const int* p_next, int* j, const int* path, int* amax_hist, int B, int T, cudaStream_t s);
 void launch_fill_i32(int* p, int v, int n, cudaStream_t s);
 
 }  // namespace dctts

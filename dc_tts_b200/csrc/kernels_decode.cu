@@ -931,8 +931,14 @@ __device__ __forceinline__ Stream prepass(const DecParams& P, Smem& S, Stream st
 // The kernel body.  STOP (decode_until_kernel): after frame j's attention every CTA applies the end-of-utterance rule to
 // S.p_next -- computed identically in every CTA -- so all 16 CTAs leave the frame loop after the same frame, with no
 // extra communication, and go through the ordinary epilogue.
-template <bool PROF, int GT, bool STOP>
-__device__ __forceinline__ void decode_body(const DecParams& Pc) {
+// PATH (decode_path_kernel, with STOP): the window of frame j + 1 is path[b][j + 1] instead of the argmax of row j, which
+// is only recorded in amax_hist[b][j] (both (B, T)).  The lengths are inputs (P.lengths): S.f_end, the longest of the
+// cluster's, is set before the first frame and never lowered (S.stop / S.ulen are not used); the host pads each path row
+// past its length with its last window, so those frames never trigger a recompute.
+template <bool PROF, int GT, bool STOP, bool PATH = false>
+__device__ __forceinline__ void decode_body(const DecParams& Pc, const int* __restrict__ path = nullptr,
+                                            int* __restrict__ amax_hist = nullptr) {
+    static_assert(!PATH || STOP, "a path decode is bounded by its lengths");
     extern __shared__ __align__(128) unsigned char smem_raw[];
     Smem& S = *reinterpret_cast<Smem*>(smem_raw);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -963,7 +969,17 @@ __device__ __forceinline__ void decode_body(const DecParams& Pc) {
     if (tid < 2) S.fmoved[tid] = 0;
     if (tid < DEC_NPROF) S.prof[tid] = 0;
     if (tid == 0) { S.n_moved_frames = 0; S.n_moved_utt = 0; }
-    if constexpr (STOP) {                                 // slots past the cluster's utterances count as ended at frame 0
+    if constexpr (PATH) {
+        if (tid < GMAX) {
+            const int p0 = tid < G ? path[(size_t)(b0 + tid) * P.T] : 0;
+            S.p_cur[tid] = p0; S.p_prev[tid] = p0;
+        }
+        if (tid == 0) {
+            int fe = 0;
+            for (int g = 0; g < G; ++g) fe = max(fe, P.lengths[b0 + g]);
+            S.f_end = fe;
+        }
+    } else if constexpr (STOP) {                          // slots past the cluster's utterances count as ended at frame 0
         if (tid < GMAX) { S.stop[tid] = tid < G ? P.stop_pos[b0 + tid] : -1; S.ulen[tid] = tid < G ? -1 : 0; }
         if (tid == 0) S.f_end = P.steps;
     }
@@ -1008,13 +1024,21 @@ __device__ __forceinline__ void decode_body(const DecParams& Pc) {
 #pragma unroll
             for (int i = 0; i < 8; ++i) qv[i] = S.xin[cb][g][lane * 8 + i];
             const int amax = attend_row(P, qv, b0 + g, S.p_cur[g], lane, ctx);
-            if (lane == 0) S.p_next[g] = amax;
+            if constexpr (PATH) {
+                if (lane == 0) {
+                    const size_t row = (size_t)(b0 + g) * P.T;
+                    if (rank == 0) amax_hist[row + j] = amax;
+                    S.p_next[g] = j + 1 < P.steps ? path[row + j + 1] : S.p_cur[g];
+                }
+            } else {
+                if (lane == 0) S.p_next[g] = amax;
+            }
 #pragma unroll
             for (int i = 0; i < 8; ++i) { S.xin[cb ^ 1][g][lane * 8 + i] = ctx[i]; S.xin[cb ^ 1][g][P.d + lane * 8 + i] = qv[i]; }
         }
         cb ^= 1;
         LAP(LP_ATT);
-        if constexpr (STOP) {
+        if constexpr (STOP && !PATH) {
             // argmax of row j = S.p_next.  Utterance g ends at min(steps, j + 1 + tail) once it reaches its stop position;
             // when every utterance has a length the cluster executes the longest.  S.f_end >= j + 1 here, and the refill
             // cursor is still inside frame j (the AudioDec chunks of a frame outnumber the ring slots: checked by the host),
@@ -1046,7 +1070,7 @@ __device__ __forceinline__ void decode_body(const DecParams& Pc) {
         }
     }
     if constexpr (STOP) {
-        if (rank == 0 && tid < G) P.lengths[b0 + tid] = S.ulen[tid] < 0 ? P.steps : S.ulen[tid];
+        if constexpr (!PATH) if (rank == 0 && tid < G) P.lengths[b0 + tid] = S.ulen[tid] < 0 ? P.steps : S.ulen[tid];
         if (rank == 0 && tid == 0) P.frames[cluster] = frames;
     }
     if (rank == 0 && tid < G) P.p_final[b0 + tid] = S.p_cur[tid];
@@ -1066,9 +1090,26 @@ template <int GT>
 __global__ void __cluster_dims__(DEC_NC, 1, 1) __launch_bounds__(DEC_THREADS, 1)
 decode_until_kernel(const __grid_constant__ DecParams Pc) { decode_body<false, GT, true>(Pc); }
 
+// the same loop along a caller's window path: path and amax_hist are (B, T), P.lengths (B) are the frames to produce
+template <int GT>
+__global__ void __cluster_dims__(DEC_NC, 1, 1) __launch_bounds__(DEC_THREADS, 1)
+decode_path_kernel(const __grid_constant__ DecParams Pc, const int* __restrict__ path, int* __restrict__ amax_hist) {
+    decode_body<false, GT, true, true>(Pc, path, amax_hist);
+}
+
 size_t decode_smem_bytes() { return sizeof(Smem) + 128; }
 
 using DecKernel = void (*)(DecParams);
+using DecPathKernel = void (*)(DecParams, const int*, int*);
+static DecPathKernel decode_path_kernel_of(int G) {
+    switch (G) {
+        case 1: return decode_path_kernel<1>;
+        case 2: return decode_path_kernel<2>;
+        case 3: return decode_path_kernel<3>;
+        case 4: return decode_path_kernel<4>;
+        default: return decode_path_kernel<5>;
+    }
+}
 // one instantiation per (lap timers, utterances per cluster) and per utterance count with a stop; exactly one runs in a launch
 static DecKernel decode_kernel_of(bool prof, int G, bool stop = false) {
     if (stop) switch (G) {
@@ -1095,8 +1136,10 @@ static cudaError_t decode_prepare() {
     if (e != cudaSuccess) return e;
     if (dev >= 0 && dev < 64 && done[dev].load(std::memory_order_acquire)) return cudaSuccess;
     for (int G = 1; G <= DEC_GMAX; ++G)
-        for (int v = 0; v < 3; ++v) {                     // decode_cluster_kernel without / with lap timers, decode_until_kernel
-            DecKernel k = decode_kernel_of(v == 1, G, v == 2);
+        for (int v = 0; v < 4; ++v) {                     // decode_cluster_kernel without / with lap timers, decode_until_kernel,
+                                                          // decode_path_kernel
+            const void* k = v < 3 ? reinterpret_cast<const void*>(decode_kernel_of(v == 1, G, v == 2))
+                                  : reinterpret_cast<const void*>(decode_path_kernel_of(G));
             e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)decode_smem_bytes());
             if (e != cudaSuccess) return e;
             e = cudaFuncSetAttribute(k, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
@@ -1126,6 +1169,16 @@ cudaError_t launch_decode_cluster(const DecParams& p, int n_clusters, cudaStream
     cfg.gridDim = dim3(n_clusters * DEC_NC); cfg.blockDim = dim3(DEC_THREADS); cfg.dynamicSmemBytes = decode_smem_bytes(); cfg.stream = s;
     cfg.attrs = nullptr; cfg.numAttrs = 0;               // cluster dims are compiled in (__cluster_dims__)
     return cudaLaunchKernelEx(&cfg, decode_kernel_of(p.prof != nullptr, p.G, p.stop_pos != nullptr), p);
+}
+
+cudaError_t launch_decode_path(const DecParams& p, const int* path, int* amax_hist, int n_clusters, cudaStream_t s) {
+    cudaError_t e = decode_prepare();
+    if (e != cudaSuccess) return e;
+    if (p.G < 1 || p.G > DEC_GMAX || !p.lengths || !p.frames || !path || !amax_hist) return cudaErrorInvalidValue;
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(n_clusters * DEC_NC); cfg.blockDim = dim3(DEC_THREADS); cfg.dynamicSmemBytes = decode_smem_bytes(); cfg.stream = s;
+    cfg.attrs = nullptr; cfg.numAttrs = 0;
+    return cudaLaunchKernelEx(&cfg, decode_path_kernel_of(p.G), p, path, amax_hist);
 }
 
 __global__ void until_finish_kernel(const int* __restrict__ stop_pos, int tail, int steps, int T, int n_mels,

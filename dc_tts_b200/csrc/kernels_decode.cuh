@@ -77,6 +77,10 @@ size_t decode_smem_bytes();
 // returns cudaSuccess or the launch / attribute error (the caller decides whether to fall back).
 // p.stop_pos != nullptr runs decode_until_kernel (end of utterance, no lap timers).
 cudaError_t launch_decode_cluster(const DecParams& p, int n_clusters, cudaStream_t s);
+// decode_path_kernel: frame j of utterance b runs under the window path[b * T + j] (frame 0 included) instead of the
+// previous frame's argmax, which goes to amax_hist[b * T + j].  p.lengths (B) are inputs, 1 <= lengths[b] <= p.steps, and
+// a cluster executes the longest of its utterances (p.frames as decode_until_kernel; p.stop_pos is not read).
+cudaError_t launch_decode_path(const DecParams& p, const int* path, int* amax_hist, int n_clusters, cudaStream_t s);
 // Rows past each utterance's length: Y (B, T, n_mels) rows 0, prev_hist (B, T) rows -1 (either may be nullptr).  With
 // `derive`, lengths[b] is first computed from the window history p_hist (B, T) of a run of `steps` frames by the rule
 // decode_until_kernel applies in its frame loop.

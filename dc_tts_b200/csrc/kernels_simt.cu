@@ -757,6 +757,23 @@ void launch_ar_advance(int* p_cur, const int* p_next, int* j, int B, cudaStream_
     launch_kernel(ar_advance_kernel, dim3((B + 127) / 128), dim3(128), 0, s, p_cur, p_next, j, B);
 }
 
+// The step's argmax (p_next) goes to amax_hist[b][j]; the next window is path[b][j + 1] (both (B, T)).  One block: every
+// thread reads *j before thread 0 advances it.
+__global__ void ar_advance_path_kernel(int* p_cur, const int* p_next, int* j, const int* path, int* amax_hist, int B, int T) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const int jj = *j;
+    for (int i = threadIdx.x; i < B; i += blockDim.x) {
+        amax_hist[(size_t)i * T + jj] = p_next[i];
+        if (jj + 1 < T) p_cur[i] = path[(size_t)i * T + jj + 1];
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) *j = jj + 1;
+}
+void launch_ar_advance_path(int* p_cur, const int* p_next, int* j, const int* path, int* amax_hist, int B, int T, cudaStream_t s) {
+    launch_kernel(ar_advance_path_kernel, dim3(1), dim3(256), 0, s, p_cur, p_next, j, path, amax_hist, B, T);
+}
+
 __global__ void fill_i32_kernel(int* p, int v, int n) {
     int i = threadIdx.x + blockIdx.x * blockDim.x;
     if (i < n) p[i] = v;

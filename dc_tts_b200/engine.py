@@ -411,6 +411,55 @@ class Engine:
         Yc[perm], Pc[perm], nc[perm] = Y, P, n
         return Yc, Pc, nc
 
+    def text2mel_generate_path(self, L, path, lengths=None, steps=0):
+        """The decode along a caller's attention windows (include/dctts.h: dctts_text2mel_generate_path): frame j of
+        utterance b runs under the window path[b, j] instead of the previous frame's argmax.  `path`: (B, S) integers,
+        S <= max_T; `lengths`: (B,) frames per utterance in [1, steps], default all `steps`; `steps` defaults to S.
+        Returns (Y, prev_hist, argmax_hist) as CUDA tensors in the caller's order: prev_hist is the path, argmax_hist the
+        model's own argmax of every frame; rows >= lengths[b] are 0 in Y and -1 in both histories.  The utterances are
+        decoded in the order of their lengths, so that those sharing a decode cluster end at similar frames."""
+        # Every host-side step comes before L is copied to the device: that copy waits for earlier work on the stream,
+        # and host work after it would leave the GPU idle.
+        B = len(L)
+        ph = np.asarray(path.cpu() if isinstance(path, torch.Tensor) else path, np.int64)
+        if ph.ndim != 2 or ph.shape[0] != B:
+            raise DcttsError("text2mel_generate_path: path must be (B, steps) for %d utterances, got %s" % (B, ph.shape))
+        steps = int(steps) or ph.shape[1]
+        if not 1 <= steps <= min(ph.shape[1], self.hp.max_T):
+            raise DcttsError("text2mel_generate_path: steps %d outside [1, %d]" % (steps, min(ph.shape[1], self.hp.max_T)))
+        n = np.full(B, steps, np.int64) if lengths is None else \
+            np.asarray(lengths.cpu() if isinstance(lengths, torch.Tensor) else lengths, np.int64).reshape(-1)
+        if n.shape[0] != B:
+            raise DcttsError("text2mel_generate_path: %d lengths for %d utterances" % (n.shape[0], B))
+        bad = np.flatnonzero((n < 1) | (n > steps))
+        if bad.size:
+            raise DcttsError("text2mel_generate_path: utterance %d has length %d outside [1, %d]" % (bad[0], n[bad[0]], steps))
+        ph = ph[:, :steps]
+        out = np.argwhere((np.arange(steps) < n[:, None]) & ((ph < 0) | (ph >= self.hp.max_N)))
+        if out.size:
+            b, j = out[0]
+            raise DcttsError("text2mel_generate_path: utterance %d has window %d at frame %d outside [0, %d)"
+                             % (b, ph[b, j], j, self.hp.max_N))
+        order = np.argsort(n, kind="stable")
+        ps = np.ascontiguousarray(ph[order], np.int32)
+        ns = np.ascontiguousarray(n[order], np.int32)
+        L = self._i32(L)
+        perm = None if np.array_equal(order, np.arange(B)) else torch.as_tensor(order, device=self.device)
+        Ls = L if perm is None else L.index_select(0, perm).contiguous()
+        # host arrays: the entry point stages them itself, without waiting for earlier work on the stream
+        Y = self._empty(B, self.hp.max_T, self.hp.n_mels)
+        P = self._empty(B, self.hp.max_T, dtype=torch.int32)
+        M = self._empty(B, self.hp.max_T, dtype=torch.int32)
+        self._check(self._lib.dctts_text2mel_generate_path_host(self._h, _ptr(Ls), B, steps, C.c_void_p(ps.ctypes.data),
+                                                                C.c_void_p(ns.ctypes.data), _ptr(Y), _ptr(P), _ptr(M),
+                                                                self._stream()),
+                    "dctts_text2mel_generate_path_host")
+        if perm is None:
+            return Y, P, M
+        Yc, Pc, Mc = torch.empty_like(Y), torch.empty_like(P), torch.empty_like(M)
+        Yc[perm], Pc[perm], Mc[perm] = Y, P, M
+        return Yc, Pc, Mc
+
     def _set_vocoder_params(self, hop=None, win=None, power=None):
         """The hyperparameters' vocoder constants on the handle, with `hop`, `win` and `power` instead when given."""
         h = self.hp

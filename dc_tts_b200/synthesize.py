@@ -21,7 +21,7 @@ from .train import Graph, Session
 
 
 def synthesize(params=None, sentences=None, fast=True, write=True, seed=0, vocoder=True, allow_random_init=False,
-               until_eos=False, tail=0, momentum=0.0):
+               until_eos=False, tail=0, momentum=0.0, duration_scale=1.0):
     """`params`: a name -> array dict to use instead of the checkpoints.  Without it the latest checkpoints of
     hp.logdir-1 (Text2Mel) and hp.logdir-2 (SSRN) are restored, and a missing one RAISES like the reference's
     `saver.restore(sess, None)` does (synthesize.py:33,39) -- seeded random weights are used only when the caller asks
@@ -33,7 +33,12 @@ def synthesize(params=None, sentences=None, fast=True, write=True, seed=0, vocod
     length are 0.
 
     `momentum`: the vocoder's fast Griffin-Lim update (librosa's griffinlim(momentum=...)); 0 is the reference's plain
-    Griffin-Lim."""
+    Griffin-Lim.
+
+    `duration_scale`: speaking rate, > 1 slower.  At any value other than 1.0 each utterance is first decoded to its EOS
+    as with `until_eos=True`, its attention-window history is stretched by that factor (utils.stretch_path), and the
+    utterance is decoded again along the stretched path (Graph.generate_along); SSRN and the vocoder then run with the
+    stretched lengths.  1.0 leaves every other route exactly as it is."""
     # Load data
     L = load_data("synthesize", sentences)
 
@@ -63,9 +68,13 @@ def synthesize(params=None, sentences=None, fast=True, write=True, seed=0, vocod
                                         "or allow_random_init=True for seeded random weights" % " and ".join(missing))
 
         lengths = None
-        if until_eos:
-            Y, _, n = g.generate_until_eos(L, tail=tail)
-            lengths = n.cpu().numpy()
+        if until_eos or duration_scale != 1.0:
+            Y, P, n = g.generate_until_eos(L, tail=tail)
+            if duration_scale != 1.0:
+                from .utils import stretch_path
+                path, n = stretch_path(P, n, duration_scale)
+                Y, _, _ = g.generate_along(L, path, n)
+            lengths = n.cpu().numpy() if hasattr(n, "cpu") else np.asarray(n)
             Tmax = int(lengths.max())
             # SSRN at the batch's longest length; rows past each utterance's length come back as 0
             _, Zd = g.engine.ssrn(Y[:, :Tmax], want_logits=False, lengths=n)

@@ -193,6 +193,12 @@ class Graph:
         returns (Y, prev_max_attentions history, lengths), rows past an utterance's length 0 / -1 (Engine.text2mel_generate_until)."""
         return self.engine.text2mel_generate_until(L, tail=tail)
 
+    def generate_along(self, L, path, lengths=None):
+        """generate() with the reference's prev_max_attentions fed from `path` (B, S) at every frame instead of the
+        previous frame's argmax: returns (Y, path history, the model's own argmax history), rows past each length 0 / -1
+        (Engine.text2mel_generate_path)."""
+        return self.engine.text2mel_generate_path(L, path, lengths)
+
 
 class Session:
     """Minimal stand-in for tf.Session used as `with Session() as sess: sess.run(...)`."""

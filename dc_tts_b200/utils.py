@@ -21,6 +21,37 @@ from .engine import get_engine
 from .hyperparams import Hyperparams as hp
 
 
+def stretch_path(path, lengths, factor, steps=None):
+    """Speaking rate: the attention-window path of each utterance slowed down (factor > 1) or sped up (factor < 1).
+    path (B, S) integers, lengths (B,) frames per utterance (numpy, or tensors that are copied to the host).  Utterance
+    b gets n'_b = max(1, round(factor * n_b)) frames (Python's round: halves go to the even integer), with
+    P'[j] = P[min(n_b - 1, floor(j / factor))].  Returns (path' (B, max n') int32 padded with each row's last window,
+    n' (B,) int32).  A stretched length above `steps` (default hp.max_T) is refused."""
+    P = np.asarray(path.cpu() if hasattr(path, "cpu") else path)
+    n = np.asarray(lengths.cpu() if hasattr(lengths, "cpu") else lengths).reshape(-1).astype(np.int64)
+    factor = float(factor)
+    if not factor > 0:
+        raise ValueError("stretch_path: factor must be > 0, got %r" % factor)
+    if P.ndim != 2 or P.shape[0] != n.shape[0]:
+        raise ValueError("stretch_path: path must be (B, S) for %d lengths, got %s" % (n.shape[0], P.shape))
+    steps = hp.max_T if steps is None else int(steps)
+    bad = np.flatnonzero((n < 1) | (n > P.shape[1]))
+    if bad.size:
+        raise ValueError("stretch_path: utterance %d has length %d outside [1, %d]" % (bad[0], n[bad[0]], P.shape[1]))
+    m = np.array([max(1, int(round(factor * int(nb)))) for nb in n], np.int64)
+    over = np.flatnonzero(m > steps)
+    if over.size:
+        b = over[0]
+        raise ValueError("stretch_path: utterance %d stretched from %d to %d frames, more than %d"
+                         % (b, n[b], m[b], steps))
+    out = np.empty((n.shape[0], int(m.max())), np.int32)
+    for b in range(n.shape[0]):
+        src = np.minimum(n[b] - 1, np.floor(np.arange(m[b]) / factor).astype(np.int64))
+        out[b, :m[b]] = P[b, src]
+        out[b, m[b]:] = out[b, m[b] - 1]
+    return out, m.astype(np.int32)
+
+
 def spectrogram2wav(mag, momentum=0.0):
     """utils.py:67-94.  mag: (T, 1+n_fft//2) normalised magnitudes -> trimmed float32 wav (numpy).  `momentum`: the
     fast Griffin-Lim update (librosa's griffinlim(momentum=...)); 0 is the reference's plain Griffin-Lim."""

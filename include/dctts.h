@@ -138,6 +138,24 @@ int dctts_text2mel_generate(dctts_handle h, const int32_t* L, int32_t B, int32_t
 int dctts_text2mel_generate_until(dctts_handle h, const int32_t* L, int32_t B, int32_t steps,
                                   const int32_t* stop_pos, int32_t tail, float* Y, int32_t* prev_hist,
                                   int32_t* lengths, void* stream);
+/* The autoregressive loop along a caller's attention windows: frame j of utterance b runs under the window path[b, j]
+ * where synthesize.py:48 feeds prev_max_attentions = path[:, j] (path[b, 0] plays the role of the initial zeros) instead
+ * of the previous frame's argmax.  path (B, steps) and lengths (B) int32 are device pointers; 1 <= steps <= max_T,
+ * 1 <= lengths[b] <= steps, and 0 <= path[b, j] < max_N for j < lengths[b] -- anything else is refused before any launch
+ * with a message that names the utterance (both arrays are read on the host).  Y rows < lengths[b] are what the
+ * step-wise loop fed those windows computes; prev_hist (B,max_T) receives the path; optional argmax_hist (B,max_T) the
+ * model's own argmax of each frame inside its forced window (where it would have moved).  Rows >= lengths[b] are 0 in Y
+ * and -1 in prev_hist and argmax_hist.  A persistent decode cluster executes its longest length
+ * ("decode_last_frames"); the graph-per-frame loop (decode_mode 0) runs `steps` frames. */
+int dctts_text2mel_generate_path(dctts_handle h, const int32_t* L, int32_t B, int32_t steps, const int32_t* path,
+                                 const int32_t* lengths, float* Y, int32_t* prev_hist, int32_t* argmax_hist,
+                                 void* stream);
+/* The same with path (B, steps) and lengths (B) in HOST memory.  Reading device arrays back makes
+ * dctts_text2mel_generate_path wait for the stream; this form does not, so a caller that holds the path on the host can
+ * queue one decode while the previous one runs.  The arrays may be reused as soon as the call returns. */
+int dctts_text2mel_generate_path_host(dctts_handle h, const int32_t* L, int32_t B, int32_t steps,
+                                      const int32_t* path_host, const int32_t* lengths_host, float* Y,
+                                      int32_t* prev_hist, int32_t* argmax_hist, void* stream);
 /* synthesize.py:45-57 end to end with HOST buffers: copies L_host in, runs
  * dctts_text2mel_generate + dctts_ssrn, copies Y_host (B,max_T,n_mels; may be NULL) and
  * Z_host (B,4*max_T,F) out, and synchronises.  Host buffers should be pinned for speed. */
