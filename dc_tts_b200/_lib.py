@@ -88,6 +88,7 @@ SIGNATURES = {
     "dctts_get_option": (C.c_int, [Handle, C.c_char_p, C.POINTER(_i32)]),
     "dctts_decode_stats": (C.c_int, [Handle, C.POINTER(_i32), C.POINTER(_i32), C.POINTER(_i32)]),
     "dctts_decode_profile": (C.c_int, [Handle, C.POINTER(_i64), _i32]),
+    "dctts_decode_history": (C.c_int, [Handle, _i32, _i32, _p, _i64, C.POINTER(_i32), _p]),
     "dctts_malloc": (C.c_int, [Handle, C.POINTER(_p), _i64]),
     "dctts_free": (C.c_int, [Handle, _p]),
     "dctts_memcpy_h2d": (C.c_int, [Handle, _p, _p, _i64, _p]),

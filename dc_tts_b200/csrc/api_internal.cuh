@@ -218,6 +218,14 @@ struct dctts_handle_s {
 
     } dec;
 
+    // What dctts_decode_history may read: set by a generation without the final attention pass, cleared by every other
+    // writer of kv, rbuf, ae_out, ad_out, ybuf or the AR planes (and by a workspace growth, which reallocates them)
+    struct {
+        bool ok = false;
+        int B = 0;                // utterances of that generation
+        unsigned planes_only = 0; // bit i: AudioDec block i wrote only its split planes (arpl[i + 1]), not ad_out[i]
+    } hist;
+
     // the device buffers free themselves after this body: the graph that points into them goes first
     ~dctts_handle_s() {
         if (ar_exec) cudaGraphExecDestroy(ar_exec);

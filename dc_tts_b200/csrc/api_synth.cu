@@ -4,6 +4,7 @@
 //   graph wiring / shift .... train.py:48-68, :74-77
 //   autoregressive loop ..... synthesize.py:45-57
 #include "api_internal.cuh"
+#include "numerics.cuh"
 
 namespace {
 
@@ -64,6 +65,7 @@ void ensure_ws(H* h, int B) {
     drop_ar_graph(h);
     CUDA_CHECK(cudaDeviceSynchronize());
     settle_decode_counts(h);                              // the counter buffers below may move
+    h->hist.ok = false;                                   // and so do the buffers dctts_decode_history reads
     const size_t ld_scr = (size_t)roundup(std::max(std::max(4 * hp.c, F), 4 * d), 4);
     h->scratch.ensure(std::max(rows_ssrn * ld_scr * sizeof(float), (size_t)64 << 20));
     const size_t ld_act = (size_t)roundup(std::max(std::max(2 * hp.c, F), 2 * d), 4);
@@ -443,6 +445,12 @@ void run_textenc(Launch& lc, const int* L, int B, float* kv_out /* (B,N,2d) */) 
     run_chain_full(lc, h->textenc, emb, h->hp.e, B, N, kv_out, nullptr);
 }
 
+// Whether AudioDec block i of the graph-per-frame step runs on the tensor cores: at large batches the wide part of the
+// pyramid (rows[i] >= 32 of the first four blocks), one 128-row tile per utterance ending at row j.
+bool ar_block_on_tc(H* h, int B, size_t i, const std::vector<int>& rows) {
+    return h->tensor_path == 1 && B >= 8 && i < 4 && rows[i] >= 32 && h->audiodec[i].tc.ok;
+}
+
 // One AR step (synthesize.py:48-54 restated incrementally, exact w.r.t. the reference's
 // full recompute): AudioEnc row j, attention over the AudioDec receptive field under the
 // CURRENT window, AudioDec pyramid, Y[j] = sigmoid(logits[j]), p <- argmax of row j, j <- j+1.
@@ -468,7 +476,7 @@ void run_ar_step(Launch& lc, int B, bool path) {
     // Large batches run the wide part of the AudioDec pyramid (85..59 rows per utterance) on the
     // tensor cores, one 128-row tile per utterance ending at row j; the narrow tail and the
     // one-row AudioEnc stay on the latency-oriented fp32 kernels.
-    auto on_tc = [&](size_t i) { return h->tensor_path == 1 && B >= 8 && i < 4 && rows[i] >= 32 && h->audiodec[i].tc.ok; };
+    auto on_tc = [&](size_t i) { return ar_block_on_tc(h, B, i, rows); };
     auto ar_planes = [&](int idx, int C) {
         Planes p; p.hi = h->arpl[2 * idx].as<__half>(); p.lo = h->arpl[2 * idx + 1].as<__half>(); p.ld = C; return p;
     };
@@ -597,6 +605,7 @@ void text2mel_generate(H* h, const int* L, int B, int steps, float* Y, int* prev
     const int T = hp.max_T, N = hp.max_N, d = hp.d;
     if (steps <= 0 || steps > T) steps = T;
     ensure_ws(h, B);
+    h->hist.ok = false;
     const bool cluster = h->dec.ok && h->opt.decode_mode == 1;
     if (!cluster) build_ar_graph(h, B, pr != nullptr);
     IntBufs ib = ints(h);
@@ -636,6 +645,13 @@ void text2mel_generate(H* h, const int* L, int B, int steps, float* Y, int* prev
         const float* K = h->kv.as<float>();
         run_attention(lc, h->ae_out.back().as<float>(), d, K, 2 * d, K + d, 2 * d, RowWin{B, T, T, nullptr}, N,
                       ib.p_prev, h->rbuf.as<float>(), align, maxatt, nullptr, nullptr);
+        return;                                            // rbuf now holds the final pass, not the decode's rows
+    }
+    h->hist.ok = true; h->hist.B = B; h->hist.planes_only = 0;
+    if (!persistent) {
+        const std::vector<int> rows = audiodec_rows(h->audiodec, T);
+        for (size_t i = 0; i + 1 < h->audiodec.size(); ++i)
+            if (ar_block_on_tc(h, B, i, rows) && ar_block_on_tc(h, B, i + 1, rows)) h->hist.planes_only |= 1u << i;
     }
 }
 
@@ -644,6 +660,7 @@ void text2mel_forward(H* h, const int* L, const float* mels, const int* pma, int
     const dctts_hparams& hp = h->hp;
     const int T = hp.max_T, N = hp.max_N, d = hp.d;
     ensure_ws(h, B);
+    h->hist.ok = false;
     Launch lc{h, s};
     run_textenc(lc, L, B, h->kv.as<float>());
     const float* K = h->kv.as<float>();
@@ -784,6 +801,7 @@ int dctts_textenc(dctts_handle h, const int32_t* L, int32_t B, float* K, float* 
         REQUIRE(h->committed, "parameters not committed");
         REQUIRE(B >= 1 && L && K && V, "dctts_textenc: bad arguments");
         ensure_ws(h, B);
+        h->hist.ok = false;
         cudaStream_t s = S(h, stream);
         Launch lc{h, s};
         run_textenc(lc, L, B, h->kv.as<float>());
@@ -1077,6 +1095,45 @@ int dctts_decode_stats(dctts_handle h, int32_t* moved_frames, int32_t* moved_utt
         if (moved_frames) *moved_frames = D.last_moved_frames;
         if (moved_utterance_frames) *moved_utterance_frames = D.last_moved_utt;
         if (clusters) *clusters = D.last_clusters;
+    });
+}
+
+int dctts_decode_history(dctts_handle h, int32_t what, int32_t layer, void* out, int64_t n, int32_t* joined, void* stream) {
+    return guarded(h, [&] {
+        REQUIRE(h->hist.ok, "dctts_decode_history: the decode buffers do not hold a generation's state (the last writer was not a "
+                            "generation without the final attention pass)");
+        const dctts_hparams& hp = h->hp;
+        const size_t B = (size_t)h->hist.B, T = hp.max_T, N = hp.max_N, d = hp.d;
+        const void* src = nullptr;
+        size_t elems = 0;
+        int plane = -1;                                   // arpl pair holding the rows instead of an fp32 buffer
+        if (what == 0 || what == 1) {
+            const auto& net = what == 0 ? h->audioenc : h->audiodec;
+            REQUIRE(layer >= 0 && layer < (int)net.size(), "dctts_decode_history: block " + std::to_string(layer) + " outside [0, " +
+                                                           std::to_string(net.size()) + ")");
+            const auto& buf = what == 0 ? h->ae_out : h->ad_out;
+            src = buf[layer].p; elems = B * T * net[layer].cout;
+            if (what == 1 && ((h->hist.planes_only >> layer) & 1u)) plane = layer + 1;
+        } else if (what == 2) { src = h->rbuf.p; elems = B * T * 2 * d; }
+        else if (what == 3) { src = h->kv.p; elems = B * N * 2 * d; }
+        else if (what == 4) { src = h->ybuf.p; elems = B * T * hp.n_mels; }
+        else if (what == 5) { src = ints(h).p_hist; elems = B * T; }
+        else REQUIRE(false, "dctts_decode_history: `what` must be 0..5");
+        REQUIRE(out && n == (int64_t)elems, "dctts_decode_history: out must hold " + std::to_string(elems) + " elements");
+        cudaStream_t s = S(h, stream);
+        if (plane < 0) {
+            CUDA_CHECK(cudaMemcpyAsync(out, src, elems * 4, cudaMemcpyDeviceToDevice, s));
+        } else {                                          // hi + lo on the host: the aid launches no kernel
+            std::vector<__half> hi(elems), lo(elems);
+            CUDA_CHECK(cudaMemcpyAsync(hi.data(), h->arpl[2 * plane].p, elems * sizeof(__half), cudaMemcpyDeviceToHost, s));
+            CUDA_CHECK(cudaMemcpyAsync(lo.data(), h->arpl[2 * plane + 1].p, elems * sizeof(__half), cudaMemcpyDeviceToHost, s));
+            CUDA_CHECK(cudaStreamSynchronize(s));
+            std::vector<float> rows(elems);
+            for (size_t i = 0; i < elems; ++i) rows[i] = join_f16(hi[i], lo[i]);
+            CUDA_CHECK(cudaMemcpyAsync(out, rows.data(), elems * 4, cudaMemcpyHostToDevice, s));
+        }
+        CUDA_CHECK(cudaStreamSynchronize(s));
+        if (joined) *joined = plane >= 0 ? 1 : 0;
     });
 }
 

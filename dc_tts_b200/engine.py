@@ -377,6 +377,7 @@ class Engine:
         A = self._empty(B, self.hp.max_N, self.hp.max_T) if want_final_attention else None
         self._check(self._lib.dctts_text2mel_generate(self._h, _ptr(L), B, int(steps), _ptr(Y), _ptr(P), _ptr(M),
                                                       _ptr(A), self._stream()), "dctts_text2mel_generate")
+        self._decode_order = np.arange(B)
         return Y, P, M, A
 
     def text2mel_generate_until(self, L, stop_pos=None, tail=0, steps=0):
@@ -405,6 +406,7 @@ class Engine:
         self._check(self._lib.dctts_text2mel_generate_until(self._h, _ptr(Ls), B, int(steps), _ptr(sps), int(tail), _ptr(Y),
                                                             _ptr(P), _ptr(n), self._stream()),
                     "dctts_text2mel_generate_until")
+        self._decode_order = order
         if perm is None:
             return Y, P, n
         Yc, Pc, nc = torch.empty_like(Y), torch.empty_like(P), torch.empty_like(n)
@@ -454,11 +456,42 @@ class Engine:
                                                                 C.c_void_p(ns.ctypes.data), _ptr(Y), _ptr(P), _ptr(M),
                                                                 self._stream()),
                     "dctts_text2mel_generate_path_host")
+        self._decode_order = order
         if perm is None:
             return Y, P, M
         Yc, Pc, Mc = torch.empty_like(Y), torch.empty_like(P), torch.empty_like(M)
         Yc[perm], Pc[perm], Mc[perm] = Y, P, M
         return Yc, Pc, Mc
+
+    _HISTORY = {"audioenc": 0, "audiodec": 1, "R": 2, "KV": 3, "Y": 4, "windows": 5}
+
+    def decode_history(self, what, layer=0):
+        """Test aid (include/dctts.h: dctts_decode_history): the decode state of the last text2mel_generate(_until, _path) on
+        this engine, in that call's order of the utterances.  what: "audioenc" / "audiodec" (block `layer`'s output rows
+        (B, T, C), the last AudioDec block's are the logits), "R" (B, T, 2d), "KV" (B, N, 2d), "Y" (B, T, n_mels) or
+        "windows" (B, T) int32.  Returns (tensor, joined): joined is True when the rows are hi + lo of the split-fp16 planes
+        the decode kept instead of float32 rows.  Raises DcttsError when the engine's decode buffers were written by anything
+        else since that call."""
+        from .arch import audiodec_layers, audioenc_layers
+        if what not in self._HISTORY:
+            raise DcttsError("decode_history: `what` must be one of %s" % sorted(self._HISTORY))
+        order = getattr(self, "_decode_order", None)
+        if order is None:
+            raise DcttsError("decode_history: no generation has run on this engine")
+        h = self.hp
+        B, T = len(order), h.max_T
+        net = {"audioenc": audioenc_layers, "audiodec": audiodec_layers}.get(what)
+        if net is not None and not 0 <= layer < len(net()):
+            raise DcttsError("decode_history: %s has no block %d" % (what, layer))
+        shape = {"audioenc": (B, T, h.d), "audiodec": (B, T, net()[layer].cout if net else 0), "R": (B, T, 2 * h.d),
+                 "KV": (B, h.max_N, 2 * h.d), "Y": (B, T, h.n_mels), "windows": (B, T)}[what]
+        out = self._empty(*shape, dtype=torch.int32 if what == "windows" else torch.float32)
+        joined = C.c_int32(0)
+        self._check(self._lib.dctts_decode_history(self._h, self._HISTORY[what], int(layer), _ptr(out), out.numel(),
+                                                   C.byref(joined), self._stream()), "dctts_decode_history")
+        res = torch.empty_like(out)
+        res[torch.as_tensor(order, device=self.device)] = out
+        return res, bool(joined.value)
 
     def _set_vocoder_params(self, hop=None, win=None, power=None):
         """The hyperparameters' vocoder constants on the handle, with `hop`, `win` and `power` instead when given."""
@@ -854,6 +887,7 @@ class Engine:
             Y_host = torch.empty((B, self.hp.max_T, self.hp.n_mels), dtype=torch.float32).pin_memory()
         self._check(self._lib.dctts_synthesize_host(self._h, _ptr(L_host), B, _ptr(Y_host), _ptr(Z_host)),
                     "dctts_synthesize_host")
+        self._decode_order = np.arange(B)
         return Y_host, Z_host
 
 

@@ -385,6 +385,21 @@ int dctts_decode_stats(dctts_handle h, int32_t* moved_frames, int32_t* moved_utt
  * Buckets of the recompute's MMA warpgroup (thread 128), which overlap the above: 18 waiting for A slabs, 19 issuing the MMAs
  * and waiting for the slab before, 20 epilogue stores. */
 int dctts_decode_profile(dctts_handle h, int64_t* cycles, int32_t n);
+/* Test aid: the decode state of the last generation on the handle (dctts_text2mel_generate without max_attentions and
+ * alignments, _generate_until, _generate_path, dctts_synthesize_host), copied into caller DEVICE memory, n elements, in the
+ * order of the utterances the library decoded (the generation's B):
+ *   what 0: AudioEnc block `layer`'s output rows (B, T, d)         what 3: K | V (B, N, 2d)
+ *   what 1: AudioDec block `layer`'s output rows (B, T, d), the     what 4: Y (B, T, n_mels), rows past a length included
+ *           last block's logits (B, T, n_mels)                      what 5: the window of every frame (B, T) int32
+ *   what 2: R = [context | Q] (B, T, 2d)
+ * with T = max_T, N = max_N.  A row holds what the decode last wrote there; which rows are current depends on the decode
+ * (DESIGN.md, "The decode one block at a time").  The graph-per-frame decode (option decode_mode 0) on the tensor path at
+ * B >= 8 keeps the outputs of the AudioDec blocks whose successor also runs on the tensor cores as split-fp16 planes only:
+ * for those, the rows are hi + lo of the planes and *joined (optional) is set to 1, else 0.
+ * Fails with a message, copying nothing, when the handle's last writer of these buffers was anything but such a generation
+ * (a generation with the final attention pass, dctts_text2mel_forward, dctts_textenc, a workspace growth), or on a bad
+ * `what`, `layer` or n.  Launches no kernel; synchronises `stream`. */
+int dctts_decode_history(dctts_handle h, int32_t what, int32_t layer, void* out, int64_t n, int32_t* joined, void* stream);
 /* Measurement aid for bench.py's roofline leg: runs the block `scope` on a synthetic
  * (B,L,Cin) input `warmup`+`iters` times and returns the mean device time of each of its
  * kernels (CUDA events on `stream` around every launch), ms_per_kernel[0..*n_kernels), <= 8. */
