@@ -130,9 +130,12 @@ struct dctts_handle_s {
     DevBuf ad_sig;                // scratch for sigmoid(logits) in full-graph mode
     DevBuf ibuf;                  // ints: j, p_cur[B], p_next[B], p_prev[B], p_hist[B*T]
     DevBuf pathbuf;               // ints of a decode along a window path: lengths[B], path[B*T], argmax[B*T]
-    int* path_pinned = nullptr;   // pinned staging of pathbuf's lengths and path, reused once path_uploaded has fired
-    size_t path_pinned_n = 0;     // ints
+    int* path_pinned = nullptr;   // pinned staging of pathbuf's lengths and path, or of the aligner's lengths and ends,
+    size_t path_pinned_n = 0;     // reused once path_uploaded has fired (ints)
     cudaEvent_t path_uploaded = nullptr;
+    // the aligner (dctts_align_search, dctts_text2mel_align): back-pointers (B, T, N) uint8, lengths and ends (2B) ints, and
+    // the alignments (B, max_N, T) when the caller does not ask for them
+    struct { DevBuf bp, meta, A; } align;
     DevBuf lbuf;                  // (B, N) ids staging for the host entry point
     DevBuf zbuf;                  // (B, 4T, F) staging for the host entry point
     DevBuf plane[4];              // tensor-core path activations: {hi,lo} x ping-pong, rows x 1032 fp16

@@ -655,13 +655,14 @@ void text2mel_generate(H* h, const int* L, int B, int steps, float* Y, int* prev
     }
 }
 
-void text2mel_forward(H* h, const int* L, const float* mels, const int* pma, int B, float* Y,
-                      long long* maxatt, float* align, cudaStream_t s) {
+// The teacher-forced front of the Text2Mel graph over T <= max_T frames: TextEnc at max_N, AudioEnc over the T rows of
+// mels (B, T, n_mels) read one frame back (train.py:51), and the attention under the window pma, or dense over all max_N
+// keys when pma is null.  R goes to rbuf; on the wgmma path (the return value) its split planes also go to arpl[0..1]
+// for AudioDec.  Shared by text2mel_forward and the aligner.
+bool text2mel_front(Launch& lc, const int* L, const float* mels, const int* pma, int B, int T, long long* maxatt, float* align) {
+    H* h = lc.h;
     const dctts_hparams& hp = h->hp;
-    const int T = hp.max_T, N = hp.max_N, d = hp.d;
-    ensure_ws(h, B);
-    h->hist.ok = false;
-    Launch lc{h, s};
+    const int N = hp.max_N, d = hp.d;
     run_textenc(lc, L, B, h->kv.as<float>());
     const float* K = h->kv.as<float>();
     if (chain_tc_ok(h, h->audioenc) && chain_tc_ok(h, h->audiodec)) {
@@ -676,8 +677,7 @@ void text2mel_forward(H* h, const int* L, const float* mels, const int* pma, int
         else
             run_attention(lc, Q, d, K, 2 * d, K + d, 2 * d, RowWin{B, T, T, nullptr}, N, pma, h->rbuf.as<float>(),
                           align, maxatt, nullptr, nullptr, Rpl);
-        run_chain_tc_planes(lc, h->audiodec, Rpl, -1, B, T, h->ad_out.back().as<float>(), Y, 0, nullptr);
-        return;
+        return true;
     }
     // AudioEnc over all rows, reading mels shifted by one frame (train.py:51)
     const float* cur = mels; int ld = hp.n_mels;
@@ -690,7 +690,22 @@ void text2mel_forward(H* h, const int* L, const float* mels, const int* pma, int
     }
     run_attention(lc, cur, d, K, 2 * d, K + d, 2 * d, RowWin{B, T, T, nullptr}, N, pma, h->rbuf.as<float>(),
                   align, maxatt, nullptr, nullptr);
-    cur = h->rbuf.as<float>(); ld = 2 * d;
+    return false;
+}
+
+void text2mel_forward(H* h, const int* L, const float* mels, const int* pma, int B, float* Y,
+                      long long* maxatt, float* align, cudaStream_t s) {
+    const dctts_hparams& hp = h->hp;
+    const int T = hp.max_T, d = hp.d;
+    ensure_ws(h, B);
+    h->hist.ok = false;
+    Launch lc{h, s};
+    if (text2mel_front(lc, L, mels, pma, B, T, maxatt, align)) {
+        Planes Rpl; Rpl.hi = h->arpl[0].as<__half>(); Rpl.lo = h->arpl[1].as<__half>(); Rpl.ld = 2 * d;
+        run_chain_tc_planes(lc, h->audiodec, Rpl, -1, B, T, h->ad_out.back().as<float>(), Y, 0, nullptr);
+        return;
+    }
+    const float* cur = h->rbuf.as<float>(); int ld = 2 * d;
     for (size_t i = 0; i < h->audiodec.size(); ++i) {
         const LayerDev& l = h->audiodec[i];
         const bool last = (i + 1 == h->audiodec.size());
@@ -903,6 +918,19 @@ int dctts_text2mel_generate_until(dctts_handle h, const int32_t* L, int32_t B, i
 
 namespace {
 
+// The pinned staging buffer for n ints of host arrays that go to the device with one asynchronous copy.  The only wait
+// is for the previous upload out of it (path_uploaded, which the caller records after its copy).
+int* pinned_staging(H* h, size_t n) {
+    if (!h->path_uploaded) CUDA_CHECK(cudaEventCreateWithFlags(&h->path_uploaded, cudaEventDisableTiming));
+    CUDA_CHECK(cudaEventSynchronize(h->path_uploaded));          // the staging buffer is free again
+    if (h->path_pinned_n < n) {
+        if (h->path_pinned) { CUDA_CHECK(cudaFreeHost(h->path_pinned)); h->path_pinned = nullptr; h->path_pinned_n = 0; }
+        CUDA_CHECK(cudaMallocHost(&h->path_pinned, n * sizeof(int)));
+        h->path_pinned_n = n;
+    }
+    return h->path_pinned;
+}
+
 // dctts_text2mel_generate_path with the path (B, steps) and the lengths (B) in host memory.  They are checked before
 // anything is launched, then staged in pinned memory and uploaded with one asynchronous copy; the only wait is for the
 // previous call's upload out of the same staging buffer, so the host keeps queueing while earlier decodes run.
@@ -926,14 +954,7 @@ void generate_path(H* h, const int* L, int B, int steps, const int* p, const int
     ensure_ws(h, B);
     const PathRun pr = path_run(h);
     const size_t n_up = (size_t)h->ws_B + (size_t)B * T;      // pathbuf's lengths, then the first B path rows
-    if (!h->path_uploaded) CUDA_CHECK(cudaEventCreateWithFlags(&h->path_uploaded, cudaEventDisableTiming));
-    CUDA_CHECK(cudaEventSynchronize(h->path_uploaded));          // the staging buffer is free again
-    if (h->path_pinned_n < n_up) {
-        if (h->path_pinned) { CUDA_CHECK(cudaFreeHost(h->path_pinned)); h->path_pinned = nullptr; h->path_pinned_n = 0; }
-        CUDA_CHECK(cudaMallocHost(&h->path_pinned, n_up * sizeof(int)));
-        h->path_pinned_n = n_up;
-    }
-    int* st = h->path_pinned;
+    int* st = pinned_staging(h, n_up);
     std::copy(n, n + B, st);
     for (int b = 0; b < B; ++b)
         for (int j = 0; j < T; ++j)     // past the length: the last window, so no frame there moves it
@@ -950,7 +971,91 @@ void generate_path(H* h, const int* L, int B, int steps, const int* p, const int
     }
 }
 
+// The aligner's host-side checks (lengths n (B), ends e (B), in host memory), made before anything is launched; each
+// refusal names the utterance.  Returns the largest end, which sizes the search's shared memory.
+int check_align(H* h, const char* who, int B, int N, int T, const int* n, const int* e) {
+    const int w = h->hp.attention_win_size;
+    REQUIRE(w >= 1 && w <= 256, std::string(who) + ": attention_win_size must be in [1, 256]");
+    int smem_max = 0;
+    CUDA_CHECK(cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
+    int max_end = 0;
+    for (int b = 0; b < B; ++b) {
+        const std::string u = std::string(who) + ": utterance " + std::to_string(b);
+        if (n[b] < 1 || n[b] > T)
+            throw std::runtime_error(u + " has length " + std::to_string(n[b]) + " outside [1, " + std::to_string(T) + "]");
+        if (e[b] < 0 || e[b] >= N)
+            throw std::runtime_error(u + " has text end " + std::to_string(e[b]) + " outside [0, " + std::to_string(N) + ")");
+        if ((long long)e[b] > (long long)(w - 1) * n[b])
+            throw std::runtime_error(u + ": its text end " + std::to_string(e[b]) + " cannot be reached in " +
+                                     std::to_string(n[b]) + " frames with attention_win_size " + std::to_string(w) +
+                                     " (at most (w - 1) * frames): the text is too long for the recording");
+        if (2 * ((size_t)e[b] + 1) * sizeof(double) > (size_t)smem_max)
+            throw std::runtime_error(u + ": the search's rows for text end " + std::to_string(e[b]) +
+                                     " do not fit in the device's " + std::to_string(smem_max) + " bytes of shared memory");
+        max_end = std::max(max_end, e[b]);
+    }
+    return max_end;
+}
+
+// The search on A (B, N, T) DEVICE, after check_align: stages the lengths and ends, then one launch for the batch.
+void align_search(Launch& lc, const float* A, int B, int N, int T, const int* n, const int* e, int max_end,
+                  int* path, int* chars, int* durations, double* score) {
+    H* h = lc.h;
+    const size_t bp_bytes = (size_t)B * T * N, meta_bytes = 2 * (size_t)B * sizeof(int);
+    if (h->align.bp.bytes < bp_bytes || h->align.meta.bytes < meta_bytes) {
+        CUDA_CHECK(cudaDeviceSynchronize());              // an earlier search may still read the old buffers
+        h->align.bp.ensure(bp_bytes);
+        h->align.meta.ensure(meta_bytes);
+    }
+    int* st = pinned_staging(h, 2 * (size_t)B);
+    std::copy(n, n + B, st);
+    std::copy(e, e + B, st + B);
+    CUDA_CHECK(cudaMemcpyAsync(h->align.meta.p, st, meta_bytes, cudaMemcpyHostToDevice, lc.s));
+    CUDA_CHECK(cudaEventRecord(h->path_uploaded, lc.s));
+    AlignArgs a{};
+    a.A = A; a.meta = h->align.meta.as<int>(); a.bp = h->align.bp.as<unsigned char>();
+    a.path = path; a.chars = chars; a.durations = durations; a.score = score;
+    a.B = B; a.N = N; a.T = T; a.win = h->hp.attention_win_size;
+    launch_align_search(a, max_end, lc.s); lc.count();
+}
+
 }  // namespace
+
+int dctts_align_search(dctts_handle h, const float* alignments, int32_t B, int32_t N, int32_t T, const int32_t* lengths_host,
+                       const int32_t* ends_host, int32_t* path, int32_t* chars, int32_t* durations, double* score,
+                       void* stream) {
+    return guarded(h, [&] {
+        REQUIRE(B >= 1 && N >= 1 && T >= 1 && alignments && lengths_host && ends_host && path && chars && durations && score,
+                "dctts_align_search: bad arguments");
+        const int max_end = check_align(h, "dctts_align_search", B, N, T, lengths_host, ends_host);
+        Launch lc{h, S(h, stream)};
+        align_search(lc, alignments, B, N, T, lengths_host, ends_host, max_end, path, chars, durations, score);
+    });
+}
+
+int dctts_text2mel_align(dctts_handle h, const int32_t* L, const float* mels, int32_t B, int32_t T, const int32_t* lengths_host,
+                         const int32_t* ends_host, int32_t* path, int32_t* chars, int32_t* durations, double* score,
+                         float* alignments, void* stream) {
+    return guarded(h, [&] {
+        REQUIRE(h->committed, "parameters not committed");
+        REQUIRE(B >= 1 && L && mels && lengths_host && ends_host && path && chars && durations && score,
+                "dctts_text2mel_align: bad arguments");
+        REQUIRE(T >= 1 && T <= h->hp.max_T, "dctts_text2mel_align: T must be in [1, max_T]");
+        const int N = h->hp.max_N;
+        const int max_end = check_align(h, "dctts_text2mel_align", B, N, T, lengths_host, ends_host);
+        ensure_ws(h, B);
+        h->hist.ok = false;
+        Launch lc{h, S(h, stream)};
+        float* A = alignments;
+        if (!A) {
+            const size_t bytes = (size_t)B * N * T * sizeof(float);
+            if (h->align.A.bytes < bytes) { CUDA_CHECK(cudaDeviceSynchronize()); h->align.A.ensure(bytes); }
+            A = h->align.A.as<float>();
+        }
+        text2mel_front(lc, L, mels, nullptr, B, T, nullptr, A);
+        align_search(lc, A, B, N, T, lengths_host, ends_host, max_end, path, chars, durations, score);
+    });
+}
 
 int dctts_text2mel_generate_path(dctts_handle h, const int32_t* L, int32_t B, int32_t steps, const int32_t* path,
                                  const int32_t* lengths, float* Y, int32_t* prev_hist, int32_t* argmax_hist, void* stream) {

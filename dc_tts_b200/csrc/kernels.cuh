@@ -322,4 +322,17 @@ void launch_ar_advance(int* p_cur, const int* p_next, int* j, int B, cudaStream_
 void launch_ar_advance_path(int* p_cur, const int* p_next, int* j, const int* path, int* amax_hist, int B, int T, cudaStream_t s);
 void launch_fill_i32(int* p, int v, int n, cudaStream_t s);
 
+// ---- the aligner's monotonic path search (kernels_align.cu; DESIGN.md section 4d) ----
+struct AlignArgs {
+    const float* A;                // (B, N, T) alignments
+    const int* meta;               // (2B): the frames T_b of every utterance, then its text end e_b
+    unsigned char* bp;             // (B, T, N) back-pointer workspace
+    int* path; int* chars;         // (B, T) out, -1 past T_b
+    int* durations;                // (B, N) out
+    double* score;                 // (B) out: D[e_b, T_b - 1]
+    int B, N, T, win;
+};
+// one CTA per utterance with 2 (max_end + 1) doubles of dynamic shared memory; 1 launch
+void launch_align_search(const AlignArgs& a, int max_end, cudaStream_t s);
+
 }  // namespace dctts

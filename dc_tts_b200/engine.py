@@ -463,6 +463,75 @@ class Engine:
         Yc[perm], Pc[perm], Mc[perm] = Y, P, M
         return Yc, Pc, Mc
 
+    def _align_inputs(self, who, B, N, T, lengths, ends):
+        """Host int32 lengths (default all T) and ends (B,), checked as the entry points check them, naming the utterance."""
+        def host(x, default):
+            v = default if x is None else np.asarray(x.cpu() if isinstance(x, torch.Tensor) else x, np.int64).reshape(-1)
+            if v.shape[0] != B:
+                raise DcttsError("%s: %d values for %d utterances" % (who, v.shape[0], B))
+            return v
+        n, e = host(lengths, np.full(B, T, np.int64)), host(ends, None)
+        w = self.hp.attention_win_size
+        for b in range(B):
+            if not 1 <= n[b] <= T:
+                raise DcttsError("%s: utterance %d has length %d outside [1, %d]" % (who, b, n[b], T))
+            if e[b] < 0:
+                raise DcttsError("%s: utterance %d has no EOS (text end %d)" % (who, b, e[b]))
+            if e[b] >= N:
+                raise DcttsError("%s: utterance %d has text end %d outside [0, %d)" % (who, b, e[b], N))
+            if e[b] > (w - 1) * n[b]:
+                raise DcttsError("%s: utterance %d: its text end %d cannot be reached in %d frames with attention_win_size %d: "
+                                 "the text is too long for the recording" % (who, b, e[b], n[b], w))
+        return np.ascontiguousarray(n, np.int32), np.ascontiguousarray(e, np.int32)
+
+    def _align_outputs(self, B, N, T):
+        return (self._empty(B, T, dtype=torch.int32), self._empty(B, T, dtype=torch.int32),
+                self._empty(B, N, dtype=torch.int32), self._empty(B, dtype=torch.float64))
+
+    def align_search(self, alignments, lengths, ends):
+        """The aligner's search alone (include/dctts.h: dctts_align_search) on alignments (B, N, T): for utterance b, the
+        best monotonic path over lengths[b] frames ending at text position ends[b].  Returns CUDA tensors (path, chars,
+        durations, score): path (B, T) the window of every frame as text2mel_generate_path takes it, chars (B, T) the
+        character of every frame (both -1 past lengths[b]), durations (B, N) frames per text position, score (B,) float64
+        the path's summed log-attention."""
+        A = self._f32(alignments)
+        if A.dim() != 3:
+            raise DcttsError("align_search: alignments must be (B, N, T), got shape %s" % (tuple(A.shape),))
+        B, N, T = A.shape
+        n, e = self._align_inputs("align_search", B, N, T, lengths, ends)
+        path, chars, dur, score = self._align_outputs(B, N, T)
+        self._check(self._lib.dctts_align_search(self._h, _ptr(A), B, N, T, C.c_void_p(n.ctypes.data), C.c_void_p(e.ctypes.data),
+                                                 _ptr(path), _ptr(chars), _ptr(dur), _ptr(score), self._stream()),
+                    "dctts_align_search")
+        return path, chars, dur, score
+
+    def text2mel_align(self, L, mels, lengths=None, ends=None, want_alignments=False):
+        """Align recorded speech to its text (include/dctts.h: dctts_text2mel_align): the teacher-forced Text2Mel front
+        on L (B, max_N) and the recorded mels (B, T, n_mels), T <= max_T, then align_search on its dense attention.
+        `lengths`: (B,) frames per recording, default all T; mels rows at and past them must be zeros, as
+        load_spectrograms_batch writes them.  `ends`: (B,) text ends, default the EOS positions of L
+        (data_load.eos_positions); an utterance without EOS is refused.  Returns CUDA tensors (path, chars, durations,
+        score) as align_search does, and the alignments (B, max_N, T) when `want_alignments`."""
+        from .data_load import eos_positions
+        # Every host-side step comes before L is copied to the device (text2mel_generate_path explains why)
+        Lh = np.asarray(L.cpu() if isinstance(L, torch.Tensor) else L)
+        if Lh.ndim != 2 or Lh.shape[1] != self.hp.max_N:
+            raise DcttsError("text2mel_align: L must be (B, max_N=%d), got shape %s" % (self.hp.max_N, Lh.shape))
+        B, N = Lh.shape
+        ms = tuple(mels.shape)
+        if len(ms) != 3 or ms[0] != B or ms[2] != self.hp.n_mels or not 1 <= ms[1] <= self.hp.max_T:
+            raise DcttsError("text2mel_align: mels must be (B=%d, T <= max_T=%d, n_mels=%d), got shape %s"
+                             % (B, self.hp.max_T, self.hp.n_mels, ms))
+        T = ms[1]
+        n, e = self._align_inputs("text2mel_align", B, N, T, lengths, eos_positions(Lh) if ends is None else ends)
+        L, mels = self._i32(Lh), self._f32(mels)
+        path, chars, dur, score = self._align_outputs(B, N, T)
+        A = self._empty(B, N, T) if want_alignments else None
+        self._check(self._lib.dctts_text2mel_align(self._h, _ptr(L), _ptr(mels), B, T, C.c_void_p(n.ctypes.data),
+                                                   C.c_void_p(e.ctypes.data), _ptr(path), _ptr(chars), _ptr(dur), _ptr(score),
+                                                   _ptr(A), self._stream()), "dctts_text2mel_align")
+        return (path, chars, dur, score, A) if want_alignments else (path, chars, dur, score)
+
     _HISTORY = {"audioenc": 0, "audiodec": 1, "R": 2, "KV": 3, "Y": 4, "windows": 5}
 
     def decode_history(self, what, layer=0):

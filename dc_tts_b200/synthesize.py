@@ -20,8 +20,22 @@ from .params import init_params
 from .train import Graph, Session
 
 
+def _timing_of(g, L, wavs):
+    """The attention-window path (B, T) and frame counts (B,) of each sentence of L spoken with the timing of its
+    recording (one WAV file per sentence, at any sample rate)."""
+    from .utils import load_spectrograms_batch
+    if len(wavs) != len(L):
+        raise ValueError("timing_from: %d recordings for %d sentences" % (len(wavs), len(L)))
+    _, mels, _, t = load_spectrograms_batch(list(wavs), g.engine, resample=True)
+    over = np.flatnonzero(t > hp.max_T)
+    if over.size:
+        raise ValueError("timing_from: %s has %d frames, more than max_T = %d" % (wavs[over[0]], t[over[0]], hp.max_T))
+    path, _, _, _ = g.align(L, mels, t)
+    return path, t
+
+
 def synthesize(params=None, sentences=None, fast=True, write=True, seed=0, vocoder=True, allow_random_init=False,
-               until_eos=False, tail=0, momentum=0.0, duration_scale=1.0):
+               until_eos=False, tail=0, momentum=0.0, duration_scale=1.0, timing_from=None):
     """`params`: a name -> array dict to use instead of the checkpoints.  Without it the latest checkpoints of
     hp.logdir-1 (Text2Mel) and hp.logdir-2 (SSRN) are restored, and a missing one RAISES like the reference's
     `saver.restore(sess, None)` does (synthesize.py:33,39) -- seeded random weights are used only when the caller asks
@@ -38,7 +52,13 @@ def synthesize(params=None, sentences=None, fast=True, write=True, seed=0, vocod
     `duration_scale`: speaking rate, > 1 slower.  At any value other than 1.0 each utterance is first decoded to its EOS
     as with `until_eos=True`, its attention-window history is stretched by that factor (utils.stretch_path), and the
     utterance is decoded again along the stretched path (Graph.generate_along); SSRN and the vocoder then run with the
-    stretched lengths.  1.0 leaves every other route exactly as it is."""
+    stretched lengths.  1.0 leaves every other route exactly as it is.
+
+    `timing_from`: a list of WAV files, one recording per sentence.  Each sentence is spoken with the timing of its
+    recording: the recording's features (resampled to hp.sr when needed) are aligned to the sentence (Graph.align), the
+    recovered path is stretched by `duration_scale` when that is not 1, and the sentence is decoded along it
+    (Graph.generate_along); SSRN and the vocoder run with each recording's frame count (or the stretched one).  A
+    recording longer than max_T frames is refused.  None leaves every other route exactly as it is."""
     # Load data
     L = load_data("synthesize", sentences)
 
@@ -68,12 +88,16 @@ def synthesize(params=None, sentences=None, fast=True, write=True, seed=0, vocod
                                         "or allow_random_init=True for seeded random weights" % " and ".join(missing))
 
         lengths = None
-        if until_eos or duration_scale != 1.0:
-            Y, P, n = g.generate_until_eos(L, tail=tail)
+        if timing_from is not None or until_eos or duration_scale != 1.0:
+            if timing_from is not None:
+                P, n = _timing_of(g, L, timing_from)
+            else:
+                Y, P, n = g.generate_until_eos(L, tail=tail)
             if duration_scale != 1.0:
                 from .utils import stretch_path
-                path, n = stretch_path(P, n, duration_scale)
-                Y, _, _ = g.generate_along(L, path, n)
+                P, n = stretch_path(P, n, duration_scale)
+            if timing_from is not None or duration_scale != 1.0:
+                Y, _, _ = g.generate_along(L, P, n)
             lengths = n.cpu().numpy() if hasattr(n, "cpu") else np.asarray(n)
             Tmax = int(lengths.max())
             # SSRN at the batch's longest length; rows past each utterance's length come back as 0

@@ -199,6 +199,11 @@ class Graph:
         (Engine.text2mel_generate_path)."""
         return self.engine.text2mel_generate_path(L, path, lengths)
 
+    def align(self, L, mels, lengths=None):
+        """The attention-window path that speaks L with the timing of recorded mels (B, T, n_mels), lengths (B,) frames
+        per recording: returns (path, chars, durations, score) (Engine.text2mel_align); `path` feeds generate_along."""
+        return self.engine.text2mel_align(L, mels, lengths)
+
 
 class Session:
     """Minimal stand-in for tf.Session used as `with Session() as sess: sess.run(...)`."""

@@ -156,6 +156,33 @@ int dctts_text2mel_generate_path(dctts_handle h, const int32_t* L, int32_t B, in
 int dctts_text2mel_generate_path_host(dctts_handle h, const int32_t* L, int32_t B, int32_t steps,
                                       const int32_t* path_host, const int32_t* lengths_host, float* Y,
                                       int32_t* prev_hist, int32_t* argmax_hist, void* stream);
+/* ---- aligning recorded speech to its text (DESIGN.md section 4d) ------------------ */
+/* The best monotonic path through alignments (B, N, T) DEVICE float32 (e.g. dctts_train_eval's or
+ * dctts_text2mel_align's): for utterance b with T_b = lengths_host[b] frames and text end e_b = ends_host[b] (its EOS
+ * position), one character n_t per frame t < T_b with 0 <= n_0 <= w - 1, 0 <= n_t - n_{t-1} <= w - 1 and
+ * n_{T_b - 1} = e_b (w = attention_win_size) -- the paths the decode can follow -- maximising the sum of
+ * log(max(A[b, n_t, t], 1e-30f)) in float64; of two equal predecessors the smaller step wins.  Outputs, all DEVICE:
+ * chars (B, T) int32 = n_t; path (B, T) int32 = the window of each frame, path[b, 0] = 0 and path[b, t] = n_{t-1}, as
+ * dctts_text2mel_generate_path takes it; rows >= T_b are -1 in both; durations (B, N) int32 = frames per text position
+ * (0 for a position the path steps over; they sum to T_b); score (B) float64 = the path's summed log-attention.
+ * Refused before any launch, naming the utterance: T_b outside [1, T], e_b outside [0, N), e_b > (w - 1) T_b (the text
+ * is too long for the recording), or 2 (e_b + 1) doubles beyond the device's shared memory per block.  The lengths and
+ * ends are read on the host; the search is one launch for the batch, with no host synchronisation. */
+int dctts_align_search(dctts_handle h, const float* alignments, int32_t B, int32_t N, int32_t T,
+                       const int32_t* lengths_host, const int32_t* ends_host,
+                       int32_t* path, int32_t* chars, int32_t* durations, double* score, void* stream);
+/* The teacher-forced Text2Mel front and the search: L (B, max_N), mels (B, T, n_mels) DEVICE, 1 <= T <= max_T.  The
+ * alignments are the dense softmax over all max_N keys of each frame's query, with AudioEnc fed the mels shifted by one
+ * frame (train.py:51 at dropout 0); optional alignments (B, max_N, T) DEVICE receives them.  Then dctts_align_search with
+ * N = max_N, with the same checks made before anything is launched.  Rows of mels at or past lengths_host[b] must be
+ * zeros (as dctts_load_spectrograms_batch writes them): on the wgmma kernel set utterance b's outputs are then bit for
+ * bit those of the call on that utterance alone at T = lengths_host[b]; on the fp32 set they agree within float32
+ * rounding.  A trained handle with stale packing runs the fp32 kernels.  Clears the decode state that
+ * dctts_decode_history reads. */
+int dctts_text2mel_align(dctts_handle h, const int32_t* L, const float* mels, int32_t B, int32_t T,
+                         const int32_t* lengths_host, const int32_t* ends_host,
+                         int32_t* path, int32_t* chars, int32_t* durations, double* score,
+                         float* alignments, void* stream);
 /* synthesize.py:45-57 end to end with HOST buffers: copies L_host in, runs
  * dctts_text2mel_generate + dctts_ssrn, copies Y_host (B,max_T,n_mels; may be NULL) and
  * Z_host (B,4*max_T,F) out, and synchronises.  Host buffers should be pinned for speed. */
