@@ -45,6 +45,7 @@ SIGNATURES = {
     "dctts_text2mel_generate_path_host": (C.c_int, [Handle, _p, _i32, _i32, _p, _p, _p, _p, _p, _p]),
     "dctts_align_search": (C.c_int, [Handle, _p, _i32, _i32, _i32, _p, _p, _p, _p, _p, _p, _p]),
     "dctts_text2mel_align": (C.c_int, [Handle, _p, _p, _i32, _i32, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "dctts_mcd_dtw": (C.c_int, [Handle, _p, _i32, _p, _p, _i32, _p, _i32, _i32, _p, _p, _p, _p]),
     "dctts_synthesize_host": (C.c_int, [Handle, _p, _i32, _p, _p]),
     "dctts_bench_block": (C.c_int, [Handle, C.c_char_p, _i32, _i32, _i32, _i32, C.POINTER(C.c_float),
                                     C.POINTER(_i32), _p]),

@@ -35,18 +35,25 @@ def _reason(engine, text_len, frames):
     return None
 
 
-def _features(engine, fpaths, from_wavs, resample):
-    """(mels (B, T_b, n_mels) zero-padded, frames (B,)) of a batch of utterances, through the trainer's loaders."""
+def _features(engine, fpaths, from_wavs, resample, mags=False):
+    """(mels (B, T_b, n_mels) zero-padded, frames (B,)) of a batch of utterances, through the trainer's loaders; with
+    `mags`, also each utterance's magnitudes (B entries of (r frames_b, F), numpy or CUDA tensors) as a third value."""
     if from_wavs:
         from .utils import _read_pcm_for
         pcms, rates = zip(*[_read_pcm_for(p, resample) for p in fpaths])
-        mels, _, t, _ = engine.load_spectrograms_batch(list(pcms), rates=list(rates))
-        return mels, np.asarray(t, np.int64)
-    ms = [_load_spectrograms_npy(p)[1] for p in fpaths]
+        mels, mg, t, _ = engine.load_spectrograms_batch(list(pcms), rates=list(rates))
+        t = np.asarray(t, np.int64)
+        if mags:
+            return mels, t, [mg[b, :engine.hp.r * int(t[b])] for b in range(len(t))]
+        return mels, t
+    loaded = [_load_spectrograms_npy(p) for p in fpaths]
+    ms = [m for _, m, _ in loaded]
     t = np.array([m.shape[0] for m in ms], np.int64)
     mels = np.zeros((len(ms), max(1, int(t.max())), engine.hp.n_mels), np.float32)
     for b, m in enumerate(ms):
         mels[b, :len(m)] = m
+    if mags:
+        return mels, t, [g for _, _, g in loaded]
     return mels, t
 
 

@@ -136,6 +136,9 @@ struct dctts_handle_s {
     // the aligner (dctts_align_search, dctts_text2mel_align): back-pointers (B, T, N) uint8, lengths and ends (2B) ints, and
     // the alignments (B, max_N, T) when the caller does not ask for them
     struct { DevBuf bp, meta, A; } align;
+    // MCD-DTW (dctts_mcd_dtw): back-pointers (sum nx_b ny_b bytes), per-pair lengths and offsets (4B int64), the cepstra
+    // of pairs too long for shared memory, and rows 1 .. n_mels - 1 of the DCT-II matrix (uploaded at the first call)
+    struct { DevBuf bp, meta, cep, dct; } mcd;
     DevBuf lbuf;                  // (B, N) ids staging for the host entry point
     DevBuf zbuf;                  // (B, 4T, F) staging for the host entry point
     DevBuf plane[4];              // tensor-core path activations: {hi,lo} x ping-pong, rows x 1032 fp16

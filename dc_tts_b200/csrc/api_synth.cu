@@ -1057,6 +1057,68 @@ int dctts_text2mel_align(dctts_handle h, const int32_t* L, const float* mels, in
     });
 }
 
+int dctts_mcd_dtw(dctts_handle h, const float* X, int32_t Tx, const int32_t* nx_host, const float* Y, int32_t Ty,
+                  const int32_t* ny_host, int32_t B, int32_t K, double* mcd, int32_t* pairs, int32_t* path, void* stream) {
+    return guarded(h, [&] {
+        const int M = h->hp.n_mels;
+        REQUIRE(B >= 1 && Tx >= 1 && Ty >= 1 && X && Y && nx_host && ny_host && mcd && pairs, "dctts_mcd_dtw: bad arguments");
+        REQUIRE(K >= 1 && K <= M - 1, "dctts_mcd_dtw: K must be in [1, n_mels - 1 = " + std::to_string(M - 1) + "], got " +
+                                      std::to_string(K));
+        int smem_max = 0;
+        CUDA_CHECK(cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
+        // per pair: lengths, back-pointer offset, and the cepstra in shared memory (-1) or at a workspace offset
+        const size_t ldc = (size_t)(K | 1);
+        std::vector<long long> meta(4 * (size_t)B);
+        size_t bp_bytes = 0, cep_doubles = 0, smem = 0;
+        for (int b = 0; b < B; ++b) {
+            const std::string u = "dctts_mcd_dtw: utterance " + std::to_string(b);
+            const long long nx = nx_host[b], ny = ny_host[b];
+            if (nx < 1 || nx > Tx)
+                throw std::runtime_error(u + " has X length " + std::to_string(nx) + " outside [1, " + std::to_string(Tx) + "]");
+            if (ny < 1 || ny > Ty)
+                throw std::runtime_error(u + " has Y length " + std::to_string(ny) + " outside [1, " + std::to_string(Ty) + "]");
+            const size_t diag = 3 * (size_t)nx * sizeof(double), cep = (size_t)(nx + ny) * ldc * sizeof(double);
+            if (diag > (size_t)smem_max)
+                throw std::runtime_error(u + ": three diagonals of " + std::to_string(nx) + " doubles do not fit in the device's " +
+                                         std::to_string(smem_max) + " bytes of shared memory");
+            const bool staged = diag + cep <= (size_t)smem_max;
+            meta[4 * b] = nx; meta[4 * b + 1] = ny; meta[4 * b + 2] = (long long)bp_bytes;
+            meta[4 * b + 3] = staged ? -1 : (long long)cep_doubles;
+            bp_bytes += (size_t)nx * ny;
+            if (!staged) cep_doubles += (size_t)(nx + ny) * ldc;
+            smem = std::max(smem, staged ? diag + cep : diag);
+        }
+        const size_t meta_bytes = meta.size() * sizeof(long long);
+        if (h->mcd.bp.bytes < bp_bytes || h->mcd.meta.bytes < meta_bytes || h->mcd.cep.bytes < cep_doubles * sizeof(double)) {
+            CUDA_CHECK(cudaDeviceSynchronize());              // an earlier call may still use the old buffers
+            h->mcd.bp.ensure(bp_bytes);
+            h->mcd.meta.ensure(meta_bytes);
+            h->mcd.cep.ensure(cep_doubles * sizeof(double));
+        }
+        if (!h->mcd.dct.p) {                                  // D[k, m] = sqrt(2 / M) cos(pi k (2m + 1) / (2M)), k >= 1
+            std::vector<double> D((size_t)(M - 1) * M);
+            const double pi = 3.141592653589793;
+            for (int k = 1; k < M; ++k)
+                for (int m = 0; m < M; ++m)
+                    D[(size_t)(k - 1) * M + m] = std::sqrt(2.0 / M) * std::cos(pi * k * (2 * m + 1) / (2.0 * M));
+            h->mcd.dct.ensure(D.size() * sizeof(double));
+            CUDA_CHECK(cudaMemcpy(h->mcd.dct.p, D.data(), D.size() * sizeof(double), cudaMemcpyHostToDevice));
+        }
+        Launch lc{h, S(h, stream)};
+        int* st = pinned_staging(h, 2 * meta.size());
+        std::memcpy(st, meta.data(), meta_bytes);
+        CUDA_CHECK(cudaMemcpyAsync(h->mcd.meta.p, st, meta_bytes, cudaMemcpyHostToDevice, lc.s));
+        CUDA_CHECK(cudaEventRecord(h->path_uploaded, lc.s));
+        McdArgs a{};
+        a.X = X; a.Y = Y; a.meta = h->mcd.meta.as<long long>(); a.dct = h->mcd.dct.as<double>();
+        a.cep = h->mcd.cep.as<double>(); a.bp = h->mcd.bp.as<unsigned char>();
+        a.mcd = mcd; a.pairs = pairs; a.path = path;
+        a.max_db = h->voc.max_db; a.ref_db = h->voc.ref_db;
+        a.B = B; a.Tx = Tx; a.Ty = Ty; a.n_mels = M; a.K = K;
+        launch_mcd_dtw(a, smem, lc.s); lc.count();
+    });
+}
+
 int dctts_text2mel_generate_path(dctts_handle h, const int32_t* L, int32_t B, int32_t steps, const int32_t* path,
                                  const int32_t* lengths, float* Y, int32_t* prev_hist, int32_t* argmax_hist, void* stream) {
     return guarded(h, [&] {

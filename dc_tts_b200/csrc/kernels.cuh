@@ -335,4 +335,19 @@ struct AlignArgs {
 // one CTA per utterance with 2 (max_end + 1) doubles of dynamic shared memory; 1 launch
 void launch_align_search(const AlignArgs& a, int max_end, cudaStream_t s);
 
+// ---- mel-cepstral distortion along a DTW alignment (kernels_mcd.cu; DESIGN.md section 8h) ----
+struct McdArgs {
+    const float* X; const float* Y;    // (B, Tx, n_mels), (B, Ty, n_mels) dB-normalised mels
+    const long long* meta;             // (4B): nx_b, ny_b, back-pointer offset, cepstrum workspace offset (-1: shared memory)
+    const double* dct;                 // (K, n_mels): rows 1 .. K of the orthonormal DCT-II matrix
+    double* cep;                       // cepstra of the pairs that do not fit in shared memory, rows of K | 1 doubles
+    unsigned char* bp;                 // back-pointers, nx_b ny_b bytes per pair
+    double* mcd; int* pairs;           // (B) out
+    int* path;                         // (B, Tx + Ty - 1, 2) out (i, j), -1 past pairs[b]; may be null
+    double max_db, ref_db;
+    int B, Tx, Ty, n_mels, K;
+};
+// one CTA per pair with `smem` bytes of dynamic shared memory; 1 launch
+void launch_mcd_dtw(const McdArgs& a, size_t smem, cudaStream_t s);
+
 }  // namespace dctts

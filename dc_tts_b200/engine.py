@@ -532,6 +532,44 @@ class Engine:
                                                    _ptr(A), self._stream()), "dctts_text2mel_align")
         return (path, chars, dur, score, A) if want_alignments else (path, chars, dur, score)
 
+    def mcd_dtw(self, X, nx, Y, ny, K=24, want_path=False):
+        """Mel-cepstral distortion along a DTW alignment (include/dctts.h: dctts_mcd_dtw) between X[b, :nx[b]] and
+        Y[b, :ny[b]], X (B, Tx, n_mels) and Y (B, Ty, n_mels) dB-normalised mels (Text2Mel's output, load_spectrograms's
+        mels), using cepstral coefficients 1 .. K of an orthonormal DCT of the log mel amplitudes.  `nx`, `ny`: (B,)
+        frames per sequence, read on the host.  Returns CUDA tensors (mcd (B,) float64, pairs (B,) int32: the cells on
+        the path), and the path (B, Tx + Ty - 1, 2) int32 of (i, j) from (0, 0), -1 past pairs[b], when `want_path`.
+        An MFCC-style distortion, not comparable to published (SPTK / WORLD) MCD figures."""
+        X, Y = self._f32(X), self._f32(Y)
+        M = self.hp.n_mels
+        if X.dim() != 3 or X.shape[2] != M:
+            raise DcttsError("mcd_dtw: X must be (B, Tx, n_mels=%d), got shape %s" % (M, tuple(X.shape)))
+        B, Tx = X.shape[0], X.shape[1]
+        if Y.dim() != 3 or Y.shape[0] != B or Y.shape[2] != M:
+            raise DcttsError("mcd_dtw: Y must be (B=%d, Ty, n_mels=%d), got shape %s" % (B, M, tuple(Y.shape)))
+        Ty = Y.shape[1]
+        if B < 1 or Tx < 1 or Ty < 1:
+            raise DcttsError("mcd_dtw: empty batch or sequences: X %s, Y %s" % (tuple(X.shape), tuple(Y.shape)))
+        if not 1 <= int(K) <= M - 1:
+            raise DcttsError("mcd_dtw: K must be in [1, n_mels - 1 = %d], got %d" % (M - 1, int(K)))
+
+        def host(x, name, T):
+            v = np.asarray(x.cpu() if isinstance(x, torch.Tensor) else x, np.int64).reshape(-1)
+            if v.shape[0] != B:
+                raise DcttsError("mcd_dtw: %d %s lengths for %d utterances" % (v.shape[0], name, B))
+            bad = np.flatnonzero((v < 1) | (v > T))
+            if bad.size:
+                raise DcttsError("mcd_dtw: utterance %d has %s length %d outside [1, %d]" % (bad[0], name, v[bad[0]], T))
+            return np.ascontiguousarray(v, np.int32)
+        nxh, nyh = host(nx, "X", Tx), host(ny, "Y", Ty)
+        self._set_vocoder_params()
+        mcd = self._empty(B, dtype=torch.float64)
+        pairs = self._empty(B, dtype=torch.int32)
+        path = self._empty(B, Tx + Ty - 1, 2, dtype=torch.int32) if want_path else None
+        self._check(self._lib.dctts_mcd_dtw(self._h, _ptr(X), Tx, C.c_void_p(nxh.ctypes.data), _ptr(Y), Ty,
+                                            C.c_void_p(nyh.ctypes.data), B, int(K), _ptr(mcd), _ptr(pairs), _ptr(path),
+                                            self._stream()), "dctts_mcd_dtw")
+        return (mcd, pairs, path) if want_path else (mcd, pairs)
+
     _HISTORY = {"audioenc": 0, "audiodec": 1, "R": 2, "KV": 3, "Y": 4, "windows": 5}
 
     def decode_history(self, what, layer=0):

@@ -351,9 +351,23 @@ def write_samples(engine, texts, logdir, global_step, writer=None):
     return wavs, lengths
 
 
+def write_heldout(engine, heldout, num, logdir, global_step, train_batch, writer=None):
+    """`heldout.run` at `global_step`: its summary appended to `logdir/heldout.tsv`, its rows in
+    `heldout_{NNN}k.tsv`, and with a `writer` one event of `heldout/...` scalars.  Returns (rows, summary)."""
+    from . import heldout as ho
+    rows, summary = heldout.run(engine, num, global_step, train_batch=train_batch)
+    ho.write_table(os.path.join(logdir, "heldout_" + str(global_step // 1000).zfill(3) + "k.tsv"), rows, num)
+    ho.append_log(os.path.join(logdir, "heldout.tsv"), global_step, summary)
+    if writer is not None:
+        from .summary import merge, scalar
+        writer.add_summary(merge(*[scalar("heldout/" + k, v) for k, v in ho.scalars(summary)]), global_step)
+        writer.flush()
+    return rows, summary
+
+
 def train(num, engine, batches, num_iterations=None, logdir=None, global_step=None, save_every=1000, log=print, resume=True,
           rank=0, world=1, allreduce=None, beyond_capacity="skip", capacity=None, summaries=False, summary_secs=120,
-          samples=None, deterministic=None):
+          samples=None, deterministic=None, heldout=None):
     """train.py:137-160 for num = 1 (Text2Mel) or 2 (SSRN).  `batches` yields (L, mels, mags, names, ...): the bucketed
     batches of `bucketed_batches` at their own shapes or fixed-size ones; `engine` is an `Engine` with parameters loaded.
     The workspace is allocated for the capacity (hp.max_N, hp.max_T), or `capacity` = (N, T) when that is larger; a batch
@@ -381,6 +395,11 @@ def train(num, engine, batches, num_iterations=None, logdir=None, global_step=No
     checkpoint writes the bundles of the run that never stopped.  Each rank's gradient arena is deterministic; the order of
     the cross-rank all-reduce belongs to torch.distributed.  `deterministic=False` sets the option to 0 (the default
     kernels); None (the default) leaves the engine's option as it is, which is 0 unless the caller set it.
+    `heldout` (default None: off): a heldout.HeldOut that rank 0 runs at every checkpoint, after the save and the samples,
+    on the weights being trained.  `logdir/heldout.txt` lists its fnames (for `python -m dc_tts_b200.heldout --list`);
+    each checkpoint appends the global step and the summary to `logdir/heldout.tsv` and writes the per-utterance table to
+    `heldout_{NNN}k.tsv`, and with `summaries` one event holds its numbers as `heldout/...` scalars.  It consumes no
+    batch and changes no training state.
     Returns the final global step."""
     if num not in (1, 2):
         raise ValueError("num: 1 for Text2Mel, 2 for SSRN (train.py:139)")
@@ -396,6 +415,9 @@ def train(num, engine, batches, num_iterations=None, logdir=None, global_step=No
     batches = iter(batches)
     writer = None
     texts = sample_texts(samples) if samples is not None and rank == 0 else None
+    if heldout is not None and rank == 0:
+        with open(os.path.join(logdir, "heldout.txt"), "w") as f:
+            f.write("".join(n + "\n" for n in heldout.fnames))
 
     def next_admitted():
         for b in batches:
@@ -458,6 +480,8 @@ def train(num, engine, batches, num_iterations=None, logdir=None, global_step=No
                     plot_alignment(ev[1]["alignments"][0].cpu().numpy(), str(gs // 1000).zfill(3) + "k", logdir)
             if texts is not None:
                 write_samples(engine, texts, logdir, gs, writer)
+            if heldout is not None:
+                write_heldout(engine, heldout, num, logdir, gs, len(L), writer)
         if writer is not None and time.time() - last_t >= summary_secs:
             ev = evaluate_next()
             now = time.time()

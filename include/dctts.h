@@ -183,6 +183,25 @@ int dctts_text2mel_align(dctts_handle h, const int32_t* L, const float* mels, in
                          const int32_t* lengths_host, const int32_t* ends_host,
                          int32_t* path, int32_t* chars, int32_t* durations, double* score,
                          float* alignments, void* stream);
+/* ---- held-out quality: mel-cepstral distortion along a DTW alignment (DESIGN.md section 8h) ------------------ */
+/* MCD-DTW between pairs of dB-normalised mel sequences (what Text2Mel produces and dctts_load_spectrograms_batch writes):
+ * X (B, Tx, n_mels) and Y (B, Ty, n_mels) DEVICE float32; pair b compares X[b, :nx_host[b]] with Y[b, :ny_host[b]].
+ * Per frame, in float64: a_m = (ln 10 / 20) (max_db x_m - max_db + ref_db) (the log amplitude, max_db and ref_db from
+ * dctts_set_vocoder_params), c_k = sum_m a_m D[k, m] for k = 1 .. K, D the orthonormal DCT-II matrix
+ * (D[k, m] = sqrt(2 / n_mels) cos(pi k (2m + 1) / (2 n_mels)); c_0, the energy, is left out).  Local cost
+ * d(i, j) = (10 / ln 10) sqrt(2 sum_k (cx_ik - cy_jk)^2); D(0, 0) = d(0, 0), D(i, j) = d(i, j) + min(D(i-1, j-1),
+ * D(i-1, j), D(i, j-1)), a tie going to the first of the three in that order (diagonal, advance X, advance Y); the
+ * path ends at (nx_b - 1, ny_b - 1).  Outputs, DEVICE: mcd (B) float64 = D(nx_b - 1, ny_b - 1) / P_b with P_b the
+ * cells on the path; pairs (B) int32 = P_b; path (B, Tx + Ty - 1, 2) int32 (i, j) from (0, 0), -1 past P_b, or NULL.
+ * This is an MFCC-style distortion (a DCT of log mel amplitudes), not an SPTK / WORLD mel-cepstrum: its values are not
+ * comparable to published MCD figures.  Refused before any launch, naming the utterance: nx_b outside [1, Tx], ny_b
+ * outside [1, Ty], or three diagonals of nx_b doubles beyond the device's shared memory per block; K outside
+ * [1, n_mels - 1].  Each pair's result does not depend on the other pairs.  One launch for the batch, with no host
+ * synchronisation except the upload of D at the handle's first call; needs no parameters and leaves the decode and
+ * training state alone. */
+int dctts_mcd_dtw(dctts_handle h, const float* X, int32_t Tx, const int32_t* nx_host,
+                  const float* Y, int32_t Ty, const int32_t* ny_host, int32_t B, int32_t K,
+                  double* mcd, int32_t* pairs, int32_t* path, void* stream);
 /* synthesize.py:45-57 end to end with HOST buffers: copies L_host in, runs
  * dctts_text2mel_generate + dctts_ssrn, copies Y_host (B,max_T,n_mels; may be NULL) and
  * Z_host (B,4*max_T,F) out, and synchronises.  Host buffers should be pinned for speed. */
