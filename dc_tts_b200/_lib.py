@@ -53,6 +53,8 @@ SIGNATURES = {
                                   _i32, _p, _i32, _p]),
     "dctts_block_bwd": (C.c_int, [Handle, _i32, _i32, _i64, _i32, _p, _i32, _p, _i32, _p, _i32, _p, C.c_float, _i32, C.c_uint32,
                                   _p, _p, _p, _p]),
+    "dctts_block_fwd": (C.c_int, [Handle, _i32, _i32, _i64, _i32, _p, _i32, _p, _i32, _p, C.c_float, _i32, C.c_uint32, _p, _i32,
+                                  _p]),
     "dctts_attn_bwd": (C.c_int, [Handle, _p, _p, _p, _p, _p, _i32, _i32, _i32, _i32, _i32, _i32, _p, _p, _p, _p]),
     "dctts_train_loss": (C.c_int, [Handle, _p, _i32, _p, _i64, _i32, _p, _i32, _p, _p, _p]),
     "dctts_vocoder_stage": (C.c_int, [Handle, _i32, _i32, _i32, _p, _p, _p, C.POINTER(_i32), _p]),
@@ -92,6 +94,8 @@ SIGNATURES = {
     "dctts_decode_stats": (C.c_int, [Handle, C.POINTER(_i32), C.POINTER(_i32), C.POINTER(_i32)]),
     "dctts_decode_profile": (C.c_int, [Handle, C.POINTER(_i64), _i32]),
     "dctts_decode_history": (C.c_int, [Handle, _i32, _i32, _p, _i64, C.POINTER(_i32), _p]),
+    "dctts_chain_history_shape": (C.c_int, [Handle, _i32, _i32, _i32, C.POINTER(_i32), C.POINTER(_i32), C.POINTER(_i32)]),
+    "dctts_chain_history": (C.c_int, [Handle, _i32, _i32, _i32, _p, _i64, C.POINTER(_i32), _p]),
     "dctts_malloc": (C.c_int, [Handle, C.POINTER(_p), _i64]),
     "dctts_free": (C.c_int, [Handle, _p]),
     "dctts_memcpy_h2d": (C.c_int, [Handle, _p, _p, _i64, _p]),

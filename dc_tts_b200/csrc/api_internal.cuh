@@ -206,6 +206,7 @@ struct dctts_handle_s {
         int train_probe = 0;      // measurement only (tools/bench_train.py --probe): the training GEMMs fetch their operands but issue no MMA
         int train_tc = 7;         // training GEMMs on wgmma, bit mask: 1 forward conv, 2 data gradient, 4 weight gradient; 0 = fp32 CUDA-core kernels
         int train_deterministic = 0;   // 1: the training step's sums in a fixed order (kernels_ordered.cu): a seeded run repeats bit for bit
+        int chain_history = 0;    // test aid: the full-sequence chains copy every block's rows for dctts_chain_history
     } opt;
 
     // persistent decode (kernels_decode.cu)
@@ -231,6 +232,16 @@ struct dctts_handle_s {
         int B = 0;                // utterances of that generation
         unsigned planes_only = 0; // bit i: AudioDec block i wrote only its split planes (arpl[i + 1]), not ad_out[i]
     } hist;
+
+    // What dctts_chain_history may read (option chain_history): copies of the rows the last full-sequence chains left,
+    // made device to device as they ran.  Per network (CH_TEXTENC .. CH_ATTENTION): rec[0] the first block's input as the
+    // kernel read it, rec[1 + i] block i's output; the attention's rec[1] is R.  A record holds fp32 rows or a plane pair.
+    struct ChainRec { DevBuf a, b; int B = 0, L = 0, C = 0, ld = 0; bool planes = false, scaled = false; DevBuf inv; };
+    struct {
+        std::vector<ChainRec> rec[5];
+        unsigned nets = 0;        // bit n: network n's records belong to the last writer
+        std::string why = "no full-sequence chain has run since the handle was created";   // why a network is not readable
+    } chist;
 
     // the device buffers free themselves after this body: the graph that points into them goes first
     ~dctts_handle_s() {
@@ -288,6 +299,7 @@ void pack_weights(H* h, cudaStream_t s);
 void mark_synthesis_stale(H* h);
 std::vector<int> audiodec_rows(const std::vector<LayerDev>& net, int T);          // api_synth.cu
 void settle_decode_counts(H* h);
+void chist_clear(H* h, const std::string& why);                                  // the chain history is stale
 void drop_ar_graph(H* h);
 void run_attention(Launch& lc, const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
                    RowWin win, int N, const int* pma, float* R, float* align, long long* maxatt,

@@ -358,7 +358,12 @@ int dctts_set_param(dctts_handle h, const char* tf_name, const float* data, cons
     });
 }
 
-int dctts_commit_params(dctts_handle h) { return guarded(h, [&] { commit_params(h); }); }
+int dctts_commit_params(dctts_handle h) {
+    return guarded(h, [&] {
+        commit_params(h);
+        chist_clear(h, "the weights were committed after the last full-sequence chain");
+    });
+}
 
 int64_t dctts_num_params(dctts_handle h) { return (h && h->committed) ? h->n_params : -1; }
 
@@ -366,6 +371,7 @@ int dctts_refresh_synthesis(dctts_handle h, void* stream) {
     return guarded(h, [&] {
         REQUIRE(h->committed, "dctts_refresh_synthesis: parameters not committed");
         if (!h->synth_stale) return;
+        chist_clear(h, "the weights were repacked after the last full-sequence chain");
         pack_weights(h, S(h, stream));
         CUDA_CHECK(cudaDeviceSynchronize());          // a replay of the captured AR step may still be in flight on another stream
         drop_ar_graph(h);

@@ -53,10 +53,70 @@ void dctts::api::drop_ar_graph(H* h) {
     if (h->ar_exec) { cudaGraphExecDestroy(h->ar_exec); h->ar_exec = nullptr; h->ar_B = 0; }
 }
 
+// Something other than a full-sequence chain wrote the synthesis buffers or the weights: no record describes the last
+// call any more.
+void dctts::api::chist_clear(H* h, const std::string& why) { h->chist.nets = 0; h->chist.why = why; }
+
 namespace {
+
+// ---------------------------------------------------------------------------- chain history (option chain_history)
+// Test aid: with the option on, the full-sequence chains copy each block's rows into handle-owned buffers as they run
+// (device to device; no kernel, so the launch sequence is the same with the option off), for dctts_chain_history.
+enum { CH_TEXTENC = 0, CH_AUDIOENC = 1, CH_AUDIODEC = 2, CH_SSRN = 3, CH_ATTENTION = 4 };
+
+int chain_net(H* h, const std::vector<LayerDev>& net) {
+    if (&net == &h->textenc) return CH_TEXTENC;
+    if (&net == &h->audioenc) return CH_AUDIOENC;
+    if (&net == &h->audiodec) return CH_AUDIODEC;
+    return CH_SSRN;
+}
+
+// The start of an entry point whose chains are recorded: the records of earlier calls go stale.
+void chist_begin(H* h, const char* who) {
+    chist_clear(h, h->opt.chain_history ? std::string("the last call (") + who + ") ran no full-sequence chain of that network"
+                                        : std::string("option chain_history was off during the last call (") + who + ")");
+}
+
+H::ChainRec& chist_slot(H* h, int net, int slot, int B, int L, int C, int ld, bool planes) {
+    auto& v = h->chist.rec[net];
+    if ((int)v.size() <= slot) v.resize((size_t)slot + 1);
+    H::ChainRec& r = v[(size_t)slot];
+    r.B = B; r.L = L; r.C = C; r.ld = ld; r.planes = planes; r.scaled = false;
+    h->chist.nets |= 1u << net;
+    return r;
+}
+
+// slot 0: the first block's input, slot 1 + i: block i's output.  fp32 rows (B * L of them, pitch ld) ...
+void chist_f32(Launch& lc, int net, int slot, const float* src, int ld, int B, int L, int C) {
+    H* h = lc.h;
+    if (!h->opt.chain_history) return;
+    H::ChainRec& r = chist_slot(h, net, slot, B, L, C, C, false);
+    if (!src) { r.B = 0; return; }                          // the caller did not ask for these rows: nothing kept
+
+    r.a.ensure((size_t)B * L * C * sizeof(float));
+    CUDA_CHECK(cudaMemcpy2DAsync(r.a.p, (size_t)C * sizeof(float), src, (size_t)ld * sizeof(float), (size_t)C * sizeof(float),
+                                 (size_t)B * L, cudaMemcpyDeviceToDevice, lc.s));
+}
+
+// ... or split planes, with the inverse per-utterance scales the first block applies to them (in_inv, or null)
+void chist_planes(Launch& lc, int net, int slot, Planes p, int B, int L, int C, const float* in_inv) {
+    H* h = lc.h;
+    if (!h->opt.chain_history) return;
+    H::ChainRec& r = chist_slot(h, net, slot, B, L, C, p.ld, true);
+    const size_t bytes = (size_t)B * L * p.ld * sizeof(__half);
+    r.a.ensure(bytes); r.b.ensure(bytes);
+    CUDA_CHECK(cudaMemcpyAsync(r.a.p, p.hi, bytes, cudaMemcpyDeviceToDevice, lc.s));
+    CUDA_CHECK(cudaMemcpyAsync(r.b.p, p.lo, bytes, cudaMemcpyDeviceToDevice, lc.s));
+    if (in_inv) {
+        r.scaled = true;
+        r.inv.ensure((size_t)B * sizeof(float));
+        CUDA_CHECK(cudaMemcpyAsync(r.inv.p, in_inv, (size_t)B * sizeof(float), cudaMemcpyDeviceToDevice, lc.s));
+    }
+}
 
 void ensure_ws(H* h, int B) {
     if (B <= h->ws_B) return;
+    chist_clear(h, "the workspace grew after the last chain");
     const dctts_hparams& hp = h->hp;
     const int T = hp.max_T, N = hp.max_N, d = hp.d, F = h->F;
     const size_t rows_ssrn = (size_t)B * T * hp.r;
@@ -198,8 +258,12 @@ void run_chain_full(Launch& lc, const std::vector<LayerDev>& net, const float* X
             if (dead && out) CUDA_CHECK(cudaMemsetAsync(out + o + live, 0, dead * sizeof(float), lc.s));
             if (dead && out_sig) CUDA_CHECK(cudaMemsetAsync(out_sig + o + live, 0, dead * sizeof(float), lc.s));
         }
+        chist_clear(h, "the last chain ran once per utterance (per-utterance lengths on the fp32 kernels): its rows are not "
+                       "kept as one batch");
         return;
     }
+    const int net_id = chain_net(h, net);
+    chist_f32(lc, net_id, 0, X, ldx, B, L, net[0].cin);
     const float* cur = X; int ld = ldx; int len = L;
     float* bufs[2] = {h->act0.as<float>(), h->act1.as<float>()};
     int which = 0;
@@ -216,6 +280,7 @@ void run_chain_full(Launch& lc, const std::vector<LayerDev>& net, const float* X
             run_block(lc, l, l.rate, l.causal, l.act, cur, ld, RowWin{B, len, len, nullptr}, dst, ldo,
                       last ? out_sig : nullptr, l.cout);
         }
+        chist_f32(lc, net_id, (int)i + 1, dst, ldo, B, len, l.cout);
         cur = dst; ld = ldo; which ^= 1;
     }
 }
@@ -327,6 +392,8 @@ void run_chain_tc_planes(Launch& lc, const std::vector<LayerDev>& net, Planes cu
     H* h = lc.h;
     int len = L, len_shift = 0;
     int nxt = (which == 0) ? 1 : 0;
+    const int net_id = chain_net(h, net);
+    chist_planes(lc, net_id, 0, cur, B, L, net[0].cin, in_inv);
     for (size_t i = 0; i < net.size(); ++i) {
         const LayerDev& l = net[i];
         const bool last = (i + 1 == net.size());
@@ -335,6 +402,8 @@ void run_chain_tc_planes(Launch& lc, const std::vector<LayerDev>& net, Planes cu
                      dst, last ? out : nullptr, l.cout, last ? out_sig : nullptr, l.cout, Planes{},
                      i == 0 ? first_extra_shift : 0, i == 0 ? in_inv : nullptr, lengths, len_shift);
         if (l.kind == K_D) { len *= 2; ++len_shift; }
+        if (last) chist_f32(lc, net_id, (int)i + 1, out, l.cout, B, len, l.cout);
+        else chist_planes(lc, net_id, (int)i + 1, dst, B, len, l.cout, nullptr);
         cur = dst; nxt ^= 1;
     }
 }
@@ -611,6 +680,7 @@ void text2mel_generate(H* h, const int* L, int B, int steps, float* Y, int* prev
     IntBufs ib = ints(h);
     Launch lc{h, s};
     run_textenc(lc, L, B, h->kv.as<float>());
+    chist_clear(h, "a decode ran after the last full-sequence chain");
     CUDA_CHECK(cudaMemsetAsync(h->ybuf.p, 0, (size_t)B * T * hp.n_mels * sizeof(float), s));
     CUDA_CHECK(cudaMemsetAsync(h->ibuf.p, 0, (size_t)(4 + 3 * h->ws_B + (size_t)h->ws_B * T) * sizeof(int), s));
     if (pr) CUDA_CHECK(cudaMemcpy2DAsync(ib.p_cur, sizeof(int), pr->path, (size_t)T * sizeof(int), sizeof(int), B,
@@ -677,19 +747,23 @@ bool text2mel_front(Launch& lc, const int* L, const float* mels, const int* pma,
         else
             run_attention(lc, Q, d, K, 2 * d, K + d, 2 * d, RowWin{B, T, T, nullptr}, N, pma, h->rbuf.as<float>(),
                           align, maxatt, nullptr, nullptr, Rpl);
+        chist_f32(lc, CH_ATTENTION, 1, h->rbuf.as<float>(), 2 * d, B, T, 2 * d);
         return true;
     }
     // AudioEnc over all rows, reading mels shifted by one frame (train.py:51)
     const float* cur = mels; int ld = hp.n_mels;
+    chist_f32(lc, CH_AUDIOENC, 0, mels, hp.n_mels, B, T, hp.n_mels);
     for (size_t i = 0; i < h->audioenc.size(); ++i) {
         const LayerDev& l = h->audioenc[i];
         float* dst = h->ae_out[i].as<float>();
         run_block(lc, l, l.rate, l.causal, l.act, cur, ld, RowWin{B, T, T, nullptr}, dst, l.cout, nullptr, 0,
                   i == 0 ? -1 : 0);
+        chist_f32(lc, CH_AUDIOENC, (int)i + 1, dst, l.cout, B, T, l.cout);
         cur = dst; ld = l.cout;
     }
     run_attention(lc, cur, d, K, 2 * d, K + d, 2 * d, RowWin{B, T, T, nullptr}, N, pma, h->rbuf.as<float>(),
                   align, maxatt, nullptr, nullptr);
+    chist_f32(lc, CH_ATTENTION, 1, h->rbuf.as<float>(), 2 * d, B, T, 2 * d);
     return false;
 }
 
@@ -697,6 +771,7 @@ void text2mel_forward(H* h, const int* L, const float* mels, const int* pma, int
                       long long* maxatt, float* align, cudaStream_t s) {
     const dctts_hparams& hp = h->hp;
     const int T = hp.max_T, d = hp.d;
+    chist_begin(h, "dctts_text2mel_forward");
     ensure_ws(h, B);
     h->hist.ok = false;
     Launch lc{h, s};
@@ -706,12 +781,14 @@ void text2mel_forward(H* h, const int* L, const float* mels, const int* pma, int
         return;
     }
     const float* cur = h->rbuf.as<float>(); int ld = 2 * d;
+    chist_f32(lc, CH_AUDIODEC, 0, cur, ld, B, T, ld);
     for (size_t i = 0; i < h->audiodec.size(); ++i) {
         const LayerDev& l = h->audiodec[i];
         const bool last = (i + 1 == h->audiodec.size());
         float* dst = h->ad_out[i].as<float>();
         run_block(lc, l, l.rate, l.causal, l.act, cur, ld, RowWin{B, T, T, nullptr}, dst, l.cout,
                   last ? Y : nullptr, hp.n_mels);
+        chist_f32(lc, CH_AUDIODEC, (int)i + 1, dst, l.cout, B, T, l.cout);
         cur = dst; ld = l.cout;
     }
 }
@@ -719,6 +796,7 @@ void text2mel_forward(H* h, const int* L, const float* mels, const int* pma, int
 // Op-level entry (modules.py signatures): fp32 in, fp32 out, on whichever path is selected.
 void run_block_op(Launch& lc, const LayerDev& l, int rate, bool causal, int act, const float* x, int B, int L, float* out) {
     H* h = lc.h;
+    chist_clear(h, "an op-level block call ran after the last full-sequence chain");
     const int Lout = (l.kind == K_D) ? 2 * L : L;
     if (h->tensor_path == 1 && l.tc.ok) {
         const size_t need = (size_t)B * L * roundup(l.cin, 8) * sizeof(__half);
@@ -764,6 +842,7 @@ int dctts_embed(dctts_handle h, const char* scope, const int32_t* ids, int32_t B
         REQUIRE(h->committed, "parameters not committed");
         auto it = h->dev_vec.find(std::string(scope ? scope : "") + "/lookup_table");
         REQUIRE(it != h->dev_vec.end(), "dctts_embed: unknown scope");
+        chist_clear(h, "an op-level embedding call ran after the last full-sequence chain");
         launch_embed(ids, it->second, out, B * N, h->hp.e, S(h, stream)); h->launches++;
     });
 }
@@ -775,6 +854,7 @@ int dctts_normalize(dctts_handle h, const char* scope, const float* x, int64_t r
         auto b = h->dev_vec.find(std::string(scope ? scope : "") + "/beta");
         REQUIRE(g != h->dev_vec.end() && b != h->dev_vec.end(), "dctts_normalize: unknown scope");
         REQUIRE(C >= 1 && C <= 1056 && rows < (1ll << 31), "dctts_normalize: unsupported width");
+        chist_clear(h, "an op-level LayerNorm call ran after the last full-sequence chain");
         LnArgs n{};
         n.Y = x; n.ldy = C; n.g1 = g->second; n.b1 = b->second; n.out = out; n.ldo = C; n.C = C;
         n.mode = 0; n.act = 0; n.win = RowWin{1, (int)rows, (int)rows, nullptr};
@@ -815,6 +895,7 @@ int dctts_textenc(dctts_handle h, const int32_t* L, int32_t B, float* K, float* 
     return guarded(h, [&] {
         REQUIRE(h->committed, "parameters not committed");
         REQUIRE(B >= 1 && L && K && V, "dctts_textenc: bad arguments");
+        chist_begin(h, "dctts_textenc");
         ensure_ws(h, B);
         h->hist.ok = false;
         cudaStream_t s = S(h, stream);
@@ -831,6 +912,7 @@ int dctts_audioenc(dctts_handle h, const float* Sin, int32_t B, int32_t T, float
     return guarded(h, [&] {
         REQUIRE(h->committed, "parameters not committed");
         REQUIRE(B >= 1 && T >= 1 && T <= h->hp.max_T && Sin && Q, "dctts_audioenc: bad arguments (T must be <= max_T)");
+        chist_begin(h, "dctts_audioenc");
         ensure_ws(h, B);
         Launch lc{h, S(h, stream)};
         run_chain_full(lc, h->audioenc, Sin, h->hp.n_mels, B, T, Q, nullptr);
@@ -843,6 +925,7 @@ int dctts_attention(dctts_handle h, const float* Q, const float* K, const float*
     return guarded(h, [&] {
         REQUIRE(B >= 1 && T >= 1 && N >= 1 && Q && K && V && R, "dctts_attention: bad arguments");
         REQUIRE(!monotonic || pma, "dctts_attention: monotonic attention needs prev_max_attentions");
+        chist_clear(h, "an op-level attention call ran after the last full-sequence chain");
         Launch lc{h, S(h, stream)};
         const int d = h->hp.d;
         if (attention_tc_ok(h))
@@ -858,6 +941,7 @@ int dctts_audiodec(dctts_handle h, const float* R, int32_t B, int32_t T, float* 
     return guarded(h, [&] {
         REQUIRE(h->committed, "parameters not committed");
         REQUIRE(B >= 1 && T >= 1 && T <= h->hp.max_T && R && Y, "dctts_audiodec: bad arguments (T must be <= max_T)");
+        chist_begin(h, "dctts_audiodec");
         ensure_ws(h, B);
         Launch lc{h, S(h, stream)};
         run_chain_full(lc, h->audiodec, R, 2 * h->hp.d, B, T, Y_logits, Y);
@@ -868,6 +952,7 @@ int dctts_ssrn(dctts_handle h, const float* Y, int32_t B, int32_t T, float* Z_lo
     return guarded(h, [&] {
         REQUIRE(h->committed, "parameters not committed");
         REQUIRE(B >= 1 && T >= 1 && T <= h->hp.max_T && Y && Z, "dctts_ssrn: bad arguments (T must be <= max_T)");
+        chist_begin(h, "dctts_ssrn");
         ensure_ws(h, B);
         Launch lc{h, S(h, stream)};
         run_chain_full(lc, h->ssrn, Y, h->hp.n_mels, B, T, Z_logits, Z);
@@ -880,6 +965,7 @@ int dctts_ssrn_ragged(dctts_handle h, const float* Y, int32_t B, int32_t T, cons
         REQUIRE(h->committed, "parameters not committed");
         REQUIRE(B >= 1 && T >= 1 && T <= h->hp.max_T && Y && Z && lengths,
                 "dctts_ssrn_ragged: bad arguments (T must be <= max_T, lengths non-null)");
+        chist_begin(h, "dctts_ssrn_ragged");
         ensure_ws(h, B);
         Launch lc{h, S(h, stream)};
         run_chain_full(lc, h->ssrn, Y, h->hp.n_mels, B, T, Z_logits, Z, lengths);
@@ -1028,6 +1114,7 @@ int dctts_align_search(dctts_handle h, const float* alignments, int32_t B, int32
         REQUIRE(B >= 1 && N >= 1 && T >= 1 && alignments && lengths_host && ends_host && path && chars && durations && score,
                 "dctts_align_search: bad arguments");
         const int max_end = check_align(h, "dctts_align_search", B, N, T, lengths_host, ends_host);
+        chist_clear(h, "an alignment search ran after the last full-sequence chain");
         Launch lc{h, S(h, stream)};
         align_search(lc, alignments, B, N, T, lengths_host, ends_host, max_end, path, chars, durations, score);
     });
@@ -1043,6 +1130,7 @@ int dctts_text2mel_align(dctts_handle h, const int32_t* L, const float* mels, in
         REQUIRE(T >= 1 && T <= h->hp.max_T, "dctts_text2mel_align: T must be in [1, max_T]");
         const int N = h->hp.max_N;
         const int max_end = check_align(h, "dctts_text2mel_align", B, N, T, lengths_host, ends_host);
+        chist_begin(h, "dctts_text2mel_align");
         ensure_ws(h, B);
         h->hist.ok = false;
         Launch lc{h, S(h, stream)};
@@ -1104,6 +1192,7 @@ int dctts_mcd_dtw(dctts_handle h, const float* X, int32_t Tx, const int32_t* nx_
             h->mcd.dct.ensure(D.size() * sizeof(double));
             CUDA_CHECK(cudaMemcpy(h->mcd.dct.p, D.data(), D.size() * sizeof(double), cudaMemcpyHostToDevice));
         }
+        chist_clear(h, "an MCD-DTW call ran after the last full-sequence chain");
         Launch lc{h, S(h, stream)};
         int* st = pinned_staging(h, 2 * meta.size());
         std::memcpy(st, meta.data(), meta_bytes);
@@ -1188,6 +1277,7 @@ int dctts_synthesize_host(dctts_handle h, const int32_t* L_host, int32_t B, floa
         }
         CUDA_CHECK(cudaStreamSynchronize(h->copy_stream));
         CUDA_CHECK(cudaStreamSynchronize(s));
+        chist_clear(h, "the last call (dctts_synthesize_host) ran a decode and SSRN in utterance chunks");
     });
 }
 
@@ -1301,6 +1391,62 @@ int dctts_decode_history(dctts_handle h, int32_t what, int32_t layer, void* out,
         }
         CUDA_CHECK(cudaStreamSynchronize(s));
         if (joined) *joined = plane >= 0 ? 1 : 0;
+    });
+}
+
+namespace {
+
+// The record dctts_chain_history reads, or a refusal naming why there is none.  what: 0 block `layer`'s output, 1 the
+// first block's input (layer 0).
+const H::ChainRec& chist_find(H* h, const char* who, int net, int layer, int what) {
+    static const char* names[5] = {"TextEnc", "AudioEnc", "AudioDec", "SSRN", "the attention"};
+    REQUIRE(net >= 0 && net < 5, std::string(who) + ": `net` must be 0..4");
+    REQUIRE(what == 0 || what == 1, std::string(who) + ": `what` must be 0 (output) or 1 (input)");
+    REQUIRE(what == 0 || layer == 0, std::string(who) + ": only the first block's input is kept");
+    REQUIRE((h->chist.nets >> net) & 1u, std::string(who) + ": no rows of " + names[net] + " from the last call: " + h->chist.why);
+    const auto& v = h->chist.rec[net];
+    const int slot = what == 1 ? 0 : 1 + layer;
+    REQUIRE(layer >= 0 && slot < (int)v.size() && v[(size_t)slot].B > 0,
+            std::string(who) + ": " + names[net] + " kept no " + (what == 1 ? "input" : "output of block " + std::to_string(layer)) +
+            " in the last call");
+    return v[(size_t)slot];
+}
+
+}  // namespace
+
+int dctts_chain_history_shape(dctts_handle h, int32_t net, int32_t layer, int32_t what, int32_t* B, int32_t* L, int32_t* C) {
+    return guarded(h, [&] {
+        const H::ChainRec& r = chist_find(h, "dctts_chain_history_shape", net, layer, what);
+        if (B) *B = r.B;
+        if (L) *L = r.L;
+        if (C) *C = r.C;
+    });
+}
+
+int dctts_chain_history(dctts_handle h, int32_t net, int32_t layer, int32_t what, float* out, int64_t n, int32_t* joined,
+                        void* stream) {
+    return guarded(h, [&] {
+        const H::ChainRec& r = chist_find(h, "dctts_chain_history", net, layer, what);
+        const size_t rows = (size_t)r.B * r.L, elems = rows * r.C;
+        REQUIRE(out && n == (int64_t)elems, "dctts_chain_history: out must hold " + std::to_string(elems) + " floats");
+        cudaStream_t s = S(h, stream);
+        if (!r.planes) {
+            CUDA_CHECK(cudaMemcpyAsync(out, r.a.p, elems * sizeof(float), cudaMemcpyDeviceToDevice, s));
+        } else {                                          // hi + lo (times the utterance's inverse scale) on the host
+            const size_t pe = rows * r.ld;
+            std::vector<__half> hi(pe), lo(pe);
+            std::vector<float> inv((size_t)r.B, 1.f), rows_f(elems);
+            CUDA_CHECK(cudaMemcpyAsync(hi.data(), r.a.p, pe * sizeof(__half), cudaMemcpyDeviceToHost, s));
+            CUDA_CHECK(cudaMemcpyAsync(lo.data(), r.b.p, pe * sizeof(__half), cudaMemcpyDeviceToHost, s));
+            if (r.scaled) CUDA_CHECK(cudaMemcpyAsync(inv.data(), r.inv.p, inv.size() * sizeof(float), cudaMemcpyDeviceToHost, s));
+            CUDA_CHECK(cudaStreamSynchronize(s));
+            for (size_t i = 0; i < rows; ++i)
+                for (int c = 0; c < r.C; ++c)
+                    rows_f[i * r.C + c] = join_f16(hi[i * r.ld + c], lo[i * r.ld + c]) * inv[i / r.L];
+            CUDA_CHECK(cudaMemcpyAsync(out, rows_f.data(), elems * sizeof(float), cudaMemcpyHostToDevice, s));
+        }
+        CUDA_CHECK(cudaStreamSynchronize(s));
+        if (joined) *joined = r.planes ? 1 : 0;
     });
 }
 

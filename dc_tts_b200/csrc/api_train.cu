@@ -517,6 +517,7 @@ size_t device_index(const H::TrainTensor& t, long long i) {
 // packs them again synthesis runs on the fp32 kernel set and the graph-per-frame decode, and dctts_set_tensor_path(1) is
 // refused.  Cheap when the handle is stale already; otherwise it synchronises the device once to drop the captured AR step.
 void dctts::api::mark_synthesis_stale(H* h) {
+    chist_clear(h, "training took over the weights after the last full-sequence chain");
     if (h->synth_stale) return;
     if (h->ar_exec) { CUDA_CHECK(cudaDeviceSynchronize()); drop_ar_graph(h); }
     h->tensor_path = 0;
@@ -588,6 +589,28 @@ int dctts_conv_gemm(dctts_handle h, int32_t impl, int32_t mode, const float* X, 
         h->launches += launches;
         CUDA_CHECK(cudaGetLastError());
         CUDA_CHECK(cudaStreamSynchronize(s));      // before the workspace is freed
+    });
+}
+
+int dctts_block_fwd(dctts_handle h, int32_t mode, int32_t act, int64_t rows, int32_t C, const float* pre, int32_t ldy,
+                    const float* X, int32_t ldx, const float* ln, float dropout_rate, int32_t layer, uint32_t seed, float* out,
+                    int32_t ldo, void* stream) {
+    return guarded(h, [&] {
+        REQUIRE(mode == 0 || mode == 1, "dctts_block_fwd: mode must be 0 (conv1d / transposed conv) or 1 (highway)");
+        REQUIRE(act == 0 || act == 1, "dctts_block_fwd: act must be 0 (none) or 1 (ReLU)");
+        REQUIRE(rows >= 1 && rows < (1ll << 31) && C >= 1 && layer >= 0 && dropout_rate >= 0.f && dropout_rate < 1.f,
+                "dctts_block_fwd: bad arguments");
+        REQUIRE(pre && ln && out && (mode == 0 || X), "dctts_block_fwd: pre, ln, out (and X for a highway block) are required");
+        REQUIRE(ldy >= (mode == 1 ? 2 * C : C) && ldo >= C && (mode == 0 || ldx >= C),
+                "dctts_block_fwd: a pitch is narrower than its tensor's width");
+        // the LayerNorm epilogue of train_fwd: one launch_ln_rows over the rows, the step's dropout mask from drop_args
+        LnArgs n{};
+        n.Y = pre; n.ldy = ldy; n.g1 = ln; n.b1 = ln + C; n.g2 = ln + 2 * C; n.b2 = ln + 3 * C; n.X = X; n.ldx = ldx;
+        n.out = out; n.ldo = ldo; n.C = C; n.mode = mode; n.act = act; n.win = RowWin{1, (int)rows, (int)rows, nullptr};
+        if (dropout_rate > 0.f) n.drop = drop_args(dropout_rate, layer, seed);
+        cudaStream_t s = S(h, stream);
+        launch_ln_rows(n, s); h->launches++;           // refuses a width past the widest LayerNorm kernel before launching
+        CUDA_CHECK(cudaStreamSynchronize(s));
     });
 }
 

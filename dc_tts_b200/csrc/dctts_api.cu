@@ -16,6 +16,7 @@ const Option kOptions[] = {
     {"decode_prof", &H::Options::decode_prof, 2}, {"decode_force_prepass", &H::Options::decode_force_prepass, 2},
     {"train_tc", &H::Options::train_tc, 7},       {"train_probe", &H::Options::train_probe, 2},
     {"train_deterministic", &H::Options::train_deterministic, 1},
+    {"chain_history", &H::Options::chain_history, 1},
 };
 
 const Option* find_option(const char* name) {

@@ -215,6 +215,26 @@ class Engine:
                     "dctts_block_bwd")
         return dy
 
+    def block_fwd(self, mode, act, C, pre, ln, out, X=None, dropout_rate=0.0, layer=0, seed=0):
+        """Test aid (include/dctts.h: dctts_block_fwd): the training forward's LayerNorm / activation / highway / dropout
+        epilogue of one block, one launch, into `out` (rows, >= C).  pre (rows, >= nconv); X (rows, >= C) for mode 1; ln (4, C)
+        = g1 | b1 | g2 | b2 contiguous.  Leading dims are flattened into rows; the pitches are the views' row strides."""
+        nconv = 2 * C if mode == 1 else C
+        if mode == 1 and X is None:
+            raise DcttsError("block_fwd: a highway block (mode 1) needs X")
+        rows = 1
+        for s in pre.shape[:-1]:
+            rows *= s
+        ts = [pre, out] + ([X] if mode == 1 else [])
+        if any(t.shape[-1] < w for t, w in zip(ts, (nconv, C, C))):
+            raise DcttsError("block_fwd: pre needs %d columns, out and X %d" % (nconv, C))
+        lds = self._pitched("block_fwd", ts, rows)
+        _require_tensors("block_fwd", [(ln, (4, C), torch.float32)])
+        self._check(self._lib.dctts_block_fwd(self._h, int(mode), int(act), rows, int(C), _ptr(pre), lds[0], _ptr(X),
+                                              lds[2] if mode == 1 else 0, _ptr(ln), float(dropout_rate), int(layer),
+                                              int(seed) & 0xffffffff, _ptr(out), lds[1], self._stream()), "dctts_block_fwd")
+        return out
+
     def attn_bwd(self, gR, Q, KV, align, gts, n_lim, t_lim, gQ, gKV, sums):
         """Test aid (include/dctts.h: dctts_attn_bwd): the attention backward of the Text2Mel step.  gR (B, T, 2d), Q (B, T, d),
         KV (B, N, 2d), align (B, N, T), gQ (B, T, d), gKV (B, N, 2d) contiguous; gts (>= n_lim, ld_gts) with a unit inner
@@ -599,6 +619,25 @@ class Engine:
         res = torch.empty_like(out)
         res[torch.as_tensor(order, device=self.device)] = out
         return res, bool(joined.value)
+
+    _CHAIN_NETS = {"textenc": 0, "audioenc": 1, "audiodec": 2, "ssrn": 3, "attention": 4}
+
+    def chain_history(self, net, layer=0, what="output"):
+        """Test aid (include/dctts.h: dctts_chain_history; needs set_option("chain_history", 1) before the call it reads):
+        the rows the last call's full-sequence chain of `net` ("textenc", "audioenc", "audiodec", "ssrn", or "attention",
+        whose output is R) left.  what: "output" (block `layer`'s) or "input" (the first block's, as its kernel read it).
+        Returns (tensor (B, L, C) float32 in the caller's order, joined): joined is True when the rows are hi + lo of the
+        split-fp16 planes the chain kept.  Raises DcttsError, naming the reason, when the last call did not keep them."""
+        if net not in self._CHAIN_NETS or what not in ("output", "input"):
+            raise DcttsError("chain_history: net must be one of %s and what 'output' or 'input'" % sorted(self._CHAIN_NETS))
+        args = (self._h, self._CHAIN_NETS[net], int(layer), int(what == "input"))
+        B, L, Cc = C.c_int32(0), C.c_int32(0), C.c_int32(0)
+        self._check(self._lib.dctts_chain_history_shape(*args, C.byref(B), C.byref(L), C.byref(Cc)), "dctts_chain_history")
+        out = self._empty(B.value, L.value, Cc.value)
+        joined = C.c_int32(0)
+        self._check(self._lib.dctts_chain_history(*args, _ptr(out), out.numel(), C.byref(joined), self._stream()),
+                    "dctts_chain_history")
+        return out, bool(joined.value)
 
     def _set_vocoder_params(self, hop=None, win=None, power=None):
         """The hyperparameters' vocoder constants on the handle, with `hop`, `win` and `power` instead when given."""

@@ -409,6 +409,7 @@ int dctts_set_tensor_path(dctts_handle h, int32_t mode);
  *   "train_tc" 0..7: training GEMMs on wgmma, bit mask 1 forward conv (+ wgmma attention), 2 data gradient, 4 weight gradient
  *   "train_deterministic" 0/1 (default 0): the training step's sums in a fixed order, so that a seeded run repeats bit for
  *                  bit (see dctts_train_step_shaped); it may change between steps and does not affect synthesis
+ *   "chain_history" 0/1 (default 0): test aid, the full-sequence chains keep every block's rows for dctts_chain_history
  * dctts_get_option also answers "decode_available" (1 when this handle / device can run the persistent decode),
  * "decode_max_clusters" (16-CTA clusters of the decode kernel that are co-resident on this device) and, once the
  * parameters are committed, "ssrn_tc_available" (1 when every SSRN block has a wgmma kernel, the F-wide ones included:
@@ -446,6 +447,25 @@ int dctts_decode_profile(dctts_handle h, int64_t* cycles, int32_t n);
  * (a generation with the final attention pass, dctts_text2mel_forward, dctts_textenc, a workspace growth), or on a bad
  * `what`, `layer` or n.  Launches no kernel; synchronises `stream`. */
 int dctts_decode_history(dctts_handle h, int32_t what, int32_t layer, void* out, int64_t n, int32_t* joined, void* stream);
+/* Test aid (option chain_history = 1, default 0): the rows the last call's full-sequence chains left, copied into caller
+ * DEVICE memory as float32, B * L rows of C, in the caller's order of the utterances.  net: 0 TextEnc, 1 AudioEnc, 2 AudioDec,
+ * 3 SSRN, 4 the attention.  what 0: block `layer`'s output (the attention's layer 0 is R = [context | Q]); what 1 (layer 0):
+ * the first block's input as its kernel read it.  Kept by dctts_textenc, _audioenc, _audiodec, _ssrn, _ssrn_ragged on the
+ * tensor path, _text2mel_forward (TextEnc, AudioEnc, the attention, AudioDec) and _text2mel_align (the first three).
+ * On the tensor path the hidden blocks' outputs and the first block's input are split-fp16 planes: the rows are then hi + lo,
+ * times the utterance's inverse input scale for a scaled network input (exact: the scale is a power of two), and *joined
+ * (optional) is set to 1, else 0.  dctts_chain_history_shape gives (B, L, C) of a record.
+ * Fails with a message naming the reason, copying nothing, when the last call that ran synthesis kernels or changed the
+ * weights did not run a full-sequence chain of `net` with the option on: a decode, an op-level block, embedding, LayerNorm
+ * or attention call, the alignment search, MCD-DTW, a workspace growth, another network's chain, the option off,
+ * dctts_synthesize_host, per-utterance lengths on the fp32 kernels (run once per utterance, not kept), a parameter commit,
+ * a training update or dctts_train_set_tensor, dctts_refresh_synthesis; or when the caller did not ask for the rows (the
+ * logits).  Calls that touch neither (the training forward and loss without an update, the training test aids, the
+ * vocoder and feature extraction) leave the records readable.  Launches no kernel; synchronises `stream`.  With the option
+ * off the chains copy nothing and launch the same kernels. */
+int dctts_chain_history_shape(dctts_handle h, int32_t net, int32_t layer, int32_t what, int32_t* B, int32_t* L, int32_t* C);
+int dctts_chain_history(dctts_handle h, int32_t net, int32_t layer, int32_t what, float* out, int64_t n, int32_t* joined,
+                        void* stream);
 /* Measurement aid for bench.py's roofline leg: runs the block `scope` on a synthetic
  * (B,L,Cin) input `warmup`+`iters` times and returns the mean device time of each of its
  * kernels (CUDA events on `stream` around every launch), ms_per_kernel[0..*n_kernels), <= 8. */
@@ -480,6 +500,15 @@ int dctts_conv_gemm(dctts_handle h, int32_t impl, int32_t mode, const float* X, 
 int dctts_block_bwd(dctts_handle h, int32_t mode, int32_t act, int64_t rows, int32_t C, const float* pre, int32_t ldy,
                     const float* gout, int32_t ldg, const float* X, int32_t ldx, const float* ln, float dropout_rate, int32_t layer,
                     uint32_t seed, float* dy, float* gin, float* dparams, void* stream);
+/* Test aid: the forward twin of dctts_block_bwd, the LayerNorm epilogue of the training forward on caller DEVICE tensors,
+ * through the launch the step makes (launch_ln_rows with the step's dropout mask):
+ *   mode 0: out = dropout(act(LN(pre[:, 0:C]; g1, b1)));  mode 1: out = dropout(h1 h2 + (1 - h1) x), as dctts_block_bwd.
+ * pre (rows, ldy), X (rows, ldx, mode 1), ln (4, C), the mask of (row C + c, layer, seed) as dctts_block_bwd's; out (rows,
+ * ldo >= C), pad columns untouched.  Fails with a message, launching nothing, on a bad mode, act, rate or pitch, or a width
+ * past the widest LayerNorm kernel (2080).  Synchronises `stream`. */
+int dctts_block_fwd(dctts_handle h, int32_t mode, int32_t act, int64_t rows, int32_t C, const float* pre, int32_t ldy,
+                    const float* X, int32_t ldx, const float* ln, float dropout_rate, int32_t layer, uint32_t seed, float* out,
+                    int32_t ldo, void* stream);
 /* Test aid: the attention backward of the Text2Mel training step (three launches: guided-attention sum, query side, key side)
  * on caller DEVICE tensors, through the launch function the step calls, with the handle's d (the kernels need d = 256).
  * gR (B,T,2d) the gradient of R = [ctx ; Q]; Q (B,T,d); KV (B,N,2d) = [K | V]; align (B,N,T) the forward's softmax over

@@ -83,30 +83,41 @@ def sigmoid(x):
     return 1.0 / (1.0 + np.exp(-x))
 
 
-def conv_block(p, layer, x, rows, xs=None):
-    """conv1d + LayerNorm (+ ReLU) of block `layer` on the rows `rows` (modules.py:91-141).  Returns (out, S)."""
-    y, Sy = causal_conv(x, p["W"], p["b"], layer.rate, rows, xs)
+def conv_epilogue(p, layer, y, Sy):
+    """LayerNorm (+ ReLU) of conv rows y with error scale Sy (modules.py:91-141).  Returns (out, S)."""
     z, S, _ = layer_norm(y, Sy, p["g1"], p["b1"])
     if layer.act == "relu":
         z = np.maximum(z, 0.0)
     return z, S
 
 
-def hc_block(p, layer, x, rows, xs=None):
-    """Highway conv of block `layer` on the rows `rows` (modules.py:143-197): h1 = sigmoid(LN(y_gate)), h2 = LN(y_info),
-    out = h1 h2 + (1 - h1) x.  The gate's error passes through h1 (1 - h1), and the float32 gate (expf or __expf, 2 + 1.2 |z|
-    ulp) adds (3 + |z1|) h1 (1 - h1) of rounding.  Returns (out, S)."""
-    y, Sy = causal_conv(x, p["W"], p["b"], layer.rate, rows, xs)
+def hc_epilogue(p, y, Sy, xr, xsr=0.0):
+    """The highway mix of conv rows y (2C wide) with error scale Sy and the residual rows xr (error scale xsr)
+    (modules.py:143-197): h1 = sigmoid(LN(y_gate)), h2 = LN(y_info), out = h1 h2 + (1 - h1) x.  The gate's error passes
+    through h1 (1 - h1), and the float32 gate (expf or __expf, 2 + 1.2 |z| ulp) adds (3 + |z1|) h1 (1 - h1) of rounding.
+    Returns (out, S)."""
     C = y.shape[1] // 2
     z1, S1, _ = layer_norm(y[:, :C], Sy[:, :C], p["g1"], p["b1"])
     z2, S2, _ = layer_norm(y[:, C:], Sy[:, C:], p["g2"], p["b2"])
     h1 = sigmoid(z1)
-    xr = _f(x)[np.asarray(rows)]
-    xsr = 0.0 if xs is None else _f(xs)[np.asarray(rows)]
     dg = h1 * (1 - h1)
     out = h1 * z2 + (1 - h1) * xr
     S = dg * (S1 + 3 + np.abs(z1)) * (np.abs(z2) + np.abs(xr)) + h1 * (S2 + np.abs(z2)) + (1 + h1) * np.abs(xr) + (1 - h1) * xsr
     return out, S
+
+
+def conv_block(p, layer, x, rows, xs=None):
+    """conv1d + LayerNorm (+ ReLU) of block `layer` on the rows `rows` (modules.py:91-141).  Returns (out, S)."""
+    y, Sy = causal_conv(x, p["W"], p["b"], layer.rate, rows, xs)
+    return conv_epilogue(p, layer, y, Sy)
+
+
+def hc_block(p, layer, x, rows, xs=None):
+    """Highway conv of block `layer` on the rows `rows` (modules.py:143-197, hc_epilogue).  Returns (out, S)."""
+    y, Sy = causal_conv(x, p["W"], p["b"], layer.rate, rows, xs)
+    xr = _f(x)[np.asarray(rows)]
+    xsr = 0.0 if xs is None else _f(xs)[np.asarray(rows)]
+    return hc_epilogue(p, y, Sy, xr, xsr)
 
 
 def block(p, layer, x, rows, xs=None):
@@ -127,13 +138,14 @@ def window_keys(p, N, win):
 
 def attention_rows(Q, KV, windows, win):
     """One query row per window: R = [sum_n a_n V_n | Q] over the window's live keys, a = softmax(Q K^T / sqrt(d)).  Q (n, d)
-    float32 rows as read, KV (N, 2d), windows (n,) ints.  Returns dict(R (n, 2d), S (n, 2d), argmax (n,) the first index among
-    equal maxima, margin (n,) top-1 minus top-2 probability (inf with one live key), Sp (n,) the error scale of the
+    float32 rows as read, KV (N, 2d), windows (n,) ints.  Returns dict(R (n, 2d), S (n, 2d), A (n, N) the probabilities (0
+    outside the window) and SA (n, N) their error scale, argmax (n,) the first index among equal maxima, margin (n,) top-1 minus top-2 probability (inf with one live key), Sp (n,) the error scale of the
     probabilities of the two leading keys, summed)."""
     Q, KV = _f(Q), _f(KV)
     n, d = Q.shape
     N = KV.shape[0]
     R, S = np.zeros((n, 2 * d)), np.zeros((n, 2 * d))
+    A, SA = np.zeros((n, N)), np.zeros((n, N))
     amax, margin, Sp = np.zeros(n, np.int64), np.full(n, np.inf), np.zeros(n)
     for i in range(n):
         lo, hi = window_keys(windows[i], N, win)
@@ -143,6 +155,7 @@ def attention_rows(Q, KV, windows, win):
         e = np.exp(s - s.max())
         a = e / e.sum()
         sa = a * (ss + (a * ss).sum() + 1)                   # scores' rounding through the softmax, and its own
+        A[i, lo:hi], SA[i, lo:hi] = a, sa
         R[i, :d] = a @ V
         R[i, d:] = Q[i]
         S[i, :d] = (a + sa) @ np.abs(V)
@@ -152,7 +165,7 @@ def attention_rows(Q, KV, windows, win):
             top = np.argsort(-a, kind="stable")[:2]
             margin[i] = a[top[0]] - a[top[1]]
             Sp[i] = sa[top[0]] + sa[top[1]]
-    return dict(R=R, S=S, argmax=amax, margin=margin, Sp=Sp)
+    return dict(R=R, S=S, A=A, SA=SA, argmax=amax, margin=margin, Sp=Sp)
 
 
 def mel_sigmoid(logits):
@@ -163,16 +176,20 @@ def mel_sigmoid(logits):
     return y, y * (3 + (1 - y) * (3 + np.abs(x)))
 
 
-def float32_block(p, layer, x, rows):
-    """The same block restated in float32 (numpy, the kernels' operation order aside): the bound tests' stand-in for a kernel."""
+def float32_block(p, layer, x, rows, shifts=None):
+    """The same block restated in float32 (numpy, the kernels' operation order aside): the bound tests' stand-in for a kernel.
+    shifts: tap j reads x[t + shifts[j]], zero outside x's rows; default the causal taps -(k - 1 - j) rate."""
     f = np.float32
     x = np.asarray(x, f)
     rows = np.asarray(rows)
     k = p["W"].shape[0]
+    if shifts is None:
+        shifts = [-(k - 1 - j) * layer.rate for j in range(k)]
     y = np.zeros((len(rows), p["W"].shape[2]), f) + p["b"].astype(f)
     for j in range(k):
-        t = rows - (k - 1 - j) * layer.rate
-        y += np.where((t >= 0)[:, None], x[np.clip(t, 0, None)], f(0)) @ p["W"][j].astype(f)
+        t = rows + shifts[j]
+        ok = (t >= 0) & (t < len(x))
+        y += np.where(ok[:, None], x[np.clip(t, 0, len(x) - 1)], f(0)) @ p["W"][j].astype(f)
 
     def ln(v, g, b):
         m = v.mean(1, keepdims=True, dtype=f)

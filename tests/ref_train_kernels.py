@@ -132,6 +132,35 @@ def block_forward(mode, act, pre, ln, keep, X=None):
     return out * keep
 
 
+def block_forward_scale(mode, act, pre, ln, keep, X=None):
+    """block_forward in float64 with its error scale S, built like block_bwd's: the same computation on absolute values, the
+    LayerNorm terms carrying (1 + kappa) per row, and kappa absolute (the float32 mean is off by 2^-24 (|mean| + spread),
+    which moves yhat by 2^-24 kappa however small yhat is: a near-constant row's middle values); the highway gate's error passes through h1 (1 - h1) with the float32
+    sigmoid's own (3 + |z1|) ulp, as the synthesis blocks' (tests/ref_decode_blocks.py hc_epilogue).  The dropout multiplier
+    scales both (a dropped element is exactly 0).  Returns (out, S), (rows, C) float64."""
+    f = lambda t: t.double()                                  # noqa: E731
+    C = ln.shape[1]
+    g1, b1, g2, b2 = (f(ln[i]) for i in range(4))
+    y1 = f(pre[:, :C])
+    yh1, r1, m1 = ln_forward(y1)
+    z1 = yh1 * g1 + b1
+    k1 = ln_sensitivity(y1, yh1, m1, r1)
+    s1 = ((1 + k1) * yh1.abs() + k1) * g1.abs() + b1.abs()
+    if mode == 0:
+        out, S = (torch.relu(z1) if act == 1 else z1), s1
+    else:
+        y2 = f(pre[:, C:2 * C])
+        yh2, r2, m2 = ln_forward(y2)
+        z2 = yh2 * g2 + b2
+        k2 = ln_sensitivity(y2, yh2, m2, r2)
+        s2 = ((1 + k2) * yh2.abs() + k2) * g2.abs() + b2.abs()
+        x = f(X)
+        h1 = torch.sigmoid(z1)
+        out = h1 * z2 + (1 - h1) * x
+        S = h1 * (1 - h1) * (s1 + 3 + z1.abs()) * (z2.abs() + x.abs()) + h1 * (s2 + z2.abs()) + (1 + h1) * x.abs()
+    return out * keep, S * keep.abs()
+
+
 # --------------------------------------------------------------------------------------------- attention backward
 def attn_bwd(gR, Q, KV, align, gts, n_lim, t_lim):
     """The softmax attention backward of the step with the guided-attention term, from the GIVEN alignments (not a

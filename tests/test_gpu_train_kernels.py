@@ -28,8 +28,9 @@ import ref_train_kernels as rk
 from sample_rates import at_rate
 
 # worst err / S over this file on an H100 80GB HBM3 at 700 W (DESIGN.md 8e): block backward per-row outputs 2.4e-7, its
-# column reductions 1.55e-5 (float atomics over up to 840 CTAs), attention 1.75e-6, losses 1.9e-7, Adam 3.3e-7
-TAU = {"block": 1e-6, "block_sum": 6e-5, "attn": 6e-6, "loss": 8e-7, "adam": 1e-6}
+# column reductions 1.55e-5 (float atomics over up to 840 CTAs), attention 1.75e-6, losses 1.9e-7, Adam 3.3e-7; the block
+# forward (dctts_block_fwd) 1.75e-7
+TAU = {"block": 1e-6, "block_sum": 6e-5, "attn": 6e-6, "loss": 8e-7, "adam": 1e-6, "block_fwd": 6e-7}
 SENTINEL = -1234.5
 _WORST = collections.defaultdict(lambda: [0.0, 0.0])            # kernel -> [max err / S, max err / tolerance]
 
@@ -276,6 +277,71 @@ def test_block_bwd_vs_float64(eng, case):
         for rows in (1, 31, 32, 33):
             run_block(eng, case, rows, rate, seed=rows + int(rate * 100))
     run_block(eng, case, 32 * 840, 0.05, seed=11)
+
+
+# The forward twin: train_fwd's LayerNorm epilogue with the dropout mask (dctts_block_fwd, one launch_ln_rows).  Every MAXV
+# instantiation of ln_rows_kernel (C = 80 and 256: 8, 512: 16, 1024: 32, 1025: 33, 2049: 65), both modes, ReLU on and off.
+# Rows 1 and 255 run 2 warps per CTA and 2051 runs 8; without dropout, C <= 256 and at most 1024 rows take ln_row_cta_kernel.
+FWD = [Block(m, C, a, "forward") for C in (80, 256, 512, 1024, 1025, 2049) for m, a in ((0, 0), (0, 1), (1, 0))]
+
+
+def _block_fwd_restated(c, pre, ln, keep, X):
+    """block_forward restated in float32 (torch, the kernel's operation order aside)."""
+    C = c.C
+    v = pre[:, :C].float()
+    m = v.mean(1, keepdim=True)
+    z1 = (v - m) / torch.sqrt(((v - m) ** 2).mean(1, keepdim=True) + rk.LN_EPS) * ln[0] + ln[1]
+    if c.mode == 0:
+        out = torch.relu(z1) if c.act else z1
+    else:
+        w = pre[:, C:2 * C].float()
+        m2 = w.mean(1, keepdim=True)
+        z2 = (w - m2) / torch.sqrt(((w - m2) ** 2).mean(1, keepdim=True) + rk.LN_EPS) * ln[2] + ln[3]
+        h1 = torch.sigmoid(z1)
+        out = h1 * z2 + (1 - h1) * X
+    return out * keep.float()
+
+
+@pytest.mark.parametrize("mode,act", [(0, 0), (0, 1), (1, 0)])
+def test_block_forward_scale(mode, act):
+    """CPU: block_forward_scale's value is block_forward's, and a float32 restatement stays below TAU / 4 of its S."""
+    c = Block(mode, 512, act, "cpu")
+    gen = torch.Generator().manual_seed(mode * 2 + act)
+    pre, ln, _, X = _block_inputs(c, 64, gen, "cpu")
+    keep = rk.drop_multiplier(64, c.C, 5, 9, 0.05)
+    ref, S = rk.block_forward_scale(mode, act, pre, ln, keep, X)
+    want = rk.block_forward(mode, act, pre.double(), ln.double(), keep, X.double())
+    assert float((ref - want).abs().max()) < 1e-12
+    got = _block_fwd_restated(c, pre, ln, keep, X).double()
+    r = (got - ref).abs() / S
+    assert bool(((S > 0) | (got == ref)).all())
+    assert float(torch.where(S > 0, r, torch.zeros_like(r)).max()) < TAU["block_fwd"] / 4
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case", FWD, ids=_block_id)
+def test_block_fwd_vs_float64(eng, case):
+    """Dropout 0, 0.05 and 0.5 at 1, 255 and 2051 rows; pad columns of out untouched."""
+    dev = eng.device
+    C, nconv = case.C, (2 * case.C if case.mode else case.C)
+    for rate in (0.0, 0.05, 0.5):
+        for rows in (1, 255, 2051):
+            seed = rows + int(rate * 100)
+            gen = torch.Generator(device=dev)
+            gen.manual_seed(seed)
+            pre, ln, _, X = _block_inputs(case, rows, gen, dev)
+            layer = 3 + seed % 40
+            keep = rk.drop_multiplier(rows, C, layer, seed, rate, dev)
+            nan = float("nan")
+            pbuf = torch.full((rows, _r4(nconv) + 4), nan, device=dev); pbuf[:, :nconv] = pre
+            xbuf = torch.full((rows, _r4(C) + 8), nan, device=dev); xbuf[:, :C] = X
+            out = torch.full((rows, _r4(C) + 4), SENTINEL, device=dev)
+            eng.block_fwd(case.mode, case.act, C, pbuf[:, :nconv], ln, out[:, :C], X=xbuf[:, :C] if case.mode else None,
+                          dropout_rate=rate, layer=layer, seed=seed)
+            ref, S = rk.block_forward_scale(case.mode, case.act, pre, ln, keep, X)
+            where = "%s rows %d rate %g" % (_block_id(case), rows, rate)
+            assert bool((out[:, C:] == SENTINEL).all()), "a pad column of out was written: " + where
+            check("block_fwd", out[:, :C], ref, S, "out " + where)
 
 
 @pytest.mark.gpu
