@@ -86,6 +86,8 @@ SIGNATURES = {
     "dctts_train_set_tensor": (C.c_int, [Handle, C.c_char_p, _i32, _p, _i64]),
     "dctts_refresh_synthesis": (C.c_int, [Handle, _p]),
     "dctts_reserve": (C.c_int, [Handle, _i32]),
+    "dctts_reserve_frames": (C.c_int, [Handle, _i32, _i32, C.POINTER(_i64)]),
+    "dctts_join_rows": (C.c_int, [Handle, _p, _i32, _i32, _p, _p, _p, _i32, C.c_float, _i32, _p, _p, _p]),
     "dctts_launch_count": (_i64, [Handle]),
     "dctts_crc32c": (C.c_uint32, [C.c_uint32, _p, _i64]),
     "dctts_set_tensor_path": (C.c_int, [Handle, _i32]),

@@ -10,7 +10,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libdctts_b200.so")
-SOURCES = ["dctts_api.cu", "api_params.cu", "api_synth.cu", "api_train.cu", "api_audio.cu", "kernels_simt.cu", "kernels_tc.cu", "kernels_attn_tc.cu", "kernels_vocoder.cu", "kernels_train.cu", "kernels_ordered.cu", "kernels_decode.cu", "kernels_gemm_tc.cu", "kernels_pack.cu", "kernels_align.cu", "kernels_mcd.cu"]
+SOURCES = ["dctts_api.cu", "api_params.cu", "api_synth.cu", "api_train.cu", "api_audio.cu", "kernels_simt.cu", "kernels_tc.cu", "kernels_attn_tc.cu", "kernels_vocoder.cu", "kernels_train.cu", "kernels_ordered.cu", "kernels_decode.cu", "kernels_gemm_tc.cu", "kernels_pack.cu", "kernels_align.cu", "kernels_mcd.cu", "kernels_longform.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--use_fast_math" if False else "-DDCTTS_NO_FAST_MATH",     # accuracy first: no fast-math

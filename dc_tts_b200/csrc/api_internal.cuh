@@ -139,6 +139,7 @@ struct dctts_handle_s {
     // MCD-DTW (dctts_mcd_dtw): back-pointers (sum nx_b ny_b bytes), per-pair lengths and offsets (4B int64), the cepstra
     // of pairs too long for shared memory, and rows 1 .. n_mels - 1 of the DCT-II matrix (uploaded at the first call)
     struct { DevBuf bp, meta, cep, dct; } mcd;
+    DevBuf join_meta;             // dctts_join_rows: each piece's text and pause (2P ints), then each text's first piece (K + 1)
     DevBuf lbuf;                  // (B, N) ids staging for the host entry point
     DevBuf zbuf;                  // (B, 4T, F) staging for the host entry point
     DevBuf plane[4];              // tensor-core path activations: {hi,lo} x ping-pong, rows x 1032 fp16

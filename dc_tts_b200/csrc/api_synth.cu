@@ -114,11 +114,20 @@ void chist_planes(Launch& lc, int net, int slot, Planes p, int B, int L, int C, 
     }
 }
 
+// Row pitches of the full-sequence chains' buffers: the pre-LN scratch and the fp32 ping-pong pair (floats), the split
+// planes (halfs)
+struct ChainLd { size_t scr, act, pl; };
+ChainLd chain_ld(H* h) {
+    const dctts_hparams& hp = h->hp;
+    const int w = std::max(std::max(2 * hp.c, h->F), 2 * hp.d);
+    return ChainLd{(size_t)roundup(std::max(std::max(4 * hp.c, h->F), 4 * hp.d), 4), (size_t)roundup(w, 4), (size_t)roundup(w, 8)};
+}
+
 void ensure_ws(H* h, int B) {
     if (B <= h->ws_B) return;
     chist_clear(h, "the workspace grew after the last chain");
     const dctts_hparams& hp = h->hp;
-    const int T = hp.max_T, N = hp.max_N, d = hp.d, F = h->F;
+    const int T = hp.max_T, N = hp.max_N, d = hp.d;
     const size_t rows_ssrn = (size_t)B * T * hp.r;
     // invalidate anything that baked pointers
     if (h->ar_exec) CUDA_CHECK(cudaStreamSynchronize(h->stream));
@@ -126,11 +135,10 @@ void ensure_ws(H* h, int B) {
     CUDA_CHECK(cudaDeviceSynchronize());
     settle_decode_counts(h);                              // the counter buffers below may move
     h->hist.ok = false;                                   // and so do the buffers dctts_decode_history reads
-    const size_t ld_scr = (size_t)roundup(std::max(std::max(4 * hp.c, F), 4 * d), 4);
-    h->scratch.ensure(std::max(rows_ssrn * ld_scr * sizeof(float), (size_t)64 << 20));
-    const size_t ld_act = (size_t)roundup(std::max(std::max(2 * hp.c, F), 2 * d), 4);
-    h->act0.ensure(rows_ssrn * ld_act * sizeof(float));
-    h->act1.ensure(rows_ssrn * ld_act * sizeof(float));
+    const ChainLd ld = chain_ld(h);
+    h->scratch.ensure(std::max(rows_ssrn * ld.scr * sizeof(float), (size_t)64 << 20));
+    h->act0.ensure(rows_ssrn * ld.act * sizeof(float));
+    h->act1.ensure(rows_ssrn * ld.act * sizeof(float));
     h->kv.ensure((size_t)B * N * 2 * d * sizeof(float));
     h->ybuf.ensure((size_t)B * T * hp.n_mels * sizeof(float));
     h->rbuf.ensure((size_t)B * T * 2 * d * sizeof(float));
@@ -144,7 +152,7 @@ void ensure_ws(H* h, int B) {
     h->ibuf.ensure((size_t)(4 + 3 * B + (size_t)B * T) * sizeof(int));
     h->pathbuf.ensure((size_t)(B + 2 * (size_t)B * T) * sizeof(int));
     h->lbuf.ensure((size_t)B * N * sizeof(int));
-    for (auto& pb : h->plane) pb.ensure(rows_ssrn * (size_t)roundup(std::max(std::max(2 * hp.c, F), 2 * d), 8) * sizeof(__half));
+    for (auto& pb : h->plane) pb.ensure(rows_ssrn * ld.pl * sizeof(__half));
     h->in_inv.ensure((size_t)B * sizeof(float));
     for (int i = 0; i < 10; ++i) {
         const size_t bytes = (size_t)B * T * (i < 2 ? 2 * d : d) * sizeof(__half);
@@ -158,6 +166,55 @@ void ensure_ws(H* h, int B) {
     h->dec.pfinal.ensure((size_t)B * sizeof(int));
     h->dec.frames.ensure((size_t)B * sizeof(int));
     h->ws_B = B;
+}
+
+// The buffers a full-sequence chain runs in (pre-LN scratch, the fp32 ping-pong pair, the split-plane pairs) hold r x rows
+// of the chain's input, ws_B x max_T as ensure_ws sizes them; SSRN past max_T (long-form synthesis) needs B x T.  Their
+// bytes per mel frame of a batch (98688 at the LJ hyperparameters), and what they hold now.
+size_t chain_bytes_per_frame(H* h) {
+    const ChainLd ld = chain_ld(h);
+    return (size_t)h->hp.r * ((ld.scr + 2 * ld.act) * sizeof(float) + 4 * ld.pl * sizeof(__half));
+}
+
+size_t chain_ws_bytes(H* h) {
+    size_t n = h->scratch.bytes + h->act0.bytes + h->act1.bytes;
+    for (auto& pb : h->plane) n += pb.bytes;
+    return n;
+}
+
+// Grow those buffers in place to B x T frames, as ensure_ws does for a batch: only ever up, the weights and every other
+// buffer kept.  The new buffers are allocated before the old ones are freed, so a size that cannot be allocated fails
+// the call with the size in its message and leaves the workspace as it was.
+void ensure_chain_frames(H* h, int B, int T, const char* who) {
+    const dctts_hparams& hp = h->hp;
+    const long long rows = (long long)B * T * hp.r;
+    REQUIRE(rows < (1ll << 31), std::string(who) + ": B x T = " + std::to_string((long long)B * T) + " frames is " +
+                                    std::to_string(rows) + " SSRN rows, more than 2^31 - 1");
+    ensure_ws(h, B);
+    const ChainLd ld = chain_ld(h);
+    const size_t scr = std::max((size_t)rows * ld.scr * sizeof(float), (size_t)64 << 20);
+    const size_t act = (size_t)rows * ld.act * sizeof(float), pl = (size_t)rows * ld.pl * sizeof(__half);
+    bool grow = h->scratch.bytes < scr || h->act0.bytes < act || h->act1.bytes < act;
+    for (auto& pb : h->plane) grow = grow || pb.bytes < pl;
+    if (!grow) return;
+    const size_t want = std::max(scr, h->scratch.bytes) + 2 * std::max(act, h->act0.bytes) + 4 * std::max(pl, h->plane[0].bytes);
+    CUDA_CHECK(cudaDeviceSynchronize());
+    DevBuf n_scr, n_act[2], n_pl[4];
+    try {
+        n_scr.ensure(std::max(scr, h->scratch.bytes));
+        for (auto& b : n_act) b.ensure(std::max(act, h->act0.bytes));
+        for (int i = 0; i < 4; ++i) n_pl[i].ensure(std::max(pl, h->plane[i].bytes));
+    } catch (const std::exception& e) {
+        cudaGetLastError();
+        throw std::runtime_error(std::string(who) + ": " + std::to_string(B) + " utterances of " + std::to_string(T) +
+                                 " frames need a synthesis workspace of " + std::to_string(want) + " bytes (" +
+                                 std::to_string(chain_bytes_per_frame(h)) + " bytes per frame), which cannot be allocated: " +
+                                 e.what());
+    }
+    chist_clear(h, "the workspace grew after the last chain");
+    drop_ar_graph(h);                                     // the captured AR step has the old pointers baked in
+    std::swap(h->scratch, n_scr); std::swap(h->act0, n_act[0]); std::swap(h->act1, n_act[1]);
+    for (int i = 0; i < 4; ++i) std::swap(h->plane[i], n_pl[i]);
 }
 
 void ensure_scratch(H* h, size_t bytes);
@@ -951,9 +1008,9 @@ int dctts_audiodec(dctts_handle h, const float* R, int32_t B, int32_t T, float* 
 int dctts_ssrn(dctts_handle h, const float* Y, int32_t B, int32_t T, float* Z_logits, float* Z, void* stream) {
     return guarded(h, [&] {
         REQUIRE(h->committed, "parameters not committed");
-        REQUIRE(B >= 1 && T >= 1 && T <= h->hp.max_T && Y && Z, "dctts_ssrn: bad arguments (T must be <= max_T)");
+        REQUIRE(B >= 1 && T >= 1 && Y && Z, "dctts_ssrn: bad arguments");
+        ensure_chain_frames(h, B, T, "dctts_ssrn");
         chist_begin(h, "dctts_ssrn");
-        ensure_ws(h, B);
         Launch lc{h, S(h, stream)};
         run_chain_full(lc, h->ssrn, Y, h->hp.n_mels, B, T, Z_logits, Z);
     });
@@ -963,10 +1020,9 @@ int dctts_ssrn_ragged(dctts_handle h, const float* Y, int32_t B, int32_t T, cons
                       void* stream) {
     return guarded(h, [&] {
         REQUIRE(h->committed, "parameters not committed");
-        REQUIRE(B >= 1 && T >= 1 && T <= h->hp.max_T && Y && Z && lengths,
-                "dctts_ssrn_ragged: bad arguments (T must be <= max_T, lengths non-null)");
+        REQUIRE(B >= 1 && T >= 1 && Y && Z && lengths, "dctts_ssrn_ragged: bad arguments (lengths non-null)");
+        ensure_chain_frames(h, B, T, "dctts_ssrn_ragged");
         chist_begin(h, "dctts_ssrn_ragged");
-        ensure_ws(h, B);
         Launch lc{h, S(h, stream)};
         run_chain_full(lc, h->ssrn, Y, h->hp.n_mels, B, T, Z_logits, Z, lengths);
     });
@@ -1327,6 +1383,66 @@ int dctts_bench_block(dctts_handle h, const char* scope, int32_t B, int32_t L, i
 
 int dctts_reserve(dctts_handle h, int32_t max_batch) {
     return guarded(h, [&] { REQUIRE(max_batch >= 1, "dctts_reserve: bad batch"); ensure_ws(h, max_batch); });
+}
+
+int dctts_reserve_frames(dctts_handle h, int32_t B, int32_t T, int64_t* bytes) {
+    return guarded(h, [&] {
+        REQUIRE(B >= 1 && T >= 1, "dctts_reserve_frames: need B >= 1 and T >= 1, got B = " + std::to_string(B) + ", T = " +
+                                      std::to_string(T));
+        ensure_chain_frames(h, B, T, "dctts_reserve_frames");
+        if (bytes) *bytes = (int64_t)chain_ws_bytes(h);
+    });
+}
+
+int dctts_join_rows(dctts_handle h, const float* Y, int32_t P, int32_t T, const int32_t* piece_len,
+                    const int32_t* piece_text_host, const int32_t* piece_pause_host, int32_t K, float silence, int32_t T_out,
+                    float* out, int32_t* out_len, void* stream) {
+    return guarded(h, [&] {
+        const std::string fn = "dctts_join_rows";
+        REQUIRE(Y && piece_len && piece_text_host && piece_pause_host && out && out_len, fn + ": bad arguments");
+        REQUIRE(P >= 1 && K >= 1 && T >= 1 && T_out >= 1, fn + ": need P, K, T and T_out >= 1, got P = " + std::to_string(P) +
+                                                              ", K = " + std::to_string(K) + ", T = " + std::to_string(T) +
+                                                              ", T_out = " + std::to_string(T_out));
+        std::vector<int> meta(2 * (size_t)P + K + 1);
+        int* first = meta.data() + 2 * (size_t)P;
+        long long need = 0, rows = 0;                    // the longest text's rows at full-length pieces
+        for (int p = 0; p < P; ++p) {
+            const int k = piece_text_host[p], pause = piece_pause_host[p];
+            REQUIRE(k >= 0 && k < K, fn + ": piece " + std::to_string(p) + " belongs to text " + std::to_string(k) +
+                                         ", outside [0, " + std::to_string(K) + ")");
+            REQUIRE(p == 0 ? k == 0 : (k == piece_text_host[p - 1] || k == piece_text_host[p - 1] + 1),
+                    fn + ": piece " + std::to_string(p) + " belongs to text " + std::to_string(k) +
+                        ": each text needs at least one piece, and a text's pieces must follow the previous text's");
+            const bool last = p + 1 == P || piece_text_host[p + 1] != k;
+            REQUIRE(pause >= 0 && (!last || pause == 0), fn + ": piece " + std::to_string(p) + " has a pause of " +
+                                                            std::to_string(pause) + " rows (need >= 0, and 0 after a text's last piece)");
+            if (p == 0 || k != piece_text_host[p - 1]) { first[k] = p; rows = 0; }
+            rows += (long long)T + pause;
+            need = std::max(need, rows);
+            meta[p] = k; meta[(size_t)P + p] = pause;
+        }
+        REQUIRE(piece_text_host[P - 1] == K - 1, fn + ": the pieces cover texts 0 .. " + std::to_string(piece_text_host[P - 1]) +
+                                                     ", not all " + std::to_string(K));
+        REQUIRE(need <= T_out, fn + ": T_out = " + std::to_string(T_out) + " rows cannot hold a text of full-length pieces (" +
+                                   std::to_string(need) + " rows)");
+        first[K] = P;
+        chist_clear(h, "the long-form join ran after the last full-sequence chain");
+        cudaStream_t s = S(h, stream);
+        if (h->join_meta.bytes < meta.size() * sizeof(int)) {
+            CUDA_CHECK(cudaStreamSynchronize(s));        // an earlier join may still read the old buffer
+            h->join_meta.ensure(meta.size() * sizeof(int));
+        }
+        int* staged = pinned_staging(h, meta.size());
+        std::copy(meta.begin(), meta.end(), staged);
+        CUDA_CHECK(cudaMemcpyAsync(h->join_meta.p, staged, meta.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+        CUDA_CHECK(cudaEventRecord(h->path_uploaded, s));
+        JoinArgs a{};
+        const int* dm = h->join_meta.as<int>();
+        a.Y = Y; a.len = piece_len; a.text = dm; a.pause = dm + P; a.first = dm + 2 * (size_t)P;
+        a.out = out; a.out_len = out_len; a.silence = silence;
+        a.P = P; a.K = K; a.T = T; a.C = h->hp.n_mels; a.T_out = T_out;
+        launch_join_rows(a, s); h->launches++;
+    });
 }
 
 int dctts_set_tensor_path(dctts_handle h, int32_t mode) {

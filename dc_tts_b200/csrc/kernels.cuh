@@ -350,4 +350,19 @@ struct McdArgs {
 // one CTA per pair with `smem` bytes of dynamic shared memory; 1 launch
 void launch_mcd_dtw(const McdArgs& a, size_t smem, cudaStream_t s);
 
+// ---- the long-form join of decoded pieces into one mel sequence per text (kernels_longform.cu; DESIGN.md section 4e) ----
+struct JoinArgs {
+    const float* Y;                    // (P, T, C) the decoded pieces
+    const int* len;                    // (P) rows of each piece (clamped to [0, T])
+    const int* text;                   // (P) the text of each piece; a text's pieces are consecutive and in order
+    const int* pause;                  // (P) rows of `silence` after each piece, 0 after a text's last piece
+    const int* first;                  // (K + 1) the first piece of each text, then P
+    float* out;                        // (K, T_out, C)
+    int* out_len;                      // (K) rows of each text's sequence
+    float silence;
+    int P, K, T, C, T_out;
+};
+// one CTA per piece; 1 launch
+void launch_join_rows(const JoinArgs& a, cudaStream_t s);
+
 }  // namespace dctts

@@ -142,6 +142,37 @@ class Engine:
     def reserve(self, batch):
         self._check(self._lib.dctts_reserve(self._h, int(batch)), "dctts_reserve")
 
+    def reserve_frames(self, batch, frames):
+        """Grow the full-sequence chains' workspace to `batch` utterances of `frames` mel frames, above max_T too
+        (include/dctts.h: dctts_reserve_frames); returns the bytes those buffers hold afterwards."""
+        n = C.c_int64(0)
+        self._check(self._lib.dctts_reserve_frames(self._h, int(batch), int(frames), C.byref(n)), "dctts_reserve_frames")
+        return n.value
+
+    def join_rows(self, Y, lengths, piece_text, piece_pause, K, silence=1e-8):
+        """The long-form join (include/dctts.h: dctts_join_rows): Y (P, T, n_mels) decoded pieces, lengths (P,) int32 CUDA
+        tensor (as text2mel_generate_until returns it), piece_text / piece_pause (P,) host integers.  Returns (out
+        (K, T_out, n_mels), out_len (K,) int32 CUDA tensor), T_out the longest text at full-length pieces; one launch and
+        no synchronisation."""
+        Y = self._f32(Y)
+        P, T, Cm = Y.shape
+        n = self._i32(lengths).reshape(-1)
+        text = np.ascontiguousarray(np.asarray(piece_text).reshape(-1), dtype=np.int32)
+        pause = np.ascontiguousarray(np.asarray(piece_pause).reshape(-1), dtype=np.int32)
+        if Cm != self.hp.n_mels or n.shape[0] != P or text.shape[0] != P or pause.shape[0] != P:
+            raise DcttsError("join_rows: Y (P, T, %d) with P lengths, texts and pauses, got Y %s and %d, %d, %d"
+                             % (self.hp.n_mels, tuple(Y.shape), n.shape[0], text.shape[0], pause.shape[0]))
+        K = int(K)
+        if K < 1 or P < 1 or text.min() < 0 or text.max() >= K:
+            raise DcttsError("join_rows: need P >= 1 pieces whose texts lie in [0, K = %d)" % K)
+        T_out = int(max(np.bincount(text, weights=T + pause.astype(np.int64), minlength=K)))
+        out = self._empty(K, T_out, Cm)
+        out_len = self._empty(K, dtype=torch.int32)
+        self._check(self._lib.dctts_join_rows(self._h, _ptr(Y), P, T, _ptr(n), text.ctypes.data_as(C.c_void_p),
+                                              pause.ctypes.data_as(C.c_void_p), K, float(silence), T_out, _ptr(out),
+                                              _ptr(out_len), self._stream()), "dctts_join_rows")
+        return out, out_len
+
     def bench_block(self, scope, B, L, iters=5, warmup=2):
         """Mean device milliseconds of each kernel of one block (roofline leg of bench.py)."""
         ms = (C.c_float * 8)()
@@ -348,6 +379,7 @@ class Engine:
 
     def ssrn(self, Y, want_logits=True, out=None, lengths=None):
         """`out`: optional preallocated contiguous (B, 4T, F) float32 CUDA tensor (e.g. a slice of a gather buffer).
+        T may exceed max_T (long-form synthesis): the workspace grows to B x T frames first (reserve_frames).
         `lengths`: optional (B,) mel frames per utterance, 1 <= lengths[b] <= T (include/dctts.h: dctts_ssrn_ragged):
         rows < 4 lengths[b] of Z and the logits are what this call gives for Y[b:b+1, :lengths[b]] alone, bit for bit, rows
         past them are 0, and Y rows >= lengths[b] are never read.  The range is checked on the host (one small copy)."""
@@ -366,6 +398,8 @@ class Engine:
             bad = np.flatnonzero((nh < 1) | (nh > T))
             if bad.size:
                 raise DcttsError("ssrn: utterance %d has length %d outside [1, %d]" % (bad[0], nh[bad[0]], T))
+        if T > self.hp.max_T:               # grow the workspace first: a size it cannot take is refused before any output
+            self.reserve_frames(B, T)
         Z = out if out is not None else self._empty(B, T * self.hp.r, self.F)
         logits = self._empty(B, T * self.hp.r, self.F) if want_logits else None
         if n is None:

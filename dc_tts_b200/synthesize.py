@@ -34,8 +34,47 @@ def _timing_of(g, L, wavs):
     return path, t
 
 
+def _restore(engine, params, seed, allow_random_init):
+    """synthesize.py:31-41: the caller's dictionary, else the parameters already on the engine, else the checkpoints."""
+    if params is not None:
+        engine.load_params(params)
+        print("Parameters loaded from the caller's dictionary")
+    elif engine.params_loaded:
+        print("Using the parameters already committed to the engine")
+    else:
+        ck1, ck2 = latest_checkpoint(hp.logdir + "-1"), latest_checkpoint(hp.logdir + "-2")
+        if ck1 and ck2:
+            engine.restore(hp.logdir + "-1", hp.logdir + "-2")
+            print("Text2Mel Restored!")
+            print("SSRN Restored!")
+        elif allow_random_init:
+            engine.load_params(init_params(seed))
+            print("WARNING: no checkpoint -- seeded random weights (allow_random_init=True); the output is noise")
+        else:
+            missing = [d for d, c in ((hp.logdir + "-1", ck1), (hp.logdir + "-2", ck2)) if not c]
+            raise FileNotFoundError("no checkpoint under %s (reference: Saver.restore(sess, None) fails); pass params=..., "
+                                    "or allow_random_init=True for seeded random weights" % " and ".join(missing))
+
+
+def _synthesize_long_form(params, sentences, write, seed, allow_random_init, tail, momentum):
+    from .longform import read_texts, synthesize_texts
+    texts = read_texts(sentences or hp.test_data, header=True)
+    g = Graph(mode="synthesize")
+    with Session():
+        _restore(g.engine, params, seed, allow_random_init)
+        wavs, report = synthesize_texts(g.engine, texts, tail=tail, momentum=momentum)
+    if write:
+        from scipy.io.wavfile import write as write_wav
+        if not os.path.exists(hp.sampledir):
+            os.makedirs(hp.sampledir)
+        for i, wav in enumerate(wavs):
+            print("Working on file", i + 1)
+            write_wav(os.path.join(hp.sampledir, "{}.wav".format(i + 1)), hp.sr, wav)
+    return wavs, report
+
+
 def synthesize(params=None, sentences=None, fast=True, write=True, seed=0, vocoder=True, allow_random_init=False,
-               until_eos=False, tail=0, momentum=0.0, duration_scale=1.0, timing_from=None):
+               until_eos=False, tail=0, momentum=0.0, duration_scale=1.0, timing_from=None, long_form=False):
     """`params`: a name -> array dict to use instead of the checkpoints.  Without it the latest checkpoints of
     hp.logdir-1 (Text2Mel) and hp.logdir-2 (SSRN) are restored, and a missing one RAISES like the reference's
     `saver.restore(sess, None)` does (synthesize.py:33,39) -- seeded random weights are used only when the caller asks
@@ -58,7 +97,14 @@ def synthesize(params=None, sentences=None, fast=True, write=True, seed=0, vocod
     recording: the recording's features (resampled to hp.sr when needed) are aligned to the sentence (Graph.align), the
     recovered path is stretched by `duration_scale` when that is not 1, and the sentence is decoded along it
     (Graph.generate_along); SSRN and the vocoder run with each recording's frame count (or the stretched one).  A
-    recording longer than max_T frames is refused.  None leaves every other route exactly as it is."""
+    recording longer than max_T frames is refused.  None leaves every other route exactly as it is.
+
+    `long_form=True`: each line of the sentences file (the first line a header, a leading "N. " removed, as load_data
+    reads it) is one text of any length, read by longform.synthesize_texts (split into pieces, decoded to their ends as
+    one batch, joined on the device, SSRN and Griffin-Lim once per text), with `tail` and `momentum`; one wav per line.
+    Returns (wavs, report).  False leaves every other route exactly as it is."""
+    if long_form:
+        return _synthesize_long_form(params, sentences, write, seed, allow_random_init, tail, momentum)
     # Load data
     L = load_data("synthesize", sentences)
 
@@ -68,24 +114,7 @@ def synthesize(params=None, sentences=None, fast=True, write=True, seed=0, vocod
 
     with Session() as sess:
         # Restore parameters (synthesize.py:31-41)
-        if params is not None:
-            g.engine.load_params(params)
-            print("Parameters loaded from the caller's dictionary")
-        elif g.engine.params_loaded:
-            print("Using the parameters already committed to the engine")
-        else:
-            ck1, ck2 = latest_checkpoint(hp.logdir + "-1"), latest_checkpoint(hp.logdir + "-2")
-            if ck1 and ck2:
-                g.engine.restore(hp.logdir + "-1", hp.logdir + "-2")
-                print("Text2Mel Restored!")
-                print("SSRN Restored!")
-            elif allow_random_init:
-                g.engine.load_params(init_params(seed))
-                print("WARNING: no checkpoint -- seeded random weights (allow_random_init=True); the output is noise")
-            else:
-                missing = [d for d, c in ((hp.logdir + "-1", ck1), (hp.logdir + "-2", ck2)) if not c]
-                raise FileNotFoundError("no checkpoint under %s (reference: Saver.restore(sess, None) fails); pass params=..., "
-                                        "or allow_random_init=True for seeded random weights" % " and ".join(missing))
+        _restore(g.engine, params, seed, allow_random_init)
 
         lengths = None
         if timing_from is not None or until_eos or duration_scale != 1.0:

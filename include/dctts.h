@@ -100,6 +100,9 @@ int dctts_audiodec(dctts_handle h, const float* R, int32_t B, int32_t T,
 /* SSRN (networks.py:214-292): Y (B,T,n_mels) -> Z_logits, Z (B,4T,F). Z_logits may be NULL. */
 int dctts_ssrn(dctts_handle h, const float* Y, int32_t B, int32_t T,
                float* Z_logits, float* Z, void* stream);
+/* dctts_ssrn and dctts_ssrn_ragged take any T, also above max_T (long-form synthesis): the buffers the SSRN chain runs in
+ * grow in place to B x T mel frames (dctts_reserve_frames), and a T <= max_T call computes and launches what it did
+ * before any growth. */
 /* SSRN with a length per utterance.  lengths: (B) int32 DEVICE mel frames, 1 <= lengths[b] <= T (as
  * dctts_text2mel_generate_until writes them).  For each b, Z[b, :4 lengths[b]] and Z_logits[b, :4 lengths[b]] are
  * dctts_ssrn of Y[b:b+1, :lengths[b]] alone on the same kernel set, bit for bit; their rows past that are 0 (Z too).
@@ -202,6 +205,18 @@ int dctts_text2mel_align(dctts_handle h, const int32_t* L, const float* mels, in
 int dctts_mcd_dtw(dctts_handle h, const float* X, int32_t Tx, const int32_t* nx_host,
                   const float* Y, int32_t Ty, const int32_t* ny_host, int32_t B, int32_t K,
                   double* mcd, int32_t* pairs, int32_t* path, void* stream);
+/* The long-form join (dc_tts_b200/longform.py): the decoded pieces of K texts into one mel sequence per text.
+ * Y (P, T, n_mels) DEVICE, the pieces as dctts_text2mel_generate_until wrote them; piece_len (P) int32 DEVICE, their
+ * lengths (clamped to [0, T]); piece_text_host (P) and piece_pause_host (P) HOST: each piece's text, 0 .. K-1 with every
+ * text's pieces consecutive and in order, and the rows of `silence` that follow it (>= 0; 0 after a text's last piece).
+ * out (K, T_out, n_mels) DEVICE: text k's pieces' rows < len in order, each but the last followed by its pause rows, then
+ * zeros up to T_out; out_len (K) int32 DEVICE: each text's rows.  T_out must hold every text at full-length pieces
+ * (sum over its pieces of T + pause), checked on the host with the other arguments before anything is launched.  One
+ * launch; the offsets are a prefix sum of the device lengths inside the kernel, so the call does not wait for the decode
+ * (only for the previous upload out of the handle's pinned staging buffer, as dctts_text2mel_generate_path_host). */
+int dctts_join_rows(dctts_handle h, const float* Y, int32_t P, int32_t T, const int32_t* piece_len,
+                    const int32_t* piece_text_host, const int32_t* piece_pause_host, int32_t K, float silence, int32_t T_out,
+                    float* out, int32_t* out_len, void* stream);
 /* synthesize.py:45-57 end to end with HOST buffers: copies L_host in, runs
  * dctts_text2mel_generate + dctts_ssrn, copies Y_host (B,max_T,n_mels; may be NULL) and
  * Z_host (B,4*max_T,F) out, and synchronises.  Host buffers should be pinned for speed. */
@@ -387,6 +402,12 @@ int dctts_refresh_synthesis(dctts_handle h, void* stream);
 /* ---- utilities ----------------------------------------------------------------- */
 /* Pre-size the workspace (otherwise grown lazily on first use) for batches up to B. */
 int dctts_reserve(dctts_handle h, int32_t max_batch);
+/* Grow the buffers the full-sequence chains run in so that dctts_ssrn / dctts_ssrn_ragged take B utterances of T mel
+ * frames, T above max_T too, without allocating: r x B x T rows, 98688 bytes per frame at the LJ hyperparameters (c 512,
+ * d 256, F 1025).  Only ever grows and keeps the weights; it synchronises the device when it grows.  The new buffers are
+ * allocated before the old ones are freed: a size that cannot be allocated fails, naming the bytes, and leaves the
+ * handle as it was.  bytes (optional) receives what those buffers hold after the call. */
+int dctts_reserve_frames(dctts_handle h, int32_t B, int32_t T, int64_t* bytes);
 /* Number of kernels this library has launched on the handle since creation (graph
  * replays count their kernel nodes). */
 int64_t dctts_launch_count(dctts_handle h);
