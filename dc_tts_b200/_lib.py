@@ -58,6 +58,8 @@ SIGNATURES = {
     "dctts_attn_bwd": (C.c_int, [Handle, _p, _p, _p, _p, _p, _i32, _i32, _i32, _i32, _i32, _i32, _p, _p, _p, _p]),
     "dctts_train_loss": (C.c_int, [Handle, _p, _i32, _p, _i64, _i32, _p, _i32, _p, _p, _p]),
     "dctts_vocoder_stage": (C.c_int, [Handle, _i32, _i32, _i32, _p, _p, _p, C.POINTER(_i32), _p]),
+    "dctts_feature_stage": (C.c_int, [Handle, _i32, _i32, _p, _i32, C.POINTER(_i64), _i32, _i32, _i32, _p, _p, C.POINTER(_i32),
+                                      _p]),
     "dctts_set_vocoder_params": (C.c_int, [Handle, _i32, _i32, C.c_float, C.c_float, C.c_float, C.c_double, _i32]),
     "dctts_spectrogram2wav": (C.c_int, [Handle, _p, _i32, _i32, _i32, _p, _p, _p]),
     "dctts_spectrogram2wav_ragged": (C.c_int, [Handle, _p, _i32, _i32, _p, _i32, _p, _p, _p]),

@@ -40,6 +40,19 @@ void feat_tables(H* h, int sample_rate, cudaStream_t s) {
     h->feat_sr = sample_rate; h->feat_win = win;
 }
 
+// The arguments of feat_run for `frames` STFT frames of B trimmed utterances (seg_dev: B + 1 device entries), with the
+// handle's tables and vocoder parameters: mag (B, r T_b, F), mel (B, T_b, n_mels)
+FeatArgs feat_args(const H* h, const void* wav, int dtype, const FeatSeg* seg_dev, int B, long long frames, float* mel, float* mag,
+                   int T_b, int r) {
+    FeatArgs a{};
+    a.wav = wav; a.dtype = dtype; a.seg = seg_dev; a.B = B; a.frames = (int)frames;
+    a.mag = mag; a.mel = mel; a.mag_rows = r * T_b; a.mel_rows = T_b; a.r = r;
+    a.melw = h->feat_melw.as<float>(); a.melrange = h->feat_range.as<int>(); a.tw = h->feat_tw.as<float2>();
+    a.window = h->feat_window.as<float>(); a.F = h->F; a.n_mels = h->hp.n_mels; a.win = h->voc.win; a.hop = h->voc.hop;
+    a.preemph = (float)h->voc.preemph; a.ref_db = h->voc.ref_db; a.max_db = h->voc.max_db;
+    return a;
+}
+
 // load_spectrograms (utils.py:147-162) for B utterances packed back to back in `wav` (offsets: B + 1 host sample
 // offsets), reduced by r and padded with zeros to the batch's longest member: mel (B, T_b, n_mels), mag (B, r T_b, F).
 // r = 1 is get_spectrograms (utils.py:20-65): every frame, T_b = T for one utterance.  Two kernels whatever B is:
@@ -106,13 +119,7 @@ void feat_batch(H* h, const char* who, const void* wav, int dtype, const int64_t
         CUDA_CHECK(cudaMemsetAsync(mel, 0, (size_t)B * T_b * n_mels * sizeof(float), s));
         CUDA_CHECK(cudaMemsetAsync(mag, 0, (size_t)B * r * T_b * F * sizeof(float), s));
     }
-    FeatArgs a{};
-    a.wav = wav; a.dtype = dtype; a.seg = seg_dev + B + 1; a.B = B; a.frames = (int)frames;
-    a.mag = mag; a.mel = mel; a.mag_rows = r * T_b; a.mel_rows = T_b; a.r = r;
-    a.melw = h->feat_melw.as<float>(); a.melrange = h->feat_range.as<int>(); a.tw = h->feat_tw.as<float2>();
-    a.window = h->feat_window.as<float>(); a.F = F; a.n_mels = n_mels; a.win = h->voc.win; a.hop = hop;
-    a.preemph = (float)h->voc.preemph; a.ref_db = h->voc.ref_db; a.max_db = h->voc.max_db;
-    feat_run(a, s);
+    feat_run(feat_args(h, wav, dtype, seg_dev + B + 1, B, frames, mel, mag, T_b, r), s);
     h->launches += 1;
     CUDA_CHECK(cudaGetLastError());
 }
@@ -292,6 +299,59 @@ int dctts_vocoder_stage(dctts_handle h, int32_t stage, int32_t B, int32_t T, con
         CUDA_CHECK(cudaGetLastError());
         if (stage == 4) voc_trims(a, trim_host, s);
         else CUDA_CHECK(cudaStreamSynchronize(s));
+    });
+}
+
+int dctts_feature_stage(dctts_handle h, int32_t stage, int32_t sample_rate, const void* wav, int32_t dtype, const int64_t* seg_host,
+                        int32_t B, int32_t r, int32_t T_b, void* out, void* out2, int32_t* host_out, void* stream) {
+    return guarded(h, [&] {
+        const std::string fn = "dctts_feature_stage";
+        REQUIRE(stage >= 0 && stage <= 2, fn + ": stage " + std::to_string(stage) + " is not one of 0 energies, 1 spectra, 2 tables");
+        REQUIRE(out && (out2 || stage == 0) && (host_out || stage == 1) && sample_rate > 0 && B >= 1, fn + ": bad arguments");
+        require_fft_size(h, fn);
+        cudaStream_t s = S(h, stream);
+        if (stage == 2) {
+            feat_tables(h, sample_rate, s);
+            CUDA_CHECK(cudaMemcpyAsync(out, h->feat_melw.p, (size_t)h->hp.n_mels * h->F * sizeof(float), cudaMemcpyDeviceToDevice, s));
+            CUDA_CHECK(cudaMemcpyAsync(out2, h->feat_window.p, (size_t)h->voc.win * sizeof(float), cudaMemcpyDeviceToDevice, s));
+            CUDA_CHECK(cudaMemcpyAsync(host_out, h->feat_range.p, 2 * (size_t)h->hp.n_mels * sizeof(int), cudaMemcpyDeviceToHost, s));
+            CUDA_CHECK(cudaStreamSynchronize(s));
+            return;
+        }
+        REQUIRE(wav && seg_host && (dtype == 0 || dtype == 1), fn + ": wav, its segments and dtype 0 or 1 are required");
+        std::vector<FeatSeg> seg(B + 1);
+        long long frames = 0;
+        for (int b = 0; b < B; ++b) {
+            const long long src = stage == 0 ? seg_host[b] : seg_host[2 * b], n = stage == 0 ? seg_host[b + 1] - src : seg_host[2 * b + 1];
+            REQUIRE(src >= 0 && n >= 2 && n < (1ll << 30), fn + ": utterance " + std::to_string(b) + " has " + std::to_string(n) +
+                                                           " samples (need 2 to 2^30)");
+            seg[b] = FeatSeg{src, (int)n, (int)frames};
+            const long long T = stage == 0 ? 1 + n / 512 : 1 + n / h->voc.hop;
+            REQUIRE(stage == 0 || (r >= 1 && (T + r - 1) / r <= T_b), fn + ": utterance " + std::to_string(b) + " needs " +
+                                                                      std::to_string((T + r - 1) / std::max(r, 1)) + " rows at r = " +
+                                                                      std::to_string(r) + ", T_b is " + std::to_string(T_b));
+            frames += T;
+        }
+        REQUIRE(frames < (1ll << 31), fn + ": batch too long");
+        seg[B] = FeatSeg{0, 0, (int)frames};
+        h->feat_seg.ensure(seg.size() * sizeof(FeatSeg));
+        FeatSeg* seg_dev = h->feat_seg.as<FeatSeg>();
+        CUDA_CHECK(cudaMemcpyAsync(seg_dev, seg.data(), seg.size() * sizeof(FeatSeg), cudaMemcpyHostToDevice, s));
+        if (stage == 0) {
+            feat_frame_mse(wav, dtype, seg_dev, B, (int)frames, static_cast<float*>(out), s);
+            h->launches += 1;
+            CUDA_CHECK(cudaGetLastError());
+            std::vector<float> mse((size_t)frames);
+            CUDA_CHECK(cudaMemcpyAsync(mse.data(), out, mse.size() * sizeof(float), cudaMemcpyDeviceToHost, s));
+            CUDA_CHECK(cudaStreamSynchronize(s));
+            for (int b = 0; b < B; ++b) trim_from_mse(mse.data() + seg[b].f0, 1 + seg[b].len / 512, seg[b].len, host_out + 2 * b);
+            return;
+        }
+        feat_tables(h, sample_rate, s);
+        feat_run(feat_args(h, wav, dtype, seg_dev, B, frames, static_cast<float*>(out2), static_cast<float*>(out), T_b, r), s);
+        h->launches += 1;
+        CUDA_CHECK(cudaGetLastError());
+        CUDA_CHECK(cudaStreamSynchronize(s));
     });
 }
 

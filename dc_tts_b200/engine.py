@@ -767,6 +767,43 @@ class Engine:
                     "dctts_vocoder_stage")
         return trim if stage == 4 else out
 
+    def feature_stage(self, stage, out, out2=None, wav=None, segments=None, r=None, sr=None):
+        """Test aid (include/dctts.h: dctts_feature_stage): ONE stage of load_spectrograms_batch on caller CUDA tensors, with
+        the hyperparameters' vocoder constants and the feature tables for `sr` (default hp.sr).  wav: packed 1-D float32 or
+        int16 CUDA samples.  F = 1 + n_fft/2:
+          0 energies  segments = (B + 1) sample offsets          -> out = mse, sum_b (1 + n_b // 512) float32
+          1 spectra   segments = (B, 2) (first sample, length)   -> out = mag (B, r T_b, F), out2 = mel (B, T_b, n_mels)
+          2 tables                                               -> out = mel weights (n_mels, F), out2 = window (win)
+        Stage 1 writes only utterance b's rows t < 1 + length // hop of mag and t / r (t % r == 0) of mel.  Returns the
+        trims (B, 2) int32 numpy for stage 0, the filter ranges (n_mels, 2) int32 numpy for stage 2, else out."""
+        h = self.hp
+        r = int(r or h.r)
+        self._set_vocoder_params()
+        f32 = torch.float32
+        seg = None if segments is None else np.ascontiguousarray(np.asarray(segments).reshape(-1), dtype=np.int64)
+        dtype, B, T_b = 0, 1, 0
+        if stage in (0, 1):
+            if wav is None or seg is None:
+                raise DcttsError("feature_stage %d: needs wav and segments" % stage)
+            dtype = 1 if wav.dtype == torch.int16 else 0
+            _require_tensors("feature_stage %d" % stage, [(wav, (wav.numel(),), wav.dtype)])
+            B = seg.size - 1 if stage == 0 else seg.size // 2
+        if stage == 0:
+            n = np.diff(seg)
+            want = [(out, (int((1 + n // 512).sum()),), f32)]
+        elif stage == 1:
+            T_b = out2.shape[1]
+            want = [(out, (B, r * T_b, self.F), f32), (out2, (B, T_b, h.n_mels), f32)]
+        else:
+            want = [(out, (h.n_mels, self.F), f32), (out2, (int(h.win_length),), f32)]
+        _require_tensors("feature_stage %d" % stage, want)
+        host = np.zeros((h.n_mels if stage == 2 else B, 2), np.int32)
+        self._check(self._lib.dctts_feature_stage(
+            self._h, int(stage), int(sr or h.sr), _ptr(wav), dtype,
+            None if seg is None else seg.ctypes.data_as(C.POINTER(C.c_int64)), B, r, T_b, _ptr(out), _ptr(out2),
+            host.ctypes.data_as(C.POINTER(C.c_int32)), self._stream()), "dctts_feature_stage")
+        return out if stage == 1 else host
+
     def get_spectrograms(self, wav, sr=None):
         """utils.py:20-65 from a loaded waveform (1-D float32, hp.sr): -> (mel (T, n_mels), mag (T, F)) CUDA tensors and
         the [start, end) sample range librosa.effects.trim keeps."""

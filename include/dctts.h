@@ -562,6 +562,20 @@ int dctts_train_loss(dctts_handle h, const float* logits, int32_t ldl, const flo
  * Fails with a message on a bad stage or shape.  Synchronises `stream`. */
 int dctts_vocoder_stage(dctts_handle h, int32_t stage, int32_t B, int32_t T, const void* in, const float* S, void* out,
                         int32_t* trim_host, void* stream);
+/* Test aid: ONE stage of dctts_load_spectrograms_batch on caller DEVICE tensors, through the launch functions the product
+ * calls, with the handle's vocoder parameters and the feature tables it builds for `sample_rate`.  wav: packed samples,
+ * dtype 0 float32 or 1 int16 (value / 32768).  F = 1 + n_fft / 2.
+ *   0 energies: seg_host = B + 1 HOST sample offsets of whole utterances -> out = mse float32, utterance b's 1 + n_b / 512
+ *               frame energies (librosa.effects.trim's) back to back; host_out (B,2) HOST int32 receives the [start, end)
+ *               ranges dctts_load_spectrograms_batch would keep.
+ *   1 spectra:  seg_host = (B,2) HOST int64 (first sample, length >= 2) of already trimmed utterances, reduction r ->
+ *               out = mag (B, r T_b, F), out2 = mel (B, T_b, n_mels) float32.  Utterance b's T = 1 + length / hop frames
+ *               write mag rows t < T and mel rows t / r for t % r == 0 (T_b >= ceil(T / r)); no other element is written.
+ *   2 tables:   out = the uploaded mel weights (n_mels, F) float32, out2 = the Hann window (win) float32, host_out
+ *               (n_mels,2) HOST int32 = each filter's [first, last + 1) non-zero FFT bins.
+ * Fails with a message on a bad stage, segment or T_b.  Synchronises `stream`. */
+int dctts_feature_stage(dctts_handle h, int32_t stage, int32_t sample_rate, const void* wav, int32_t dtype, const int64_t* seg_host,
+                        int32_t B, int32_t r, int32_t T_b, void* out, void* out2, int32_t* host_out, void* stream);
 /* Test aid: ONE fast Griffin-Lim phase step of dctts_spectrogram2wav_momentum on caller DEVICE tensors, through the
  * same launch function, like dctts_vocoder_stage 2: in = wav (B,Ly) float32 and S (B,T,F) float32; E (B,T,F) complex64
  * holds est_{i-1} on entry and est_i on return; X (B,T,F) complex64 receives S c / max(1e-8, |c|).  partials: NULL, or

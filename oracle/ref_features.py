@@ -49,25 +49,26 @@ def mel_basis(sr=None, n_fft=None, n_mels=None):
     return w * (2.0 / (mel_f[2:n_mels + 2] - mel_f[:n_mels]))[:, None]
 
 
-def get_spectrograms(y):
-    """utils.py:33-65 from the loaded waveform `y` (float32, hp.sr) -> (mel (T, n_mels), mag (T, 1+n_fft/2))."""
+def get_spectrograms(y, dtype=np.float32):
+    """utils.py:33-65 from the loaded waveform `y` (float32, hp.sr) -> (mel (T, n_mels), mag (T, 1+n_fft/2)).
+    dtype=np.float64 runs everything after the (float32) trim and pre-emphasis in float64."""
     y = np.asarray(y, np.float32)
     s, e = rv.trim_indices(y)                                             # :36
     y = y[s:e]
     y = np.append(y[0], y[1:] - hp.preemphasis * y[:-1]).astype(np.float32)   # :39 (float32 in, float32 out)
-    linear = rv.stft(y)                                                   # :42-45  (F, T) complex64
+    linear = rv.stft(y.astype(dtype))                                     # :42-45  (F, T) complex64
     mag = np.abs(linear)                                                  # :48
     mel = np.dot(mel_basis(), mag)                                        # :51-52
     mel = 20 * np.log10(np.maximum(1e-5, mel))                            # :55-56
     mag = 20 * np.log10(np.maximum(1e-5, mag))
     mel = np.clip((mel - hp.ref_db + hp.max_db) / hp.max_db, 1e-8, 1)     # :59-60
     mag = np.clip((mag - hp.ref_db + hp.max_db) / hp.max_db, 1e-8, 1)
-    return mel.T.astype(np.float32), mag.T.astype(np.float32)
+    return mel.T.astype(dtype), mag.T.astype(dtype)
 
 
-def load_spectrograms(y):
+def load_spectrograms(y, dtype=np.float32):
     """utils.py:147-162 (without the file name): pad T to a multiple of hp.r, keep every r-th mel frame."""
-    mel, mag = get_spectrograms(y)
+    mel, mag = get_spectrograms(y, dtype)
     t = mel.shape[0]
     num_paddings = hp.r - (t % hp.r) if t % hp.r != 0 else 0
     mel = np.pad(mel, [[0, num_paddings], [0, 0]], mode="constant")
