@@ -166,14 +166,6 @@ void voc_trims(const VocoderArgs& a, int32_t* trim_host, cudaStream_t s, const i
         }
 }
 
-// A ragged call's frame counts: 2 <= lengths_host[b] <= T, else the call fails naming the utterance, before any launch
-void require_frame_counts(const std::string& fn, const int32_t* lengths_host, int B, int T) {
-    for (int b = 0; b < B; ++b)
-        REQUIRE(lengths_host[b] >= 2 && lengths_host[b] <= T, fn + ": utterance " + std::to_string(b) + " has " +
-                                                              std::to_string(lengths_host[b]) + " frames (need 2 to T = " +
-                                                              std::to_string(T) + ")");
-}
-
 // The fast Griffin-Lim weight alpha = momentum / (1 + momentum), formed in float64 and rounded to float32 as numpy does
 // when it multiplies a complex64 array by a Python float
 float momentum_alpha(const std::string& fn, double momentum) {
@@ -188,7 +180,7 @@ float momentum_alpha(const std::string& fn, double momentum) {
 void griffin_lim(H* h, const char* fn, const float* mag, int B, int T, const int32_t* lengths_host, int n_iter,
                  double momentum, float* wav, int32_t* trim_host, double* convergence, cudaStream_t s) {
     const float alpha = momentum_alpha(fn, momentum);
-    if (lengths_host) require_frame_counts(fn, lengths_host, B, T);
+    if (lengths_host) require_each(fn, "frame count", lengths_host, B, 2, T);
     VocoderArgs a = voc_args(h, fn, B, T, s);
     a.mag = mag; a.wav = wav;
     if (n_iter >= 0) a.n_iter = n_iter;

@@ -80,9 +80,11 @@ struct DevBuf {
     DevBuf(DevBuf&& o) noexcept : p(std::exchange(o.p, nullptr)), bytes(std::exchange(o.bytes, 0)) {}
     DevBuf& operator=(DevBuf&& o) noexcept { std::swap(p, o.p); std::swap(bytes, o.bytes); return *this; }
     ~DevBuf() { if (p) cudaFree(p); }
+    // At least n bytes; the contents are not kept.  A growth first waits for all work on the device, since kernels queued
+    // on any stream may still read the old allocation; so no growth may happen inside a stream capture.
     void ensure(size_t n) {
         if (n <= bytes) return;
-        if (p) CUDA_CHECK(cudaFree(p));
+        if (p) { CUDA_CHECK(cudaDeviceSynchronize()); CUDA_CHECK(cudaFree(p)); }
         p = nullptr; bytes = 0;
         CUDA_CHECK(cudaMalloc(&p, n));
         bytes = n;
@@ -130,8 +132,8 @@ struct dctts_handle_s {
     DevBuf ad_sig;                // scratch for sigmoid(logits) in full-graph mode
     DevBuf ibuf;                  // ints: j, p_cur[B], p_next[B], p_prev[B], p_hist[B*T]
     DevBuf pathbuf;               // ints of a decode along a window path: lengths[B], path[B*T], argmax[B*T]
-    int* path_pinned = nullptr;   // pinned staging of pathbuf's lengths and path, or of the aligner's lengths and ends,
-    size_t path_pinned_n = 0;     // reused once path_uploaded has fired (ints)
+    void* path_pinned = nullptr;  // pinned staging of the host arrays upload_host copies to the device (api_synth.cu),
+    size_t path_pinned_bytes = 0; // reused once path_uploaded has fired
     cudaEvent_t path_uploaded = nullptr;
     // the aligner (dctts_align_search, dctts_text2mel_align): back-pointers (B, T, N) uint8, lengths and ends (2B) ints, and
     // the alignments (B, max_N, T) when the caller does not ask for them
@@ -288,6 +290,21 @@ int guarded(dctts_handle h, Fn&& fn) {
         h->err = "unknown failure";
         return 3;
     }
+}
+
+// Per-utterance integers from the caller's host memory, checked before anything is launched: values[b] in [lo, hi] for
+// b < B or, with `counts`, the first counts[b] values of row b of the (B, ld) array `values`, one per frame.  The first
+// value outside fails the call, naming its utterance (and frame): "<fn>: utterance <b> has <what> <v> outside [lo, hi]".
+inline void require_each(const std::string& fn, const char* what, const int* values, int B, long long lo, long long hi,
+                         const int* counts = nullptr, size_t ld = 0) {
+    for (int b = 0; b < B; ++b)
+        for (int j = 0; j < (counts ? counts[b] : 1); ++j) {
+            const int v = counts ? values[(size_t)b * ld + j] : values[b];
+            if (v < lo || v > hi)
+                throw std::runtime_error(fn + ": utterance " + std::to_string(b) + " has " + what + " " + std::to_string(v) +
+                                         (counts ? " at frame " + std::to_string(j) : std::string()) + " outside [" +
+                                         std::to_string(lo) + ", " + std::to_string(hi) + "]");
+        }
 }
 
 // NULL means the legacy default stream (what torch's default stream is), so calls made from a

@@ -198,7 +198,6 @@ void ensure_chain_frames(H* h, int B, int T, const char* who) {
     for (auto& pb : h->plane) grow = grow || pb.bytes < pl;
     if (!grow) return;
     const size_t want = std::max(scr, h->scratch.bytes) + 2 * std::max(act, h->act0.bytes) + 4 * std::max(pl, h->plane[0].bytes);
-    CUDA_CHECK(cudaDeviceSynchronize());
     DevBuf n_scr, n_act[2], n_pl[4];
     try {
         n_scr.ensure(std::max(scr, h->scratch.bytes));
@@ -213,6 +212,7 @@ void ensure_chain_frames(H* h, int B, int T, const char* who) {
     }
     chist_clear(h, "the workspace grew after the last chain");
     drop_ar_graph(h);                                     // the captured AR step has the old pointers baked in
+    CUDA_CHECK(cudaDeviceSynchronize());                  // the old buffers are freed with n_* below, unread by then
     std::swap(h->scratch, n_scr); std::swap(h->act0, n_act[0]); std::swap(h->act1, n_act[1]);
     for (int i = 0; i < 4; ++i) std::swap(h->plane[i], n_pl[i]);
 }
@@ -306,9 +306,7 @@ void run_chain_full(Launch& lc, const std::vector<LayerDev>& net, const float* X
         int up = 1;                                        // output rows per input row
         for (auto& l : net) if (l.kind == K_D) up *= 2;
         const int Lout = L * up, C = net.back().cout;
-        for (int b = 0; b < B; ++b)
-            REQUIRE(n[b] >= 1 && n[b] <= L, "utterance " + std::to_string(b) + ": length " + std::to_string(n[b]) +
-                                                " outside [1, " + std::to_string(L) + "]");
+        require_each("ragged chain", "length", n.data(), B, 1, L);
         for (int b = 0; b < B; ++b) {
             const size_t o = (size_t)b * Lout * C, live = (size_t)n[b] * up * C, dead = (size_t)Lout * C - live;
             run_chain_full(lc, net, X + (size_t)b * L * ldx, ldx, 1, n[b], out ? out + o : nullptr, out_sig ? out_sig + o : nullptr);
@@ -465,15 +463,6 @@ void run_chain_tc_planes(Launch& lc, const std::vector<LayerDev>& net, Planes cu
     }
 }
 
-// (B) device floats for the inverse input scales; grows (after a device sync) for an op-level call beyond the workspace
-float* input_inv_scales(H* h, int B) {
-    if (h->in_inv.bytes < (size_t)B * sizeof(float)) {
-        CUDA_CHECK(cudaDeviceSynchronize());
-        h->in_inv.ensure((size_t)B * sizeof(float));
-    }
-    return h->in_inv.as<float>();
-}
-
 // The fp32 (B, L, l.cin) input of block l -> its split planes, the way the chains carry that block's input: the first
 // block of AudioEnc, AudioDec and SSRN reads audio-level data (mels, R), which silence puts at 1e-8 and below, so its
 // planes get a power-of-two scale per utterance (the inverses are returned for the block's epilogue).  Every other
@@ -491,7 +480,8 @@ const float* block_input_planes(Launch& lc, const LayerDev& l, const float* x, i
         launch_f32_to_planes(x, ldx, p, (long long)B * L, l.cin, lc.s); lc.count();
         return nullptr;
     }
-    float* in_inv = input_inv_scales(h, B);
+    h->in_inv.ensure((size_t)B * sizeof(float));         // an op-level call may exceed the workspace's batch
+    float* in_inv = h->in_inv.as<float>();
     launch_f32_to_planes_scaled(x, ldx, p, B, L, l.cin, in_inv, lc.s, lengths); lc.count();
     return in_inv;
 }
@@ -528,8 +518,7 @@ void dctts::api::run_attention_tc(Launch& lc, const float* Q, int ldq, const flo
     H* h = lc.h;
     const int d = h->hp.d, NP = attn_tc_padded_keys(N);
     const size_t need[3] = {(size_t)B * T * d * sizeof(__half), (size_t)B * N * d * sizeof(__half), (size_t)B * d * NP * sizeof(__half)};
-    for (int i = 0; i < 6; ++i)
-        if (h->attpl[i].bytes < need[i / 2]) { CUDA_CHECK(cudaDeviceSynchronize()); h->attpl[i].ensure(need[i / 2]); }
+    for (int i = 0; i < 6; ++i) h->attpl[i].ensure(need[i / 2]);
     Planes qp, kp, vp;
     qp.hi = h->attpl[0].as<__half>(); qp.lo = h->attpl[1].as<__half>(); qp.ld = d;
     kp.hi = h->attpl[2].as<__half>(); kp.lo = h->attpl[3].as<__half>(); kp.ld = d;
@@ -857,10 +846,7 @@ void run_block_op(Launch& lc, const LayerDev& l, int rate, bool causal, int act,
     const int Lout = (l.kind == K_D) ? 2 * L : L;
     if (h->tensor_path == 1 && l.tc.ok) {
         const size_t need = (size_t)B * L * roundup(l.cin, 8) * sizeof(__half);
-        if (h->plane[0].bytes < need || h->plane[1].bytes < need) {
-            CUDA_CHECK(cudaDeviceSynchronize());
-            h->plane[0].ensure(need); h->plane[1].ensure(need);
-        }
+        h->plane[0].ensure(need); h->plane[1].ensure(need);
         Planes X = ws_planes(h, 0, l.cin);
         const float* in_inv = block_input_planes(lc, l, x, l.cin, X, B, L);
         run_block_tc(lc, l, rate, causal, act, X, RowWin{B, L, L, nullptr}, 128, 1, (L + 127) / 128, Planes{}, out, l.cout,
@@ -885,9 +871,8 @@ LayerDev* find_layer(H* h, const char* scope, int kind) {
 void ensure_scratch(H* h, size_t bytes) {
     bytes = std::max(bytes, (size_t)64 << 20);     // room for the skinny GEMM's split-K partials
     if (bytes <= h->scratch.bytes) return;
-    CUDA_CHECK(cudaDeviceSynchronize());
+    h->scratch.ensure(bytes);                      // synchronises: no replay of the graph is in flight below
     drop_ar_graph(h);
-    h->scratch.ensure(bytes);
 }
 
 }  // namespace
@@ -1060,49 +1045,38 @@ int dctts_text2mel_generate_until(dctts_handle h, const int32_t* L, int32_t B, i
 
 namespace {
 
-// The pinned staging buffer for n ints of host arrays that go to the device with one asynchronous copy.  The only wait
-// is for the previous upload out of it (path_uploaded, which the caller records after its copy).
-int* pinned_staging(H* h, size_t n) {
+// `bytes` of host memory to the device at dst, one asynchronous copy on s.  They are staged in the handle's pinned
+// buffer, whose only wait is for the previous upload out of it, so the host keeps queueing while earlier work runs.
+void upload_host(H* h, void* dst, const void* src, size_t bytes, cudaStream_t s) {
     if (!h->path_uploaded) CUDA_CHECK(cudaEventCreateWithFlags(&h->path_uploaded, cudaEventDisableTiming));
     CUDA_CHECK(cudaEventSynchronize(h->path_uploaded));          // the staging buffer is free again
-    if (h->path_pinned_n < n) {
-        if (h->path_pinned) { CUDA_CHECK(cudaFreeHost(h->path_pinned)); h->path_pinned = nullptr; h->path_pinned_n = 0; }
-        CUDA_CHECK(cudaMallocHost(&h->path_pinned, n * sizeof(int)));
-        h->path_pinned_n = n;
+    if (h->path_pinned_bytes < bytes) {
+        if (h->path_pinned) { CUDA_CHECK(cudaFreeHost(h->path_pinned)); h->path_pinned = nullptr; h->path_pinned_bytes = 0; }
+        CUDA_CHECK(cudaMallocHost(&h->path_pinned, bytes));
+        h->path_pinned_bytes = bytes;
     }
-    return h->path_pinned;
+    std::memcpy(h->path_pinned, src, bytes);
+    CUDA_CHECK(cudaMemcpyAsync(dst, h->path_pinned, bytes, cudaMemcpyHostToDevice, s));
+    CUDA_CHECK(cudaEventRecord(h->path_uploaded, s));
 }
 
 // dctts_text2mel_generate_path with the path (B, steps) and the lengths (B) in host memory.  They are checked before
-// anything is launched, then staged in pinned memory and uploaded with one asynchronous copy; the only wait is for the
-// previous call's upload out of the same staging buffer, so the host keeps queueing while earlier decodes run.
+// anything is launched, then uploaded without waiting for the stream (upload_host).
 void generate_path(H* h, const int* L, int B, int steps, const int* p, const int* n, float* Y, int* prev_hist,
                    int* argmax_hist, cudaStream_t s) {
     const dctts_hparams& hp = h->hp;
-    const int T = hp.max_T, N = hp.max_N;
-    for (int b = 0; b < B; ++b) {
-        const int nb = n[b];
-        if (nb < 1 || nb > steps)
-            throw std::runtime_error("dctts_text2mel_generate_path: utterance " + std::to_string(b) + " has length " +
-                                     std::to_string(nb) + " outside [1, " + std::to_string(steps) + "]");
-        for (int j = 0; j < nb; ++j) {
-            const int w = p[(size_t)b * steps + j];
-            if (w < 0 || w >= N)
-                throw std::runtime_error("dctts_text2mel_generate_path: utterance " + std::to_string(b) + " has window " +
-                                         std::to_string(w) + " at frame " + std::to_string(j) + " outside [0, " +
-                                         std::to_string(N) + ")");
-        }
-    }
+    const int T = hp.max_T;
+    const std::string fn = "dctts_text2mel_generate_path";
+    require_each(fn, "length", n, B, 1, steps);
+    require_each(fn, "window", p, B, 0, hp.max_N - 1, n, steps);
     ensure_ws(h, B);
     const PathRun pr = path_run(h);
-    const size_t n_up = (size_t)h->ws_B + (size_t)B * T;      // pathbuf's lengths, then the first B path rows
-    int* st = pinned_staging(h, n_up);
-    std::copy(n, n + B, st);
+    std::vector<int> up((size_t)h->ws_B + (size_t)B * T);      // pathbuf's lengths, then the first B path rows
+    std::copy(n, n + B, up.begin());
     for (int b = 0; b < B; ++b)
         for (int j = 0; j < T; ++j)     // past the length: the last window, so no frame there moves it
-            st[h->ws_B + (size_t)b * T + j] = p[(size_t)b * steps + std::min(j, n[b] - 1)];
-    CUDA_CHECK(cudaMemcpyAsync(const_cast<int*>(pr.lengths), st, n_up * sizeof(int), cudaMemcpyHostToDevice, s));
-    CUDA_CHECK(cudaEventRecord(h->path_uploaded, s));
+            up[h->ws_B + (size_t)b * T + j] = p[(size_t)b * steps + std::min(j, n[b] - 1)];
+    upload_host(h, const_cast<int*>(pr.lengths), up.data(), up.size() * sizeof(int), s);
     text2mel_generate(h, L, B, steps, Y, prev_hist, nullptr, nullptr, s, nullptr, &pr);
     // rows at and past each length: 0 in Y, -1 in the histories
     int* len = const_cast<int*>(pr.lengths);
@@ -1120,13 +1094,14 @@ int check_align(H* h, const char* who, int B, int N, int T, const int* n, const 
     REQUIRE(w >= 1 && w <= 256, std::string(who) + ": attention_win_size must be in [1, 256]");
     int smem_max = 0;
     CUDA_CHECK(cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
+    require_each(who, "length", n, B, 1, T);
+    for (int b = 0; b < B; ++b)
+        REQUIRE(e[b] >= 0, std::string(who) + ": utterance " + std::to_string(b) + " has no EOS (text end " +
+                               std::to_string(e[b]) + ")");
+    require_each(who, "text end", e, B, 0, N - 1);
     int max_end = 0;
     for (int b = 0; b < B; ++b) {
         const std::string u = std::string(who) + ": utterance " + std::to_string(b);
-        if (n[b] < 1 || n[b] > T)
-            throw std::runtime_error(u + " has length " + std::to_string(n[b]) + " outside [1, " + std::to_string(T) + "]");
-        if (e[b] < 0 || e[b] >= N)
-            throw std::runtime_error(u + " has text end " + std::to_string(e[b]) + " outside [0, " + std::to_string(N) + ")");
         if ((long long)e[b] > (long long)(w - 1) * n[b])
             throw std::runtime_error(u + ": its text end " + std::to_string(e[b]) + " cannot be reached in " +
                                      std::to_string(n[b]) + " frames with attention_win_size " + std::to_string(w) +
@@ -1143,17 +1118,11 @@ int check_align(H* h, const char* who, int B, int N, int T, const int* n, const 
 void align_search(Launch& lc, const float* A, int B, int N, int T, const int* n, const int* e, int max_end,
                   int* path, int* chars, int* durations, double* score) {
     H* h = lc.h;
-    const size_t bp_bytes = (size_t)B * T * N, meta_bytes = 2 * (size_t)B * sizeof(int);
-    if (h->align.bp.bytes < bp_bytes || h->align.meta.bytes < meta_bytes) {
-        CUDA_CHECK(cudaDeviceSynchronize());              // an earlier search may still read the old buffers
-        h->align.bp.ensure(bp_bytes);
-        h->align.meta.ensure(meta_bytes);
-    }
-    int* st = pinned_staging(h, 2 * (size_t)B);
-    std::copy(n, n + B, st);
-    std::copy(e, e + B, st + B);
-    CUDA_CHECK(cudaMemcpyAsync(h->align.meta.p, st, meta_bytes, cudaMemcpyHostToDevice, lc.s));
-    CUDA_CHECK(cudaEventRecord(h->path_uploaded, lc.s));
+    std::vector<int> meta(n, n + B);
+    meta.insert(meta.end(), e, e + B);
+    h->align.bp.ensure((size_t)B * T * N);
+    h->align.meta.ensure(meta.size() * sizeof(int));
+    upload_host(h, h->align.meta.p, meta.data(), meta.size() * sizeof(int), lc.s);
     AlignArgs a{};
     a.A = A; a.meta = h->align.meta.as<int>(); a.bp = h->align.bp.as<unsigned char>();
     a.path = path; a.chars = chars; a.durations = durations; a.score = score;
@@ -1192,8 +1161,7 @@ int dctts_text2mel_align(dctts_handle h, const int32_t* L, const float* mels, in
         Launch lc{h, S(h, stream)};
         float* A = alignments;
         if (!A) {
-            const size_t bytes = (size_t)B * N * T * sizeof(float);
-            if (h->align.A.bytes < bytes) { CUDA_CHECK(cudaDeviceSynchronize()); h->align.A.ensure(bytes); }
+            h->align.A.ensure((size_t)B * N * T * sizeof(float));
             A = h->align.A.as<float>();
         }
         text2mel_front(lc, L, mels, nullptr, B, T, nullptr, A);
@@ -1214,13 +1182,11 @@ int dctts_mcd_dtw(dctts_handle h, const float* X, int32_t Tx, const int32_t* nx_
         const size_t ldc = (size_t)(K | 1);
         std::vector<long long> meta(4 * (size_t)B);
         size_t bp_bytes = 0, cep_doubles = 0, smem = 0;
+        require_each("dctts_mcd_dtw", "X length", nx_host, B, 1, Tx);
+        require_each("dctts_mcd_dtw", "Y length", ny_host, B, 1, Ty);
         for (int b = 0; b < B; ++b) {
             const std::string u = "dctts_mcd_dtw: utterance " + std::to_string(b);
             const long long nx = nx_host[b], ny = ny_host[b];
-            if (nx < 1 || nx > Tx)
-                throw std::runtime_error(u + " has X length " + std::to_string(nx) + " outside [1, " + std::to_string(Tx) + "]");
-            if (ny < 1 || ny > Ty)
-                throw std::runtime_error(u + " has Y length " + std::to_string(ny) + " outside [1, " + std::to_string(Ty) + "]");
             const size_t diag = 3 * (size_t)nx * sizeof(double), cep = (size_t)(nx + ny) * ldc * sizeof(double);
             if (diag > (size_t)smem_max)
                 throw std::runtime_error(u + ": three diagonals of " + std::to_string(nx) + " doubles do not fit in the device's " +
@@ -1233,12 +1199,9 @@ int dctts_mcd_dtw(dctts_handle h, const float* X, int32_t Tx, const int32_t* nx_
             smem = std::max(smem, staged ? diag + cep : diag);
         }
         const size_t meta_bytes = meta.size() * sizeof(long long);
-        if (h->mcd.bp.bytes < bp_bytes || h->mcd.meta.bytes < meta_bytes || h->mcd.cep.bytes < cep_doubles * sizeof(double)) {
-            CUDA_CHECK(cudaDeviceSynchronize());              // an earlier call may still use the old buffers
-            h->mcd.bp.ensure(bp_bytes);
-            h->mcd.meta.ensure(meta_bytes);
-            h->mcd.cep.ensure(cep_doubles * sizeof(double));
-        }
+        h->mcd.bp.ensure(bp_bytes);
+        h->mcd.meta.ensure(meta_bytes);
+        h->mcd.cep.ensure(cep_doubles * sizeof(double));
         if (!h->mcd.dct.p) {                                  // D[k, m] = sqrt(2 / M) cos(pi k (2m + 1) / (2M)), k >= 1
             std::vector<double> D((size_t)(M - 1) * M);
             const double pi = 3.141592653589793;
@@ -1250,10 +1213,7 @@ int dctts_mcd_dtw(dctts_handle h, const float* X, int32_t Tx, const int32_t* nx_
         }
         chist_clear(h, "an MCD-DTW call ran after the last full-sequence chain");
         Launch lc{h, S(h, stream)};
-        int* st = pinned_staging(h, 2 * meta.size());
-        std::memcpy(st, meta.data(), meta_bytes);
-        CUDA_CHECK(cudaMemcpyAsync(h->mcd.meta.p, st, meta_bytes, cudaMemcpyHostToDevice, lc.s));
-        CUDA_CHECK(cudaEventRecord(h->path_uploaded, lc.s));
+        upload_host(h, h->mcd.meta.p, meta.data(), meta_bytes, lc.s);
         McdArgs a{};
         a.X = X; a.Y = Y; a.meta = h->mcd.meta.as<long long>(); a.dct = h->mcd.dct.as<double>();
         a.cep = h->mcd.cep.as<double>(); a.bp = h->mcd.bp.as<unsigned char>();
@@ -1428,14 +1388,8 @@ int dctts_join_rows(dctts_handle h, const float* Y, int32_t P, int32_t T, const 
         first[K] = P;
         chist_clear(h, "the long-form join ran after the last full-sequence chain");
         cudaStream_t s = S(h, stream);
-        if (h->join_meta.bytes < meta.size() * sizeof(int)) {
-            CUDA_CHECK(cudaStreamSynchronize(s));        // an earlier join may still read the old buffer
-            h->join_meta.ensure(meta.size() * sizeof(int));
-        }
-        int* staged = pinned_staging(h, meta.size());
-        std::copy(meta.begin(), meta.end(), staged);
-        CUDA_CHECK(cudaMemcpyAsync(h->join_meta.p, staged, meta.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-        CUDA_CHECK(cudaEventRecord(h->path_uploaded, s));
+        h->join_meta.ensure(meta.size() * sizeof(int));
+        upload_host(h, h->join_meta.p, meta.data(), meta.size() * sizeof(int), s);
         JoinArgs a{};
         const int* dm = h->join_meta.as<int>();
         a.Y = Y; a.len = piece_len; a.text = dm; a.pause = dm + P; a.first = dm + 2 * (size_t)P;

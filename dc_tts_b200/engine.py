@@ -31,6 +31,24 @@ def _require_tensors(who, want):
                              (who, dt, shape, t.dtype, tuple(t.shape)))
 
 
+def _host(x):
+    """A list, numpy array or tensor on any device as a host numpy array."""
+    return np.asarray(x.cpu() if isinstance(x, torch.Tensor) else x)
+
+
+def _host_ints(who, x, B, name, lo=-2 ** 31, hi=2 ** 31 - 1):
+    """`x` (a list, numpy array or tensor on any device) as a host int64 vector of B values, each in [lo, hi]; else
+    DcttsError "<who>: <n> <name>s for <B> utterances" or "<who>: utterance <b> has <name> <v> outside [lo, hi]".  The
+    default range is int32's, the type every entry point takes."""
+    v = _host(x).astype(np.int64).reshape(-1)
+    if v.shape[0] != B:
+        raise DcttsError("%s: %d %ss for %d utterances" % (who, v.shape[0], name, B))
+    bad = np.flatnonzero((v < lo) | (v > hi))
+    if bad.size:
+        raise DcttsError("%s: utterance %d has %s %d outside [%d, %d]" % (who, bad[0], name, v[bad[0]], lo, hi))
+    return v
+
+
 class Engine:
     def __init__(self, device=0, hparams=hp):
         self._lib = _lib.load()
@@ -157,11 +175,11 @@ class Engine:
         Y = self._f32(Y)
         P, T, Cm = Y.shape
         n = self._i32(lengths).reshape(-1)
-        text = np.ascontiguousarray(np.asarray(piece_text).reshape(-1), dtype=np.int32)
-        pause = np.ascontiguousarray(np.asarray(piece_pause).reshape(-1), dtype=np.int32)
-        if Cm != self.hp.n_mels or n.shape[0] != P or text.shape[0] != P or pause.shape[0] != P:
-            raise DcttsError("join_rows: Y (P, T, %d) with P lengths, texts and pauses, got Y %s and %d, %d, %d"
-                             % (self.hp.n_mels, tuple(Y.shape), n.shape[0], text.shape[0], pause.shape[0]))
+        if Cm != self.hp.n_mels or n.shape[0] != P:
+            raise DcttsError("join_rows: Y (P, T, %d) with P lengths, got Y %s and %d lengths"
+                             % (self.hp.n_mels, tuple(Y.shape), n.shape[0]))
+        text = np.ascontiguousarray(_host_ints("join_rows", piece_text, P, "piece text"), np.int32)
+        pause = np.ascontiguousarray(_host_ints("join_rows", piece_pause, P, "piece pause"), np.int32)
         K = int(K)
         if K < 1 or P < 1 or text.min() < 0 or text.max() >= K:
             raise DcttsError("join_rows: need P >= 1 pieces whose texts lie in [0, K = %d)" % K)
@@ -392,12 +410,7 @@ class Engine:
         n = None
         if lengths is not None:
             n = self._i32(lengths).reshape(-1)
-            nh = n.cpu().numpy()
-            if nh.shape[0] != B:
-                raise DcttsError("ssrn: %d lengths for %d utterances" % (nh.shape[0], B))
-            bad = np.flatnonzero((nh < 1) | (nh > T))
-            if bad.size:
-                raise DcttsError("ssrn: utterance %d has length %d outside [1, %d]" % (bad[0], nh[bad[0]], T))
+            _host_ints("ssrn", n, B, "length", 1, T)
         if T > self.hp.max_T:               # grow the workspace first: a size it cannot take is refused before any output
             self.reserve_frames(B, T)
         Z = out if out is not None else self._empty(B, T * self.hp.r, self.F)
@@ -447,25 +460,19 @@ class Engine:
         L = self._i32(L)
         B = L.shape[0]
         sp = eos_positions(L.cpu().numpy()) if stop_pos is None else \
-            np.asarray(stop_pos.cpu() if isinstance(stop_pos, torch.Tensor) else stop_pos, np.int64).reshape(-1)
-        if sp.shape[0] != B:
-            raise DcttsError("text2mel_generate_until: %d stop positions for %d utterances" % (sp.shape[0], B))
+            _host_ints("text2mel_generate_until", stop_pos, B, "stop position")
         order = np.argsort(np.where(sp < 0, np.iinfo(np.int32).max, sp), kind="stable")
-        perm = None if np.array_equal(order, np.arange(B)) else torch.as_tensor(order, device=self.device)
-        Ls = L if perm is None else L.index_select(0, perm).contiguous()
-        sps = self._i32(sp[order])
-        Y = self._empty(B, self.hp.max_T, self.hp.n_mels)
-        P = self._empty(B, self.hp.max_T, dtype=torch.int32)
-        n = self._empty(B, dtype=torch.int32)
-        self._check(self._lib.dctts_text2mel_generate_until(self._h, _ptr(Ls), B, int(steps), _ptr(sps), int(tail), _ptr(Y),
-                                                            _ptr(P), _ptr(n), self._stream()),
-                    "dctts_text2mel_generate_until")
-        self._decode_order = order
-        if perm is None:
+
+        def decode(Ls):
+            sps = self._i32(sp[order])
+            Y = self._empty(B, self.hp.max_T, self.hp.n_mels)
+            P = self._empty(B, self.hp.max_T, dtype=torch.int32)
+            n = self._empty(B, dtype=torch.int32)
+            self._check(self._lib.dctts_text2mel_generate_until(self._h, _ptr(Ls), B, int(steps), _ptr(sps), int(tail),
+                                                                _ptr(Y), _ptr(P), _ptr(n), self._stream()),
+                        "dctts_text2mel_generate_until")
             return Y, P, n
-        Yc, Pc, nc = torch.empty_like(Y), torch.empty_like(P), torch.empty_like(n)
-        Yc[perm], Pc[perm], nc[perm] = Y, P, n
-        return Yc, Pc, nc
+        return self._decode_in_order(L, order, decode)
 
     def text2mel_generate_path(self, L, path, lengths=None, steps=0):
         """The decode along a caller's attention windows (include/dctts.h: dctts_text2mel_generate_path): frame j of
@@ -477,19 +484,15 @@ class Engine:
         # Every host-side step comes before L is copied to the device: that copy waits for earlier work on the stream,
         # and host work after it would leave the GPU idle.
         B = len(L)
-        ph = np.asarray(path.cpu() if isinstance(path, torch.Tensor) else path, np.int64)
+        ph = _host(path).astype(np.int64)
         if ph.ndim != 2 or ph.shape[0] != B:
             raise DcttsError("text2mel_generate_path: path must be (B, steps) for %d utterances, got %s" % (B, ph.shape))
         steps = int(steps) or ph.shape[1]
         if not 1 <= steps <= min(ph.shape[1], self.hp.max_T):
             raise DcttsError("text2mel_generate_path: steps %d outside [1, %d]" % (steps, min(ph.shape[1], self.hp.max_T)))
+        # the library sees the utterances sorted: only here can a refusal name them in the caller's order
         n = np.full(B, steps, np.int64) if lengths is None else \
-            np.asarray(lengths.cpu() if isinstance(lengths, torch.Tensor) else lengths, np.int64).reshape(-1)
-        if n.shape[0] != B:
-            raise DcttsError("text2mel_generate_path: %d lengths for %d utterances" % (n.shape[0], B))
-        bad = np.flatnonzero((n < 1) | (n > steps))
-        if bad.size:
-            raise DcttsError("text2mel_generate_path: utterance %d has length %d outside [1, %d]" % (bad[0], n[bad[0]], steps))
+            _host_ints("text2mel_generate_path", lengths, B, "length", 1, steps)
         ph = ph[:, :steps]
         out = np.argwhere((np.arange(steps) < n[:, None]) & ((ph < 0) | (ph >= self.hp.max_N)))
         if out.size:
@@ -499,44 +502,37 @@ class Engine:
         order = np.argsort(n, kind="stable")
         ps = np.ascontiguousarray(ph[order], np.int32)
         ns = np.ascontiguousarray(n[order], np.int32)
+
+        def decode(Ls):
+            # host arrays: the entry point stages them itself, without waiting for earlier work on the stream
+            Y = self._empty(B, self.hp.max_T, self.hp.n_mels)
+            P = self._empty(B, self.hp.max_T, dtype=torch.int32)
+            M = self._empty(B, self.hp.max_T, dtype=torch.int32)
+            self._check(self._lib.dctts_text2mel_generate_path_host(self._h, _ptr(Ls), B, steps, C.c_void_p(ps.ctypes.data),
+                                                                    C.c_void_p(ns.ctypes.data), _ptr(Y), _ptr(P), _ptr(M),
+                                                                    self._stream()),
+                        "dctts_text2mel_generate_path_host")
+            return Y, P, M
+        return self._decode_in_order(L, order, decode)
+
+    def _decode_in_order(self, L, order, decode):
+        """decode(Ls) on the texts L (B, max_N) taken in `order`, its (B, ...) CUDA outputs returned in the caller's order.
+        decode_history reads the decode's own order from _decode_order."""
         L = self._i32(L)
-        perm = None if np.array_equal(order, np.arange(B)) else torch.as_tensor(order, device=self.device)
-        Ls = L if perm is None else L.index_select(0, perm).contiguous()
-        # host arrays: the entry point stages them itself, without waiting for earlier work on the stream
-        Y = self._empty(B, self.hp.max_T, self.hp.n_mels)
-        P = self._empty(B, self.hp.max_T, dtype=torch.int32)
-        M = self._empty(B, self.hp.max_T, dtype=torch.int32)
-        self._check(self._lib.dctts_text2mel_generate_path_host(self._h, _ptr(Ls), B, steps, C.c_void_p(ps.ctypes.data),
-                                                                C.c_void_p(ns.ctypes.data), _ptr(Y), _ptr(P), _ptr(M),
-                                                                self._stream()),
-                    "dctts_text2mel_generate_path_host")
+        perm = None if np.array_equal(order, np.arange(len(order))) else torch.as_tensor(order, device=self.device)
+        outs = decode(L if perm is None else L.index_select(0, perm).contiguous())
         self._decode_order = order
         if perm is None:
-            return Y, P, M
-        Yc, Pc, Mc = torch.empty_like(Y), torch.empty_like(P), torch.empty_like(M)
-        Yc[perm], Pc[perm], Mc[perm] = Y, P, M
-        return Yc, Pc, Mc
+            return outs
+        res = tuple(torch.empty_like(t) for t in outs)
+        for r, t in zip(res, outs):
+            r[perm] = t
+        return res
 
-    def _align_inputs(self, who, B, N, T, lengths, ends):
-        """Host int32 lengths (default all T) and ends (B,), checked as the entry points check them, naming the utterance."""
-        def host(x, default):
-            v = default if x is None else np.asarray(x.cpu() if isinstance(x, torch.Tensor) else x, np.int64).reshape(-1)
-            if v.shape[0] != B:
-                raise DcttsError("%s: %d values for %d utterances" % (who, v.shape[0], B))
-            return v
-        n, e = host(lengths, np.full(B, T, np.int64)), host(ends, None)
-        w = self.hp.attention_win_size
-        for b in range(B):
-            if not 1 <= n[b] <= T:
-                raise DcttsError("%s: utterance %d has length %d outside [1, %d]" % (who, b, n[b], T))
-            if e[b] < 0:
-                raise DcttsError("%s: utterance %d has no EOS (text end %d)" % (who, b, e[b]))
-            if e[b] >= N:
-                raise DcttsError("%s: utterance %d has text end %d outside [0, %d)" % (who, b, e[b], N))
-            if e[b] > (w - 1) * n[b]:
-                raise DcttsError("%s: utterance %d: its text end %d cannot be reached in %d frames with attention_win_size %d: "
-                                 "the text is too long for the recording" % (who, b, e[b], n[b], w))
-        return np.ascontiguousarray(n, np.int32), np.ascontiguousarray(e, np.int32)
+    def _align_inputs(self, who, B, T, lengths, ends):
+        """Host int32 lengths (default all T) and text ends (B,); the entry points check their ranges, naming the utterance."""
+        n = np.full(B, T) if lengths is None else _host_ints(who, lengths, B, "length")
+        return np.ascontiguousarray(n, np.int32), np.ascontiguousarray(_host_ints(who, ends, B, "text end"), np.int32)
 
     def _align_outputs(self, B, N, T):
         return (self._empty(B, T, dtype=torch.int32), self._empty(B, T, dtype=torch.int32),
@@ -552,7 +548,7 @@ class Engine:
         if A.dim() != 3:
             raise DcttsError("align_search: alignments must be (B, N, T), got shape %s" % (tuple(A.shape),))
         B, N, T = A.shape
-        n, e = self._align_inputs("align_search", B, N, T, lengths, ends)
+        n, e = self._align_inputs("align_search", B, T, lengths, ends)
         path, chars, dur, score = self._align_outputs(B, N, T)
         self._check(self._lib.dctts_align_search(self._h, _ptr(A), B, N, T, C.c_void_p(n.ctypes.data), C.c_void_p(e.ctypes.data),
                                                  _ptr(path), _ptr(chars), _ptr(dur), _ptr(score), self._stream()),
@@ -568,7 +564,7 @@ class Engine:
         score) as align_search does, and the alignments (B, max_N, T) when `want_alignments`."""
         from .data_load import eos_positions
         # Every host-side step comes before L is copied to the device (text2mel_generate_path explains why)
-        Lh = np.asarray(L.cpu() if isinstance(L, torch.Tensor) else L)
+        Lh = _host(L)
         if Lh.ndim != 2 or Lh.shape[1] != self.hp.max_N:
             raise DcttsError("text2mel_align: L must be (B, max_N=%d), got shape %s" % (self.hp.max_N, Lh.shape))
         B, N = Lh.shape
@@ -577,7 +573,7 @@ class Engine:
             raise DcttsError("text2mel_align: mels must be (B=%d, T <= max_T=%d, n_mels=%d), got shape %s"
                              % (B, self.hp.max_T, self.hp.n_mels, ms))
         T = ms[1]
-        n, e = self._align_inputs("text2mel_align", B, N, T, lengths, eos_positions(Lh) if ends is None else ends)
+        n, e = self._align_inputs("text2mel_align", B, T, lengths, eos_positions(Lh) if ends is None else ends)
         L, mels = self._i32(Lh), self._f32(mels)
         path, chars, dur, score = self._align_outputs(B, N, T)
         A = self._empty(B, N, T) if want_alignments else None
@@ -605,16 +601,8 @@ class Engine:
             raise DcttsError("mcd_dtw: empty batch or sequences: X %s, Y %s" % (tuple(X.shape), tuple(Y.shape)))
         if not 1 <= int(K) <= M - 1:
             raise DcttsError("mcd_dtw: K must be in [1, n_mels - 1 = %d], got %d" % (M - 1, int(K)))
-
-        def host(x, name, T):
-            v = np.asarray(x.cpu() if isinstance(x, torch.Tensor) else x, np.int64).reshape(-1)
-            if v.shape[0] != B:
-                raise DcttsError("mcd_dtw: %d %s lengths for %d utterances" % (v.shape[0], name, B))
-            bad = np.flatnonzero((v < 1) | (v > T))
-            if bad.size:
-                raise DcttsError("mcd_dtw: utterance %d has %s length %d outside [1, %d]" % (bad[0], name, v[bad[0]], T))
-            return np.ascontiguousarray(v, np.int32)
-        nxh, nyh = host(nx, "X", Tx), host(ny, "Y", Ty)
+        nxh = np.ascontiguousarray(_host_ints("mcd_dtw", nx, B, "X length"), np.int32)
+        nyh = np.ascontiguousarray(_host_ints("mcd_dtw", ny, B, "Y length"), np.int32)
         self._set_vocoder_params()
         mcd = self._empty(B, dtype=torch.float64)
         pairs = self._empty(B, dtype=torch.int32)
@@ -702,10 +690,7 @@ class Engine:
         trim = np.zeros((B, 2), np.int32)
         n = None
         if lengths is not None:
-            n = np.ascontiguousarray(np.asarray(lengths.cpu() if isinstance(lengths, torch.Tensor) else lengths).reshape(-1),
-                                     dtype=np.int32)
-            if n.shape[0] != B:
-                raise DcttsError("spectrogram2wav: %d lengths for %d utterances" % (n.shape[0], B))
+            n = np.ascontiguousarray(_host_ints("spectrogram2wav", lengths, B, "length"), np.int32)
         momentum = float(momentum)
         if momentum > 1:
             warnings.warn("Griffin-Lim with momentum=%g > 1 can be unstable. Proceed with caution!" % momentum, stacklevel=2)

@@ -168,9 +168,10 @@ int dctts_text2mel_generate_path_host(dctts_handle h, const int32_t* L, int32_t 
  * chars (B, T) int32 = n_t; path (B, T) int32 = the window of each frame, path[b, 0] = 0 and path[b, t] = n_{t-1}, as
  * dctts_text2mel_generate_path takes it; rows >= T_b are -1 in both; durations (B, N) int32 = frames per text position
  * (0 for a position the path steps over; they sum to T_b); score (B) float64 = the path's summed log-attention.
- * Refused before any launch, naming the utterance: T_b outside [1, T], e_b outside [0, N), e_b > (w - 1) T_b (the text
- * is too long for the recording), or 2 (e_b + 1) doubles beyond the device's shared memory per block.  The lengths and
- * ends are read on the host; the search is one launch for the batch, with no host synchronisation. */
+ * Refused before any launch, naming the utterance: T_b outside [1, T], e_b < 0 (the text has no EOS), e_b >= N,
+ * e_b > (w - 1) T_b (the text is too long for the recording), or 2 (e_b + 1) doubles beyond the device's shared memory
+ * per block.  The lengths and ends are read on the host; the search is one launch for the batch, with no host
+ * synchronisation. */
 int dctts_align_search(dctts_handle h, const float* alignments, int32_t B, int32_t N, int32_t T,
                        const int32_t* lengths_host, const int32_t* ends_host,
                        int32_t* path, int32_t* chars, int32_t* durations, double* score, void* stream);
