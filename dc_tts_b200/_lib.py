@@ -65,6 +65,9 @@ SIGNATURES = {
     "dctts_spectrogram2wav_ragged": (C.c_int, [Handle, _p, _i32, _i32, _p, _i32, _p, _p, _p]),
     "dctts_spectrogram2wav_momentum": (C.c_int, [Handle, _p, _i32, _i32, _p, _i32, C.c_double, _p, _p, _p, _p]),
     "dctts_vocoder_momentum_step": (C.c_int, [Handle, _i32, _i32, _p, _p, _p, _p, C.c_double, _p, _p]),
+    "dctts_vocoder_stream_open": (C.c_int, [Handle, _i32, _i32, _i32, C.c_double, _p, C.POINTER(_p)]),
+    "dctts_vocoder_stream_push": (C.c_int, [_p, _p, _i32, _p, _p, _p, _i64, _p]),
+    "dctts_vocoder_stream_close": (C.c_int, [_p, _p]),
     "dctts_get_spectrograms": (C.c_int, [Handle, _p, _i64, _i32, _p, _p, _i32, C.POINTER(_i32), C.POINTER(_i32), _p]),
     "dctts_load_spectrograms_batch": (C.c_int, [Handle, _p, _i32, C.POINTER(_i64), _i32, _i32, _p, _p, _i32, C.POINTER(_i32),
                                                 C.POINTER(_i32), C.POINTER(_i32), _p]),

@@ -207,7 +207,186 @@ void griffin_lim(H* h, const char* fn, const float* mag, int B, int T, const int
 
 }  // namespace
 
+// Look-ahead margin of the streaming vocoder, in frames: a push commits up to the support start of frame t_r - M, t_r the
+// first frame whose window reaches the prefix's reflected tail.  The smallest of {0, 2, 4, 8} whose streamed spectral
+// convergence stays within 1.5x of whole-signal Griffin-Lim (DESIGN.md section 8i)
+constexpr int VOC_STREAM_MARGIN = 0;
+
+// One vocoder stream: the Griffin-Lim state of B utterances of up to T frames, the de-emphasised waveform they committed,
+// and the host's account of each utterance (frames received, samples committed, final).
+struct dctts_vocoder_stream_s {
+    H* h = nullptr;
+    cudaStream_t s = nullptr;
+    int B = 0, T = 0, F = 0, n_iter = 0;
+    float alpha = 0.f;
+    DevBuf S, X, E, frames, y, wav, mse, tw, window, wss, wsq, deemph, state, meta;
+    std::vector<int> A, c, ended;
+    VocoderArgs args;          // the buffers and tables; each push fills the per-step bounds
+};
+
+namespace {
+
+// Window support of frame t in the centre-trimmed signal: [hop t + a0, hop t + a1)
+struct VocSupport { int a0, a1; };
+VocSupport voc_support(int n_fft, int win) {
+    const int lpad = (n_fft - win) / 2;
+    return {lpad - n_fft / 2, lpad + win - n_fft / 2};
+}
+
+// The first frame whose window reaches a sample >= c: the frames below touch only committed samples
+int voc_first_active(int c, int hop, VocSupport w) { return c < w.a1 ? 0 : (c - w.a1) / hop + 1; }
+
+// The committed sample count after a step over A frames from c (tests/ref_stream_vocoder.py: commit_end)
+int voc_commit_end(int c, int A, bool final, int hop, VocSupport w) {
+    const int Ly = hop * (A - 1);
+    if (final) return Ly;
+    const int t_r = std::max(0, (Ly - w.a1 + 1 + hop - 1) / hop);     // first frame reading a sample >= Ly (reflected)
+    return std::min(Ly, std::max(c, hop * (t_r - VOC_STREAM_MARGIN) + w.a0));
+}
+
+void vocoder_stream_open(H* h, int B, int T, int n_iter, double momentum, cudaStream_t s, dctts_vocoder_stream* out) {
+    const std::string fn = "dctts_vocoder_stream_open";
+    REQUIRE(out, fn + ": out is required");
+    REQUIRE(B >= 1 && T >= 2, fn + ": need B >= 1 and T_cap >= 2 frames, got B = " + std::to_string(B) + ", T_cap = " +
+                              std::to_string(T));
+    require_fft_size(h, fn);
+    auto vs = std::make_unique<dctts_vocoder_stream_s>();
+    vs->h = h; vs->s = s; vs->B = B; vs->T = T; vs->F = h->F;
+    vs->n_iter = n_iter >= 0 ? n_iter : h->voc.n_iter;
+    vs->alpha = momentum_alpha(fn, momentum);
+    const int F = h->F, n_fft = 2 * (F - 1), win = h->voc.win, hop = h->voc.hop, Ly = hop * (T - 1);
+    const size_t n = (size_t)B * T * F;
+    vs->S.ensure(n * sizeof(float)); vs->X.ensure(n * sizeof(float2)); vs->E.ensure(n * sizeof(float2));
+    vs->frames.ensure((size_t)B * T * win * sizeof(float));
+    vs->y.ensure((size_t)B * Ly * sizeof(float)); vs->wav.ensure((size_t)B * Ly * sizeof(float));
+    vs->mse.ensure((size_t)B * (1 + Ly / 512) * sizeof(float));
+    vs->deemph.ensure(voc_deemph_scratch_bytes(B, T, hop)); vs->state.ensure((size_t)B * sizeof(double));
+    vs->meta.ensure((size_t)B * 6 * sizeof(int));
+    vs->tw.ensure(n_fft * sizeof(float2)); vs->window.ensure(win * sizeof(float));
+    vs->wss.ensure((size_t)(n_fft + Ly) * sizeof(float)); vs->wsq.ensure(n_fft * sizeof(float));
+    voc_make_tables(n_fft, vs->tw.as<float2>(), vs->window.as<float>(), vs->wss.as<float>(), T, win, hop, s, vs->wsq.as<float>());
+    // est_{-1} = 0 for every frame: a frame's E is written only once it has been active, so this covers every new frame
+    CUDA_CHECK(cudaMemsetAsync(vs->E.p, 0, n * sizeof(float2), s));
+    CUDA_CHECK(cudaMemsetAsync(vs->y.p, 0, (size_t)B * Ly * sizeof(float), s));
+    CUDA_CHECK(cudaMemsetAsync(vs->wav.p, 0, (size_t)B * Ly * sizeof(float), s));
+    CUDA_CHECK(cudaMemsetAsync(vs->state.p, 0, (size_t)B * sizeof(double), s));
+    VocoderArgs& a = vs->args;
+    a = VocoderArgs{};
+    a.S = vs->S.as<float>(); a.X = vs->X.as<float2>(); a.frames = vs->frames.as<float>(); a.wav = vs->y.as<float>();
+    a.mse = vs->mse.as<float>(); a.tw = vs->tw.as<float2>(); a.window = vs->window.as<float>(); a.wss = vs->wss.as<float>();
+    a.wsq = vs->wsq.as<float>(); a.deemph = vs->deemph.as<double>(); a.B = B; a.T = T; a.F = F; a.win = win; a.hop = hop;
+    a.n_iter = vs->n_iter; a.max_db = h->voc.max_db; a.ref_db = h->voc.ref_db; a.power = h->voc.power;
+    a.preemphasis = h->voc.preemph;
+    if (vs->alpha != 0.f) { a.E = vs->E.as<float2>(); a.alpha = vs->alpha; }
+    int* m = vs->meta.as<int>();          // lengths, new_lo, frame_lo, sample_lo (B each), span (B int2)
+    a.lengths = m; a.new_lo = m + B; a.frame_lo = m + 2 * B; a.sample_lo = m + 3 * B;
+    a.span = reinterpret_cast<const int2*>(m + 4 * B); a.state = vs->state.as<double>();
+    vs->A.assign(B, 0); vs->c.assign(B, 0); vs->ended.assign(B, 0);
+    CUDA_CHECK(cudaGetLastError());
+    *out = vs.release();
+}
+
+void vocoder_stream_push(dctts_vocoder_stream vs, const float* mag, int R, const int32_t* rows, const int32_t* final_host,
+                         float* wav_out, int64_t ld, int32_t* counts) {
+    const std::string fn = "dctts_vocoder_stream_push";
+    REQUIRE(rows && counts && R >= 0 && (mag || R == 0) && (wav_out || ld == 0) && ld >= 0, fn + ": bad arguments");
+    const int B = vs->B, T = vs->T, hop = vs->args.hop, Ly_row = hop * (T - 1);
+    const VocSupport w = voc_support(2 * (vs->F - 1), vs->args.win);
+    require_each(fn, "row count", rows, B, 0, R);
+    // lengths, new_lo, frame_lo, sample_lo, span: utterances without a step get empty ranges
+    std::vector<int> m((size_t)B * 6);
+    std::vector<int> c_new(vs->c);
+    int n_active = 0, n_samples = 0, n_span = 0, stepping = 0;
+    for (int b = 0; b < B; ++b) {
+        const std::string who = fn + ": utterance " + std::to_string(b);
+        const bool fin = final_host && final_host[b];
+        REQUIRE(!vs->ended[b] || (rows[b] == 0 && !fin), who + " has had its final push");
+        const int A = vs->A[b] + rows[b];
+        REQUIRE(A <= T, who + " would have " + std::to_string(A) + " frames, past T_cap = " + std::to_string(T));
+        REQUIRE(!fin || A >= 2, who + " ends with " + std::to_string(A) + " frame(s); an utterance needs at least 2");
+        m[b] = A; m[B + b] = vs->A[b];
+        m[2 * B + b] = T; m[3 * B + b] = Ly_row; m[4 * B + 2 * b] = m[4 * B + 2 * b + 1] = vs->c[b];
+        if ((rows[b] > 0 || fin) && A >= 2) {
+            const int lo = voc_first_active(vs->c[b], hop, w), Ly = hop * (A - 1);
+            c_new[b] = voc_commit_end(vs->c[b], A, fin, hop, w);
+            m[2 * B + b] = lo; m[3 * B + b] = vs->c[b]; m[4 * B + 2 * b + 1] = c_new[b];
+            n_active = std::max(n_active, A - lo);
+            n_samples = std::max(n_samples, Ly - vs->c[b]);
+            n_span = std::max(n_span, c_new[b] - vs->c[b]);
+            ++stepping;
+        }
+        REQUIRE(c_new[b] - vs->c[b] <= ld, who + " commits " + std::to_string(c_new[b] - vs->c[b]) + " samples, past ld = " +
+                                           std::to_string(ld));
+    }
+    H* h = vs->h;
+    cudaStream_t s = vs->s;
+    VocoderArgs a = vs->args;
+    a.mag = mag; a.n_new = R; a.n_active = n_active; a.n_samples = n_samples; a.n_span = n_span;
+    CUDA_CHECK(cudaMemcpyAsync(vs->meta.p, m.data(), m.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    if (R > 0) { voc_prepare(a, s); h->launches += 1; }
+    if (stepping) {
+        for (int it = 0; it <= a.n_iter; ++it) {
+            voc_istft(a, s);
+            if (it < a.n_iter) voc_stft_phase(a, s, it);
+        }
+        h->launches += 3 * a.n_iter + 2;
+    }
+    if (n_span > 0) {
+        a.deemph_in = vs->y.as<float>(); a.wav = vs->wav.as<float>();
+        voc_deemph(a, s);
+        h->launches += 3;
+    }
+    for (int b = 0; b < B; ++b) {
+        counts[b] = c_new[b] - vs->c[b];
+        if (counts[b] > 0)
+            CUDA_CHECK(cudaMemcpyAsync(wav_out + (size_t)b * ld, vs->wav.as<float>() + (size_t)b * Ly_row + vs->c[b],
+                                       (size_t)counts[b] * sizeof(float), cudaMemcpyDeviceToDevice, s));
+        vs->A[b] += rows[b];
+        vs->c[b] = c_new[b];
+        if (final_host && final_host[b]) vs->ended[b] = 1;
+    }
+    CUDA_CHECK(cudaGetLastError());
+}
+
+void vocoder_stream_trims(dctts_vocoder_stream vs, int32_t* trim_host) {
+    const int B = vs->B;
+    for (int b = 0; b < B; ++b)
+        REQUIRE(vs->ended[b], "dctts_vocoder_stream_close: utterance " + std::to_string(b) + " has not had its final push, so "
+                              "it has no trim");
+    VocoderArgs a = vs->args;
+    a.wav = vs->wav.as<float>();
+    CUDA_CHECK(cudaMemcpyAsync(vs->meta.p, vs->A.data(), B * sizeof(int), cudaMemcpyHostToDevice, vs->s));
+    voc_energies(a, vs->s);
+    vs->h->launches += 1;
+    CUDA_CHECK(cudaGetLastError());
+    voc_trims(a, trim_host, vs->s, vs->A.data());
+}
+
+}  // namespace
+
 extern "C" {
+
+int dctts_vocoder_stream_open(dctts_handle h, int32_t B, int32_t T_cap, int32_t n_iter, double momentum, void* stream,
+                              dctts_vocoder_stream* out) {
+    return guarded(h, [&] { vocoder_stream_open(h, B, T_cap, n_iter, momentum, S(h, stream), out); });
+}
+
+int dctts_vocoder_stream_push(dctts_vocoder_stream vs, const float* mag, int32_t R, const int32_t* rows_host,
+                              const int32_t* final_host, float* wav, int64_t ld, int32_t* counts_host) {
+    if (!vs) { g_create_error = "null vocoder stream"; return 1; }
+    return guarded(vs->h, [&] { vocoder_stream_push(vs, mag, R, rows_host, final_host, wav, ld, counts_host); });
+}
+
+int dctts_vocoder_stream_close(dctts_vocoder_stream vs, int32_t* trim_host) {
+    if (!vs) { g_create_error = "null vocoder stream"; return 1; }
+    const int rc = guarded(vs->h, [&] {
+        if (trim_host) vocoder_stream_trims(vs, trim_host);
+        else CUDA_CHECK(cudaStreamSynchronize(vs->s));
+    });
+    if (rc != 0) cudaStreamSynchronize(vs->s);      // the buffers go now: nothing queued may still use them
+    delete vs;
+    return rc;
+}
 
 int dctts_set_vocoder_params(dctts_handle h, int32_t hop_length, int32_t win_length, float power, float max_db,
                              float ref_db, double preemphasis, int32_t n_iter) {

@@ -138,6 +138,22 @@ struct VocoderArgs {
     // Null part: no convergence, and no extra STFT of the final waveform.
     float* part;
     double* conv;
+    // streaming step (dctts_vocoder_stream_push; null / 0 in every whole-signal call, which then launches the kernels'
+    // STREAM = false instantiations, compiled to the code they had before these bounds existed).  lengths[b]
+    // is the frames utterance b has received, and the launches cover only what the step changes, from (B) DEVICE bounds:
+    //   prepare   mag (B, n_new, F) holds frames [new_lo[b], new_lo[b] + n_new); those below lengths[b] (not clamped) are set
+    //   istft, stft_phase  frames [frame_lo[b], lengths[b]): n_active CTAs per utterance, frame frame_lo[b] + blockIdx.x
+    //   ola       samples [sample_lo[b], hop (lengths[b] - 1)): n_samples per utterance; the samples below stay as they are
+    //   deemph    samples [span[b].x, span[b].y) of deemph_in (B, Ly) into wav, from the float64 state state[b] (the output
+    //             before span[b].x), which is replaced by the state at span[b].y - 1; n_span >= the longest span
+    const int* new_lo;
+    const int* frame_lo;
+    const int* sample_lo;
+    int n_new, n_active, n_samples;
+    const int2* span;
+    const float* deemph_in;
+    double* state;
+    int n_span;
 };
 // n_fft 1024, 2048 and 4096 have kernel instantiations (F = 1 + n_fft / 2 = 513, 1025, 2049); the launchers take n_fft
 // from F and throw for any other size

@@ -117,32 +117,46 @@ __global__ void voc_twiddle_kernel(float2* tw) {
 }
 
 // utils.py:78-85: amplitude target S = (10 ^ ((clip(z,0,1)*max_db - max_db + ref_db) * 0.05)) ^ power; X <- S (zero phase)
+// STREAM (a streaming step, new_lo set): i runs over mag (B, n_new, F), whose row j of utterance b is frame new_lo[b] + j;
+// the frames at or past lengths[b] are left alone.  Every vocoder kernel with a STREAM parameter compiles its STREAM = false
+// instantiation, which the whole-signal calls launch, to the code it had before the streaming bounds existed.
+template <bool STREAM>
 __global__ void voc_prepare_kernel(const float* __restrict__ mag, float* __restrict__ S, float2* __restrict__ X, long long n,
-                                   float max_db, float ref_db, float power, const int* __restrict__ lengths, int T, int F) {
+                                   float max_db, float ref_db, float power, const int* __restrict__ lengths, int T, int F,
+                                   const int* __restrict__ new_lo, int n_new) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    if (lengths) {                                       // rows past the utterance's frames: not read, zero
+    long long o = i;                                     // the element of S and X
+    if constexpr (STREAM) {
+        const long long row = i / F;
+        const int b = (int)(row / n_new), t = __ldg(new_lo + b) + (int)(row % n_new);
+        if (t >= min(__ldg(lengths + b), T)) return;
+        o = ((long long)b * T + t) * F + i % F;
+    } else if (lengths) {                                // rows past the utterance's frames: not read, zero
         const long long row = i / F;
         if ((int)(row % T) >= voc_frames_of(lengths, (int)(row / T), T)) { S[i] = 0.f; X[i] = make_float2(0.f, 0.f); return; }
     }
     float m = fminf(fmaxf(mag[i], 0.f), 1.f) * max_db - max_db + ref_db;
     float v = powf(powf(10.0f, m * 0.05f), power);
-    S[i] = v;
-    X[i] = make_float2(v, 0.f);
+    S[o] = v;
+    X[o] = make_float2(v, 0.f);
 }
 
 // librosa.core.istft, one frame: grid (T, B).  fr: (B, T, win) windowed time-domain frames.
 // The N-point Hermitian inverse is an N/2-point complex one: with E/O the spectra of the even/odd
 // samples, X[k] = E[k] + W^k O[k], X[k+N/2] = conj(X[N/2-k]) = E[k] - W^k O[k]; z = IFFT(E + i O)
 // carries x[2n] in its real and x[2n+1] in its imaginary part.
-template <int N>
+// STREAM: frames frame_lo[b] + blockIdx.x.
+template <int N, bool STREAM>
 __global__ void __launch_bounds__(VcSize<N>::THREADS, VcSize<N>::ISTFT_MIN_BLOCKS)
 voc_istft_kernel(const float2* __restrict__ X, float* __restrict__ fr, const float2* __restrict__ tw, const float* __restrict__ window,
-                 int T, int F, int win, int lpad, const int* __restrict__ lengths) {
+                 int T, int F, int win, int lpad, const int* __restrict__ lengths, const int* __restrict__ frame_lo) {
     constexpr int H = VcSize<N>::H, NT = VcSize<N>::THREADS;
     __shared__ __align__(16) float2 s0[H];
     __shared__ __align__(16) float2 s1[H];
-    const int t = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
+    const int b = blockIdx.y, tid = threadIdx.x;
+    int t = blockIdx.x;
+    if constexpr (STREAM) t += __ldg(frame_lo + b);
     if (t >= voc_frames_of(lengths, b, T)) return;       // whole CTA
     const float2* x = X + ((size_t)b * T + t) * F;
     float2 v[4];
@@ -171,11 +185,14 @@ voc_istft_kernel(const float2* __restrict__ X, float* __restrict__ fr, const flo
 // Tb frames and Ly_b = hop*(Tb-1) samples, the rest of its row is 0.  The table wss (T frames) equals the sum-square of Tb
 // frames below Tb*hop + lpad (the later frames add zeros of the squared window there, which is exact); above it the
 // sum is formed here from wsq, over frames < Tb in ascending order in float32 like voc_make_tables.
-template <int N>
+// STREAM: samples sample_lo[b] + blockIdx.x * blockDim.x + threadIdx.x.
+template <int N, bool STREAM>
 __global__ void voc_ola_kernel(const float* __restrict__ fr, const float* __restrict__ wss, float* __restrict__ y,
                                int T, int win, int lpad, int hop, int Ly, float tiny, const int* __restrict__ lengths,
-                               const float* __restrict__ wsq) {
-    const int sidx = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
+                               const float* __restrict__ wsq, const int* __restrict__ sample_lo) {
+    const int b = blockIdx.y;
+    int sidx = blockIdx.x * blockDim.x + threadIdx.x;
+    if constexpr (STREAM) sidx += __ldg(sample_lo + b);
     if (sidx >= Ly) return;
     const int Tb = voc_frames_of(lengths, b, T);
     if (sidx >= hop * (Tb - 1)) { y[(size_t)b * Ly + sidx] = 0.f; return; }
@@ -207,16 +224,20 @@ __global__ void voc_ola_kernel(const float* __restrict__ fr, const float* __rest
 // est[k] over it and updates with c = est - alpha E[k] (a float32 product, then a float32 difference, as numpy forms it for
 // complex64): X = S * c / max(1e-8, |c|).  CONV: the frame's sum_k (S - |est|)^2 goes to part[b * T + t], summed in a fixed
 // order (each thread's bins in ascending order, a warp butterfly, then the warp sums in ascending order; no atomics).
-template <int N, bool MOM, bool CONV>
+// STREAM: frames frame_lo[b] + blockIdx.x.
+template <int N, bool MOM, bool CONV, bool STREAM>
 __global__ void __launch_bounds__(VcSize<N>::THREADS) voc_stft_phase_kernel(const float* __restrict__ y, const float* __restrict__ S,
                                                                            float2* __restrict__ X, const float2* __restrict__ tw,
                                                                            const float* __restrict__ window, int T, int F, int win,
                                                                            int lpad, int hop, int Ly, const int* __restrict__ lengths,
-                                                                           float2* __restrict__ E, float alpha, float* __restrict__ part) {
+                                                                           float2* __restrict__ E, float alpha, float* __restrict__ part,
+                                                                           const int* __restrict__ frame_lo) {
     constexpr int H = VcSize<N>::H, NT = VcSize<N>::THREADS;
     __shared__ __align__(16) float2 s0[H];
     __shared__ __align__(16) float2 s1[H];
-    const int t = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
+    int t = blockIdx.x;
+    const int b = blockIdx.y, tid = threadIdx.x;
+    if constexpr (STREAM) t += __ldg(frame_lo + b);
     const int Tb = voc_frames_of(lengths, b, T), Lyb = hop * (Tb - 1);
     if (t >= Tb) return;                                            // whole CTA
     const float* yb = y + (size_t)b * Ly;
@@ -295,7 +316,7 @@ __global__ void __launch_bounds__(VcSize<N>::THREADS) voc_stft_phase_kernel(cons
 }
 
 // Spectral convergence ||S - |est_i||| / ||S|| of utterance b for i < n_hist: conv (B, n_hist) float64.  part (n_hist, B, T)
-// holds the per-frame sums of voc_stft_phase_kernel<N, *, true>; frames t < T_b are summed in ascending order in float64.
+// holds the per-frame sums of voc_stft_phase_kernel<N, *, true, false>; frames t < T_b are summed in ascending order in float64.
 // sum S^2 over the utterance's rows is formed once, in float64, each thread over a fixed stride, then a fixed tree.
 // grid B, 256 threads.
 __global__ void __launch_bounds__(256) voc_convergence_kernel(const float* __restrict__ S, const float* __restrict__ part,
@@ -334,39 +355,68 @@ __device__ __forceinline__ int voc_samples_of(const int* __restrict__ lengths, i
     return hop * (voc_frames_of(lengths, b, T) - 1);
 }
 
+// A streaming de-emphasis's samples of row b: (first, count) from span[b] = [first, end)
+__device__ __forceinline__ int2 voc_deemph_range(const int2* __restrict__ span, int b) {
+    const int2 s = span[b];
+    return make_int2(s.x, s.y - s.x);
+}
+
+// STREAM: the span's samples (voc_deemph_range) instead of the utterance's
+template <bool STREAM>
 __global__ void voc_deemph_local_kernel(const float* __restrict__ y, double* __restrict__ ends, int Ly, int nch, double c,
-                                        const int* __restrict__ lengths, int T, int hop) {
+                                        const int* __restrict__ lengths, int T, int hop, const int2* __restrict__ span) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
-    const int Lyb = lengths ? voc_samples_of(lengths, b, T, hop) : Ly;
+    int first = 0, Lyb = lengths ? voc_samples_of(lengths, b, T, hop) : Ly;
+    if constexpr (STREAM) { const int2 r = voc_deemph_range(span, b); first = r.x; Lyb = r.y; }
     if (j >= (Lyb + DE_LC - 1) / DE_LC) return;
-    const float* p = y + (size_t)b * Ly + (size_t)j * DE_LC;
+    const float* p = y + (size_t)b * Ly + first + (size_t)j * DE_LC;
     const int n = min(DE_LC, Lyb - j * DE_LC);
     double acc = 0.0;
     for (int i = 0; i < n; ++i) acc = (double)p[i] + c * acc;
     ends[(size_t)b * nch + j] = acc;
 }
 
+// STREAM: the span's chunks, and the carry into the first chunk is state[b] instead of 0
+template <bool STREAM>
 __global__ void voc_deemph_carry_kernel(double* __restrict__ ends, int nch, int B, double c, const int* __restrict__ lengths, int T,
-                                        int hop) {
+                                        int hop, const int2* __restrict__ span, const double* __restrict__ state) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= B) return;
     double cl = 1.0;
     for (int i = 0; i < DE_LC; ++i) cl *= c;
     double* e = ends + (size_t)b * nch;
     double carry = 0.0;
-    const int nchb = lengths ? (voc_samples_of(lengths, b, T, hop) + DE_LC - 1) / DE_LC : nch;
+    int nchb = lengths ? (voc_samples_of(lengths, b, T, hop) + DE_LC - 1) / DE_LC : nch;
+    if constexpr (STREAM) { carry = state[b]; nchb = (voc_deemph_range(span, b).y + DE_LC - 1) / DE_LC; }
     for (int j = 0; j < nchb; ++j) { const double local = e[j]; e[j] = carry; carry = local + cl * carry; }
 }
 
+// STREAM: the span's samples of `in` (another buffer than y) into y, and the last chunk's thread stores the state after its
+// last sample; else y in place.
+template <bool STREAM>
 __global__ void voc_deemph_apply_kernel(float* __restrict__ y, const double* __restrict__ carry, int Ly, int nch, double c,
-                                        const int* __restrict__ lengths, int T, int hop) {
+                                        const int* __restrict__ lengths, int T, int hop, const int2* __restrict__ span,
+                                        const float* __restrict__ in, double* __restrict__ state) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
-    const int Lyb = lengths ? voc_samples_of(lengths, b, T, hop) : Ly;
-    if (j >= (Lyb + DE_LC - 1) / DE_LC) return;
-    float* p = y + (size_t)b * Ly + (size_t)j * DE_LC;
-    const int n = min(DE_LC, Lyb - j * DE_LC);
-    double acc = carry[(size_t)b * nch + j];
-    for (int i = 0; i < n; ++i) { acc = (double)p[i] + c * acc; p[i] = (float)acc; }
+    if constexpr (STREAM) {
+        const int2 r = voc_deemph_range(span, b);
+        const int Lyb = r.y;
+        if (j >= (Lyb + DE_LC - 1) / DE_LC) return;
+        const size_t o = (size_t)b * Ly + r.x + (size_t)j * DE_LC;
+        float* p = y + o;
+        const float* q = in + o;
+        const int n = min(DE_LC, Lyb - j * DE_LC);
+        double acc = carry[(size_t)b * nch + j];
+        for (int i = 0; i < n; ++i) { acc = (double)q[i] + c * acc; p[i] = (float)acc; }
+        if ((j + 1) * DE_LC >= Lyb) state[b] = acc;
+    } else {
+        const int Lyb = lengths ? voc_samples_of(lengths, b, T, hop) : Ly;
+        if (j >= (Lyb + DE_LC - 1) / DE_LC) return;
+        float* p = y + (size_t)b * Ly + (size_t)j * DE_LC;
+        const int n = min(DE_LC, Lyb - j * DE_LC);
+        double acc = carry[(size_t)b * nch + j];
+        for (int i = 0; i < n; ++i) { acc = (double)p[i] + c * acc; p[i] = (float)acc; }
+    }
 }
 
 // A waveform sample as float32: float input as is, int16 PCM as value / 32768 (exact: what utils._load_wav returns)
@@ -724,19 +774,23 @@ size_t voc_deemph_scratch_bytes(int B, int T, int hop) { return (size_t)B * ((ho
 
 // The stages of voc_run, each a fixed sequence of launches (dctts_vocoder_stage runs them one at a time).
 void voc_prepare(const VocoderArgs& a, cudaStream_t s) {
-    const long long n = (long long)a.B * a.T * a.F;
-    voc_prepare_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a.mag, a.S, a.X, n, a.max_db, a.ref_db, a.power, a.lengths,
-                                                                   a.T, a.F);
+    const long long n = (long long)a.B * (a.new_lo ? a.n_new : a.T) * a.F;
+    auto kern = a.new_lo ? voc_prepare_kernel<true> : voc_prepare_kernel<false>;
+    kern<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a.mag, a.S, a.X, n, a.max_db, a.ref_db, a.power, a.lengths, a.T, a.F, a.new_lo,
+                                                     a.n_new);
 }
 
 void voc_istft(const VocoderArgs& a, cudaStream_t s) {
     voc_dispatch(2 * (a.F - 1), [&](auto n) {
         constexpr int N = decltype(n)::value;
         const int Ly = a.hop * (a.T - 1), lpad = (N - a.win) / 2;
-        voc_istft_kernel<N><<<dim3(a.T, a.B), VcSize<N>::THREADS, 0, s>>>(a.X, a.frames, a.tw, a.window, a.T, a.F, a.win, lpad,
-                                                                              a.lengths);
-        voc_ola_kernel<N><<<dim3((Ly + 255) / 256, a.B), 256, 0, s>>>(a.frames, a.wss, a.wav, a.T, a.win, lpad, a.hop, Ly,
-                                                                     1.17549435e-38f, a.lengths, a.wsq);
+        const bool st = a.frame_lo != nullptr;           // a streaming step sets frame_lo and sample_lo together
+        const int nt = st ? a.n_active : a.T, ns = st ? a.n_samples : Ly;
+        auto istft = st ? voc_istft_kernel<N, true> : voc_istft_kernel<N, false>;
+        auto ola = st ? voc_ola_kernel<N, true> : voc_ola_kernel<N, false>;
+        istft<<<dim3(nt, a.B), VcSize<N>::THREADS, 0, s>>>(a.X, a.frames, a.tw, a.window, a.T, a.F, a.win, lpad, a.lengths, a.frame_lo);
+        ola<<<dim3((ns + 255) / 256, a.B), 256, 0, s>>>(a.frames, a.wss, a.wav, a.T, a.win, lpad, a.hop, Ly, 1.17549435e-38f,
+                                                       a.lengths, a.wsq, a.sample_lo);
     });
 }
 
@@ -746,13 +800,15 @@ void voc_stft_phase(const VocoderArgs& a, cudaStream_t s, int it) {
         constexpr int N = decltype(n)::value;
         const int Ly = a.hop * (a.T - 1), lpad = (N - a.win) / 2;
         auto launch = [&](auto kern) {
-            kern<<<dim3(a.T, a.B), VcSize<N>::THREADS, 0, s>>>(a.wav, a.S, a.X, a.tw, a.window, a.T, a.F, a.win, lpad, a.hop, Ly,
-                                                               a.lengths, a.E, a.alpha, part);
+            kern<<<dim3(a.frame_lo ? a.n_active : a.T, a.B), VcSize<N>::THREADS, 0, s>>>(
+                a.wav, a.S, a.X, a.tw, a.window, a.T, a.F, a.win, lpad, a.hop, Ly, a.lengths, a.E, a.alpha, part, a.frame_lo);
         };
-        if (a.E) {
-            if (part) launch(voc_stft_phase_kernel<N, true, true>); else launch(voc_stft_phase_kernel<N, true, false>);
+        if (a.frame_lo) {                              // a streaming step keeps no convergence history
+            if (a.E) launch(voc_stft_phase_kernel<N, true, false, true>); else launch(voc_stft_phase_kernel<N, false, false, true>);
+        } else if (a.E) {
+            if (part) launch(voc_stft_phase_kernel<N, true, true, false>); else launch(voc_stft_phase_kernel<N, true, false, false>);
         } else {
-            if (part) launch(voc_stft_phase_kernel<N, false, true>); else launch(voc_stft_phase_kernel<N, false, false>);
+            if (part) launch(voc_stft_phase_kernel<N, false, true, false>); else launch(voc_stft_phase_kernel<N, false, false, false>);
         }
     });
 }
@@ -762,11 +818,15 @@ void voc_convergence(const VocoderArgs& a, cudaStream_t s) {
 }
 
 void voc_deemph(const VocoderArgs& a, cudaStream_t s) {
-    const int Ly = a.hop * (a.T - 1), nch = (Ly + DE_LC - 1) / DE_LC;
+    const int Ly = a.hop * (a.T - 1), nch = ((a.span ? a.n_span : Ly) + DE_LC - 1) / DE_LC;
     const dim3 gch((nch + 63) / 64, a.B);
-    voc_deemph_local_kernel<<<gch, 64, 0, s>>>(a.wav, a.deemph, Ly, nch, a.preemphasis, a.lengths, a.T, a.hop);
-    voc_deemph_carry_kernel<<<(a.B + 31) / 32, 32, 0, s>>>(a.deemph, nch, a.B, a.preemphasis, a.lengths, a.T, a.hop);
-    voc_deemph_apply_kernel<<<gch, 64, 0, s>>>(a.wav, a.deemph, Ly, nch, a.preemphasis, a.lengths, a.T, a.hop);
+    const bool st = a.span != nullptr;                   // a streaming step sets span, deemph_in and state together
+    auto local = st ? voc_deemph_local_kernel<true> : voc_deemph_local_kernel<false>;
+    auto carry = st ? voc_deemph_carry_kernel<true> : voc_deemph_carry_kernel<false>;
+    auto apply = st ? voc_deemph_apply_kernel<true> : voc_deemph_apply_kernel<false>;
+    local<<<gch, 64, 0, s>>>(st ? a.deemph_in : a.wav, a.deemph, Ly, nch, a.preemphasis, a.lengths, a.T, a.hop, a.span);
+    carry<<<(a.B + 31) / 32, 32, 0, s>>>(a.deemph, nch, a.B, a.preemphasis, a.lengths, a.T, a.hop, a.span, a.state);
+    apply<<<gch, 64, 0, s>>>(a.wav, a.deemph, Ly, nch, a.preemphasis, a.lengths, a.T, a.hop, a.span, a.deemph_in, a.state);
 }
 
 void voc_energies(const VocoderArgs& a, cudaStream_t s) {

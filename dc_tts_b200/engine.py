@@ -6,6 +6,7 @@ the C-ABI (include/dctts.h).  This object plays the role of the reference's
 """
 import ctypes as C
 import warnings
+import weakref
 
 import numpy as np
 import torch
@@ -68,9 +69,12 @@ class Engine:
             raise DcttsError("dctts_create: " + self._lib.dctts_last_error(None).decode())
         self._h = h
         self.params_loaded = False
+        self._streams = weakref.WeakSet()   # open VocoderStreams: closed before the handle they hold
 
     # ------------------------------------------------------------------ plumbing
     def close(self):
+        for vs in list(getattr(self, "_streams", ())):
+            vs._free()
         if getattr(self, "_h", None):
             self._lib.dctts_destroy(self._h)
             self._h = None
@@ -701,6 +705,20 @@ class Engine:
             trim.ctypes.data_as(C.c_void_p), _ptr(conv), self._stream()), "dctts_spectrogram2wav_momentum")
         return (wav, trim, conv) if convergence else (wav, trim)
 
+    def vocoder_stream(self, B, T_cap=None, n_iter=-1, momentum=0.0):
+        """Streaming Griffin-Lim (include/dctts.h: dctts_vocoder_stream_*) for B utterances of at most T_cap magnitude
+        frames (default hp.r * hp.max_T), with spectrogram2wav's n_iter and momentum.  Returns a VocoderStream:
+        push(mag, counts, final) appends counts[b] rows of mag (B, R, F) to utterance b and returns, per utterance, the
+        float32 numpy samples that became final; close() returns the trims (B, 2) as spectrogram2wav reports them.  The
+        samples of one utterance concatenate to spectrogram2wav's untrimmed waveform of its frames, bit for bit when
+        a single push delivers them all."""
+        T_cap = int(T_cap or self.hp.r * self.hp.max_T)
+        momentum = float(momentum)
+        if momentum > 1:
+            warnings.warn("Griffin-Lim with momentum=%g > 1 can be unstable. Proceed with caution!" % momentum, stacklevel=2)
+        self._set_vocoder_params()
+        return VocoderStream(self, int(B), T_cap, int(n_iter), momentum)
+
     def vocoder_momentum_step(self, wav, S, E, X, momentum, partials=None, hop=None, win=None):
         """Test aid (include/dctts.h: dctts_vocoder_momentum_step): ONE fast Griffin-Lim phase step on caller CUDA tensors.
         wav (B, Ly) and S (B, T, F) float32 in; E (B, T, F) complex64 holds est_{i-1} on entry and est_i on return;
@@ -1094,6 +1112,65 @@ class Engine:
 
 
 _default = None
+
+
+class VocoderStream:
+    """One dctts_vocoder_stream on an engine (Engine.vocoder_stream).  Its output buffer is allocated at open and every
+    call runs on the stream that was current then."""
+
+    def __init__(self, eng, B, T_cap, n_iter, momentum):
+        self._eng, self.B, self.T_cap = eng, B, T_cap
+        self.ld = eng.hp.hop_length * (T_cap - 1)           # the most samples one push can commit for an utterance
+        self._wav = eng._empty(B, self.ld)
+        self._tstream = torch.cuda.current_stream(eng.device)
+        self._stream = C.c_void_p(self._tstream.cuda_stream)
+        vs = C.c_void_p()
+        self._vs = None
+        eng._check(eng._lib.dctts_vocoder_stream_open(eng._h, B, T_cap, n_iter, momentum, self._stream, C.byref(vs)),
+                   "dctts_vocoder_stream_open")
+        self._vs = vs
+        eng._streams.add(self)
+
+    def push(self, mag, counts, final=False):
+        """mag (B, R, F) magnitudes (CUDA tensor or array), counts (B) rows of it per utterance, final: one flag or (B)
+        flags -> B float32 numpy arrays of newly committed samples."""
+        eng, B = self._eng, self.B
+        if self._vs is None:
+            raise DcttsError("dctts_vocoder_stream_push: the stream is closed")
+        mag = eng._f32(mag)
+        if mag.dim() != 3 or mag.shape[0] != B or mag.shape[2] != eng.F:
+            raise DcttsError("dctts_vocoder_stream_push: expected mag (%d, R, %d), got %s" % (B, eng.F, tuple(mag.shape)))
+        rows = np.ascontiguousarray(_host_ints("dctts_vocoder_stream_push", counts, B, "row count"), np.int32)
+        fin = np.ascontiguousarray(np.broadcast_to(np.asarray(final, bool), (B,)), np.int32)
+        n = np.zeros(B, np.int32)
+        eng._check(eng._lib.dctts_vocoder_stream_push(
+            self._vs, _ptr(mag), mag.shape[1], rows.ctypes.data_as(C.c_void_p), fin.ctypes.data_as(C.c_void_p),
+            _ptr(self._wav), self.ld, n.ctypes.data_as(C.c_void_p)), "dctts_vocoder_stream_push")
+        with torch.cuda.stream(self._tstream):
+            host = self._wav[:, :int(n.max(initial=0))].cpu().numpy()
+        return [host[b, :n[b]].copy() for b in range(B)]
+
+    def close(self):
+        """Frees the stream and returns the trims (B, 2) int32; DcttsError (the stream is freed all the same) when an
+        utterance has not had its final push."""
+        if self._vs is None:
+            return None
+        trim = np.zeros((self.B, 2), np.int32)
+        vs, self._vs = self._vs, None
+        self._eng._streams.discard(self)
+        rc = self._eng._lib.dctts_vocoder_stream_close(vs, trim.ctypes.data_as(C.c_void_p))
+        self._eng._check(rc, "dctts_vocoder_stream_close")
+        return trim
+
+    def _free(self):
+        """Frees the stream without trims (Engine.close and garbage collection); its engine's handle is still open."""
+        if getattr(self, "_vs", None) is not None:
+            vs, self._vs = self._vs, None
+            self._eng._streams.discard(self)
+            self._eng._lib.dctts_vocoder_stream_close(vs, None)
+
+    def __del__(self):
+        self._free()
 
 
 def get_engine():

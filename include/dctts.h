@@ -260,6 +260,33 @@ int dctts_spectrogram2wav_momentum(dctts_handle h, const float* mag, int32_t B, 
                                    int32_t n_iter, double momentum, float* wav, int32_t* trim_host, double* convergence,
                                    void* stream);
 
+/* Streaming Griffin-Lim (DESIGN.md section 8i): magnitude frames arrive in pieces, and each piece returns the samples
+ * that are final.  For each utterance with A frames received, a push runs dctts_spectrogram2wav_momentum's iterations on
+ * the prefix of A frames, with the samples already returned held at their values and only the frames that reach past
+ * them taking part (warm-started from the previous push); it then returns the samples up to a look-ahead margin before
+ * the prefix's end, or all of them once the utterance is final, de-emphasised from the float64 state the last push left.
+ * A stream owns its buffers and tables (sized at open for T_cap frames per utterance), takes the vocoder parameters of
+ * dctts_set_vocoder_params at open, and runs every launch on `stream`; close each stream before destroying its handle.
+ * Errors are reported by dctts_last_error(h). */
+typedef struct dctts_vocoder_stream_s* dctts_vocoder_stream;
+/* B utterances of at most T_cap >= 2 frames each; n_iter < 0 means the configured value; momentum as for
+ * dctts_spectrogram2wav_momentum.  *out receives the stream. */
+int dctts_vocoder_stream_open(dctts_handle h, int32_t B, int32_t T_cap, int32_t n_iter, double momentum, void* stream,
+                              dctts_vocoder_stream* out);
+/* Appends rows_host[b] frames of mag (B, R, F) DEVICE float32 (row j of utterance b is its next frame j, j < rows_host[b] <= R)
+ * and marks utterance b final where final_host[b] != 0 (final_host may be NULL: none).  One step runs for each utterance
+ * that received rows or became final and has at least 2 frames.  counts_host (B) HOST receives the samples it committed,
+ * and wav (B, ld) DEVICE float32 row b receives them, from its start; a count above ld fails the call before any launch.
+ * Fails, naming the utterance, when rows arrive for an utterance after its final push, when T_cap would be exceeded, or
+ * when a final utterance has fewer than 2 frames.  The returned samples concatenate, per utterance, to one waveform of
+ * hop (T_b - 1) samples, untrimmed; with a single final push it is dctts_spectrogram2wav_momentum's with
+ * lengths_host, bit for bit.  Asynchronous: the counts are known on the host, wav is written on `stream`. */
+int dctts_vocoder_stream_push(dctts_vocoder_stream vs, const float* mag, int32_t R, const int32_t* rows_host,
+                              const int32_t* final_host, float* wav, int64_t ld, int32_t* counts_host);
+/* trim_host: NULL, or (B, 2) HOST int32 receiving the [start, end) librosa.effects.trim keeps of each streamed waveform
+ * (every utterance must then be final).  Frees the stream whether or not the trims could be formed; synchronises `stream`. */
+int dctts_vocoder_stream_close(dctts_vocoder_stream vs, int32_t* trim_host);
+
 /* Feature extraction (next row, SURVEY 8f-4): get_spectrograms -- utils.py:20-65 -- for ONE utterance from the
  * loaded waveform on: trim (librosa.effects.trim), pre-emphasis, STFT, |.|, mel filterbank
  * (librosa.filters.mel(sample_rate, n_fft, n_mels)), 20 log10, normalisation with the constants of
