@@ -68,6 +68,11 @@ SIGNATURES = {
     "dctts_vocoder_stream_open": (C.c_int, [Handle, _i32, _i32, _i32, C.c_double, _p, C.POINTER(_p)]),
     "dctts_vocoder_stream_push": (C.c_int, [_p, _p, _i32, _p, _p, _p, _i64, _p]),
     "dctts_vocoder_stream_close": (C.c_int, [_p, _p]),
+    "dctts_ssrn_halo": (C.c_int, [Handle, C.POINTER(_i32), C.POINTER(_i32)]),
+    "dctts_ssrn_windows": (C.c_int, [Handle, _p, _i32, _i32, _p, _p, _p, _p, _i32, _p]),
+    "dctts_synth_stream_open": (C.c_int, [Handle, _p, _i32, _p, _i32, _i32, _i32, C.c_double, _p, C.POINTER(_p)]),
+    "dctts_synth_stream_poll": (C.c_int, [_p, _i32, _p, _i64, _p, _p, _p]),
+    "dctts_synth_stream_close": (C.c_int, [_p, _p, _p, _p, _p, _p]),
     "dctts_get_spectrograms": (C.c_int, [Handle, _p, _i64, _i32, _p, _p, _i32, C.POINTER(_i32), C.POINTER(_i32), _p]),
     "dctts_load_spectrograms_batch": (C.c_int, [Handle, _p, _i32, C.POINTER(_i64), _i32, _i32, _p, _p, _i32, C.POINTER(_i32),
                                                 C.POINTER(_i32), C.POINTER(_i32), _p]),

@@ -17,6 +17,7 @@
 #include <stdexcept>
 #include <string>
 #include <utility>
+#include <thread>
 #include <vector>
 
 using namespace dctts;
@@ -210,7 +211,12 @@ struct dctts_handle_s {
         int train_tc = 7;         // training GEMMs on wgmma, bit mask: 1 forward conv, 2 data gradient, 4 weight gradient; 0 = fp32 CUDA-core kernels
         int train_deterministic = 0;   // 1: the training step's sums in a fixed order (kernels_ordered.cu): a seeded run repeats bit for bit
         int chain_history = 0;    // test aid: the full-sequence chains copy every block's rows for dctts_chain_history
+        int decode_group = 0;     // measurement: utterances per persistent-decode cluster (1..5); 0 = decode_group's rule
+        int decode_timing = 0;    // measurement: CUDA events around every persistent-decode launch (dctts_get_option "decode_last_us")
     } opt;
+
+    // the open synthesis stream (dctts_synth_stream_open), or null: it owns the decode workspace until it is closed
+    dctts_synth_stream_s* synth = nullptr;
 
     // persistent decode (kernels_decode.cu)
     struct {
@@ -225,6 +231,8 @@ struct dctts_handle_s {
         int last_moved_frames = -1, last_moved_utt = -1, last_clusters = 0;
         int last_frames = -1;     // frames the last generation executed, summed over clusters (-1: none yet)
         bool frames_pending = false;   // last_frames is still in `frames` (per cluster) on the device
+        cudaEvent_t ev[2] = {nullptr, nullptr};   // option decode_timing: around the last persistent-decode launch
+        bool timed = false;
 
     } dec;
 
@@ -251,6 +259,7 @@ struct dctts_handle_s {
         if (ar_exec) cudaGraphExecDestroy(ar_exec);
         if (copy_stream) { cudaStreamDestroy(copy_stream); for (auto e : chunk_done) if (e) cudaEventDestroy(e); }
         if (path_uploaded) { cudaEventSynchronize(path_uploaded); cudaEventDestroy(path_uploaded); }
+        for (auto e : dec.ev) if (e) cudaEventDestroy(e);
         if (path_pinned) cudaFreeHost(path_pinned);
         if (stream) cudaStreamDestroy(stream);
     }
@@ -307,6 +316,13 @@ inline void require_each(const std::string& fn, const char* what, const int* val
         }
 }
 
+// Entry points that write the decode workspace, the weights or grow buffers are refused while a synthesis stream is open:
+// its decode and SSRN windows are still reading them.
+inline void require_no_synth_stream(const H* h, const std::string& what) {
+    if (h->synth)
+        throw std::runtime_error(what + ": a synthesis stream is open on this handle (dctts_synth_stream_open); close it first");
+}
+
 // NULL means the legacy default stream (what torch's default stream is), so calls made from a
 // torch program are ordered with the surrounding torch work without extra synchronisation.
 inline cudaStream_t S(dctts_handle, void* s) { return reinterpret_cast<cudaStream_t>(s); }
@@ -319,6 +335,7 @@ std::vector<int> audiodec_rows(const std::vector<LayerDev>& net, int T);        
 void settle_decode_counts(H* h);
 void chist_clear(H* h, const std::string& why);                                  // the chain history is stale
 void drop_ar_graph(H* h);
+void synth_stream_free(dctts_synth_stream_s* ss);                                 // close without outputs (dctts_destroy)
 void run_attention(Launch& lc, const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
                    RowWin win, int N, const int* pma, float* R, float* align, long long* maxatt,
                    int* p_next, int* p_hist, Planes Rpl = Planes{});

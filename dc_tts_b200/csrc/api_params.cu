@@ -360,6 +360,7 @@ int dctts_set_param(dctts_handle h, const char* tf_name, const float* data, cons
 
 int dctts_commit_params(dctts_handle h) {
     return guarded(h, [&] {
+        require_no_synth_stream(h, "dctts_commit_params");
         commit_params(h);
         chist_clear(h, "the weights were committed after the last full-sequence chain");
     });
@@ -369,6 +370,7 @@ int64_t dctts_num_params(dctts_handle h) { return (h && h->committed) ? h->n_par
 
 int dctts_refresh_synthesis(dctts_handle h, void* stream) {
     return guarded(h, [&] {
+        require_no_synth_stream(h, "dctts_refresh_synthesis");
         REQUIRE(h->committed, "dctts_refresh_synthesis: parameters not committed");
         if (!h->synth_stale) return;
         chist_clear(h, "the weights were repacked after the last full-sequence chain");

@@ -125,6 +125,7 @@ ChainLd chain_ld(H* h) {
 
 void ensure_ws(H* h, int B) {
     if (B <= h->ws_B) return;
+    require_no_synth_stream(h, "growing the synthesis workspace");
     chist_clear(h, "the workspace grew after the last chain");
     const dctts_hparams& hp = h->hp;
     const int T = hp.max_T, N = hp.max_N, d = hp.d;
@@ -197,6 +198,7 @@ void ensure_chain_frames(H* h, int B, int T, const char* who) {
     bool grow = h->scratch.bytes < scr || h->act0.bytes < act || h->act1.bytes < act;
     for (auto& pb : h->plane) grow = grow || pb.bytes < pl;
     if (!grow) return;
+    require_no_synth_stream(h, who);
     const size_t want = std::max(scr, h->scratch.bytes) + 2 * std::max(act, h->act0.bytes) + 4 * std::max(pl, h->plane[0].bytes);
     DevBuf n_scr, n_act[2], n_pl[4];
     try {
@@ -284,7 +286,8 @@ void run_deconv(Launch& lc, const LayerDev& l, const float* X, int ldx, int B, i
 
 bool chain_tc_ok(H* h, const std::vector<LayerDev>& net);
 void run_chain_tc_planes(Launch& lc, const std::vector<LayerDev>& net, Planes cur, int which, int B, int L,
-                         float* out, float* out_sig, int first_extra_shift, const float* in_inv, const int* lengths = nullptr);
+                         float* out, float* out_sig, int first_extra_shift, const float* in_inv, const int* lengths = nullptr,
+                         const DevBuf* pl = nullptr);
 void run_chain_full_tc(Launch& lc, const std::vector<LayerDev>& net, const float* X, int ldx, int B, int L,
                        float* out, float* out_sig, const int* lengths = nullptr);
 
@@ -441,23 +444,27 @@ bool chain_tc_ok(H* h, const std::vector<LayerDev>& net) {
 // Whole chain on the tensor-core path, starting from split planes `cur` (buffer index `which`
 // of the ping-pong pair, or -1 for an external buffer): ... -> fp32 out (+ sigmoid).
 // in_inv: inverse per-utterance scales of `cur` (launch_f32_to_planes_scaled), or null.  lengths: per-utterance lengths
-// at L (device), or null; every block stores its rows past them as zeros (run_chain_full).
+// at L (device), or null; every block stores its rows past them as zeros (run_chain_full).  pl: four plane buffers to
+// ping-pong in instead of the workspace's (a synthesis stream's own), or null; with them no chain history is kept.
 void run_chain_tc_planes(Launch& lc, const std::vector<LayerDev>& net, Planes cur, int which, int B, int L,
-                         float* out, float* out_sig, int first_extra_shift, const float* in_inv, const int* lengths) {
+                         float* out, float* out_sig, int first_extra_shift, const float* in_inv, const int* lengths,
+                         const DevBuf* pl) {
     H* h = lc.h;
     int len = L, len_shift = 0;
     int nxt = (which == 0) ? 1 : 0;
-    const int net_id = chain_net(h, net);
-    chist_planes(lc, net_id, 0, cur, B, L, net[0].cin, in_inv);
+    const int net_id = pl ? -1 : chain_net(h, net);
+    if (!pl) chist_planes(lc, net_id, 0, cur, B, L, net[0].cin, in_inv);
     for (size_t i = 0; i < net.size(); ++i) {
         const LayerDev& l = net[i];
         const bool last = (i + 1 == net.size());
-        Planes dst = last ? Planes{} : ws_planes(h, nxt, l.cout);
+        Planes dst = last ? Planes{} : pl ? Planes{pl[2 * nxt].as<__half>(), pl[2 * nxt + 1].as<__half>(), roundup(l.cout, 8)}
+                                          : ws_planes(h, nxt, l.cout);
         run_block_tc(lc, l, l.rate, l.causal, l.act, cur, RowWin{B, len, len, nullptr}, 128, 1, (len + 127) / 128,
                      dst, last ? out : nullptr, l.cout, last ? out_sig : nullptr, l.cout, Planes{},
                      i == 0 ? first_extra_shift : 0, i == 0 ? in_inv : nullptr, lengths, len_shift);
         if (l.kind == K_D) { len *= 2; ++len_shift; }
-        if (last) chist_f32(lc, net_id, (int)i + 1, out, l.cout, B, len, l.cout);
+        if (pl) {}
+        else if (last) chist_f32(lc, net_id, (int)i + 1, out, l.cout, B, len, l.cout);
         else chist_planes(lc, net_id, (int)i + 1, dst, B, len, l.cout, nullptr);
         cur = dst; nxt ^= 1;
     }
@@ -663,8 +670,22 @@ PathRun path_run(H* h) {
     return PathRun{pb, pb + h->ws_B, pb + h->ws_B + (size_t)h->ws_B * h->hp.max_T};
 }
 
+// Utterances per decode cluster: the fewest that let every cluster be co-resident (a second wave doubles the time).
+// reserve (a synthesis stream): the fewest that leave one co-resident cluster slot -- one GPC -- free for the stream's
+// SSRN and Griffin-Lim launches, when five per cluster allow it (B <= 5 (max_clusters - 1)); else the usual rule.
+int decode_group(const H* h, int B, bool reserve) {
+    if (h->opt.decode_group > 0) return h->opt.decode_group;     // measurement override
+    int mc = std::max(1, h->dec.max_clusters);
+    if (reserve && mc > 1 && (B + DEC_GMAX - 1) / DEC_GMAX <= mc - 1) --mc;
+    int G = 1;
+    while (G < DEC_GMAX && (B + G - 1) / G > mc) ++G;
+    return G;
+}
+
 // The whole AR loop as one persistent launch (kernels_decode.cu).  Returns false when this handle / device cannot run it.
-bool decode_cluster(H* h, int B, int steps, cudaStream_t s, const Until* u, const PathRun* pr = nullptr) {
+// progress (with u; mapped host memory, DEC_PROG_INTS per cluster): run decode_progress_kernel, with decode_group's
+// reserving rule.
+bool decode_cluster(H* h, int B, int steps, cudaStream_t s, const Until* u, const PathRun* pr = nullptr, int* progress = nullptr) {
     auto& D = h->dec;
     if (!D.ok || h->opt.decode_mode != 1) return false;
     const dctts_hparams& hp = h->hp;
@@ -689,16 +710,17 @@ bool decode_cluster(H* h, int B, int steps, cudaStream_t s, const Until* u, cons
         P.lengths = const_cast<int*>(pr->lengths); P.frames = D.frames.as<int>();
     } else if (h->opt.decode_prof) { D.prof.ensure(DEC_NPROF * sizeof(long long)); CUDA_CHECK(cudaMemsetAsync(D.prof.p, 0, DEC_NPROF * sizeof(long long), s)); P.prof = D.prof.as<long long>(); }
     P.B = B;
-    {   // utterances per cluster: the fewest that let every cluster be co-resident (a second wave doubles the time)
-        const int mc = std::max(1, D.max_clusters);
-        int G = 1;
-        while (G < DEC_GMAX && (B + G - 1) / G > mc) ++G;
-        P.G = G;
-    }
+    P.G = decode_group(h, B, progress != nullptr);
     P.T = hp.max_T; P.N = hp.max_N; P.d = hp.d; P.n_mels = hp.n_mels;
     P.win_size = hp.attention_win_size; P.steps = steps;
     const int n_clusters = (B + P.G - 1) / P.G;
-    cudaError_t e = pr ? launch_decode_path(P, pr->path, pr->amax, n_clusters, s) : launch_decode_cluster(P, n_clusters, s);
+    D.timed = false;
+    if (h->opt.decode_timing) {
+        for (auto& ev : D.ev) if (!ev) CUDA_CHECK(cudaEventCreate(&ev));
+        CUDA_CHECK(cudaEventRecord(D.ev[0], s));
+    }
+    cudaError_t e = pr ? launch_decode_path(P, pr->path, pr->amax, n_clusters, s)
+                  : (u && progress) ? launch_decode_progress(P, progress, n_clusters, s) : launch_decode_cluster(P, n_clusters, s);
     if (e != cudaSuccess) {
         // a device on which the 16-CTA cluster cannot be placed after all: remember it and let the caller take the
         // graph-per-frame loop (another GPU path, not a CPU fallback)
@@ -707,6 +729,7 @@ bool decode_cluster(H* h, int B, int steps, cudaStream_t s, const Until* u, cons
         return false;
     }
     h->launches += 1;
+    if (h->opt.decode_timing) { CUDA_CHECK(cudaEventRecord(D.ev[1], s)); D.timed = true; }
     D.last_clusters = n_clusters; D.last_moved_frames = -1;
     D.frames_pending = u != nullptr || pr != nullptr;
     D.last_frames = D.frames_pending ? -1 : n_clusters * steps;
@@ -714,11 +737,14 @@ bool decode_cluster(H* h, int B, int steps, cudaStream_t s, const Until* u, cons
 }
 
 // `pr`: the workspace's path (path_run) is already uploaded; the windows follow it
+// `progress` (with u): the persistent decode publishes its progress there (decode_cluster); no other loop may run.
 void text2mel_generate(H* h, const int* L, int B, int steps, float* Y, int* prev_hist,
-                       long long* maxatt, float* align, cudaStream_t s, const Until* u = nullptr, const PathRun* pr = nullptr) {
+                       long long* maxatt, float* align, cudaStream_t s, const Until* u = nullptr, const PathRun* pr = nullptr,
+                       int* progress = nullptr) {
     const dctts_hparams& hp = h->hp;
     const int T = hp.max_T, N = hp.max_N, d = hp.d;
     if (steps <= 0 || steps > T) steps = T;
+    require_no_synth_stream(h, "the decode");
     ensure_ws(h, B);
     h->hist.ok = false;
     const bool cluster = h->dec.ok && h->opt.decode_mode == 1;
@@ -731,7 +757,8 @@ void text2mel_generate(H* h, const int* L, int B, int steps, float* Y, int* prev
     CUDA_CHECK(cudaMemsetAsync(h->ibuf.p, 0, (size_t)(4 + 3 * h->ws_B + (size_t)h->ws_B * T) * sizeof(int), s));
     if (pr) CUDA_CHECK(cudaMemcpy2DAsync(ib.p_cur, sizeof(int), pr->path, (size_t)T * sizeof(int), sizeof(int), B,
                                          cudaMemcpyDeviceToDevice, s));   // the window of frame 0
-    bool persistent = cluster && decode_cluster(h, B, steps, s, u, pr);
+    bool persistent = cluster && decode_cluster(h, B, steps, s, u, pr, progress);
+    REQUIRE(persistent || !progress, "the persistent decode is not available: " + h->dec.why);
     if (persistent) {
         // the whole loop ran as one launch
     } else {
@@ -777,6 +804,7 @@ void text2mel_generate(H* h, const int* L, int B, int steps, float* Y, int* prev
 // for AudioDec.  Shared by text2mel_forward and the aligner.
 bool text2mel_front(Launch& lc, const int* L, const float* mels, const int* pma, int B, int T, long long* maxatt, float* align) {
     H* h = lc.h;
+    require_no_synth_stream(h, "the teacher-forced Text2Mel");
     const dctts_hparams& hp = h->hp;
     const int N = hp.max_N, d = hp.d;
     run_textenc(lc, L, B, h->kv.as<float>());
@@ -937,6 +965,7 @@ int dctts_textenc(dctts_handle h, const int32_t* L, int32_t B, float* K, float* 
     return guarded(h, [&] {
         REQUIRE(h->committed, "parameters not committed");
         REQUIRE(B >= 1 && L && K && V, "dctts_textenc: bad arguments");
+        require_no_synth_stream(h, "dctts_textenc");
         chist_begin(h, "dctts_textenc");
         ensure_ws(h, B);
         h->hist.ok = false;
@@ -1342,13 +1371,18 @@ int dctts_bench_block(dctts_handle h, const char* scope, int32_t B, int32_t L, i
 }
 
 int dctts_reserve(dctts_handle h, int32_t max_batch) {
-    return guarded(h, [&] { REQUIRE(max_batch >= 1, "dctts_reserve: bad batch"); ensure_ws(h, max_batch); });
+    return guarded(h, [&] {
+        REQUIRE(max_batch >= 1, "dctts_reserve: bad batch");
+        require_no_synth_stream(h, "dctts_reserve");
+        ensure_ws(h, max_batch);
+    });
 }
 
 int dctts_reserve_frames(dctts_handle h, int32_t B, int32_t T, int64_t* bytes) {
     return guarded(h, [&] {
         REQUIRE(B >= 1 && T >= 1, "dctts_reserve_frames: need B >= 1 and T >= 1, got B = " + std::to_string(B) + ", T = " +
                                       std::to_string(T));
+        require_no_synth_stream(h, "dctts_reserve_frames");
         ensure_chain_frames(h, B, T, "dctts_reserve_frames");
         if (bytes) *bytes = (int64_t)chain_ws_bytes(h);
     });
@@ -1531,6 +1565,339 @@ int dctts_decode_profile(dctts_handle h, int64_t* cycles, int32_t n) {
         CUDA_CHECK(cudaMemcpy(v, h->dec.prof.p, sizeof(v), cudaMemcpyDeviceToHost));
         for (int i = 0; i < n; ++i) cycles[i] = v[i];
     });
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------- streaming synthesis (DESIGN.md section 8j)
+namespace {
+
+// Mel frames of context SSRN needs on each side of a run of committed frames, from the layer table: an output interval at
+// the final rate, walked back through the blocks (SAME taps [t - left, t + right]; the transposed conv's output 2t reads
+// x[t], x[t - 1] and 2t + 1 reads x[t]).  The walk starts at a whole mel frame, so the result holds for every frame.
+void ssrn_halo(const H* h, int& left, int& right) {
+    int up = 1;
+    for (const LayerDev& l : h->ssrn) if (l.kind == K_D) up *= 2;
+    const long long a = 1 << 12, b = a + 1;
+    long long lo = a * up, hi = b * up;
+    for (int i = (int)h->ssrn.size() - 1; i >= 0; --i) {
+        const LayerDev& l = h->ssrn[(size_t)i];
+        if (l.kind == K_D) {
+            lo = (lo % 2 == 0) ? lo / 2 - 1 : lo / 2;
+            hi = (hi - 1) / 2 + 1;
+        } else {
+            const int tot = (l.size - 1) * l.rate, lft = l.causal ? tot : tot / 2;
+            lo -= lft; hi += tot - lft;
+        }
+    }
+    left = (int)(a - lo); right = (int)(hi - b);
+}
+
+// The buffers of windowed SSRN: the ping-pong plane pairs, the sigmoid output (W, r L, F), the windows' inverse scales and
+// their description (len | utt | row0, `slots` rounds of W each), for up to W windows of L mel frames.
+struct SsrnWindows {
+    DevBuf pl[4], z, inv, meta;
+    int W = 0, L = 0;
+};
+
+void ssrn_windows_alloc(H* h, SsrnWindows& sw, int W, int L, int slots) {
+    const size_t rows = (size_t)W * L * h->hp.r;
+    for (auto& b : sw.pl) b.ensure(rows * chain_ld(h).pl * sizeof(__half));
+    sw.z.ensure(rows * h->F * sizeof(float));
+    sw.inv.ensure((size_t)W * sizeof(float));
+    sw.meta.ensure((size_t)slots * 3 * W * sizeof(int));
+    sw.W = W; sw.L = L;
+}
+
+// One launch set of windowed SSRN on s: windows `win` (device, len | utt | row0 of W) of Y (B, T, n_mels) -> sw.z, window w's
+// rows [0, r len[w]) being what the whole-sequence SSRN gives for those rows of a sequence of len[w] frames, at the fixed
+// input scale (launch_mel_windows_to_planes).  L: the longest window.
+void ssrn_window_run(H* h, SsrnWindows& sw, const float* Y, int T, const int* win, int W, int L, cudaStream_t s) {
+    Launch lc{h, s};
+    Planes cur{sw.pl[0].as<__half>(), sw.pl[1].as<__half>(), roundup(h->hp.n_mels, 8)};
+    launch_mel_windows_to_planes(Y, T, h->hp.n_mels, win, W, L, cur, sw.inv.as<float>(), s); lc.count();
+    run_chain_tc_planes(lc, h->ssrn, cur, 0, W, L, nullptr, sw.z.as<float>(), 0, sw.inv.as<float>(), win, sw.pl);
+}
+
+void require_ssrn_windows(H* h, const std::string& fn) {
+    REQUIRE(h->committed, fn + ": parameters not committed");
+    REQUIRE(chain_tc_ok(h, h->ssrn), fn + ": SSRN has no tensor-core chain on this handle" +
+                                         (h->tc16_why.empty() ? std::string() : " (" + h->tc16_why + ")"));
+}
+
+}  // namespace
+
+// One synthesis stream: the decode of B utterances publishing its progress, and the SSRN windows and vocoder pushes of
+// their chunks on the stream's own side stream.  Host state per utterance: the next chunk, samples committed, done.
+struct dctts_synth_stream_s {
+    H* h = nullptr;
+    cudaStream_t ds = nullptr, ss = nullptr;       // the decode's stream (the caller's), the side stream (owned)
+    int B = 0, G = 1, T = 0, chunk = 1, tail = 0, left = 0, right = 0, r = 4, F = 0, slots = 1, Lyw = 0, ldr = 0, rmax = 0;
+    int* prog = nullptr;                           // pinned, mapped: DEC_PROG_INTS per cluster
+    int* meta_host = nullptr;                      // pinned: the windows of one poll's rounds
+    DevBuf stop, len, zfull, push, wavr, wav;
+    SsrnWindows sw;
+    dctts_vocoder_stream vs = nullptr;
+    std::vector<int> next, committed, done, first_frames;
+
+    ~dctts_synth_stream_s() {
+        if (ds || ss) { cudaStreamSynchronize(ds); if (ss) cudaStreamSynchronize(ss); }
+        if (vs) dctts_vocoder_stream_close(vs, nullptr);
+        if (prog) cudaFreeHost(prog);
+        if (meta_host) cudaFreeHost(meta_host);
+        if (ss) cudaStreamDestroy(ss);
+    }
+};
+
+namespace {
+
+// What the host knows of utterance b: frames published by its cluster, and its length (-1 while unknown)
+struct UttProgress { int frames, len; };
+UttProgress utt_progress(const dctts_synth_stream_s* st, int b) {
+    const int* p = st->prog + (size_t)(b / st->G) * DEC_PROG_INTS;
+    const int f = __atomic_load_n(p, __ATOMIC_ACQUIRE);
+    int n = __atomic_load_n(p + 1 + b % st->G, __ATOMIC_RELAXED);
+    if (n < 0 && f >= st->T) n = st->T;            // the loop ran every frame without reaching the stop
+    return {f, n};
+}
+
+// The fixed grid: chunk k of utterance b is mel rows [k chunk, min(len, (k + 1) chunk)), ready once the rows its window
+// reads are published.  A chunk that starts at or past a known length does not exist.
+bool chunk_ready(const dctts_synth_stream_s* st, int b, UttProgress p) {
+    const int a = st->next[b] * st->chunk;
+    if (p.len >= 0) return a < p.len && p.frames >= std::min(p.len, a + st->chunk + st->right);
+    return p.frames >= a + st->chunk + st->right;
+}
+
+// Rounds of one chunk per utterance with a ready one, until none is ready: one SSRN launch set and one vocoder push each.
+void synth_rounds(dctts_synth_stream_s* st, const char* fn) {
+    H* h = st->h;
+    const int B = st->B, r = st->r, F = st->F;
+    std::vector<UttProgress> p((size_t)B);
+    for (int b = 0; b < B; ++b) p[(size_t)b] = utt_progress(st, b);
+    std::vector<int> rows((size_t)B), fin((size_t)B), cnt((size_t)B), a0((size_t)B), e0((size_t)B), s0((size_t)B);
+    for (int slot = 0;; ++slot) {
+        std::vector<int> ws;
+        for (int b = 0; b < B; ++b) if (!st->done[b] && chunk_ready(st, b, p[(size_t)b])) ws.push_back(b);
+        std::fill(fin.begin(), fin.end(), 0);
+        if (ws.empty()) return;
+        REQUIRE(slot < st->slots, std::string(fn) + ": more rounds than chunks per utterance");
+        const int W = (int)ws.size();
+        int* m = st->meta_host + (size_t)slot * 3 * B;
+        int L = 1;
+        for (int w = 0; w < W; ++w) {
+            const int b = ws[(size_t)w];
+            const int n = p[(size_t)b].len >= 0 ? p[(size_t)b].len : st->T;
+            const int a = st->next[b] * st->chunk, e = std::min(n, a + st->chunk);
+            const int s = std::max(0, a - st->left), t = std::min(n, e + st->right);
+            m[w] = t - s; m[W + w] = b; m[2 * W + w] = s;
+            a0[(size_t)b] = a; e0[(size_t)b] = e; s0[(size_t)b] = s;
+            fin[(size_t)b] = (e == p[(size_t)b].len) ? 1 : 0;
+            L = std::max(L, t - s);
+        }
+        int* md = st->sw.meta.as<int>() + (size_t)slot * 3 * B;
+        CUDA_CHECK(cudaMemcpyAsync(md, m, (size_t)3 * W * sizeof(int), cudaMemcpyHostToDevice, st->ss));
+        ssrn_window_run(h, st->sw, h->ybuf.as<float>(), st->T, md, W, L, st->ss);
+        std::fill(rows.begin(), rows.end(), 0);
+        for (int w = 0; w < W; ++w) {
+            const int b = ws[(size_t)w];
+            const size_t n = (size_t)r * (e0[(size_t)b] - a0[(size_t)b]) * F * sizeof(float);
+            const float* src = st->sw.z.as<float>() + ((size_t)w * r * L + (size_t)r * (a0[(size_t)b] - s0[(size_t)b])) * F;
+            CUDA_CHECK(cudaMemcpyAsync(st->zfull.as<float>() + ((size_t)b * r * st->T + (size_t)r * a0[(size_t)b]) * F, src, n,
+                                       cudaMemcpyDeviceToDevice, st->ss));
+            CUDA_CHECK(cudaMemcpyAsync(st->push.as<float>() + (size_t)b * st->rmax * F, src, n, cudaMemcpyDeviceToDevice, st->ss));
+            rows[(size_t)b] = r * (e0[(size_t)b] - a0[(size_t)b]);
+        }
+        if (dctts_vocoder_stream_push(st->vs, st->push.as<float>(), st->rmax, rows.data(), fin.data(), st->wavr.as<float>(),
+                                      st->ldr, cnt.data()) != 0)
+            throw std::runtime_error(h->err);
+        for (int b : ws) {
+            if (cnt[(size_t)b] > 0)
+                CUDA_CHECK(cudaMemcpyAsync(st->wav.as<float>() + (size_t)b * st->Lyw + st->committed[b],
+                                           st->wavr.as<float>() + (size_t)b * st->ldr, (size_t)cnt[(size_t)b] * sizeof(float),
+                                           cudaMemcpyDeviceToDevice, st->ss));
+            st->committed[b] += cnt[(size_t)b];
+            if (st->next[b] == 0) st->first_frames[b] = p[(size_t)b].frames;
+            ++st->next[b];
+            if (fin[(size_t)b]) st->done[b] = 1;
+        }
+    }
+}
+
+void synth_open(H* h, const int* L, int B, const int* stop_host, int tail, int chunk, int n_iter, double momentum,
+                cudaStream_t s, dctts_synth_stream* out) {
+    const std::string fn = "dctts_synth_stream_open";
+    REQUIRE(out && L && stop_host && B >= 1, fn + ": bad arguments");
+    REQUIRE(chunk >= 1, fn + ": chunk must be >= 1 mel frame, got " + std::to_string(chunk));
+    REQUIRE(tail >= 0, fn + ": tail must be >= 0");
+    REQUIRE(!h->synth, fn + ": a synthesis stream is already open on this handle; close it first");
+    REQUIRE(h->committed, fn + ": parameters not committed");
+    REQUIRE(h->dec.ok && h->opt.decode_mode == 1,
+            fn + ": needs the persistent decode, which this handle cannot run: " +
+            (h->dec.ok ? std::string("option decode_mode is 0") : h->dec.why) +
+            " (after training, refresh_synthesis() / dctts_refresh_synthesis repacks the weights)");
+    require_ssrn_windows(h, fn);
+    ensure_ws(h, B);                                  // any growth (and its device synchronisation) before this stream starts
+    auto st = std::make_unique<dctts_synth_stream_s>();
+    st->h = h; st->ds = s; st->B = B; st->T = h->hp.max_T; st->chunk = std::min(chunk, h->hp.max_T);
+    st->tail = std::min(tail, h->hp.max_T); st->r = h->hp.r; st->F = h->F;
+    st->G = decode_group(h, B, true);
+    ssrn_halo(h, st->left, st->right);
+    const int T = st->T, r = st->r, F = st->F, clusters = (B + st->G - 1) / st->G;
+    st->slots = (T + st->chunk - 1) / st->chunk;
+    st->rmax = r * st->chunk;
+    st->Lyw = h->voc.hop * (r * T - 1);
+    st->ldr = st->Lyw;
+    const int Lw = std::min(T, st->chunk + st->left + st->right);
+    CUDA_CHECK(cudaStreamCreateWithFlags(&st->ss, cudaStreamNonBlocking));
+    CUDA_CHECK(cudaHostAlloc(reinterpret_cast<void**>(&st->prog), (size_t)clusters * DEC_PROG_INTS * sizeof(int), cudaHostAllocMapped));
+    for (int c = 0; c < clusters; ++c) {
+        st->prog[c * DEC_PROG_INTS] = 0;
+        for (int g = 1; g < DEC_PROG_INTS; ++g) st->prog[c * DEC_PROG_INTS + g] = -1;
+    }
+    CUDA_CHECK(cudaHostAlloc(reinterpret_cast<void**>(&st->meta_host), (size_t)st->slots * 3 * B * sizeof(int), cudaHostAllocDefault));
+    ssrn_windows_alloc(h, st->sw, B, Lw, st->slots);
+    st->stop.ensure((size_t)B * sizeof(int)); st->len.ensure((size_t)B * sizeof(int));
+    st->zfull.ensure((size_t)B * r * T * F * sizeof(float));
+    st->push.ensure((size_t)B * st->rmax * F * sizeof(float));
+    st->wavr.ensure((size_t)B * st->ldr * sizeof(float)); st->wav.ensure((size_t)B * st->Lyw * sizeof(float));
+    CUDA_CHECK(cudaMemsetAsync(st->zfull.p, 0, st->zfull.bytes, st->ss));
+    if (dctts_vocoder_stream_open(h, B, r * T, n_iter, momentum, st->ss, &st->vs) != 0) throw std::runtime_error(h->err);
+    st->next.assign(B, 0); st->committed.assign(B, 0); st->done.assign(B, 0); st->first_frames.assign(B, -1);
+    int* prog_dev = nullptr;
+    CUDA_CHECK(cudaHostGetDevicePointer(reinterpret_cast<void**>(&prog_dev), st->prog, 0));
+    upload_host(h, st->stop.p, stop_host, (size_t)B * sizeof(int), s);
+    const Until u{st->stop.as<int>(), st->tail, st->len.as<int>()};
+    text2mel_generate(h, L, B, T, nullptr, nullptr, nullptr, nullptr, s, &u, nullptr, prog_dev);
+    h->hist.ok = false;                               // the stream's decode is not kept for dctts_decode_history
+    h->synth = st.get();
+    *out = st.release();
+}
+
+void synth_poll(dctts_synth_stream st, int wait, float* wav, int64_t ld, int32_t* counts, int32_t* done, int32_t* frames) {
+    const char* fn = "dctts_synth_stream_poll";
+    REQUIRE(counts && done && (wav || ld == 0), std::string(fn) + ": bad arguments");
+    REQUIRE(ld >= st->Lyw, std::string(fn) + ": ld must hold a whole utterance, " + std::to_string(st->Lyw) + " samples");
+    const int B = st->B;
+    auto any_ready = [&] {
+        for (int b = 0; b < B; ++b) if (!st->done[b] && chunk_ready(st, b, utt_progress(st, b))) return true;
+        return false;
+    };
+    auto all_done = [&] { return std::all_of(st->done.begin(), st->done.end(), [](int d) { return d != 0; }); };
+    while (wait && !all_done() && !any_ready()) {
+        const cudaError_t e = cudaStreamQuery(st->ds);
+        if (e == cudaErrorNotReady) { cudaGetLastError(); std::this_thread::yield(); continue; }
+        CUDA_CHECK(e);                                // a failed decode ends the wait with its error
+        REQUIRE(any_ready() || all_done(), std::string(fn) + ": the decode ended without publishing every utterance's frames");
+    }
+    const std::vector<int> c0 = st->committed;
+    synth_rounds(st, fn);
+    for (int b = 0; b < B; ++b) {
+        counts[b] = st->committed[b] - c0[b];
+        if (counts[b] > 0)
+            CUDA_CHECK(cudaMemcpyAsync(wav + (size_t)b * ld, st->wav.as<float>() + (size_t)b * st->Lyw + c0[b],
+                                       (size_t)counts[b] * sizeof(float), cudaMemcpyDeviceToHost, st->ss));
+    }
+    CUDA_CHECK(cudaStreamSynchronize(st->ss));
+    for (int b = 0; b < B; ++b) {
+        done[b] = st->done[b];
+        if (frames) frames[b] = utt_progress(st, b).frames;
+    }
+}
+
+void synth_close(dctts_synth_stream st, int32_t* lengths, int32_t* trim, float* Y, float* Z, int32_t* first_frames) {
+    H* h = st->h;
+    const int B = st->B, T = st->T;
+    CUDA_CHECK(cudaStreamSynchronize(st->ds));
+    synth_rounds(st, "dctts_synth_stream_close");     // the decode has ended: every remaining chunk is ready
+    if (lengths) CUDA_CHECK(cudaMemcpy(lengths, st->len.p, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost));
+    if (first_frames) std::copy(st->first_frames.begin(), st->first_frames.end(), first_frames);
+    if (Y) {
+        launch_until_finish(st->stop.as<int>(), st->tail, T, T, h->hp.n_mels, nullptr, false, st->len.as<int>(), h->ybuf.as<float>(),
+                            nullptr, B, st->ds);
+        h->launches += 1;
+        CUDA_CHECK(cudaMemcpyAsync(Y, h->ybuf.p, (size_t)B * T * h->hp.n_mels * sizeof(float), cudaMemcpyDeviceToDevice, st->ds));
+        CUDA_CHECK(cudaStreamSynchronize(st->ds));
+    }
+    if (Z) CUDA_CHECK(cudaMemcpyAsync(Z, st->zfull.p, st->zfull.bytes, cudaMemcpyDeviceToDevice, st->ss));
+    CUDA_CHECK(cudaStreamSynchronize(st->ss));
+    dctts_vocoder_stream vs = st->vs;
+    st->vs = nullptr;
+    if (dctts_vocoder_stream_close(vs, trim) != 0) throw std::runtime_error(h->err);
+}
+
+}  // namespace
+
+void dctts::api::synth_stream_free(dctts_synth_stream_s* st) {
+    if (st->h && st->h->synth == st) st->h->synth = nullptr;
+    delete st;
+}
+
+extern "C" {
+
+int dctts_ssrn_halo(dctts_handle h, int32_t* left, int32_t* right) {
+    return guarded(h, [&] {
+        REQUIRE(left && right, "dctts_ssrn_halo: bad arguments");
+        REQUIRE(h->committed, "dctts_ssrn_halo: parameters not committed");
+        int l = 0, r = 0;
+        ssrn_halo(h, l, r);
+        *left = l; *right = r;
+    });
+}
+
+int dctts_ssrn_windows(dctts_handle h, const float* Y, int32_t B, int32_t T, const int32_t* starts_host, const int32_t* counts_host,
+                       const int32_t* lengths_host, float* Z, int32_t ldz_frames, void* stream) {
+    return guarded(h, [&] {
+        const std::string fn = "dctts_ssrn_windows";
+        REQUIRE(Y && Z && starts_host && counts_host && lengths_host && B >= 1 && T >= 1 && ldz_frames >= 1, fn + ": bad arguments");
+        require_ssrn_windows(h, fn);
+        require_each(fn, "length", lengths_host, B, 1, T);
+        int left = 0, right = 0;
+        ssrn_halo(h, left, right);
+        std::vector<int> m((size_t)3 * B);
+        int L = 1;
+        for (int b = 0; b < B; ++b) {
+            const int a = starts_host[b], e = a + counts_host[b], n = lengths_host[b];
+            REQUIRE(a >= 0 && e > a && e <= n && e - a <= ldz_frames,
+                    fn + ": utterance " + std::to_string(b) + " has the window [" + std::to_string(a) + ", " + std::to_string(e) +
+                        ") outside its length " + std::to_string(n) + " or past ldz_frames");
+            const int s = std::max(0, a - left), t = std::min(n, e + right);
+            m[(size_t)b] = t - s; m[(size_t)B + b] = b; m[(size_t)2 * B + b] = s;
+            L = std::max(L, t - s);
+        }
+        cudaStream_t s = S(h, stream);
+        SsrnWindows sw;
+        ssrn_windows_alloc(h, sw, B, L, 1);
+        CUDA_CHECK(cudaMemcpyAsync(sw.meta.p, m.data(), m.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+        ssrn_window_run(h, sw, Y, T, sw.meta.as<int>(), B, L, s);
+        const int r = h->hp.r, F = h->F;
+        for (int b = 0; b < B; ++b)
+            CUDA_CHECK(cudaMemcpyAsync(Z + (size_t)b * r * ldz_frames * F,
+                                       sw.z.as<float>() + ((size_t)b * r * L + (size_t)r * (starts_host[b] - m[(size_t)2 * B + b])) * F,
+                                       (size_t)r * counts_host[b] * F * sizeof(float), cudaMemcpyDeviceToDevice, s));
+        CUDA_CHECK(cudaStreamSynchronize(s));         // the window buffers are freed on return
+    });
+}
+
+int dctts_synth_stream_open(dctts_handle h, const int32_t* L, int32_t B, const int32_t* stop_pos_host, int32_t tail, int32_t chunk,
+                            int32_t n_iter, double momentum, void* stream, dctts_synth_stream* out) {
+    return guarded(h, [&] { synth_open(h, L, B, stop_pos_host, tail, chunk, n_iter, momentum, S(h, stream), out); });
+}
+
+int dctts_synth_stream_poll(dctts_synth_stream ss, int32_t wait, float* wav, int64_t ld, int32_t* counts_host, int32_t* done_host,
+                            int32_t* frames_host) {
+    if (!ss) { g_create_error = "null synthesis stream"; return 1; }
+    return guarded(ss->h, [&] { synth_poll(ss, wait, wav, ld, counts_host, done_host, frames_host); });
+}
+
+int dctts_synth_stream_close(dctts_synth_stream ss, int32_t* lengths_host, int32_t* trim_host, float* Y, float* Z,
+                             int32_t* first_frames_host) {
+    if (!ss) { g_create_error = "null synthesis stream"; return 1; }
+    H* h = ss->h;
+    const bool outputs = lengths_host || trim_host || Y || Z || first_frames_host;
+    const int rc = outputs ? guarded(h, [&] { synth_close(ss, lengths_host, trim_host, Y, Z, first_frames_host); }) : 0;
+    synth_stream_free(ss);                            // waits for the decode and the side stream
+    return rc;
 }
 
 }  // extern "C"

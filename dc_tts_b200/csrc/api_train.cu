@@ -676,12 +676,13 @@ int dctts_train_loss(dctts_handle h, const float* logits, int32_t ldl, const flo
 }
 
 int dctts_train_init(dctts_handle h, int32_t B, float dropout_rate) {
-    return guarded(h, [&] { train_init(h, B, dropout_rate, 1, h->hp.max_T); });
+    return guarded(h, [&] { require_no_synth_stream(h, "dctts_train_init"); train_init(h, B, dropout_rate, 1, h->hp.max_T); });
 }
 
 int dctts_train_step_shaped(dctts_handle h, const int32_t* L, int32_t N, const float* mels, int32_t T, int32_t B, int64_t global_step,
                             uint32_t seed, float lr, int32_t apply, float* losses_host, void* stream) {
     return guarded(h, [&] {
+        require_no_synth_stream(h, "dctts_train_step_shaped");
         REQUIRE(L && mels && B >= 1 && global_step >= 0, "dctts_train_step: bad arguments");
         cudaStream_t s = S(h, stream);
         train_forward_backward(h, reinterpret_cast<const int*>(L), N, mels, T, B, seed, losses_host, s);
@@ -711,11 +712,11 @@ int dctts_train_eval_ssrn(dctts_handle h, const float* mels, const float* mags, 
 }
 
 int dctts_train_apply(dctts_handle h, int64_t global_step, float lr, void* stream) {
-    return guarded(h, [&] { REQUIRE(global_step >= 0, "dctts_train_apply: bad step"); train_apply(h, global_step, lr, S(h, stream)); });
+    return guarded(h, [&] { require_no_synth_stream(h, "dctts_train_apply"); REQUIRE(global_step >= 0, "dctts_train_apply: bad step"); train_apply(h, global_step, lr, S(h, stream)); });
 }
 
 int dctts_train_reserve(dctts_handle h, int32_t N, int32_t T) {
-    return guarded(h, [&] { train_reserve(h, N, T); });
+    return guarded(h, [&] { require_no_synth_stream(h, "dctts_train_reserve"); train_reserve(h, N, T); });
 }
 
 int dctts_train_capacity(dctts_handle h, int32_t* N, int32_t* T) {
@@ -733,12 +734,13 @@ int dctts_train_grads(dctts_handle h, float** grads, int64_t* count) {
 }
 
 int dctts_train_init_ssrn(dctts_handle h, int32_t B, int32_t T, float dropout_rate) {
-    return guarded(h, [&] { train_init(h, B, dropout_rate, 2, T); });
+    return guarded(h, [&] { require_no_synth_stream(h, "dctts_train_init_ssrn"); train_init(h, B, dropout_rate, 2, T); });
 }
 
 int dctts_train_step_ssrn_shaped(dctts_handle h, const float* mels, const float* mags, int32_t B, int32_t T, int64_t global_step,
                                  uint32_t seed, float lr, int32_t apply, float* losses_host, void* stream) {
     return guarded(h, [&] {
+        require_no_synth_stream(h, "dctts_train_step_ssrn_shaped");
         REQUIRE(mels && mags && B >= 1 && global_step >= 0, "dctts_train_step_ssrn: bad arguments");
         cudaStream_t s = S(h, stream);
         train_forward_backward_ssrn(h, mels, mags, B, T, seed, losses_host, s);
@@ -776,6 +778,7 @@ int dctts_train_tensor(dctts_handle h, const char* tf_name, int32_t what, float*
 // what Supervisor's restore does for a resumed run (train.py:144; ADVICE r1: training could not resume).
 int dctts_train_set_tensor(dctts_handle h, const char* tf_name, int32_t what, const float* host_in, int64_t count) {
     return guarded(h, [&] {
+        require_no_synth_stream(h, "dctts_train_set_tensor");
         REQUIRE(h->tr.ready && tf_name && host_in && (what == 0 || what == 2 || what == 3), "dctts_train_set_tensor: bad arguments");
         auto it = h->tr.tensors.find(tf_name);
         REQUIRE(it != h->tr.tensors.end(), "dctts_train_set_tensor: not a variable of the network being trained");

@@ -17,6 +17,7 @@ const Option kOptions[] = {
     {"train_tc", &H::Options::train_tc, 7},       {"train_probe", &H::Options::train_probe, 2},
     {"train_deterministic", &H::Options::train_deterministic, 1},
     {"chain_history", &H::Options::chain_history, 1},
+    {"decode_group", &H::Options::decode_group, 5},  {"decode_timing", &H::Options::decode_timing, 1},
 };
 
 const Option* find_option(const char* name) {
@@ -64,6 +65,7 @@ int dctts_create(const dctts_hparams* hp, int device, dctts_handle* out) {
 int dctts_destroy(dctts_handle h) {
     if (!h) return 1;
     cudaSetDevice(h->device);
+    if (h->synth) synth_stream_free(h->synth);      // waits for its decode
     cudaDeviceSynchronize();
     delete h;
     return 0;
@@ -129,6 +131,14 @@ int dctts_get_option(dctts_handle h, const char* name, int32_t* value) {
             REQUIRE(h->dec.last_frames >= 0 || h->dec.frames_pending, "dctts_get_option(decode_last_frames): no generation has run");
             settle_decode_counts(h);
             *value = h->dec.last_frames;
+            return;
+        }
+        if (name && std::string(name) == "decode_last_us") {        // option decode_timing: the last persistent decode's GPU time
+            REQUIRE(h->dec.timed, "dctts_get_option(decode_last_us): no persistent decode has run with option decode_timing");
+            CUDA_CHECK(cudaEventSynchronize(h->dec.ev[1]));
+            float ms = 0.f;
+            CUDA_CHECK(cudaEventElapsedTime(&ms, h->dec.ev[0], h->dec.ev[1]));
+            *value = (int32_t)std::lround(1e3 * ms);
             return;
         }
         if (name && std::string(name) == "ssrn_tc_available") {     // every SSRN block has a wgmma kernel (needs committed parameters)

@@ -136,6 +136,22 @@ __device__ __forceinline__ void bulk_g2s_mc(void* dst, const void* src, uint32_t
                  :: "r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)), "h"(mask) : "memory");
 }
 __device__ __forceinline__ void cluster_sync_all() { cluster_arrive(); cluster_wait(); }
+
+// The progress of one cluster after frame j (decode_progress_kernel; rank 0, thread 0, after the frame's closing
+// cluster_sync_all): p[1 + g] = S.ulen[g] (-1 while utterance g's length is unknown), then p[0] = j + 1 frames done.
+// p is host memory mapped into the device; the host reads p[0] with acquire and then p[1..].
+// Memory ordering: Y is written only by rank 0 (layer_row's last block, one thread per channel), and every thread of
+// rank 0 -- every thread of the cluster -- has passed barrier.cluster.arrive.release of this frame's closing barrier before
+// this thread's wait.acquire returned.  So this frame's Y rows, and the other 15 CTAs' history rows (which the host never
+// reads), happen before the fence in causality order; fence.sc.sys then orders them, and the lengths below, before the
+// release store of the count at system scope.  A host thread that reads the count with acquire and then launches work
+// that reads ybuf sees every Y row of frames < count.
+__device__ __forceinline__ void publish_progress(int* p, int frames, const int* ulen) {
+#pragma unroll
+    for (int g = 0; g < DEC_GMAX; ++g) asm volatile("st.relaxed.sys.u32 [%0], %1;" :: "l"(p + 1 + g), "r"(ulen[g]) : "memory");
+    __threadfence_system();
+    asm volatile("st.release.sys.u32 [%0], %1;" :: "l"(p), "r"(frames) : "memory");
+}
 // generic-proxy global stores (the plane histories) -> visible to later bulk copies (async proxy) once a barrier orders them
 __device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
 
@@ -935,10 +951,13 @@ __device__ __forceinline__ Stream prepass(const DecParams& P, Smem& S, Stream st
 // is only recorded in amax_hist[b][j] (both (B, T)).  The lengths are inputs (P.lengths): S.f_end, the longest of the
 // cluster's, is set before the first frame and never lowered (S.stop / S.ulen are not used); the host pads each path row
 // past its length with its last window, so those frames never trigger a recompute.
-template <bool PROF, int GT, bool STOP, bool PATH = false>
+// PROG (decode_progress_kernel, with STOP): at the end of every frame the cluster publishes its progress to `prog`, host
+// memory mapped into the device (publish_progress).
+template <bool PROF, int GT, bool STOP, bool PATH = false, bool PROG = false>
 __device__ __forceinline__ void decode_body(const DecParams& Pc, const int* __restrict__ path = nullptr,
-                                            int* __restrict__ amax_hist = nullptr) {
+                                            int* __restrict__ amax_hist = nullptr, int* prog = nullptr) {
     static_assert(!PATH || STOP, "a path decode is bounded by its lengths");
+    static_assert(!PROG || (STOP && !PATH), "progress is published by the until-EOS decode");
     extern __shared__ __align__(128) unsigned char smem_raw[];
     Smem& S = *reinterpret_cast<Smem*>(smem_raw);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -1065,6 +1084,9 @@ __device__ __forceinline__ void decode_body(const DecParams& Pc, const int* __re
         fence_proxy_async_global();                       // this frame's plane rows: read by bulk copies in later frames
         cluster_sync_all();                               // this frame's history rows are visible to the whole cluster
         LAP(LP_FRAME);
+        if constexpr (PROG) {
+            if (rank == 0 && tid == 0) publish_progress(prog + (size_t)cluster * DEC_PROG_INTS, j + 1, S.ulen);
+        }
         if constexpr (STOP) {                             // S.f_end is the same in every CTA: the whole cluster leaves here
             if (j + 1 >= S.f_end) { frames = j + 1; break; }
         }
@@ -1090,6 +1112,13 @@ template <int GT>
 __global__ void __cluster_dims__(DEC_NC, 1, 1) __launch_bounds__(DEC_THREADS, 1)
 decode_until_kernel(const __grid_constant__ DecParams Pc) { decode_body<false, GT, true>(Pc); }
 
+// decode_until_kernel that publishes its progress at the end of every frame: progress[cluster * DEC_PROG_INTS ...]
+template <int GT>
+__global__ void __cluster_dims__(DEC_NC, 1, 1) __launch_bounds__(DEC_THREADS, 1)
+decode_progress_kernel(const __grid_constant__ DecParams Pc, int* progress) {
+    decode_body<false, GT, true, false, true>(Pc, nullptr, nullptr, progress);
+}
+
 // the same loop along a caller's window path: path and amax_hist are (B, T), P.lengths (B) are the frames to produce
 template <int GT>
 __global__ void __cluster_dims__(DEC_NC, 1, 1) __launch_bounds__(DEC_THREADS, 1)
@@ -1101,6 +1130,16 @@ size_t decode_smem_bytes() { return sizeof(Smem) + 128; }
 
 using DecKernel = void (*)(DecParams);
 using DecPathKernel = void (*)(DecParams, const int*, int*);
+using DecProgKernel = void (*)(DecParams, int*);
+static DecProgKernel decode_progress_kernel_of(int G) {
+    switch (G) {
+        case 1: return decode_progress_kernel<1>;
+        case 2: return decode_progress_kernel<2>;
+        case 3: return decode_progress_kernel<3>;
+        case 4: return decode_progress_kernel<4>;
+        default: return decode_progress_kernel<5>;
+    }
+}
 static DecPathKernel decode_path_kernel_of(int G) {
     switch (G) {
         case 1: return decode_path_kernel<1>;
@@ -1136,10 +1175,11 @@ static cudaError_t decode_prepare() {
     if (e != cudaSuccess) return e;
     if (dev >= 0 && dev < 64 && done[dev].load(std::memory_order_acquire)) return cudaSuccess;
     for (int G = 1; G <= DEC_GMAX; ++G)
-        for (int v = 0; v < 4; ++v) {                     // decode_cluster_kernel without / with lap timers, decode_until_kernel,
-                                                          // decode_path_kernel
+        for (int v = 0; v < 5; ++v) {                     // decode_cluster_kernel without / with lap timers, decode_until_kernel,
+                                                          // decode_path_kernel, decode_progress_kernel
             const void* k = v < 3 ? reinterpret_cast<const void*>(decode_kernel_of(v == 1, G, v == 2))
-                                  : reinterpret_cast<const void*>(decode_path_kernel_of(G));
+                          : v == 3 ? reinterpret_cast<const void*>(decode_path_kernel_of(G))
+                                   : reinterpret_cast<const void*>(decode_progress_kernel_of(G));
             e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)decode_smem_bytes());
             if (e != cudaSuccess) return e;
             e = cudaFuncSetAttribute(k, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
@@ -1179,6 +1219,16 @@ cudaError_t launch_decode_path(const DecParams& p, const int* path, int* amax_hi
     cfg.gridDim = dim3(n_clusters * DEC_NC); cfg.blockDim = dim3(DEC_THREADS); cfg.dynamicSmemBytes = decode_smem_bytes(); cfg.stream = s;
     cfg.attrs = nullptr; cfg.numAttrs = 0;
     return cudaLaunchKernelEx(&cfg, decode_path_kernel_of(p.G), p, path, amax_hist);
+}
+
+cudaError_t launch_decode_progress(const DecParams& p, int* progress, int n_clusters, cudaStream_t s) {
+    cudaError_t e = decode_prepare();
+    if (e != cudaSuccess) return e;
+    if (p.G < 1 || p.G > DEC_GMAX || !p.stop_pos || !p.lengths || !p.frames || !progress) return cudaErrorInvalidValue;
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(n_clusters * DEC_NC); cfg.blockDim = dim3(DEC_THREADS); cfg.dynamicSmemBytes = decode_smem_bytes(); cfg.stream = s;
+    cfg.attrs = nullptr; cfg.numAttrs = 0;
+    return cudaLaunchKernelEx(&cfg, decode_progress_kernel_of(p.G), p, progress);
 }
 
 __global__ void until_finish_kernel(const int* __restrict__ stop_pos, int tail, int steps, int T, int n_mels,

@@ -81,6 +81,12 @@ cudaError_t launch_decode_cluster(const DecParams& p, int n_clusters, cudaStream
 // previous frame's argmax, which goes to amax_hist[b * T + j].  p.lengths (B) are inputs, 1 <= lengths[b] <= p.steps, and
 // a cluster executes the longest of its utterances (p.frames as decode_until_kernel; p.stop_pos is not read).
 cudaError_t launch_decode_path(const DecParams& p, const int* path, int* amax_hist, int n_clusters, cudaStream_t s);
+// decode_progress_kernel: decode_until_kernel (p.stop_pos, p.lengths, p.frames required) that, at the end of every frame,
+// publishes to progress[c * DEC_PROG_INTS + ...] (host memory mapped into the device) cluster c's frames done (int 0,
+// release store at system scope) and each of its utterance slots' length, -1 while unknown (ints 1 .. DEC_GMAX).  Y rows
+// of frames below the count are visible to a host thread that read the count with acquire.
+constexpr int DEC_PROG_INTS = 8;
+cudaError_t launch_decode_progress(const DecParams& p, int* progress, int n_clusters, cudaStream_t s);
 // Rows past each utterance's length: Y (B, T, n_mels) rows 0, prev_hist (B, T) rows -1 (either may be nullptr).  With
 // `derive`, lengths[b] is first computed from the window history p_hist (B, T) of a run of `steps` frames by the rule
 // decode_until_kernel applies in its frame loop.

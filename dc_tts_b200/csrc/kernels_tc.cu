@@ -581,6 +581,25 @@ void launch_f32_to_planes_scaled(const float* x, int ldx, Planes p, int B, int L
     if (B > 0 && (long long)L * C > 0x7fffffffLL) throw std::runtime_error("f32_to_planes_scaled: L x C exceeds 2^31");
     if (B > 0) f32_to_planes_scaled_kernel<<<(unsigned)B, PLANES_SCALED_THREADS, 0, s>>>(x, ldx, p, L, C, in_inv, lengths);
 }
+// grid (x: row blocks, y: windows); the product and split are f32_to_planes_scaled_kernel's, with the scale fixed
+__global__ void mel_windows_to_planes_kernel(const float* __restrict__ Y, int T, int C, const int* __restrict__ win, int W,
+                                             int L, Planes p, float* __restrict__ in_inv) {
+    const int w = blockIdx.y;
+    const int n = __ldg(win + w), utt = __ldg(win + W + w), row0 = __ldg(win + 2 * W + w);
+    if (blockIdx.x == 0 && threadIdx.x == 0) in_inv[w] = 1.f / SSRN_WINDOW_SCALE;
+    const float* yb = Y + ((size_t)utt * T + row0) * C;
+    const size_t prow = (size_t)w * L;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < L * C; i += gridDim.x * blockDim.x) {
+        const int r = i / C, c = i - r * C;
+        split_f16(r < n ? yb[(size_t)r * C + c] * SSRN_WINDOW_SCALE : 0.f, p.hi[(prow + r) * p.ld + c], p.lo[(prow + r) * p.ld + c]);
+    }
+}
+void launch_mel_windows_to_planes(const float* Y, int T, int C, const int* win, int W, int L, Planes p, float* in_inv,
+                                  cudaStream_t s) {
+    if (W <= 0 || L <= 0) return;
+    const int blocks = std::min(64, (L * C + 255) / 256);
+    mel_windows_to_planes_kernel<<<dim3((unsigned)blocks, (unsigned)W), 256, 0, s>>>(Y, T, C, win, W, L, p, in_inv);
+}
 void launch_planes_to_f32(Planes p, float* y, int ldy, long long rows, int C, cudaStream_t s) {
     long long n = rows * C;
     if (n > 0) planes_to_f32_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(p, y, ldy, rows, C);

@@ -94,5 +94,13 @@ void launch_f32_to_planes(const float* x, int ldx, Planes p, long long rows, int
 void launch_f32_to_planes_scaled(const float* x, int ldx, Planes p, int B, int L, int C, float* in_inv, cudaStream_t s,
                                  const int* lengths = nullptr);
 void launch_planes_to_f32(Planes p, float* y, int ldy, long long rows, int C, cudaStream_t s);
+// Windows of mel rows for the windowed SSRN of a synthesis stream: window w is rows [row0[w], row0[w] + len[w]) of
+// utterance utt[w] of Y (B, T, C) fp32, as rows [0, len[w]) of a (W, L, C) plane batch at the fixed scale
+// SSRN_WINDOW_SCALE; rows [len[w], L) become zero planes.  in_inv[w] = 1 / SSRN_WINDOW_SCALE.  win: len[W] | utt[W] | row0[W]
+// (device ints).  The scale is utterance_scale's for an abs-max in [0.5, 1), which a sigmoid output below 1 reaches
+// whenever its loudest value is >= 0.5: then the planes equal launch_f32_to_planes_scaled's on the whole utterance.
+constexpr float SSRN_WINDOW_SCALE = 32768.f;
+void launch_mel_windows_to_planes(const float* Y, int T, int C, const int* win, int W, int L, Planes p, float* in_inv,
+                                  cudaStream_t s);
 
 }  // namespace dctts

@@ -69,7 +69,7 @@ class Engine:
             raise DcttsError("dctts_create: " + self._lib.dctts_last_error(None).decode())
         self._h = h
         self.params_loaded = False
-        self._streams = weakref.WeakSet()   # open VocoderStreams: closed before the handle they hold
+        self._streams = weakref.WeakSet()   # open VocoderStreams and SynthesisStreams: closed before the handle they hold
 
     # ------------------------------------------------------------------ plumbing
     def close(self):
@@ -719,6 +719,50 @@ class Engine:
         self._set_vocoder_params()
         return VocoderStream(self, int(B), T_cap, int(n_iter), momentum)
 
+    def synthesis_stream(self, L, stop_pos=None, tail=0, chunk=16, n_iter=-1, momentum=0.0):
+        """Streaming synthesis from text (include/dctts.h: dctts_synth_stream_*): the until-EOS decode of the texts L
+        (B, max_N) starts now, and poll() returns audio while it is still running.  stop_pos and tail are
+        text2mel_generate_until's, n_iter and momentum spectrogram2wav's; each utterance's mel frames are turned into
+        audio in chunks of `chunk` frames on a fixed grid, so the samples do not depend on when poll() runs.  Returns a
+        SynthesisStream: poll(wait=True) gives B float32 numpy arrays of new samples (iterating yields them until every
+        utterance is done), close() gives (lengths, trims) as text2mel_generate_until and spectrogram2wav report them.
+        The utterances are decoded in the order of their stop positions, as text2mel_generate_until does; everything
+        comes back in the caller's order."""
+        from .data_load import eos_positions
+        if tail < 0:
+            raise DcttsError("synthesis_stream: tail must be >= 0")
+        L = self._i32(L)
+        B = L.shape[0]
+        sp = eos_positions(L.cpu().numpy()) if stop_pos is None else _host_ints("synthesis_stream", stop_pos, B, "stop position")
+        order = np.argsort(np.where(sp < 0, np.iinfo(np.int32).max, sp), kind="stable")
+        momentum = float(momentum)
+        if momentum > 1:
+            warnings.warn("Griffin-Lim with momentum=%g > 1 can be unstable. Proceed with caution!" % momentum, stacklevel=2)
+        self._set_vocoder_params()
+        return SynthesisStream(self, L, order, sp, int(tail), int(chunk), int(n_iter), momentum)
+
+    def ssrn_halo(self):
+        """(left, right): the mel frames of context SSRN needs on each side of a run of frames (dctts_ssrn_halo)."""
+        left, right = C.c_int32(), C.c_int32()
+        self._check(self._lib.dctts_ssrn_halo(self._h, C.byref(left), C.byref(right)), "dctts_ssrn_halo")
+        return left.value, right.value
+
+    def ssrn_windows(self, Y, starts, counts, lengths):
+        """Test aid (include/dctts.h: dctts_ssrn_windows): a synthesis stream's windowed SSRN on Y (B, T, n_mels).
+        Utterance b commits mel rows [starts[b], starts[b] + counts[b]) at length lengths[b]; returns Z (B, 4 max(counts),
+        F) with each utterance's 4 counts[b] sigmoid rows first and zeros after."""
+        Y = self._f32(Y)
+        B, T, _ = Y.shape
+        st = np.ascontiguousarray(_host_ints("ssrn_windows", starts, B, "start"), np.int32)
+        ct = np.ascontiguousarray(_host_ints("ssrn_windows", counts, B, "count", 1), np.int32)
+        n = np.ascontiguousarray(_host_ints("ssrn_windows", lengths, B, "length", 1, T), np.int32)
+        ld = int(ct.max())
+        Z = torch.zeros(B, self.hp.r * ld, self.F, device=self.device)
+        self._check(self._lib.dctts_ssrn_windows(self._h, _ptr(Y), B, T, st.ctypes.data_as(C.c_void_p),
+                                                 ct.ctypes.data_as(C.c_void_p), n.ctypes.data_as(C.c_void_p), _ptr(Z), ld,
+                                                 self._stream()), "dctts_ssrn_windows")
+        return Z
+
     def vocoder_momentum_step(self, wav, S, E, X, momentum, partials=None, hop=None, win=None):
         """Test aid (include/dctts.h: dctts_vocoder_momentum_step): ONE fast Griffin-Lim phase step on caller CUDA tensors.
         wav (B, Ly) and S (B, T, F) float32 in; E (B, T, F) complex64 holds est_{i-1} on entry and est_i on return;
@@ -1168,6 +1212,86 @@ class VocoderStream:
             vs, self._vs = self._vs, None
             self._eng._streams.discard(self)
             self._eng._lib.dctts_vocoder_stream_close(vs, None)
+
+    def __del__(self):
+        self._free()
+
+
+class SynthesisStream:
+    """One dctts_synth_stream on an engine (Engine.synthesis_stream).  The decode runs on the stream that was current at
+    open; the SSRN windows and the vocoder run on the library's own side stream."""
+
+    def __init__(self, eng, L, order, stop_pos, tail, chunk, n_iter, momentum):
+        self._eng, self.B = eng, L.shape[0]
+        self._order = np.asarray(order)
+        perm = torch.as_tensor(self._order, device=eng.device)
+        self._L = L.index_select(0, perm).contiguous()          # kept alive while the decode reads it
+        sps = np.ascontiguousarray(stop_pos[self._order], np.int32)
+        self.ld = eng.hp.hop_length * (eng.hp.r * eng.hp.max_T - 1)
+        self._wav = np.zeros((self.B, self.ld), np.float32)
+        self.done = np.zeros(self.B, bool)
+        self.frames = np.zeros(self.B, np.int32)             # decode frames published for each utterance at the last poll
+        self.first_frames = None
+        ss = C.c_void_p()
+        self._ss = None
+        eng._check(eng._lib.dctts_synth_stream_open(eng._h, _ptr(self._L), self.B, sps.ctypes.data_as(C.c_void_p), tail, chunk,
+                                                    n_iter, momentum, eng._stream(), C.byref(ss)), "dctts_synth_stream_open")
+        self._ss = ss
+        eng._streams.add(self)
+
+    def poll(self, wait=True):
+        """B float32 numpy arrays (caller's order) of the samples committed since the last poll; with `wait`, blocks until
+        there is something to return or every utterance is done."""
+        if self._ss is None:
+            raise DcttsError("dctts_synth_stream_poll: the stream is closed")
+        B = self.B
+        n, d, f = np.zeros(B, np.int32), np.zeros(B, np.int32), np.zeros(B, np.int32)
+        self._eng._check(self._eng._lib.dctts_synth_stream_poll(self._ss, int(bool(wait)), self._wav.ctypes.data_as(C.c_void_p),
+                                                                self.ld, n.ctypes.data_as(C.c_void_p), d.ctypes.data_as(C.c_void_p),
+                                                                f.ctypes.data_as(C.c_void_p)),
+                         "dctts_synth_stream_poll")
+        out = [None] * B
+        for i, b in enumerate(self._order):
+            out[b] = self._wav[i, :n[i]].copy()
+            self.done[b] = bool(d[i])
+            self.frames[b] = f[i]
+        return out
+
+    def __iter__(self):
+        while not self.done.all():
+            yield self.poll()
+
+    def close(self, outputs=False):
+        """Waits for the decode, runs what is left and frees the stream.  Returns (lengths, trims) in the caller's order,
+        as text2mel_generate_until and spectrogram2wav report them; with outputs=True also Y (B, max_T, n_mels) and Z
+        (B, 4 max_T, F), CUDA tensors with rows past each length 0.  Sets first_frames: the decode frames published when
+        each utterance's first chunk was pushed."""
+        if self._ss is None:
+            return None
+        eng, B, h = self._eng, self.B, self._eng.hp
+        n, trim, ff = np.zeros(B, np.int32), np.zeros((B, 2), np.int32), np.zeros(B, np.int32)
+        Y = eng._empty(B, h.max_T, h.n_mels) if outputs else None
+        Z = eng._empty(B, h.r * h.max_T, eng.F) if outputs else None
+        ss, self._ss = self._ss, None
+        eng._streams.discard(self)
+        rc = eng._lib.dctts_synth_stream_close(ss, n.ctypes.data_as(C.c_void_p), trim.ctypes.data_as(C.c_void_p), _ptr(Y), _ptr(Z),
+                                               ff.ctypes.data_as(C.c_void_p))
+        eng._check(rc, "dctts_synth_stream_close")
+        inv = np.empty(B, np.int64)
+        inv[self._order] = np.arange(B)
+        self.first_frames = ff[inv]
+        res = (n[inv], trim[inv])
+        if outputs:
+            perm = torch.as_tensor(inv, device=eng.device)
+            res += (Y.index_select(0, perm), Z.index_select(0, perm))
+        return res
+
+    def _free(self):
+        """Frees the stream without outputs (Engine.close and garbage collection); its engine's handle is still open."""
+        if getattr(self, "_ss", None) is not None:
+            ss, self._ss = self._ss, None
+            self._eng._streams.discard(self)
+            self._eng._lib.dctts_synth_stream_close(ss, None, None, None, None, None)
 
     def __del__(self):
         self._free()

@@ -287,6 +287,50 @@ int dctts_vocoder_stream_push(dctts_vocoder_stream vs, const float* mag, int32_t
  * (every utterance must then be final).  Frees the stream whether or not the trims could be formed; synchronises `stream`. */
 int dctts_vocoder_stream_close(dctts_vocoder_stream vs, int32_t* trim_host);
 
+/* Streaming synthesis from text (DESIGN.md section 8j): the until-EOS decode publishes its progress to the host, SSRN runs
+ * over windows of the published mel frames with the halo it needs, and a dctts_vocoder_stream turns them into samples while
+ * the decode is still running.  Utterance b's mel frames are committed on a fixed grid of `chunk` frames (the last chunk
+ * ends at its length); each chunk is one SSRN window and one vocoder push, in order, so the samples depend on the texts,
+ * the weights and `chunk` alone, not on when the host polls.  Committed magnitude rows equal dctts_ssrn_ragged's on the
+ * decode's Y bit for bit when the utterance's Y abs-max lies in [0.5, 1) (the windows' input planes use that fixed scale,
+ * 2^15).  One stream per handle; while it is open, every entry point that writes the decode workspace or the weights or
+ * grows a buffer (dctts_textenc, the generations, the teacher-forced graph, dctts_ssrn past max_T, dctts_reserve*, training, commit,
+ * refresh) fails naming the open stream.  dctts_destroy closes an open stream (waiting for its decode).
+ * Errors are reported by dctts_last_error(h). */
+typedef struct dctts_synth_stream_s* dctts_synth_stream;
+/* The mel frames of context SSRN needs before (*left) and after (*right) a run of committed frames, derived from the
+ * committed layer table. */
+int dctts_ssrn_halo(dctts_handle h, int32_t* left, int32_t* right);
+/* Test aid: the stream's windowed SSRN on a caller's Y (B, T, n_mels) DEVICE.  Window b commits mel rows
+ * [starts_host[b], starts_host[b] + counts_host[b]) of utterance b of length lengths_host[b] (1 .. T), reading rows
+ * [max(0, start - left), min(length, end + right)); Z (B, 4 ldz_frames, F) DEVICE row b receives its 4 counts_host[b]
+ * sigmoid rows from its start.  Synchronises `stream`. */
+int dctts_ssrn_windows(dctts_handle h, const float* Y, int32_t B, int32_t T, const int32_t* starts_host, const int32_t* counts_host,
+                       const int32_t* lengths_host, float* Z, int32_t ldz_frames, void* stream);
+/* Opens a stream for B utterances of texts L (B, max_N) DEVICE int32, with dctts_text2mel_generate_until's stop positions
+ * (stop_pos_host, HOST) and tail, `chunk` >= 1 mel frames per commit, and dctts_vocoder_stream_open's n_iter and momentum.
+ * Allocates everything the stream needs, runs TextEnc and launches the decode on `stream`, and returns without waiting.
+ * The decode takes the fewest utterances per cluster that leave one co-resident 16-CTA cluster slot free for the SSRN
+ * and vocoder launches, where five per cluster allow it.  Fails without the persistent decode (after training:
+ * dctts_refresh_synthesis), without a tensor-core SSRN chain, with chunk < 1, or when a stream is already open. */
+int dctts_synth_stream_open(dctts_handle h, const int32_t* L, int32_t B, const int32_t* stop_pos_host, int32_t tail, int32_t chunk,
+                            int32_t n_iter, double momentum, void* stream, dctts_synth_stream* out);
+/* Runs every chunk that is ready (one SSRN launch set and one vocoder push per round, on the stream's own side stream) and
+ * returns each utterance's newly committed samples, de-emphasised and untrimmed as dctts_vocoder_stream_push returns them:
+ * wav (B, ld) HOST row b receives counts_host[b] samples, ld >= hop (4 max_T - 1); done_host[b] != 0 once utterance b
+ * has had its last chunk; frames_host (B, HOST, or NULL) the mel frames utterance b's decode cluster had published when
+ * the poll returned (never decreasing).  With `wait`, first blocks until a chunk is ready or every utterance is done,
+ * failing with the decode's error if it failed.  Never synchronises the device. */
+int dctts_synth_stream_poll(dctts_synth_stream ss, int32_t wait, float* wav, int64_t ld, int32_t* counts_host,
+                            int32_t* done_host, int32_t* frames_host);
+/* Waits for the decode, runs the remaining chunks, and frees the stream.  Outputs (each may be NULL; with all NULL the
+ * stream is freed without running the rest): lengths_host (B) as dctts_text2mel_generate_until reports them; trim_host
+ * (B, 2) as dctts_vocoder_stream_close; Y (B, max_T, n_mels) DEVICE the decode's mels, rows past each length 0; Z
+ * (B, 4 max_T, F) DEVICE the committed magnitudes, rows past each length 0; first_frames_host (B) the frames the
+ * utterance's decode cluster had published when its first chunk was pushed. */
+int dctts_synth_stream_close(dctts_synth_stream ss, int32_t* lengths_host, int32_t* trim_host, float* Y, float* Z,
+                             int32_t* first_frames_host);
+
 /* Feature extraction (next row, SURVEY 8f-4): get_spectrograms -- utils.py:20-65 -- for ONE utterance from the
  * loaded waveform on: trim (librosa.effects.trim), pre-emphasis, STFT, |.|, mel filterbank
  * (librosa.filters.mel(sample_rate, n_fft, n_mels)), 20 log10, normalisation with the constants of
@@ -459,6 +503,10 @@ int dctts_set_tensor_path(dctts_handle h, int32_t mode);
  *   "train_deterministic" 0/1 (default 0): the training step's sums in a fixed order, so that a seeded run repeats bit for
  *                  bit (see dctts_train_step_shaped); it may change between steps and does not affect synthesis
  *   "chain_history" 0/1 (default 0): test aid, the full-sequence chains keep every block's rows for dctts_chain_history
+ *   "decode_group" 0..5 (default 0): measurement switch, utterances per persistent-decode cluster; 0 = the library's rule
+ *                  (the fewest that keep every cluster co-resident; a synthesis stream's leaves one cluster slot free)
+ *   "decode_timing" 0/1 (default 0): measurement switch, CUDA events around every persistent-decode launch; dctts_get_option
+ *                  "decode_last_us" then gives the last launch's GPU time in microseconds (waits for it)
  * dctts_get_option also answers "decode_available" (1 when this handle / device can run the persistent decode),
  * "decode_max_clusters" (16-CTA clusters of the decode kernel that are co-resident on this device) and, once the
  * parameters are committed, "ssrn_tc_available" (1 when every SSRN block has a wgmma kernel, the F-wide ones included:
